@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of VQVAE.forward (enc + VQ + dec) on N B200s.
+"""bench.py -- images/sec of VQVAE.forward (enc + VQ + dec) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one VQVAE.forward over one batch of synthetic images per GPU.  Prints ONE JSON line (rank 0).
 
   headline   BASELINE.json configs[1] (cfg2: B=256 per GPU, 3x32x32, K=512, D=64), per-GPU batch fixed as N grows
-             (weak scaling, batch-sharded, no data-path collective).  Convs = tcgen05 kind::tf32 on fp32 activations
+             (weak scaling, batch-sharded, no data-path collective).  Convs = wgmma tf32 on fp32 activations
              (what the reference itself computes on a GPU), VQ bit-exact fp32; the all-FFMA fp32 numbers ride along.
     value      whole-job images/sec, inputs resident in HBM, device time (CUDA events per step, L2 flushed between
                steps, max over ranks)
@@ -57,7 +57,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm=float(d["hbm_gbs"]), bf16=float(d["bf16_tflops"]),
                     bf16_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W card, dense): 3.35 TB/s HBM3, 989 TFLOP/s bf16 -- ceilings, not measurements
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet")
 
 
 # --------------------------------------------------------------------------- synthetic weights / images (no oracle import)
@@ -291,7 +292,7 @@ def kernel_entry(label, ms, calls, share, B, K, D, peaks, traffic=None):
     except Exception as e:  # pragma: no cover - an unparsable label must not kill the line
         row["error"] = repr(e)[:100]
         return row
-    tpeak = peaks["bf16"] * (1.0 if tdt == "bf16" else 0.5)      # TF32 = half the measured bf16 cuBLAS peak
+    tpeak = peaks["bf16"] * (1.0 if tdt == "bf16" else 0.5)      # TF32 = half the bf16 peak
     t_hbm, t_tc = byts / (peaks["hbm"] * 1e9), flops / (tpeak * 1e12)
     if t_tc >= t_hbm:
         ach = flops / (ms * 1e-3) / 1e12
@@ -301,15 +302,6 @@ def kernel_entry(label, ms, calls, share, B, K, D, peaks, traffic=None):
         row.update(bound="hbm", achieved=ach, peak=peaks["hbm"], unit="GB/s", frac=ach / peaks["hbm"])
     row["traffic"] = traffic
     return row
-
-
-def ncu_traffic_table():
-    """DRAM bytes (read + write) per launch from this round's committed `ncu --set full` capture, keyed by label."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_step_kernels_traffic.json")) as f:
-            return json.load(f)
-    except (OSError, ValueError):
-        return {}
 
 
 def build_model(wl, dev):
@@ -370,6 +362,9 @@ def main():
     ap.add_argument("--skip-cpu", action="store_true")
     ap.add_argument("--quick", action="store_true", help="headline only: no fp32 mode, cfg3, cfg5, vq_sweep")
     ap.add_argument("--no-extra-modes", action="store_true", help="alias of --quick")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the headline's last timed step returned (loss, x_hat, perplexity, "
+                         "min_encoding_indices) as DIR/<name>.npy; same arguments -> same inputs")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     args.quick = args.quick or args.no_extra_modes
@@ -397,8 +392,7 @@ def main():
     from vqvae_b200.synth import make_images
 
     peaks = load_peaks()
-    traffic_tab = ncu_traffic_table()
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         if dist is not None:
@@ -413,10 +407,10 @@ def main():
         return [float(v) for v in t.tolist()]
 
     def breakdown(model, x, Bx, K, D):
-        """Per-kernel CUDA-event times (eager launches behind a spin kernel, L2 flushed) -> `kernels` rows."""
+        """Per-kernel CUDA-event times over --steps eager forwards (behind a spin kernel, L2 flushed) -> `kernels` rows."""
         per = {}
         saved_group, model.process_group = model.process_group, None     # rank-local: no collective here
-        reps = 5
+        reps = args.steps
         for _ in range(reps):
             flush.zero_()
             ops.PROFILE = []
@@ -429,19 +423,22 @@ def main():
         model.process_group = saved_group
         tot = {k: float(np.sum(v)) / reps for k, v in per.items()}
         step_ms = sum(tot.values())
-        rows = [kernel_entry(k, float(np.mean(v)), len(v) // reps, tot[k] / step_ms, Bx, K, D, peaks, traffic_tab.get(k))
+        rows = [kernel_entry(k, float(np.mean(v)), len(v) // reps, tot[k] / step_ms, Bx, K, D, peaks)
                 for k, v in per.items()]
         return sorted(rows, key=lambda r: -r["share"])
 
-    def device_time(step, steps):
+    def device_time(step, steps, last=None):
         evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
         barrier()
+        o = None
         for s0, s1 in evs:
             flush.zero_()
             s0.record()
-            step()
+            o = step()
             s1.record()
         barrier()
+        if last is not None:
+            last.append(o)
         return sum(a.elapsed_time(b) for a, b in evs)
 
     # =============================================================== headline workload
@@ -471,7 +468,10 @@ def main():
             step()
         barrier()
         clocks = ClockSampler(local_rank if (full and not os.environ.get("VQB_BENCH_NOSAMPLER")) else -1)
-        dev_ms = device_time(step, args.steps)
+        last = []
+        dev_ms = device_time(step, args.steps, last)
+        if full and args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last[0], model.last_min_encoding_indices)
         res = dict(launches=int(launches_per_step * args.steps), graph=is_graph)
         if full:
             # ---- end to end: host buffers, copies inside the timed region ----
@@ -542,7 +542,7 @@ def main():
         mb = run_mode("bf16", False)
         line_extra["bf16_mode"] = {"value": mb["value"], "unit": "images/sec", "ms_per_step": mb["ms_per_step"], "dtype": "bf16",
                                    "gpu_launches": mb["launches"], "kernels": mb.get("kernels", [])[:12], "flips": mb.get("flips"),
-                                   "note": "same workload through the bf16 pipeline (tcgen05 kind::f16 on bf16 operands, bf16 NHWC "
+                                   "note": "same workload through the bf16 pipeline (wgmma on bf16 operands, bf16 NHWC "
                                            "activations, exact fp32 VQ): the arithmetic of the reference under torch.autocast(bfloat16)"}
         vqvae_b200.set_precision(prec_main)
 
@@ -578,7 +578,7 @@ def main():
         step, out, is_graph = capture(m, xb)
         for _ in range(3):
             step()
-        nsteps = max(3, min(args.steps, 10))
+        nsteps = args.steps
         ms, = allmax([device_time(step, nsteps)])
         o = {"workload": w["desc"], "dtype": "bf16", "per_gpu_batch": per_gpu_batch, "n_gpus": world, "steps": nsteps,
              "value": per_gpu_batch * world * nsteps / (ms * 1e-3), "unit": "images/sec", "ms_per_step": ms / nsteps,
@@ -615,12 +615,11 @@ def main():
     if top and "frac" in top:
         roofline = {k: top[k] for k in ("kernel", "bound", "achieved", "peak", "unit", "frac", "traffic")}
         roofline["peak_source"] = peaks["src"]
-        roofline["traffic_source"] = "profiles/r02_step_kernels_traffic.json (this round's ncu --set full capture)" if top.get("traffic") else None
-        roofline["note"] = "tf32 layers are held against half the measured bf16 cuBLAS peak"
-    dtype_note = {"tf32": "fp32 tensors end to end; convs = tcgen05 kind::tf32 with fp32 accumulation (PyTorch/cuDNN's default conv "
+        roofline["note"] = "tf32 layers are held against half the bf16 peak (peaks: see peak_source)"
+    dtype_note = {"tf32": "fp32 tensors end to end; convs = wgmma tf32 with fp32 accumulation (PyTorch/cuDNN's default conv "
                           "arithmetic on this GPU); VQ distances/argmin bit-exact fp32; fp32_mode = all-FFMA numbers",
                   "fp32": "all arithmetic fp32 (FFMA)",
-                  "bf16": "bf16 activations and operands between layers (tcgen05 kind::f16), fp32 accumulation, fp32 z_e, "
+                  "bf16": "bf16 activations and operands between layers (wgmma bf16), fp32 accumulation, fp32 z_e, "
                           "VQ distances/argmin bit-exact fp32 on that z_e"}[prec_main]
     line = {
         "metric": METRIC, "value": main_mode["value"], "unit": "images/sec", "n_gpus": world, "steps": args.steps,
@@ -659,19 +658,38 @@ def main():
     if cfg5 is not None:
         line["cfg5"] = cfg5
     if not args.quick:
-        line["vq_sweep"] = vq_sweep(ops, peaks, dev)
+        line["vq_sweep"] = vq_sweep(ops, peaks, dev, args.steps)
         line["vq_kernel"] = line["vq_sweep"][0]
     else:
-        line["vq_kernel"] = vq_point(ops, peaks, dev, 512, 64)
+        line["vq_kernel"] = vq_point(ops, peaks, dev, 512, 64, reps=args.steps)
     print(json.dumps(line), flush=True)
     if dist is not None:
         dist.destroy_process_group()
 
 
-def vq_point(ops, peaks, dev, K, D, N=1 << 20):
+def dump_outputs(d, out, idx):
+    """What VQVAE.forward returned in the last timed step, as float32 / float64 .npy files.  An x_hat larger than 2^22
+    elements (cfg3: 25M) is written as a fixed seeded sample of 2^22 of them with their flat indices, so the dump
+    stays under 64 MB."""
+    os.makedirs(d, exist_ok=True)
+    loss, x_hat, perp = out
+    xh = x_hat.detach().float().reshape(-1)
+    if xh.numel() > (1 << 22):
+        g = torch.Generator(device="cpu").manual_seed(0)
+        pick = torch.randperm(xh.numel(), generator=g)[:1 << 22].sort().values
+        np.save(os.path.join(d, "x_hat_sample_index.npy"), pick.numpy().astype(np.float64))
+        np.save(os.path.join(d, "x_hat_sample.npy"), xh.cpu()[pick].numpy().astype(np.float32))
+    else:
+        np.save(os.path.join(d, "x_hat.npy"), x_hat.detach().float().cpu().numpy())
+    np.save(os.path.join(d, "loss.npy"), loss.detach().float().cpu().numpy().astype(np.float32).reshape(1))
+    np.save(os.path.join(d, "perplexity.npy"), perp.detach().float().cpu().numpy().astype(np.float32).reshape(1))
+    np.save(os.path.join(d, "min_encoding_indices.npy"), idx.detach().cpu().numpy().astype(np.float64).reshape(-1))
+
+
+def vq_point(ops, peaks, dev, K, D, N=1 << 20, reps=5):
     """The VQ kernel alone at a streaming size (N rows in, N rows + indices out: larger than L2, no flush needed),
-    CUDA events around `reps` calls of vqb_vq_forward_f32; algorithmic bytes = (2*D*4 + 8) per row (SURVEY 8d), held
-    against max(T_hbm, T_tensor) with the TF32 ceiling = half the measured bf16 peak."""
+    CUDA events around `reps` (= --steps) calls of vqb_vq_forward_f32; algorithmic bytes = (2*D*4 + 8) per row (SURVEY 8d), held
+    against max(T_hbm, T_tensor) with the TF32 ceiling = half the bf16 peak."""
     try:
         rng = np.random.RandomState(0)
         z = torch.from_numpy(rng.standard_normal((N, D)).astype(np.float32)).to(dev)
@@ -680,7 +698,6 @@ def vq_point(ops, peaks, dev, K, D, N=1 << 20):
             ops.vq_forward(z, E)
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        reps = 5 if K * D <= 1024 * 64 else 2
         e0.record()
         for _ in range(reps):
             ops.vq_forward(z, E)
@@ -694,7 +711,7 @@ def vq_point(ops, peaks, dev, K, D, N=1 << 20):
         out = {"rows": N, "K": K, "D": D, "ms_per_call": ms, "bound": bound,
                "hbm_gbs": byts / (ms * 1e-3) / 1e9, "tensor_tflops": flops / (ms * 1e-3) / 1e12,
                "frac": max(t_hbm, t_tc) / (ms * 1e-3), "algorithmic_bytes_per_row": 2 * D * 4 + 8, "peak_source": peaks["src"],
-               "kernel": "tcgen05 (vq2.cu)" if D == 64 and K <= 8192 else "FFMA (vq_exact.cu)",
+               "kernel": "wgmma tf32 selection + canonical fp32 re-scoring (vq_tc_kernel)" if D == 64 else "FFMA (vq_exact.cu)",
                "note": "codebook N(0,1), rows N(0,1); idx/z_q bit-exact vs the canonical fp32 order (tests)"}
         if bound == "hbm":
             out.update(achieved=out["hbm_gbs"], peak=peaks["hbm"], unit="GB/s")
@@ -705,8 +722,8 @@ def vq_point(ops, peaks, dev, K, D, N=1 << 20):
         return {"K": K, "D": D, "error": repr(e)[:200]}
 
 
-def vq_sweep(ops, peaks, dev):
-    return [vq_point(ops, peaks, dev, K, D, N=(1 << 20) if D == 64 else (1 << 18))
+def vq_sweep(ops, peaks, dev, reps):
+    return [vq_point(ops, peaks, dev, K, D, N=(1 << 20) if D == 64 else (1 << 18), reps=reps)
             for K, D in ((512, 64), (1024, 64), (8192, 64), (512, 256), (1024, 256), (8192, 256))]
 
 

@@ -1,5 +1,5 @@
 /*
- * vqvae_b200.h -- C ABI of the B200 (sm_100a) VQ-VAE inference hot path.
+ * vqvae_b200.h -- C ABI of the H100 (sm_90a) VQ-VAE inference hot path.
  *
  * The reference (MishaLaskin/vqvae) is pure Python on top of PyTorch and exposes no
  * FFI of its own (SURVEY.md 8b); its "plugin API" for this path is the nn.Module
@@ -43,7 +43,7 @@ enum vqb_status {
     VQB_ERR_BAD_ARG = -1,       /* NULL pointer, non-positive size, bad enum          */
     VQB_ERR_UNSUPPORTED = -2,   /* shape outside what the kernels implement          */
     VQB_ERR_WORKSPACE = -3,     /* workspace too small (see *_workspace_bytes)       */
-    VQB_ERR_NO_DEVICE = -4,     /* no sm_100 device / driver                         */
+    VQB_ERR_NO_DEVICE = -4,     /* no sm_90 device / driver                          */
     VQB_ERR_ALIGNMENT = -5      /* pointer not aligned as documented                 */
 };
 
@@ -54,13 +54,13 @@ enum vqb_layout { VQB_NCHW = 0, VQB_NHWC = 1 };
  * the *_f32 entry points answer VQB_ERR_UNSUPPORTED to it -- use vqb_conv2d_bf16 & co.   */
 enum vqb_precision {
     VQB_FP32 = 0,  /* fp32 FFMA accumulate (CUDA cores): the reference's CPU numerics   */
-    VQB_TF32 = 1,  /* tcgen05 kind::tf32, fp32 accumulate in TMEM (cuDNN's default)     */
-    VQB_BF16 = 2   /* tcgen05 kind::f16 on bf16 operands and activations (bf16 entry points only) */
+    VQB_TF32 = 1,  /* wgmma tf32, fp32 accumulate (cuDNN's default)                    */
+    VQB_BF16 = 2   /* wgmma on bf16 operands and activations (bf16 entry points only) */
 };
 
 int vqb_abi_version(void);
 /* 0: release library -- never reads the environment, no diagnostic / work-skipping code paths
- * compiled in.  1: built with -DVQB_DIAG=1 (tools/diag experiments only).                  */
+ * compiled in.  1: built with -DVQB_DIAG=1 (environment knobs for experiments).         */
 int vqb_diag_build(void);
 const char *vqb_error_string(int code);
 /* SM count and compute capability of the current device. */
@@ -76,7 +76,7 @@ unsigned long long vqb_launch_count(void);
  * nn.ConvTranspose2d weight (Cin,Cout,kh,kw) decoder.py:28-35   (transposed = 1)
  * -> `packed` holds 2*Cout*Cin*kh*kw + 144*Cin floats: the tap-major GEMM operand in both
  *    layouts the kernels read, [(r*kw+s)*Cin + ci][co] (FFMA path) followed by
- *    [(r*kw+s)][co][ci] (K-major rows for the tcgen05 path); for a k4 s2 transposed
+ *    [(r*kw+s)][co][ci] (K-major rows for the wgmma path); for a k4 s2 transposed
  *    conv with Cout <= 4 a third region [9][16][Cin] (3x3-neighbourhood + pixel-shuffle
  *    form of decoder.py:34-35) follows.                                           */
 int vqb_pack_conv_weight_f32(const float *w, float *packed, int Cout, int Cin, int kh,
@@ -96,9 +96,9 @@ int vqb_conv2d_f32(const float *in, const float *w_packed, const float *bias,
                    int kh, int kw, int stride, int pad, int transposed, int in_layout,
                    int out_layout, int relu, int precision, void *stream);
 
-/* ---- bf16 activation path (VQB_BF16): persistent tcgen05 kind::f16 kernels ------------
+/* ---- bf16 activation path (VQB_BF16): wgmma kernels on bf16 operands ----------------------
  * Between layers the activations are bf16 NHWC; weights are packed to bf16 once per
- * load_state_dict; accumulation is fp32 in TMEM.  This is the arithmetic the reference
+ * load_state_dict; accumulation is fp32 in registers.  This is the arithmetic the reference
  * reaches through torch.autocast(dtype=torch.bfloat16) around vqvae.py:29-44 (SURVEY Q6).
  * The layer shapes are named, not parameterised:                                         */
 enum vqb_conv_kind {
@@ -137,7 +137,7 @@ int vqb_vq_forward_bf16zq_f32(const float *z, const float *codebook, int64_t N, 
  * SURVEY Q2):  out = act( r + W2 . relu( W1 (*) r ) ),  act = ReLU iff relu_out.
  * w1_packed: vqb_pack_conv_weight_bf16(kind VQB_CONV_K3, Cout = Cmid, Cin = C) of res_block.1.weight;
  * w2_packed: vqb_pack_conv_weight_bf16(kind VQB_RES_W2 = 6, Cout = C, Cin = Cmid) of res_block.3.weight.
- * One persistent tcgen05 kernel: both GEMMs chained per tile, W1 and W2 resident in shared memory.
+ * One wgmma launch: per 128-pixel tile both GEMMs chained, the bf16 intermediate and W2 in shared memory.
  * C in {64, 128}, Cmid % 16 == 0, Cmid <= 64; other shapes return VQB_ERR_UNSUPPORTED.      */
 #define VQB_RES_W2 6
 int vqb_residual_layer_bf16(const void *r, const void *w1_packed, const void *w2_packed, void *out,
@@ -149,8 +149,8 @@ int vqb_residual_layer_bf16(const void *r, const void *w1_packed, const void *w2
  * r, out NHWC (B,H,W,C); W1 = res_block.1.weight (Cmid,C,3,3), W2 = res_block.3.weight
  * (C,Cmid,1,1), both packed by vqb_pack_conv_weight_f32; act = ReLU iff relu_out (inside
  * a ResidualStack the next consumer always applies ReLU first, residual.py:19,50).
- * tmp: B*H*W*Cmid floats of scratch (used only by the two-launch FFMA fallback).
- * With precision != VQB_FP32 and C % 32 == Cmid % 32 == 0 this is ONE tcgen05 kernel
+ * tmp: B*H*W*Cmid floats of scratch (used only by the two-launch paths).
+ * With precision VQB_TF32, C in {64, 128} and Cmid in {32, 64} this is ONE wgmma launch
  * (two chained GEMMs, the Cmid-channel intermediate never leaves the SM).            */
 int vqb_residual_layer_f32(const float *r, const float *w1_packed, const float *w2_packed,
                            float *out, float *tmp, int B, int H, int W, int C, int Cmid,
@@ -162,10 +162,11 @@ int vqb_residual_layer_f32(const float *r, const float *w1_packed, const float *
  * ReLU, or the stack's F.relu at :50):  r_{i+1} = relu( r_i + W2 . relu( W1 (*) r_i ) ),
  * r_0 = r = relu(stack input), out = r_{n_layers}.   r, out NHWC (B,H,W,C).
  * scratch: B*H*W*C floats (needed when n_layers > 1; used when the applications run as
- * separate launches), tmp: B*H*W*Cmid floats (FFMA fallback only).
- * With precision != VQB_FP32, whole images per 128-pixel tile (W <= 8, H <= 16) and the
- * layer shape vqb_residual_layer_f32 accepts, ALL applications run inside ONE tcgen05
- * kernel: the activation tile stays in shared memory and is rewritten in place.        */
+ * separate launches), tmp: B*H*W*Cmid floats (two-launch paths only).
+ * With precision VQB_TF32, the layer shapes the one-launch vqb_residual_layer_f32 takes and
+ * whole images per 128-pixel tile (pow2(W) <= 16 and pow2(W) * pow2(H) <= 128), ALL
+ * applications run inside ONE wgmma launch: each tile's output goes to `out` and is read
+ * back by the next application (no other CTA touches those images).                   */
 int vqb_residual_stack_f32(const float *r, const float *w1_packed, const float *w2_packed,
                            float *out, float *scratch, float *tmp, int B, int H, int W, int C,
                            int Cmid, int n_layers, int precision, void *stream);
@@ -189,22 +190,23 @@ int vqb_vq_forward_f32(const float *z, const float *codebook, int64_t N, int K, 
 
 /* Deferred variant: identical outputs, except that `sse` is only final after
  * vqb_vq_reduce_sse_f32 has run on the same workspace (stream-ordered after this call).
- * The per-CTA SSE partials stay in the workspace, so the tiny reduction -- and the scalar
- * finisher that needs it -- can run on a side stream while the decoder consumes zq
- * (vqvae.py:36 does not depend on the loss terms of quantizer.py:63-64).              */
+ * The sm_90a kernels finish the SSE inside their own launch sequence, so `sse` is already
+ * final here and vqb_vq_reduce_sse_f32 only validates its arguments; the pair stays so
+ * that callers may run the scalar finisher on a side stream (vqvae.py:36 does not depend
+ * on the loss terms of quantizer.py:63-64).                                            */
 int vqb_vq_forward_deferred_f32(const float *z, const float *codebook, int64_t N, int K, int D,
                                 int64_t *idx, float *zq, double *sse, int32_t *hist,
                                 void *workspace, size_t workspace_bytes, void *stream);
 int vqb_vq_reduce_sse_f32(const void *workspace, int64_t N, int K, int D, double *sse,
                           void *stream);
 
-/* Kernel choice of vqb_vq_forward_f32: 0 = auto (tcgen05 kernel when D == 64 and K <= 8192,
- * else the exact FFMA kernel), 1 = always the FFMA kernel, 2 = require the tcgen05 kernel
- * (vq2.cu), 3 = the round-1 tcgen05 kernel (vq_tc.cu, kept for comparison).  All produce
+/* Kernel choice of vqb_vq_forward_f32: 0 = auto (see vqb_vq_forward_f32's dispatch),
+ * 1 = always the exact FFMA kernel, 2 and 3 = require the wgmma kernel (TF32 candidate
+ * selection + canonical fp32 re-scoring; D == 64, 1 <= K <= 2^20).  All produce
  * bit-identical idx / zq; the switch exists for tests and benchmarks.                 */
 int vqb_set_vq_kernel(int which);
 
-/* Diagnostic twin of vqb_vq_forward_f32 (tcgen05 kernel only): additionally dumps the
+/* Diagnostic twin of vqb_vq_forward_f32 (wgmma kernel, D == 64): additionally dumps the
  * approximate TF32 scores s = ||e||^2 - 2 z.e as (N, ceil(K/256)*256) floats.        */
 int vqb_debug_vq_scores_f32(const float *z, const float *codebook, int64_t N, int K, int D,
                             int64_t *idx, float *zq, double *sse, int32_t *hist,
@@ -242,13 +244,10 @@ int vqb_gather_rows_f32(const int64_t *idx, const float *codebook, int64_t N, in
  * the caller's tensor when a ResidualLayer is called directly (SURVEY Q2).         */
 int vqb_relu_f32(float *x, int64_t n, void *stream);
 
-/* Diagnostic: copy the first n (<= 32) entries of the in-kernel timeline (globaltimer ns of CTA 0
- * of the last fused residual kernel) to host memory.  Synchronises the device.          */
+/* In-kernel timeline readers, kept for ABI version 2 compatibility: the sm_90a kernels record
+ * no timelines, so these always return VQB_ERR_UNSUPPORTED.                              */
 int vqb_debug_read_trace(unsigned long long *dst, int n);
-/* Same for the tcgen05 VQ kernel (epilogue warp 4 of CTA 0, local tiles 1-2, 16 marks each; enabled with
- * the environment variable VQB_TC_FLAGS=8).                                                              */
 int vqb_debug_read_trace_vq(unsigned long long *dst, int n);
-/* Per-CTA (start, end<<10 | smid) globaltimer pairs of the last traced tcgen05 VQ launch.               */
 int vqb_debug_read_cta_times(unsigned long long *dst, int n);
 
 /* ---- layout changes at the module boundary (quantizer.py:45, :74) ---------------- */

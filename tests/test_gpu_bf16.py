@@ -1,9 +1,9 @@
-"""VQB_BF16 path: the persistent tcgen05 kind::f16 kernels (hconv.cu, res_bf16.cu) against the C oracle.
+"""VQB_BF16 path: the wgmma bf16 kernels (wgconv.cu via hconv.cu) against the C oracle.
 
 Operands are rounded to bf16 (8-bit mantissa) and accumulated in fp32, so each kernel is compared with the oracle
 evaluated on the SAME bf16-rounded inputs and weights: what is left is the fp32 accumulation order (~1e-5) plus, for
 bf16 outputs, one rounding of the result (relative 2^-9).  Tolerances: bf16 outputs rtol 2^-8 + atol 2e-3, fp32
-outputs atol 2e-4.  Needs a B200 (``-m gpu``).
+outputs atol 2e-4.  Needs an H100 (``-m gpu``).
 """
 import numpy as np
 import pytest
@@ -84,7 +84,7 @@ def test_bf16_conv_layers_vs_oracle(case):
 
 
 def test_bf16_conv_many_tiles_persistent_loop():
-    """More tiles than SMs: every CTA walks several tiles (ring wrap-around, TMEM double buffering)."""
+    """More tiles than SMs: every CTA walks several tiles (ring wrap-around)."""
     rng = np.random.RandomState(7)
     _run_layer(rng, 8, 128, 64, 64, 128, 3, 1, False, True, False)        # 512 tiles of 256 pixels
     _run_layer(rng, 4, 128, 64, 64, 64, 4, 2, True, True, False)          # 2 passes x 256 tiles

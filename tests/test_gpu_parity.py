@@ -1,5 +1,5 @@
 """Parity of the CUDA path (through the C ABI) against the oracle and the committed
-golden vectors of the unmodified reference.  Needs a B200: run with ``-m gpu``.
+golden vectors of the unmodified reference.  Needs an H100: run with ``-m gpu``.
 
 Bars: integer / index outputs bit-exact; fp32 z_q bitwise at the VQ boundary; fp32
 conv outputs within 2e-6 absolute of the double-accumulated oracle at |y| = O(1e-1)
@@ -15,8 +15,8 @@ from tests.helpers import (MODEL_CASES, VQ_CASES, assert_zq_matches, build_model
 
 pytestmark = pytest.mark.gpu
 
-# The tcgen05 VQ kernel sums (e - z)^2 of one row in four fp32 partials (64 terms) and adds rows in double; the FFMA kernel and
-# the oracle add every term in double.  Per-row relative error <= 16 * 2^-24 ~ 1e-6, random in sign across rows.
+# The VQ kernels and the oracle add the (e - z)^2 terms in double, in different orders (per-thread row sums, per-CTA
+# partials); the tolerance leaves room for a per-row relative error of 16 * 2^-24 ~ 1e-6.
 SSE_RTOL = 2e-6
 
 CONV_ATOL = 2e-6     # fp32 FFMA vs double-accumulated oracle, activations O(0.1..1)
@@ -147,7 +147,7 @@ def test_conv_layers_vs_oracle(case):
     _conv_case(rng, *case)
 
 
-# tcgen05 implicit-GEMM path (VQB_TF32): operands truncated to TF32 (rel. 2^-10 each),
+# wgmma implicit-GEMM path (VQB_TF32): operands truncated to TF32 (rel. 2^-10 each),
 # fp32 accumulation -> |err| <= 2^-9 * sum|x||w| ~ 2e-3 * O(1) per output at these scales.
 TC_CONV_CASES = [
     (2, 64, 16, 16, 128, 4, 2, 1, False, 1, 1, True, False),   # encoder.py:32-34 (element-strided TMA)
@@ -171,6 +171,28 @@ TC_CONV_CASES = [
     (2, 3, 32, 32, 128, 4, 2, 1, False, 0, 1, True, False),    # fast path, Cout=128 (direct stores)
     (3, 3, 6, 8, 64, 4, 2, 1, False, 0, 1, True, False),       # partial tile (36 pixels), TMA store clips
 ]
+
+
+def test_tc_transposed_k4s2_is_one_launch():
+    """decoder.py:31-33 in VQB_TF32: the four sub-pixel phases of the stride-2 transposed conv run as ONE tensor-core
+    launch (blockIdx.y = phase), not as four CUDA-core launches, and the result is within the TF32 tolerance."""
+    from vqvae_b200 import ops
+    from vqvae_b200._lib import NHWC, TF32
+    rng = np.random.RandomState(31)
+    B, Cin, H, W, Cout = 4, 128, 8, 8, 64
+    x = rng.standard_normal((B, Cin, H, W)).astype(np.float32)
+    w = (rng.standard_normal((Cin, Cout, 4, 4)) / np.sqrt(Cin * 16)).astype(np.float32)
+    b = rng.standard_normal(Cout).astype(np.float32) * 0.1
+    ref = np.maximum(cref.conv_transpose2d(x, w, b, 2, 1), 0)
+    wp = ops.pack_conv_weight(_cuda(w), True)
+    xin = _cuda(np.ascontiguousarray(x.transpose(0, 2, 3, 1)))
+    bd = _cuda(b)
+    torch.cuda.synchronize()
+    l0 = ops.launch_count()
+    y = ops.conv2d(xin, wp, bd, B=B, Cin=Cin, H=H, W=W, Cout=Cout, kh=4, kw=4, stride=2, pad=1, transposed=True,
+                   in_layout=NHWC, out_layout=NHWC, relu=True, precision=TF32)
+    assert ops.launch_count() - l0 == 1
+    np.testing.assert_allclose(y.cpu().numpy().transpose(0, 3, 1, 2), ref, atol=4e-3, rtol=2e-3)
 
 
 def test_tf32_full_size_properties_cfg2():
@@ -358,7 +380,7 @@ def test_full_size_properties_cfg2():
 @pytest.mark.parametrize("B,H,W,C,Cmid,relu_out", [(2, 8, 8, 128, 32, True), (3, 5, 7, 64, 32, False),
                                                    (1, 20, 36, 128, 64, True), (5, 4, 4, 32, 32, True)])
 def test_fused_residual_layer_tc_vs_oracle(B, H, W, C, Cmid, relu_out):
-    """res_tc.cu (one tcgen05 kernel, two chained GEMMs) vs residual.py:18-29 semantics."""
+    """The TF32 residual layer (one wgmma launch, two chained GEMMs) vs residual.py:18-29 semantics."""
     from vqvae_b200 import ops
     from vqvae_b200._lib import FP32, TF32
     rng = np.random.RandomState(B * 1000 + H * 100 + C)
@@ -378,7 +400,7 @@ def test_fused_residual_layer_tc_vs_oracle(B, H, W, C, Cmid, relu_out):
 @pytest.mark.parametrize("B,H,W,C,Cmid,n", [(256, 8, 8, 128, 32, 2), (5, 8, 8, 128, 32, 3), (3, 6, 7, 128, 32, 2),
                                             (9, 4, 4, 64, 32, 4), (2, 16, 16, 128, 32, 2), (1, 8, 8, 128, 32, 1)])
 def test_fused_residual_stack_tc(B, H, W, C, Cmid, n):
-    """vqb_residual_stack_f32 (residual.py:45-51): all n shared-weight applications in ONE tcgen05 launch when a
+    """vqb_residual_stack_f32 (residual.py:45-51): all n shared-weight applications in ONE wgmma launch when a
     128-pixel tile holds whole images.  Same arithmetic as n separate vqb_residual_layer_f32 launches, so the two
     are bit-identical; both are held to the oracle at the TF32 tolerance, the fp32 mode at 1e-5 per layer."""
     from vqvae_b200 import ops

@@ -1,5 +1,5 @@
-"""The tcgen05 VQ kernel (vq_tc.cu) against the exact FFMA kernel, the C oracle and
-float64 scores.  Needs a B200: run with ``-m gpu``."""
+"""The tensor-core VQ kernel (vq_tc_kernel in vq_exact.cu) against the exact FFMA kernel, the C oracle and
+float64 scores.  Needs an H100: run with ``-m gpu``."""
 import numpy as np
 import pytest
 import torch
@@ -8,8 +8,8 @@ from oracle import cref
 
 pytestmark = pytest.mark.gpu
 
-# The tcgen05 VQ kernel sums (e - z)^2 of one row in four fp32 partials (64 terms) and adds rows in double; the FFMA kernel and
-# the oracle add every term in double.  Per-row relative error <= 16 * 2^-24 ~ 1e-6, random in sign across rows.
+# The tensor-core kernel, the FFMA kernel and the oracle all add the (e - z)^2 terms in double, in different orders
+# (per-thread row sums, per-CTA partials).  The tolerance leaves room for a per-row relative error of 16 * 2^-24 ~ 1e-6.
 SSE_RTOL = 2e-6
 
 
@@ -108,7 +108,7 @@ def test_tc_kernel_large_n_matches_exact_kernel(K, kind):
 @pytest.mark.parametrize("N,K,D,kernel", [(5000, 512, 64, "auto"), (777, 1000, 64, "auto"), (640, 512, 64, "exact"), (300, 96, 32, "auto")])
 def test_deferred_sse_reduction(N, K, D, kernel):
     """vqb_vq_forward_deferred_f32 + vqb_vq_reduce_sse_f32 (the reduction may run later / on a side stream)
-    give exactly the outputs of vqb_vq_forward_f32, on the tcgen05 kernel and on the exact FFMA kernel."""
+    give exactly the outputs of vqb_vq_forward_f32, on the wgmma kernel and on the exact FFMA kernel."""
     from vqvae_b200 import ops
     rng = np.random.RandomState(N + K)
     z = torch.from_numpy(rng.standard_normal((N, D)).astype(np.float32)).cuda()

@@ -1,5 +1,5 @@
 """Host-side logic of vqvae_b200.HostPipeline that needs no GPU: argument checks and the packed-scalar
-detection (the kernels themselves are covered by tests/test_gpu_pipeline.py on the B200)."""
+detection (the kernels themselves are covered by tests/test_gpu_pipeline.py on an H100)."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""vqvae_b200 -- B200-native (sm_100a) VQ-VAE inference hot path.
+"""vqvae_b200 -- H100-native (sm_90a) VQ-VAE inference hot path.
 
 Hand-written CUDA kernels behind a C ABI (include/vqvae_b200.h), plus the host-side
 mirror of the reference's nn.Module API (vqvae_b200.modules; re-exported by the

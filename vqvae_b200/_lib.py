@@ -1,6 +1,6 @@
 """ctypes binding of include/vqvae_b200.h (the C-ABI boundary).
 
-The library is built in-tree by vqvae_b200/build.py (nvcc, sm_100a).  Loading never
+The library is built in-tree by vqvae_b200/build.py (nvcc, sm_90a).  Loading never
 falls back to anything: if the shared object is missing the import of the product
 fails loudly.
 """

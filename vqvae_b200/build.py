@@ -1,4 +1,4 @@
-"""In-tree nvcc build of libvqvae_b200.so (sm_100a only; no torch in the library)."""
+"""In-tree nvcc build of libvqvae_b200.so (sm_90a only; no torch in the library)."""
 import glob
 import os
 import shutil
@@ -33,9 +33,9 @@ def build(force: bool = False, verbose: bool = False) -> str:
     for src in sources():
         obj = os.path.join(LIB_DIR, os.path.basename(src)[:-3] + ".o")
         objs.append(obj)
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
                "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c", src, "-o", obj]
-        if os.environ.get("VQB_DIAG") == "1":        # diagnostic build: env knobs + in-kernel timelines (tools/diag)
+        if os.environ.get("VQB_DIAG") == "1":        # diagnostic build: environment knobs for experiments
             cmd.insert(1, "-DVQB_DIAG=1")
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     log = []
@@ -44,7 +44,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         log.append(f"== {os.path.basename(src)}\n{out}")
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed for {src}:\n{out}")
-    link = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs + \
+    link = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + objs + \
         ["-cudart", "static"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

@@ -4,46 +4,18 @@
 #include "common.cuh"
 
 size_t vq_exact_workspace_bytes(int K);
-int launch_vq_exact(const float *z, const float *E, long long N, int K, int D, long long *idx, float *zq,
+int launch_vq_exact(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, int zq_bf16,
                     double *sse, int *hist, void *ws, cudaStream_t s);
-
-size_t vq_tc_workspace_bytes(int K);
-bool vq_tc_supported(long long N, int K, int D);
-size_t vq_ws_marker_offset(int K);
-int launch_vq_reduce_sse(const void *ws, int K, double *sse, cudaStream_t s);
-int launch_vq_tc(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, double *sse,
-                 int *hist, void *ws, float *dbg, int defer, int zq_bf16, cudaStream_t s);
-int launch_conv_in_tc_ex(const float *x, const float *wp, const float *bias, void *y, int B, int H, int W, int Cout,
-                         int relu, int out_bf16, cudaStream_t s);
-
-bool conv_in_bf16_persistent_ok(int H, int W, const void *x);
-int launch_conv_in_bf16_persistent(const float *x, const float *wp, const float *bias, void *y, int B, int H, int W, int relu,
-                                   cudaStream_t s);
-bool vq2_supported(long long N, int K, int D);
-int launch_vq2(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, double *sse, int *hist,
-               void *ws, int defer, int zq_bf16, cudaStream_t s);
-int launch_conv_in_k4s2(const float *x, const float *wp, const float *bias, float *y, int B, int Cin, int H, int W,
-                        int Cout, int relu, cudaStream_t s);
+int launch_conv_in_k4s2(const float *x, const float *wp, const float *bias, void *y, int out_bf16, int B, int Cin, int H,
+                        int W, int Cout, int relu, cudaStream_t s);
 int launch_convt_out_k4s2(const float *x, const float *wp, const float *bias, float *y, int B, int Cin, int H, int W,
                           int Cout, int relu, cudaStream_t s);
-bool res_tc_supported(int C, int Cmid, const void *r, const void *out);
-int launch_res_tc(const float *r, const float *w1_tc, const float *w2_tc, float *out, int B, int H, int W, int C,
-                  int Cmid, int relu_out, int napp, cudaStream_t s);
-bool conv_in_tc_supported(int Cin, int Cout, int H, int W, const void *y);
-int launch_conv_in_tc(const float *x, const float *wp, const float *bias, float *y, int B, int H, int W, int Cout,
-                      int relu, cudaStream_t s);
-bool convt_shuffle_supported(int Cin, int Cout, const void *in, const void *out);
-int launch_convt_shuffle(const float *in, const float *w_shuffle, const float *bias, float *out, int B, int Cin, int H,
-                         int W, int Cout, int relu, cudaStream_t s);
-bool conv_halo_supported(const ConvLaunch &p);
-int launch_conv_halo(const ConvLaunch &p, const float *w_tc, cudaStream_t s);
+#include "wgconv.h"
+bool vq_tc_supported(long long N, int K, int D);
+int launch_vq_tc(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, int zq_bf16, double *sse,
+                 int *hist, void *ws, float *dbg, cudaStream_t s);
 bool conv_tc_supported(const ConvLaunch &p);
 int launch_conv_tc(const ConvLaunch *ph, int nph, const float *w_tc, int total_taps, cudaStream_t s);
-
-int vqb_halo_wp() {
-    static const int wp = [] { const char *e = vqb_getenv("VQB_HALO_WP"); return (e && atoi(e) == 16) ? 16 : 10; }();
-    return wp;
-}
 
 int vqb_pdl_enabled() {
     static int on = -1;
@@ -55,7 +27,7 @@ int vqb_pdl_enabled() {
 }
 
 unsigned long long g_vqb_launches = 0;
-static int g_vq_kernel = 0;   // 0 auto, 1 exact FFMA kernel, 2 tcgen05 kernel (vq2.cu), 3 round-1 tcgen05 kernel (vq_tc.cu)
+static int g_vq_kernel = 0;   // 0 auto (tensor-core kernel when D == 64), 1 exact FFMA kernel, 2 / 3 tensor-core kernel
 extern "C" int vqb_set_vq_kernel(int which) {
     if (which < 0 || which > 3) return VQB_ERR_BAD_ARG;
     g_vq_kernel = which;
@@ -72,7 +44,7 @@ extern "C" const char *vqb_error_string(int code) {
     switch (code) {
         case VQB_OK: return "success";
         case VQB_ERR_BAD_ARG: return "bad argument (null pointer, non-positive size or bad enum)";
-        case VQB_ERR_UNSUPPORTED: return "shape not supported by the sm_100a kernels";
+        case VQB_ERR_UNSUPPORTED: return "shape not supported by the sm_90a kernels";
         case VQB_ERR_WORKSPACE: return "workspace too small";
         case VQB_ERR_NO_DEVICE: return "no CUDA device";
         case VQB_ERR_ALIGNMENT: return "pointer not 16-byte aligned";
@@ -121,33 +93,31 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     const int OW = transposed ? (W - 1) * stride - 2 * pad + kw : (W + 2 * pad - kw) / stride + 1;
     if (OH <= 0 || OW <= 0) return VQB_ERR_BAD_ARG;
 
-    // the two HBM-bound end layers have dedicated kernels (conv_edge.cu)
+    // the two end layers: the output ConvTranspose2d (Cout <= 4) as one wgmma GEMM over the 3x3 input neighbourhood
+    // (N = 16 columns, pixel shuffle); the input conv (Cin = 3: K = 48 fp32 values per pixel straight from the NCHW
+    // image, HBM bound) and the fp32 mode on dedicated CUDA-core kernels (conv_edge.cu)
     if (kh == 4 && kw == 4 && stride == 2 && pad == 1 && !skip) {
-        if (!transposed && precision != VQB_FP32 && in_layout == VQB_NCHW && out_layout == VQB_NHWC &&
-            conv_in_tc_supported(Cin, Cout, H, W, out)) {     // tcgen05 with a hand-built im2col tile
-            const int rc = launch_conv_in_tc(in, w_packed, bias, out, B, H, W, Cout, relu, s);
+        if (transposed && precision != VQB_FP32 && in_layout == VQB_NHWC && out_layout == VQB_NCHW &&
+            convt_shuffle_supported(Cin, Cout)) {
+            const int rc = launch_convt_shuffle_wg(in, w_packed + (size_t)2 * 16 * Cin * Cout, bias, out, B, Cin, H, W, Cout,
+                                                   relu, s);
             if (rc != VQB_ERR_UNSUPPORTED) return rc;
         }
         if (!transposed && Cin == 3 && Cout % 32 == 0 && in_layout == VQB_NCHW && out_layout == VQB_NHWC &&
             H % 2 == 0 && W % 2 == 0 && (size_t)16 * Cin * Cout * 4 <= 48 * 1024)
-            return launch_conv_in_k4s2(in, w_packed, bias, out, B, Cin, H, W, Cout, relu, s);
-        if (transposed && precision != VQB_FP32 && in_layout == VQB_NHWC && out_layout == VQB_NCHW &&
-            convt_shuffle_supported(Cin, Cout, in, out)) {    // tcgen05: one 3x3-neighbourhood GEMM + pixel shuffle
-            const int rc = launch_convt_shuffle(in, w_packed + (size_t)2 * 16 * Cin * Cout, bias, out, B, Cin, H, W, Cout, relu, s);
-            if (rc != VQB_ERR_UNSUPPORTED) return rc;
-        }
+            return launch_conv_in_k4s2(in, w_packed, bias, out, 0, B, Cin, H, W, Cout, relu, s);
         if (transposed && Cout == 3 && Cin % 4 == 0 && Cin <= 128 && ((Cin / 4) & (Cin / 4 - 1)) == 0 &&
             in_layout == VQB_NHWC && out_layout == VQB_NCHW)
             return launch_convt_out_k4s2(in, w_packed, bias, out, B, Cin, H, W, Cout, relu, s);
     }
 
-    ConvLaunch p;
+    ConvLaunch p = {};
     p.in = in; p.w = w_packed; p.bias = bias; p.skip = skip; p.out = out;
     p.B = B; p.Cin = Cin; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu;
     set_strides(in_layout, Cin, H, W, p.in_sn, p.in_sh, p.in_sw, p.in_sc);
     set_strides(out_layout, Cout, OH, OW, p.out_sn, p.out_sh, p.out_sw, p.out_sc);
     const bool small = (Cout <= 4);
-    const float *w_tc = w_packed + (size_t)kh * kw * Cin * Cout;   // K-major copy for the tcgen05 path
+    const float *w_tc = w_packed + (size_t)kh * kw * Cin * Cout;   // K-major copy for the wgmma path
     const bool want_tc = precision != VQB_FP32;
 
     if (!transposed || stride == 1) {
@@ -162,12 +132,8 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
                 p.tap_dy[t] = transposed ? pad - r : r - pad;
                 p.tap_dx[t] = transposed ? pad - c : c - pad;
             }
-        // a tensor-core launcher that cannot fit the shape (shared memory, ring depth) answers VQB_ERR_UNSUPPORTED
-        // before launching anything: fall through to the next kernel that can run it
-        if (want_tc && conv_halo_supported(p)) {
-            const int rc = launch_conv_halo(p, w_tc, s);
-            if (rc != VQB_ERR_UNSUPPORTED) return rc;
-        }
+        // the tensor-core launcher answers VQB_ERR_UNSUPPORTED before launching anything when it cannot take the
+        // shape (layouts, channel counts, step table): the FFMA kernels run it then
         if (want_tc && conv_tc_supported(p)) {
             const int rc = launch_conv_tc(&p, 1, w_tc, kh * kw, s);
             if (rc != VQB_ERR_UNSUPPORTED) return rc;
@@ -221,94 +187,64 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
 extern "C" size_t vqb_vq_workspace_bytes(int64_t N, int K, int D) {
     (void)N; (void)D;
     if (K <= 0) return 0;
-    return vq_ws_marker_offset(K) + 256;
+    return vq_exact_workspace_bytes(K);
 }
 
-// [exact / tcgen05 kernel workspace (whichever is larger)][256 B: deferred-reduction marker]
-size_t vq_ws_marker_offset(int K) {
-    const size_t a = vq_exact_workspace_bytes(K), b = vq_tc_workspace_bytes(K);
-    return ((a > b ? a : b) + 255) / 256 * 256;
-}
-
-static int vq_forward_impl(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx, float *zq,
-                           double *sse, int32_t *hist, void *workspace, size_t workspace_bytes, int defer,
-                           void *stream);
-
-extern "C" int vqb_vq_forward_deferred_f32(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx,
-                                           float *zq, double *sse, int32_t *hist, void *workspace,
-                                           size_t workspace_bytes, void *stream) {
-    return vq_forward_impl(z, codebook, N, K, D, idx, zq, sse, hist, workspace, workspace_bytes, 1, stream);
-}
-
-extern "C" int vqb_vq_reduce_sse_f32(const void *workspace, int64_t N, int K, int D, double *sse, void *stream) {
-    if (!workspace || !sse || N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
-    return launch_vq_reduce_sse(workspace, K, sse, (cudaStream_t)stream);
+static int vq_forward_impl(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx, void *zq,
+                           int zq_bf16, double *sse, int32_t *hist, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!z || !codebook || !idx || !zq || !sse || !hist || !workspace) return VQB_ERR_BAD_ARG;
+    if (N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
+    if (D % 4 != 0) return VQB_ERR_UNSUPPORTED;
+    const bool tc_ok = vq_tc_supported(N, K, D);
+    if (g_vq_kernel >= 2 && !tc_ok) return VQB_ERR_UNSUPPORTED;
+    if (workspace_bytes < vqb_vq_workspace_bytes(N, K, D)) return VQB_ERR_WORKSPACE;
+    const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(codebook) |
+                         reinterpret_cast<uintptr_t>(zq) | reinterpret_cast<uintptr_t>(workspace);
+    if (al & 15) return VQB_ERR_ALIGNMENT;
+    if (tc_ok && g_vq_kernel != 1)
+        return launch_vq_tc(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, zq_bf16, sse, hist, workspace,
+                            nullptr, (cudaStream_t)stream);
+    return launch_vq_exact(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, zq_bf16, sse, hist, workspace,
+                           (cudaStream_t)stream);
 }
 
 extern "C" int vqb_vq_forward_f32(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx,
                                   float *zq, double *sse, int32_t *hist, void *workspace,
                                   size_t workspace_bytes, void *stream) {
-    return vq_forward_impl(z, codebook, N, K, D, idx, zq, sse, hist, workspace, workspace_bytes, 0, stream);
+    return vq_forward_impl(z, codebook, N, K, D, idx, zq, 0, sse, hist, workspace, workspace_bytes, stream);
 }
 
-static int vq_forward_impl(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx, float *zq,
-                           double *sse, int32_t *hist, void *workspace, size_t workspace_bytes, int defer,
-                           void *stream) {
-    if (!z || !codebook || !idx || !zq || !sse || !hist || !workspace) return VQB_ERR_BAD_ARG;
-    if (N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
-    if (D % 4 != 0) return VQB_ERR_UNSUPPORTED;
-    if (workspace_bytes < vqb_vq_workspace_bytes(N, K, D)) return VQB_ERR_WORKSPACE;
-    const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(codebook) |
-                         reinterpret_cast<uintptr_t>(zq) | reinterpret_cast<uintptr_t>(workspace);
-    if (al & 15) return VQB_ERR_ALIGNMENT;
-    const bool tc_ok = vq_tc_supported(N, K, D), v2_ok = vq2_supported(N, K, D);
-    if (g_vq_kernel == 2 && !v2_ok) return VQB_ERR_UNSUPPORTED;
-    if (g_vq_kernel == 3 && !tc_ok) return VQB_ERR_UNSUPPORTED;
-    if (v2_ok && (g_vq_kernel == 0 || g_vq_kernel == 2))
-        return launch_vq2(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, sse, hist, workspace, defer, 0,
-                          (cudaStream_t)stream);
-    if (tc_ok && g_vq_kernel != 1)
-        return launch_vq_tc(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, sse, hist, workspace,
-                            nullptr, defer, 0, (cudaStream_t)stream);
-    const int rc = launch_vq_exact(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, sse, hist, workspace,
-                                   (cudaStream_t)stream);
-    if (rc || !defer) return rc;
-    // sse is final: nothing pending for vqb_vq_reduce_sse_f32
-    return vqb_cuda_status(cudaMemsetAsync(reinterpret_cast<unsigned char *>(workspace) + vq_ws_marker_offset(K), 0, 4,
-                                           (cudaStream_t)stream));
+// The exact kernel finishes the SSE inside its own launch sequence, so the deferred variant has nothing left
+// for vqb_vq_reduce_sse_f32 to do; both keep the contract of the header.
+extern "C" int vqb_vq_forward_deferred_f32(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx,
+                                           float *zq, double *sse, int32_t *hist, void *workspace,
+                                           size_t workspace_bytes, void *stream) {
+    return vq_forward_impl(z, codebook, N, K, D, idx, zq, 0, sse, hist, workspace, workspace_bytes, stream);
+}
+
+extern "C" int vqb_vq_reduce_sse_f32(const void *workspace, int64_t N, int K, int D, double *sse, void *stream) {
+    (void)stream;
+    if (!workspace || !sse || N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
+    return 0;
 }
 
 // VQB_BF16 pipeline: same contract as vqb_vq_forward_deferred_f32 (fp32 z in, bit-exact idx) but z_q leaves as bf16
-// rows for the decoder's first conv; tcgen05 kernel only (D == 64).
+// rows for the decoder's first conv.
 extern "C" int vqb_vq_forward_bf16zq_f32(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx,
                                          void *zq_bf16, double *sse, int32_t *hist, void *workspace,
                                          size_t workspace_bytes, void *stream) {
-    if (!z || !codebook || !idx || !zq_bf16 || !sse || !hist || !workspace) return VQB_ERR_BAD_ARG;
-    if (N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
-    if (workspace_bytes < vqb_vq_workspace_bytes(N, K, D)) return VQB_ERR_WORKSPACE;
-    const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(codebook) |
-                         reinterpret_cast<uintptr_t>(zq_bf16) | reinterpret_cast<uintptr_t>(workspace);
-    if (al & 15) return VQB_ERR_ALIGNMENT;
-    if (vq2_supported(N, K, D) && g_vq_kernel != 3)
-        return launch_vq2(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq_bf16, sse, hist, workspace, 1, 1,
-                          (cudaStream_t)stream);
-    if (!vq_tc_supported(N, K, D)) return VQB_ERR_UNSUPPORTED;
-    return launch_vq_tc(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq_bf16, sse, hist, workspace, nullptr, 1, 1,
-                        (cudaStream_t)stream);
+    return vq_forward_impl(z, codebook, N, K, D, idx, zq_bf16, 1, sse, hist, workspace, workspace_bytes, stream);
 }
 
-// encoder.py:29-31 in the VQB_BF16 pipeline: fp32 NCHW image in, bf16 NHWC activation out (Cout == 64); the 48-tap
-// contraction itself runs as kind::tf32 on the fp32 pixels.  w_packed: vqb_pack_conv_weight_f32 of the layer.
+// encoder.py:29-31 in the VQB_BF16 pipeline: fp32 NCHW image in, bf16 NHWC activation out (Cout == 64), fp32 FFMA
+// arithmetic (conv_edge.cu).  w_packed: vqb_pack_conv_weight_f32 of the layer.
 extern "C" int vqb_conv_in_bf16(const float *x, const float *w_packed, const float *bias, void *out, int B, int H, int W,
                                 int Cout, int relu, void *stream) {
     if (!x || !w_packed || !out) return VQB_ERR_BAD_ARG;
     if (B <= 0 || H <= 0 || W <= 0 || Cout <= 0) return VQB_ERR_BAD_ARG;
-    if (!conv_in_tc_supported(3, Cout, H, W, out) || Cout != 64) return VQB_ERR_UNSUPPORTED;
-    if (conv_in_bf16_persistent_ok(H, W, x)) {          // one CTA per SM, pipelined over tiles (conv_in_bf16.cu)
-        const int rc = launch_conv_in_bf16_persistent(x, w_packed, bias, out, B, H, W, relu, (cudaStream_t)stream);
-        if (rc != VQB_ERR_UNSUPPORTED) return rc;
-    }
-    return launch_conv_in_tc_ex(x, w_packed, bias, out, B, H, W, Cout, relu, 1, (cudaStream_t)stream);
+    if (Cout != 64) return VQB_ERR_UNSUPPORTED;
+    if ((reinterpret_cast<uintptr_t>(out) & 15)) return VQB_ERR_ALIGNMENT;
+    return launch_conv_in_k4s2(x, w_packed, bias, out, 1, B, 3, H, W, Cout, relu, (cudaStream_t)stream);
 }
 
 extern "C" int vqb_debug_vq_scores_f32(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx,
@@ -317,9 +253,14 @@ extern "C" int vqb_debug_vq_scores_f32(const float *z, const float *codebook, in
     if (!z || !codebook || !idx || !zq || !sse || !hist || !workspace || !scores) return VQB_ERR_BAD_ARG;
     if (!vq_tc_supported(N, K, D)) return VQB_ERR_UNSUPPORTED;
     if (workspace_bytes < vqb_vq_workspace_bytes(N, K, D)) return VQB_ERR_WORKSPACE;
-    return launch_vq_tc(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, sse, hist, workspace, scores, 0, 0,
+    return launch_vq_tc(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, 0, sse, hist, workspace, scores,
                         (cudaStream_t)stream);
 }
+
+// In-kernel timeline readers of ABI version 2: the sm_90a kernels record none, so they answer VQB_ERR_UNSUPPORTED.
+extern "C" int vqb_debug_read_trace(unsigned long long *, int) { return VQB_ERR_UNSUPPORTED; }
+extern "C" int vqb_debug_read_trace_vq(unsigned long long *, int) { return VQB_ERR_UNSUPPORTED; }
+extern "C" int vqb_debug_read_cta_times(unsigned long long *, int) { return VQB_ERR_UNSUPPORTED; }
 
 extern "C" int vqb_residual_layer_f32(const float *r, const float *w1_packed, const float *w2_packed, float *out,
                                       float *tmp, int B, int H, int W, int C, int Cmid, int relu_out, int precision,
@@ -328,12 +269,13 @@ extern "C" int vqb_residual_layer_f32(const float *r, const float *w1_packed, co
     if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cmid <= 0) return VQB_ERR_BAD_ARG;
     if (precision < VQB_FP32 || precision > VQB_BF16) return VQB_ERR_BAD_ARG;
     if (precision == VQB_BF16) return VQB_ERR_UNSUPPORTED;      // see vqb_residual_layer_bf16
-    if (precision != VQB_FP32 && res_tc_supported(C, Cmid, r, out)) {
-        const int rc = launch_res_tc(r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
+    if (precision == VQB_TF32 && res_wg_supported(C, Cmid)) {      // one wgmma launch, the intermediate stays on chip
+        const int rc = launch_res_wg(r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
                                      relu_out, 1, (cudaStream_t)stream);
-        if (rc != VQB_ERR_UNSUPPORTED) return rc;               // (e.g. C = 256, Cmid = 128: shared memory) -> generic path
+        if (rc != VQB_ERR_UNSUPPORTED) return rc;
     }
-    // two launches through the generic path (residual.py:20-24 then :23-24,:28)
+    // two launches (residual.py:20-24 then :23-24,:28)
+
     int rc = vqb_conv2d_f32(r, w1_packed, nullptr, nullptr, tmp, B, C, H, W, Cmid, 3, 3, 1, 1, 0, VQB_NHWC, VQB_NHWC, 1,
                             precision, stream);
     if (rc) return rc;
@@ -349,11 +291,10 @@ extern "C" int vqb_residual_stack_f32(const float *r, const float *w1_packed, co
     if (n_layers > 1 && !scratch) return VQB_ERR_BAD_ARG;
     if (precision < VQB_FP32 || precision > VQB_BF16) return VQB_ERR_BAD_ARG;
     if (precision == VQB_BF16) return VQB_ERR_UNSUPPORTED;
-    static const bool fuse = [] { const char *e = vqb_getenv("VQB_RES_FUSE"); return !(e && e[0] == '0'); }();
-    if (fuse && n_layers > 1 && precision != VQB_FP32 && res_tc_supported(C, Cmid, r, out)) {
-        // all applications in ONE launch: the activation never leaves shared memory between them
-        const int rc = launch_res_tc(r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C,
-                                     Cmid, 1, n_layers, (cudaStream_t)stream);
+    if (n_layers > 1 && precision == VQB_TF32 && res_wg_supported(C, Cmid)) {
+        // all applications in ONE launch when a tile holds whole images (answers VQB_ERR_UNSUPPORTED otherwise)
+        const int rc = launch_res_wg(r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
+                                     1, n_layers, (cudaStream_t)stream);
         if (rc != VQB_ERR_UNSUPPORTED) return rc;
     }
     // one launch per application, ping-ponging so that the last one lands in `out`

@@ -1,51 +1,9 @@
-// bf16_common.cuh -- helpers shared by the bf16 (tcgen05 kind::f16) kernels: hconv.cu, res_bf16.cu.
+// bf16_common.cuh -- helpers shared by the bf16 pipeline's sources (hconv.cu, conv_edge.cu).
 #pragma once
 #include <cuda_bf16.h>
 
-#include "ptx.cuh"
 
 namespace {
-
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap *m, uint32_t bar, int c0, int c1, int c2,
-                                            int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::
-            "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-
-__device__ __forceinline__ void mma_bf16_w(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                           uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-        "}" ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float *v) {
-    uint32_t *r = reinterpret_cast<uint32_t *>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :: "memory");
-}
-
-// one 32-byte (full-sector) store per thread: sm_100 has 256-bit global stores (STG.E.ENL2.256)
-__device__ __forceinline__ void st_global_256(void *p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f,
-                                              uint32_t g, uint32_t h) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::
-                     "l"(p), "r"(a), "r"(b), "r"(c), "r"(d), "r"(e), "r"(f), "r"(g), "r"(h) : "memory");
-}
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);

@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations of the sm_100a VQ-VAE kernels (internal).
+// common.cuh -- shared declarations of the sm_90a VQ-VAE kernels (internal).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,8 +8,7 @@
 #define VQB_MAX_TAPS 16
 
 // Experiment / diagnostic knobs (VQB_* environment variables, the work-skipping VQB_TC_FLAGS bits, in-kernel
-// timelines) exist only in a library built with -DVQB_DIAG=1 (VQB_DIAG=1 python -m vqvae_b200.build, used by
-// tools/diag).  The release library never reads the environment: vqb_getenv() is a constant nullptr there and the
+// timelines) exist only in a library built with -DVQB_DIAG=1 (VQB_DIAG=1 python -m vqvae_b200.build).  The release library never reads the environment: vqb_getenv() is a constant nullptr there and the
 // flag tests in the kernels fold away.
 #ifndef VQB_DIAG
 #define VQB_DIAG 0
@@ -45,10 +44,9 @@ extern unsigned long long g_vqb_launches;
 #define VQB_COUNT_LAUNCH(n) (g_vqb_launches += (n))
 
 // Programmatic dependent launch: the next kernel of the layer chain may start its prologue (barrier init,
-// TMEM allocation, tensor-map prefetch) while this one drains; it blocks in pdl_wait() until the previous
+// tensor-map prefetch) while this one drains; it blocks in pdl_wait() until the previous
 // grid has completed and its writes are visible.  VQB_PDL=0 in the environment disables the attribute.
 int vqb_pdl_enabled();
-int vqb_halo_wp();           // halo tile width of conv_halo.cu / res_tc.cu: 10, or 16 with VQB_HALO_WP=16
 #ifdef __CUDACC__
 #include <utility>
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

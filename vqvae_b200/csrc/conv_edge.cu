@@ -1,8 +1,8 @@
-// conv_edge.cu -- the two HBM-bound end layers of the hot path (sm_100a, CUDA cores).
+// conv_edge.cu -- the two HBM-bound end layers of the hot path (sm_90a, CUDA cores).
 //
 //   conv_in_k4s2:   encoder.py:29-31  Conv2d(3 -> 64, k4 s2 p1) + ReLU, reads the NCHW module
-//                   input, writes NHWC.  K_red = 48: far too thin for a tensor-core tile
-//                   (SURVEY 7.3.4); arithmetic intensity ~20 F/B.
+//                   input, writes NHWC (fp32, or bf16 for the bf16 pipeline).  K_red = 48: far too thin for a
+//                   tensor-core tile (SURVEY 7.3.4); arithmetic intensity ~20 F/B.
 //   convt_out_k4s2: decoder.py:34-35  ConvTranspose2d(64 -> 3, k4 s2 p1), reads NHWC, writes
 //                   the NCHW module output.  One thread owns one INPUT pixel and produces its
 //                   2x2 output block for every output channel from the 3x3 input
@@ -10,16 +10,17 @@
 // Both keep the (tiny) weight tensor in shared memory, read activations through L1 and
 // write fully coalesced rows.  fp32 FFMA arithmetic in every precision mode.
 #include "common.cuh"
+#include "bf16_common.cuh"
 
 namespace {
 
 // ------------------------------------------------------------------ Conv2d(Cin<=4 -> Cout), k4 s2 p1
 // thread = (output pixel, group of 32 output channels); warp = 32 consecutive pixels of one
 // channel group, so weight reads are warp-wide broadcasts.
-template <int CIN>
+template <int CIN, bool OUT_BF16>
 __global__ void __launch_bounds__(256, 2)
 conv_in_k4s2_kernel(const float *__restrict__ x, const float *__restrict__ wp, const float *__restrict__ bias,
-                    float *__restrict__ y, int B, int H, int W, int Cout, int relu) {
+                    void *__restrict__ y, int B, int H, int W, int Cout, int relu) {
     extern __shared__ __align__(16) float wsm[];          // [16*CIN][Cout]
     const int K = 16 * CIN;
     for (int i = threadIdx.x; i < K * Cout; i += blockDim.x) wsm[i] = __ldg(wp + i);
@@ -65,12 +66,20 @@ conv_in_k4s2_kernel(const float *__restrict__ x, const float *__restrict__ wp, c
             }
         }
     }
-    float4 *dst = reinterpret_cast<float4 *>(y + pix * Cout + cg * 32);
+    if (relu) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        float4 o = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-        if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-        dst[j] = o;
+        for (int j = 0; j < 32; ++j) acc[j] = fmaxf(acc[j], 0.f);
+    }
+    if constexpr (OUT_BF16) {
+        uint4 *dst = reinterpret_cast<uint4 *>(reinterpret_cast<__nv_bfloat16 *>(y) + pix * Cout + cg * 32);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            dst[j] = make_uint4(pack_bf16(acc[8 * j], acc[8 * j + 1]), pack_bf16(acc[8 * j + 2], acc[8 * j + 3]),
+                                pack_bf16(acc[8 * j + 4], acc[8 * j + 5]), pack_bf16(acc[8 * j + 6], acc[8 * j + 7]));
+    } else {
+        float4 *dst = reinterpret_cast<float4 *>(reinterpret_cast<float *>(y) + pix * Cout + cg * 32);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) dst[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
     }
 }
 
@@ -173,9 +182,10 @@ convt_out_k4s2_kernel(const float *__restrict__ x, const float *__restrict__ wk,
 
 }  // namespace
 
-// Conv2d(Cin in {1..4} -> Cout % 32 == 0), k4 s2 p1, NCHW in, NHWC out.  wp = FFMA packing.
-int launch_conv_in_k4s2(const float *x, const float *wp, const float *bias, float *y, int B, int Cin, int H, int W,
-                        int Cout, int relu, cudaStream_t s) {
+// Conv2d(Cin in {1..4} -> Cout % 32 == 0), k4 s2 p1, NCHW in, NHWC out (fp32, or bf16 when out_bf16).
+// wp = FFMA packing.
+int launch_conv_in_k4s2(const float *x, const float *wp, const float *bias, void *y, int out_bf16, int B, int Cin, int H,
+                        int W, int Cout, int relu, cudaStream_t s) {
     if (Cin != 3 || Cout % 32 != 0 || H % 2 || W % 2) return VQB_ERR_UNSUPPORTED;
     const size_t smem = (size_t)16 * Cin * Cout * sizeof(float);
     if (smem > 48 * 1024) return VQB_ERR_UNSUPPORTED;
@@ -183,7 +193,10 @@ int launch_conv_in_k4s2(const float *x, const float *wp, const float *bias, floa
     const long long warps = (npix + 31) / 32 * (Cout / 32);
     const long long blocks = (warps + 7) / 8;
     if (blocks > 0x7fffffffLL) return VQB_ERR_UNSUPPORTED;
-    conv_in_k4s2_kernel<3><<<(unsigned)blocks, 256, smem, s>>>(x, wp, bias, y, B, H, W, Cout, relu);
+    if (out_bf16)
+        conv_in_k4s2_kernel<3, true><<<(unsigned)blocks, 256, smem, s>>>(x, wp, bias, y, B, H, W, Cout, relu);
+    else
+        conv_in_k4s2_kernel<3, false><<<(unsigned)blocks, 256, smem, s>>>(x, wp, bias, y, B, H, W, Cout, relu);
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -198,7 +211,7 @@ int launch_convt_out_k4s2(const float *x, const float *wp, const float *bias, fl
     const long long npix = (long long)B * H * W;
     const long long warps = (npix + (32 / L) - 1) / (32 / L);
     long long blocks = (warps + 7) / 8;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (blocks > (long long)sms * 2) blocks = (long long)sms * 2;       // persistent: weights staged once per CTA

@@ -1,9 +1,9 @@
-// conv_ffma.cu -- fp32 (FFMA, CUDA-core) gather-form convolution for sm_100a.
+// conv_ffma.cu -- fp32 (FFMA, CUDA-core) gather-form convolution for sm_90a.
 //
 // This is the VQB_FP32 arithmetic of vqb_conv2d_f32: every product and every
 // accumulation is fp32, like the reference's CPU path (oneDNN), so it is the path
 // the parity tests hold to the tightest tolerance, the fallback for shapes the
-// tcgen05 implicit-GEMM kernels do not cover, and their on-GPU cross-check.
+// wgmma implicit-GEMM kernels do not cover, and their on-GPU cross-check.
 // Replaces nn.Conv2d / nn.ConvTranspose2d call sites: encoder.py:29-36,
 // residual.py:20-24, vqvae.py:16-17, decoder.py:28-35.
 //

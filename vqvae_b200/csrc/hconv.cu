@@ -1,30 +1,16 @@
-// hconv.cu -- persistent tcgen05 implicit-GEMM convolution on bf16 activations (VQB_BF16 mode), sm_100a.
-//
-// One kernel for every tensor-core conv layer of the hot path when the activations between layers are bf16 NHWC:
-//   encoder.py:32-34  Conv2d k4 s2 p1        (space-to-depth view: a 2x2-tap conv on four parity planes)
+// hconv.cu -- the bf16 pipeline's convolution layers (VQB_BF16 mode): weight packing plans and the entry points
+// vqb_conv2d_bf16 / vqb_residual_layer_bf16, all computed by the wgmma implicit-GEMM kernel of wgconv.cu on bf16 NHWC
+// activations with fp32 accumulation:
+//   encoder.py:32-34  Conv2d k4 s2 p1          (taps read through stride-2 element strides of the input tensor map)
 //   encoder.py:35-36  Conv2d k3 s1 p1
-//   vqvae.py:16-17    Conv2d k1               (fp32 output: z_e feeds the bit-exact VQ)
+//   vqvae.py:16-17    Conv2d k1                 (fp32 output: z_e feeds the bit-exact VQ)
 //   decoder.py:28-29  ConvTranspose2d k3 s1 p1
-//   decoder.py:31-33  ConvTranspose2d k4 s2 p1 (two passes = output row parities; each pass accumulates both output
-//                                               column parities side by side: shift dx = 0 feeds both -> one N = 2 Cout MMA)
+//   decoder.py:31-33  ConvTranspose2d k4 s2 p1  (four sub-pixel phases of 4 taps in one launch)
 //   decoder.py:34-35  ConvTranspose2d k4 s2 p1 to <= 4 channels (one 3x3-neighbourhood GEMM, N = 16, pixel-shuffle
-//                                               epilogue writing the NCHW fp32 module output)
-//
-// Shape of the kernel (measured facts behind it: profiles/r02_ubench_mma_rate.txt, r02_ubench_l2_stream.txt):
-//   * ONE CTA per SM, persistent over tiles of TW x BH x BN pixels (TW = 16 -> two M = 128 tiles that share every
-//     weight stage; 8 when the image is narrower).  An M128 N128 K16 bf16 MMA issued from one converged warp runs at
-//     the 64-cycle floor from a single CTA (8158 flop/cycle/SM), so no cta_group::2 is needed for peak; N = 64 costs
-//     48 cycles and N = 32 costs 40, which is why the k4s2 transposed conv pairs its column parities.
-//   * the input tile is loaded ONCE per 64-channel chunk with its 1-pixel halo (5-D TMA box, 128-byte swizzle) and
-//     the taps are shifted UMMA descriptors into it (conv_halo.cu's trick; the swizzle phase comes from absolute
-//     shared-memory address bits so operand windows may start on any 128-byte row).  No im2col anywhere.
-//   * weights stream through a ring of 16 KB stages (one L2-resident weight set read by all SMs streams at
-//     121 GB/s per SM, 18 TB/s chip-wide; a 256-pixel tile needs 61 GB/s at the full MMA rate) -- or stay resident
-//     when the whole set fits the ring.
-//   * fp32 accumulators double-buffered in TMEM (2 x 256 columns): 8 epilogue warps drain tile t (tcgen05.ld ->
-//     +bias -> ReLU -> bf16 pack -> 16-byte NHWC stores) under the MMAs of tile t+1.
-//   * warps: 0 = halo producer, 1 = MMA issuer (converged warp, elected lane), 2 = TMEM allocator, 3 = weight
-//     producer, 4-11 = epilogue.
+//                                                epilogue writing the NCHW fp32 module output)
+//   residual.py:18-29 one ResidualLayer: 3x3 conv, ReLU and 1x1 conv chained inside one CTA per tile
+// A packed weight is one 128-byte row of 64 bf16 input channels per (k-step, output column) in plan order, followed
+// by the plan's row table (RowDesc per row); the kernel reads the rows of each k-step as one TMA box.
 #include <cuda_bf16.h>
 
 #include <cstdlib>
@@ -32,420 +18,18 @@
 #include <vector>
 
 #include "common.cuh"
-#include "ptx.cuh"
 #include "bf16_common.cuh"
+#include "wgconv.h"
 
 void convt_out_scatter_column(int n, int *co, int *ky, int *kx);
-int launch_convt_out_scatter(const void *in, const void *packed, int packed_rows, int w_row0, const float *bias, float *out, int B, int H,
-                             int W, cudaStream_t s);
-
-#if VQB_DIAG
-// in-kernel timeline of CTA 0 (SM cycle counter), tools/diag/hconv_timeline.py; diagnostic builds only
-__device__ unsigned long long g_hconv_tl[32 * 16];
-extern "C" int vqb_debug_read_hconv_timeline(unsigned long long *dst, int n) {
-    if (!dst || n < 1 || n > 32 * 16) return VQB_ERR_BAD_ARG;
-    return vqb_cuda_status(cudaMemcpyFromSymbol(dst, g_hconv_tl, sizeof(unsigned long long) * n));
-}
-#define HC_TL(it_, ev_)                                                                       \
-    do {                                                                                      \
-        if (blockIdx.x == 0 && (it_) >= 0 && (it_) < 32) {                                    \
-            unsigned long long t_;                                                            \
-            asm volatile("mov.u64 %0, %%clock64;" : "=l"(t_));                                \
-            g_hconv_tl[(it_) * 16 + (ev_)] = t_;                                              \
-        }                                                                                     \
-    } while (0)
-#else
-#define HC_TL(it_, ev_) do { } while (0)
-#endif
 
 namespace {
 
-constexpr int HC_THREADS = 384;
 constexpr int HC_MAX_STEPS = 40;      // per pass
-constexpr int HC_MAX_STAGES = 40;
 constexpr int HC_MAX_CHUNKS = 8;
-constexpr int HC_MAX_HB = 3;
 
-enum { ST_FIRST = 1, ST_NEWCHUNK = 2, ST_ENDCHUNK = 4, ST_HALFBOX = 8, ST_GSTART = 16, ST_GEND = 32 };
+enum { ST_FIRST = 1, ST_NEWCHUNK = 2, ST_ENDCHUNK = 4, ST_HALFBOX = 8 };
 enum { EPI_NHWC = 0, EPI_SHUFFLE_NCHW = 1 };
-
-// One k-step (tap x 64-channel chunk), 16 bytes, copied to shared memory at kernel start so that the single-warp issue
-// loops read it with one LDS.128 (the first version indexed the kernel parameters: ~150 dependent scalar instructions
-// and ~1100 cycles per step whatever the MMA shape -- every layer ran at the same 0.55-0.6 us per step).
-//   x: tap offset inside the halo tile, 16-byte units (M-tile 0)         y: UMMA instruction descriptor (N of this step)
-//   z: [0,8) accumulator column offset  [8,20) offset of the weight tile inside its ring stage / 16  [20,32) bytes of the
-//      whole stage group / 16 (valid on the group's first step)
-//   w: [0,8) flags  [8,24) first row of the weight tile in the packed matrix  [24,32) N / 8
-// Weight tiles travel in GROUPS of consecutive steps (<= 32 KB, <= 4 steps) sharing one ring stage and one full / empty
-// barrier pair: one mbarrier wait and one tcgen05.commit per 16 MMAs instead of per 8.
-struct HStep { uint32_t x, y, z, w; };
-
-struct HParams {
-    const float *bias;
-    void *out;
-    int B, H, W;                    // the GEMM's pixel grid (= input grid of a stride-1 / s2d view)
-    int TW, BH, BN, MT, WP, halo;
-    int tiles_x, tiles_y, tiles_n, npass;
-    long long ntiles;
-    int NCOL;                       // accumulator columns per M-tile
-    int nsteps[2], nchunks;
-    int chunk_c0[HC_MAX_CHUNKS], chunk_p[HC_MAX_CHUNKS];
-    int S, wst_bytes, resident, nhb, halo_bytes, halo_stride;     // S ring stages of wst_bytes (= largest step group)
-    int epi_mode, cg, sy, sx, OH, OW, Cout, relu, out_f32, bias_mod;
-    int res_groups0;                // resident mode: number of step groups (= ring stages) of pass 0
-    int cluster;                    // 2: CTA pairs share the weight stream (each loads every other step, multicast to both)
-    HStep steps[2][HC_MAX_STEPS];
-};
-
-__device__ __forceinline__ void prefetch_l2_5d(const CUtensorMap *m, int c0, int c1, int c2, int c3, int c4) {
-    asm volatile("cp.async.bulk.prefetch.tensor.5d.L2.global.tile [%0, {%1, %2, %3, %4, %5}];" ::
-                     "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap *m, uint32_t bar, int c0, int c1, uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::
-            "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-                     "r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// CTA pairs sharing the weight stream (see the launcher): compiled in only on request -- measured to make no difference
-#ifndef HC_PAIR_WEIGHTS
-#define HC_PAIR_WEIGHTS 0
-#endif
-
-template <int MT, bool RES>
-__global__ void __launch_bounds__(HC_THREADS, 1)
-hconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant__ CUtensorMap tma_w,
-             const __grid_constant__ CUtensorMap tma_wh, const __grid_constant__ HParams p) {
-    extern __shared__ unsigned char smem_raw[];
-    const uint32_t raw = ptx::smem_u32(smem_raw);
-    const uint32_t sbase = (raw + 1023u) & ~1023u;
-    unsigned char *sm = smem_raw + (sbase - raw);
-
-    const uint32_t ring_off = (uint32_t)(p.nhb * p.halo_stride);
-    const uint32_t bar_off = ring_off + (uint32_t)(p.S * p.wst_bytes);
-    const uint32_t bars = sbase + bar_off;
-    auto wfull = [&](int s) { return bars + 8u * s; };
-    auto wempty = [&](int s) { return bars + 8u * (HC_MAX_STAGES + s); };
-    auto hfull = [&](int b) { return bars + 8u * (2 * HC_MAX_STAGES + b); };
-    auto hempty = [&](int b) { return bars + 8u * (2 * HC_MAX_STAGES + HC_MAX_HB + b); };
-    auto tfull = [&](int a) { return bars + 8u * (2 * HC_MAX_STAGES + 2 * HC_MAX_HB + a); };
-    auto tempty = [&](int a) { return bars + 8u * (2 * HC_MAX_STAGES + 2 * HC_MAX_HB + 2 + a); };
-    constexpr int MISC = 8 * (2 * HC_MAX_STAGES + 2 * HC_MAX_HB + 4);
-    volatile uint32_t *tmem_holder = reinterpret_cast<volatile uint32_t *>(sm + bar_off + MISC);
-    float *bias_s = reinterpret_cast<float *>(sm + bar_off + MISC + 16);
-    uint4 *steps_s = reinterpret_cast<uint4 *>(sm + bar_off + MISC + 16 + 256 * 4);        // [2][HC_MAX_STEPS]
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-    const bool paired = HC_PAIR_WEIGHTS ? p.cluster == 2 : false;      // CTA pair sharing one weight stream (non-resident layers)
-    uint32_t crank = 0;
-    if (paired) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
-    // MT = 2: two MMA issuer warps (one per M half), each commits its own MMAs to every barrier the tensor pipe signals
-    constexpr uint32_t NISS = MT == 2 ? 2u : 1u;
-    if (tid < p.S) { ptx::mbar_init(wfull(tid), 1); ptx::mbar_init(wempty(tid), (paired ? 2u : 1u) * NISS); }
-    if (tid >= 64 && tid < 64 + p.nhb) { ptx::mbar_init(hfull(tid - 64), 1); ptx::mbar_init(hempty(tid - 64), NISS); }
-    if (tid >= 96 && tid < 98) { ptx::mbar_init(tfull(tid - 96), NISS); ptx::mbar_init(tempty(tid - 96), 8); }
-    if (tid == 128) { ptx::prefetch_tmap(&tma_in); ptx::prefetch_tmap(&tma_w); ptx::prefetch_tmap(&tma_wh); }
-    ptx::fence_mbar_init();
-    for (int c = tid; c < p.NCOL; c += HC_THREADS) {
-        float b = 0.f;
-        if (p.bias) {
-            if (p.epi_mode == EPI_SHUFFLE_NCHW) b = c < 4 * p.bias_mod ? __ldg(p.bias + c % p.bias_mod) : 0.f;
-            else b = __ldg(p.bias + c % p.bias_mod);
-        }
-        bias_s[c] = b;
-    }
-    for (int i = tid; i < 2 * HC_MAX_STEPS; i += HC_THREADS) {
-        const HStep st = p.steps[i / HC_MAX_STEPS][i % HC_MAX_STEPS];
-        steps_s[i] = make_uint4(st.x, st.y, st.z, st.w);
-    }
-    if (warp == 2) ptx::tmem_alloc(sbase + bar_off + MISC, 512);
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-    if (paired) cluster_sync_all();                      // the peer's barriers exist before anything is multicast to them
-    pdl_launch_dependents();
-
-    const long long ntiles = p.ntiles;
-    const int G = (int)gridDim.x;
-    // a CTA pair walks the weight stream in lockstep: both run as many iterations as the pair's first CTA has tiles; the
-    // second one may end with a "dry" iteration that only consumes (and helps to load) the weights
-    const long long pair_first = (long long)blockIdx.x - (long long)crank;
-    const long long niter = pair_first < ntiles ? (ntiles - pair_first + G - 1) / G : 0;
-
-    if (warp == 0) {
-        // ===================== halo producer =====================
-        const bool leader = ptx::elect_one();
-        pdl_wait();                                  // the input activation is the previous layer's output
-        uint32_t hb = 0, hpar = 0;
-        auto tile_origin = [&](long long tile, int &gx0, int &gy0, int &n0) {
-            long long t = tile / p.npass;
-            const int tx = (int)(t % p.tiles_x); t /= p.tiles_x;
-            const int ty = (int)(t % p.tiles_y); t /= p.tiles_y;
-            gx0 = tx * p.TW; gy0 = ty * p.BH; n0 = (int)t * p.BN;
-        };
-        int hit = 0;
-        for (long long tile = blockIdx.x; tile < ntiles; tile += G, ++hit) {
-            int gx0, gy0, n0;
-            tile_origin(tile, gx0, gy0, n0);
-            // pull the halo tiles of the tile after next into L2 now: with <= 3 halo buffers the shared-memory load of a
-            // tile can only be issued one tile ahead, which does not cover an HBM round trip under full load
-            const long long tpf = tile + (p.nchunks >= 4 ? 1LL : 2LL) * G;      // (four-chunk tiles: 166 KB each; two tiles ahead on 148 SMs crowd L2)
-            if (leader && tpf < ntiles && (p.npass == 1 || (tpf % p.npass) == 0)) {
-                int px0, py0, pn0;
-                tile_origin(tpf, px0, py0, pn0);
-                for (int k = 0; k < p.nchunks; ++k) prefetch_l2_5d(&tma_in, p.chunk_c0[k], px0 - p.halo, pn0, p.chunk_p[k], py0 - p.halo);
-            }
-            for (int k = 0; k < p.nchunks; ++k) {
-                ptx::mbar_wait_sleep(hempty((int)hb), hpar ^ 1, 100);
-                if (leader) {
-                    if (k < 2) HC_TL(hit, k);
-                    ptx::mbar_expect_tx(hfull((int)hb), (uint32_t)p.halo_bytes);
-                    tma_load_5d(sbase + hb * (uint32_t)p.halo_stride, &tma_in, hfull((int)hb), p.chunk_c0[k], gx0 - p.halo, n0,
-                                p.chunk_p[k], gy0 - p.halo);
-                }
-                if (++hb == (uint32_t)p.nhb) { hb = 0; hpar ^= 1; }
-            }
-        }
-    } else if (warp == 3) {
-        // ===================== weight producer: one ring stage (and one barrier) per step GROUP =====================
-        const bool leader = ptx::elect_one();
-        auto load_group = [&](const uint4 *sp, int i, int ns, uint32_t stage) -> int {       // returns the index after the group
-            const uint32_t gbytes = ((sp[i].z >> 20) & 0xfffu) << 4;
-            if (leader) ptx::mbar_expect_tx(wfull((int)stage), gbytes);
-            for (;; ++i) {
-                const uint4 st = sp[i];
-                if (leader) {
-                    const uint32_t dst = sbase + ring_off + stage * (uint32_t)p.wst_bytes + (((st.z >> 8) & 0xfffu) << 4);
-                    const CUtensorMap *wm = (st.w & ST_HALFBOX) ? &tma_wh : &tma_w;
-                    if (!paired) ptx::tma_load_2d(dst, wm, wfull((int)stage), 0, (int)((st.w >> 8) & 0xffffu));
-                    else if (((uint32_t)i & 1u) == crank) tma_load_2d_mc(dst, wm, wfull((int)stage), 0, (int)((st.w >> 8) & 0xffffu), (uint16_t)3);
-                }
-                if (st.w & ST_GEND) break;
-            }
-            (void)ns;
-            return i + 1;
-        };
-        if (RES) {
-            uint32_t stage = 0;
-            for (int ps = 0; ps < p.npass; ++ps)
-                for (int i = 0; i < p.nsteps[ps]; ++stage) i = load_group(steps_s + ps * HC_MAX_STEPS, i, p.nsteps[ps], stage);
-        } else {
-            uint32_t ws = 0, wpar = 0;
-            int wit = 0;
-            for (long long k = 0, tile = blockIdx.x; k < niter; ++k, tile += G, ++wit) {
-                const int ps = (int)((tile < ntiles ? tile : pair_first + k * G) % p.npass);      // (a dry iteration follows the pair's first CTA)
-                const int ns = p.nsteps[ps];
-                for (int i = 0; i < ns;) {
-                    ptx::mbar_wait_sleep(wempty((int)ws), wpar ^ 1, 64);
-                    if (leader && i == 0) HC_TL(wit, 2);
-                    i = load_group(steps_s + ps * HC_MAX_STEPS, i, ns, ws);
-                    if (++ws == (uint32_t)p.S) { ws = 0; wpar ^= 1; }
-                }
-                if (leader) HC_TL(wit, 3);
-            }
-        }
-    } else if (warp == 1 || (MT == 2 && warp == 2)) {
-        // ===================== MMA issuer(s) =====================
-        // The issue loop is ~16 dependent scalar instructions per MMA (descriptor arithmetic, register -> uniform-register
-        // moves, flag branches): one warp sustains an M128 N128 K16 MMA per ~96 cycles against the 64 the tensor pipe needs
-        // (r02_hconv_timeline_before.txt; tools/ubench/mma_rate2.cu shows that neither the halo-tile descriptors, nor
-        // concurrent tcgen05.ld, nor shared-memory stores slow the pipe itself).  With 256-pixel tiles the two M halves have
-        // separate accumulators, so warp 1 issues half 0 and warp 2 (free after the TMEM allocation) half 1.
-        const uint32_t mh = MT == 2 ? (uint32_t)(warp - 1) : 0u;
-        const bool leader = ptx::elect_one();
-        const uint32_t a_hi = ptx::desc_hi_sw128((uint32_t)(p.WP * 128)), b_hi = ptx::desc_hi_sw128(1024);
-        const uint32_t ring16 = (sbase + ring_off) >> 4, wst16 = (uint32_t)p.wst_bytes >> 4;
-        const uint32_t halo16 = sbase >> 4, hstride16 = (uint32_t)p.halo_stride >> 4;
-        const uint32_t ncol = (uint32_t)p.NCOL;
-        constexpr bool resident = RES;              // the whole weight set stays in shared memory: no ring hand-shake in the loop
-        const uint32_t nS = (uint32_t)p.S, nHB = (uint32_t)p.nhb;       // (kept in registers: the loop below is issue-latency bound)
-        uint32_t hb = 0, hpar = 0, ws = 0, wpar = 0;
-        int it = 0;
-        for (long long k = 0, tile = blockIdx.x; k < (paired ? niter : (ntiles - blockIdx.x + G - 1) / G); ++k, tile += G, ++it) {
-            if (tile >= ntiles) {
-                // dry iteration of a CTA pair: take part in the weight ring's hand-shake, nothing else
-                const int psd = (int)((pair_first + k * G) % p.npass);
-                const uint4 *spd = steps_s + psd * HC_MAX_STEPS;
-                for (int i = 0; i < p.nsteps[psd]; ++i) {
-                    const uint32_t fl = spd[i].w;
-                    if (fl & ST_GSTART) ptx::mbar_wait(wfull((int)ws), wpar);
-                    if (fl & ST_GEND) {
-                        if (leader) tc_commit_mc(wempty((int)ws), (uint16_t)3);
-                        if (++ws == nS) { ws = 0; wpar ^= 1; }
-                    }
-                }
-                __syncwarp();
-                continue;
-            }
-            const int ps = (int)(tile % p.npass);
-            const int ns = p.nsteps[ps];
-            const int acc = it & 1;
-            const uint4 *sp = steps_s + ps * HC_MAX_STEPS;
-            uint4 st = sp[0];
-            if (leader && mh == 0) HC_TL(it, 4);
-            ptx::mbar_wait(tempty(acc), (uint32_t)(((it >> 1) & 1) ^ 1));
-            if (leader && mh == 0) HC_TL(it, 5);
-            const uint32_t dbase = tmem_base + (uint32_t)(acc * 256);
-            if (resident) ws = ps == 0 ? 0u : (uint32_t)p.res_groups0;          // stage = group index over both passes
-            for (int i = 0; i < ns; ++i) {
-                const uint4 nx = sp[i + 1];                                       // (one entry of slack behind the table)
-                const uint32_t fl = st.w;
-                if (fl & ST_NEWCHUNK) {
-                    ptx::mbar_wait(hfull((int)hb), hpar);
-                    if (leader && i == 0 && mh == 0) HC_TL(it, 6);
-                }
-                if (fl & ST_GSTART) {
-                    if (!resident) ptx::mbar_wait(wfull((int)ws), wpar);
-                    else if (it < 2) ptx::mbar_wait(wfull((int)ws), 0);          // each pass first occurs at it <= 1
-                }
-                ptx::tc_fence_after();
-                const uint32_t a_lo = halo16 + hb * hstride16 + st.x + mh * 64u;
-                const uint32_t b_lo = ring16 + ws * wst16 + ((st.z >> 8) & 0xfffu);
-                const uint32_t d0 = dbase + (st.z & 0xffu) + mh * ncol;
-                const uint32_t idesc = st.y;
-                const uint32_t accf = (fl & ST_FIRST) ? 0u : 1u;
-                if (leader) {
-                    mma_bf16_w(d0, a_lo, a_hi, b_lo, b_hi, idesc, accf);
-                    mma_bf16_w(d0, a_lo + 2u, a_hi, b_lo + 2u, b_hi, idesc, 1u);
-                    mma_bf16_w(d0, a_lo + 4u, a_hi, b_lo + 4u, b_hi, idesc, 1u);
-                    mma_bf16_w(d0, a_lo + 6u, a_hi, b_lo + 6u, b_hi, idesc, 1u);
-                }
-                if (fl & ST_GEND) {
-                    if (!resident) {
-                        if (leader) { if (paired) tc_commit_mc(wempty((int)ws), (uint16_t)3); else ptx::tc_commit(wempty((int)ws)); }
-                        if (++ws == nS) { ws = 0; wpar ^= 1; }
-                    } else ++ws;
-                }
-                if (fl & ST_ENDCHUNK) {
-                    if (leader) ptx::tc_commit(hempty((int)hb));
-                    if (++hb == nHB) { hb = 0; hpar ^= 1; }
-                }
-                st = nx;
-            }
-            if (leader) { if (mh == 0) HC_TL(it, 7); ptx::tc_commit(tfull(acc)); }
-            __syncwarp();
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const int q = warp & 3, g = (warp - 4) >> 2;
-        const int row = q * 32 + lane;
-        const int em = MT == 2 ? g : 0;
-        const int ncol_thr = MT == 2 ? p.NCOL : (p.NCOL >= 64 ? p.NCOL / 2 : (g == 0 ? p.NCOL : 0));
-        const int c_lo = (MT == 2 || p.NCOL < 64) ? 0 : g * (p.NCOL / 2);
-        const int xx = row & 7, grp = row >> 3;
-        const int bn = grp % p.BN, yy = grp / p.BN;
-        int it = 0;
-        for (long long tile = blockIdx.x; tile < ntiles; tile += G, ++it) {
-            long long t = tile;
-            const int ps = (int)(t % p.npass); t /= p.npass;
-            const int tx = (int)(t % p.tiles_x); t /= p.tiles_x;
-            const int ty = (int)(t % p.tiles_y); t /= p.tiles_y;
-            const int gx = tx * p.TW + em * 8 + xx, gy = ty * p.BH + yy, n = (int)t * p.BN + bn;
-            const bool valid = gx < p.W && gy < p.H && n < p.B;
-            const int acc = it & 1;
-            ptx::mbar_wait_sleep(tfull(acc), (uint32_t)((it >> 1) & 1), 200);     // (parked warps must not poll: they outrank the MMA warp)
-            ptx::tc_fence_after();
-            if (tid == 128) HC_TL(it, 8);
-            const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 256 + em * p.NCOL);
-            if (p.epi_mode == EPI_SHUFFLE_NCHW) {
-                // decoder.py:34-35: column (py*2+px)*Cout+co of input pixel (gy,gx) is output pixel (2gy+py, 2gx+px),
-                // channel co, of the NCHW fp32 module output
-                if (ncol_thr > 0) {
-                    float v[16];
-                    tmem_ld16(trow, v);
-                    if (valid) {
-                        const int co_n = p.Cout;
-                        float *o = reinterpret_cast<float *>(p.out);
-                        for (int co = 0; co < co_n; ++co)
-#pragma unroll
-                            for (int py = 0; py < 2; ++py) {
-                                float2 w2 = make_float2(v[(py * 2 + 0) * co_n + co] + bias_s[co], v[(py * 2 + 1) * co_n + co] + bias_s[co]);
-                                if (p.relu) { w2.x = fmaxf(w2.x, 0.f); w2.y = fmaxf(w2.y, 0.f); }
-                                *reinterpret_cast<float2 *>(o + (((long long)n * co_n + co) * p.OH + 2 * gy + py) * p.OW + 2 * gx) = w2;
-                            }
-                    }
-                }
-            } else {
-                // NHWC store; column group j (cg columns) is output pixel (gy*sy + pass, gx*sx + j)
-                const long long prow = ((long long)n * p.OH + (long long)gy * p.sy + ps) * p.OW + (long long)gx * p.sx;
-                float va[32], vb[32];
-                auto emit = [&](const float (&v)[32], int c0, int nc) {       // nc = live columns of this group (16 or 32)
-                    if (!valid) return;
-                    const int j = c0 / p.cg, cc = c0 - j * p.cg;
-                    const long long off = (prow + j) * p.Cout + cc;
-                    // 32-byte stores: each thread writes whole sectors of its pixel's channel run (16-byte stores left half-written
-                    // sectors behind and cost twice the store instructions: the epilogue, not the MMAs, bounded the transposed
-                    // convolutions -- profiles/r02_hconv_timeline_before.txt)
-                    if (p.out_f32) {
-                        float *dst = reinterpret_cast<float *>(p.out) + off;
-#pragma unroll
-                        for (int i = 0; i < 32; i += 8) {
-                            if (i < nc) {
-                                float o[8];
-#pragma unroll
-                                for (int u = 0; u < 8; ++u) {
-                                    o[u] = v[i + u] + bias_s[c0 + i + u];
-                                    if (p.relu) o[u] = fmaxf(o[u], 0.f);
-                                }
-                                st_global_256(dst + i, __float_as_uint(o[0]), __float_as_uint(o[1]), __float_as_uint(o[2]), __float_as_uint(o[3]),
-                                              __float_as_uint(o[4]), __float_as_uint(o[5]), __float_as_uint(o[6]), __float_as_uint(o[7]));
-                            }
-                        }
-                    } else {
-                        __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(p.out) + off;
-#pragma unroll
-                        for (int i = 0; i < 32; i += 16) {
-                            if (i < nc) {
-                                float o[16];
-#pragma unroll
-                                for (int u = 0; u < 16; ++u) {
-                                    o[u] = v[i + u] + bias_s[c0 + i + u];
-                                    if (p.relu) o[u] = fmaxf(o[u], 0.f);
-                                }
-                                st_global_256(dst + i, pack_bf16(o[0], o[1]), pack_bf16(o[2], o[3]), pack_bf16(o[4], o[5]), pack_bf16(o[6], o[7]),
-                                              pack_bf16(o[8], o[9]), pack_bf16(o[10], o[11]), pack_bf16(o[12], o[13]), pack_bf16(o[14], o[15]));
-                            }
-                        }
-                    }
-                };
-                // the TMEM load of the next 32 columns travels while the current ones are stored
-                if (ncol_thr > 0) {
-                    const int c_hi = c_lo + ncol_thr;
-                    ptx::tmem_ld32(trow + (uint32_t)c_lo, va);
-                    for (int c0 = c_lo; c0 < c_hi; c0 += 64) {
-                        ptx::tmem_ld_wait32(va);
-                        if (c0 + 32 < c_hi) ptx::tmem_ld32(trow + (uint32_t)(c0 + 32), vb);
-                        emit(va, c0, c_hi - c0);
-                        if (c0 + 32 < c_hi) {
-                            ptx::tmem_ld_wait32(vb);
-                            if (c0 + 64 < c_hi) ptx::tmem_ld32(trow + (uint32_t)(c0 + 64), va);
-                            emit(vb, c0 + 32, c_hi - c0 - 32);
-                        }
-                    }
-                }
-            }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (tid == 128) HC_TL(it, 9);
-            if (tid == 352) HC_TL(it, 10);
-            if (lane == 0) ptx::mbar_arrive(tempty(acc));
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) ptx::tmem_dealloc(tmem_base, 512);
-    if (paired) cluster_sync_all();                      // neither CTA leaves while the other may still signal its barriers
-}
 
 // ------------------------------------------------------------------------------------------------ host side: plans
 struct RowDesc { int co, ci0, r, s; };          // one packed weight row = 64 input channels of (co, r, s); co < 0: zeros
@@ -616,7 +200,6 @@ __global__ void hconv_pack_kernel(const float *__restrict__ w, const int4 *__res
     out[i] = __float2bfloat16_rn(v);
 }
 
-int pow2_ceil_h(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 
 void kernel_dims(int kind, int &kh, int &kw) {
     kh = kw = (kind == VQB_CONV_K1 || kind == VQB_RES_W2_KIND) ? 1 : (kind == VQB_CONV_K3 || kind == VQB_CONVT_K3) ? 3 : 4;
@@ -654,6 +237,21 @@ extern "C" int vqb_pack_conv_weight_bf16(const float *w, void *packed, int kind,
     return vqb_cuda_status(cudaGetLastError());
 }
 
+namespace {
+
+// first row of the block of Cout packed rows (co = 0 .. Cout-1) holding input channels [ci0, ci0 + 64) of tap (r, s)
+int find_rows(const Plan &pl, int ci0, int r, int s) {
+    const int n = (int)pl.rows.size();
+    for (int i = 0; i + pl.Cout <= n; ++i) {
+        const RowDesc &a = pl.rows[i], &b = pl.rows[i + pl.Cout - 1];
+        if (a.co == 0 && a.ci0 == ci0 && a.r == r && a.s == s && b.co == pl.Cout - 1 && b.ci0 == ci0 && b.r == r && b.s == s)
+            return i;
+    }
+    return -1;
+}
+
+}  // namespace
+
 // in: bf16 NHWC (B, H, W, Cin).  out: bf16 NHWC (out_f32 = 0) / fp32 NHWC (out_f32 = 1) / fp32 NCHW (VQB_CONVT_K4S2_OUT).
 extern "C" int vqb_conv2d_bf16(const void *in, const void *packed, const float *bias, void *out, int B, int Cin, int H, int W,
                                int Cout, int kind, int relu, int out_f32, void *stream) {
@@ -664,138 +262,126 @@ extern "C" int vqb_conv2d_bf16(const void *in, const void *packed, const float *
     if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(packed)) & 15) return VQB_ERR_ALIGNMENT;
     if (pl->s2d && ((H | W) & 1)) return VQB_ERR_UNSUPPORTED;
     if (kind == VQB_CONVT_K4S2_OUT) out_f32 = 1;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (kind == VQB_CONVT_K4S2_OUT && pl->scatter_row0 >= 0 && !relu)
-        return launch_convt_out_scatter(in, packed, (int)pl->rows.size(), pl->scatter_row0, bias, reinterpret_cast<float *>(out), B, H, W, s);
 
-    HParams q;
-    // the GEMM's pixel grid: the input grid, or the space-to-depth grid of a stride-2 conv
-    const int GH = pl->s2d ? H / 2 : H, GW = pl->s2d ? W / 2 : W;
-    constexpr int MISC = 8 * (2 * HC_MAX_STAGES + 2 * HC_MAX_HB + 4) + 16 + 256 * 4 + 2 * HC_MAX_STEPS * 16 + 16 + 1024;
-    memset(&q, 0, sizeof(q));
-    q.bias = bias; q.out = out;
-    q.B = B; q.H = GH; q.W = GW;
-    q.MT = (GW > 8 && 2 * pl->NCOL <= 256) ? 2 : 1;
-    q.TW = 8 * q.MT;
-    q.BH = pow2_ceil_h(GH) < 16 ? pow2_ceil_h(GH) : 16;
-    q.BN = 16 / q.BH;
-    q.halo = pl->halo;
-    q.WP = q.TW + 2 * q.halo;
-    q.tiles_x = (GW + q.TW - 1) / q.TW;
-    q.tiles_y = (GH + q.BH - 1) / q.BH;
-    q.tiles_n = (B + q.BN - 1) / q.BN;
-    q.npass = pl->npass;
-    q.ntiles = (long long)q.tiles_x * q.tiles_y * q.tiles_n * q.npass;
-    q.NCOL = pl->NCOL;
-    q.nchunks = pl->nchunks;
-    for (int k = 0; k < pl->nchunks; ++k) { q.chunk_c0[k] = pl->chunk_c0[k]; q.chunk_p[k] = pl->chunk_p[k]; }
-    // ---- step table: groups of consecutive steps (<= 32 KB of weight tiles, <= 4 steps) share a ring stage ----
-    constexpr int GROUP_BYTES = 32 * 1024, GROUP_STEPS = 4;
-    int ngroups[2] = {0, 0}, max_group_bytes = 0;
-    long long total_group_bytes = 0;
-    for (int ps = 0; ps < pl->npass; ++ps) {
-        q.nsteps[ps] = pl->nsteps[ps];
-        int gstart = 0, gbytes = 0, gcount = 0;
-        for (int i = 0; i < pl->nsteps[ps]; ++i) {
-            const PlanStep &a = pl->steps[ps][i];
-            const int bytes = a.nb * 128;
-            if (gcount > 0 && (gbytes + bytes > GROUP_BYTES || gcount == GROUP_STEPS)) {      // close the running group
-                q.steps[ps][gstart].z |= (uint32_t)(gbytes >> 4) << 20;
-                q.steps[ps][i - 1].w |= ST_GEND;
-                if (gbytes > max_group_bytes) max_group_bytes = gbytes;
-                total_group_bytes += gbytes; ++ngroups[ps];
-                gbytes = 0; gcount = 0;
+    WgLaunch L;
+    L.bf16 = 1;
+    L.in = in; L.B = B; L.Cin = Cin; L.H = H; L.W = W; L.in_step = 1;
+    L.w = packed; L.w_rows = (long long)pl->rows.size(); L.w_inner = 64;
+    L.bias = bias; L.out = out; L.out_bf16 = !out_f32; L.relu = relu;
+    L.ncols = Cout;
+    // output: NHWC of the layer's output grid (strides in elements)
+    const bool up = kind == VQB_CONVT_K4S2 || kind == VQB_CONVT_K4S2_OUT;
+    const int OH = up ? 2 * H : pl->s2d ? H / 2 : H, OW = up ? 2 * W : pl->s2d ? W / 2 : W;
+    L.out_sn = (long long)OH * OW * Cout; L.out_sh = (long long)OW * Cout; L.out_sw = Cout; L.out_sc = 1;
+    L.nph = 1;
+    L.OHg[0] = OH; L.OWg[0] = OW;
+    const int kc = Cin / 64;
+    auto add = [&](int ph, int c0, int dx, int dy, int row) {
+        if (row < 0 || L.nsteps[ph] >= WG_MAX_STEPS) return false;
+        L.steps[ph][L.nsteps[ph]++] = WgStep{c0, 0, dx, dy, row};
+        return true;
+    };
+    switch (kind) {
+        case VQB_CONV_K4S2:                 // out(y) reads in(2y + r - 1)
+            L.in_step = 2;
+            for (int r = 0; r < 4; ++r)
+                for (int s = 0; s < 4; ++s)
+                    for (int k = 0; k < kc; ++k)
+                        if (!add(0, 64 * k, s - 1, r - 1, find_rows(*pl, 64 * k, r, s))) return VQB_ERR_UNSUPPORTED;
+            break;
+        case VQB_CONVT_K4S2:                // output (2y + py, 2x + px) takes input (y + dy, x + dx), kernel row r = py + 1 - 2 dy
+            L.nph = 4; L.out_step = 2;
+            for (int ph = 0; ph < 4; ++ph) {
+                const int py = ph >> 1, px = ph & 1;
+                L.OHg[ph] = H; L.OWg[ph] = W; L.out_py[ph] = py; L.out_px[ph] = px;
+                for (int r = 0; r < 4; ++r) {
+                    if ((py + 1 - r) % 2 != 0) continue;
+                    for (int s = 0; s < 4; ++s) {
+                        if ((px + 1 - s) % 2 != 0) continue;
+                        for (int k = 0; k < kc; ++k)
+                            if (!add(ph, 64 * k, (px + 1 - s) / 2, (py + 1 - r) / 2, find_rows(*pl, 64 * k, r, s))) return VQB_ERR_UNSUPPORTED;
+                    }
+                }
             }
-            HStep &d = q.steps[ps][i];
-            d.x = (uint32_t)((((a.dy + q.halo) * q.BN) * q.WP + (a.dx + q.halo)) * 8);
-            d.y = ptx::instr_desc(ptx::FMT_BF16, 128, (uint32_t)a.nb);
-            d.z = (uint32_t)a.d_col | ((uint32_t)(gbytes >> 4) << 8);
-            d.w = (uint32_t)a.flags | ((uint32_t)a.w_row << 8) | ((uint32_t)(a.nb / 8) << 24);
-            if (gcount == 0) { d.w |= ST_GSTART; gstart = i; }
-            gbytes += bytes; ++gcount;
-        }
-        if (gcount > 0) {
-            q.steps[ps][gstart].z |= (uint32_t)(gbytes >> 4) << 20;
-            q.steps[ps][pl->nsteps[ps] - 1].w |= ST_GEND;
-            if (gbytes > max_group_bytes) max_group_bytes = gbytes;
-            total_group_bytes += gbytes; ++ngroups[ps];
-        }
+            break;
+        case VQB_CONVT_K4S2_OUT:            // N = 16 columns (sub-pixel phase, channel) per input pixel
+            L.OHg[0] = H; L.OWg[0] = W; L.ncols = 4 * Cout; L.shuffle_cg = Cout;
+            L.out_sn = (long long)Cout * OH * OW; L.out_sc = (long long)OH * OW; L.out_sh = OW; L.out_sw = 1;
+            for (int i = 0; i < pl->nsteps[0]; ++i) {
+                const PlanStep &st = pl->steps[0][i];
+                if (!add(0, pl->chunk_c0[st.chunk], st.dx, st.dy, st.w_row)) return VQB_ERR_UNSUPPORTED;
+            }
+            break;
+        default:                            // k1 / k3 convs and the k3 transposed conv: the plan's steps as they are
+            for (int i = 0; i < pl->nsteps[0]; ++i) {
+                const PlanStep &st = pl->steps[0][i];
+                if (!add(0, pl->chunk_c0[st.chunk], st.dx, st.dy, st.w_row)) return VQB_ERR_UNSUPPORTED;
+            }
+            break;
     }
-    q.res_groups0 = ngroups[0];
-    q.halo_bytes = (q.BH + 2 * q.halo) * q.BN * q.WP * 128;
-    q.halo_stride = (q.halo_bytes + 1023) & ~1023;
-    q.wst_bytes = (max_group_bytes + 1023) & ~1023;
-    q.nhb = HC_MAX_HB;
-    int S = (227 * 1024 - q.nhb * q.halo_stride - MISC) / q.wst_bytes;
-    {
-        // The weight ring is latency bound (profiles/r02_hconv_timeline_before.txt: 3 x 32 KB in flight deliver ~21 B per
-        // cycle against the 32 B per cycle a full-rate N = 128 MMA stream consumes), so shared memory is worth more as a
-        // ring stage than as a third halo buffer when a tile has at most two chunks: the next tile's first chunk then loads
-        // (from L2, prefetched two tiles ahead) behind the MMAs of this tile's last chunk.
-        const int S2 = (227 * 1024 - 2 * q.halo_stride - MISC) / q.wst_bytes;
-        if (S < 2 || (pl->nchunks <= 2 && S2 > S)) { q.nhb = 2; S = S2; }
-    }
-    if (S > HC_MAX_STAGES) S = HC_MAX_STAGES;
-    if (S < 2) return VQB_ERR_UNSUPPORTED;
-    const int all_groups = ngroups[0] + ngroups[1];
-    q.resident = all_groups <= S ? 1 : 0;
-    if (q.resident) S = all_groups;
-    else if (S > 6) S = 6;
-    q.S = S;
-    q.epi_mode = pl->epi_mode; q.cg = pl->cg; q.sy = pl->sy; q.sx = pl->sx;
-    q.OH = GH * pl->sy; q.OW = GW * pl->sx;
-    if (pl->epi_mode == EPI_SHUFFLE_NCHW) { q.OH = 2 * GH; q.OW = 2 * GW; }
-    q.Cout = Cout; q.relu = relu; q.out_f32 = out_f32;
-    q.bias_mod = Cout;
-
-    CUtensorMap tin, tw, twh;
-    {
-        // 5-D view (c, x, n, p, y); p is the row parity of the space-to-depth view (size 1 otherwise)
-        typedef unsigned long long u64;
-        u64 dims[5], strides[4];
-        if (pl->s2d) {
-            dims[0] = 2ull * Cin; dims[1] = (u64)GW; dims[2] = (u64)B; dims[3] = 2; dims[4] = (u64)GH;
-            strides[0] = 2ull * Cin * 2; strides[1] = (u64)H * W * Cin * 2; strides[2] = (u64)W * Cin * 2; strides[3] = 2ull * W * Cin * 2;
-        } else {
-            dims[0] = (u64)Cin; dims[1] = (u64)W; dims[2] = (u64)B; dims[3] = 1; dims[4] = (u64)H;
-            strides[0] = (u64)Cin * 2; strides[1] = (u64)H * W * Cin * 2; strides[2] = (u64)H * W * Cin * 2; strides[3] = (u64)W * Cin * 2;
-        }
-        const uint32_t box[5] = {64u, (uint32_t)q.WP, (uint32_t)q.BN, 1u, (uint32_t)(q.BH + 2 * q.halo)};
-        int rc = vqb_encode_tmap_nd(&tin, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, in, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        const int nrows = (int)pl->rows.size();
-        rc = vqb_encode_tmap_2d(&tw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, packed, 64, (uint64_t)nrows, 128, 64, (uint32_t)pl->nbmax,
-                                CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-        rc = vqb_encode_tmap_2d(&twh, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, packed, 64, (uint64_t)nrows, 128, 64,
-                                (uint32_t)(pl->nbhalf ? pl->nbhalf : pl->nbmax), CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-    }
-    const int smem = q.nhb * q.halo_stride + q.S * q.wst_bytes + MISC;
-    typedef void (*hconv_fn)(CUtensorMap, CUtensorMap, CUtensorMap, HParams);
-    const int variant = (q.MT - 1) * 2 + (q.resident ? 1 : 0);
-    const hconv_fn fns[4] = {hconv_kernel<1, false>, hconv_kernel<1, true>, hconv_kernel<2, false>, hconv_kernel<2, true>};
-    const hconv_fn fn = fns[variant];
-    static int attr_max[4] = {0, 0, 0, 0};
-    if (smem > attr_max[variant]) {
-        cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return (int)e;
-        attr_max[variant] = smem;
-    }
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int grid = (int)(q.ntiles < sms ? q.ntiles : sms);
-    // Streamed weights CAN be shared by CTA pairs (clusters of 2, -DHC_PAIR_WEIGHTS=1): each CTA loads every other step and
-    // multicasts it to both, halving the L2 -> shared-memory requests per SM; the ring's empty barriers take the commits of
-    // both CTAs (tcgen05.commit multicast), a pair's last CTA may end with a dry iteration.  Parity-green (all bf16 tests incl.
-    // the back-to-back stress), but within box-to-box noise both with one issuer (E3 133 vs 130 us) and with two (E3 117 vs
-    // 121, while the unpaired two-pass layer moved by the same 2-3 % on that box): the weight stream is not the limit.
-    q.cluster = (HC_PAIR_WEIGHTS && !q.resident && q.npass == 1 && grid >= 2) ? 2 : 1;
-    if (q.cluster == 2) grid &= ~1;
-    const cudaError_t le = q.cluster == 2 ? vqb_launch_cluster(fn, dim3((unsigned)grid), dim3(HC_THREADS), (size_t)smem, s, 2u, tin, tw, twh, q)
-                                          : vqb_launch(fn, dim3((unsigned)grid), dim3(HC_THREADS), (size_t)smem, s, tin, tw, twh, q);
-    if (le != cudaSuccess) return (int)le;
-    VQB_COUNT_LAUNCH(1);
-    return vqb_cuda_status(cudaGetLastError());
+    L.N = wg_gemm_cols(L.ncols);
+    if (L.N == 0) return VQB_ERR_UNSUPPORTED;
+    return launch_wgconv(L, (cudaStream_t)stream);
 }
+
+bool res_bf16_supported(int C, int Cmid) {
+    return (C == 64 || C == 128) && Cmid % 16 == 0 && Cmid >= 16 && Cmid <= 64;
+}
+
+// r, out: bf16 NHWC (B,H,W,C).  w1: packing of kind VQB_CONV_K3 with (Cout = Cmid, Cin = C); w2: VQB_RES_W2_KIND with
+// (Cout = C, Cin = Cmid) -- both made by vqb_pack_conv_weight_bf16.  One launch: per 128-pixel tile the 3x3 GEMM, ReLU,
+// and the 1x1 GEMM on the bf16 intermediate held in shared memory, + r, optional ReLU.
+extern "C" int vqb_residual_layer_bf16(const void *r, const void *w1_packed, const void *w2_packed, void *out, int B, int H,
+                                       int W, int C, int Cmid, int relu_out, void *stream) {
+    if (!r || !w1_packed || !w2_packed || !out) return VQB_ERR_BAD_ARG;
+    if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cmid <= 0) return VQB_ERR_BAD_ARG;
+    if (!res_bf16_supported(C, Cmid)) return VQB_ERR_UNSUPPORTED;
+    if (r == out) return VQB_ERR_BAD_ARG;                       // neighbouring tiles read each other's halo: not in place
+    if ((reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(w1_packed) |
+         reinterpret_cast<uintptr_t>(w2_packed)) & 15) return VQB_ERR_ALIGNMENT;
+    const Plan *p1 = get_plan(VQB_CONV_K3, C, Cmid), *p2 = get_plan(VQB_RES_W2_KIND, Cmid, C);
+    if (!p1 || !p2) return VQB_ERR_UNSUPPORTED;
+    WgLaunch L;
+    L.bf16 = 1;
+    L.in = r; L.B = B; L.Cin = C; L.H = H; L.W = W; L.in_step = 1;
+    L.w = w1_packed; L.w_rows = (long long)p1->rows.size(); L.w_inner = 64;
+    L.ncols = Cmid; L.N = wg_gemm_cols(Cmid);
+    L.w2 = w2_packed; L.w2_rows = (long long)p2->rows.size(); L.N2 = C;
+    L.skip = r; L.out = out; L.out_bf16 = 1; L.relu = relu_out;
+    L.out_sn = (long long)H * W * C; L.out_sh = (long long)W * C; L.out_sw = C; L.out_sc = 1;
+    L.nph = 1; L.OHg[0] = H; L.OWg[0] = W;
+    for (int i = 0; i < p1->nsteps[0]; ++i) {
+        const PlanStep &st = p1->steps[0][i];
+        L.steps[0][i] = WgStep{p1->chunk_c0[st.chunk], 0, st.dx, st.dy, st.w_row};
+    }
+    L.nsteps[0] = p1->nsteps[0];
+    return launch_wgconv(L, (cudaStream_t)stream);
+}
+
+// GEMM column n of the scatter form -> (co, ky, kx) of the ConvTranspose2d weight, or co = -1 for a padding column.
+void convt_out_scatter_column(int n, int *co, int *ky, int *kx) {
+    *co = -1; *ky = 0; *kx = 0;
+    if (n < 12) { const int r = n / 6, s = (n / 3) & 1; *co = n % 3; *ky = r + 1; *kx = s + 1; return; }
+    const int grp = (n - 12) / 8, j = (n - 12) % 8;
+    if (n < 44) {
+        if (j >= 6) return;
+        const int a = j / 3;                     // s for the up / down groups, r for the left / right groups
+        *co = j % 3;
+        if (grp == 0) { *ky = 0; *kx = a + 1; }
+        else if (grp == 1) { *ky = 3; *kx = a + 1; }
+        else if (grp == 2) { *ky = a + 1; *kx = 0; }
+        else { *ky = a + 1; *kx = 3; }
+        return;
+    }
+    const int c = (n - 44) / 4, jj = (n - 44) % 4;
+    if (c > 3 || jj >= 3) return;
+    *co = jj; *ky = (c >> 1) ? 3 : 0; *kx = (c & 1) ? 3 : 0;
+}
+
+// (test hook, tests/test_abi_cpu.py: the column layout is host logic and is pinned without a GPU)
+extern "C" int vqb_debug_convt_out_scatter_column(int n, int *co, int *ky, int *kx) {
+    if (n < 0 || n >= 64 || !co || !ky || !kx) return VQB_ERR_BAD_ARG;
+    convt_out_scatter_column(n, co, ky, kx);
+    return 0;
+}
+

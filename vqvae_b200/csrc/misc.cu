@@ -1,11 +1,11 @@
-// misc.cu -- small bandwidth kernels around the hot path (sm_100a).
+// misc.cu -- small bandwidth kernels around the hot path (sm_90a).
 #include "common.cuh"
 
 namespace {
 
 // (Cout,Cin,kh,kw) or ConvTranspose (Cin,Cout,kh,kw)  ->  two GEMM operand layouts, back to back:
 //   out[0 .. T)        [(r*kw+s)*Cin + ci][co]   (N-major, the FFMA kernel's B tile)
-//   out[T .. 2T)       [(r*kw+s)][co][ci]        (K-major rows of Cin, the tcgen05 B operand)
+//   out[T .. 2T)       [(r*kw+s)][co][ci]        (K-major rows of Cin, the wgmma B operand)
 __global__ void pack_weight_kernel(const float *__restrict__ w, float *__restrict__ out, int Cout, int Cin,
                                    int kh, int kw, int transposed) {
     const long long total = (long long)Cout * Cin * kh * kw;
@@ -26,7 +26,7 @@ __global__ void pack_weight_kernel(const float *__restrict__ w, float *__restric
 
 // ConvTranspose2d k4 s2 p1 weight (Cin,Cout,4,4), Cout <= 4  ->  [9 neighbour taps (dy,dx)][16][Cin]:
 // row (py*2+px)*Cout+co of tap (dy,dx) holds W[ci][co][py-2dy+1][px-2dx+1] when that kernel index
-// exists (the neighbour contributes to that output phase), else 0.  See conv_halo.cu.
+// exists (the neighbour contributes to that output phase), else 0.  Read by launch_convt_shuffle_wg (wgconv.cu).
 __global__ void pack_convt_shuffle_kernel(const float *__restrict__ w, float *__restrict__ out, int Cout, int Cin) {
     const int total = 9 * 16 * Cin;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {

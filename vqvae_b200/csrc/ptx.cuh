@@ -1,7 +1,5 @@
-// ptx.cuh -- thin inline-PTX wrappers for the Blackwell (sm_100a) async machinery:
-// mbarrier, TMA (cp.async.bulk[.tensor]), tcgen05 (TMEM alloc / mma / commit / ld).
-// Encodings of the UMMA instruction and shared-memory descriptors follow the PTX ISA
-// tables (same bit layout as cute/arch/mma_sm100_desc.hpp, read for reference only).
+// ptx.cuh -- thin inline-PTX wrappers for the Hopper (sm_90a) async machinery: mbarrier and TMA
+// (cp.async.bulk[.tensor]).  The warpgroup MMA wrappers are in wgmma.cuh.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -13,11 +11,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// One leader lane of a fully converged warp.  The single-thread issuers (TMA, tcgen05.mma/commit)
-// run their loops with ALL lanes converged and guard only the issuing instruction with this
-// predicate: inside an `if (lane == 0)` region the compiler wraps every UTCHMMA in an
-// ELECT/branch sequence (~14 SASS instructions, ~100 cycles per MMA, profiles/r01_mma_issue_*),
-// in converged code the UTCHMMAs issue back to back.
+// One leader lane of a fully converged warp.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -41,10 +35,7 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 // Wait for the phase with the given parity.  try_wait carries a suspend-time hint: the hardware parks the thread until
-// the phase completes (or the hint expires) instead of returning early and being re-polled.  Without the hint a waiting
-// warp re-executes try_wait + branch a few hundred times per microsecond: in the persistent kernels (8-12 warps parked on
-// barriers most of the time) those polls were ~20 % of all issued instructions and competed with the single MMA-issuer
-// warp for issue slots (profiles/r02_vq2_poll_loops.txt).
+// the phase completes (or the hint expires) instead of returning early and being re-polled.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
         "{\n\t"
@@ -55,24 +46,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "bra LAB_WAIT_%=;\n\t"
         "LAB_DONE_%=:\n\t"
         "}" ::"r"(bar), "r"(parity), "r"(0x989680u) : "memory");
-}
-
-// Waiting variant for warps that wait LONG (an epilogue waiting for a whole GEMM): back off with
-// nanosleep between polls.  On sm_100 the warp scheduler favours higher warp ids, so a tight poll
-// loop in an epilogue warp starves the single-thread TMA / MMA issuers sharing its SM sub-partition
-// (measured: profiles/r01_res_tc_timeline.txt -- an empty 36-iteration issue loop took 10 us).
-__device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity, uint32_t ns = 256) {
-    uint32_t done = 0;
-    while (true) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t"
-            "}" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (done) break;
-        __nanosleep(ns);
-    }
 }
 
 // ---------------------------------------------------------------- TMA
@@ -95,118 +68,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap *m, 
 __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::
                      "r"(dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar) : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t holder_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(holder_smem), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// Arrive on an mbarrier when every tcgen05.mma issued so far by this thread has completed.
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows of 128 B,
-// 8-row groups 1024 B apart (SBO), LBO unused for swizzled K-major.  bits: [0,14)
-// addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version=1, [61,64) layout (2=SW128).
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)(1024u >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// Same layout with an explicit stride between 8-row groups (operand windows inside a larger
-// shared-memory tile, e.g. a conv halo tile).  base_offset stays 0 even when saddr is not
-// 1024-byte aligned: the tensor core takes the swizzle phase from the absolute address
-// (measured: setting base_offset = (saddr >> 7) & 7 gives wrong results, see conv_halo.cu).
-__device__ __forceinline__ uint64_t smem_desc_sw128_sbo(uint32_t saddr, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)(sbo_bytes >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// Instruction descriptor: c_format F32 (1) at [4,6); a/b format at [7,10)/[10,13)
-// (0 F16, 1 BF16, 2 TF32); a/b K-major (0) at [15]/[16]; N>>3 at [17,23); M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t instr_desc(uint32_t ab_format, uint32_t M, uint32_t N) {
-    return (1u << 4) | (ab_format << 7) | (ab_format << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-constexpr uint32_t FMT_F16 = 0, FMT_BF16 = 1, FMT_TF32 = 2;
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; one thread issues on behalf of the CTA.
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-// The issue loops of the conv kernels are bound by the scalar instructions around each MMA
-// (profiles/r01_res_tc_timeline.txt), so they keep descriptors as running 32-bit words: lo = smem
-// address >> 4 (advance by +2 per 32-byte K slice), hi = constant per operand layout.
-__host__ __device__ constexpr uint32_t desc_hi_sw128(uint32_t sbo_bytes) {
-    return (sbo_bytes >> 4) | (1u << 14) | (2u << 29);      // SBO, version 1 (bit 46), SWIZZLE_128B (bits 61-63)
-}
-__device__ __forceinline__ void mma_tf32_w(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                           uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t"
-        "}" ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-// TMEM -> registers: this thread's lane (= accumulator row), 32 consecutive columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float *v) {
-    uint32_t *r = reinterpret_cast<uint32_t *>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// Same wait, but carrying the 32 destination registers of the load as in/out operands so
-// that no consumer of v[] can be scheduled above the wait.
-__device__ __forceinline__ void tmem_ld_wait32(float *v) {
-    uint32_t *r = reinterpret_cast<uint32_t *>(v);
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]),
-                   "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]),
-                   "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]),
-                   "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :: "memory");
 }
 
 __device__ __forceinline__ float fmin3(float a, float b, float c) {

@@ -48,7 +48,10 @@ extern "C" int vqb_vq_backward_f32(const float *g_zq, const float *g_loss, const
     if (e != cudaSuccess) return (int)e;
     const long long total = N * (D / 4);
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;
     vq_backward_kernel<<<(unsigned)blocks, 256, 0, s>>>(g_zq, g_loss, z, codebook, reinterpret_cast<const long long *>(idx), N, K, D, beta,
                                                         dz, dE);
     VQB_COUNT_LAUNCH(1);

@@ -1,0 +1,487 @@
+// wgconv.cu -- implicit-GEMM convolution on Hopper tensor cores (wgmma, sm_90a): the tensor-core conv of the TF32
+// mode (fp32 NHWC activations read as TF32) and of the bf16 pipeline (bf16 NHWC activations).
+//
+// GEMM view (one CTA = one 128-pixel output tile = BN images x BH rows x BW cols, all N columns):
+//   D[128 px][N] = sum over k-steps i of A_i[128 px][128 B of channels] * B_i[N][128 B]^T
+//   * A_i is ONE 4-D TMA box {128 B of channels, BW, BH, BN} of the NHWC input shifted by the step's tap
+//     (dy, dx): it lands as 128 rows of 128 bytes in the 128-byte-swizzled K-major layout wgmma reads;
+//     out-of-image pixels are zero-filled by TMA (= the zero padding), stride-2 convolutions use the tensor
+//     map's element strides.  No im2col matrix exists.
+//   * B_i is a 2-D TMA box of N K-major weight rows.
+//   * warp 0 = TMA producer over an mbarrier ring of up to 8 stages; warpgroups 1 and 2 = consumers, each owns
+//     64 pixel rows of the tile: 4 wgmma per stage (m64nNk8 tf32 / m64nNk16 bf16) into N/2 fp32 registers per
+//     thread, then the epilogue straight from the registers: + bias, + skip, ReLU, fp32 or bf16 stores.
+//   * the sub-pixel phases of a stride-2 transposed conv run in one launch (blockIdx.y = phase).
+//   * N2 > 0 (residual layer of the bf16 pipeline): the first GEMM's result is ReLU'd, rounded to bf16 and written
+//     to shared memory as the A operand of a second GEMM against an N2 x 64 weight tile loaded once, so
+//     out = act(skip + W2 . relu(W1 (*) r)) and the intermediate never leaves the SM.
+#include <cuda_bf16.h>
+
+#include "ptx.cuh"
+#include "wgconv.h"
+#include "wgmma.cuh"
+
+namespace {
+
+constexpr int WG_THREADS = 384;
+constexpr int WG_MAX_STAGES = 8;
+constexpr int A_BYTES = 128 * 128;             // 128 pixels x 128 bytes
+
+struct WgParams {
+    const float *bias;
+    const void *skip;
+    void *out;
+    int B, ncols, mid_cols;
+    int BW, BH, BN, tiles_x, tiles_y;
+    int in_step, out_step, stages;
+    int relu, out_bf16, shuffle_cg;
+    int napps;                                // applications of a chained residual layer (whole-image tiles when > 1)
+    int OHg[4], OWg[4], out_py[4], out_px[4], nsteps[4];
+    long long out_sn, out_sh, out_sw, out_sc;
+    int4 steps[4][WG_MAX_STEPS];              // x = a_c0 | b_c0 << 16, y = dx, z = dy, w = w_row
+};
+
+__device__ __forceinline__ uint32_t bf16x2(float a, float b) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<const uint32_t *>(&h);
+}
+
+// Epilogue of one accumulator fragment (wgmma D layout, see wgmma.cuh) for the pixel rows of this thread.
+template <int N>
+__device__ __forceinline__ void store_tile(const WgParams &p, const float *acc, int ph, int wgi, int gx0, int gy0, int n0,
+                                           const void *skip, int relu) {
+    const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = wgi * 64 + warp * 16 + (lane >> 2) + 8 * h;
+        const int bw = row % p.BW, bh = (row / p.BW) % p.BH, bn = row / (p.BW * p.BH);
+        const int gx = gx0 + bw, gy = gy0 + bh, n = n0 + bn;
+        if (gx >= p.OWg[ph] || gy >= p.OHg[ph] || n >= p.B) continue;
+        if (p.shuffle_cg > 0) {
+            // k4 s2 transposed conv to a few channels: column = (sub-pixel phase, channel), fp32 NCHW output
+            float *out = reinterpret_cast<float *>(p.out);
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int c = 8 * j + cq + e;
+                    if (c >= p.ncols) continue;
+                    const int sp = c / p.shuffle_cg, co = c % p.shuffle_cg;
+                    float v = acc[4 * j + 2 * h + e] + (p.bias ? __ldg(p.bias + co) : 0.f);
+                    if (relu) v = fmaxf(v, 0.f);
+                    out[(long long)n * p.out_sn + (long long)(gy * 2 + (sp >> 1)) * p.out_sh +
+                        (long long)(gx * 2 + (sp & 1)) * p.out_sw + (long long)co * p.out_sc] = v;
+                }
+            continue;
+        }
+        const long long ob = (long long)n * p.out_sn + (long long)(gy * p.out_step + p.out_py[ph]) * p.out_sh +
+                             (long long)(gx * p.out_step + p.out_px[ph]) * p.out_sw;
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+            const int c = 8 * j + cq;
+            if (c >= p.ncols) continue;                 // ncols is even: a pair is wholly in or out
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if (p.bias) { v0 += __ldg(p.bias + c); v1 += __ldg(p.bias + c + 1); }
+            if (p.out_bf16) {
+                if (skip) {
+                    const __nv_bfloat162 sk = *reinterpret_cast<const __nv_bfloat162 *>(
+                        reinterpret_cast<const __nv_bfloat16 *>(skip) + ob + c);
+                    v0 += __bfloat162float(sk.x); v1 += __bfloat162float(sk.y);
+                }
+                if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                *reinterpret_cast<uint32_t *>(reinterpret_cast<__nv_bfloat16 *>(p.out) + ob + c) = bf16x2(v0, v1);
+            } else {
+                if (skip) {
+                    // plain load: with chained applications skip is `out`, written earlier by this kernel
+                    const float2 sk = *reinterpret_cast<const float2 *>(reinterpret_cast<const float *>(skip) + ob + c);
+                    v0 += sk.x; v1 += sk.y;
+                }
+                if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + ob + c) = make_float2(v0, v1);
+            }
+        }
+    }
+}
+
+// chunks of the chained second GEMM's K (the first GEMM's N columns): one 64-channel bf16 chunk, or 32-channel fp32 ones
+template <bool BF16, int N>
+__host__ __device__ constexpr int chain_chunks() { return BF16 ? 1 : (N >= 32 ? N / 32 : 1); }
+
+template <bool BF16, int N, int N2>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant__ CUtensorMap tma_w,
+              const __grid_constant__ CUtensorMap tma_w2, const __grid_constant__ CUtensorMap tma_out,
+              const __grid_constant__ WgParams p) {
+    extern __shared__ unsigned char smem_raw[];
+    const uint32_t raw = ptx::smem_u32(smem_raw);
+    const uint32_t sbase = (raw + 1023u) & ~1023u;
+    constexpr int STAGE = A_BYTES + N * 128;
+    constexpr int KC2 = chain_chunks<BF16, N>();
+    const int S = p.stages;
+    // N2 > 0: KC2 intermediate tiles [128 px][128 B], then the KC2 W2 tiles [N2][128 B]
+    const uint32_t mid = sbase + (uint32_t)(S * STAGE);
+    const uint32_t w2s = mid + (uint32_t)(KC2 * A_BYTES);
+    const uint32_t bars = mid + (N2 > 0 ? (uint32_t)(KC2 * (A_BYTES + N2 * 128)) : 0u);
+    auto full = [&](int s) { return bars + 8u * s; };
+    auto empty = [&](int s) { return bars + 8u * (WG_MAX_STAGES + s); };
+    const uint32_t w2bar = bars + 8u * (2 * WG_MAX_STAGES);
+    constexpr int APP_BAR = 3, APP_THREADS = 32 + 256;       // producer warp + both consumer warpgroups
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int ph = blockIdx.y;
+    int tile = blockIdx.x;
+    const int tx = tile % p.tiles_x; tile /= p.tiles_x;
+    const int ty = tile % p.tiles_y; tile /= p.tiles_y;
+    const int gx0 = tx * p.BW, gy0 = ty * p.BH, n0 = tile * p.BN;
+    const int nsteps = p.nsteps[ph];
+
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), 2); }
+        ptx::mbar_init(w2bar, 1);
+        ptx::fence_mbar_init();
+    }
+    if (tid == 32) {
+        ptx::prefetch_tmap(&tma_in);
+        ptx::prefetch_tmap(&tma_w);
+        if (N2 > 0) ptx::prefetch_tmap(&tma_w2);
+        if (p.napps > 1) ptx::prefetch_tmap(&tma_out);
+    }
+    __syncthreads();
+    pdl_launch_dependents();           // the next layer may start its prologue
+
+    if (warp == 0) {
+        if constexpr (N2 > 0) {        // weights do not depend on the previous layer
+            if (lane == 0) {
+                constexpr int ck = BF16 ? 64 : 32;
+                ptx::mbar_expect_tx(w2bar, (uint32_t)(KC2 * N2 * 128));
+                for (int c = 0; c < KC2; ++c) ptx::tma_load_2d(w2s + (uint32_t)(c * N2 * 128), &tma_w2, w2bar, c * ck, 0);
+            }
+        }
+        pdl_wait();                    // ... the activations do
+        int g = 0;                     // ring position, continued across applications
+        for (int app = 0; app < p.napps; ++app) {
+            // application app > 0 reads what app - 1 wrote to `out` (whole images per tile: no other CTA touches them)
+            if (app > 0) ptx::named_bar_sync(APP_BAR, APP_THREADS);
+            const CUtensorMap *src = app == 0 ? &tma_in : &tma_out;
+            if (lane == 0) {
+                for (int i = 0; i < nsteps; ++i, ++g) {
+                    const int s = g % S;
+                    if (g >= S) ptx::mbar_wait(empty(s), (uint32_t)((g / S - 1) & 1));
+                    const int4 st = p.steps[ph][i];
+                    const uint32_t dst = sbase + (uint32_t)(s * STAGE);
+                    ptx::mbar_expect_tx(full(s), (uint32_t)STAGE);
+                    ptx::tma_load_4d(dst, src, full(s), st.x & 0xffff, gx0 * p.in_step + st.y, gy0 * p.in_step + st.z, n0);
+                    ptx::tma_load_2d(dst + A_BYTES, &tma_w, full(s), st.x >> 16, st.w);
+                }
+            }
+            __syncwarp();
+        }
+        return;
+    }
+    if (warp < 4) return;
+
+    pdl_wait();                        // skip / out may belong to the previous layer
+    const int wgi = (warp >> 2) - 1;   // pixel rows 64 * wgi .. + 63 of the tile
+    int g = 0;
+    for (int app = 0; app < p.napps; ++app) {
+        const bool last = app + 1 == p.napps;
+        const void *skip = app == 0 ? p.skip : p.out;
+        const int relu = last ? p.relu : 1;
+        float acc[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+        for (int i = 0; i < nsteps; ++i, ++g) {
+            const int s = g % S;
+            ptx::mbar_wait(full(s), (uint32_t)((g / S) & 1));
+            const uint32_t a = sbase + (uint32_t)(s * STAGE) + (uint32_t)(wgi * 64 * 128), b = sbase + (uint32_t)(s * STAGE) + A_BYTES;
+            wg::fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wg::mma<BF16, N>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+            wg::commit();
+            wg::wait<0>();
+            wg::fence_regs<N>(acc);
+            if ((warp & 3) == 0 && lane == 0) ptx::mbar_arrive(empty(s));
+        }
+
+        if constexpr (N2 == 0) {
+            store_tile<N>(p, acc, ph, wgi, gx0, gy0, n0, skip, relu);
+        } else {
+            // relu(first GEMM) -> rows of 128 bytes (64 bf16 / 32 fp32 channels per chunk), 128-byte swizzle: 16-byte
+            // piece j of row r sits at j ^ (r & 7)
+            const int wl = warp & 3, cq = 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
+                const uint32_t rb = mid + (uint32_t)(row * 128);
+                if constexpr (BF16) {
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const int c = 8 * j + cq;
+                        float v0 = 0.f, v1 = 0.f;
+                        if (j < N / 8 && c < p.mid_cols) { v0 = fmaxf(acc[4 * j + 2 * h], 0.f); v1 = fmaxf(acc[4 * j + 2 * h + 1], 0.f); }
+                        const uint32_t addr = rb + (uint32_t)(((j ^ (row & 7)) << 4) + cq * 2);
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(bf16x2(v0, v1)) : "memory");
+                    }
+                } else {
+#pragma unroll
+                    for (int j = 0; j < N / 8; ++j) {
+                        const int c = 8 * j + cq, piece = (c & 31) >> 2;
+                        const float v0 = fmaxf(acc[4 * j + 2 * h], 0.f), v1 = fmaxf(acc[4 * j + 2 * h + 1], 0.f);
+                        const uint32_t addr = rb + (uint32_t)((c >> 5) * A_BYTES) + (uint32_t)(((piece ^ (row & 7)) << 4) + (c & 3) * 4);
+                        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
+                    }
+                }
+            }
+            ptx::fence_proxy_async();                        // generic-proxy writes -> visible to wgmma
+            ptx::named_bar_sync(1 + wgi, 128);               // this warpgroup's 64 rows are complete
+            ptx::mbar_wait(w2bar, 0);
+            float acc2[N2 > 0 ? N2 / 2 : 1];
+#pragma unroll
+            for (int i = 0; i < N2 / 2; ++i) acc2[i] = 0.f;
+            wg::fence();
+#pragma unroll
+            for (int c = 0; c < KC2; ++c) {
+                const uint32_t a = mid + (uint32_t)(c * A_BYTES + wgi * 64 * 128), b = w2s + (uint32_t)(c * N2 * 128);
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk)
+                    wg::mma<BF16, N2>(acc2, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+            }
+            wg::commit();
+            wg::wait<0>();
+            wg::fence_regs<N2>(acc2);
+            store_tile<N2>(p, acc2, ph, wgi, gx0, gy0, n0, skip, relu);
+        }
+        if (!last) {
+            asm volatile("fence.proxy.async.global;" ::: "memory");      // these stores -> the next application's TMA reads
+            ptx::named_bar_sync(APP_BAR, APP_THREADS);
+        }
+    }
+}
+
+int pow2_ceil(int x) {
+    int p = 1;
+    while (p < x) p <<= 1;
+    return p;
+}
+
+typedef void (*wg_fn)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, WgParams);
+
+template <bool BF16, int N2>
+wg_fn pick_n(int N) {
+    switch (N) {
+        case 16: return wgconv_kernel<BF16, 16, N2>;
+        case 32: return wgconv_kernel<BF16, 32, N2>;
+        case 64: return wgconv_kernel<BF16, 64, N2>;
+        case 128: return wgconv_kernel<BF16, 128, N2>;
+        case 256: return N2 == 0 ? wgconv_kernel<BF16, 256, 0> : nullptr;
+        default: return nullptr;
+    }
+}
+
+wg_fn pick(int bf16, int N, int N2) {
+    if (!bf16) {
+        switch (N2) {
+            case 0: return pick_n<false, 0>(N);
+            case 64: return (N == 32 || N == 64) ? pick_n<false, 64>(N) : nullptr;
+            case 128: return (N == 32 || N == 64) ? pick_n<false, 128>(N) : nullptr;
+            default: return nullptr;
+        }
+    }
+    switch (N2) {
+        case 0: return pick_n<true, 0>(N);
+        case 64: return N <= 64 ? pick_n<true, 64>(N) : nullptr;
+        case 128: return N <= 64 ? pick_n<true, 128>(N) : nullptr;
+        default: return nullptr;
+    }
+}
+
+}  // namespace
+
+int wg_gemm_cols(int ncols) {
+    for (int n : {16, 32, 64, 128, 256})
+        if (ncols <= n) return n;
+    return 0;
+}
+
+int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
+    if (L.nph < 1 || L.nph > 4 || wg_gemm_cols(L.N) != L.N || L.ncols > L.N) return VQB_ERR_UNSUPPORTED;
+    const wg_fn fn = pick(L.bf16, L.N, L.N2);
+    if (!fn) return VQB_ERR_UNSUPPORTED;
+    const int esz = L.bf16 ? 2 : 4, ck = 128 / esz;       // elements per 128-byte K chunk
+    if (L.Cin % ck != 0 || L.w_inner % ck != 0) return VQB_ERR_UNSUPPORTED;
+    if (L.shuffle_cg == 0 && L.out_sc != 1) return VQB_ERR_UNSUPPORTED;
+    WgParams q;
+    memset(&q, 0, sizeof(q));
+    q.bias = L.bias; q.skip = L.skip; q.out = L.out;
+    q.B = L.B; q.ncols = L.ncols; q.mid_cols = L.ncols;
+    q.in_step = L.in_step; q.out_step = L.out_step;
+    q.relu = L.relu; q.out_bf16 = L.out_bf16; q.shuffle_cg = L.shuffle_cg;
+    q.napps = L.napps;
+    if (L.napps < 1 || (L.napps > 1 && (L.N2 == 0 || L.Cin != L.N2 || L.skip != L.in))) return VQB_ERR_UNSUPPORTED;
+    q.out_sn = L.out_sn; q.out_sh = L.out_sh; q.out_sw = L.out_sw; q.out_sc = L.out_sc;
+    int maxw = 0, maxh = 0, maxk = 1;
+    for (int i = 0; i < L.nph; ++i) {
+        if (L.nsteps[i] > WG_MAX_STEPS) return VQB_ERR_UNSUPPORTED;
+        q.OHg[i] = L.OHg[i]; q.OWg[i] = L.OWg[i]; q.out_py[i] = L.out_py[i]; q.out_px[i] = L.out_px[i];
+        q.nsteps[i] = L.nsteps[i];
+        for (int t = 0; t < L.nsteps[i]; ++t) {
+            const WgStep &st = L.steps[i][t];
+            q.steps[i][t] = make_int4(st.a_c0 | (st.b_c0 << 16), st.dx, st.dy, st.w_row);
+        }
+        if (L.OWg[i] > maxw) maxw = L.OWg[i];
+        if (L.OHg[i] > maxh) maxh = L.OHg[i];
+        if (L.nsteps[i] > maxk) maxk = L.nsteps[i];
+    }
+    if (maxw <= 0 || maxh <= 0) return 0;
+    q.BW = pow2_ceil(maxw) < 16 ? pow2_ceil(maxw) : 16;
+    q.BH = pow2_ceil(maxh) < 128 / q.BW ? pow2_ceil(maxh) : 128 / q.BW;
+    q.BN = 128 / (q.BW * q.BH);
+    q.tiles_x = (maxw + q.BW - 1) / q.BW;
+    q.tiles_y = (maxh + q.BH - 1) / q.BH;
+    const long long tiles_n = (L.B + q.BN - 1) / q.BN;
+    if (L.napps > 1 && (q.tiles_x != 1 || q.tiles_y != 1 || L.nph != 1)) return VQB_ERR_UNSUPPORTED;     // whole images per tile
+
+    const CUtensorMapDataType dt = L.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    CUtensorMap tin, tw, tw2, tout;
+    const uint64_t dims[4] = {(uint64_t)L.Cin, (uint64_t)L.W, (uint64_t)L.H, (uint64_t)L.B};
+    const uint64_t strides[3] = {(uint64_t)L.Cin * esz, (uint64_t)L.W * L.Cin * esz, (uint64_t)L.H * L.W * L.Cin * esz};
+    const uint32_t box[4] = {(uint32_t)ck, (uint32_t)(q.BW * L.in_step), (uint32_t)(q.BH * L.in_step), (uint32_t)q.BN};
+    const uint32_t es[4] = {1u, (uint32_t)L.in_step, (uint32_t)L.in_step, 1u};
+    int rc = vqb_encode_tmap_4d(&tin, dt, L.in, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = vqb_encode_tmap_2d(&tw, dt, L.w, (uint64_t)L.w_inner, (uint64_t)L.w_rows, (uint64_t)L.w_inner * esz, (uint32_t)ck,
+                            (uint32_t)L.N, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    tw2 = tw;
+    tout = tin;
+    int kc2 = 0;
+    if (L.N2 > 0) {
+        if (L.ncols > 64 || L.w2_inner % ck != 0) return VQB_ERR_UNSUPPORTED;
+        if (!L.bf16 && L.ncols != L.N) return VQB_ERR_UNSUPPORTED;          // fp32 intermediate: whole 32-channel chunks
+        kc2 = L.bf16 ? 1 : L.N / 32;
+        q.mid_cols = L.ncols; q.ncols = L.N2;
+        rc = vqb_encode_tmap_2d(&tw2, dt, L.w2, (uint64_t)L.w2_inner, (uint64_t)L.w2_rows, (uint64_t)L.w2_inner * esz, (uint32_t)ck,
+                                (uint32_t)L.N2, CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+    }
+    if (L.napps > 1) {
+        rc = vqb_encode_tmap_4d(&tout, dt, L.out, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+    }
+    const int stage = A_BYTES + L.N * 128;
+    const int fixed = kc2 * (A_BYTES + L.N2 * 128) + 8 * (2 * WG_MAX_STAGES + 1) + 1024;
+    int stages = (220 * 1024 - fixed) / stage;
+    if (stages > WG_MAX_STAGES) stages = WG_MAX_STAGES;
+    if (stages > maxk) stages = maxk;
+    if (stages < 1) return VQB_ERR_UNSUPPORTED;
+    q.stages = stages;
+    const int smem = stages * stage + fixed;
+    static int attr_max[64] = {0};      // per instantiation (slot below)
+    const int slot = (L.bf16 ? 32 : 0) + (L.N2 == 128 ? 16 : L.N2 == 64 ? 8 : 0) + (L.N == 16 ? 0 : L.N == 32 ? 1 : L.N == 64 ? 2 : L.N == 128 ? 3 : 4);
+    if (smem > attr_max[slot]) {
+        cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e != cudaSuccess) return (int)e;
+        attr_max[slot] = smem;
+    }
+    const long long grid = (long long)q.tiles_x * q.tiles_y * tiles_n;
+    if (grid <= 0 || grid > 0x7fffffffLL) return VQB_ERR_UNSUPPORTED;
+    if (cudaError_t le = vqb_launch(fn, dim3((unsigned)grid, (unsigned)L.nph), dim3(WG_THREADS), (size_t)smem, s, tin, tw, tw2, tout, q))
+        return (int)le;
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------------ TF32 entry
+bool conv_tc_supported(const ConvLaunch &p) {
+    const bool in_nhwc = p.in_sc == 1 && p.in_sw == p.Cin;
+    const bool out_nhwc = p.out_sc == 1 && p.out_sw == p.Cout;
+    return in_nhwc && out_nhwc && p.Cin % 32 == 0 && p.Cout % 16 == 0 && p.Cout >= 16 && p.Cout <= 256 &&
+           p.in_step >= 1 && p.in_step <= 2 &&
+           (reinterpret_cast<uintptr_t>(p.in) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 &&
+           (p.skip == nullptr || (reinterpret_cast<uintptr_t>(p.skip) & 15) == 0);
+}
+
+// ph[0..nph): the phases of ONE layer (same tensors, strides and steps; they differ in the output grid, the
+// sub-pixel offset and the tap list).  w_tc: tap-major K-major weight [tap][Cout][Cin] (vqb_pack_conv_weight_f32,
+// second half).
+int launch_conv_tc(const ConvLaunch *ph, int nph, const float *w_tc, int total_taps, cudaStream_t s) {
+    if (nph < 1 || nph > 4) return VQB_ERR_UNSUPPORTED;
+    const ConvLaunch &p = ph[0];
+    WgLaunch L;
+    L.bf16 = 0;
+    L.in = p.in; L.B = p.B; L.Cin = p.Cin; L.H = p.H; L.W = p.W; L.in_step = p.in_step;
+    L.w = w_tc; L.w_rows = (long long)total_taps * p.Cout; L.w_inner = p.Cin;
+    L.N = wg_gemm_cols(p.Cout); L.ncols = p.Cout;
+    L.bias = p.bias; L.skip = p.skip; L.out = p.out; L.relu = p.relu;
+    L.out_step = p.out_step; L.out_sn = p.out_sn; L.out_sh = p.out_sh; L.out_sw = p.out_sw; L.out_sc = p.out_sc;
+    L.nph = nph;
+    const int kchunks = p.Cin / 32;
+    for (int i = 0; i < nph; ++i) {
+        const ConvLaunch &r = ph[i];
+        if (r.ntaps * kchunks > WG_MAX_STEPS) return VQB_ERR_UNSUPPORTED;
+        L.OHg[i] = r.OHg; L.OWg[i] = r.OWg; L.out_py[i] = r.out_py; L.out_px[i] = r.out_px;
+        int n = 0;
+        for (int t = 0; t < r.ntaps; ++t)
+            for (int cc = 0; cc < kchunks; ++cc)
+                L.steps[i][n++] = WgStep{0, cc * 32, r.tap_dx[t], r.tap_dy[t], r.tap_w[t] * p.Cout};
+        for (int t = 0; t < n; ++t) L.steps[i][t].a_c0 = L.steps[i][t].b_c0;
+        L.nsteps[i] = n;
+    }
+    return launch_wgconv(L, s);
+}
+
+// ------------------------------------------------------------------------------------------------ TF32 residual layer
+// residual.py:18-29 on fp32 NHWC activations: per 128-pixel tile the 3x3 GEMM (C -> Cmid), ReLU, the 1x1 GEMM (Cmid -> C)
+// on the fp32 intermediate held in shared memory, + r, ReLU -- the arithmetic of the two separate conv launches (same
+// k-step order, same TF32 operands), in one launch.  napps > 1 (a ResidualStack of one shared layer): whole images per
+// tile, every application inside the same launch, the activation round-tripping through `out` (L2) between them.
+bool res_wg_supported(int C, int Cmid) { return (C == 64 || C == 128) && (Cmid == 32 || Cmid == 64); }
+
+int launch_res_wg(const float *r, const float *w1_tc, const float *w2_tc, float *out, int B, int H, int W, int C, int Cmid,
+                  int relu_out, int napps, cudaStream_t s) {
+    if (!res_wg_supported(C, Cmid) || r == out) return VQB_ERR_UNSUPPORTED;
+    if ((reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(out)) & 15) return VQB_ERR_UNSUPPORTED;
+    WgLaunch L;
+    L.bf16 = 0;
+    L.in = r; L.B = B; L.Cin = C; L.H = H; L.W = W; L.in_step = 1;
+    L.w = w1_tc; L.w_rows = 9LL * Cmid; L.w_inner = C;
+    L.N = Cmid; L.ncols = Cmid;
+    L.w2 = w2_tc; L.w2_rows = C; L.w2_inner = Cmid; L.N2 = C;
+    L.skip = r; L.out = out; L.relu = relu_out; L.napps = napps;
+    L.out_sn = (long long)H * W * C; L.out_sh = (long long)W * C; L.out_sw = C; L.out_sc = 1;
+    L.nph = 1; L.OHg[0] = H; L.OWg[0] = W;
+    int n = 0;
+    for (int t = 0; t < 9; ++t)                  // tap-major, then 32-channel chunks: the order of launch_conv_tc
+        for (int cc = 0; cc < C / 32; ++cc)
+            L.steps[0][n++] = WgStep{cc * 32, cc * 32, t % 3 - 1, t / 3 - 1, t * Cmid};
+    L.nsteps[0] = n;
+    return launch_wgconv(L, s);
+}
+
+// ------------------------------------------------------------------------------------------------ TF32 output layer
+// decoder.py:34-35, ConvTranspose2d(Cin -> Cout <= 4, k4 s2 p1), NHWC fp32 in, NCHW fp32 out: one GEMM over the
+// 3x3 input neighbourhood with N = 16 columns (sub-pixel phase, channel) and a pixel-shuffle epilogue.
+// w_shuffle: the third region of vqb_pack_conv_weight_f32, [9 taps (dy, dx)][16][Cin].
+bool convt_shuffle_supported(int Cin, int Cout) { return Cout >= 1 && Cout <= 4 && Cin % 32 == 0 && 9 * (Cin / 32) <= WG_MAX_STEPS; }
+
+int launch_convt_shuffle_wg(const float *in, const float *w_shuffle, const float *bias, float *out, int B, int Cin, int H,
+                            int W, int Cout, int relu, cudaStream_t s) {
+    if (!convt_shuffle_supported(Cin, Cout)) return VQB_ERR_UNSUPPORTED;
+    if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(w_shuffle)) & 15) return VQB_ERR_UNSUPPORTED;
+    WgLaunch L;
+    L.bf16 = 0;
+    L.in = in; L.B = B; L.Cin = Cin; L.H = H; L.W = W; L.in_step = 1;
+    L.w = w_shuffle; L.w_rows = 9LL * 16; L.w_inner = Cin;
+    L.N = 16; L.ncols = 4 * Cout; L.shuffle_cg = Cout;
+    L.bias = bias; L.out = out; L.relu = relu;
+    const int OH = 2 * H, OW = 2 * W;
+    L.out_sn = (long long)Cout * OH * OW; L.out_sc = (long long)OH * OW; L.out_sh = OW; L.out_sw = 1;
+    L.nph = 1; L.OHg[0] = H; L.OWg[0] = W;
+    int n = 0;
+    for (int t = 0; t < 9; ++t)
+        for (int cc = 0; cc < Cin / 32; ++cc)
+            L.steps[0][n++] = WgStep{cc * 32, cc * 32, t % 3 - 1, t / 3 - 1, t * 16};
+    L.nsteps[0] = n;
+    return launch_wgconv(L, s);
+}

@@ -1,0 +1,46 @@
+// wgconv.h -- host description of one launch of the wgmma implicit-GEMM convolution (wgconv.cu).
+#pragma once
+#include "common.cuh"
+
+#define WG_MAX_STEPS 72        // k-steps per phase: taps x 128-byte channel chunks (e.g. 9 taps x 8 chunks)
+
+// One k-step: the A box starts at channel a_c0 of the input pixel shifted by (dy, dx); the B box is the N weight
+// rows starting at w_row, channel b_c0 within the row.
+struct WgStep { int a_c0, b_c0, dx, dy, w_row; };
+
+struct WgLaunch {
+    int bf16 = 0;                         // operands: 0 = fp32 activations read as TF32, 1 = bf16
+    const void *in = nullptr;             // NHWC (B, H, W, Cin)
+    int B = 0, Cin = 0, H = 0, W = 0, in_step = 1;
+    const void *w = nullptr;              // weight rows, w_inner elements each (K-major)
+    long long w_rows = 0;
+    int w_inner = 0;
+    int N = 0;                            // GEMM columns per tile: 16, 32, 64, 128 or 256
+    int ncols = 0;                        // columns that carry output (<= N)
+    // chained second GEMM (residual layer): N2 output columns from N2 rows of w2_inner channels; 0 = none
+    const void *w2 = nullptr;
+    long long w2_rows = 0;
+    int w2_inner = 64;
+    int N2 = 0;
+    int napps = 1;                        // > 1: that many chained applications (skip = in, whole-image tiles)
+    const float *bias = nullptr;          // per output channel, may be null
+    const void *skip = nullptr;           // same layout and type as out, may be null
+    void *out = nullptr;
+    int out_bf16 = 0, relu = 0;
+    int shuffle_cg = 0;                   // > 0: column c = (sub-pixel phase c / cg, channel c % cg), fp32 out
+    int out_step = 1;
+    long long out_sn = 0, out_sh = 0, out_sw = 0, out_sc = 1;    // element strides of out (and skip)
+    int nph = 1;
+    int OHg[4] = {0, 0, 0, 0}, OWg[4] = {0, 0, 0, 0}, out_py[4] = {0, 0, 0, 0}, out_px[4] = {0, 0, 0, 0};
+    int nsteps[4] = {0, 0, 0, 0};
+    WgStep steps[4][WG_MAX_STEPS];
+};
+
+int launch_wgconv(const WgLaunch &L, cudaStream_t s);
+int wg_gemm_cols(int ncols);           // smallest supported N >= ncols, 0 if none
+bool res_wg_supported(int C, int Cmid);
+bool convt_shuffle_supported(int Cin, int Cout);
+int launch_convt_shuffle_wg(const float *in, const float *w_shuffle, const float *bias, float *out, int B, int Cin, int H,
+                            int W, int Cout, int relu, cudaStream_t s);
+int launch_res_wg(const float *r, const float *w1_tc, const float *w2_tc, float *out, int B, int H, int W, int C, int Cmid,
+                  int relu_out, int napps, cudaStream_t s);

@@ -6,7 +6,7 @@ so ``from models.vqvae import VQVAE`` keeps working (the top-level ``models`` pa
 re-exports these classes).  The nn.Conv2d / nn.ConvTranspose2d / nn.Embedding children
 are kept ONLY as parameter containers (identical init order => identical weights under
 the same torch seed, identical ``state_dict()``); their own ``forward`` is never used.
-Every ``forward`` here launches the hand-written sm_100a kernels through the C ABI
+Every ``forward`` here launches the hand-written sm_90a kernels through the C ABI
 (``include/vqvae_b200.h``).  Inference only: outputs carry no autograd graph.
 
 Reference semantics reproduced on purpose (SURVEY 3.3):
@@ -35,9 +35,9 @@ _PRECISION = {"value": DEFAULT_PRECISION}
 
 def set_precision(name: str):
     """Arithmetic of the convolution layers:
-    "tf32" (default) tcgen05 kind::tf32 on fp32 activations, fp32 accumulation -- the reference's GPU arithmetic;
+    "tf32" (default) wgmma tf32 on fp32 activations, fp32 accumulation -- the reference's GPU arithmetic;
     "fp32"  FFMA on CUDA cores -- the reference's CPU numerics (end-to-end indices equal the CPU reference);
-    "bf16"  bf16 activations and operands between layers (tcgen05 kind::f16), fp32 accumulation -- the arithmetic the
+    "bf16"  bf16 activations and operands between layers (wgmma bf16), fp32 accumulation -- the arithmetic the
             reference reaches through torch.autocast(dtype=torch.bfloat16); fastest.
     The VQ distances / argmin are bit-exact fp32 in every mode."""
     if name not in PRECISIONS:
@@ -227,7 +227,7 @@ class ResidualStack(nn.Module):
             c1.out_channels % 16 == 0 and c1.out_channels <= 64
 
     def _apply_nhwc_bf16(self, r, B, H, W):
-        """bf16 NHWC twin of _apply_nhwc: one persistent tcgen05 kernel per application of the shared layer."""
+        """bf16 NHWC twin of _apply_nhwc: one wgmma launch per application of the shared layer."""
         if len(self.stack) == 0:
             return r
         c1, c2 = self.stack[0].res_block[1], self.stack[0].res_block[3]
@@ -336,7 +336,7 @@ class Decoder(nn.Module):
                 and ics[2].out_channels <= 128 and ics[4].in_channels % 64 == 0 and ics[4].out_channels <= 4)
 
     def _forward_from_nhwc_bf16(self, z, B, H, W):
-        """z: bf16 NHWC (B,H,W,in_dim) -> x_hat fp32 NCHW, every layer on the bf16 tcgen05 kernels."""
+        """z: bf16 NHWC (B,H,W,in_dim) -> x_hat fp32 NCHW, every layer on the bf16 kernels."""
         ics = self.inverse_conv_stack
         h = ops.conv2d_bf16(z, _PACKED.bf16(ics[0].weight, CONVT_K3), _bias(ics[0]), B=B, Cin=ics[0].in_channels, H=H, W=W,
                             Cout=ics[0].out_channels, kind=CONVT_K3, relu=True)
@@ -470,7 +470,7 @@ class VQVAE(nn.Module):
         self.last_min_encoding_indices = None
 
     def _bf16_pipeline(self):
-        """True when set_precision("bf16") is active AND every layer of this model has a bf16 tcgen05 kernel
+        """True when set_precision("bf16") is active AND every layer of this model has a bf16 kernel
         (h_dim = 128 family: 64-channel first layer, channel counts in multiples of 64, embedding_dim = 64).
         Other shapes run the TF32 kernels on fp32 activations, with a one-time warning."""
         if get_precision() != "bf16":

@@ -12,7 +12,7 @@ from ._lib import BF16, FP32, NCHW, NHWC, TF32, check, lib  # noqa: F401
 def _require_cuda(t, what):
     if not t.is_cuda:
         raise RuntimeError(
-            f"vqvae_b200: {what} must be a CUDA tensor -- this implementation is sm_100a-only "
+            f"vqvae_b200: {what} must be a CUDA tensor -- this implementation is sm_90a (H100) only "
             "and has no CPU fallback")
     if t.device.index != torch.cuda.current_device():
         # the C ABI launches on the CURRENT device's stream (header: "the caller selects the device"); a tensor that lives
@@ -62,7 +62,7 @@ def _f32c(t):
 def pack_conv_weight(w, transposed, out=None):
     """(Cout,Cin,kh,kw) conv / (Cin,Cout,kh,kw) conv-transpose weight -> the two tap-major
     fp32 GEMM operand layouts of vqb_pack_conv_weight_f32, back to back:
-    [(r*kw+s)*Cin+ci][co] for the FFMA kernel and [(r*kw+s)][co][ci] for tcgen05."""
+    [(r*kw+s)*Cin+ci][co] for the FFMA kernel and [(r*kw+s)][co][ci] for wgmma."""
     _require_cuda(w, "weight")
     w = _f32c(w.detach())
     if transposed:
@@ -191,7 +191,7 @@ def vq_forward_bf16zq(z_rows, codebook):
 
 
 def residual_layer_bf16(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, relu_out):
-    """out = act(r + W2.relu(W1 (*) r)) on bf16 NHWC buffers, one persistent tcgen05 kernel (vqb_residual_layer_bf16)."""
+    """out = act(r + W2.relu(W1 (*) r)) on bf16 NHWC buffers, one wgmma launch (vqb_residual_layer_bf16)."""
     _require_cuda(r, "input")
     if r.dtype != torch.bfloat16 or not r.is_contiguous():
         raise RuntimeError("residual_layer_bf16: input must be a contiguous bf16 NHWC tensor")
@@ -328,12 +328,12 @@ VQ_KERNELS = {"auto": 0, "exact": 1, "tc": 2, "tc_r1": 3}
 
 
 def set_vq_kernel(name: str):
-    """Kernel used by vq_forward: "auto" (tcgen05 when D == 64), "exact" (FFMA) or "tc"."""
+    """Kernel used by vq_forward: "auto" (see vqb_vq_forward_f32), "exact" (FFMA) or "tc"."""
     check(lib().vqb_set_vq_kernel(VQ_KERNELS[name]), "set_vq_kernel")
 
 
 def vq_debug_scores(z_rows, codebook):
-    """Diagnostic: tcgen05 VQ kernel + dump of its approximate TF32 scores (N, Kpad)."""
+    """Diagnostic: wgmma VQ kernel + dump of its approximate TF32 scores (N, Kpad)."""
     N, D = z_rows.shape
     K = codebook.shape[0]
     dev = z_rows.device

@@ -1,9 +1,9 @@
 """Host-buffer streaming front end of ``VQVAE.forward`` (models/vqvae.py:29-44 called in a loop,
 as main.py:60-75 does with its DataLoader batches).
 
-The reference's caller hands the model one host batch after another.  On a B200 a cfg2 step is
-~0.17 ms of kernels next to ~0.06 ms of PCIe traffic in each direction, so a caller that copies,
-runs and reads back synchronously leaves the GPU idle half of the time.  ``HostPipeline`` keeps
+The reference's caller hands the model one host batch after another.  A cfg2 step's input and output
+cross PCIe in each direction next to its kernels, so a caller that copies, runs and reads back
+synchronously leaves the GPU idle while the copies run.  ``HostPipeline`` keeps
 ``depth`` batches in flight on three streams -- host->device copy, the captured forward graph,
 device->host copy -- with one set of device buffers (and one captured graph) per slot.  Every
 batch still goes host -> HBM -> kernels -> host; only the waiting is overlapped.
