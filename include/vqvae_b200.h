@@ -112,8 +112,9 @@ enum vqb_conv_kind {
 /* Bytes of the packed bf16 weight of one layer (0 = shape not covered: Cin % 64 != 0, ...). */
 size_t vqb_conv_bf16_packed_bytes(int kind, int Cout, int Cin);
 /* w: the layer's fp32 weight as PyTorch stores it ((Cout,Cin,kh,kw), or (Cin,Cout,kh,kw) for
- * the transposed kinds) -> `packed` (128-byte aligned): one 128-byte row of 64 input channels
- * per (k-step, output column), in the order the kernel's k-steps consume them.            */
+ * the transposed kinds) -> `packed` (128-byte aligned): K-major bf16 rows, tap-major,
+ * [kh*kw][Cout][Cin] (VQB_RES_W2: Cin zero padded to 64), or [9][16][Cin] for
+ * VQB_CONVT_K4S2_OUT -- the layouts vqb_pack_conv_weight_f32 writes for the wgmma path.    */
 int vqb_pack_conv_weight_bf16(const float *w, void *packed, int kind, int Cout, int Cin,
                               void *stream);
 /* One layer forward on bf16 NHWC input (B,H,W,Cin):  out = act(conv(in) + bias).

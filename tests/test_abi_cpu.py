@@ -8,6 +8,8 @@ import re
 import pytest
 import torch
 
+from vqvae_b200 import _lib
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -130,7 +132,7 @@ def test_new_entry_points_validate_arguments_without_a_gpu():
     assert lib.vqb_conv2d_bf16(None, None, None, None, 1, 64, 8, 8, 64, _lib.CONV_K3, 0, 0, None) == -1
     assert lib.vqb_conv2d_bf16(p, p, None, p, 1, 48, 8, 8, 64, _lib.CONV_K3, 0, 0, None) == -2          # Cin % 64
     assert lib.vqb_conv2d_bf16(p, p, None, p, 1, 64, 7, 8, 64, _lib.CONV_K4S2, 0, 0, None) == -2        # odd height
-    assert lib.vqb_conv_bf16_packed_bytes(_lib.CONV_K3, 128, 128) == 9 * 2 * 128 * (128 + 16) + 256
+    assert lib.vqb_conv_bf16_packed_bytes(_lib.CONV_K3, 128, 128) == 9 * 128 * 128 * 2
     assert lib.vqb_conv_bf16_packed_bytes(_lib.CONV_K3, 128, 100) == 0                                  # not covered
     assert lib.vqb_conv_bf16_packed_bytes(_lib.CONVT_K4S2, 64, 128) > 0
     assert lib.vqb_pack_conv_weight_bf16(None, None, _lib.CONV_K3, 128, 128, None) == -1
@@ -189,62 +191,50 @@ def test_reference_checkpoint_loads_on_cpu():
             os.remove(out)
 
 
-def test_convt_out_scatter_column_layout():
-    """convt_out_bf16.cu orders the 64 GEMM columns of the output layer by DESTINATION pixel.  Host logic, pinned here:
-    every (ky, kx, co) of the 4x4x3 ConvTranspose2d weight appears exactly once, the 16 pad columns are marked, and the
-    group a column sits in is the one the epilogue reads it from: a tap (ky, kx) of input pixel (y, x) lands on output pixel
-    (2y - 1 + ky, 2x - 1 + kx) (decoder.py:34, k4 s2 p1), i.e. in the 2x2 block of input pixel (y + dy, x + dx) with
-    dy = -1 for ky = 0, +1 for ky = 3, else 0 (same for dx), at block row r = (2y - 1 + ky) - 2(y + dy)."""
-    import ctypes
-    from vqvae_b200 import _lib
-    fn = _lib.lib().vqb_debug_convt_out_scatter_column
-    fn.argtypes = [ctypes.c_int] + [ctypes.POINTER(ctypes.c_int)] * 3
-    seen = {}
-    pads = 0
-    for n in range(64):
-        co, ky, kx = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        assert fn(n, ctypes.byref(co), ctypes.byref(ky), ctypes.byref(kx)) == 0
-        if co.value < 0:
-            pads += 1
-            continue
-        key = (ky.value, kx.value, co.value)
-        assert key not in seen
-        seen[key] = n
-        dy = -1 if ky.value == 0 else (1 if ky.value == 3 else 0)
-        dx = -1 if kx.value == 0 else (1 if kx.value == 3 else 0)
-        r, s_ = (ky.value - 1) - 2 * dy, (kx.value - 1) - 2 * dx          # position inside the destination's 2x2 block
-        assert r in (0, 1) and s_ in (0, 1)
-        # the column groups the epilogue addresses: own [0,12), up [12,20), down [20,28), left [28,36), right [36,44), corners
-        if (dy, dx) == (0, 0):
-            assert n == (r * 2 + s_) * 3 + co.value
-        elif dx == 0:
-            assert n == (12 if dy == -1 else 20) + s_ * 3 + co.value and r == (1 if dy == -1 else 0)
-        elif dy == 0:
-            assert n == (28 if dx == -1 else 36) + r * 3 + co.value and s_ == (1 if dx == -1 else 0)
-        else:
-            base = {(-1, -1): 44, (-1, 1): 48, (1, -1): 52, (1, 1): 56}[(dy, dx)]
-            assert n == base + co.value and (r, s_) == ((1 if dy == -1 else 0), (1 if dx == -1 else 0))
-    assert len(seen) == 48 and pads == 16
-    assert fn(64, ctypes.byref(ctypes.c_int()), ctypes.byref(ctypes.c_int()), ctypes.byref(ctypes.c_int())) != 0
+# The shapes each bf16 layer kind takes (vqb_conv_bf16_packed_bytes != 0): kind -> (Cin step, Cin max, Cout step,
+# Cout max); each size must be a multiple of its step and at least one step.
+BF16_KIND_LIMITS = {
+    _lib.CONV_K1: (64, 512, 16, 256),
+    _lib.CONV_K3: (64, 256, 16, 256),
+    _lib.CONVT_K3: (64, 256, 16, 256),
+    _lib.CONV_K4S2: (64, 128, 16, 256),
+    _lib.CONVT_K4S2: (64, 384, 32, 128),
+    _lib.CONVT_K4S2_OUT: (64, 256, 1, 4),
+    _lib.RES_W2: (16, 64, 16, 256),
+}
 
 
-def test_bf16_conv_plans_row_counts():
-    """hconv.cu's host-built GEMM step plans (no GPU needed): one packed 128-byte weight row per (output column, tap,
-    64-channel chunk).  Every useful row count follows from the layer: conv Cout x taps x chunks; the stride-2 conv on its
-    space-to-depth view 4 chunks x 4 taps; the stride-2 transposed conv 2 passes x chunks x 2 row taps x (2 Cout + Cout +
-    Cout) columns; the output layer 9 x 16 gather-form rows + the 64 scatter-form columns."""
-    from vqvae_b200 import _lib
+def check_bf16_kind_limits(L):
+    """Both sides of every shape limit of BF16_KIND_LIMITS, through the library handle L."""
+    for kind, (cstep, cmax, ostep, omax) in BF16_KIND_LIMITS.items():
+        def ok(cout, cin):
+            return L.vqb_conv_bf16_packed_bytes(kind, cout, cin) != 0
+        for cout in (ostep, omax):
+            assert ok(cout, cstep) and ok(cout, cmax), (kind, cout)
+            for cin in (0, -cstep, cstep // 2, cstep + cstep // 2, cmax + cstep):
+                assert not ok(cout, cin), (kind, cout, cin)
+        for cin in (cstep, cmax):
+            bad = [0, -ostep, omax + ostep] + ([ostep // 2, ostep + ostep // 2] if ostep > 1 else [])
+            for cout in bad:
+                assert not ok(cout, cin), (kind, cout, cin)
+    for kind in (-1, _lib.RES_W2 + 1):
+        assert L.vqb_conv_bf16_packed_bytes(kind, 64, 64) == 0
+
+
+def test_bf16_conv_packed_bytes():
+    """vqb_pack_conv_weight_bf16 writes the K-major layout the TF32 mode reads, in bf16: [kh*kw taps][Cout][Cin] with Cin
+    zero padded to a multiple of 64 (only RES_W2's Cmid <= 64 pads), or [9 neighbour taps][16][Cin] for the output layer."""
     L = _lib.lib()
     expect = [
-        (_lib.CONV_K1, 64, 128, 2 * 64),                     # vqvae.py:16
-        (_lib.CONV_K3, 128, 128, 9 * 2 * 128),               # encoder.py:35
-        (_lib.CONV_K3, 32, 128, 9 * 2 * 32),                 # residual.py:20 (W1)
-        (_lib.CONVT_K3, 128, 64, 9 * 128),                   # decoder.py:28
-        (_lib.CONV_K4S2, 128, 64, 4 * 4 * 128),              # encoder.py:32
-        (_lib.CONVT_K4S2, 64, 128, 2 * 2 * 2 * 4 * 64),      # decoder.py:31
-        (_lib.CONVT_K4S2_OUT, 3, 64, 9 * 16 + 64),           # decoder.py:34
-        (_lib.RES_W2, 128, 32, 128),                         # residual.py:23 (W2, Cmid padded to one 64-channel chunk)
+        (_lib.CONV_K1, 64, 128, 1 * 64 * 128),               # vqvae.py:16
+        (_lib.CONV_K3, 128, 128, 9 * 128 * 128),             # encoder.py:35
+        (_lib.CONV_K3, 32, 128, 9 * 32 * 128),               # residual.py:20 (W1)
+        (_lib.CONVT_K3, 128, 64, 9 * 128 * 64),              # decoder.py:28
+        (_lib.CONV_K4S2, 128, 64, 16 * 128 * 64),            # encoder.py:32
+        (_lib.CONVT_K4S2, 64, 128, 16 * 64 * 128),           # decoder.py:31
+        (_lib.CONVT_K4S2_OUT, 3, 64, 9 * 16 * 64),           # decoder.py:34
+        (_lib.RES_W2, 128, 32, 128 * 64),                    # residual.py:23 (W2, Cmid padded to one 64-channel chunk)
     ]
-    for kind, cout, cin, rows in expect:
-        assert L.vqb_conv_bf16_packed_bytes(kind, cout, cin) == rows * (128 + 16) + 256, (kind, cout, cin)
-    assert L.vqb_conv_bf16_packed_bytes(_lib.CONV_K3, 128, 100) == 0          # Cin must be a multiple of 64: not covered
+    for kind, cout, cin, elems in expect:
+        assert L.vqb_conv_bf16_packed_bytes(kind, cout, cin) == 2 * elems, (kind, cout, cin)
+    check_bf16_kind_limits(L)

@@ -1,4 +1,4 @@
-"""VQB_BF16 path: the wgmma bf16 kernels (wgconv.cu via hconv.cu) against the C oracle.
+"""VQB_BF16 path: the wgmma bf16 kernel (wgconv.cu, driven by hconv.cu) against the C oracle.
 
 Operands are rounded to bf16 (8-bit mantissa) and accumulated in fp32, so each kernel is compared with the oracle
 evaluated on the SAME bf16-rounded inputs and weights: what is left is the fp32 accumulation order (~1e-5) plus, for
@@ -58,18 +58,18 @@ BF16_LAYER_CASES = [
     (1, 128, 64, 64, 128, 3, 1, False, False, False),   # same at the cfg3 latent size (32 tiles)
     (3, 128, 8, 8, 128, 3, 1, False, True, False),      # cfg2 latent size: TW = 8, two images per tile
     (2, 64, 20, 36, 128, 3, 1, True, True, False),      # decoder.py:28-29, ragged tiles in x and y
-    (2, 64, 32, 32, 128, 4, 2, False, True, False),     # encoder.py:32-34 (space-to-depth planes)
+    (2, 64, 32, 32, 128, 4, 2, False, True, False),     # encoder.py:32-34 (stride-2 taps)
     (1, 64, 128, 128, 128, 4, 2, False, True, False),   # same, cfg3 size
     (3, 64, 16, 16, 128, 4, 2, False, False, False),    # cfg2 size
-    (2, 128, 16, 16, 64, 4, 2, True, True, False),      # decoder.py:31-33: two passes, paired column parities
+    (2, 128, 16, 16, 64, 4, 2, True, True, False),      # decoder.py:31-33: four sub-pixel phases in one launch
     (1, 128, 64, 64, 64, 4, 2, True, True, False),      # cfg3 size
     (3, 128, 8, 8, 64, 4, 2, True, False, False),       # cfg2 size
-    (2, 128, 16, 32, 64, 1, 1, False, False, True),     # vqvae.py:16-17 -> fp32 z_e, resident weights
+    (2, 128, 16, 32, 64, 1, 1, False, False, True),     # vqvae.py:16-17 -> fp32 z_e
     (5, 128, 8, 8, 64, 1, 1, False, False, True),       # cfg2 size, ragged batch (5 images, 2 per tile)
     (2, 64, 32, 32, 3, 4, 2, True, False, True),        # decoder.py:34-35 -> fp32 NCHW, pixel shuffle
     (1, 64, 128, 128, 3, 4, 2, True, False, True),      # cfg3 size
     (3, 64, 16, 16, 3, 4, 2, True, True, True),         # cfg2 size (ReLU asked: the gather-form kernel)
-    (2, 64, 20, 37, 3, 4, 2, True, False, True),        # scatter form (convt_out_bf16.cu), ragged 14x14 interiors, odd width
+    (2, 64, 20, 37, 3, 4, 2, True, False, True),        # ragged tiles, odd width
     (5, 64, 14, 14, 3, 4, 2, True, False, True),        # one exact tile per image
     (3, 64, 15, 29, 3, 4, 2, True, False, True),        # one-pixel remainders
     (1, 64, 12, 20, 48, 3, 1, False, True, False),      # Cout = 48 (16-column tail group), ragged
@@ -84,16 +84,16 @@ def test_bf16_conv_layers_vs_oracle(case):
 
 
 def test_bf16_conv_many_tiles_persistent_loop():
-    """More tiles than SMs: every CTA walks several tiles (ring wrap-around)."""
+    """More tiles than SMs: several waves of CTAs, each running its k-steps around the mbarrier ring."""
     rng = np.random.RandomState(7)
-    _run_layer(rng, 8, 128, 64, 64, 128, 3, 1, False, True, False)        # 512 tiles of 256 pixels
-    _run_layer(rng, 4, 128, 64, 64, 64, 4, 2, True, True, False)          # 2 passes x 256 tiles
+    _run_layer(rng, 8, 128, 64, 64, 128, 3, 1, False, True, False)        # 256 tiles of 128 pixels
+    _run_layer(rng, 4, 128, 64, 64, 64, 4, 2, True, True, False)          # 4 phases x 128 tiles
 
 
 def test_bf16_kernels_back_to_back_launches():
-    """40 launches of each persistent kernel enqueued without a host sync (programmatic dependent launch lets a launch start
-    while its predecessor drains): every launch must give the first launch's bits.  Written after a two-issuer variant of
-    the residual kernel passed all single-launch tests and faulted about once in thirty launches (r02_hconv_notes.txt)."""
+    """40 launches of each kernel enqueued without a host sync (programmatic dependent launch lets a launch start while its
+    predecessor drains): every launch must give the first launch's bits.  Written after a variant of the residual kernel
+    passed all single-launch tests and faulted about once in thirty back-to-back launches."""
     from vqvae_b200 import ops, _lib
     g = torch.Generator(device="cuda").manual_seed(5)
     B, L = 48, 64
@@ -109,11 +109,11 @@ def test_bf16_kernels_back_to_back_launches():
         jobs.append(lambda: ops.conv2d_bf16(x, pk, b, B=B, Cin=Cin, H=H, W=W, Cout=Cout, kind=kind, relu=relu, out_f32=out_f32))
 
     conv(64, 2 * L, 2 * L, 128, 4, 2, False)          # E2
-    conv(128, L, L, 128, 3, 1, False)                 # E3 (two MMA issuer warps, streamed weights)
+    conv(128, L, L, 128, 3, 1, False)                 # E3
     conv(64, L, L, 128, 3, 1, True)                   # D1
-    conv(128, L, L, 64, 4, 2, True)                   # D2 (two passes)
-    conv(128, L, L, 64, 1, 1, False, True, False)     # pre-quant 1x1 (resident weights)
-    conv(64, 2 * L, 2 * L, 3, 4, 2, True, True, False)  # D3, scatter form
+    conv(128, L, L, 64, 4, 2, True)                   # D2 (four sub-pixel phases)
+    conv(128, L, L, 64, 1, 1, False, True, False)     # pre-quant 1x1
+    conv(64, 2 * L, 2 * L, 3, 4, 2, True, True, False)  # D3, pixel shuffle
     r = torch.randn((B, L, L, 128), device="cuda", generator=g).clamp_min(0).to(torch.bfloat16)
     w1 = torch.randn((32, 128, 3, 3), device="cuda", generator=g) / np.sqrt(1152)
     w2 = torch.randn((128, 32, 1, 1), device="cuda", generator=g) / np.sqrt(32)
@@ -134,7 +134,7 @@ def test_bf16_kernels_back_to_back_launches():
 @pytest.mark.parametrize("B,H,W,C,Cmid,relu_out", [(2, 16, 32, 128, 32, True), (1, 64, 64, 128, 32, True), (3, 8, 8, 128, 32, True),
                                                    (2, 20, 36, 128, 32, False), (5, 8, 8, 64, 16, True), (6, 64, 64, 128, 32, True)])
 def test_bf16_residual_layer_vs_oracle(B, H, W, C, Cmid, relu_out):
-    """res_bf16.cu: out = act(r + W2.relu(W1 (*) r)) with bf16 operands; the intermediate relu(W1 (*) r) is rounded
+    """vqb_residual_layer_bf16: out = act(r + W2.relu(W1 (*) r)) with bf16 operands; the intermediate relu(W1 (*) r) is rounded
     to bf16 before the second GEMM (it is that GEMM's A operand), which the oracle side mirrors."""
     from vqvae_b200 import ops, _lib
     rng = np.random.RandomState(B * 1000 + H * 100 + C)
@@ -198,8 +198,8 @@ def test_bf16_model_forward_tolerance(name):
 
 @pytest.mark.parametrize("B,H,W,relu", [(2, 256, 256, True), (5, 32, 32, True), (3, 64, 64, False), (2, 16, 16, True), (1, 12, 20, True), (300, 32, 32, True)])
 def test_bf16_input_conv_vs_oracle(B, H, W, relu):
-    """encoder.py:29-31 in the bf16 pipeline: fp32 NCHW image -> bf16 NHWC.  The 48-tap contraction runs as kind::tf32 on the
-    fp32 pixels (operands truncated to 10-bit mantissas), the result is rounded once to bf16."""
+    """encoder.py:29-31 in the bf16 pipeline: fp32 NCHW image -> bf16 NHWC.  The 48-tap contraction runs in fp32 FFMA
+    (conv_edge.cu), the result is rounded once to bf16."""
     from vqvae_b200 import ops
     rng = np.random.RandomState(B + H)
     x = (2 * rng.random_sample((B, 3, H, W)) - 1).astype(np.float32)

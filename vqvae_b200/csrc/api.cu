@@ -14,8 +14,6 @@ int launch_convt_out_k4s2(const float *x, const float *wp, const float *bias, fl
 bool vq_tc_supported(long long N, int K, int D);
 int launch_vq_tc(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, int zq_bf16, double *sse,
                  int *hist, void *ws, float *dbg, cudaStream_t s);
-bool conv_tc_supported(const ConvLaunch &p);
-int launch_conv_tc(const ConvLaunch *ph, int nph, const float *w_tc, int total_taps, cudaStream_t s);
 
 int vqb_pdl_enabled() {
     static int on = -1;
@@ -89,9 +87,8 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     if (kh * kw > VQB_MAX_TAPS) return VQB_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
 
-    const int OH = transposed ? (H - 1) * stride - 2 * pad + kh : (H + 2 * pad - kh) / stride + 1;
-    const int OW = transposed ? (W - 1) * stride - 2 * pad + kw : (W + 2 * pad - kw) / stride + 1;
-    if (OH <= 0 || OW <= 0) return VQB_ERR_BAD_ARG;
+    const ConvGeom g = conv_geom(kh, kw, stride, pad, transposed, H, W);
+    if (g.OH <= 0 || g.OW <= 0) return VQB_ERR_BAD_ARG;
 
     // the two end layers: the output ConvTranspose2d (Cout <= 4) as one wgmma GEMM over the 3x3 input neighbourhood
     // (N = 16 columns, pixel shuffle); the input conv (Cin = 3: K = 48 fp32 values per pixel straight from the NCHW
@@ -99,7 +96,7 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     if (kh == 4 && kw == 4 && stride == 2 && pad == 1 && !skip) {
         if (transposed && precision != VQB_FP32 && in_layout == VQB_NHWC && out_layout == VQB_NCHW &&
             convt_shuffle_supported(Cin, Cout)) {
-            const int rc = launch_convt_shuffle_wg(in, w_packed + (size_t)2 * 16 * Cin * Cout, bias, out, B, Cin, H, W, Cout,
+            const int rc = launch_convt_shuffle_wg(0, in, w_packed + (size_t)2 * 16 * Cin * Cout, bias, out, B, Cin, H, W, Cout,
                                                    relu, s);
             if (rc != VQB_ERR_UNSUPPORTED) return rc;
         }
@@ -115,73 +112,72 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     p.in = in; p.w = w_packed; p.bias = bias; p.skip = skip; p.out = out;
     p.B = B; p.Cin = Cin; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu;
     set_strides(in_layout, Cin, H, W, p.in_sn, p.in_sh, p.in_sw, p.in_sc);
-    set_strides(out_layout, Cout, OH, OW, p.out_sn, p.out_sh, p.out_sw, p.out_sc);
-    const bool small = (Cout <= 4);
-    const float *w_tc = w_packed + (size_t)kh * kw * Cin * Cout;   // K-major copy for the wgmma path
-    const bool want_tc = precision != VQB_FP32;
-
-    if (!transposed || stride == 1) {
-        p.OHg = OH; p.OWg = OW;
-        p.in_step = transposed ? 1 : stride;
-        p.out_step = 1; p.out_py = 0; p.out_px = 0;
-        p.ntaps = kh * kw;
-        for (int r = 0; r < kh; ++r)
-            for (int c = 0; c < kw; ++c) {
-                const int t = r * kw + c;
-                p.tap_w[t] = t;
-                p.tap_dy[t] = transposed ? pad - r : r - pad;
-                p.tap_dx[t] = transposed ? pad - c : c - pad;
-            }
-        // the tensor-core launcher answers VQB_ERR_UNSUPPORTED before launching anything when it cannot take the
-        // shape (layouts, channel counts, step table): the FFMA kernels run it then
-        if (want_tc && conv_tc_supported(p)) {
-            const int rc = launch_conv_tc(&p, 1, w_tc, kh * kw, s);
-            if (rc != VQB_ERR_UNSUPPORTED) return rc;
-        }
-        return small ? launch_conv_small_cout(p, s) : launch_conv_ffma(p, s);
-    }
-    // stride-s transposed conv: s*s sub-pixel phases, each a stride-1 gather conv
-    // over the taps whose parity matches (decoder.py:31-35).
-    p.in_step = 1; p.out_step = stride;
-    ConvLaunch phases[4];
+    set_strides(out_layout, Cout, g.OH, g.OW, p.out_sn, p.out_sh, p.out_sw, p.out_sc);
+    auto run_ffma = [&](const ConvPhase &ph) {
+        static_cast<ConvPhase &>(p) = ph;
+        return Cout <= 4 ? launch_conv_small_cout(p, s) : launch_conv_ffma(p, s);
+    };
+    // the wgmma path takes every phase of the layer in one launch (blockIdx.y = phase); a phase no tap reaches still
+    // gets bias/skip/activation
+    const bool tc = precision != VQB_FP32 && stride <= 2 && conv_tc_supported(p);
+    ConvPhase phases[4];
     int nph = 0;
-    const bool tc_multi = want_tc && stride == 2 && conv_tc_supported(p);
-    for (int py = 0; py < stride; ++py)
-        for (int px = 0; px < stride; ++px) {
-            p.out_py = py; p.out_px = px;
-            p.OHg = (OH - py + stride - 1) / stride;
-            p.OWg = (OW - px + stride - 1) / stride;
-            if (p.OHg <= 0 || p.OWg <= 0) continue;
-            int nt = 0;
-            for (int r = 0; r < kh; ++r) {
-                if ((py + pad - r) % stride != 0) continue;
-                for (int c = 0; c < kw; ++c) {
-                    if ((px + pad - c) % stride != 0) continue;
-                    p.tap_w[nt] = r * kw + c;
-                    p.tap_dy[nt] = (py + pad - r) / stride;
-                    p.tap_dx[nt] = (px + pad - c) / stride;
-                    ++nt;
-                }
-            }
-            p.ntaps = nt;
-            int rc;
-            if (nt == 0) {
-                // a phase no tap reaches still gets bias/skip/activation
-                p.ntaps = 0;
-            }
-            if (tc_multi) { phases[nph++] = p; continue; }
-            rc = small ? launch_conv_small_cout(p, s) : launch_conv_ffma(p, s);
-            if (rc != 0) return rc;
-        }
-    if (tc_multi && nph > 0) {
-        const int rc = launch_conv_tc(phases, nph, w_tc, kh * kw, s);   // one launch, blockIdx.y = phase
+    for (int i = 0; i < g.nph; ++i) {
+        ConvPhase ph;
+        if (!conv_phase(g, i, ph)) continue;
+        if (tc) { phases[nph++] = ph; continue; }
+        const int rc = run_ffma(ph);
+        if (rc != 0) return rc;
+    }
+    if (tc && nph > 0) {
+        WgLaunch L;
+        L.in = in; L.B = B; L.Cin = Cin; L.H = H; L.W = W;
+        L.w = w_packed + (size_t)kh * kw * Cin * Cout;              // the K-major region
+        L.ncols = Cout;
+        L.bias = bias; L.skip = skip; L.out = out; L.relu = relu;
+        L.out_sn = p.out_sn; L.out_sh = p.out_sh; L.out_sw = p.out_sw; L.out_sc = p.out_sc;
+        // the launcher answers VQB_ERR_UNSUPPORTED before launching anything when it cannot take the shape (step
+        // table, shared memory): the FFMA kernels run it then
+        const int rc = launch_conv_tc(L, phases, nph, kh * kw, false, s);
         if (rc != VQB_ERR_UNSUPPORTED) return rc;
-        for (int i = 0; i < nph; ++i) {                                 // did not fit: the phases one by one on CUDA cores
-            const int rc2 = small ? launch_conv_small_cout(phases[i], s) : launch_conv_ffma(phases[i], s);
+        for (int i = 0; i < nph; ++i) {
+            const int rc2 = run_ffma(phases[i]);
             if (rc2 != 0) return rc2;
         }
     }
     return 0;
+}
+
+ConvGeom conv_geom(int kh, int kw, int stride, int pad, int transposed, int H, int W) {
+    ConvGeom g = {kh, kw, stride, pad, transposed};
+    g.OH = transposed ? (H - 1) * stride - 2 * pad + kh : (H + 2 * pad - kh) / stride + 1;
+    g.OW = transposed ? (W - 1) * stride - 2 * pad + kw : (W + 2 * pad - kw) / stride + 1;
+    g.nph = transposed ? stride * stride : 1;
+    return g;
+}
+
+// Phase i = py * s + px.  A conv reads in(gy * stride + r - pad) through kernel row r; output row y = s gy + py of a
+// stride-s transposed conv takes input row gy + dy through kernel row r = py + pad - s dy, so phase (py, px) is a
+// stride-1 gather conv over the taps whose (py + pad - r, px + pad - c) are multiples of s.
+bool conv_phase(const ConvGeom &g, int i, ConvPhase &ph) {
+    const int up = g.transposed ? g.stride : 1;
+    ph.in_step = g.transposed ? 1 : g.stride;
+    ph.out_step = up;
+    ph.out_py = i / up; ph.out_px = i % up;
+    ph.OHg = (g.OH - ph.out_py + up - 1) / up;
+    ph.OWg = (g.OW - ph.out_px + up - 1) / up;
+    ph.ntaps = 0;
+    for (int r = 0; r < g.kh; ++r)
+        for (int c = 0; c < g.kw; ++c) {
+            const int ny = g.transposed ? ph.out_py + g.pad - r : r - g.pad;
+            const int nx = g.transposed ? ph.out_px + g.pad - c : c - g.pad;
+            if (ny % up != 0 || nx % up != 0) continue;
+            ph.tap_w[ph.ntaps] = r * g.kw + c;
+            ph.tap_dy[ph.ntaps] = ny / up;
+            ph.tap_dx[ph.ntaps] = nx / up;
+            ++ph.ntaps;
+        }
+    return ph.OHg > 0 && ph.OWg > 0;
 }
 
 extern "C" size_t vqb_vq_workspace_bytes(int64_t N, int K, int D) {
@@ -269,8 +265,8 @@ extern "C" int vqb_residual_layer_f32(const float *r, const float *w1_packed, co
     if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cmid <= 0) return VQB_ERR_BAD_ARG;
     if (precision < VQB_FP32 || precision > VQB_BF16) return VQB_ERR_BAD_ARG;
     if (precision == VQB_BF16) return VQB_ERR_UNSUPPORTED;      // see vqb_residual_layer_bf16
-    if (precision == VQB_TF32 && res_wg_supported(C, Cmid)) {      // one wgmma launch, the intermediate stays on chip
-        const int rc = launch_res_wg(r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
+    if (precision == VQB_TF32 && res_wg_supported(0, C, Cmid)) {      // one wgmma launch, the intermediate stays on chip
+        const int rc = launch_res_wg(0, r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
                                      relu_out, 1, (cudaStream_t)stream);
         if (rc != VQB_ERR_UNSUPPORTED) return rc;
     }
@@ -291,9 +287,9 @@ extern "C" int vqb_residual_stack_f32(const float *r, const float *w1_packed, co
     if (n_layers > 1 && !scratch) return VQB_ERR_BAD_ARG;
     if (precision < VQB_FP32 || precision > VQB_BF16) return VQB_ERR_BAD_ARG;
     if (precision == VQB_BF16) return VQB_ERR_UNSUPPORTED;
-    if (n_layers > 1 && precision == VQB_TF32 && res_wg_supported(C, Cmid)) {
+    if (n_layers > 1 && precision == VQB_TF32 && res_wg_supported(0, C, Cmid)) {
         // all applications in ONE launch when a tile holds whole images (answers VQB_ERR_UNSUPPORTED otherwise)
-        const int rc = launch_res_wg(r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
+        const int rc = launch_res_wg(0, r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
                                      1, n_layers, (cudaStream_t)stream);
         if (rc != VQB_ERR_UNSUPPORTED) return rc;
     }

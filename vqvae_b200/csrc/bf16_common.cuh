@@ -1,4 +1,4 @@
-// bf16_common.cuh -- helpers shared by the bf16 pipeline's sources (hconv.cu, conv_edge.cu).
+// bf16_common.cuh -- helpers shared by the sources that write bf16 (wgconv.cu, conv_edge.cu, vq_exact.cu).
 #pragma once
 #include <cuda_bf16.h>
 
@@ -12,7 +12,3 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 
 
 }  // namespace
-
-// internal weight-packing kind (next to enum vqb_conv_kind): the 1x1 conv of a residual layer, Cmid <= 64 input
-// channels zero-padded to one 64-channel K chunk
-#define VQB_RES_W2_KIND 6

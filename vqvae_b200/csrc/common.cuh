@@ -16,21 +16,38 @@
 #include <stdlib.h>
 static inline const char *vqb_getenv(const char *name) { return VQB_DIAG ? getenv(name) : nullptr; }
 
-// One launch of the generalised gather-form convolution
+// A conv layer on an H x W input: its output size and its sub-pixel phases.  A conv or a stride-1 transposed conv
+// is one phase; a stride-s transposed conv is s*s phases (decoder.py:31-35).  No pointers: the fp32 and the bf16
+// entry points share it.
+struct ConvGeom {
+    int kh, kw, stride, pad, transposed;
+    int OH, OW;
+    int nph;
+};
+
+// One sub-pixel phase of a layer as a gather-form convolution
 //   out[n, gy*out_step+out_py, gx*out_step+out_px, co] =
 //       act( bias[co] + skip + sum_{t<ntaps, ci} in[n, gy*in_step+dy[t], gx*in_step+dx[t], ci]
 //                                                * w[tap_w[t]*Cin + ci][co] )
 // which covers nn.Conv2d (in_step = stride, out_step = 1, dy = r - pad), stride-1
-// nn.ConvTranspose2d (dy = pad - r) and one sub-pixel phase of a stride-2
-// nn.ConvTranspose2d (in_step = 1, out_step = 2, taps of matching parity).
-struct ConvLaunch {
-    const float *in, *w, *bias, *skip;
-    float *out;
-    int B, Cin, H, W, Cout;
-    int OHg, OWg;                 // output grid of this launch
+// nn.ConvTranspose2d (dy = pad - r) and one sub-pixel phase of a stride-s
+// nn.ConvTranspose2d (in_step = 1, out_step = s, taps of matching parity).
+struct ConvPhase {
+    int OHg, OWg;                 // output grid of this phase
     int in_step, out_step, out_py, out_px;
     int ntaps;
     int tap_w[VQB_MAX_TAPS], tap_dy[VQB_MAX_TAPS], tap_dx[VQB_MAX_TAPS];
+};
+
+ConvGeom conv_geom(int kh, int kw, int stride, int pad, int transposed, int H, int W);
+// phase i < g.nph of g; false when its output grid is empty
+bool conv_phase(const ConvGeom &g, int i, ConvPhase &ph);
+
+// One launch of a CUDA-core conv kernel: one phase of a layer on fp32 tensors.
+struct ConvLaunch : ConvPhase {
+    const float *in, *w, *bias, *skip;
+    float *out;
+    int B, Cin, H, W, Cout;
     long long in_sn, in_sh, in_sw, in_sc;      // element strides of `in`
     long long out_sn, out_sh, out_sw, out_sc;  // element strides of `out` (and `skip`)
     int relu;
@@ -38,6 +55,11 @@ struct ConvLaunch {
 
 int launch_conv_ffma(const ConvLaunch &p, cudaStream_t s);
 int launch_conv_small_cout(const ConvLaunch &p, cudaStream_t s);
+
+// The weight vqb_pack_conv_weight_bf16 writes: K-major bf16 rows [kh*kw][Cout][Cin_pad] (zero padded from Cin), or
+// for shuffle != 0 the [9][16][Cin] form of the k4 s2 output layer.
+int launch_pack_weight_bf16(const float *w, void *out, int Cout, int Cin, int Cin_pad, int kh, int kw, int transposed,
+                            int shuffle, cudaStream_t s);
 
 // process-wide count of kernels launched through the C ABI (vqb_launch_count)
 extern unsigned long long g_vqb_launches;

@@ -1,33 +1,38 @@
 // misc.cu -- small bandwidth kernels around the hot path (sm_90a).
+#include <cuda_bf16.h>
+
 #include "common.cuh"
 
 namespace {
 
-// (Cout,Cin,kh,kw) or ConvTranspose (Cin,Cout,kh,kw)  ->  two GEMM operand layouts, back to back:
-//   out[0 .. T)        [(r*kw+s)*Cin + ci][co]   (N-major, the FFMA kernel's B tile)
-//   out[T .. 2T)       [(r*kw+s)][co][ci]        (K-major rows of Cin, the wgmma B operand)
-__global__ void pack_weight_kernel(const float *__restrict__ w, float *__restrict__ out, int Cout, int Cin,
-                                   int kh, int kw, int transposed) {
-    const long long total = (long long)Cout * Cin * kh * kw;
+// (Cout,Cin,kh,kw) or ConvTranspose (Cin,Cout,kh,kw)  ->  the tap-major GEMM operand layouts:
+//   nmajor   [(r*kw+s)*Cin + ci][co]     (N-major, the FFMA kernel's B tile; fp32 only, may be null)
+//   kmajor   [(r*kw+s)][co][ci]          (K-major rows of Cin_pad >= Cin channels, zero padded: the wgmma B operand)
+// T = float or __nv_bfloat16 (rounded to nearest even).  nmajor requires Cin_pad == Cin.
+template <typename T>
+__global__ void pack_weight_kernel(const float *__restrict__ w, float *__restrict__ nmajor, T *__restrict__ kmajor,
+                                   int Cout, int Cin, int Cin_pad, int kh, int kw, int transposed) {
+    const long long total = (long long)Cout * Cin_pad * kh * kw;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
         const int co = (int)(i % Cout);
         long long t = i / Cout;
-        const int ci = (int)(t % Cin);
-        const int tap = (int)(t / Cin);
+        const int ci = (int)(t % Cin_pad);
+        const int tap = (int)(t / Cin_pad);
         const int r = tap / kw, s = tap % kw;
         const long long src = transposed ? ((((long long)ci * Cout + co) * kh + r) * kw + s)
                                          : ((((long long)co * Cin + ci) * kh + r) * kw + s);
-        const float v = w[src];
-        out[i] = v;
-        out[total + ((long long)tap * Cout + co) * Cin + ci] = v;
+        const float v = ci < Cin ? w[src] : 0.f;
+        if (nmajor) nmajor[i] = v;
+        kmajor[((long long)tap * Cout + co) * Cin_pad + ci] = T(v);
     }
 }
 
 // ConvTranspose2d k4 s2 p1 weight (Cin,Cout,4,4), Cout <= 4  ->  [9 neighbour taps (dy,dx)][16][Cin]:
 // row (py*2+px)*Cout+co of tap (dy,dx) holds W[ci][co][py-2dy+1][px-2dx+1] when that kernel index
 // exists (the neighbour contributes to that output phase), else 0.  Read by launch_convt_shuffle_wg (wgconv.cu).
-__global__ void pack_convt_shuffle_kernel(const float *__restrict__ w, float *__restrict__ out, int Cout, int Cin) {
+template <typename T>
+__global__ void pack_convt_shuffle_kernel(const float *__restrict__ w, T *__restrict__ out, int Cout, int Cin) {
     const int total = 9 * 16 * Cin;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
         const int ci = i % Cin, row = (i / Cin) % 16, tap = i / (16 * Cin);
@@ -38,7 +43,7 @@ __global__ void pack_convt_shuffle_kernel(const float *__restrict__ w, float *__
             const int kh = py - 2 * dy + 1, kw = px - 2 * dx + 1;
             if (kh >= 0 && kh < 4 && kw >= 0 && kw < 4) v = w[(((size_t)ci * Cout + co) * 4 + kh) * 4 + kw];
         }
-        out[i] = v;
+        out[i] = T(v);
     }
 }
 
@@ -139,13 +144,25 @@ extern "C" int vqb_pack_conv_weight_f32(const float *w, float *packed, int Cout,
                                         int transposed, void *stream) {
     if (!w || !packed || Cout <= 0 || Cin <= 0 || kh <= 0 || kw <= 0) return VQB_ERR_BAD_ARG;
     const long long total = (long long)Cout * Cin * kh * kw;
-    pack_weight_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(w, packed, Cout, Cin, kh, kw,
-                                                                              transposed);
+    pack_weight_kernel<float><<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(w, packed, packed + total, Cout, Cin,
+                                                                                     Cin, kh, kw, transposed);
     if (transposed && kh == 4 && kw == 4 && Cout <= 4) {
-        pack_convt_shuffle_kernel<<<grid_for(9 * 16 * Cin, 256), 256, 0, (cudaStream_t)stream>>>(w, packed + 2 * total,
-                                                                                               Cout, Cin);
+        pack_convt_shuffle_kernel<float><<<grid_for(9 * 16 * Cin, 256), 256, 0, (cudaStream_t)stream>>>(w, packed + 2 * total,
+                                                                                                      Cout, Cin);
         VQB_COUNT_LAUNCH(1);
     }
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+int launch_pack_weight_bf16(const float *w, void *out, int Cout, int Cin, int Cin_pad, int kh, int kw, int transposed,
+                            int shuffle, cudaStream_t s) {
+    __nv_bfloat16 *o = reinterpret_cast<__nv_bfloat16 *>(out);
+    if (shuffle)
+        pack_convt_shuffle_kernel<<<grid_for(9 * 16 * Cin, 256), 256, 0, s>>>(w, o, Cout, Cin);
+    else
+        pack_weight_kernel<<<grid_for((long long)Cout * Cin_pad * kh * kw, 256), 256, 0, s>>>(w, nullptr, o, Cout, Cin,
+                                                                                            Cin_pad, kh, kw, transposed);
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }

@@ -15,9 +15,8 @@
 //   * N2 > 0 (residual layer of the bf16 pipeline): the first GEMM's result is ReLU'd, rounded to bf16 and written
 //     to shared memory as the A operand of a second GEMM against an N2 x 64 weight tile loaded once, so
 //     out = act(skip + W2 . relu(W1 (*) r)) and the intermediate never leaves the SM.
-#include <cuda_bf16.h>
-
 #include "ptx.cuh"
+#include "bf16_common.cuh"
 #include "wgconv.h"
 #include "wgmma.cuh"
 
@@ -40,11 +39,6 @@ struct WgParams {
     long long out_sn, out_sh, out_sw, out_sc;
     int4 steps[4][WG_MAX_STEPS];              // x = a_c0 | b_c0 << 16, y = dx, z = dy, w = w_row
 };
-
-__device__ __forceinline__ uint32_t bf16x2(float a, float b) {
-    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<const uint32_t *>(&h);
-}
 
 // Epilogue of one accumulator fragment (wgmma D layout, see wgmma.cuh) for the pixel rows of this thread.
 template <int N>
@@ -90,7 +84,7 @@ __device__ __forceinline__ void store_tile(const WgParams &p, const float *acc, 
                     v0 += __bfloat162float(sk.x); v1 += __bfloat162float(sk.y);
                 }
                 if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                *reinterpret_cast<uint32_t *>(reinterpret_cast<__nv_bfloat16 *>(p.out) + ob + c) = bf16x2(v0, v1);
+                *reinterpret_cast<uint32_t *>(reinterpret_cast<__nv_bfloat16 *>(p.out) + ob + c) = pack_bf16(v0, v1);
             } else {
                 if (skip) {
                     // plain load: with chained applications skip is `out`, written earlier by this kernel
@@ -221,7 +215,7 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
                         float v0 = 0.f, v1 = 0.f;
                         if (j < N / 8 && c < p.mid_cols) { v0 = fmaxf(acc[4 * j + 2 * h], 0.f); v1 = fmaxf(acc[4 * j + 2 * h + 1], 0.f); }
                         const uint32_t addr = rb + (uint32_t)(((j ^ (row & 7)) << 4) + cq * 2);
-                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(bf16x2(v0, v1)) : "memory");
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16(v0, v1)) : "memory");
                     }
                 } else {
 #pragma unroll
@@ -392,96 +386,95 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     return vqb_cuda_status(cudaGetLastError());
 }
 
-// ------------------------------------------------------------------------------------------------ TF32 entry
+// ------------------------------------------------------------------------------------------------ layer launchers
+// The k-steps of one phase: each tap of the phase x each 128-byte channel chunk (32 fp32 / 64 bf16 channels), tap t
+// reading the N weight rows from tap_w[t] * rows_per_tap.  Every k-step adds into the fp32 accumulators, so the
+// order fixes the result bits: tap outer / chunk inner, or chunk outer / tap inner (chunk_outer).
+static bool set_phase(WgLaunch &L, int i, const ConvPhase &ph, int rows_per_tap, bool chunk_outer) {
+    const int ck = L.bf16 ? 64 : 32, nc = L.Cin / ck;
+    if (ph.ntaps * nc > WG_MAX_STEPS) return false;
+    L.in_step = ph.in_step; L.out_step = ph.out_step;
+    L.OHg[i] = ph.OHg; L.OWg[i] = ph.OWg; L.out_py[i] = ph.out_py; L.out_px[i] = ph.out_px;
+    int n = 0;
+    for (int a = 0; a < (chunk_outer ? nc : ph.ntaps); ++a)
+        for (int b = 0; b < (chunk_outer ? ph.ntaps : nc); ++b) {
+            const int t = chunk_outer ? b : a, c0 = (chunk_outer ? a : b) * ck;
+            L.steps[i][n++] = WgStep{c0, c0, ph.tap_dx[t], ph.tap_dy[t], ph.tap_w[t] * rows_per_tap};
+        }
+    L.nsteps[i] = n;
+    return true;
+}
+
+// the 3x3 neighbourhood of an output pixel of a stride-1 layer: taps t = r * 3 + s, dy = r - 1, dx = s - 1
+static ConvPhase taps3x3(int H, int W) {
+    ConvPhase ph;
+    conv_phase(conv_geom(3, 3, 1, 1, 0, H, W), 0, ph);
+    return ph;
+}
+
 bool conv_tc_supported(const ConvLaunch &p) {
     const bool in_nhwc = p.in_sc == 1 && p.in_sw == p.Cin;
     const bool out_nhwc = p.out_sc == 1 && p.out_sw == p.Cout;
     return in_nhwc && out_nhwc && p.Cin % 32 == 0 && p.Cout % 16 == 0 && p.Cout >= 16 && p.Cout <= 256 &&
-           p.in_step >= 1 && p.in_step <= 2 &&
            (reinterpret_cast<uintptr_t>(p.in) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 &&
            (p.skip == nullptr || (reinterpret_cast<uintptr_t>(p.skip) & 15) == 0);
 }
 
-// ph[0..nph): the phases of ONE layer (same tensors, strides and steps; they differ in the output grid, the
-// sub-pixel offset and the tap list).  w_tc: tap-major K-major weight [tap][Cout][Cin] (vqb_pack_conv_weight_f32,
-// second half).
-int launch_conv_tc(const ConvLaunch *ph, int nph, const float *w_tc, int total_taps, cudaStream_t s) {
+int launch_conv_tc(WgLaunch &L, const ConvPhase *ph, int nph, int total_taps, bool chunk_outer, cudaStream_t s) {
     if (nph < 1 || nph > 4) return VQB_ERR_UNSUPPORTED;
-    const ConvLaunch &p = ph[0];
-    WgLaunch L;
-    L.bf16 = 0;
-    L.in = p.in; L.B = p.B; L.Cin = p.Cin; L.H = p.H; L.W = p.W; L.in_step = p.in_step;
-    L.w = w_tc; L.w_rows = (long long)total_taps * p.Cout; L.w_inner = p.Cin;
-    L.N = wg_gemm_cols(p.Cout); L.ncols = p.Cout;
-    L.bias = p.bias; L.skip = p.skip; L.out = p.out; L.relu = p.relu;
-    L.out_step = p.out_step; L.out_sn = p.out_sn; L.out_sh = p.out_sh; L.out_sw = p.out_sw; L.out_sc = p.out_sc;
+    L.w_rows = (long long)total_taps * L.ncols; L.w_inner = L.Cin;
+    L.N = wg_gemm_cols(L.ncols);
     L.nph = nph;
-    const int kchunks = p.Cin / 32;
-    for (int i = 0; i < nph; ++i) {
-        const ConvLaunch &r = ph[i];
-        if (r.ntaps * kchunks > WG_MAX_STEPS) return VQB_ERR_UNSUPPORTED;
-        L.OHg[i] = r.OHg; L.OWg[i] = r.OWg; L.out_py[i] = r.out_py; L.out_px[i] = r.out_px;
-        int n = 0;
-        for (int t = 0; t < r.ntaps; ++t)
-            for (int cc = 0; cc < kchunks; ++cc)
-                L.steps[i][n++] = WgStep{0, cc * 32, r.tap_dx[t], r.tap_dy[t], r.tap_w[t] * p.Cout};
-        for (int t = 0; t < n; ++t) L.steps[i][t].a_c0 = L.steps[i][t].b_c0;
-        L.nsteps[i] = n;
-    }
+    for (int i = 0; i < nph; ++i)
+        if (!set_phase(L, i, ph[i], L.ncols, chunk_outer)) return VQB_ERR_UNSUPPORTED;
     return launch_wgconv(L, s);
 }
 
-// ------------------------------------------------------------------------------------------------ TF32 residual layer
-// residual.py:18-29 on fp32 NHWC activations: per 128-pixel tile the 3x3 GEMM (C -> Cmid), ReLU, the 1x1 GEMM (Cmid -> C)
-// on the fp32 intermediate held in shared memory, + r, ReLU -- the arithmetic of the two separate conv launches (same
-// k-step order, same TF32 operands), in one launch.  napps > 1 (a ResidualStack of one shared layer): whole images per
-// tile, every application inside the same launch, the activation round-tripping through `out` (L2) between them.
-bool res_wg_supported(int C, int Cmid) { return (C == 64 || C == 128) && (Cmid == 32 || Cmid == 64); }
+// ------------------------------------------------------------------------------------------------ residual layer
+// residual.py:18-29 on NHWC activations: per 128-pixel tile the 3x3 GEMM (C -> Cmid), ReLU, the 1x1 GEMM (Cmid -> C)
+// on the intermediate held in shared memory (fp32, or rounded to bf16), + r, ReLU.  In TF32 this is the arithmetic of
+// the two separate conv launches (same k-step order, same TF32 operands), in one launch.  napps > 1 (a ResidualStack
+// of one shared layer): whole images per tile, every application inside the same launch, the activation
+// round-tripping through `out` (L2) between them.
+bool res_wg_supported(int bf16, int C, int Cmid) {
+    return (C == 64 || C == 128) && (bf16 ? Cmid % 16 == 0 && Cmid >= 16 && Cmid <= 64 : Cmid == 32 || Cmid == 64);
+}
 
-int launch_res_wg(const float *r, const float *w1_tc, const float *w2_tc, float *out, int B, int H, int W, int C, int Cmid,
+// w1: [9][Cmid][C]; w2: [C][Cmid] (TF32) or [C][64] (bf16, Cmid zero padded to one chunk)
+int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void *out, int B, int H, int W, int C, int Cmid,
                   int relu_out, int napps, cudaStream_t s) {
-    if (!res_wg_supported(C, Cmid) || r == out) return VQB_ERR_UNSUPPORTED;
+    if (!res_wg_supported(bf16, C, Cmid) || r == out) return VQB_ERR_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(out)) & 15) return VQB_ERR_UNSUPPORTED;
     WgLaunch L;
-    L.bf16 = 0;
-    L.in = r; L.B = B; L.Cin = C; L.H = H; L.W = W; L.in_step = 1;
-    L.w = w1_tc; L.w_rows = 9LL * Cmid; L.w_inner = C;
-    L.N = Cmid; L.ncols = Cmid;
-    L.w2 = w2_tc; L.w2_rows = C; L.w2_inner = Cmid; L.N2 = C;
-    L.skip = r; L.out = out; L.relu = relu_out; L.napps = napps;
+    L.bf16 = bf16;
+    L.in = r; L.B = B; L.Cin = C; L.H = H; L.W = W;
+    L.w = w1; L.w_rows = 9LL * Cmid; L.w_inner = C;
+    L.N = wg_gemm_cols(Cmid); L.ncols = Cmid;
+    L.w2 = w2; L.w2_rows = C; L.w2_inner = bf16 ? 64 : Cmid; L.N2 = C;
+    L.skip = r; L.out = out; L.out_bf16 = bf16; L.relu = relu_out; L.napps = napps;
     L.out_sn = (long long)H * W * C; L.out_sh = (long long)W * C; L.out_sw = C; L.out_sc = 1;
-    L.nph = 1; L.OHg[0] = H; L.OWg[0] = W;
-    int n = 0;
-    for (int t = 0; t < 9; ++t)                  // tap-major, then 32-channel chunks: the order of launch_conv_tc
-        for (int cc = 0; cc < C / 32; ++cc)
-            L.steps[0][n++] = WgStep{cc * 32, cc * 32, t % 3 - 1, t / 3 - 1, t * Cmid};
-    L.nsteps[0] = n;
+    set_phase(L, 0, taps3x3(H, W), Cmid, bf16);
     return launch_wgconv(L, s);
 }
 
-// ------------------------------------------------------------------------------------------------ TF32 output layer
-// decoder.py:34-35, ConvTranspose2d(Cin -> Cout <= 4, k4 s2 p1), NHWC fp32 in, NCHW fp32 out: one GEMM over the
+// ------------------------------------------------------------------------------------------------ output layer
+// decoder.py:34-35, ConvTranspose2d(Cin -> Cout <= 4, k4 s2 p1), NHWC in, NCHW fp32 out: one GEMM over the
 // 3x3 input neighbourhood with N = 16 columns (sub-pixel phase, channel) and a pixel-shuffle epilogue.
-// w_shuffle: the third region of vqb_pack_conv_weight_f32, [9 taps (dy, dx)][16][Cin].
+// w_shuffle: [9 taps (dy, dx)][16][Cin] (the third region of vqb_pack_conv_weight_f32, or vqb_pack_conv_weight_bf16).
 bool convt_shuffle_supported(int Cin, int Cout) { return Cout >= 1 && Cout <= 4 && Cin % 32 == 0 && 9 * (Cin / 32) <= WG_MAX_STEPS; }
 
-int launch_convt_shuffle_wg(const float *in, const float *w_shuffle, const float *bias, float *out, int B, int Cin, int H,
-                            int W, int Cout, int relu, cudaStream_t s) {
+int launch_convt_shuffle_wg(int bf16, const void *in, const void *w_shuffle, const float *bias, float *out, int B, int Cin,
+                            int H, int W, int Cout, int relu, cudaStream_t s) {
     if (!convt_shuffle_supported(Cin, Cout)) return VQB_ERR_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(w_shuffle)) & 15) return VQB_ERR_UNSUPPORTED;
     WgLaunch L;
-    L.bf16 = 0;
-    L.in = in; L.B = B; L.Cin = Cin; L.H = H; L.W = W; L.in_step = 1;
+    L.bf16 = bf16;
+    L.in = in; L.B = B; L.Cin = Cin; L.H = H; L.W = W;
     L.w = w_shuffle; L.w_rows = 9LL * 16; L.w_inner = Cin;
     L.N = 16; L.ncols = 4 * Cout; L.shuffle_cg = Cout;
     L.bias = bias; L.out = out; L.relu = relu;
     const int OH = 2 * H, OW = 2 * W;
     L.out_sn = (long long)Cout * OH * OW; L.out_sc = (long long)OH * OW; L.out_sh = OW; L.out_sw = 1;
-    L.nph = 1; L.OHg[0] = H; L.OWg[0] = W;
-    int n = 0;
-    for (int t = 0; t < 9; ++t)
-        for (int cc = 0; cc < Cin / 32; ++cc)
-            L.steps[0][n++] = WgStep{cc * 32, cc * 32, t % 3 - 1, t / 3 - 1, t * 16};
-    L.nsteps[0] = n;
+    set_phase(L, 0, taps3x3(H, W), 16, bf16);
     return launch_wgconv(L, s);
 }

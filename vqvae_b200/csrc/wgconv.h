@@ -38,9 +38,17 @@ struct WgLaunch {
 
 int launch_wgconv(const WgLaunch &L, cudaStream_t s);
 int wg_gemm_cols(int ncols);           // smallest supported N >= ncols, 0 if none
-bool res_wg_supported(int C, int Cmid);
-bool convt_shuffle_supported(int Cin, int Cout);
-int launch_convt_shuffle_wg(const float *in, const float *w_shuffle, const float *bias, float *out, int B, int Cin, int H,
-                            int W, int Cout, int relu, cudaStream_t s);
-int launch_res_wg(const float *r, const float *w1_tc, const float *w2_tc, float *out, int B, int H, int W, int C, int Cmid,
+
+// The layer launchers take the operand type (bf16 = 0: fp32 activations read as TF32, 1: bf16) and a weight of
+// K-major rows per tap, [tap][rows][Cin], as vqb_pack_conv_weight_f32 (its K-major regions) and
+// vqb_pack_conv_weight_bf16 write them.
+bool conv_tc_supported(const ConvLaunch &p);
+// L: the tensors, ncols = Cout, output strides and epilogue of one layer; ph[0..nph): its phases, one launch
+// (blockIdx.y = phase) over the weight [total_taps][Cout][Cin]
+int launch_conv_tc(WgLaunch &L, const ConvPhase *ph, int nph, int total_taps, bool chunk_outer, cudaStream_t s);
+bool res_wg_supported(int bf16, int C, int Cmid);
+int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void *out, int B, int H, int W, int C, int Cmid,
                   int relu_out, int napps, cudaStream_t s);
+bool convt_shuffle_supported(int Cin, int Cout);
+int launch_convt_shuffle_wg(int bf16, const void *in, const void *w_shuffle, const float *bias, float *out, int B, int Cin,
+                            int H, int W, int Cout, int relu, cudaStream_t s);

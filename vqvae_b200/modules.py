@@ -72,8 +72,8 @@ def _param_tag(param):
 
 class _PackedWeights:
     """Packed conv weights cached ON the parameter object (so the cache dies with it) per packing kind:
-    ("f32", transposed) = the tap-major fp32 layouts of vqb_pack_conv_weight_f32, ("bf16", kind) = the k-step-ordered
-    bf16 layout of vqb_pack_conv_weight_bf16.  When the parameter changes (load_state_dict, optimizer step, .to())
+    ("f32", transposed) = the tap-major fp32 layouts of vqb_pack_conv_weight_f32, ("bf16", kind) = the same K-major
+    layout in bf16, from vqb_pack_conv_weight_bf16.  When the parameter changes (load_state_dict, optimizer step, .to())
     the SAME device buffer is repacked in place whenever its size still fits, so CUDA graphs captured around a
     forward keep reading current weights after ``repack`` (HostPipeline checks the tags before every replay)."""
 

@@ -118,7 +118,7 @@ def conv_kind(kh, stride, transposed, cout):
 
 
 def pack_conv_weight_bf16(w, kind, out=None):
-    """fp32 conv / conv-transpose weight -> the bf16 k-step-ordered packing of vqb_pack_conv_weight_bf16
+    """fp32 conv / conv-transpose weight -> the bf16 K-major tap-major packing of vqb_pack_conv_weight_bf16
     (None when the shape is not covered).  `out`: repack into an existing buffer (same shape) in place."""
     _require_cuda(w, "weight")
     w = _f32c(w.detach())
