@@ -123,6 +123,33 @@ def test_default_precision_is_the_reference_gpu_arithmetic():
         vqvae_b200.set_precision("fp8")
 
 
+@pytest.mark.parametrize("args, distinct_layers, covered", [
+    ((128, 32, 2, 512, 64), False, True),        # cfg2
+    ((128, 16, 2, 512, 64), False, True),        # res_h_dim: one 16-channel step ...
+    ((128, 64, 2, 512, 64), False, True),        # ... up to 64
+    ((128, 80, 2, 512, 64), False, False),
+    ((128, 32, 0, 512, 64), False, True),        # no residual layers
+    ((64, 32, 2, 512, 64), False, False),        # the input conv must write 64 channels
+    ((256, 32, 2, 512, 64), False, False),
+    ((128, 32, 2, 512, 32), False, False),       # the bf16-z_q VQ takes D = 64 only
+    ((128, 32, 2, 512, 64), True, False),        # not the reference's one shared ResidualLayer
+])
+def test_bf16_pipeline_coverage(args, distinct_layers, covered):
+    """Which architectures the fused bf16 forward covers; the others run the TF32 kernels (with a warning)."""
+    import warnings
+    import vqvae_b200
+    from models.residual import ResidualLayer
+    h_dim, res_h_dim, n_res, K, D = args
+    m = vqvae_b200.VQVAE(h_dim, res_h_dim, n_res, K, D, 0.25)
+    if distinct_layers:
+        for st in (m.encoder.conv_stack[5], m.decoder.inverse_conv_stack[1]):
+            st.stack = torch.nn.ModuleList([ResidualLayer(h_dim, h_dim, res_h_dim) for _ in range(n_res)])
+    with vqvae_b200.precision("bf16"), warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        assert m._bf16_pipeline() is covered
+    assert m._bf16_pipeline() is False           # other precisions never take the bf16 pipeline
+
+
 def test_new_entry_points_validate_arguments_without_a_gpu():
     """bf16 pipeline entry points: bad arguments / unsupported shapes are rejected before any CUDA call."""
     from vqvae_b200 import _lib

@@ -24,8 +24,7 @@ import torch.nn as nn
 
 from . import ops
 from .dist import reduce_vq_stats
-from ._lib import (CONV_K1, CONV_K3, CONV_K4S2, CONVT_K3, CONVT_K4S2, CONVT_K4S2_OUT, NCHW, NHWC, PRECISIONS,
-                   RES_W2)
+from ._lib import NCHW, NHWC, PRECISIONS, RES_W2
 
 # Default = what the reference itself computes on a GPU: fp32 tensors, convolutions on tensor cores in TF32 with fp32
 # accumulation (PyTorch's torch.backends.cudnn.allow_tf32 default, SURVEY 2.2), bit-exact fp32 VQ.
@@ -70,38 +69,41 @@ def _param_tag(param):
     return (ver, param.data_ptr(), str(param.device))
 
 
-class _PackedWeights:
-    """Packed conv weights cached ON the parameter object (so the cache dies with it) per packing kind:
-    ("f32", transposed) = the tap-major fp32 layouts of vqb_pack_conv_weight_f32, ("bf16", kind) = the same K-major
-    layout in bf16, from vqb_pack_conv_weight_bf16.  When the parameter changes (load_state_dict, optimizer step, .to())
-    the SAME device buffer is repacked in place whenever its size still fits, so CUDA graphs captured around a
-    forward keep reading current weights after ``repack`` (HostPipeline checks the tags before every replay)."""
-
-    def get(self, param, key):
-        tag = _param_tag(param)
-        cache = getattr(param, "_vqb_packed", None)
-        if cache is None:
-            cache = {}
-            param._vqb_packed = cache
-        hit = cache.get(key)
-        if hit is not None and hit[0] == tag and tag[0] is not None:
-            return hit[1]
-        old = hit[1] if hit is not None and hit[1] is not None and hit[1].device == param.device else None
-        if key[0] == "f32":
-            buf = ops.pack_conv_weight(param, key[1], out=old)
-        else:
-            buf = ops.pack_conv_weight_bf16(param, key[1], out=old)
-        cache[key] = (tag, buf)
-        return buf
-
-    def f32(self, param, transposed):
-        return self.get(param, ("f32", bool(transposed)))
-
-    def bf16(self, param, kind):
-        return self.get(param, ("bf16", int(kind)))
+def _pack_key(conv, bf16):
+    """The packing of a conv container's weight that the forward reads in a mode: ("f32", transposed), the tap-major
+    fp32 layouts of vqb_pack_conv_weight_f32, or in the bf16 pipeline ("bf16", kind), the same K-major layout in bf16
+    from vqb_pack_conv_weight_bf16, for the kind the layer's geometry names.  A container that the bf16 pipeline
+    reads differently carries its key as ``_bf16_key``, set by the module that builds it."""
+    transposed = isinstance(conv, nn.ConvTranspose2d)
+    if not bf16:
+        return ("f32", transposed)
+    return getattr(conv, "_bf16_key", None) or \
+        ("bf16", ops.conv_kind(conv.kernel_size[0], conv.stride[0], transposed, conv.out_channels))
 
 
-_PACKED = _PackedWeights()
+def _packed(param, key):
+    """The packing `key` (see _pack_key) of a conv weight, cached ON the parameter object (so the cache dies with it).
+    When the parameter changes (load_state_dict, optimizer step, .to()) the SAME device buffer is repacked in place
+    whenever its size still fits, so CUDA graphs captured around a forward keep reading current weights after
+    ``repack`` (HostPipeline checks the tags before every replay)."""
+    tag = _param_tag(param)
+    cache = getattr(param, "_vqb_packed", None)
+    if cache is None:
+        cache = {}
+        param._vqb_packed = cache
+    hit = cache.get(key)
+    if hit is not None and hit[0] == tag and tag[0] is not None:
+        return hit[1]
+    old = hit[1] if hit is not None and hit[1] is not None and hit[1].device == param.device else None
+    pack = ops.pack_conv_weight if key[0] == "f32" else ops.pack_conv_weight_bf16
+    buf = pack(param, key[1], out=old)
+    cache[key] = (tag, buf)
+    return buf
+
+
+def _convs(module):
+    """Every conv container under `module`, each once (a shared ResidualLayer included once)."""
+    return [m for m in module.modules() if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d))]
 
 
 _INVALIDATIONS = {"n": 0}
@@ -138,16 +140,22 @@ def _bias(conv):
     return b if b.dtype == torch.float32 else b.float()
 
 
-def _run_conv(conv, x, B, H, W, *, in_layout=NHWC, out_layout=NHWC, relu=False, skip=None):
-    """Forward of one nn.Conv2d / nn.ConvTranspose2d container through vqb_conv2d_f32."""
-    transposed = isinstance(conv, nn.ConvTranspose2d)
+def _run_conv(conv, x, B, H, W, bf16=False, *, in_layout=NHWC, out_layout=NHWC, relu=False, out_f32=False):
+    """Forward of one nn.Conv2d / nn.ConvTranspose2d container -> (output, OH, OW): vqb_conv2d_f32 on fp32
+    activations in `in_layout` / `out_layout`, or (bf16) vqb_conv2d_bf16 on bf16 NHWC activations, fp32 out if
+    `out_f32` (the output layer's kind always writes the fp32 NCHW module output)."""
     kh, kw = conv.kernel_size
     stride, pad = conv.stride[0], conv.padding[0]
-    w = _PACKED.f32(conv.weight, transposed)
-    return ops.conv2d(x, w, _bias(conv), B=B, Cin=conv.in_channels, H=H, W=W, Cout=conv.out_channels,
-                      kh=kh, kw=kw, stride=stride, pad=pad, transposed=transposed, in_layout=in_layout,
-                      out_layout=out_layout, relu=relu, skip=skip,
-                      precision=_conv_precision())
+    key = _pack_key(conv, bf16)
+    w = _packed(conv.weight, key)
+    if bf16:
+        y = ops.conv2d_bf16(x, w, _bias(conv), B=B, Cin=conv.in_channels, H=H, W=W, Cout=conv.out_channels,
+                            kind=key[1], relu=relu, out_f32=out_f32)
+    else:
+        y = ops.conv2d(x, w, _bias(conv), B=B, Cin=conv.in_channels, H=H, W=W, Cout=conv.out_channels,
+                       kh=kh, kw=kw, stride=stride, pad=pad, transposed=key[1], in_layout=in_layout,
+                       out_layout=out_layout, relu=relu, precision=_conv_precision())
+    return (y,) + ops.conv_out_hw(H, W, kh, kw, stride, pad, isinstance(conv, nn.ConvTranspose2d))
 
 
 def _prep_input(x, channels, what):
@@ -162,6 +170,18 @@ def _prep_input(x, channels, what):
     return x if x.is_contiguous() else x.contiguous()
 
 
+def _prep_relu_input(x, channels, what, in_place=True):
+    """(relu(x) NHWC, B, H, W) for a residual module's forward.  Q2: nn.ReLU(True) rewrites the caller's tensor before
+    the sum is formed, so with `in_place` a contiguous fp32 `x` is ReLU'd where it lies."""
+    xp = _prep_input(x, channels, what)
+    B, _, H, W = xp.shape
+    if in_place and x.is_contiguous() and x.dtype == torch.float32 and not x.requires_grad:
+        xp = ops.relu_(x)
+    else:
+        xp = ops.relu_(xp.clone())
+    return ops.nchw_to_nhwc(xp), B, H, W
+
+
 class ResidualLayer(nn.Module):
     """One residual layer (reference models/residual.py:8-29)."""
 
@@ -173,26 +193,21 @@ class ResidualLayer(nn.Module):
             nn.ReLU(True),
             nn.Conv2d(res_h_dim, h_dim, kernel_size=1, stride=1, bias=False),
         )
+        self.res_block[3]._bf16_key = ("bf16", RES_W2)      # bf16: the fused layer's second GEMM, Cmid padded to 64
 
-    def _apply_nhwc(self, r, B, H, W, relu_out):
-        """r = relu(x) in NHWC.  Returns r + W2.relu(W1 (*) r), optionally ReLU'd
-        (the next consumer always applies ReLU first, residual.py:19,50)."""
+    def _apply_nhwc(self, r, B, H, W, relu_out, bf16=False):
+        """r = relu(x) in NHWC (bf16 in the bf16 pipeline).  Returns r + W2.relu(W1 (*) r), optionally ReLU'd
+        (the next consumer always applies ReLU first, residual.py:19,50).  One fused launch in either mode."""
         c1, c2 = self.res_block[1], self.res_block[3]
-        return ops.residual_layer(r, _PACKED.f32(c1.weight, False), _PACKED.f32(c2.weight, False), B=B, H=H, W=W,
-                                  C=c1.in_channels, Cmid=c1.out_channels, relu_out=relu_out,
+        w1, w2 = _packed(c1.weight, _pack_key(c1, bf16)), _packed(c2.weight, _pack_key(c2, bf16))
+        if bf16:
+            return ops.residual_layer_bf16(r, w1, w2, B=B, H=H, W=W, C=c1.in_channels, Cmid=c1.out_channels,
+                                           relu_out=relu_out)
+        return ops.residual_layer(r, w1, w2, B=B, H=H, W=W, C=c1.in_channels, Cmid=c1.out_channels, relu_out=relu_out,
                                   precision=_conv_precision())
 
     def forward(self, x):
-        xin = x
-        x = _prep_input(x, self.res_block[1].in_channels, "ResidualLayer")
-        B, _, H, W = x.shape
-        # Q2: nn.ReLU(True) rewrites the caller's tensor before the sum is formed.
-        if xin.is_contiguous() and xin.dtype == torch.float32 and not xin.requires_grad:
-            ops.relu_(xin)
-            x = xin
-        else:
-            x = ops.relu_(x.clone())
-        r = ops.nchw_to_nhwc(x)
+        r, B, H, W = _prep_relu_input(x, self.res_block[1].in_channels, "ResidualLayer")
         return ops.nhwc_to_nchw(self._apply_nhwc(r, B, H, W, relu_out=False))
 
 
@@ -204,50 +219,27 @@ class ResidualStack(nn.Module):
         self.n_res_layers = n_res_layers
         self.stack = nn.ModuleList([ResidualLayer(in_dim, h_dim, res_h_dim)] * n_res_layers)
 
-    def _apply_nhwc(self, r, B, H, W):
-        """r = relu(stack input), NHWC.  Output = the stack's result (post F.relu)."""
+    def _apply_nhwc(self, r, B, H, W, bf16=False):
+        """r = relu(stack input), NHWC (bf16 in the bf16 pipeline).  Output = the stack's result (post F.relu)."""
         if len(self.stack) == 0:
             return r
         layer = self.stack[0]
-        if any(l is not layer for l in self.stack):      # not the reference's [layer] * n construction
+        # bf16: one launch per application.  fp32 / tf32: one per layer when the layers are not the reference's
+        # [layer] * n construction, else the whole stack in one call.
+        if bf16 or any(l is not layer for l in self.stack):
             for l in self.stack:
-                r = l._apply_nhwc(r, B, H, W, relu_out=True)
+                r = l._apply_nhwc(r, B, H, W, relu_out=True, bf16=bf16)
             return r
         c1, c2 = layer.res_block[1], layer.res_block[3]
-        return ops.residual_stack(r, _PACKED.f32(c1.weight, False), _PACKED.f32(c2.weight, False), B=B, H=H, W=W,
-                                  C=c1.in_channels, Cmid=c1.out_channels, n_layers=len(self.stack),
+        return ops.residual_stack(r, _packed(c1.weight, _pack_key(c1, False)), _packed(c2.weight, _pack_key(c2, False)),
+                                  B=B, H=H, W=W, C=c1.in_channels, Cmid=c1.out_channels, n_layers=len(self.stack),
                                   precision=_conv_precision())
-
-    def _bf16_ok(self):
-        if len(self.stack) == 0:
-            return True
-        layer = self.stack[0]
-        c1 = layer.res_block[1]
-        return all(l is layer for l in self.stack) and c1.in_channels in (64, 128) and \
-            c1.out_channels % 16 == 0 and c1.out_channels <= 64
-
-    def _apply_nhwc_bf16(self, r, B, H, W):
-        """bf16 NHWC twin of _apply_nhwc: one wgmma launch per application of the shared layer."""
-        if len(self.stack) == 0:
-            return r
-        c1, c2 = self.stack[0].res_block[1], self.stack[0].res_block[3]
-        w1, w2 = _PACKED.bf16(c1.weight, CONV_K3), _PACKED.bf16(c2.weight, RES_W2)
-        for _ in range(len(self.stack)):
-            r = ops.residual_layer_bf16(r, w1, w2, B=B, H=H, W=W, C=c1.in_channels, Cmid=c1.out_channels, relu_out=True)
-        return r
 
     def forward(self, x):
         ch = self.stack[0].res_block[1].in_channels if len(self.stack) else x.shape[1]
-        xin = x
-        x = _prep_input(x, ch, "ResidualStack")
-        B, _, H, W = x.shape
-        if len(self.stack) and xin.is_contiguous() and xin.dtype == torch.float32 \
-                and not xin.requires_grad:
-            ops.relu_(xin)      # side effect of the first layer's in-place ReLU (Q2)
-            x = xin
-        else:
-            x = ops.relu_(x.clone())
-        return ops.nhwc_to_nchw(self._apply_nhwc(ops.nchw_to_nhwc(x), B, H, W))
+        # an empty stack has no in-place ReLU: only its final F.relu, on a copy
+        r, B, H, W = _prep_relu_input(x, ch, "ResidualStack", in_place=len(self.stack) > 0)
+        return ops.nhwc_to_nchw(self._apply_nhwc(r, B, H, W))
 
 
 class Encoder(nn.Module):
@@ -264,39 +256,23 @@ class Encoder(nn.Module):
             nn.Conv2d(h_dim, h_dim, kernel_size=kernel - 1, stride=stride - 1, padding=1),
             ResidualStack(h_dim, h_dim, res_h_dim, n_res_layers),
         )
+        self.conv_stack[0]._bf16_key = ("f32", False)      # bf16: vqb_conv_in_bf16 reads the fp32 packing
 
-    def _forward_nhwc(self, x):
-        """x: prepared NCHW fp32 CUDA tensor -> (NHWC activation, B, H, W)."""
+    def _forward_nhwc(self, x, bf16=False):
+        """x: prepared NCHW fp32 CUDA tensor -> (NHWC activation, bf16 in the bf16 pipeline, B, H, W)."""
         B, _, H, W = x.shape
         cs = self.conv_stack
-        h = _run_conv(cs[0], x, B, H, W, in_layout=NCHW, relu=True)
-        H, W = h.shape[1], h.shape[2]
-        h = _run_conv(cs[2], h, B, H, W, relu=True)
-        H, W = h.shape[1], h.shape[2]
+        if bf16:      # the 3-channel image has its own entry point: fp32 NCHW in, bf16 NHWC out
+            h = ops.conv_in_bf16(x, _packed(cs[0].weight, _pack_key(cs[0], True)), _bias(cs[0]), B=B, H=H, W=W,
+                                 Cout=cs[0].out_channels, relu=True)
+            H, W = H // 2, W // 2
+        else:
+            h, H, W = _run_conv(cs[0], x, B, H, W, in_layout=NCHW, relu=True)
+        h, H, W = _run_conv(cs[2], h, B, H, W, bf16, relu=True)
         # the only consumer of conv 4 is the stack, whose first op is ReLU (or, with an
         # empty stack, its final F.relu): fold that ReLU into this epilogue (Q2/Q3).
-        h = _run_conv(cs[4], h, B, H, W, relu=True)
-        h = cs[5]._apply_nhwc(h, B, H, W)
-        return h, B, H, W
-
-    def _bf16_ok(self):
-        cs = self.conv_stack
-        return (cs[0].in_channels == 3 and cs[0].out_channels == 64 and cs[2].out_channels % 16 == 0
-                and cs[2].out_channels <= 256 and cs[4].in_channels % 64 == 0 and cs[4].in_channels <= 512
-                and cs[5]._bf16_ok())
-
-    def _forward_nhwc_bf16(self, x):
-        """VQB_BF16 pipeline: fp32 NCHW image -> bf16 NHWC latent activation (ReLU of the stack applied)."""
-        B, _, H, W = x.shape
-        cs = self.conv_stack
-        h = ops.conv_in_bf16(x, _PACKED.f32(cs[0].weight, False), _bias(cs[0]), B=B, H=H, W=W, Cout=cs[0].out_channels, relu=True)
-        H, W = H // 2, W // 2
-        h = ops.conv2d_bf16(h, _PACKED.bf16(cs[2].weight, CONV_K4S2), _bias(cs[2]), B=B, Cin=cs[2].in_channels, H=H, W=W,
-                            Cout=cs[2].out_channels, kind=CONV_K4S2, relu=True)
-        H, W = H // 2, W // 2
-        h = ops.conv2d_bf16(h, _PACKED.bf16(cs[4].weight, CONV_K3), _bias(cs[4]), B=B, Cin=cs[4].in_channels, H=H, W=W,
-                            Cout=cs[4].out_channels, kind=CONV_K3, relu=True)      # the stack's first ReLU folded in (Q2/Q3)
-        h = cs[5]._apply_nhwc_bf16(h, B, H, W)
+        h, H, W = _run_conv(cs[4], h, B, H, W, bf16, relu=True)
+        h = cs[5]._apply_nhwc(h, B, H, W, bf16)
         return h, B, H, W
 
     def forward(self, x):
@@ -319,33 +295,13 @@ class Decoder(nn.Module):
             nn.ConvTranspose2d(h_dim // 2, 3, kernel_size=kernel, stride=stride, padding=1),
         )
 
-    def _forward_from_nhwc(self, z, B, H, W):
-        """z: NHWC (B,H,W,in_dim) -> x_hat NCHW."""
+    def _forward_from_nhwc(self, z, B, H, W, bf16=False):
+        """z: NHWC (B,H,W,in_dim), bf16 in the bf16 pipeline -> x_hat fp32 NCHW."""
         ics = self.inverse_conv_stack
-        h = _run_conv(ics[0], z, B, H, W, relu=True)     # ReLU of the stack folded in (Q2/Q3)
-        H, W = h.shape[1], h.shape[2]
-        h = ics[1]._apply_nhwc(h, B, H, W)
-        h = _run_conv(ics[2], h, B, H, W, relu=True)
-        H, W = h.shape[1], h.shape[2]
-        return _run_conv(ics[4], h, B, H, W, out_layout=NCHW)
-
-    def _bf16_ok(self):
-        ics = self.inverse_conv_stack
-        return (ics[0].in_channels % 64 == 0 and ics[0].out_channels % 16 == 0 and ics[0].out_channels <= 256
-                and ics[1]._bf16_ok() and ics[2].in_channels % 64 == 0 and ics[2].out_channels % 32 == 0
-                and ics[2].out_channels <= 128 and ics[4].in_channels % 64 == 0 and ics[4].out_channels <= 4)
-
-    def _forward_from_nhwc_bf16(self, z, B, H, W):
-        """z: bf16 NHWC (B,H,W,in_dim) -> x_hat fp32 NCHW, every layer on the bf16 kernels."""
-        ics = self.inverse_conv_stack
-        h = ops.conv2d_bf16(z, _PACKED.bf16(ics[0].weight, CONVT_K3), _bias(ics[0]), B=B, Cin=ics[0].in_channels, H=H, W=W,
-                            Cout=ics[0].out_channels, kind=CONVT_K3, relu=True)
-        h = ics[1]._apply_nhwc_bf16(h, B, H, W)
-        h = ops.conv2d_bf16(h, _PACKED.bf16(ics[2].weight, CONVT_K4S2), _bias(ics[2]), B=B, Cin=ics[2].in_channels, H=H, W=W,
-                            Cout=ics[2].out_channels, kind=CONVT_K4S2, relu=True)
-        H, W = 2 * H, 2 * W
-        return ops.conv2d_bf16(h, _PACKED.bf16(ics[4].weight, CONVT_K4S2_OUT), _bias(ics[4]), B=B, Cin=ics[4].in_channels,
-                               H=H, W=W, Cout=ics[4].out_channels, kind=CONVT_K4S2_OUT, relu=False)
+        h, H, W = _run_conv(ics[0], z, B, H, W, bf16, relu=True)     # ReLU of the stack folded in (Q2/Q3)
+        h = ics[1]._apply_nhwc(h, B, H, W, bf16)
+        h, H, W = _run_conv(ics[2], h, B, H, W, bf16, relu=True)
+        return _run_conv(ics[4], h, B, H, W, bf16, out_layout=NCHW)[0]
 
     def forward(self, x):
         x = _prep_input(x, self.inverse_conv_stack[0].in_channels, "Decoder")
@@ -441,7 +397,7 @@ class _PointwiseConv2d(nn.Conv2d):
     def forward(self, x):
         x = _prep_input(x, self.in_channels, "pre_quantization_conv")
         B, _, H, W = x.shape
-        return _run_conv(self, x, B, H, W, in_layout=NCHW, out_layout=NCHW)
+        return _run_conv(self, x, B, H, W, in_layout=NCHW, out_layout=NCHW)[0]
 
 
 class VQVAE(nn.Module):
@@ -468,34 +424,45 @@ class VQVAE(nn.Module):
         self.last_vq_stats = None            # (hist int32 (K,), sse f64 (1,), rows of this shard) of the last forward
         self._side_stream = None
         self.last_min_encoding_indices = None
+        self._bf16_covered = None            # _bf16_pipeline's answer for this architecture, once asked
 
     def _bf16_pipeline(self):
         """True when set_precision("bf16") is active AND every layer of this model has a bf16 kernel
         (h_dim = 128 family: 64-channel first layer, channel counts in multiples of 64, embedding_dim = 64).
-        Other shapes run the TF32 kernels on fp32 activations, with a one-time warning."""
+        Other shapes run the TF32 kernels on fp32 activations, with a one-time warning.  The constructor fixes the
+        architecture, so the answer is worked out on first use and kept."""
         if get_precision() != "bf16":
             return False
-        pq = self.pre_quantization_conv
-        ok = (self.encoder._bf16_ok() and self.decoder._bf16_ok() and pq.in_channels % 64 == 0
-              and pq.out_channels == 64 and self.vector_quantization.e_dim == 64)
-        if not ok and not getattr(self, "_warned_bf16", False):
-            import warnings
-            warnings.warn("vqvae_b200: this model shape has no bf16 kernels; precision 'bf16' runs the TF32 kernels")
-            self._warned_bf16 = True
-        return ok
+        if self._bf16_covered is None:
+            self._bf16_covered = self._bf16_coverage()
+            if not self._bf16_covered:
+                import warnings
+                warnings.warn("vqvae_b200: this model shape has no bf16 kernels; precision 'bf16' runs the TF32 kernels")
+        return self._bf16_covered
+
+    def _bf16_coverage(self):
+        """Whether the library has a bf16 kernel for every layer.  vqb_conv_bf16_packed_bytes answers for each conv that
+        takes a bf16 packing; the entry points with no such query take the shapes include/vqvae_b200.h documents."""
+        conv_in = self.encoder.conv_stack[0]
+        if (conv_in.in_channels, conv_in.out_channels) != (3, 64):                      # vqb_conv_in_bf16
+            return False
+        for st in (m for m in self.modules() if isinstance(m, ResidualStack) and len(m.stack)):
+            layer = st.stack[0]                                                         # vqb_residual_layer_bf16
+            if any(l is not layer for l in st.stack) or layer.res_block[1].in_channels not in (64, 128):
+                return False
+        if self.vector_quantization.e_dim != 64:                                        # vqb_vq_forward_bf16zq_f32
+            return False
+        keys = [(c, _pack_key(c, True)) for c in _convs(self)]
+        return all(ops.lib().vqb_conv_bf16_packed_bytes(key[1], c.out_channels, c.in_channels) != 0
+                   for c, key in keys if key[0] == "bf16")
 
     def _encode_rows(self, x, bf16=False):
         x = _prep_input(x, 3, "VQVAE")
         if x.shape[2] % 4 or x.shape[3] % 4:
             raise RuntimeError("VQVAE: image height and width must be divisible by 4 (Q11)")
-        if bf16:
-            h, B, H, W = self.encoder._forward_nhwc_bf16(x)
-            pq = self.pre_quantization_conv
-            z_e = ops.conv2d_bf16(h, _PACKED.bf16(pq.weight, CONV_K1), _bias(pq), B=B, Cin=pq.in_channels, H=H, W=W,
-                                  Cout=pq.out_channels, kind=CONV_K1, relu=False, out_f32=True)   # fp32: feeds the exact VQ
-            return z_e, B, H, W
-        h, B, H, W = self.encoder._forward_nhwc(x)
-        z_e = _run_conv(self.pre_quantization_conv, h, B, H, W)              # NHWC (B,H,W,D)
+        h, B, H, W = self.encoder._forward_nhwc(x, bf16)
+        # NHWC (B,H,W,D) rows, fp32 in every mode: they feed the exact VQ
+        z_e = _run_conv(self.pre_quantization_conv, h, B, H, W, bf16, out_f32=True)[0]
         return z_e, B, H, W
 
     def forward(self, x, verbose=False):
@@ -509,10 +476,8 @@ class VQVAE(nn.Module):
         # stream and overlap the decoder; fork/join with events, so the whole forward stays capturable in one
         # CUDA graph.
         n_rows = z_e.shape[0] * H * W
-        if bf16:
-            idx, zq, sse, hist, ws = ops.vq_forward_bf16zq(z_e.view(-1, D), vq._codebook())
-        else:
-            idx, zq, sse, hist, ws = ops.vq_forward(z_e.view(-1, D), vq._codebook(), defer=True)
+        idx, zq, sse, hist, ws = ops.vq_forward(z_e.view(-1, D), vq._codebook(), defer=True,
+                                                zq_dtype=torch.bfloat16 if bf16 else torch.float32)
         main = torch.cuda.current_stream()
         if self._side_stream is None or self._side_stream.device != z_e.device:
             self._side_stream = torch.cuda.Stream(device=z_e.device)
@@ -525,10 +490,7 @@ class VQVAE(nn.Module):
             if not torch.cuda.is_current_stream_capturing():
                 for t in (ws, sse, hist, embedding_loss, perplexity):
                     t.record_stream(side)
-        if bf16:
-            x_hat = self.decoder._forward_from_nhwc_bf16(zq.view(B, H, W, D), B, H, W)
-        else:
-            x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W)  # :36
+        x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16)  # :36
         main.wait_stream(side)
         if not torch.cuda.is_current_stream_capturing():
             # the two scalars were allocated in the side stream's pool and are consumed on the caller's stream: without this
@@ -556,24 +518,9 @@ class VQVAE(nn.Module):
         """Refresh every cached weight packing whose parameter changed (load_state_dict, optimizer step), IN PLACE
         in the buffers earlier forwards -- and CUDA graphs captured around them -- already read.  A plain forward
         does this by itself; HostPipeline calls it before replaying a captured graph."""
-        enc, dec, pq = self.encoder.conv_stack, self.decoder.inverse_conv_stack, self.pre_quantization_conv
         bf16 = self._bf16_pipeline()
-        _PACKED.f32(enc[0].weight, False)
-        stacks = [s for s in (enc[5], dec[1]) if len(s.stack)]
-        if bf16:
-            _PACKED.bf16(enc[2].weight, CONV_K4S2); _PACKED.bf16(enc[4].weight, CONV_K3); _PACKED.bf16(pq.weight, CONV_K1)
-            _PACKED.bf16(dec[0].weight, CONVT_K3); _PACKED.bf16(dec[2].weight, CONVT_K4S2)
-            _PACKED.bf16(dec[4].weight, CONVT_K4S2_OUT)
-            for st in stacks:
-                _PACKED.bf16(st.stack[0].res_block[1].weight, CONV_K3); _PACKED.bf16(st.stack[0].res_block[3].weight, RES_W2)
-        else:
-            for conv in (enc[2], enc[4], pq):
-                _PACKED.f32(conv.weight, False)
-            for conv in (dec[0], dec[2], dec[4]):
-                _PACKED.f32(conv.weight, True)
-            for st in stacks:
-                for layer in set(st.stack):
-                    _PACKED.f32(layer.res_block[1].weight, False); _PACKED.f32(layer.res_block[3].weight, False)
+        for conv in _convs(self):
+            _packed(conv.weight, _pack_key(conv, bf16))
 
     # ---- SURVEY 8(f) rank 1: the two halves callers use around the path ----------
     def encode(self, x):
@@ -589,6 +536,7 @@ class VQVAE(nn.Module):
         vq = self.vector_quantization
         rows = ops.gather_rows(indices, vq._codebook())
         B = rows.shape[0] // (H * W)
-        if self._bf16_pipeline():
-            return self.decoder._forward_from_nhwc_bf16(rows.to(torch.bfloat16).view(B, H, W, vq.e_dim), B, H, W)
-        return self.decoder._forward_from_nhwc(rows.view(B, H, W, vq.e_dim), B, H, W)
+        bf16 = self._bf16_pipeline()
+        if bf16:
+            rows = rows.to(torch.bfloat16)
+        return self.decoder._forward_from_nhwc(rows.view(B, H, W, vq.e_dim), B, H, W, bf16)

@@ -106,14 +106,20 @@ def conv2d(x, w_packed, bias, *, B, Cin, H, W, Cout, kh, kw, stride, pad, transp
     return out
 
 
+# enum vqb_conv_kind -> (kernel size, stride, transposed) of the layer it names
+KIND_GEOMETRY = {_lib.CONV_K1: (1, 1, False), _lib.CONV_K3: (3, 1, False), _lib.CONVT_K3: (3, 1, True),
+                 _lib.CONV_K4S2: (4, 2, False), _lib.CONVT_K4S2: (4, 2, True), _lib.CONVT_K4S2_OUT: (4, 2, True),
+                 _lib.RES_W2: (1, 1, False)}
+
+
 def conv_kind(kh, stride, transposed, cout):
-    """enum vqb_conv_kind of a layer of the hot path, or None when the bf16 kernels do not cover it."""
-    if not transposed:
-        return {(1, 1): _lib.CONV_K1, (3, 1): _lib.CONV_K3, (4, 2): _lib.CONV_K4S2}.get((kh, stride))
-    if (kh, stride) == (3, 1):
-        return _lib.CONVT_K3
-    if (kh, stride) == (4, 2):
-        return _lib.CONVT_K4S2_OUT if cout <= 4 else _lib.CONVT_K4S2
+    """enum vqb_conv_kind of a layer of the hot path, or None when the bf16 kernels do not cover it.  (RES_W2, the
+    residual layer's 1x1 weight, is never a layer of its own.)"""
+    if cout <= 4 and KIND_GEOMETRY[_lib.CONVT_K4S2_OUT] == (kh, stride, bool(transposed)):
+        return _lib.CONVT_K4S2_OUT
+    for kind in (_lib.CONV_K1, _lib.CONV_K3, _lib.CONVT_K3, _lib.CONV_K4S2, _lib.CONVT_K4S2):
+        if KIND_GEOMETRY[kind] == (kh, stride, bool(transposed)):
+            return kind
     return None
 
 
@@ -122,7 +128,7 @@ def pack_conv_weight_bf16(w, kind, out=None):
     (None when the shape is not covered).  `out`: repack into an existing buffer (same shape) in place."""
     _require_cuda(w, "weight")
     w = _f32c(w.detach())
-    transposed = kind in (_lib.CONVT_K3, _lib.CONVT_K4S2, _lib.CONVT_K4S2_OUT)
+    transposed = KIND_GEOMETRY[kind][2]
     cin, cout = (w.shape[0], w.shape[1]) if transposed else (w.shape[1], w.shape[0])
     nbytes = lib().vqb_conv_bf16_packed_bytes(kind, cout, cin)
     if nbytes == 0:
@@ -140,18 +146,14 @@ def conv2d_bf16(x, packed, bias, *, B, Cin, H, W, Cout, kind, relu=False, out_f3
     _require_cuda(x, "input")
     if x.dtype != torch.bfloat16 or not x.is_contiguous():
         raise RuntimeError("conv2d_bf16: input must be a contiguous bf16 NHWC tensor")
-    if kind == _lib.CONV_K4S2:
-        shape, dt = (B, H // 2, W // 2, Cout), (torch.float32 if out_f32 else torch.bfloat16)
-    elif kind == _lib.CONVT_K4S2:
-        shape, dt = (B, 2 * H, 2 * W, Cout), (torch.float32 if out_f32 else torch.bfloat16)
-    elif kind == _lib.CONVT_K4S2_OUT:
-        shape, dt = (B, Cout, 2 * H, 2 * W), torch.float32
+    k, stride, transposed = KIND_GEOMETRY[kind]
+    oh, ow = (H * stride, W * stride) if transposed else (H // stride, W // stride)
+    if kind == _lib.CONVT_K4S2_OUT:
+        shape, dt = (B, Cout, oh, ow), torch.float32
     else:
-        shape, dt = (B, H, W, Cout), (torch.float32 if out_f32 else torch.bfloat16)
+        shape, dt = (B, oh, ow, Cout), (torch.float32 if out_f32 else torch.bfloat16)
     out = torch.empty(shape, dtype=dt, device=x.device)
-    k, st, tr = {_lib.CONV_K1: (1, 1, ""), _lib.CONV_K3: (3, 1, ""), _lib.CONVT_K3: (3, 1, "T"), _lib.CONV_K4S2: (4, 2, ""),
-                 _lib.CONVT_K4S2: (4, 2, "T"), _lib.CONVT_K4S2_OUT: (4, 2, "T")}[kind]
-    span = _Span(f"bf16 conv{tr} {Cin}->{Cout} k{k}s{st} {H}x{W}")
+    span = _Span(f"bf16 conv{'T' if transposed else ''} {Cin}->{Cout} k{k}s{stride} {H}x{W}")
     check(lib().vqb_conv2d_bf16(x.data_ptr(), packed.data_ptr(), bias.data_ptr() if bias is not None else None,
                                 out.data_ptr(), B, Cin, H, W, Cout, kind, int(bool(relu)), int(bool(out_f32)),
                                 _stream()), "conv2d_bf16")
@@ -168,26 +170,6 @@ def conv_in_bf16(x, w_packed_f32, bias, *, B, H, W, Cout, relu=True):
                                  out.data_ptr(), B, H, W, Cout, int(bool(relu)), _stream()), "conv_in_bf16")
     span.done()
     return out
-
-
-def vq_forward_bf16zq(z_rows, codebook):
-    """Fused VectorQuantizer core, fp32 rows in, bit-exact int64 idx, z_q as bf16 rows (vqb_vq_forward_bf16zq_f32).
-    Deferred SSE: returns (idx, zq_bf16, sse, hist, ws); run vq_reduce_sse(ws, ...) before reading sse."""
-    _require_cuda(z_rows, "z")
-    N, D = z_rows.shape
-    K = codebook.shape[0]
-    dev = z_rows.device
-    idx = torch.empty((N,), dtype=torch.int64, device=dev)
-    zq = torch.empty((N, D), dtype=torch.bfloat16, device=dev)
-    sse = torch.empty((1,), dtype=torch.float64, device=dev)
-    hist = torch.empty((K,), dtype=torch.int32, device=dev)
-    ws_bytes = lib().vqb_vq_workspace_bytes(N, K, D)
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-    span = _Span(f"vq N={N} K={K} D={D} (bf16 zq)")
-    check(lib().vqb_vq_forward_bf16zq_f32(z_rows.data_ptr(), codebook.data_ptr(), N, K, D, idx.data_ptr(), zq.data_ptr(),
-                                          sse.data_ptr(), hist.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "vq_forward_bf16zq")
-    span.done()
-    return idx, zq, sse, hist, ws
 
 
 def residual_layer_bf16(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, relu_out):
@@ -233,22 +215,29 @@ def residual_stack(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, n_layers, preci
     return out
 
 
-def vq_forward(z_rows, codebook, defer=False):
-    """Fused VectorQuantizer core on (N,D) rows -> (idx int64 (N,), zq (N,D), sse f64 (1,),
+def vq_forward(z_rows, codebook, defer=False, zq_dtype=torch.float32):
+    """Fused VectorQuantizer core on (N,D) fp32 rows -> (idx int64 (N,), zq (N,D), sse f64 (1,),
     hist int32 (K,)).  defer=True (vqb_vq_forward_deferred_f32) additionally returns the workspace:
-    `sse` is final only after vq_reduce_sse(ws, ...) has run (e.g. on a side stream)."""
+    `sse` is final only after vq_reduce_sse(ws, ...) has run (e.g. on a side stream).  zq_dtype=torch.bfloat16
+    (vqb_vq_forward_bf16zq_f32, D == 64, deferred only) writes z_q as bf16 rows for the bf16 pipeline."""
     _require_cuda(z_rows, "z")
+    bf16zq = zq_dtype == torch.bfloat16
+    if zq_dtype not in (torch.float32, torch.bfloat16) or (bf16zq and not defer):
+        raise ValueError("vq_forward: z_q is fp32, or bf16 rows with the deferred SSE (defer=True)")
     N, D = z_rows.shape
     K = codebook.shape[0]
     dev = z_rows.device
     idx = torch.empty((N,), dtype=torch.int64, device=dev)
-    zq = torch.empty((N, D), dtype=torch.float32, device=dev)
+    zq = torch.empty((N, D), dtype=zq_dtype, device=dev)
     sse = torch.empty((1,), dtype=torch.float64, device=dev)
     hist = torch.empty((K,), dtype=torch.int32, device=dev)
     ws_bytes = lib().vqb_vq_workspace_bytes(N, K, D)
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-    span = _Span(f"vq N={N} K={K} D={D}")
-    fn = lib().vqb_vq_forward_deferred_f32 if defer else lib().vqb_vq_forward_f32
+    span = _Span(f"vq N={N} K={K} D={D}{' (bf16 zq)' if bf16zq else ''}")
+    if bf16zq:
+        fn = lib().vqb_vq_forward_bf16zq_f32
+    else:
+        fn = lib().vqb_vq_forward_deferred_f32 if defer else lib().vqb_vq_forward_f32
     check(fn(z_rows.data_ptr(), codebook.data_ptr(), N, K, D, idx.data_ptr(), zq.data_ptr(), sse.data_ptr(),
              hist.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "vq_forward")
     span.done()
