@@ -19,7 +19,8 @@
  *     SURVEY.md 8e): the opt-in shared-memory size of each kernel is configured once
  *     per process, on the device that is current at its first launch; calls may come
  *     from any host thread but are not re-entrant on the same workspace;
- *   - host pointers appear only in vqb_memcpy_async and the vqb_debug_* readers;
+ *   - host pointers appear only in vqb_memcpy_async, the vqb_debug_* readers and the
+ *     weight tables of the vqb_prior_* entry points;
  *   - return value: 0 = success, >0 = cudaError_t, <0 = vqb_status below; no C++
  *     exception crosses the boundary;
  *   - activations between layers are NHWC ("pixel rows": (B*H*W, C) row-major); the
@@ -259,6 +260,60 @@ int vqb_nhwc_to_nchw_f32(const float *in, float *out, int B, int C, int H, int W
  * kind 1 = host -> device, 2 = device -> host, 3 = device -> device.  Host buffers should be
  * pinned (the copy is only asynchronous then).                                          */
 int vqb_memcpy_async(void *dst, const void *src, size_t bytes, int kind, void *stream);
+
+/* ---- Gated PixelCNN prior, pixelcnn/models.py (inference, fp32 on CUDA cores) ----------------------------
+ * The prior over VQ code grids: teacher-forced logits (GatedPixelCNN.forward, models.py:121-130) and the whole
+ * sampling loop (GatedPixelCNN.generate, :132-143) in one call.  Activations are NHWC rows.  Shapes: dim % 32 == 0
+ * and dim <= 256, 1 <= input_dim (K) <= 8192, 1 <= n_layers <= VQB_PRIOR_MAX_LAYERS, odd kernel <= 15, any
+ * n_classes; other dims return VQB_ERR_UNSUPPORTED.  Out-of-range codes and labels are clamped to the nearest
+ * valid row in the kernels (as vqb_gather_rows_f32 does): a host-side range check would need a device sync.
+ * The weight tables below are HOST structs holding device pointers; they are read during the call only.     */
+#define VQB_PRIOR_MAX_LAYERS 32
+#define VQB_PRIOR_MAX_KERNEL 15
+
+/* One GatedMaskedConv2d (models.py:29-86).  *_w from vqb_prior_pack_f32, *_b the conv biases, class_emb the
+ * class_cond_embedding weight (n_classes, 2*dim).  vert_w keeps rows [0, kernel/2 + 1 - mask_a) of vert_stack's
+ * (2dim, dim, kernel/2+1, kernel) weight, horiz_w columns [0, kernel/2 + 1 - mask_a) of horiz_stack's
+ * (2dim, dim, 1, kernel/2+1) weight: mask A's zeroed taps (models.py:61-63) are not stored.                   */
+typedef struct vqb_prior_layer_weights {
+    const float *vert_w, *vert_b, *v2h_w, *v2h_b, *horiz_w, *horiz_b, *resid_w, *resid_b, *class_emb;
+    int kernel, mask_a, residual;
+} vqb_prior_layer_weights;
+
+/* The whole GatedPixelCNN: `layers` is a host array of n_layers entries; embedding (input_dim, dim);
+ * output_conv.0 (dim -> 512) and output_conv.2 (512 -> input_dim) packed by vqb_prior_pack_f32 (1x1).        */
+typedef struct vqb_prior_net {
+    const vqb_prior_layer_weights *layers;
+    int n_layers;
+    const float *embedding, *out1_w, *out1_b, *out2_w, *out2_b;
+    int input_dim, dim, n_classes;
+} vqb_prior_net;
+
+/* Conv weight (Cout, Cin, kh, kw) -> [(r*cols + s)*Cin + ci][co] for the taps r < rows, s < cols.            */
+int vqb_prior_pack_f32(const float *w, float *packed, int Cout, int Cin, int kh, int kw, int rows, int cols,
+                       void *stream);
+/* Workspace of vqb_prior_forward_f32 and vqb_prior_generate_f32 on a (B, H, W) grid (0 = bad sizes).        */
+size_t vqb_prior_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K);
+/* GatedActivation (models.py:20-26): x (outer, 2C, inner) -> out (outer, C, inner) = tanh(x_a) * sigmoid(x_b). */
+int vqb_prior_gate_f32(const float *x, float *out, int64_t outer, int C, int64_t inner, void *stream);
+/* GatedMaskedConv2d.forward (models.py:65-86) on NHWC x_v, x_h (B,H,W,dim), labels (B) int64 ->
+ * out_v, out_h NHWC (B,H,W,dim); vh: B*H*W*2*dim floats of scratch.  Two launches.                        */
+int vqb_prior_layer_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                        const int64_t *labels, int B, int H, int W, int dim, int n_classes, float *out_v,
+                        float *out_h, float *vh, void *stream);
+/* GatedPixelCNN.forward: codes (B,H,W) int64, labels (B) int64 -> logits (B, input_dim, H, W) fp32 NCHW.
+ * 2 + 2*n_layers launches.                                                                               */
+int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                          int W, float *logits, void *workspace, size_t workspace_bytes, void *stream);
+/* GatedPixelCNN.generate: samples codes (B,H,W) int64 in raster order.  Code (b,i,j) is the smallest k with
+ * u[b,i,j] < CDF_k, CDF the fp32 running sum of the softmax of the logits at (i,j) (DESIGN.md gives the order).
+ * u: (B,H,W) uniforms in [0,1).  H*(n_layers + W) launches: per row one vertical-stack pass per layer, then one
+ * launch per position running every layer's horizontal stack, the head and the draw.  No host synchronisation.
+ * step_logits: NULL, or (B,H,W,input_dim) fp32 receiving the logits each step sampled from -- bitwise equal to
+ * vqb_prior_forward_f32's logits on the returned codes.                                                    */
+int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, int B, int H, int W,
+                           int64_t *codes, float *step_logits, void *workspace, size_t workspace_bytes,
+                           void *stream);
 
 #ifdef __cplusplus
 }

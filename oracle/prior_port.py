@@ -1,0 +1,117 @@
+"""The Gated PixelCNN prior restated functionally with torch CPU ops -- TEST INFRASTRUCTURE ONLY.
+
+``prior_forward`` is the reference's GatedPixelCNN.forward (pixelcnn/models.py:121-130) on a state dict, op for op,
+mask-A zeroing included; ``prior_generate`` its sampling loop (one full forward per position), which
+tools/bench_prior.py times ("kind": "port") only when the verbatim copy of the reference (oracle/prior_ref.py) is
+absent.  Pinned against the unmodified reference by tests/test_prior_cpu.py through the tests/golden/prior_*
+vectors that ``python -m oracle.make_prior_golden`` writes.  The product (vqvae_b200/, models/, pixelcnn/) never
+imports this module.
+"""
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+# name -> (K, dim, n_layers, n_classes, grid, batch, weight seed, input seed[, stored positions])
+PRIOR_CASES = {
+    "prior_default": dict(K=512, dim=64, n_layers=15, n_classes=10, size=8, batch=4, wseed=30, xseed=31),
+    "prior_ragged": dict(K=37, dim=32, n_layers=4, n_classes=3, size=5, batch=3, wseed=32, xseed=33),
+    # cfg3 latent (256x256 images): logits are stored at 64 seeded positions only
+    "prior_cfg3": dict(K=1024, dim=64, n_layers=15, n_classes=10, size=64, batch=1, wseed=34, xseed=35,
+                       positions=64),
+}
+
+HIDDEN = 512
+
+
+def prior_shapes(K, dim, n_layers, n_classes):
+    """(key, shape) of every tensor of GatedPixelCNN(K, dim, n_layers, n_classes).state_dict(), in order."""
+    out = [("embedding.weight", (K, dim))]
+    for i in range(n_layers):
+        k = 7 if i == 0 else 3
+        p = f"layers.{i}."
+        out += [(p + "class_cond_embedding.weight", (n_classes, 2 * dim)),
+                (p + "vert_stack.weight", (2 * dim, dim, k // 2 + 1, k)), (p + "vert_stack.bias", (2 * dim,)),
+                (p + "vert_to_horiz.weight", (2 * dim, 2 * dim, 1, 1)), (p + "vert_to_horiz.bias", (2 * dim,)),
+                (p + "horiz_stack.weight", (2 * dim, dim, 1, k // 2 + 1)), (p + "horiz_stack.bias", (2 * dim,)),
+                (p + "horiz_resid.weight", (dim, dim, 1, 1)), (p + "horiz_resid.bias", (dim,))]
+    out += [("output_conv.0.weight", (HIDDEN, dim, 1, 1)), ("output_conv.0.bias", (HIDDEN,)),
+            ("output_conv.2.weight", (K, HIDDEN, 1, 1)), ("output_conv.2.bias", (K,))]
+    return out
+
+
+def make_prior_state_dict(K, dim, n_layers, n_classes, seed):
+    """Seeded float32 weights: Xavier-range conv weights (mask A's taps deliberately non-zero), small random biases,
+    unit-normal embeddings."""
+    rng = np.random.RandomState(seed)
+    sd = {}
+    for key, shape in prior_shapes(K, dim, n_layers, n_classes):
+        if key.endswith("bias"):
+            v = rng.uniform(-0.1, 0.1, size=shape)
+        elif len(shape) == 4:
+            fan_in, fan_out = shape[1] * shape[2] * shape[3], shape[0] * shape[2] * shape[3]
+            a = np.sqrt(6.0 / (fan_in + fan_out))
+            v = rng.uniform(-a, a, size=shape)
+        else:
+            v = rng.standard_normal(shape)
+        sd[key] = v.astype(np.float32)
+    return sd
+
+
+def make_prior_inputs(case):
+    """(codes (B,H,W) int64, labels (B,) int64[, positions (P,2)]) of a case."""
+    rng = np.random.RandomState(case["xseed"])
+    B, S = case["batch"], case["size"]
+    codes = rng.randint(0, case["K"], size=(B, S, S)).astype(np.int64)
+    labels = rng.randint(0, case["n_classes"], size=(B,)).astype(np.int64)
+    pos = None
+    if case.get("positions"):
+        flat = rng.choice(S * S, size=case["positions"], replace=False)
+        pos = np.stack([flat // S, flat % S], axis=1).astype(np.int64)
+    return codes, labels, pos
+
+
+def _gate(t):
+    a, b = t.chunk(2, dim=1)
+    return torch.tanh(a) * torch.sigmoid(b)
+
+
+@torch.no_grad()
+def prior_forward(sd, x, label, n_layers, dtype=torch.float32):
+    """Logits (B, K, H, W) of codes x (B,H,W) int64 and labels (B,) int64; sd maps keys to tensors or arrays."""
+    g = {k: torch.as_tensor(v).to(dtype) for k, v in sd.items()}
+    x, label = torch.as_tensor(x), torch.as_tensor(label)
+    h = F.embedding(x, g["embedding.weight"]).permute(0, 3, 1, 2)
+    x_v = x_h = h
+    for i in range(n_layers):
+        p = f"layers.{i}."
+        k = 7 if i == 0 else 3
+        wv, wh = g[p + "vert_stack.weight"], g[p + "horiz_stack.weight"]
+        if i == 0:                                        # mask A (models.py:61-63)
+            wv, wh = wv.clone(), wh.clone()
+            wv[:, :, -1] = 0
+            wh[:, :, :, -1] = 0
+        c = F.embedding(label, g[p + "class_cond_embedding.weight"])[:, :, None, None]
+        hv = F.conv2d(x_v, wv, g[p + "vert_stack.bias"], 1, (k // 2, k // 2))[:, :, :x_v.size(-1), :]
+        out_v = _gate(hv + c)
+        hh = F.conv2d(x_h, wh, g[p + "horiz_stack.bias"], 1, (0, k // 2))[:, :, :, :x_h.size(-2)]
+        v2h = F.conv2d(hv, g[p + "vert_to_horiz.weight"], g[p + "vert_to_horiz.bias"])
+        out = _gate(v2h + hh + c)
+        r = F.conv2d(out, g[p + "horiz_resid.weight"], g[p + "horiz_resid.bias"])
+        x_h = r + x_h if i > 0 else r
+        x_v = out_v
+    y = F.relu(F.conv2d(x_h, g["output_conv.0.weight"], g["output_conv.0.bias"]))
+    return F.conv2d(y, g["output_conv.2.weight"], g["output_conv.2.bias"])
+
+
+@torch.no_grad()
+def prior_generate(sd, label, shape, batch_size, n_layers, device="cpu", rows=None):
+    """The reference's sampling schedule (models.py:132-143): one full forward per position, softmax, multinomial.
+    `rows` limits the loop to the first rows (timing a part of a large grid)."""
+    g = {k: torch.as_tensor(v).to(device) for k, v in sd.items()}
+    x = torch.zeros((batch_size,) + tuple(shape), dtype=torch.int64, device=device)
+    for i in range(shape[0] if rows is None else rows):
+        for j in range(shape[1]):
+            logits = prior_forward(g, x, label, n_layers)
+            probs = F.softmax(logits[:, :, i, j], -1)
+            x[:, i, j].copy_(probs.multinomial(1).squeeze())
+    return x

@@ -8,7 +8,8 @@ from .modules import (Decoder, Encoder, ResidualLayer, ResidualStack, VectorQuan
                       get_precision, invalidate_packed, packed_state, precision, set_precision)
 from .pipeline import HostPipeline, HostResult  # noqa: F401
 from .checkpoint import load_checkpoint, save_checkpoint  # noqa: F401
+from .prior import GatedPixelCNN  # noqa: F401
 
 __all__ = ["VQVAE", "VectorQuantizer", "Encoder", "Decoder", "ResidualLayer", "ResidualStack",
            "set_precision", "get_precision", "precision", "invalidate_packed", "packed_state", "HostPipeline",
-           "HostResult", "load_checkpoint", "save_checkpoint"]
+           "HostResult", "load_checkpoint", "save_checkpoint", "GatedPixelCNN"]

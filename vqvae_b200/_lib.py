@@ -54,7 +54,27 @@ SIGNATURES = {
     "vqb_vq_forward_bf16zq_f32": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "vqb_residual_layer_bf16": (_i, [_vp] * 4 + [_i] * 6 + [_vp]),
     "vqb_debug_vq_scores_f32": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "vqb_prior_pack_f32": (_i, [_vp, _vp] + [_i] * 6 + [_vp]),
+    "vqb_prior_workspace_bytes": (_sz, [_i] * 6),
+    "vqb_prior_gate_f32": (_i, [_vp, _vp, _i64, _i, _i64, _vp]),
+    "vqb_prior_layer_f32": (_i, [_vp] * 4 + [_i] * 5 + [_vp] * 4),
+    "vqb_prior_forward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
+    "vqb_prior_generate_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
 }
+
+PRIOR_MAX_LAYERS = 32       # VQB_PRIOR_MAX_LAYERS
+
+
+class PriorLayerWeights(C.Structure):
+    """struct vqb_prior_layer_weights"""
+    _fields_ = [(n, _vp) for n in ("vert_w", "vert_b", "v2h_w", "v2h_b", "horiz_w", "horiz_b", "resid_w", "resid_b",
+                                   "class_emb")] + [("kernel", _i), ("mask_a", _i), ("residual", _i)]
+
+
+class PriorNet(C.Structure):
+    """struct vqb_prior_net"""
+    _fields_ = [("layers", C.POINTER(PriorLayerWeights)), ("n_layers", _i), ("embedding", _vp), ("out1_w", _vp),
+                ("out1_b", _vp), ("out2_w", _vp), ("out2_b", _vp), ("input_dim", _i), ("dim", _i), ("n_classes", _i)]
 
 
 def lib():

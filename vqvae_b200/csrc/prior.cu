@@ -1,0 +1,541 @@
+// prior.cu -- the Gated PixelCNN prior (pixelcnn/models.py of the reference), fp32 on CUDA cores (sm_90a).
+//
+// Activations are NHWC rows.  A buffer holds `ring` rows of a (B, ring, W, C) grid and row r lives in slot r % ring:
+// ring = H is a whole grid (the teacher-forced forward), ring = 1 or 2 the one or two rows the incremental sampler
+// keeps.  Every output element is one fmaf chain over its inputs in a fixed order (taps, then input channels),
+// started from 0, then the bias: the value of an element does not depend on which positions share a block or on how
+// many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
+// sampler's logits are bitwise the forward's logits on the grid it produced.
+#include "common.cuh"
+
+namespace {
+
+constexpr int NT = 256;           // threads of every prior kernel
+constexpr int MAXC = 256;         // dim <= 256, dim % 32 == 0
+constexpr int HID = 512;          // output_conv.0: dim -> 512 (models.py:109)
+constexpr int MAXK = 8192;
+
+struct Act {                      // one NHWC activation buffer, C channels, `ring` rows of W positions per image
+    float *p;
+    int ring, C;
+    __device__ __forceinline__ float *at(int b, int r, int c, int W) const {
+        return p + (((long long)b * ring + r % ring) * W + c) * C;
+    }
+};
+
+struct Net {
+    vqb_prior_layer_weights layer[VQB_PRIOR_MAX_LAYERS];
+    const float *emb, *w1, *b1, *w2, *b2;
+    int L, C, K, NC;
+};
+
+// one block's positions: image, row, column and clamped label of each of its P slots (b < 0: slot unused)
+template <int P>
+struct Smem {
+    float x[MAXC * P];            // [ci][p]: one tap of the input, or the gated activations
+    float pre[HID * P];           // [c][p]: pre-activations (2*dim) or the head's hidden layer (512)
+    int b[P], r[P], c[P], lab[P];
+};
+
+__device__ __forceinline__ float gate(float a, float g) {      // GatedActivation: tanh(x) * sigmoid(y)
+    return tanhf(a) * (1.f / (1.f + expf(-g)));
+}
+
+template <int P>
+__device__ __forceinline__ void load_vec(float (&v)[P], const float *s) {
+    if constexpr (P % 4 == 0) {
+#pragma unroll
+        for (int q = 0; q < P / 4; ++q) {
+            const float4 t = reinterpret_cast<const float4 *>(s)[q];
+            v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+        }
+    } else {
+#pragma unroll
+        for (int p = 0; p < P; ++p) v[p] = s[p];
+    }
+}
+
+// acc[q][p] = fmaf-chain over k < n of x[k][p] * Wt[k][c0 + tid + q*NT]   (Wt: [n][Cout], output channel fastest)
+template <int P, int Q>
+__device__ __forceinline__ void mac(float (&acc)[Q][P], const float *xs, const float *__restrict__ Wt, int n,
+                                    int Cout, int c0) {
+    const int tid = threadIdx.x;
+    for (int k = 0; k < n; ++k) {
+        float v[P];
+        load_vec<P>(v, xs + k * P);
+#pragma unroll
+        for (int q = 0; q < Q; ++q) {
+            const int c = c0 + tid + q * NT;
+            if (c < Cout) {
+                const float w = __ldg(Wt + (long long)k * Cout + c);
+#pragma unroll
+                for (int p = 0; p < P; ++p) acc[q][p] = fmaf(v[p], w, acc[q][p]);
+            }
+        }
+    }
+}
+
+// x[ci][p] = in at (b, r + dy, c + dx) of slot p, 0 outside the grid or for an unused slot
+template <int P>
+__device__ __forceinline__ void load_tap(Smem<P> &s, const Act &in, int dy, int dx, int H, int W) {
+    const int C = in.C;
+    for (int i = threadIdx.x; i < P * C; i += NT) {
+        const int p = i / C, ci = i % C;
+        const int rr = s.r[p] + dy, cc = s.c[p] + dx;
+        float v = 0.f;
+        if (s.b[p] >= 0 && rr >= 0 && rr < H && cc >= 0 && cc < W) v = in.at(s.b[p], rr, cc, W)[ci];
+        s.x[ci * P + p] = v;
+    }
+}
+
+// kept taps of a masked conv: vert_stack (kernel//2+1, kernel) and horiz_stack (1, kernel//2+1); mask A drops the
+// last row / column (models.py:61-63).  Tap (t_r, t_c) reads offset (t_r - kernel//2, t_c - kernel//2).
+__device__ __forceinline__ int vert_rows(const vqb_prior_layer_weights &w) { return w.kernel / 2 + 1 - (w.mask_a ? 1 : 0); }
+__device__ __forceinline__ int horiz_cols(const vqb_prior_layer_weights &w) { return w.kernel / 2 + 1 - (w.mask_a ? 1 : 0); }
+
+// Vertical stack of one layer at the P positions of the block (models.py:69-72, :77):
+//   h_vert = vert_stack(x_v) ; out_v = gate(h_vert + emb[label]) ; vh = vert_to_horiz(h_vert) + emb[label]
+template <int P>
+__device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &out_v,
+                               const Act &vh, int H, int W) {
+    const int C = in.C, C2 = 2 * C, tid = threadIdx.x;
+    float acc[2][P];
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+#pragma unroll
+        for (int p = 0; p < P; ++p) acc[q][p] = 0.f;
+    const int rows = vert_rows(w), k = w.kernel, half = k / 2;
+    for (int tr = 0; tr < rows; ++tr)
+        for (int tc = 0; tc < k; ++tc) {
+            __syncthreads();
+            load_tap(s, in, tr - half, tc - half, H, W);
+            __syncthreads();
+            mac<P, 2>(acc, s.x, w.vert_w + (long long)(tr * k + tc) * C * C2, C, C2, 0);
+        }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const int c = tid + q * NT;
+        if (c < C2)
+#pragma unroll
+            for (int p = 0; p < P; ++p) s.pre[c * P + p] = acc[q][p] + __ldg(w.vert_b + c);
+    }
+    __syncthreads();
+    for (int i = tid; i < P * C; i += NT) {
+        const int p = i / C, c = i % C;
+        if (s.b[p] < 0) continue;
+        const float *e = w.class_emb + (long long)s.lab[p] * C2;
+        out_v.at(s.b[p], s.r[p], s.c[p], W)[c] = gate(s.pre[c * P + p] + __ldg(e + c), s.pre[(c + C) * P + p] + __ldg(e + c + C));
+    }
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+#pragma unroll
+        for (int p = 0; p < P; ++p) acc[q][p] = 0.f;
+    mac<P, 2>(acc, s.pre, w.v2h_w, C2, C2, 0);
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const int c = tid + q * NT;
+        if (c >= C2) continue;
+#pragma unroll
+        for (int p = 0; p < P; ++p)
+            if (s.b[p] >= 0)
+                vh.at(s.b[p], s.r[p], s.c[p], W)[c] =
+                    (acc[q][p] + __ldg(w.v2h_b + c)) + __ldg(w.class_emb + (long long)s.lab[p] * C2 + c);
+    }
+}
+
+// Horizontal stack of one layer at the P positions of the block (models.py:74-83):
+//   out = gate(horiz_stack(x_h) + vh) ; out_h = horiz_resid(out) [+ x_h]
+// The forward's per-layer kernel and the sampler's position step both run this.
+template <int P>
+__device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &vh,
+                                const Act &out_h, int H, int W) {
+    const int C = in.C, C2 = 2 * C, tid = threadIdx.x;
+    float acc[2][P];
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+#pragma unroll
+        for (int p = 0; p < P; ++p) acc[q][p] = 0.f;
+    const int cols = horiz_cols(w), half = w.kernel / 2;
+    for (int tc = 0; tc < cols; ++tc) {
+        __syncthreads();
+        load_tap(s, in, 0, tc - half, H, W);
+        __syncthreads();
+        mac<P, 2>(acc, s.x, w.horiz_w + (long long)tc * C * C2, C, C2, 0);
+    }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const int c = tid + q * NT;
+        if (c >= C2) continue;
+#pragma unroll
+        for (int p = 0; p < P; ++p)
+            s.pre[c * P + p] = s.b[p] >= 0 ? (acc[q][p] + __ldg(w.horiz_b + c)) + vh.at(s.b[p], s.r[p], s.c[p], W)[c] : 0.f;
+    }
+    __syncthreads();
+    for (int i = tid; i < P * C; i += NT) {
+        const int p = i % P, c = i / P;
+        s.x[c * P + p] = gate(s.pre[c * P + p], s.pre[(c + C) * P + p]);
+    }
+    __syncthreads();
+    float r[1][P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) r[0][p] = 0.f;
+    mac<P, 1>(r, s.x, w.resid_w, C, C, 0);
+    if (tid < C) {
+#pragma unroll
+        for (int p = 0; p < P; ++p) {
+            if (s.b[p] < 0) continue;
+            float v = r[0][p] + __ldg(w.resid_b + tid);
+            if (w.residual) v = v + in.at(s.b[p], s.r[p], s.c[p], W)[tid];
+            out_h.at(s.b[p], s.r[p], s.c[p], W)[tid] = v;
+        }
+    }
+}
+
+// output_conv (models.py:107-111): logits = W2 . relu(W1 . x_h + b1) + b2 at the P positions of the block.
+// Logit k of slot p goes to out[p] + k * kstride.
+template <int P>
+__device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, float *const (&out)[P], long long kstride,
+                               int H, int W) {
+    const int C = n.C, tid = threadIdx.x;
+    __syncthreads();
+    load_tap(s, in, 0, 0, H, W);
+    __syncthreads();
+    for (int c0 = 0; c0 < HID; c0 += NT) {
+        float acc[1][P];
+#pragma unroll
+        for (int p = 0; p < P; ++p) acc[0][p] = 0.f;
+        mac<P, 1>(acc, s.x, n.w1, C, HID, c0);
+#pragma unroll
+        for (int p = 0; p < P; ++p) s.pre[(c0 + tid) * P + p] = fmaxf(acc[0][p] + __ldg(n.b1 + c0 + tid), 0.f);
+    }
+    __syncthreads();
+    for (int c0 = 0; c0 < n.K; c0 += NT) {
+        float acc[1][P];
+#pragma unroll
+        for (int p = 0; p < P; ++p) acc[0][p] = 0.f;
+        mac<P, 1>(acc, s.pre, n.w2, HID, n.K, c0);
+        const int k = c0 + tid;
+        if (k < n.K)
+#pragma unroll
+            for (int p = 0; p < P; ++p)
+                if (s.b[p] >= 0) out[p][k * kstride] = acc[0][p] + __ldg(n.b2 + k);
+    }
+}
+
+__device__ __forceinline__ int clampi(long long v, int n) { return v < 0 ? 0 : (v >= n ? n - 1 : (int)v); }
+
+// Slots of a block over the positions [row0, row0 + nrows) x [0, W) of all B images, position-major in (b, row, col).
+template <int P>
+__device__ void set_slots(Smem<P> &s, int B, int row0, int nrows, int W, const long long *labels, int NC) {
+    if (threadIdx.x < P) {
+        const int p = threadIdx.x;
+        const long long g = (long long)blockIdx.x * P + p;
+        const long long per = (long long)nrows * W;
+        if (g < B * per) {
+            s.b[p] = (int)(g / per);
+            s.r[p] = row0 + (int)((g % per) / W);
+            s.c[p] = (int)(g % W);
+            s.lab[p] = clampi(labels[s.b[p]], NC);
+        } else {
+            s.b[p] = -1; s.r[p] = 0; s.c[p] = 0; s.lab[p] = 0;
+        }
+    }
+    __syncthreads();
+}
+
+template <int P>
+__global__ void __launch_bounds__(NT) vert_kernel(vqb_prior_layer_weights w, Act in, Act out_v, Act vh,
+                                                  const long long *labels, int NC, int B, int H, int W, int row0,
+                                                  int nrows) {
+    __shared__ __align__(16) Smem<P> s;
+    set_slots(s, B, row0, nrows, W, labels, NC);
+    vert_positions(s, w, in, out_v, vh, H, W);
+}
+
+template <int P>
+__global__ void __launch_bounds__(NT) horiz_kernel(vqb_prior_layer_weights w, Act in, Act vh, Act out_h,
+                                                   const long long *labels, int NC, int B, int H, int W) {
+    __shared__ __align__(16) Smem<P> s;
+    set_slots(s, B, 0, H, W, labels, NC);
+    horiz_positions(s, w, in, vh, out_h, H, W);
+}
+
+// logits NCHW (B, K, H, W)
+template <int P>
+__global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long *labels, int B, int H, int W,
+                                                  float *logits) {
+    __shared__ __align__(16) Smem<P> s;
+    __shared__ float *out[P];
+    set_slots(s, B, 0, H, W, labels, n.NC);
+    if (threadIdx.x < P) {
+        const int p = threadIdx.x;
+        out[p] = s.b[p] >= 0 ? logits + (long long)s.b[p] * n.K * H * W + (long long)s.r[p] * W + s.c[p] : nullptr;
+    }
+    head_positions(s, n, in, out, (long long)H * W, H, W);
+}
+
+// embedding (models.py:122): x0[n] = E[clamp(codes[n])]
+__global__ void embed_kernel(const long long *__restrict__ codes, const float *__restrict__ E, long long N, int K,
+                             int C, float *__restrict__ x0) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < N * C; i += (long long)gridDim.x * blockDim.x)
+        x0[i] = __ldg(E + (long long)clampi(codes[i / C], K) * C + i % C);
+}
+
+// One sampling step at (i, j) for P images: every layer's horizontal stack, the head, the softmax and the inverse-CDF
+// draw.  The code goes to codes[b, i, j] and its embedding to x0[b, i, j], which later steps and row passes read.
+template <int P>
+__global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act vh0, long long vh_stride,
+                                                  long long x_stride, const long long *labels, const float *u, int B,
+                                                  int H, int W, int i, int j, float *logits, long long logit_img,
+                                                  long long *codes) {
+    __shared__ __align__(16) Smem<P> s;
+    __shared__ float *out[P];
+    if (threadIdx.x < P) {
+        const int p = threadIdx.x, b = blockIdx.x * P + p;
+        s.b[p] = b < B ? b : -1;
+        s.r[p] = i; s.c[p] = j;
+        s.lab[p] = b < B ? clampi(labels[b], n.NC) : 0;
+        out[p] = b < B ? logits + (long long)b * logit_img : nullptr;
+    }
+    __syncthreads();
+    for (int l = 0; l < n.L; ++l) {
+        const Act in = l == 0 ? x0 : Act{xrow0.p + (l - 1) * x_stride, 1, n.C};
+        const Act vh{vh0.p + l * vh_stride, 1, 2 * n.C};
+        const Act o{xrow0.p + l * x_stride, 1, n.C};
+        horiz_positions(s, n.layer[l], in, vh, o, H, W);
+        __syncthreads();
+    }
+    head_positions(s, n, Act{xrow0.p + (n.L - 1) * x_stride, 1, n.C}, out, 1, H, W);
+    __syncthreads();
+    // softmax + inverse CDF, one warp per image: lane L owns logits [L*cs, L*cs + cs); the CDF is the fp32 running sum
+    // of p_k = expf(l_k - max) / sum, over the lanes' chunk sums scanned in lane order and then within the chunk.
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    const int K = n.K;
+    for (int p = warp; p < P; p += NT / 32) {
+        if (s.b[p] < 0) continue;
+        const int b = s.b[p];
+        const float *lg = out[p];
+        const int cs = (K + 31) / 32, k0 = min(K, lane * cs), k1 = min(K, k0 + cs);
+        float m = -INFINITY;
+        for (int k = k0; k < k1; ++k) m = fmaxf(m, lg[k]);
+        for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        float sum = 0.f;
+        for (int k = k0; k < k1; ++k) sum += expf(lg[k] - m);
+        for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        float part = 0.f;
+        int last = -1;
+        for (int k = k0; k < k1; ++k) {
+            const float pk = expf(lg[k] - m) / sum;
+            part += pk;
+            if (pk > 0.f) last = k;
+        }
+        float incl = part;
+        for (int o = 1; o < 32; o <<= 1) {
+            const float t = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += t;
+        }
+        float cdf = __shfl_up_sync(0xffffffffu, incl, 1);
+        if (lane == 0) cdf = 0.f;
+        const float uu = u[((long long)b * H + i) * W + j];
+        int hit = -1;
+        for (int k = k0; k < k1; ++k) {
+            cdf += expf(lg[k] - m) / sum;
+            if (uu < cdf) { hit = k; break; }
+        }
+        const unsigned found = __ballot_sync(0xffffffffu, hit >= 0);
+        int code;
+        if (found) {
+            code = __shfl_sync(0xffffffffu, hit, __ffs(found) - 1);
+        } else {                    // u above the rounded total: the last code with non-zero probability
+            for (int o = 16; o; o >>= 1) last = max(last, __shfl_xor_sync(0xffffffffu, last, o));
+            code = last < 0 ? K - 1 : last;
+        }
+        if (lane == 0) codes[((long long)b * H + i) * W + j] = code;
+        float *x = x0.at(b, i, j, W);
+        for (int c = lane; c < n.C; c += 32) x[c] = __ldg(n.emb + (long long)code * n.C + c);
+    }
+}
+
+// conv weight (Cout, Cin, kh, kw) -> [(r*cols + s)*Cin + ci][co] for the kept taps r < rows, s < cols
+__global__ void pack_kernel(const float *__restrict__ w, float *__restrict__ out, int Cout, int Cin, int kh, int kw,
+                            int rows, int cols) {
+    const long long total = (long long)rows * cols * Cin * Cout;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int co = (int)(i % Cout);
+        const long long t = i / Cout;
+        const int ci = (int)(t % Cin), tap = (int)(t / Cin);
+        const int r = tap / cols, sc = tap % cols;
+        out[i] = w[(((long long)co * Cin + ci) * kh + r) * kw + sc];
+    }
+}
+
+__global__ void gate_kernel(const float *__restrict__ x, float *__restrict__ out, long long outer, int C,
+                            long long inner) {
+    const long long total = outer * C * inner;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long o = i / ((long long)C * inner), rest = i % ((long long)C * inner);
+        const float *src = x + o * 2 * C * inner + rest;
+        out[i] = gate(src[0], src[(long long)C * inner]);
+    }
+}
+
+unsigned grid_for(long long total) {
+    long long g = (total + NT - 1) / NT;
+    return (unsigned)(g > 148LL * 32 ? 148LL * 32 : (g < 1 ? 1 : g));
+}
+
+bool layer_ok(const vqb_prior_layer_weights &w) {
+    return w.vert_w && w.vert_b && w.v2h_w && w.v2h_b && w.horiz_w && w.horiz_b && w.resid_w && w.resid_b &&
+           w.class_emb && w.kernel >= 1 && w.kernel <= VQB_PRIOR_MAX_KERNEL && (w.kernel & 1);
+}
+
+bool dim_ok(int C) { return C % 32 == 0 && C <= MAXC; }
+
+// workspace regions, in floats
+struct Ws {
+    long long fwd_v, fwd_vh, fwd_x;               // forward: x0 | v[2] | vh | x[2]  (whole grids)
+    long long gen_x0, gen_v, gen_vh, gen_x, gen_lg;  // sampler: x0 | v[L] (2 rows) | vh[L] (1 row) | x[L] (1 row) | logits
+    long long fwd_total, gen_total;
+};
+
+Ws ws_layout(long long B, long long H, long long W, long long C, long long L, long long K) {
+    Ws w;
+    const long long grid = B * H * W * C;
+    w.fwd_v = grid;
+    w.fwd_vh = 3 * grid;
+    w.fwd_x = 5 * grid;
+    w.fwd_total = 7 * grid;
+    w.gen_x0 = 0;
+    w.gen_v = grid;
+    w.gen_vh = w.gen_v + L * B * 2 * W * C;
+    w.gen_x = w.gen_vh + L * B * W * 2 * C;
+    w.gen_lg = w.gen_x + L * B * W * C;
+    w.gen_total = w.gen_lg + B * K;
+    return w;
+}
+
+int net_from(const vqb_prior_net *net, Net &n) {
+    if (!net || !net->layers || !net->embedding || !net->out1_w || !net->out1_b || !net->out2_w || !net->out2_b)
+        return VQB_ERR_BAD_ARG;
+    if (net->n_layers <= 0 || net->dim <= 0 || net->input_dim <= 0 || net->n_classes <= 0) return VQB_ERR_BAD_ARG;
+    if (net->n_layers > VQB_PRIOR_MAX_LAYERS || !dim_ok(net->dim) || net->input_dim > MAXK) return VQB_ERR_UNSUPPORTED;
+    for (int l = 0; l < net->n_layers; ++l) {
+        if (!layer_ok(net->layers[l])) return VQB_ERR_BAD_ARG;
+        n.layer[l] = net->layers[l];
+    }
+    n.emb = net->embedding; n.w1 = net->out1_w; n.b1 = net->out1_b; n.w2 = net->out2_w; n.b2 = net->out2_b;
+    n.L = net->n_layers; n.C = net->dim; n.K = net->input_dim; n.NC = net->n_classes;
+    return 0;
+}
+
+constexpr int PF = 8;             // positions per block of the whole-grid kernels and the row pass
+constexpr int PS = 4;             // images per block of the sampling step
+
+unsigned blocks(long long positions, int P) { return (unsigned)((positions + P - 1) / P); }
+
+}  // namespace
+
+extern "C" int vqb_prior_pack_f32(const float *w, float *packed, int Cout, int Cin, int kh, int kw, int rows, int cols,
+                                  void *stream) {
+    if (!w || !packed || Cout <= 0 || Cin <= 0 || kh <= 0 || kw <= 0 || rows < 0 || cols < 0 || rows > kh || cols > kw)
+        return VQB_ERR_BAD_ARG;
+    const long long total = (long long)rows * cols * Cin * Cout;
+    if (total == 0) return 0;
+    pack_kernel<<<grid_for(total), NT, 0, (cudaStream_t)stream>>>(w, packed, Cout, Cin, kh, kw, rows, cols);
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_prior_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K) {
+    if (B <= 0 || H <= 0 || W <= 0 || dim <= 0 || n_layers <= 0 || K <= 0) return 0;
+    const Ws w = ws_layout(B, H, W, dim, n_layers, K);
+    return (size_t)(w.fwd_total > w.gen_total ? w.fwd_total : w.gen_total) * sizeof(float);
+}
+
+extern "C" int vqb_prior_gate_f32(const float *x, float *out, int64_t outer, int C, int64_t inner, void *stream) {
+    if (!x || !out || outer <= 0 || C <= 0 || inner <= 0) return VQB_ERR_BAD_ARG;
+    gate_kernel<<<grid_for(outer * C * inner), NT, 0, (cudaStream_t)stream>>>(x, out, outer, C, inner);
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_prior_layer_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                                   const int64_t *labels, int B, int H, int W, int dim, int n_classes, float *out_v,
+                                   float *out_h, float *vh, void *stream) {
+    if (!layer || !x_v || !x_h || !labels || !out_v || !out_h || !vh || B <= 0 || H <= 0 || W <= 0 || dim <= 0 ||
+        n_classes <= 0 || !layer_ok(*layer))
+        return VQB_ERR_BAD_ARG;
+    if (!dim_ok(dim)) return VQB_ERR_UNSUPPORTED;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *lab = reinterpret_cast<const long long *>(labels);
+    const long long n = (long long)B * H * W;
+    Act in_v{const_cast<float *>(x_v), H, dim}, in_h{const_cast<float *>(x_h), H, dim};
+    Act ov{out_v, H, dim}, oh{out_h, H, dim}, vha{vh, H, 2 * dim};
+    vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H);
+    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W);
+    VQB_COUNT_LAUNCH(2);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                     int H, int W, float *logits, void *workspace, size_t workspace_bytes,
+                                     void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!codes || !labels || !logits || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (workspace_bytes < vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *lab = reinterpret_cast<const long long *>(labels);
+    const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
+    float *ws = static_cast<float *>(workspace);
+    const long long npos = (long long)B * H * W, grid = npos * n.C;
+    Act x0{ws, H, n.C}, vh{ws + wl.fwd_vh, H, 2 * n.C};
+    Act v[2] = {{ws + wl.fwd_v, H, n.C}, {ws + wl.fwd_v + grid, H, n.C}};
+    Act x[2] = {{ws + wl.fwd_x, H, n.C}, {ws + wl.fwd_x + grid, H, n.C}};
+    embed_kernel<<<grid_for(grid), NT, 0, s>>>(reinterpret_cast<const long long *>(codes), net->embedding, npos, n.K,
+                                               n.C, x0.p);
+    for (int l = 0; l < n.L; ++l) {
+        const Act vin = l == 0 ? x0 : v[(l - 1) & 1], xin = l == 0 ? x0 : x[(l - 1) & 1];
+        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H);
+        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W);
+    }
+    head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, x[(n.L - 1) & 1], lab, B, H, W, logits);
+    VQB_COUNT_LAUNCH(2 + 2 * n.L);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, int B, int H,
+                                      int W, int64_t *codes, float *step_logits, void *workspace,
+                                      size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!labels || !u || !codes || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (workspace_bytes < vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *lab = reinterpret_cast<const long long *>(labels);
+    const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
+    float *ws = static_cast<float *>(workspace);
+    const long long v_stride = (long long)B * 2 * W * n.C, vh_stride = (long long)B * W * 2 * n.C,
+                    x_stride = (long long)B * W * n.C;
+    const Act x0{ws + wl.gen_x0, H, n.C};
+    for (int i = 0; i < H; ++i) {
+        // row pass: every layer's vertical stack at row i (codes of rows < i are final)
+        for (int l = 0; l < n.L; ++l) {
+            const Act vin = l == 0 ? x0 : Act{ws + wl.gen_v + (l - 1) * v_stride, 2, n.C};
+            vert_kernel<PF><<<blocks((long long)B * W, PF), NT, 0, s>>>(
+                n.layer[l], vin, Act{ws + wl.gen_v + l * v_stride, 2, n.C}, Act{ws + wl.gen_vh + l * vh_stride, 1, 2 * n.C},
+                lab, n.NC, B, H, W, i, 1);
+        }
+        for (int j = 0; j < W; ++j) {
+            float *lg = step_logits ? step_logits + ((long long)i * W + j) * n.K : ws + wl.gen_lg;
+            const long long img = step_logits ? (long long)H * W * n.K : n.K;
+            step_kernel<PS><<<blocks(B, PS), NT, 0, s>>>(n, x0, Act{ws + wl.gen_x, 1, n.C}, Act{ws + wl.gen_vh, 1, 2 * n.C},
+                                                         vh_stride, x_stride, lab, u, B, H, W, i, j, lg, img,
+                                                         reinterpret_cast<long long *>(codes));
+        }
+    }
+    VQB_COUNT_LAUNCH((unsigned long long)H * (n.L + W));
+    return vqb_cuda_status(cudaGetLastError());
+}

@@ -81,22 +81,32 @@ def _pack_key(conv, bf16):
         ("bf16", ops.conv_kind(conv.kernel_size[0], conv.stride[0], transposed, conv.out_channels))
 
 
+def _packed_current(param, key):
+    """Whether _packed(param, key) would return its cached packing without packing again."""
+    tag = _param_tag(param)
+    hit = getattr(param, "_vqb_packed", {}).get(key)
+    return hit is not None and hit[0] == tag and tag[0] is not None
+
+
 def _packed(param, key):
     """The packing `key` (see _pack_key) of a conv weight, cached ON the parameter object (so the cache dies with it).
     When the parameter changes (load_state_dict, optimizer step, .to()) the SAME device buffer is repacked in place
     whenever its size still fits, so CUDA graphs captured around a forward keep reading current weights after
     ``repack`` (HostPipeline checks the tags before every replay)."""
-    tag = _param_tag(param)
     cache = getattr(param, "_vqb_packed", None)
     if cache is None:
         cache = {}
         param._vqb_packed = cache
     hit = cache.get(key)
-    if hit is not None and hit[0] == tag and tag[0] is not None:
+    if _packed_current(param, key):
         return hit[1]
+    tag = _param_tag(param)
     old = hit[1] if hit is not None and hit[1] is not None and hit[1].device == param.device else None
-    pack = ops.pack_conv_weight if key[0] == "f32" else ops.pack_conv_weight_bf16
-    buf = pack(param, key[1], out=old)
+    if key[0] == "prior":            # ("prior", rows, cols): the kept taps of a prior conv (vqvae_b200/prior.py)
+        buf = ops.prior_pack_weight(param, key[1], key[2], out=old)
+    else:
+        pack = ops.pack_conv_weight if key[0] == "f32" else ops.pack_conv_weight_bf16
+        buf = pack(param, key[1], out=old)
     cache[key] = (tag, buf)
     return buf
 

@@ -338,3 +338,79 @@ def vq_debug_scores(z_rows, codebook):
                                         zq.data_ptr(), sse.data_ptr(), hist.data_ptr(), ws.data_ptr(),
                                         ws_bytes, scores.data_ptr(), _stream()), "vq_debug_scores")
     return idx, zq, sse, hist, scores
+
+
+# ---- Gated PixelCNN prior (vqb_prior_*) ------------------------------------------------------------------------
+def prior_pack_weight(w, rows, cols, out=None):
+    """(Cout,Cin,kh,kw) conv weight -> [(r*cols+s)*Cin+ci][co] for the taps r < rows, s < cols (vqb_prior_pack_f32)."""
+    _require_cuda(w, "weight")
+    w = _f32c(w.detach())
+    cout, cin, kh, kw = w.shape
+    n = max(rows * cols * cin * cout, 1)
+    if out is None or out.numel() != n or out.dtype != torch.float32 or out.device != w.device:
+        out = torch.empty((n,), dtype=torch.float32, device=w.device)
+    check(lib().vqb_prior_pack_f32(w.data_ptr(), out.data_ptr(), cout, cin, kh, kw, rows, cols, _stream()),
+          "prior_pack_weight")
+    return out
+
+
+def prior_gate(x):
+    """GatedActivation on (B, 2C, ...) fp32 CUDA -> (B, C, ...) (vqb_prior_gate_f32)."""
+    _require_cuda(x, "input")
+    x = _f32c(x.detach())
+    if x.dim() < 2 or x.shape[1] % 2:
+        raise RuntimeError(f"GatedActivation: expected (B, 2C, ...) with an even channel count, got {tuple(x.shape)}")
+    c = x.shape[1] // 2
+    inner = x[0, 0].numel()
+    out = torch.empty((x.shape[0], c) + tuple(x.shape[2:]), dtype=torch.float32, device=x.device)
+    if out.numel():
+        check(lib().vqb_prior_gate_f32(x.data_ptr(), out.data_ptr(), x.shape[0], c, inner, _stream()), "prior_gate")
+    return out
+
+
+def prior_layer(layer_w, x_v, x_h, labels, *, B, H, W, dim, n_classes):
+    """One GatedMaskedConv2d on NHWC (B,H,W,dim) fp32 buffers -> (out_v, out_h) NHWC (vqb_prior_layer_f32)."""
+    out_v = torch.empty((B, H, W, dim), dtype=torch.float32, device=x_v.device)
+    out_h = torch.empty_like(out_v)
+    vh = torch.empty((B, H, W, 2 * dim), dtype=torch.float32, device=x_v.device)
+    span = _Span(f"prior layer dim={dim} {H}x{W}")
+    check(lib().vqb_prior_layer_f32(_lib.C.byref(layer_w), x_v.data_ptr(), x_h.data_ptr(), labels.data_ptr(), B, H, W,
+                                    dim, n_classes, out_v.data_ptr(), out_h.data_ptr(), vh.data_ptr(), _stream()),
+          "prior_layer")
+    span.done()
+    return out_v, out_h
+
+
+def _prior_workspace(net, B, H, W, dev):
+    n = lib().vqb_prior_workspace_bytes(B, H, W, net.dim, net.n_layers, net.input_dim)
+    if n == 0:
+        raise RuntimeError("prior: bad sizes")
+    return torch.empty((n,), dtype=torch.uint8, device=dev)
+
+
+def prior_forward(net, codes, labels):
+    """Teacher-forced logits (B, K, H, W) of int64 codes (B,H,W) and labels (B,) (vqb_prior_forward_f32)."""
+    B, H, W = codes.shape
+    dev = codes.device
+    logits = torch.empty((B, net.input_dim, H, W), dtype=torch.float32, device=dev)
+    ws = _prior_workspace(net, B, H, W, dev)
+    span = _Span(f"prior forward K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(lib().vqb_prior_forward_f32(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W,
+                                      logits.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "prior_forward")
+    span.done()
+    return logits
+
+
+def prior_generate(net, labels, u, step_logits=None):
+    """The whole sampling loop (vqb_prior_generate_f32): int64 codes (B,H,W) drawn with the uniforms u (B,H,W).
+    step_logits: None, or a (B,H,W,K) fp32 tensor receiving the logits of every step."""
+    B, H, W = u.shape
+    dev = u.device
+    codes = torch.empty((B, H, W), dtype=torch.int64, device=dev)
+    ws = _prior_workspace(net, B, H, W, dev)
+    span = _Span(f"prior generate K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(lib().vqb_prior_generate_f32(_lib.C.byref(net), labels.data_ptr(), u.data_ptr(), B, H, W, codes.data_ptr(),
+                                       step_logits.data_ptr() if step_logits is not None else None, ws.data_ptr(),
+                                       ws.numel(), _stream()), "prior_generate")
+    span.done()
+    return codes

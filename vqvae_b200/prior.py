@@ -1,0 +1,185 @@
+"""Host-side mirror of the reference's Gated PixelCNN prior (``pixelcnn/models.py``), inference only.
+
+Same class names, constructor signatures, attribute names and state-dict keys as the reference, so a state dict saved
+by its ``gated_pixelcnn.py`` loads unchanged and ``from pixelcnn.models import GatedPixelCNN`` (the top-level
+``pixelcnn`` package re-exports these classes) drops in.  As in ``modules.py`` the nn.Conv2d / nn.Embedding children
+are parameter containers only: every forward runs the sm_90a kernels of ``csrc/prior.cu`` through the C ABI, in fp32
+whatever ``set_precision`` says.  Outputs carry no autograd graph.
+
+Reference behaviour kept on purpose:
+  P2  ``self.apply(weights_init)``: Xavier-uniform conv weights, zero biases, and one "Skipping initialization of"
+      line per GatedMaskedConv2d (it matches 'Conv' by name but has no weight of its own)
+  P3  mask A zeroes the last row of ``vert_stack.weight`` and the last column of ``horiz_stack.weight`` in the
+      caller's parameters.  Here that happens when layer 0's weights are (re)packed, i.e. once per change of the
+      parameter, so the packing cache and CUDA graphs around a forward stay valid
+  P4  square grids only: the reference crops the vertical stack with the width and the horizontal one with the
+      height, which fails for H != W; here that is a RuntimeError before any launch
+"""
+import torch
+import torch.nn as nn
+
+from . import ops
+from ._lib import PriorLayerWeights, PriorNet
+from .modules import _packed, _packed_current
+
+HIDDEN = 512          # output_conv's hidden width
+
+
+def weights_init(m):
+    """Xavier-uniform weight and zero bias for every module whose class name contains 'Conv'."""
+    name = type(m).__name__
+    if "Conv" not in name:
+        return
+    try:
+        nn.init.xavier_uniform_(m.weight.data)
+        m.bias.data.fill_(0)
+    except AttributeError:
+        print("Skipping initialization of ", name)
+
+
+def _f32(t):
+    t = t.detach()
+    t = t if t.dtype == torch.float32 else t.float()
+    return t if t.is_contiguous() else t.contiguous()
+
+
+def _square(H, W, what):
+    if H != W:
+        raise RuntimeError(f"{what}: the Gated PixelCNN takes square code grids only, got {H}x{W} (the reference "
+                           "crops its vertical stack by the width and its horizontal stack by the height)")
+
+
+def _labels(label, B, dev, what):
+    if not torch.is_tensor(label):
+        label = torch.as_tensor(label, device=dev)
+    ops._require_cuda(label, what + " label")
+    label = label.reshape(-1)
+    if label.numel() != B:
+        raise RuntimeError(f"{what}: expected {B} labels, got {label.numel()}")
+    return label.to(torch.int64).contiguous()
+
+
+class GatedActivation(nn.Module):
+    """tanh(first half of the channels) * sigmoid(second half) (models.py:20-26)."""
+
+    def forward(self, x):
+        return ops.prior_gate(x)
+
+
+class GatedMaskedConv2d(nn.Module):
+    """One gated layer with a vertical and a horizontal stack (models.py:29-86)."""
+
+    def __init__(self, mask_type, dim, kernel, residual=True, n_classes=10):
+        super().__init__()
+        if kernel % 2 != 1:
+            raise AssertionError("Kernel size must be odd")
+        self.mask_type = mask_type
+        self.residual = residual
+        half = kernel // 2
+        self.class_cond_embedding = nn.Embedding(n_classes, 2 * dim)
+        self.vert_stack = nn.Conv2d(dim, dim * 2, (half + 1, kernel), 1, (half, half))
+        self.vert_to_horiz = nn.Conv2d(2 * dim, 2 * dim, 1)
+        self.horiz_stack = nn.Conv2d(dim, dim * 2, (1, half + 1), 1, (0, half))
+        self.horiz_resid = nn.Conv2d(dim, dim, 1)
+        self.gate = GatedActivation()
+
+    def make_causal(self):
+        """Zero the taps mask A excludes: the vertical stack's last row, the horizontal stack's last column."""
+        self.vert_stack.weight.data[:, :, -1].zero_()
+        self.horiz_stack.weight.data[:, :, :, -1].zero_()
+
+    def _weights(self, keep):
+        """struct vqb_prior_layer_weights of this layer; tensors it points into are appended to `keep`."""
+        mask_a = self.mask_type == "A"
+        vs, hs = self.vert_stack, self.horiz_stack
+        vkey = ("prior", vs.kernel_size[0] - mask_a, vs.kernel_size[1])
+        hkey = ("prior", 1, hs.kernel_size[1] - mask_a)
+        if mask_a and not (_packed_current(vs.weight, vkey) and _packed_current(hs.weight, hkey)):
+            self.make_causal()          # P3: once per change of the parameters, right before they are packed
+        t = dict(vert_w=_packed(vs.weight, vkey), vert_b=_f32(vs.bias),
+                 v2h_w=_packed(self.vert_to_horiz.weight, ("prior", 1, 1)), v2h_b=_f32(self.vert_to_horiz.bias),
+                 horiz_w=_packed(hs.weight, hkey), horiz_b=_f32(hs.bias),
+                 resid_w=_packed(self.horiz_resid.weight, ("prior", 1, 1)), resid_b=_f32(self.horiz_resid.bias),
+                 class_emb=_f32(self.class_cond_embedding.weight))
+        keep.extend(t.values())
+        return PriorLayerWeights(**{k: v.data_ptr() for k, v in t.items()}, kernel=vs.kernel_size[1],
+                                 mask_a=int(mask_a), residual=int(bool(self.residual)))
+
+    def forward(self, x_v, x_h, h):
+        dim = self.horiz_resid.in_channels
+        for x, what in ((x_v, "x_v"), (x_h, "x_h")):
+            if x.dim() != 4 or x.shape[1] != dim:
+                raise RuntimeError(f"GatedMaskedConv2d: expected {what} of shape (B,{dim},H,W), got {tuple(x.shape)}")
+            ops._require_cuda(x, "GatedMaskedConv2d " + what)
+        if x_v.shape != x_h.shape:
+            raise RuntimeError(f"GatedMaskedConv2d: x_v {tuple(x_v.shape)} and x_h {tuple(x_h.shape)} differ")
+        B, _, H, W = x_v.shape
+        _square(H, W, "GatedMaskedConv2d")
+        label = _labels(h, B, x_v.device, "GatedMaskedConv2d")
+        keep = []
+        w = self._weights(keep)
+        out_v, out_h = ops.prior_layer(w, ops.nchw_to_nhwc(x_v.detach()), ops.nchw_to_nhwc(x_h.detach()), label,
+                                       B=B, H=H, W=W, dim=dim, n_classes=self.class_cond_embedding.num_embeddings)
+        return ops.nhwc_to_nchw(out_v), ops.nhwc_to_nchw(out_h)
+
+
+class GatedPixelCNN(nn.Module):
+    """Prior over code grids (models.py:89-143): layer 0 is a mask-A 7x7 layer without residual, the others mask-B
+    3x3 layers with residual, then a 1x1 -> ReLU -> 1x1 head to input_dim logits."""
+
+    def __init__(self, input_dim=256, dim=64, n_layers=15, n_classes=10):
+        super().__init__()
+        self.dim = dim
+        self.embedding = nn.Embedding(input_dim, dim)
+        self.layers = nn.ModuleList()
+        for i in range(n_layers):
+            first = i == 0
+            self.layers.append(GatedMaskedConv2d("A" if first else "B", dim, 7 if first else 3, not first, n_classes))
+        self.output_conv = nn.Sequential(
+            nn.Conv2d(dim, HIDDEN, 1),
+            nn.ReLU(True),
+            nn.Conv2d(HIDDEN, input_dim, 1),
+        )
+        self.apply(weights_init)
+
+    def _net(self, keep):
+        """(struct vqb_prior_net, its layer array); every tensor it points into is appended to `keep`."""
+        layers = (PriorLayerWeights * len(self.layers))(*[l._weights(keep) for l in self.layers])
+        o1, o2 = self.output_conv[0], self.output_conv[2]
+        t = dict(embedding=_f32(self.embedding.weight), out1_w=_packed(o1.weight, ("prior", 1, 1)), out1_b=_f32(o1.bias),
+                 out2_w=_packed(o2.weight, ("prior", 1, 1)), out2_b=_f32(o2.bias))
+        keep.extend(t.values())
+        keep.append(layers)
+        return PriorNet(layers=layers, n_layers=len(self.layers), input_dim=self.embedding.num_embeddings, dim=self.dim,
+                        n_classes=self.layers[0].class_cond_embedding.num_embeddings if len(self.layers) else 1,
+                        **{k: v.data_ptr() for k, v in t.items()})
+
+    def forward(self, x, label):
+        """int64 codes (B,H,W) and labels (B,) -> fp32 logits (B, input_dim, H, W)."""
+        if x.dim() != 3:
+            raise RuntimeError(f"GatedPixelCNN: expected codes of shape (B,H,W), got {tuple(x.shape)}")
+        B, H, W = x.shape
+        _square(H, W, "GatedPixelCNN")
+        ops._require_cuda(x, "GatedPixelCNN codes")
+        label = _labels(label, B, x.device, "GatedPixelCNN")
+        keep = []
+        return ops.prior_forward(self._net(keep), x.detach().to(torch.int64).contiguous(), label)
+
+    def _sample(self, label, u, step_logits=None):
+        """generate() with given uniforms u (B,H,W) fp32: the code at (b,i,j) is the smallest k with u < CDF_k."""
+        B, H, W = u.shape
+        _square(H, W, "GatedPixelCNN.generate")
+        ops._require_cuda(u, "GatedPixelCNN.generate uniforms")
+        label = _labels(label, B, u.device, "GatedPixelCNN.generate")
+        keep = []
+        return ops.prior_generate(self._net(keep), label, _f32(u), step_logits)
+
+    def generate(self, label, shape=(8, 8), batch_size=64):
+        """Sample (batch_size, *shape) int64 codes in raster order on the model's device.  Draws exactly one
+        torch.rand((batch_size, H, W)) from the current CUDA generator, so torch.manual_seed makes it reproducible."""
+        H, W = shape
+        _square(H, W, "GatedPixelCNN.generate")
+        dev = next(self.parameters()).device
+        ops._require_cuda(torch.empty(0, device=dev), "GatedPixelCNN parameters")
+        u = torch.rand((batch_size, H, W), device=dev)
+        return self._sample(label, u)
