@@ -75,11 +75,10 @@ unsigned long long vqb_launch_count(void);
  * nn.Conv2d weight (Cout,Cin,kh,kw)          encoder.py:29-36, residual.py:20-24,
  *                                            vqvae.py:16-17
  * nn.ConvTranspose2d weight (Cin,Cout,kh,kw) decoder.py:28-35   (transposed = 1)
- * -> `packed` holds 2*Cout*Cin*kh*kw + 144*Cin floats: the tap-major GEMM operand in both
- *    layouts the kernels read, [(r*kw+s)*Cin + ci][co] (FFMA path) followed by
- *    [(r*kw+s)][co][ci] (K-major rows for the wgmma path); for a k4 s2 transposed
- *    conv with Cout <= 4 a third region [9][16][Cin] (3x3-neighbourhood + pixel-shuffle
- *    form of decoder.py:34-35) follows.                                           */
+ * -> `packed` holds Cout*Cin*kh*kw + 144*Cin floats (a larger buffer also does): the
+ *    tap-major K-major rows [(r*kw+s)][co][ci] that every conv kernel reads; for a k4 s2
+ *    transposed conv with Cout <= 4 the [9][16][Cin] form (3x3-neighbourhood +
+ *    pixel-shuffle form of decoder.py:34-35) follows them.                        */
 int vqb_pack_conv_weight_f32(const float *w, float *packed, int Cout, int Cin, int kh,
                              int kw, int transposed, void *stream);
 
@@ -115,7 +114,7 @@ size_t vqb_conv_bf16_packed_bytes(int kind, int Cout, int Cin);
 /* w: the layer's fp32 weight as PyTorch stores it ((Cout,Cin,kh,kw), or (Cin,Cout,kh,kw) for
  * the transposed kinds) -> `packed` (128-byte aligned): K-major bf16 rows, tap-major,
  * [kh*kw][Cout][Cin] (VQB_RES_W2: Cin zero padded to 64), or [9][16][Cin] for
- * VQB_CONVT_K4S2_OUT -- the layouts vqb_pack_conv_weight_f32 writes for the wgmma path.    */
+ * VQB_CONVT_K4S2_OUT -- the layouts vqb_pack_conv_weight_f32 writes, in bf16.              */
 int vqb_pack_conv_weight_bf16(const float *w, void *packed, int kind, int Cout, int Cin,
                               void *stream);
 /* One layer forward on bf16 NHWC input (B,H,W,Cin):  out = act(conv(in) + bias).
@@ -126,7 +125,8 @@ int vqb_conv2d_bf16(const void *in, const void *packed, const float *bias, void 
                     void *stream);
 
 /* encoder.py:29-31 for the bf16 pipeline: fp32 NCHW image (B,3,H,W) -> bf16 NHWC (B,H/2,W/2,Cout),
- * Cout == 64; w_packed from vqb_pack_conv_weight_f32.                                       */
+ * Cout == 64; w_packed from vqb_pack_conv_weight_f32 (its fp32 K-major rows, as in the fp32
+ * and tf32 modes).                                                                          */
 int vqb_conv_in_bf16(const float *x, const float *w_packed, const float *bias, void *out, int B,
                      int H, int W, int Cout, int relu, void *stream);
 /* VectorQuantizer core for the bf16 pipeline: as vqb_vq_forward_deferred_f32 (fp32 z, bit-exact

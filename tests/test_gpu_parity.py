@@ -163,14 +163,38 @@ TC_CONV_CASES = [
     (1, 32, 33, 17, 32, 4, 2, 1, False, 1, 1, False, False),   # odd sizes, stride 2
     (2, 64, 16, 16, 3, 4, 2, 1, True, 1, 0, False, False),     # decoder.py:34-35: 3x3-neighbourhood GEMM + pixel shuffle
     (1, 32, 5, 9, 2, 4, 2, 1, True, 1, 0, True, False),        # same, ragged tile, Cout=2
-    (2, 3, 32, 32, 64, 4, 2, 1, False, 0, 1, True, False),     # encoder.py:29-31: hand-built im2col tile
-    (3, 3, 12, 20, 128, 4, 2, 1, False, 0, 1, False, False),   # same, partial last tile, Cout=128 (generic gather)
-    (3, 3, 64, 64, 64, 4, 2, 1, False, 0, 1, True, False),     # staged-rows fast path, 4 output rows per tile
-    (1, 3, 8, 256, 64, 4, 2, 1, False, 0, 1, False, False),    # fast path, one output row per tile (OW = 128)
-    (5, 3, 16, 16, 64, 4, 2, 1, False, 0, 1, True, False),     # tile straddles images: generic gather + TMA store
-    (2, 3, 32, 32, 128, 4, 2, 1, False, 0, 1, True, False),    # fast path, Cout=128 (direct stores)
-    (3, 3, 6, 8, 64, 4, 2, 1, False, 0, 1, True, False),       # partial tile (36 pixels), TMA store clips
+    # encoder.py:29-31 runs conv_in_k4s2 in every mode: a warp owns 32 output pixels x 32 channels, a CTA 8 warps
+    (2, 3, 32, 32, 64, 4, 2, 1, False, 0, 1, True, False),     # no ragged tile: 32 full warps in 4 full CTAs
+    (3, 3, 12, 20, 128, 4, 2, 1, False, 0, 1, False, False),   # 180 pixels: 20 live lanes in the last warps, Cout=128
+    (3, 3, 64, 64, 64, 4, 2, 1, False, 0, 1, True, False),     # 3072 pixels, 24 full CTAs
+    (1, 3, 8, 256, 64, 4, 2, 1, False, 0, 1, False, False),    # OW = 128: every warp inside one output row
+    (5, 3, 16, 16, 64, 4, 2, 1, False, 0, 1, True, False),     # 20 warps: the last CTA is half empty
+    (2, 3, 32, 32, 128, 4, 2, 1, False, 0, 1, True, False),    # Cout=128: four channel groups, full CTAs
+    (3, 3, 6, 8, 64, 4, 2, 1, False, 0, 1, True, False),       # 36 pixels: one CTA of 4 warps, 4 live lanes in 2 of them
 ]
+
+
+@pytest.mark.parametrize("Cin,Cout,k,stride,transposed", [(64, 128, 4, 2, False), (128, 32, 3, 1, False),
+                                                          (32, 128, 1, 1, False), (64, 128, 3, 1, True),
+                                                          (128, 64, 4, 2, True), (64, 3, 4, 2, True)])
+def test_fp32_packing_is_the_k_major_layout(Cin, Cout, k, stride, transposed):
+    """vqb_pack_conv_weight_f32 writes K-major rows [kh][kw][Cout][Cin] (bitwise the weight permuted; rounded to bf16,
+    the packing of vqb_pack_conv_weight_bf16), then room for the [9][16][Cin] pixel-shuffle form, which the k4 s2
+    transposed conv to <= 4 channels fills with the CONVT_K4S2_OUT packing."""
+    from vqvae_b200 import _lib, ops
+    rng = np.random.RandomState(Cin * 1000 + Cout * 10 + k)
+    w = _cuda((rng.standard_normal((Cin, Cout, k, k) if transposed else (Cout, Cin, k, k)) / np.sqrt(Cin * k * k))
+              .astype(np.float32))
+    packed = ops.pack_conv_weight(w, transposed)
+    n = k * k * Cin * Cout
+    assert packed.numel() == n + 144 * Cin
+    rows = packed[:n]
+    assert torch.equal(rows, w.permute(2, 3, 1, 0).reshape(-1) if transposed else w.permute(2, 3, 0, 1).reshape(-1))
+    kind = ops.conv_kind(k, stride, transposed, Cout)
+    if kind == _lib.CONVT_K4S2_OUT:
+        assert torch.equal(packed[n:].to(torch.bfloat16), ops.pack_conv_weight_bf16(w, kind).view(torch.bfloat16))
+    elif Cin % 64 == 0:
+        assert torch.equal(rows.to(torch.bfloat16), ops.pack_conv_weight_bf16(w, kind).view(torch.bfloat16))
 
 
 def test_tc_transposed_k4s2_is_one_launch():

@@ -96,8 +96,8 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     if (kh == 4 && kw == 4 && stride == 2 && pad == 1 && !skip) {
         if (transposed && precision != VQB_FP32 && in_layout == VQB_NHWC && out_layout == VQB_NCHW &&
             convt_shuffle_supported(Cin, Cout)) {
-            const int rc = launch_convt_shuffle_wg(0, in, w_packed + (size_t)2 * 16 * Cin * Cout, bias, out, B, Cin, H, W, Cout,
-                                                   relu, s);
+            const int rc = launch_convt_shuffle_wg(0, in, w_packed + conv_pack_shuffle_offset(Cout, Cin, kh, kw), bias, out,
+                                                   B, Cin, H, W, Cout, relu, s);
             if (rc != VQB_ERR_UNSUPPORTED) return rc;
         }
         if (!transposed && Cin == 3 && Cout % 32 == 0 && in_layout == VQB_NCHW && out_layout == VQB_NHWC &&
@@ -132,8 +132,7 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     if (tc && nph > 0) {
         WgLaunch L;
         L.in = in; L.B = B; L.Cin = Cin; L.H = H; L.W = W;
-        L.w = w_packed + (size_t)kh * kw * Cin * Cout;              // the K-major region
-        L.ncols = Cout;
+        L.w = w_packed; L.ncols = Cout;
         L.bias = bias; L.skip = skip; L.out = out; L.relu = relu;
         L.out_sn = p.out_sn; L.out_sh = p.out_sh; L.out_sw = p.out_sw; L.out_sc = p.out_sc;
         // the launcher answers VQB_ERR_UNSUPPORTED before launching anything when it cannot take the shape (step
@@ -233,7 +232,7 @@ extern "C" int vqb_vq_forward_bf16zq_f32(const float *z, const float *codebook, 
 }
 
 // encoder.py:29-31 in the VQB_BF16 pipeline: fp32 NCHW image in, bf16 NHWC activation out (Cout == 64), fp32 FFMA
-// arithmetic (conv_edge.cu).  w_packed: vqb_pack_conv_weight_f32 of the layer.
+// arithmetic (conv_edge.cu).  w_packed: vqb_pack_conv_weight_f32 of the layer (K-major rows, the same as the fp32 mode).
 extern "C" int vqb_conv_in_bf16(const float *x, const float *w_packed, const float *bias, void *out, int B, int H, int W,
                                 int Cout, int relu, void *stream) {
     if (!x || !w_packed || !out) return VQB_ERR_BAD_ARG;
@@ -266,8 +265,7 @@ extern "C" int vqb_residual_layer_f32(const float *r, const float *w1_packed, co
     if (precision < VQB_FP32 || precision > VQB_BF16) return VQB_ERR_BAD_ARG;
     if (precision == VQB_BF16) return VQB_ERR_UNSUPPORTED;      // see vqb_residual_layer_bf16
     if (precision == VQB_TF32 && res_wg_supported(0, C, Cmid)) {      // one wgmma launch, the intermediate stays on chip
-        const int rc = launch_res_wg(0, r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
-                                     relu_out, 1, (cudaStream_t)stream);
+        const int rc = launch_res_wg(0, r, w1_packed, w2_packed, out, B, H, W, C, Cmid, relu_out, 1, (cudaStream_t)stream);
         if (rc != VQB_ERR_UNSUPPORTED) return rc;
     }
     // two launches (residual.py:20-24 then :23-24,:28)
@@ -289,8 +287,7 @@ extern "C" int vqb_residual_stack_f32(const float *r, const float *w1_packed, co
     if (precision == VQB_BF16) return VQB_ERR_UNSUPPORTED;
     if (n_layers > 1 && precision == VQB_TF32 && res_wg_supported(0, C, Cmid)) {
         // all applications in ONE launch when a tile holds whole images (answers VQB_ERR_UNSUPPORTED otherwise)
-        const int rc = launch_res_wg(0, r, w1_packed + (size_t)9 * C * Cmid, w2_packed + (size_t)C * Cmid, out, B, H, W, C, Cmid,
-                                     1, n_layers, (cudaStream_t)stream);
+        const int rc = launch_res_wg(0, r, w1_packed, w2_packed, out, B, H, W, C, Cmid, 1, n_layers, (cudaStream_t)stream);
         if (rc != VQB_ERR_UNSUPPORTED) return rc;
     }
     // one launch per application, ping-ponging so that the last one lands in `out`

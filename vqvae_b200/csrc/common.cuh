@@ -28,7 +28,7 @@ struct ConvGeom {
 // One sub-pixel phase of a layer as a gather-form convolution
 //   out[n, gy*out_step+out_py, gx*out_step+out_px, co] =
 //       act( bias[co] + skip + sum_{t<ntaps, ci} in[n, gy*in_step+dy[t], gx*in_step+dx[t], ci]
-//                                                * w[tap_w[t]*Cin + ci][co] )
+//                                                * w[tap_w[t]][co][ci] )
 // which covers nn.Conv2d (in_step = stride, out_step = 1, dy = r - pad), stride-1
 // nn.ConvTranspose2d (dy = pad - r) and one sub-pixel phase of a stride-s
 // nn.ConvTranspose2d (in_step = 1, out_step = s, taps of matching parity).
@@ -45,7 +45,7 @@ bool conv_phase(const ConvGeom &g, int i, ConvPhase &ph);
 
 // One launch of a CUDA-core conv kernel: one phase of a layer on fp32 tensors.
 struct ConvLaunch : ConvPhase {
-    const float *in, *w, *bias, *skip;
+    const float *in, *w, *bias, *skip;         // w: the K-major rows [kh*kw][Cout][Cin] of vqb_pack_conv_weight_f32
     float *out;
     int B, Cin, H, W, Cout;
     long long in_sn, in_sh, in_sw, in_sc;      // element strides of `in`
@@ -55,6 +55,10 @@ struct ConvLaunch : ConvPhase {
 
 int launch_conv_ffma(const ConvLaunch &p, cudaStream_t s);
 int launch_conv_small_cout(const ConvLaunch &p, cudaStream_t s);
+
+// vqb_pack_conv_weight_f32 writes the K-major rows [kh*kw][Cout][Cin] from element 0; the [9][16][Cin] pixel-shuffle
+// form of a k4 s2 transposed conv to Cout <= 4 channels starts here, in floats.
+static inline size_t conv_pack_shuffle_offset(int Cout, int Cin, int kh, int kw) { return (size_t)kh * kw * Cout * Cin; }
 
 // The weight vqb_pack_conv_weight_bf16 writes: K-major bf16 rows [kh*kw][Cout][Cin_pad] (zero padded from Cin), or
 // for shuffle != 0 the [9][16][Cin] form of the k4 s2 output layer.

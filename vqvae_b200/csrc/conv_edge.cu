@@ -21,9 +21,13 @@ template <int CIN, bool OUT_BF16>
 __global__ void __launch_bounds__(256, 2)
 conv_in_k4s2_kernel(const float *__restrict__ x, const float *__restrict__ wp, const float *__restrict__ bias,
                     void *__restrict__ y, int B, int H, int W, int Cout, int relu) {
-    extern __shared__ __align__(16) float wsm[];          // [16*CIN][Cout]
-    const int K = 16 * CIN;
-    for (int i = threadIdx.x; i < K * Cout; i += blockDim.x) wsm[i] = __ldg(wp + i);
+    extern __shared__ __align__(16) float wsm[];          // [16*CIN][Cout], from the K-major packing [16][Cout][CIN]
+    // a warp copies the K-major rows of 32 output channels of one tap: 32 * CIN contiguous floats
+    for (int g = threadIdx.x >> 5; g < 16 * (Cout / 32); g += blockDim.x >> 5) {
+        const int tap = g % 16, co = (g / 16) * 32 + (threadIdx.x & 31);
+#pragma unroll
+        for (int ci = 0; ci < CIN; ++ci) wsm[(tap * CIN + ci) * Cout + co] = __ldg(wp + (tap * Cout + co) * CIN + ci);
+    }
     __syncthreads();
     const int OH = H / 2, OW = W / 2;                      // (H + 2 - 4)/2 + 1
     const int groups = Cout / 32;
@@ -183,7 +187,7 @@ convt_out_k4s2_kernel(const float *__restrict__ x, const float *__restrict__ wk,
 }  // namespace
 
 // Conv2d(Cin in {1..4} -> Cout % 32 == 0), k4 s2 p1, NCHW in, NHWC out (fp32, or bf16 when out_bf16).
-// wp = FFMA packing.
+// wp = vqb_pack_conv_weight_f32.
 int launch_conv_in_k4s2(const float *x, const float *wp, const float *bias, void *y, int out_bf16, int B, int Cin, int H,
                         int W, int Cout, int relu, cudaStream_t s) {
     if (Cin != 3 || Cout % 32 != 0 || H % 2 || W % 2) return VQB_ERR_UNSUPPORTED;
@@ -201,7 +205,7 @@ int launch_conv_in_k4s2(const float *x, const float *wp, const float *bias, void
     return vqb_cuda_status(cudaGetLastError());
 }
 
-// ConvTranspose2d(Cin % 4 == 0 -> Cout == 3), k4 s2 p1, NHWC in, NCHW out.  wp = FFMA packing.
+// ConvTranspose2d(Cin % 4 == 0 -> Cout == 3), k4 s2 p1, NHWC in, NCHW out.  wp = vqb_pack_conv_weight_f32.
 int launch_convt_out_k4s2(const float *x, const float *wp, const float *bias, float *y, int B, int Cin, int H, int W,
                           int Cout, int relu, cudaStream_t s) {
     const int L = Cin / 4;
@@ -216,9 +220,7 @@ int launch_convt_out_k4s2(const float *x, const float *wp, const float *bias, fl
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (blocks > (long long)sms * 2) blocks = (long long)sms * 2;       // persistent: weights staged once per CTA
     if (blocks < 1) blocks = 1;
-    // K-major half of the packed weight: [tap][Cout][Cin]
-    convt_out_k4s2_kernel<3><<<(unsigned)blocks, 256, smem, s>>>(x, wp + (size_t)16 * Cin * Cout, bias, y, B, H, W,
-                                                                 Cin, relu);
+    convt_out_k4s2_kernel<3><<<(unsigned)blocks, 256, smem, s>>>(x, wp, bias, y, B, H, W, Cin, relu);
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }

@@ -8,9 +8,10 @@
 // residual.py:20-24, vqvae.py:16-17, decoder.py:28-35.
 //
 // Implicit GEMM:  C[m][co] = sum_k A[m][k] * Wp[k][co],  m = (n, gy, gx) output
-// pixel, k = (tap, ci).  A is gathered on the fly (never materialised), Wp is the
-// tap-major packed weight.  Tile BM x BN x 16, 256 threads, TM x TN registers per
-// thread, global->register prefetch of the next k-tile overlapped with the FFMAs.
+// pixel, k = (tap, ci).  A is gathered on the fly (never materialised); Wp[k][co] is
+// read from the K-major packed weight [tap][co][ci] and stored transposed into shared
+// memory.  Tile BM x BN x 16, 256 threads, TM x TN registers per thread,
+// global->register prefetch of the next k-tile overlapped with the FFMAs.
 #include "common.cuh"
 
 namespace {
@@ -21,9 +22,9 @@ constexpr int NT = 256;
 template <int BM, int BN, int TM, int TN, bool VEC_A>
 __global__ void __launch_bounds__(NT) conv_ffma_kernel(const ConvLaunch p) {
     static_assert((BM / TM) * (BN / TN) == NT, "thread tiling");
-    constexpr int APAD = 4;
+    constexpr int APAD = 4, BPAD = 4;
     __shared__ __align__(16) float As[2][BK][BM + APAD];
-    __shared__ __align__(16) float Bs[2][BK][BN];
+    __shared__ __align__(16) float Bs[2][BK][BN + BPAD];
     __shared__ long long row_in[BM];   // n * in_sn
     __shared__ long long row_out[BM];  // full output offset (without co)
     __shared__ int row_iy[BM], row_ix[BM];
@@ -60,8 +61,7 @@ __global__ void __launch_bounds__(NT) conv_ffma_kernel(const ConvLaunch p) {
     constexpr int A_VEC_PER_THREAD = BM * BK / 4 / NT;  // float4s
     constexpr int B_VEC_PER_THREAD = (BK * BN / 4 + NT - 1) / NT;
     float a_reg[A_PER_THREAD];
-    float4 b_reg[B_VEC_PER_THREAD];
-    const bool vec_b = (p.Cout % 4 == 0);
+    float4 b_reg[B_VEC_PER_THREAD];   // Bs[k][c..c+3], k = f % BK, c = (f / BK) * 4
 
     auto load_tile = [&](int k0) {
         if (VEC_A) {
@@ -106,21 +106,16 @@ __global__ void __launch_bounds__(NT) conv_ffma_kernel(const ConvLaunch p) {
         for (int i = 0; i < B_VEC_PER_THREAD; ++i) {
             int f = tid + i * NT;
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (f < BK * BN / 4) {
-                int k = f / (BN / 4), c = (f % (BN / 4)) * 4;
-                int gk = k0 + k, co = n0 + c;
-                if (gk < Ktot) {
-                    int t = gk / p.Cin, ci = gk - t * p.Cin;
-                    const float *wr = p.w + ((long long)p.tap_w[t] * p.Cin + ci) * p.Cout;
-                    if (vec_b && co + 3 < p.Cout) {
-                        v = __ldg(reinterpret_cast<const float4 *>(wr + co));
-                    } else {
-                        if (co + 0 < p.Cout) v.x = __ldg(wr + co + 0);
-                        if (co + 1 < p.Cout) v.y = __ldg(wr + co + 1);
-                        if (co + 2 < p.Cout) v.z = __ldg(wr + co + 2);
-                        if (co + 3 < p.Cout) v.w = __ldg(wr + co + 3);
-                    }
-                }
+            const int gk = k0 + f % BK, co = n0 + (f / BK) * 4;
+            if (f < BK * BN / 4 && gk < Ktot) {
+                // B[k = t*Cin + ci][co] is w[tap_w[t]][co][ci]: lanes run along ci, so a warp reads 64 contiguous
+                // bytes of each of its weight rows
+                const int t = gk / p.Cin, ci = gk - t * p.Cin;
+                const float *wr = p.w + ((long long)p.tap_w[t] * p.Cout + co) * p.Cin + ci;
+                if (co + 0 < p.Cout) v.x = __ldg(wr);
+                if (co + 1 < p.Cout) v.y = __ldg(wr + p.Cin);
+                if (co + 2 < p.Cout) v.z = __ldg(wr + 2 * p.Cin);
+                if (co + 3 < p.Cout) v.w = __ldg(wr + 3 * p.Cin);
             }
             b_reg[i] = v;
         }
@@ -144,10 +139,9 @@ __global__ void __launch_bounds__(NT) conv_ffma_kernel(const ConvLaunch p) {
 #pragma unroll
         for (int i = 0; i < B_VEC_PER_THREAD; ++i) {
             int f = tid + i * NT;
-            if (f < BK * BN / 4) {
-                int k = f / (BN / 4), c = (f % (BN / 4)) * 4;
-                *reinterpret_cast<float4 *>(&Bs[buf][k][c]) = b_reg[i];
-            }
+            // (row pitch BN + BPAD = 4 mod 32 floats: the eight float4s of a quarter warp, k = 0..7 or 8..15, hit
+            // distinct banks)
+            if (f < BK * BN / 4) *reinterpret_cast<float4 *>(&Bs[buf][f % BK][(f / BK) * 4]) = b_reg[i];
         }
     };
 
@@ -226,10 +220,10 @@ __global__ void __launch_bounds__(NT) conv_ffma_kernel(const ConvLaunch p) {
 __global__ void __launch_bounds__(256) conv_small_cout_kernel(const ConvLaunch p) {
     extern __shared__ float wsm[];  // [ntaps][Cin][4]
     const int Cin = p.Cin;
-    for (int i = threadIdx.x; i < p.ntaps * Cin * 4; i += blockDim.x) {
-        int co = i & 3, rest = i >> 2;
-        int t = rest / Cin, ci = rest - t * Cin;
-        wsm[i] = co < p.Cout ? __ldg(p.w + ((long long)p.tap_w[t] * Cin + ci) * p.Cout + co) : 0.f;
+    // each tap's K-major rows, read along ci, padded with zero rows to 4 output channels
+    for (int i = threadIdx.x; i < p.ntaps * 4 * Cin; i += blockDim.x) {
+        const int ci = i % Cin, row = i / Cin, co = row & 3, t = row >> 2;
+        wsm[(t * Cin + ci) * 4 + co] = co < p.Cout ? __ldg(p.w + ((long long)p.tap_w[t] * p.Cout + co) * Cin + ci) : 0.f;
     }
     __syncthreads();
     const long long M = (long long)p.B * p.OHg * p.OWg;

@@ -5,26 +5,22 @@
 
 namespace {
 
-// (Cout,Cin,kh,kw) or ConvTranspose (Cin,Cout,kh,kw)  ->  the tap-major GEMM operand layouts:
-//   nmajor   [(r*kw+s)*Cin + ci][co]     (N-major, the FFMA kernel's B tile; fp32 only, may be null)
-//   kmajor   [(r*kw+s)][co][ci]          (K-major rows of Cin_pad >= Cin channels, zero padded: the wgmma B operand)
-// T = float or __nv_bfloat16 (rounded to nearest even).  nmajor requires Cin_pad == Cin.
+// (Cout,Cin,kh,kw) or ConvTranspose (Cin,Cout,kh,kw)  ->  K-major rows [(r*kw+s)][co][ci] of Cin_pad >= Cin
+// channels, zero padded: the B operand of every conv kernel.  T = float or __nv_bfloat16 (rounded to nearest even).
 template <typename T>
-__global__ void pack_weight_kernel(const float *__restrict__ w, float *__restrict__ nmajor, T *__restrict__ kmajor,
-                                   int Cout, int Cin, int Cin_pad, int kh, int kw, int transposed) {
+__global__ void pack_weight_kernel(const float *__restrict__ w, T *__restrict__ out, int Cout, int Cin, int Cin_pad,
+                                   int kh, int kw, int transposed) {
     const long long total = (long long)Cout * Cin_pad * kh * kw;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
-        const int co = (int)(i % Cout);
-        long long t = i / Cout;
-        const int ci = (int)(t % Cin_pad);
-        const int tap = (int)(t / Cin_pad);
+        const int ci = (int)(i % Cin_pad);
+        long long t = i / Cin_pad;
+        const int co = (int)(t % Cout);
+        const int tap = (int)(t / Cout);
         const int r = tap / kw, s = tap % kw;
         const long long src = transposed ? ((((long long)ci * Cout + co) * kh + r) * kw + s)
                                          : ((((long long)co * Cin + ci) * kh + r) * kw + s);
-        const float v = ci < Cin ? w[src] : 0.f;
-        if (nmajor) nmajor[i] = v;
-        kmajor[((long long)tap * Cout + co) * Cin_pad + ci] = T(v);
+        out[i] = T(ci < Cin ? w[src] : 0.f);
     }
 }
 
@@ -143,12 +139,11 @@ unsigned grid_for(long long total, int block) {
 extern "C" int vqb_pack_conv_weight_f32(const float *w, float *packed, int Cout, int Cin, int kh, int kw,
                                         int transposed, void *stream) {
     if (!w || !packed || Cout <= 0 || Cin <= 0 || kh <= 0 || kw <= 0) return VQB_ERR_BAD_ARG;
-    const long long total = (long long)Cout * Cin * kh * kw;
-    pack_weight_kernel<float><<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(w, packed, packed + total, Cout, Cin,
-                                                                                     Cin, kh, kw, transposed);
+    pack_weight_kernel<float><<<grid_for((long long)Cout * Cin * kh * kw, 256), 256, 0, (cudaStream_t)stream>>>(
+        w, packed, Cout, Cin, Cin, kh, kw, transposed);
     if (transposed && kh == 4 && kw == 4 && Cout <= 4) {
-        pack_convt_shuffle_kernel<float><<<grid_for(9 * 16 * Cin, 256), 256, 0, (cudaStream_t)stream>>>(w, packed + 2 * total,
-                                                                                                      Cout, Cin);
+        pack_convt_shuffle_kernel<float><<<grid_for(9 * 16 * Cin, 256), 256, 0, (cudaStream_t)stream>>>(
+            w, packed + conv_pack_shuffle_offset(Cout, Cin, kh, kw), Cout, Cin);
         VQB_COUNT_LAUNCH(1);
     }
     VQB_COUNT_LAUNCH(1);
@@ -161,8 +156,8 @@ int launch_pack_weight_bf16(const float *w, void *out, int Cout, int Cin, int Ci
     if (shuffle)
         pack_convt_shuffle_kernel<<<grid_for(9 * 16 * Cin, 256), 256, 0, s>>>(w, o, Cout, Cin);
     else
-        pack_weight_kernel<<<grid_for((long long)Cout * Cin_pad * kh * kw, 256), 256, 0, s>>>(w, nullptr, o, Cout, Cin,
-                                                                                            Cin_pad, kh, kw, transposed);
+        pack_weight_kernel<<<grid_for((long long)Cout * Cin_pad * kh * kw, 256), 256, 0, s>>>(w, o, Cout, Cin, Cin_pad,
+                                                                                            kh, kw, transposed);
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }

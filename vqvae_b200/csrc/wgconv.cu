@@ -460,7 +460,8 @@ int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void 
 // ------------------------------------------------------------------------------------------------ output layer
 // decoder.py:34-35, ConvTranspose2d(Cin -> Cout <= 4, k4 s2 p1), NHWC in, NCHW fp32 out: one GEMM over the
 // 3x3 input neighbourhood with N = 16 columns (sub-pixel phase, channel) and a pixel-shuffle epilogue.
-// w_shuffle: [9 taps (dy, dx)][16][Cin] (the third region of vqb_pack_conv_weight_f32, or vqb_pack_conv_weight_bf16).
+// w_shuffle: [9 taps (dy, dx)][16][Cin] (the region of vqb_pack_conv_weight_f32 at conv_pack_shuffle_offset, or
+// vqb_pack_conv_weight_bf16).
 bool convt_shuffle_supported(int Cin, int Cout) { return Cout >= 1 && Cout <= 4 && Cin % 32 == 0 && 9 * (Cin / 32) <= WG_MAX_STEPS; }
 
 int launch_convt_shuffle_wg(int bf16, const void *in, const void *w_shuffle, const float *bias, float *out, int B, int Cin,

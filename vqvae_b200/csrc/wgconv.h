@@ -40,8 +40,7 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s);
 int wg_gemm_cols(int ncols);           // smallest supported N >= ncols, 0 if none
 
 // The layer launchers take the operand type (bf16 = 0: fp32 activations read as TF32, 1: bf16) and a weight of
-// K-major rows per tap, [tap][rows][Cin], as vqb_pack_conv_weight_f32 (its K-major regions) and
-// vqb_pack_conv_weight_bf16 write them.
+// K-major rows per tap, [tap][rows][Cin], as vqb_pack_conv_weight_f32 and vqb_pack_conv_weight_bf16 write them.
 bool conv_tc_supported(const ConvLaunch &p);
 // L: the tensors, ncols = Cout, output strides and epilogue of one layer; ph[0..nph): its phases, one launch
 // (blockIdx.y = phase) over the weight [total_taps][Cout][Cin]

@@ -70,8 +70,8 @@ def _param_tag(param):
 
 
 def _pack_key(conv, bf16):
-    """The packing of a conv container's weight that the forward reads in a mode: ("f32", transposed), the tap-major
-    fp32 layouts of vqb_pack_conv_weight_f32, or in the bf16 pipeline ("bf16", kind), the same K-major layout in bf16
+    """The packing of a conv container's weight that the forward reads in a mode: ("f32", transposed), the K-major
+    fp32 layout of vqb_pack_conv_weight_f32, or in the bf16 pipeline ("bf16", kind), the same K-major layout in bf16
     from vqb_pack_conv_weight_bf16, for the kind the layer's geometry names.  A container that the bf16 pipeline
     reads differently carries its key as ``_bf16_key``, set by the module that builds it."""
     transposed = isinstance(conv, nn.ConvTranspose2d)

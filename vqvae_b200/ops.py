@@ -60,17 +60,16 @@ def _f32c(t):
 
 
 def pack_conv_weight(w, transposed, out=None):
-    """(Cout,Cin,kh,kw) conv / (Cin,Cout,kh,kw) conv-transpose weight -> the two tap-major
-    fp32 GEMM operand layouts of vqb_pack_conv_weight_f32, back to back:
-    [(r*kw+s)*Cin+ci][co] for the FFMA kernel and [(r*kw+s)][co][ci] for wgmma."""
+    """(Cout,Cin,kh,kw) conv / (Cin,Cout,kh,kw) conv-transpose weight -> the fp32 packing of
+    vqb_pack_conv_weight_f32: K-major rows [(r*kw+s)][co][ci], which every conv kernel reads, then
+    room for the [9][16][Cin] pixel-shuffle form that a k4 s2 transposed conv to <= 4 channels adds."""
     _require_cuda(w, "weight")
     w = _f32c(w.detach())
     if transposed:
         cin, cout, kh, kw = w.shape
     else:
         cout, cin, kh, kw = w.shape
-    # 2 GEMM layouts + (for the k4s2 output layer) the 9x16xCin pixel-shuffle packing
-    n = 2 * kh * kw * cin * cout + 9 * 16 * cin
+    n = kh * kw * cin * cout + 9 * 16 * cin
     if out is None or out.numel() != n or out.dtype != torch.float32 or out.device != w.device:
         out = torch.empty((n,), dtype=torch.float32, device=w.device)      # else: repacked in place
     check(lib().vqb_pack_conv_weight_f32(w.data_ptr(), out.data_ptr(), cout, cin, kh, kw,
