@@ -315,6 +315,40 @@ int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *labels, cons
                            int64_t *codes, float *step_logits, void *workspace, size_t workspace_bytes,
                            void *stream);
 
+/* ---- Gated PixelCNN prior, training (fp32 on CUDA cores) ------------------------------------------------------
+ * The forward keeps its activations in `saved`; the backward turns d_logits into the gradient of every parameter.
+ * Shape limits and argument checks are those of vqb_prior_forward_f32.                                          */
+/* Bytes of `saved` on a (B, H, W) grid: 4*B*H*W*(dim*(6*n_layers + 3) + 512) (0 = bad sizes).                   */
+size_t vqb_prior_train_saved_bytes(int B, int H, int W, int dim, int n_layers);
+/* vqb_prior_forward_f32 that also stores, per layer, x_v, x_h, h_vert (bias included, class embedding not) and the
+ * horizontal gate's pre-activation, and the head's 512-wide hidden layer.  The same kernels and arithmetic: the
+ * logits are bitwise those of vqb_prior_forward_f32.  2 + 2*n_layers launches.                                   */
+int vqb_prior_forward_train_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                                int W, float *logits, void *saved, size_t saved_bytes, void *stream);
+
+/* Device output pointers of every gradient, shaped like vqb_prior_layer_weights / vqb_prior_net, each in its
+ * parameter's own layout: (Cout, Cin, kh, kw) for the convs, (rows, cols) for the embeddings.  The conv gradients
+ * cover all kh*kw taps, mask A's included.                                                                        */
+typedef struct vqb_prior_layer_grads {
+    float *vert_w, *vert_b, *v2h_w, *v2h_b, *horiz_w, *horiz_b, *resid_w, *resid_b, *class_emb;
+} vqb_prior_layer_grads;
+
+typedef struct vqb_prior_grads {
+    const vqb_prior_layer_grads *layers;      /* host array of n_layers entries */
+    int n_layers;
+    float *embedding, *out1_w, *out1_b, *out2_w, *out2_b;
+} vqb_prior_grads;
+
+/* Workspace of vqb_prior_backward_f32 for this net on a (B, H, W) grid (0 = bad arguments).                     */
+size_t vqb_prior_backward_workspace_bytes(const vqb_prior_net *net, int B, int H, int W);
+/* Gradients of every parameter from d_logits (B, input_dim, H, W) fp32 NCHW, codes, labels and the `saved` of a
+ * vqb_prior_forward_train_f32 call with the same net and inputs.  Overwrites every gradient (no accumulation).
+ * Deterministic: fixed-order sums, no atomics; two calls give bitwise-equal gradients.  No host synchronisation.
+ * 7 + 10*n_layers launches.                                                                                      */
+int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                           const float *d_logits, const void *saved, const vqb_prior_grads *grads, void *workspace,
+                           size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

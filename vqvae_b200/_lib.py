@@ -60,6 +60,10 @@ SIGNATURES = {
     "vqb_prior_layer_f32": (_i, [_vp] * 4 + [_i] * 5 + [_vp] * 4),
     "vqb_prior_forward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
     "vqb_prior_generate_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
+    "vqb_prior_train_saved_bytes": (_sz, [_i] * 5),
+    "vqb_prior_forward_train_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
+    "vqb_prior_backward_workspace_bytes": (_sz, [_vp] + [_i] * 3),
+    "vqb_prior_backward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 4 + [_sz, _vp]),
 }
 
 PRIOR_MAX_LAYERS = 32       # VQB_PRIOR_MAX_LAYERS
@@ -75,6 +79,18 @@ class PriorNet(C.Structure):
     """struct vqb_prior_net"""
     _fields_ = [("layers", C.POINTER(PriorLayerWeights)), ("n_layers", _i), ("embedding", _vp), ("out1_w", _vp),
                 ("out1_b", _vp), ("out2_w", _vp), ("out2_b", _vp), ("input_dim", _i), ("dim", _i), ("n_classes", _i)]
+
+
+class PriorLayerGrads(C.Structure):
+    """struct vqb_prior_layer_grads"""
+    _fields_ = [(n, _vp) for n in ("vert_w", "vert_b", "v2h_w", "v2h_b", "horiz_w", "horiz_b", "resid_w", "resid_b",
+                                   "class_emb")]
+
+
+class PriorGrads(C.Structure):
+    """struct vqb_prior_grads"""
+    _fields_ = [("layers", C.POINTER(PriorLayerGrads)), ("n_layers", _i), ("embedding", _vp), ("out1_w", _vp),
+                ("out1_b", _vp), ("out2_w", _vp), ("out2_b", _vp)]
 
 
 def lib():

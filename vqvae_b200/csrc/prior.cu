@@ -6,28 +6,9 @@
 // started from 0, then the bias: the value of an element does not depend on which positions share a block or on how
 // many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
 // sampler's logits are bitwise the forward's logits on the grid it produced.
-#include "common.cuh"
+#include "prior.cuh"
 
 namespace {
-
-constexpr int NT = 256;           // threads of every prior kernel
-constexpr int MAXC = 256;         // dim <= 256, dim % 32 == 0
-constexpr int HID = 512;          // output_conv.0: dim -> 512 (models.py:109)
-constexpr int MAXK = 8192;
-
-struct Act {                      // one NHWC activation buffer, C channels, `ring` rows of W positions per image
-    float *p;
-    int ring, C;
-    __device__ __forceinline__ float *at(int b, int r, int c, int W) const {
-        return p + (((long long)b * ring + r % ring) * W + c) * C;
-    }
-};
-
-struct Net {
-    vqb_prior_layer_weights layer[VQB_PRIOR_MAX_LAYERS];
-    const float *emb, *w1, *b1, *w2, *b2;
-    int L, C, K, NC;
-};
 
 // one block's positions: image, row, column and clamped label of each of its P slots (b < 0: slot unused)
 template <int P>
@@ -36,10 +17,6 @@ struct Smem {
     float pre[HID * P];           // [c][p]: pre-activations (2*dim) or the head's hidden layer (512)
     int b[P], r[P], c[P], lab[P];
 };
-
-__device__ __forceinline__ float gate(float a, float g) {      // GatedActivation: tanh(x) * sigmoid(y)
-    return tanhf(a) * (1.f / (1.f + expf(-g)));
-}
 
 template <int P>
 __device__ __forceinline__ void load_vec(float (&v)[P], const float *s) {
@@ -95,9 +72,10 @@ __device__ __forceinline__ int horiz_cols(const vqb_prior_layer_weights &w) { re
 
 // Vertical stack of one layer at the P positions of the block (models.py:69-72, :77):
 //   h_vert = vert_stack(x_v) ; out_v = gate(h_vert + emb[label]) ; vh = vert_to_horiz(h_vert) + emb[label]
+// keep.p != nullptr (the training forward) also stores h_vert there for the backward.
 template <int P>
 __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &out_v,
-                               const Act &vh, int H, int W) {
+                               const Act &vh, int H, int W, const Act &keep) {
     const int C = in.C, C2 = 2 * C, tid = threadIdx.x;
     float acc[2][P];
 #pragma unroll
@@ -117,7 +95,10 @@ __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, con
         const int c = tid + q * NT;
         if (c < C2)
 #pragma unroll
-            for (int p = 0; p < P; ++p) s.pre[c * P + p] = acc[q][p] + __ldg(w.vert_b + c);
+            for (int p = 0; p < P; ++p) {
+                s.pre[c * P + p] = acc[q][p] + __ldg(w.vert_b + c);
+                if (keep.p && s.b[p] >= 0) keep.at(s.b[p], s.r[p], s.c[p], W)[c] = s.pre[c * P + p];
+            }
     }
     __syncthreads();
     for (int i = tid; i < P * C; i += NT) {
@@ -145,10 +126,11 @@ __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, con
 
 // Horizontal stack of one layer at the P positions of the block (models.py:74-83):
 //   out = gate(horiz_stack(x_h) + vh) ; out_h = horiz_resid(out) [+ x_h]
-// The forward's per-layer kernel and the sampler's position step both run this.
+// The forward's per-layer kernel and the sampler's position step both run this.  keep.p != nullptr (the training
+// forward) also stores the gate's pre-activation there.
 template <int P>
 __device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &vh,
-                                const Act &out_h, int H, int W) {
+                                const Act &out_h, int H, int W, const Act &keep) {
     const int C = in.C, C2 = 2 * C, tid = threadIdx.x;
     float acc[2][P];
 #pragma unroll
@@ -167,8 +149,10 @@ __device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, co
         const int c = tid + q * NT;
         if (c >= C2) continue;
 #pragma unroll
-        for (int p = 0; p < P; ++p)
+        for (int p = 0; p < P; ++p) {
             s.pre[c * P + p] = s.b[p] >= 0 ? (acc[q][p] + __ldg(w.horiz_b + c)) + vh.at(s.b[p], s.r[p], s.c[p], W)[c] : 0.f;
+            if (keep.p && s.b[p] >= 0) keep.at(s.b[p], s.r[p], s.c[p], W)[c] = s.pre[c * P + p];
+        }
     }
     __syncthreads();
     for (int i = tid; i < P * C; i += NT) {
@@ -192,10 +176,11 @@ __device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, co
 }
 
 // output_conv (models.py:107-111): logits = W2 . relu(W1 . x_h + b1) + b2 at the P positions of the block.
-// Logit k of slot p goes to out[p] + k * kstride.
+// Logit k of slot p goes to out[p] + k * kstride.  keep.p != nullptr (the training forward) also stores the hidden
+// layer there.
 template <int P>
 __device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, float *const (&out)[P], long long kstride,
-                               int H, int W) {
+                               int H, int W, const Act &keep) {
     const int C = n.C, tid = threadIdx.x;
     __syncthreads();
     load_tap(s, in, 0, 0, H, W);
@@ -206,7 +191,10 @@ __device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, float *c
         for (int p = 0; p < P; ++p) acc[0][p] = 0.f;
         mac<P, 1>(acc, s.x, n.w1, C, HID, c0);
 #pragma unroll
-        for (int p = 0; p < P; ++p) s.pre[(c0 + tid) * P + p] = fmaxf(acc[0][p] + __ldg(n.b1 + c0 + tid), 0.f);
+        for (int p = 0; p < P; ++p) {
+            s.pre[(c0 + tid) * P + p] = fmaxf(acc[0][p] + __ldg(n.b1 + c0 + tid), 0.f);
+            if (keep.p && s.b[p] >= 0) keep.at(s.b[p], s.r[p], s.c[p], W)[c0 + tid] = s.pre[(c0 + tid) * P + p];
+        }
     }
     __syncthreads();
     for (int c0 = 0; c0 < n.K; c0 += NT) {
@@ -221,8 +209,6 @@ __device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, float *c
                 if (s.b[p] >= 0) out[p][k * kstride] = acc[0][p] + __ldg(n.b2 + k);
     }
 }
-
-__device__ __forceinline__ int clampi(long long v, int n) { return v < 0 ? 0 : (v >= n ? n - 1 : (int)v); }
 
 // Slots of a block over the positions [row0, row0 + nrows) x [0, W) of all B images, position-major in (b, row, col).
 template <int P>
@@ -246,24 +232,24 @@ __device__ void set_slots(Smem<P> &s, int B, int row0, int nrows, int W, const l
 template <int P>
 __global__ void __launch_bounds__(NT) vert_kernel(vqb_prior_layer_weights w, Act in, Act out_v, Act vh,
                                                   const long long *labels, int NC, int B, int H, int W, int row0,
-                                                  int nrows) {
+                                                  int nrows, Act keep) {
     __shared__ __align__(16) Smem<P> s;
     set_slots(s, B, row0, nrows, W, labels, NC);
-    vert_positions(s, w, in, out_v, vh, H, W);
+    vert_positions(s, w, in, out_v, vh, H, W, keep);
 }
 
 template <int P>
 __global__ void __launch_bounds__(NT) horiz_kernel(vqb_prior_layer_weights w, Act in, Act vh, Act out_h,
-                                                   const long long *labels, int NC, int B, int H, int W) {
+                                                   const long long *labels, int NC, int B, int H, int W, Act keep) {
     __shared__ __align__(16) Smem<P> s;
     set_slots(s, B, 0, H, W, labels, NC);
-    horiz_positions(s, w, in, vh, out_h, H, W);
+    horiz_positions(s, w, in, vh, out_h, H, W, keep);
 }
 
 // logits NCHW (B, K, H, W)
 template <int P>
 __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long *labels, int B, int H, int W,
-                                                  float *logits) {
+                                                  float *logits, Act keep) {
     __shared__ __align__(16) Smem<P> s;
     __shared__ float *out[P];
     set_slots(s, B, 0, H, W, labels, n.NC);
@@ -271,7 +257,7 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
         const int p = threadIdx.x;
         out[p] = s.b[p] >= 0 ? logits + (long long)s.b[p] * n.K * H * W + (long long)s.r[p] * W + s.c[p] : nullptr;
     }
-    head_positions(s, n, in, out, (long long)H * W, H, W);
+    head_positions(s, n, in, out, (long long)H * W, H, W, keep);
 }
 
 // embedding (models.py:122): x0[n] = E[clamp(codes[n])]
@@ -302,10 +288,10 @@ __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act 
         const Act in = l == 0 ? x0 : Act{xrow0.p + (l - 1) * x_stride, 1, n.C};
         const Act vh{vh0.p + l * vh_stride, 1, 2 * n.C};
         const Act o{xrow0.p + l * x_stride, 1, n.C};
-        horiz_positions(s, n.layer[l], in, vh, o, H, W);
+        horiz_positions(s, n.layer[l], in, vh, o, H, W, Act{});
         __syncthreads();
     }
-    head_positions(s, n, Act{xrow0.p + (n.L - 1) * x_stride, 1, n.C}, out, 1, H, W);
+    head_positions(s, n, Act{xrow0.p + (n.L - 1) * x_stride, 1, n.C}, out, 1, H, W, Act{});
     __syncthreads();
     // softmax + inverse CDF, one warp per image: lane L owns logits [L*cs, L*cs + cs); the CDF is the fp32 running sum
     // of p_k = expf(l_k - max) / sum, over the lanes' chunk sums scanned in lane order and then within the chunk.
@@ -379,18 +365,6 @@ __global__ void gate_kernel(const float *__restrict__ x, float *__restrict__ out
     }
 }
 
-unsigned grid_for(long long total) {
-    long long g = (total + NT - 1) / NT;
-    return (unsigned)(g > 148LL * 32 ? 148LL * 32 : (g < 1 ? 1 : g));
-}
-
-bool layer_ok(const vqb_prior_layer_weights &w) {
-    return w.vert_w && w.vert_b && w.v2h_w && w.v2h_b && w.horiz_w && w.horiz_b && w.resid_w && w.resid_b &&
-           w.class_emb && w.kernel >= 1 && w.kernel <= VQB_PRIOR_MAX_KERNEL && (w.kernel & 1);
-}
-
-bool dim_ok(int C) { return C % 32 == 0 && C <= MAXC; }
-
 // workspace regions, in floats
 struct Ws {
     long long fwd_v, fwd_vh, fwd_x;               // forward: x0 | v[2] | vh | x[2]  (whole grids)
@@ -412,20 +386,6 @@ Ws ws_layout(long long B, long long H, long long W, long long C, long long L, lo
     w.gen_lg = w.gen_x + L * B * W * C;
     w.gen_total = w.gen_lg + B * K;
     return w;
-}
-
-int net_from(const vqb_prior_net *net, Net &n) {
-    if (!net || !net->layers || !net->embedding || !net->out1_w || !net->out1_b || !net->out2_w || !net->out2_b)
-        return VQB_ERR_BAD_ARG;
-    if (net->n_layers <= 0 || net->dim <= 0 || net->input_dim <= 0 || net->n_classes <= 0) return VQB_ERR_BAD_ARG;
-    if (net->n_layers > VQB_PRIOR_MAX_LAYERS || !dim_ok(net->dim) || net->input_dim > MAXK) return VQB_ERR_UNSUPPORTED;
-    for (int l = 0; l < net->n_layers; ++l) {
-        if (!layer_ok(net->layers[l])) return VQB_ERR_BAD_ARG;
-        n.layer[l] = net->layers[l];
-    }
-    n.emb = net->embedding; n.w1 = net->out1_w; n.b1 = net->out1_b; n.w2 = net->out2_w; n.b2 = net->out2_b;
-    n.L = net->n_layers; n.C = net->dim; n.K = net->input_dim; n.NC = net->n_classes;
-    return 0;
 }
 
 constexpr int PF = 8;             // positions per block of the whole-grid kernels and the row pass
@@ -471,8 +431,8 @@ extern "C" int vqb_prior_layer_f32(const vqb_prior_layer_weights *layer, const f
     const long long n = (long long)B * H * W;
     Act in_v{const_cast<float *>(x_v), H, dim}, in_h{const_cast<float *>(x_h), H, dim};
     Act ov{out_v, H, dim}, oh{out_h, H, dim}, vha{vh, H, 2 * dim};
-    vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H);
-    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W);
+    vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H, Act{});
+    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W, Act{});
     VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -497,10 +457,11 @@ extern "C" int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *co
                                                n.C, x0.p);
     for (int l = 0; l < n.L; ++l) {
         const Act vin = l == 0 ? x0 : v[(l - 1) & 1], xin = l == 0 ? x0 : x[(l - 1) & 1];
-        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H);
-        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W);
+        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H,
+                                                        Act{});
+        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W, Act{});
     }
-    head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, x[(n.L - 1) & 1], lab, B, H, W, logits);
+    head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, x[(n.L - 1) & 1], lab, B, H, W, logits, Act{});
     VQB_COUNT_LAUNCH(2 + 2 * n.L);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -526,7 +487,7 @@ extern "C" int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *l
             const Act vin = l == 0 ? x0 : Act{ws + wl.gen_v + (l - 1) * v_stride, 2, n.C};
             vert_kernel<PF><<<blocks((long long)B * W, PF), NT, 0, s>>>(
                 n.layer[l], vin, Act{ws + wl.gen_v + l * v_stride, 2, n.C}, Act{ws + wl.gen_vh + l * vh_stride, 1, 2 * n.C},
-                lab, n.NC, B, H, W, i, 1);
+                lab, n.NC, B, H, W, i, 1, Act{});
         }
         for (int j = 0; j < W; ++j) {
             float *lg = step_logits ? step_logits + ((long long)i * W + j) * n.K : ws + wl.gen_lg;
@@ -537,5 +498,42 @@ extern "C" int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *l
         }
     }
     VQB_COUNT_LAUNCH((unsigned long long)H * (n.L + W));
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_prior_train_saved_bytes(int B, int H, int W, int dim, int n_layers) {
+    if (B <= 0 || H <= 0 || W <= 0 || dim <= 0 || n_layers <= 0) return 0;
+    return (size_t)Saved{(long long)B * H * W, dim, n_layers}.total() * sizeof(float);
+}
+
+// The teacher-forced forward's kernels, writing every activation into `saved` (prior.cuh: Saved) instead of the
+// ping-pong workspace, plus the three stores the backward needs: the same arithmetic, so bitwise the same logits.
+extern "C" int vqb_prior_forward_train_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                           int B, int H, int W, float *logits, void *saved, size_t saved_bytes,
+                                           void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!codes || !labels || !logits || !saved || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (saved_bytes < vqb_prior_train_saved_bytes(B, H, W, n.C, n.L)) return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *lab = reinterpret_cast<const long long *>(labels);
+    const long long npos = (long long)B * H * W;
+    const Saved sv{npos, n.C, n.L};
+    float *sp = static_cast<float *>(saved);
+    const Act vh{sp + sv.vh(), H, 2 * n.C};
+    embed_kernel<<<grid_for(npos * n.C), NT, 0, s>>>(reinterpret_cast<const long long *>(codes), net->embedding, npos,
+                                                     n.K, n.C, sp + sv.xv(0));
+    for (int l = 0; l < n.L; ++l) {
+        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xv(l), H, n.C},
+                                                        Act{sp + sv.xv(l + 1), H, n.C}, vh, lab, n.NC, B, H, W, 0, H,
+                                                        Act{sp + sv.hv(l), H, 2 * n.C});
+        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xh(l), H, n.C}, vh,
+                                                         Act{sp + sv.xh(l + 1), H, n.C}, lab, n.NC, B, H, W,
+                                                         Act{sp + sv.ph(l), H, 2 * n.C});
+    }
+    head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, Act{sp + sv.xh(n.L), H, n.C}, lab, B, H, W, logits,
+                                                    Act{sp + sv.hid(), H, HID});
+    VQB_COUNT_LAUNCH(2 + 2 * n.L);
     return vqb_cuda_status(cudaGetLastError());
 }

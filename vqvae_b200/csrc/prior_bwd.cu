@@ -1,0 +1,487 @@
+// prior_bwd.cu -- backward of the Gated PixelCNN prior (GatedPixelCNN.forward, pixelcnn/models.py:121-130), fp32 on
+// CUDA cores (sm_90a).
+//
+// Every gradient is a matrix product, run by one shared-memory tiled GEMM (`gemm_kernel`) whose operands are read
+// through small accessor structs: the activations the training forward saved (prior.cuh: Saved), NHWC grids read at a
+// tap's shifted position (im2col on the fly), the forward's packed weights, a one-hot of codes or labels.
+//   dgrad: rows = positions, columns = input channels, reduction = kept taps x output channels
+//   wgrad: rows = output channels, columns = taps x input channels (+ a column of ones: the bias), reduction =
+//          positions, split into fixed chunks; the chunk partials are summed in chunk order by `reduce_kernel`, which
+//          also writes each gradient in its parameter's layout.
+// Every output element is one fmaf chain in a fixed order and no float atomics are used, so the gradients are bitwise
+// reproducible.  Weight gradients cover all kh*kw taps, mask A's included (the reference convolves with the full,
+// zeroed weight, so autograd gives those taps a gradient); dgrad reads the taps the forward kept.
+#include "prior.cuh"
+
+namespace {
+
+constexpr int BM = 64, BN = 64, BK = 16, GT = 256;       // CTA tile, k-step, threads (16 x 16, 4 x 4 outputs each)
+constexpr long long WG_CHUNK = 2048;                     // at most this many positions per wgrad partial
+
+struct Grid {                     // position n of a (B, H, W) grid
+    int H, W;
+    __device__ __forceinline__ void split(int n, int &b, int &r, int &c) const {
+        b = n / (H * W);
+        const int rem = n - b * H * W;
+        r = rem / W;
+        c = rem - r * W;
+    }
+};
+
+// ---- operand accessors: (i, j) -> float; j_fast: consecutive j are consecutive addresses -------------------------
+struct Mat {                      // p[i][j], row length ld
+    const float *p;
+    int ld;
+    static constexpr bool j_fast = true;
+    __device__ __forceinline__ float operator()(int i, int j) const { return __ldg(p + (long long)i * ld + j); }
+};
+
+struct MatT {                     // p[j][i]
+    const float *p;
+    int ld;
+    static constexpr bool j_fast = false;
+    __device__ __forceinline__ float operator()(int i, int j) const { return __ldg(p + (long long)j * ld + i); }
+};
+
+struct Nchw {                     // d_logits (B, K, H, W) as a (positions x K) matrix
+    const float *p;
+    int K, HW;
+    static constexpr bool j_fast = false;
+    __device__ __forceinline__ float operator()(int n, int k) const {
+        const int b = n / HW;
+        return __ldg(p + ((long long)b * K + k) * HW + (n - b * HW));
+    }
+};
+
+struct NchwT {                    // the same as a (K x positions) matrix
+    Nchw a;
+    static constexpr bool j_fast = true;
+    __device__ __forceinline__ float operator()(int k, int n) const { return a(n, k); }
+};
+
+// NHWC grid g (C channels) as (positions x taps*C): column j = tap*C + c reads channel c at row r + sgn*(tr - hr),
+// column c + sgn*(tc - hc) of tap (tr, tc) = (tap / cols, tap % cols); 0 outside the grid.  sgn = +1 is the forward
+// conv's im2col (wgrad), sgn = -1 the transposed conv (dgrad).
+struct Tap {
+    const float *g;
+    int C, cols, hr, hc, sgn;
+    Grid grid;
+    static constexpr bool j_fast = true;
+    __device__ __forceinline__ float operator()(int n, int j) const {
+        const int tap = j / C, c = j - tap * C, tr = tap / cols, tc = tap - tr * cols;
+        int b, r, col;
+        grid.split(n, b, r, col);
+        const int rr = r + sgn * (tr - hr), cc = col + sgn * (tc - hc);
+        if (rr < 0 || rr >= grid.H || cc < 0 || cc >= grid.W) return 0.f;
+        return __ldg(g + (((long long)b * grid.H + rr) * grid.W + cc) * C + c);
+    }
+};
+
+struct Gated {                    // gate(pre) of a saved (positions x 2C) pre-activation: the gated layer's output
+    const float *pre;
+    int C;
+    static constexpr bool j_fast = true;
+    __device__ __forceinline__ float operator()(int n, int c) const {
+        const float *q = pre + (long long)n * 2 * C;
+        return gate(__ldg(q + c), __ldg(q + c + C));
+    }
+};
+
+// a forward packing [tap][ci][co] (vqb_prior_pack_f32) as the dgrad operand (tap*Cout + co) x ci
+struct WPacked {
+    const float *p;
+    int Cin, Cout;
+    static constexpr bool j_fast = false;
+    __device__ __forceinline__ float operator()(int k, int ci) const {
+        const int tap = k / Cout, co = k - tap * Cout;
+        return __ldg(p + ((long long)tap * Cin + ci) * Cout + co);
+    }
+};
+
+struct OneHot {                   // (m, n) -> 1 if the clamped index of position n is m: idx[n / per]
+    const long long *idx;
+    int per, count;
+    static constexpr bool j_fast = true;
+    __device__ __forceinline__ float operator()(int m, int n) const { return clampi(idx[n / per], count) == m ? 1.f : 0.f; }
+};
+
+template <class L>
+struct WithOnes {                 // column `cols` of ones after the columns of b: the bias gradient's column
+    L b;
+    int cols;
+    static constexpr bool j_fast = L::j_fast;
+    __device__ __forceinline__ float operator()(int k, int n) const { return n < cols ? b(k, n) : 1.f; }
+};
+
+// ---- epilogues: (m, n, value) -----------------------------------------------------------------------------------
+struct Store {                    // out[m][n] = v (+ add[m][n])
+    float *out;
+    const float *add;
+    int ld;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        const long long i = (long long)m * ld + n;
+        out[i] = add ? v + add[i] : v;
+    }
+};
+
+struct ReluBack {                 // d_hidden = relu'(hidden) * v
+    float *out;
+    const float *hid;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        const long long i = (long long)m * HID + n;
+        out[i] = __ldg(hid + i) > 0.f ? v : 0.f;
+    }
+};
+
+// d(tanh(a) * sigmoid(g)) by a and by g, times d
+__device__ __forceinline__ void gate_back(float a, float g, float d, float &da, float &dg) {
+    const float t = tanhf(a), s = 1.f / (1.f + expf(-g));
+    da = d * (1.f - t * t) * s;
+    dg = d * t * s * (1.f - s);
+}
+
+struct GateBack {                 // v = d out[m][c] of the horizontal gate -> d pre_h[m][c], d pre_h[m][c + C]
+    float *dpre;
+    const float *pre;
+    int C;
+    __device__ __forceinline__ void operator()(int m, int c, float v) const {
+        const long long i = (long long)m * 2 * C + c;
+        float da, dg;
+        gate_back(__ldg(pre + i), __ldg(pre + i + C), v, da, dg);
+        dpre[i] = da;
+        dpre[i + C] = dg;
+    }
+};
+
+// v = (W_v2h^T d pre_h)[m][c]: d h_vert = v + d pre_v, with d pre_v = gate'(h_vert + class) * d x_v of the next layer
+// (gv == nullptr: the last layer, whose vertical output nothing reads).  Also writes cls = d pre_v + d pre_h, the
+// per-position gradient of the class embedding, which enters both gates.
+struct VertBack {
+    float *dhv, *cls;
+    const float *hv, *gv, *dph, *emb;
+    const long long *labels;
+    int C, HW, NC;
+    __device__ __forceinline__ void operator()(int m, int c, float v) const {
+        const long long i = (long long)m * 2 * C + c;
+        float dpv = 0.f;
+        if (gv) {
+            const int c0 = c < C ? c : c - C;
+            const float *e = emb + (long long)clampi(labels[m / HW], NC) * 2 * C;
+            const long long i0 = (long long)m * 2 * C + c0;
+            float da, dg;
+            gate_back(__ldg(hv + i0) + __ldg(e + c0), __ldg(hv + i0 + C) + __ldg(e + c0 + C),
+                      __ldg(gv + (long long)m * C + c0), da, dg);
+            dpv = c < C ? da : dg;
+        }
+        dhv[i] = v + dpv;
+        cls[i] = dpv + __ldg(dph + i);
+    }
+};
+
+struct Partial {                  // wgrad: chunk z's partial of element (m, n) of an (M x cols) gradient
+    float *part;
+    long long M, cols;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        part[(long long)blockIdx.z * M * cols + (long long)m * cols + n] = v;
+    }
+};
+
+// ---- the GEMM: out(m, n) = sum over k in [z*chunk, min(K, (z+1)*chunk)) of A(m, k) * B(k, n), k ascending ----------
+template <class LA, class LB, class EP>
+__global__ void __launch_bounds__(GT) gemm_kernel(LA a, LB b, EP ep, int M, int N, int K, int chunk) {
+    __shared__ __align__(16) float As[BK][BM + 4];
+    __shared__ __align__(16) float Bs[BK][BN + 4];
+    const int tid = threadIdx.x, tm = tid / 16, tn = tid % 16;
+    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
+    const int k_begin = blockIdx.z * chunk, k_end = min(K, k_begin + chunk);
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int k0 = k_begin; k0 < k_end; k0 += BK) {
+#pragma unroll
+        for (int q = 0; q < BM * BK / GT; ++q) {
+            const int e = tid + q * GT;
+            const int mm = LA::j_fast ? e / BK : e % BM, kk = LA::j_fast ? e % BK : e / BM;
+            const int m = m0 + mm, k = k0 + kk;
+            As[kk][mm] = (m < M && k < k_end) ? a(m, k) : 0.f;
+        }
+#pragma unroll
+        for (int q = 0; q < BN * BK / GT; ++q) {
+            const int e = tid + q * GT;
+            const int nn = LB::j_fast ? e % BN : e / BK, kk = LB::j_fast ? e / BN : e % BK;
+            const int n = n0 + nn, k = k0 + kk;
+            Bs[kk][nn] = (n < N && k < k_end) ? b(k, n) : 0.f;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kk = 0; kk < BK; ++kk) {
+            const float4 av = *reinterpret_cast<const float4 *>(&As[kk][tm * 4]);
+            const float4 bv = *reinterpret_cast<const float4 *>(&Bs[kk][tn * 4]);
+            const float ar[4] = {av.x, av.y, av.z, av.w}, br[4] = {bv.x, bv.y, bv.z, bv.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(ar[i], br[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int m = m0 + tm * 4 + i, n = n0 + tn * 4 + j;
+            if (m < M && n < N) ep(m, n, acc[i][j]);
+        }
+}
+
+// ---- split-K reduction of the wgrad partials, into the parameters' layouts --------------------------------------
+// Job: partials [splits][M][cols] with cols = taps*Cin (+1 for the bias); column tap*Cin + ci -> w[m][ci][tap]
+// (the (Cout, Cin, kh, kw) layout with tap = r*kw + s), the ones column -> bias[m].
+struct RJob {
+    const float *part;
+    float *w, *bias;
+    int M, Cin, taps, cols, splits;
+};
+constexpr int MAX_JOBS = 5;
+struct RJobs {
+    RJob j[MAX_JOBS];
+};
+
+__global__ void reduce_kernel(RJobs jobs) {
+    const RJob J = jobs.j[blockIdx.y];
+    const long long total = (long long)J.M * J.cols, stride = total;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        float v = 0.f;
+        for (int z = 0; z < J.splits; ++z) v += J.part[z * stride + i];
+        const int m = (int)(i / J.cols), j = (int)(i % J.cols);
+        if (j >= J.taps * J.Cin) {
+            J.bias[m] = v;
+        } else {
+            const int tap = j / J.Cin, ci = j % J.Cin;
+            J.w[((long long)m * J.Cin + ci) * J.taps + tap] = v;
+        }
+    }
+}
+
+// ---- host side ---------------------------------------------------------------------------------------------------
+int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+struct Split {                    // wgrad reduction over K positions: `splits` chunks of `chunk` positions
+    int splits, chunk;
+};
+
+Split wsplit(int M, int N, long long K) {
+    const long long tiles = (long long)cdiv(M, BM) * cdiv(N, BN);
+    long long s = cdiv(2 * 132, tiles);                      // about two CTAs per SM
+    s = s > cdiv(K, WG_CHUNK) ? s : cdiv(K, WG_CHUNK);       // and short fmaf chains
+    s = s < cdiv(K, BK) ? s : cdiv(K, BK);
+    const int chunk = cdiv(cdiv(K, s), BK) * BK;
+    return {cdiv(K, chunk), chunk};
+}
+
+template <class LA, class LB, class EP>
+void gemm(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K, Split sp) {
+    const dim3 grid(cdiv(M, BM), cdiv(N, BN), sp.splits);
+    gemm_kernel<LA, LB, EP><<<grid, GT, 0, st>>>(a, b, ep, M, N, K, sp.chunk);
+}
+
+template <class LA, class LB, class EP>
+void dgrad(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K) { gemm(st, a, b, ep, M, N, K, Split{1, K}); }
+
+// A wgrad job in the partial region: M x cols partials of a reduction over `npos` positions, at `off` floats.
+struct WJob {
+    int M, Cin, taps;
+    bool bias;
+    Split sp;
+    long long off;
+    int cols() const { return Cin * taps + (bias ? 1 : 0); }
+    long long floats() const { return (long long)sp.splits * M * cols(); }
+};
+
+// The wgrad jobs of one phase, laid out one after the other.
+struct Phase {
+    WJob job[MAX_JOBS];
+    int n = 0;
+    long long floats = 0;
+    WJob &add(int M, int Cin, int taps, bool bias, long long npos) {
+        WJob &j = job[n++];
+        j.M = M; j.Cin = Cin; j.taps = taps; j.bias = bias;
+        j.sp = wsplit(M, j.cols(), npos);
+        j.off = floats;
+        floats += j.floats();
+        return j;
+    }
+};
+
+int vrows(const vqb_prior_layer_weights &w) { return w.kernel / 2 + 1; }     // vert_stack (k/2 + 1, k)
+int hcols(const vqb_prior_layer_weights &w) { return w.kernel / 2 + 1; }     // horiz_stack (1, k/2 + 1)
+
+// the wgrad jobs of the head (dW2, dW1), of layer l (resid, horiz, v2h, class, vert) and of the embedding
+Phase head_phase(const Net &n, long long npos) {
+    Phase p;
+    p.add(n.K, HID, 1, true, npos);
+    p.add(HID, n.C, 1, true, npos);
+    return p;
+}
+
+Phase layer_phase(const Net &n, int l, long long npos) {
+    const vqb_prior_layer_weights &w = n.layer[l];
+    const int C = n.C;
+    Phase p;
+    p.add(C, C, 1, true, npos);
+    p.add(2 * C, C, hcols(w), true, npos);
+    p.add(2 * C, 2 * C, 1, true, npos);
+    p.add(n.NC, 2 * C, 1, false, npos);
+    p.add(2 * C, C, vrows(w) * w.kernel, true, npos);
+    return p;
+}
+
+Phase emb_phase(const Net &n, long long npos) {
+    Phase p;
+    p.add(n.K, n.C, 1, false, npos);
+    return p;
+}
+
+// workspace regions, in floats: d x_h (2 grids), d x_v (2 grids), the head's d_hidden or a layer's d pre_h, d h_vert
+// and class gradient (union), then the wgrad partials of the largest phase
+struct Bws {
+    long long gh, gv, work, part, total;
+};
+
+Bws bws_layout(const Net &n, long long npos) {
+    Bws w;
+    const long long grid = npos * n.C;
+    w.gh = 0;
+    w.gv = 2 * grid;
+    w.work = 4 * grid;
+    const long long head = npos * HID, layer = 6 * grid;
+    w.part = w.work + (head > layer ? head : layer);
+    long long part = head_phase(n, npos).floats;
+    const long long e = emb_phase(n, npos).floats;
+    part = part > e ? part : e;
+    for (int l = 0; l < n.L; ++l) {
+        const long long f = layer_phase(n, l, npos).floats;
+        part = part > f ? part : f;
+    }
+    w.total = w.part + part;
+    return w;
+}
+
+void reduce(cudaStream_t st, const Phase &p, float *part, float *const (&w)[MAX_JOBS], float *const (&b)[MAX_JOBS]) {
+    RJobs jobs;
+    long long most = 0;
+    for (int i = 0; i < p.n; ++i) {
+        const WJob &j = p.job[i];
+        jobs.j[i] = RJob{part + j.off, w[i], b[i], j.M, j.Cin, j.taps, j.cols(), j.sp.splits};
+        most = most > (long long)j.M * j.cols() ? most : (long long)j.M * j.cols();
+    }
+    reduce_kernel<<<dim3(cdiv(most, NT) < 1024 ? cdiv(most, NT) : 1024, p.n), NT, 0, st>>>(jobs);
+}
+
+bool grads_ok(const vqb_prior_grads *g, int L) {
+    if (!g || !g->layers || g->n_layers != L || !g->embedding || !g->out1_w || !g->out1_b || !g->out2_w || !g->out2_b)
+        return false;
+    for (int l = 0; l < L; ++l) {
+        const vqb_prior_layer_grads &q = g->layers[l];
+        if (!q.vert_w || !q.vert_b || !q.v2h_w || !q.v2h_b || !q.horiz_w || !q.horiz_b || !q.resid_w || !q.resid_b ||
+            !q.class_emb)
+            return false;
+    }
+    return true;
+}
+
+}  // namespace
+
+extern "C" size_t vqb_prior_backward_workspace_bytes(const vqb_prior_net *net, int B, int H, int W) {
+    Net n;
+    if (net_from(net, n) || B <= 0 || H <= 0 || W <= 0) return 0;
+    return (size_t)bws_layout(n, (long long)B * H * W).total * sizeof(float);
+}
+
+extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                      int H, int W, const float *d_logits, const void *saved,
+                                      const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
+                                      void *stream) {
+    Net n;
+    const int st_ = net_from(net, n);
+    if (st_) return st_;
+    if (!codes || !labels || !d_logits || !saved || !workspace || B <= 0 || H <= 0 || W <= 0 || !grads_ok(grads, n.L))
+        return VQB_ERR_BAD_ARG;
+    if (workspace_bytes < vqb_prior_backward_workspace_bytes(net, B, H, W)) return VQB_ERR_WORKSPACE;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int npos = B * H * W, C = n.C, C2 = 2 * C, K = n.K;
+    const long long grid = (long long)npos * C;
+    const long long *lab = reinterpret_cast<const long long *>(labels);
+    const Saved sv{npos, C, n.L};
+    const float *sp = static_cast<const float *>(saved);
+    float *ws = static_cast<float *>(workspace);
+    const Bws wl = bws_layout(n, npos);
+    float *gh[2] = {ws + wl.gh, ws + wl.gh + grid}, *gv[2] = {ws + wl.gv, ws + wl.gv + grid};
+    float *part = ws + wl.part;
+    const Grid g{H, W};
+    unsigned long long launches = 0;
+
+    // head: d_hidden = relu' * (W2^T d_logits); dW2, db2; dW1, db1; d x_h^L = W1^T d_hidden
+    {
+        float *dhid = ws + wl.work;
+        const float *hid = sp + sv.hid(), *xL = sp + sv.xh(n.L);
+        const Nchw dl{d_logits, K, H * W};
+        dgrad(st, dl, WPacked{n.w2, HID, K}, ReluBack{dhid, hid}, npos, HID, K);
+        const Phase p = head_phase(n, npos);
+        gemm(st, NchwT{dl}, WithOnes<Mat>{Mat{hid, HID}, HID}, Partial{part + p.job[0].off, K, HID + 1}, K, HID + 1,
+             npos, p.job[0].sp);
+        gemm(st, MatT{dhid, HID}, WithOnes<Mat>{Mat{xL, C}, C}, Partial{part + p.job[1].off, HID, C + 1}, HID, C + 1,
+             npos, p.job[1].sp);
+        dgrad(st, Mat{dhid, HID}, WPacked{n.w1, C, HID}, Store{gh[0], nullptr, C}, npos, C, HID);
+        reduce(st, p, part, {grads->out2_w, grads->out1_w}, {grads->out2_b, grads->out1_b});
+        launches += 5;
+    }
+    // layers, last to first.  gh[cur] = d x_h^{l+1}, gv[cur] = d x_v^{l+1} (none for the last layer)
+    int cur = 0;
+    for (int l = n.L - 1; l >= 0; --l) {
+        const vqb_prior_layer_weights &w = n.layer[l];
+        const vqb_prior_layer_grads &q = grads->layers[l];
+        const int half = w.kernel / 2, vr = vrows(w) - (w.mask_a ? 1 : 0), hc = hcols(w) - (w.mask_a ? 1 : 0);
+        float *dph = ws + wl.work, *dhv = dph + 2 * grid, *cls = dhv + 2 * grid;
+        const float *ph = sp + sv.ph(l), *hv = sp + sv.hv(l), *xv = sp + sv.xv(l), *xh = sp + sv.xh(l);
+        const float *ghi = gh[cur], *gvi = l == n.L - 1 ? nullptr : gv[cur];
+        float *gho = gh[cur ^ 1], *gvo = gv[cur ^ 1];
+        const Phase p = layer_phase(n, l, npos);
+        // out_h = horiz_resid(gate(pre_h)) [+ x_h]: d pre_h, then d x_h = [d out_h +] horiz_stack^T * d pre_h
+        dgrad(st, Mat{ghi, C}, WPacked{w.resid_w, C, C}, GateBack{dph, ph, C}, npos, C, C);
+        gemm(st, MatT{ghi, C}, WithOnes<Gated>{Gated{ph, C}, C}, Partial{part + p.job[0].off, C, C + 1}, C, C + 1,
+             npos, p.job[0].sp);
+        dgrad(st, Tap{dph, C2, hc, 0, half, -1, g}, WPacked{w.horiz_w, C, C2}, Store{gho, w.residual ? ghi : nullptr, C},
+              npos, C, hc * C2);
+        gemm(st, MatT{dph, C2}, WithOnes<Tap>{Tap{xh, C, hcols(w), 0, half, 1, g}, hcols(w) * C},
+             Partial{part + p.job[1].off, C2, p.job[1].cols()}, C2, p.job[1].cols(), npos, p.job[1].sp);
+        gemm(st, MatT{dph, C2}, WithOnes<Mat>{Mat{hv, C2}, C2}, Partial{part + p.job[2].off, C2, C2 + 1}, C2, C2 + 1,
+             npos, p.job[2].sp);
+        // d h_vert = W_v2h^T d pre_h + gate'(h_vert + class) * d x_v^{l+1}; class gradient; d x_v = vert_stack^T * d h_vert
+        dgrad(st, Mat{dph, C2}, WPacked{w.v2h_w, C2, C2},
+              VertBack{dhv, cls, hv, gvi, dph, w.class_emb, lab, C, H * W, n.NC}, npos, C2, C2);
+        gemm(st, OneHot{lab, H * W, n.NC}, Mat{cls, C2}, Partial{part + p.job[3].off, n.NC, C2}, n.NC, C2, npos,
+             p.job[3].sp);
+        gemm(st, MatT{dhv, C2}, WithOnes<Tap>{Tap{xv, C, w.kernel, half, half, 1, g}, vrows(w) * w.kernel * C},
+             Partial{part + p.job[4].off, C2, p.job[4].cols()}, C2, p.job[4].cols(), npos, p.job[4].sp);
+        // layer 0: x_v and x_h are both the embedding, so d x_v^0 + d x_h^0 is its gradient per position
+        dgrad(st, Tap{dhv, C2, w.kernel, half, half, -1, g}, WPacked{w.vert_w, C, C2},
+              Store{gvo, l == 0 ? gho : nullptr, C}, npos, C, vr * w.kernel * C2);
+        reduce(st, p, part, {q.resid_w, q.horiz_w, q.v2h_w, q.class_emb, q.vert_w},
+               {q.resid_b, q.horiz_b, q.v2h_b, nullptr, q.vert_b});
+        launches += 10;
+        cur ^= 1;
+    }
+    // embedding: the per-position gradient summed by (clamped) code
+    {
+        const Phase p = emb_phase(n, npos);
+        gemm(st, OneHot{reinterpret_cast<const long long *>(codes), 1, K}, Mat{gv[cur], C},
+             Partial{part + p.job[0].off, K, C}, K, C, npos, p.job[0].sp);
+        reduce(st, p, part, {grads->embedding}, {nullptr});
+        launches += 2;
+    }
+    VQB_COUNT_LAUNCH(launches);
+    return vqb_cuda_status(cudaGetLastError());
+}

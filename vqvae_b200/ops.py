@@ -413,3 +413,36 @@ def prior_generate(net, labels, u, step_logits=None):
                                        ws.numel(), _stream()), "prior_generate")
     span.done()
     return codes
+
+
+def prior_forward_train(net, codes, labels):
+    """prior_forward that also keeps the activations the backward needs: (logits, saved) with saved a uint8 buffer
+    of vqb_prior_train_saved_bytes (vqb_prior_forward_train_f32; the logits are bitwise prior_forward's)."""
+    B, H, W = codes.shape
+    dev = codes.device
+    n = lib().vqb_prior_train_saved_bytes(B, H, W, net.dim, net.n_layers)
+    if n == 0:
+        raise RuntimeError("prior: bad sizes")
+    saved = torch.empty((n,), dtype=torch.uint8, device=dev)
+    logits = torch.empty((B, net.input_dim, H, W), dtype=torch.float32, device=dev)
+    span = _Span(f"prior forward (train) K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(lib().vqb_prior_forward_train_f32(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W,
+                                            logits.data_ptr(), saved.data_ptr(), saved.numel(), _stream()),
+          "prior_forward_train")
+    span.done()
+    return logits, saved
+
+
+def prior_backward(net, codes, labels, d_logits, saved, grads):
+    """Every parameter gradient of the prior (vqb_prior_backward_f32) into the tensors `grads` (a PriorGrads struct)
+    points at; d_logits (B, K, H, W) fp32 contiguous, saved from prior_forward_train on the same net and inputs."""
+    B, H, W = codes.shape
+    n = lib().vqb_prior_backward_workspace_bytes(_lib.C.byref(net), B, H, W)
+    if n == 0:
+        raise RuntimeError("prior backward: bad sizes")
+    ws = torch.empty((n,), dtype=torch.uint8, device=codes.device)
+    span = _Span(f"prior backward K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(lib().vqb_prior_backward_f32(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W,
+                                       d_logits.data_ptr(), saved.data_ptr(), _lib.C.byref(grads), ws.data_ptr(),
+                                       ws.numel(), _stream()), "prior_backward")
+    span.done()

@@ -1,10 +1,16 @@
-"""Host-side mirror of the reference's Gated PixelCNN prior (``pixelcnn/models.py``), inference only.
+"""Host-side mirror of the reference's Gated PixelCNN prior (``pixelcnn/models.py``), trainable.
 
 Same class names, constructor signatures, attribute names and state-dict keys as the reference, so a state dict saved
 by its ``gated_pixelcnn.py`` loads unchanged and ``from pixelcnn.models import GatedPixelCNN`` (the top-level
 ``pixelcnn`` package re-exports these classes) drops in.  As in ``modules.py`` the nn.Conv2d / nn.Embedding children
 are parameter containers only: every forward runs the sm_90a kernels of ``csrc/prior.cu`` through the C ABI, in fp32
-whatever ``set_precision`` says.  Outputs carry no autograd graph.
+whatever ``set_precision`` says.
+
+``GatedPixelCNN.forward`` is differentiable with respect to every parameter when grad is enabled and a parameter
+requires grad (``_PriorFunction``: the training forward keeps its activations, and the backward of
+``csrc/prior_bwd.cu`` writes one gradient per parameter), so the reference's training loop runs unchanged.  Under
+``torch.no_grad()`` it is the inference forward.  ``GatedMaskedConv2d`` and ``GatedActivation`` called on their own
+are inference only: their outputs carry no autograd graph.
 
 Reference behaviour kept on purpose:
   P2  ``self.apply(weights_init)``: Xavier-uniform conv weights, zero biases, and one "Skipping initialization of"
@@ -19,7 +25,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from ._lib import PriorLayerWeights, PriorNet
+from ._lib import C, PriorGrads, PriorLayerGrads, PriorLayerWeights, PriorNet
 from .modules import _packed, _packed_current
 
 HIDDEN = 512          # output_conv's hidden width
@@ -60,14 +66,16 @@ def _labels(label, B, dev, what):
 
 
 class GatedActivation(nn.Module):
-    """tanh(first half of the channels) * sigmoid(second half) (models.py:20-26)."""
+    """tanh(first half of the channels) * sigmoid(second half) (models.py:20-26).  Inference only: the output carries
+    no autograd graph (GatedPixelCNN.forward is the differentiable entry point)."""
 
     def forward(self, x):
         return ops.prior_gate(x)
 
 
 class GatedMaskedConv2d(nn.Module):
-    """One gated layer with a vertical and a horizontal stack (models.py:29-86)."""
+    """One gated layer with a vertical and a horizontal stack (models.py:29-86).  Called on its own it is inference
+    only: the outputs carry no autograd graph (GatedPixelCNN.forward is the differentiable entry point)."""
 
     def __init__(self, mask_type, dim, kernel, residual=True, n_classes=10):
         super().__init__()
@@ -123,6 +131,47 @@ class GatedMaskedConv2d(nn.Module):
         return ops.nhwc_to_nchw(out_v), ops.nhwc_to_nchw(out_h)
 
 
+# PriorLayerGrads / PriorGrads field -> parameter name (within a layer / the model)
+_LAYER_GRADS = dict(vert_w="vert_stack.weight", vert_b="vert_stack.bias", v2h_w="vert_to_horiz.weight",
+                    v2h_b="vert_to_horiz.bias", horiz_w="horiz_stack.weight", horiz_b="horiz_stack.bias",
+                    resid_w="horiz_resid.weight", resid_b="horiz_resid.bias", class_emb="class_cond_embedding.weight")
+_NET_GRADS = dict(embedding="embedding.weight", out1_w="output_conv.0.weight", out1_b="output_conv.0.bias",
+                  out2_w="output_conv.2.weight", out2_b="output_conv.2.bias")
+
+
+class _PriorFunction(torch.autograd.Function):
+    """GatedPixelCNN.forward with gradients: inputs are the model, codes, labels and every parameter in
+    ``parameters()`` order.  The forward keeps the activations vqb_prior_backward_f32 reads; the backward returns one
+    gradient per parameter in its shape and dtype, mask A's taps included (the reference's autograd gives them one)."""
+
+    @staticmethod
+    def forward(ctx, model, codes, labels, *params):
+        keep = []
+        net = model._net(keep)
+        logits, saved = ops.prior_forward_train(net, codes, labels)
+        ctx.model, ctx.net, ctx.keep, ctx.saved = model, net, keep, saved
+        ctx.save_for_backward(codes, labels)
+        return logits
+
+    @staticmethod
+    def backward(ctx, d_logits):
+        if ctx.saved is None:           # the first backward freed the saved activations
+            raise RuntimeError("GatedPixelCNN: backward through the same forward twice is not supported "
+                               "(its saved activations are freed by the first backward)")
+        codes, labels = ctx.saved_tensors
+        params = dict(ctx.model.named_parameters())
+        grads = {k: torch.empty(p.shape, dtype=torch.float32, device=codes.device) for k, p in params.items()}
+        n_layers = len(ctx.model.layers)
+        layers = (PriorLayerGrads * n_layers)(*[
+            PriorLayerGrads(**{f: grads[f"layers.{i}.{k}"].data_ptr() for f, k in _LAYER_GRADS.items()})
+            for i in range(n_layers)])
+        table = PriorGrads(layers=C.cast(layers, C.POINTER(PriorLayerGrads)), n_layers=n_layers,
+                           **{f: grads[k].data_ptr() for f, k in _NET_GRADS.items()})
+        ops.prior_backward(ctx.net, codes, labels, _f32(d_logits), ctx.saved, table)
+        ctx.saved = ctx.keep = None
+        return (None, None, None) + tuple(grads[k].to(p.dtype) for k, p in params.items())
+
+
 class GatedPixelCNN(nn.Module):
     """Prior over code grids (models.py:89-143): layer 0 is a mask-A 7x7 layer without residual, the others mask-B
     3x3 layers with residual, then a 1x1 -> ReLU -> 1x1 head to input_dim logits."""
@@ -155,15 +204,19 @@ class GatedPixelCNN(nn.Module):
                         **{k: v.data_ptr() for k, v in t.items()})
 
     def forward(self, x, label):
-        """int64 codes (B,H,W) and labels (B,) -> fp32 logits (B, input_dim, H, W)."""
+        """int64 codes (B,H,W) and labels (B,) -> fp32 logits (B, input_dim, H, W).  Differentiable with respect to
+        the parameters when grad is enabled and any parameter requires grad."""
         if x.dim() != 3:
             raise RuntimeError(f"GatedPixelCNN: expected codes of shape (B,H,W), got {tuple(x.shape)}")
         B, H, W = x.shape
         _square(H, W, "GatedPixelCNN")
         ops._require_cuda(x, "GatedPixelCNN codes")
         label = _labels(label, B, x.device, "GatedPixelCNN")
+        x = x.detach().to(torch.int64).contiguous()
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            return _PriorFunction.apply(self, x, label, *self.parameters())
         keep = []
-        return ops.prior_forward(self._net(keep), x.detach().to(torch.int64).contiguous(), label)
+        return ops.prior_forward(self._net(keep), x, label)
 
     def _sample(self, label, u, step_logits=None):
         """generate() with given uniforms u (B,H,W) fp32: the code at (b,i,j) is the smallest k with u < CDF_k."""
