@@ -309,6 +309,9 @@ int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *codes, const 
  * u[b,i,j] < CDF_k, CDF the fp32 running sum of the softmax of the logits at (i,j) (DESIGN.md gives the order).
  * u: (B,H,W) uniforms in [0,1).  H*(n_layers + W) launches: per row one vertical-stack pass per layer, then one
  * launch per position running every layer's horizontal stack, the head and the draw.  No host synchronisation.
+ * The workspace keeps min(H, VQB_PRIOR_MAX_KERNEL/2 + 1) rows of each layer's vertical output, the most a later
+ * layer reads (a layer with kernel k reads k/2 + 1 rows of the previous one's).  Layer 0 must be mask A without residual (anything else reads the code being drawn, so the logits are not
+ * causal in raster order): VQB_ERR_UNSUPPORTED before any launch otherwise.
  * step_logits: NULL, or (B,H,W,input_dim) fp32 receiving the logits each step sampled from -- bitwise equal to
  * vqb_prior_forward_f32's logits on the returned codes.                                                    */
 int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, int B, int H, int W,

@@ -4,7 +4,9 @@ TEST INFRASTRUCTURE ONLY.  Run from the repository root where a checkout of the 
 (``python -m oracle.make_prior_golden [--ref DIR] [prior_... ...]``; only the named cases are regenerated, so the
 other fixtures stay byte-identical).  The reference is imported in a subprocess with cwd = the reference root and
 CUDA hidden.  Weights and inputs are not stored: tests regenerate them from the seeds in
-oracle.prior_port.PRIOR_CASES, so each fixture holds the reference's outputs only.
+oracle.prior_port.PRIOR_CASES, so each fixture holds the reference's outputs only.  prior_layers.npz is the
+PRIOR_SHAPE_CASES["kernels"] stack: the reference's GatedPixelCNN with each of its layers replaced by the reference's
+own GatedMaskedConv2d(mask_type, dim, kernel, residual, n_classes).
 """
 import argparse
 import json
@@ -16,16 +18,17 @@ import tempfile
 import numpy as np
 
 from .build import REF_SRC
-from .prior_port import PRIOR_CASES, make_prior_inputs, make_prior_state_dict
+from .prior_port import PRIOR_CASES, PRIOR_SHAPE_CASES, make_prior_inputs, make_prior_state_dict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 OUT = os.path.join(ROOT, "tests", "golden")
+LAYER_FIXTURES = {"prior_layers": "kernels"}          # fixture -> PRIOR_SHAPE_CASES entry
 
 _SCRIPT = r"""
 import sys, json, hashlib, numpy as np, torch
 sys.path.insert(0, %(ref)r)
-from pixelcnn.models import GatedPixelCNN
+from pixelcnn.models import GatedMaskedConv2d, GatedPixelCNN
 torch.set_num_threads(1)
 job = json.load(open(sys.argv[1]))
 if job["kind"] == "fingerprint":
@@ -40,6 +43,8 @@ else:
     c = job["case"]
     data = np.load(job["in"])
     m = GatedPixelCNN(c["K"], c["dim"], c["n_layers"], c["n_classes"]).eval()
+    for i, (mask, k, residual) in enumerate(c.get("layers", [])):
+        m.layers[i] = GatedMaskedConv2d(mask, c["dim"], k, residual, c["n_classes"])
     m.load_state_dict({k: torch.from_numpy(data[k]) for k in m.state_dict().keys()})
     with torch.no_grad():
         logits = m(torch.from_numpy(data["__codes"]), torch.from_numpy(data["__labels"]))
@@ -72,10 +77,11 @@ def main():
                    for n in ("prior_default", "prior_ragged")}
         _run(a.ref, dict(kind="fingerprint", configs=configs, out=os.path.join(OUT, "prior_init_fingerprint.json")))
         print("prior_init_fingerprint.json")
-    for name, c in PRIOR_CASES.items():
+    cases = list(PRIOR_CASES.items()) + [(f, PRIOR_SHAPE_CASES[n]) for f, n in LAYER_FIXTURES.items()]
+    for name, c in cases:
         if only and name not in only:
             continue
-        sd = make_prior_state_dict(c["K"], c["dim"], c["n_layers"], c["n_classes"], c["wseed"])
+        sd = make_prior_state_dict(c["K"], c["dim"], c["n_layers"], c["n_classes"], c["wseed"], c.get("layers"))
         codes, labels, pos = make_prior_inputs(c)
         arrays = dict(sd, __codes=codes, __labels=labels)
         if pos is not None:

@@ -20,14 +20,58 @@ PRIOR_CASES = {
                        positions=64),
 }
 
+A7, B3 = ["A", 7, False], ["B", 3, True]
+
+# Cases over the documented shape range with their own layer stacks: `layers` lists (mask_type, kernel, residual)
+# per layer, and the model is GatedPixelCNN(K, dim, n_layers, n_classes) with layers[i] replaced by
+# GatedMaskedConv2d(mask_type, dim, kernel, residual, n_classes).  `parts` says what the GPU tests run on a case.
+PRIOR_SHAPE_CASES = {
+    # 2*dim = 512: both accumulators of every thread live; K = 8192: 256 codes per lane in the draw
+    "wide": dict(K=8192, dim=256, n_layers=2, n_classes=10, size=6, batch=3, wseed=40, xseed=41, layers=[A7, B3]),
+    # 2*dim = 320: the second accumulator partly live; K = 33: lanes 17..31 of the draw empty; 65 classes: 2 row tiles
+    "mid": dict(K=33, dim=160, n_layers=3, n_classes=65, size=7, batch=5, wseed=42, xseed=43, layers=[A7, B3, B3]),
+    # 2*dim = 192: ragged GEMM tiles; one class
+    "narrow": dict(K=2, dim=96, n_layers=4, n_classes=1, size=4, batch=9, wseed=44, xseed=45,
+                   layers=[A7, B3, B3, B3]),
+    # every kernel path, mask A after layer 0 (kernel 1: no kept taps), a mask-B 15 reading 8 vertical rows of 9
+    "kernels": dict(K=37, dim=32, n_layers=7, n_classes=3, size=9, batch=2, wseed=46, xseed=47,
+                    layers=[["A", 15, False], ["B", 5, True], ["B", 1, True], ["A", 3, True], ["A", 1, True],
+                            ["B", 15, False], B3]),
+    # VQB_PRIOR_MAX_LAYERS layers
+    "deep": dict(K=16, dim=32, n_layers=32, n_classes=10, size=6, batch=2, wseed=48, xseed=49,
+                 layers=[A7] + [B3] * 31),
+    "single": dict(K=1, dim=32, n_layers=1, n_classes=10, size=1, batch=1, wseed=50, xseed=51, layers=[A7]),
+    "single3": dict(K=1, dim=32, n_layers=1, n_classes=10, size=3, batch=1, wseed=52, xseed=53, layers=[A7]),
+    # 4608 positions: weight gradients over many chunks; 48 sampler rows
+    "long": dict(K=512, dim=32, n_layers=2, n_classes=10, size=48, batch=2, wseed=54, xseed=55, layers=[A7, B3]),
+    # residual on layer 0 (teacher-forced only: the sampler refuses it)
+    "resid0": dict(K=37, dim=32, n_layers=2, n_classes=3, size=5, batch=2, wseed=56, xseed=57,
+                   layers=[["A", 5, True], B3], parts=["forward", "backward"]),
+    # the cfg3 latent with the reference's stack: the sampler's vertical rings over 64 rows
+    "cfg3_sampler": dict(K=1024, dim=64, n_layers=15, n_classes=10, size=64, batch=2, wseed=58, xseed=59,
+                         layers=[A7] + [B3] * 14, parts=["sampler"]),
+}
+
 HIDDEN = 512
 
 
-def prior_shapes(K, dim, n_layers, n_classes):
-    """(key, shape) of every tensor of GatedPixelCNN(K, dim, n_layers, n_classes).state_dict(), in order."""
+def reference_layers(n_layers):
+    """(mask_type, kernel, residual) of every layer of the reference's GatedPixelCNN: mask A 7x7 without residual,
+    then mask B 3x3 with residual."""
+    return [A7] + [B3] * (n_layers - 1)
+
+
+def _stack(n_layers, layers):
+    layers = reference_layers(n_layers) if layers is None else [list(l) for l in layers]
+    assert len(layers) == n_layers, (len(layers), n_layers)
+    return layers
+
+
+def prior_shapes(K, dim, n_layers, n_classes, layers=None):
+    """(key, shape) of every tensor of GatedPixelCNN(K, dim, n_layers, n_classes).state_dict(), in order, with the
+    layer stack `layers` ((mask_type, kernel, residual) per layer; default the reference's)."""
     out = [("embedding.weight", (K, dim))]
-    for i in range(n_layers):
-        k = 7 if i == 0 else 3
+    for i, (_, k, _) in enumerate(_stack(n_layers, layers)):
         p = f"layers.{i}."
         out += [(p + "class_cond_embedding.weight", (n_classes, 2 * dim)),
                 (p + "vert_stack.weight", (2 * dim, dim, k // 2 + 1, k)), (p + "vert_stack.bias", (2 * dim,)),
@@ -39,12 +83,12 @@ def prior_shapes(K, dim, n_layers, n_classes):
     return out
 
 
-def make_prior_state_dict(K, dim, n_layers, n_classes, seed):
+def make_prior_state_dict(K, dim, n_layers, n_classes, seed, layers=None):
     """Seeded float32 weights: Xavier-range conv weights (mask A's taps deliberately non-zero), small random biases,
     unit-normal embeddings."""
     rng = np.random.RandomState(seed)
     sd = {}
-    for key, shape in prior_shapes(K, dim, n_layers, n_classes):
+    for key, shape in prior_shapes(K, dim, n_layers, n_classes, layers):
         if key.endswith("bias"):
             v = rng.uniform(-0.1, 0.1, size=shape)
         elif len(shape) == 4:
@@ -76,17 +120,17 @@ def _gate(t):
 
 
 @torch.no_grad()
-def prior_forward(sd, x, label, n_layers, dtype=torch.float32):
-    """Logits (B, K, H, W) of codes x (B,H,W) int64 and labels (B,) int64; sd maps keys to tensors or arrays."""
+def prior_forward(sd, x, label, n_layers, dtype=torch.float32, layers=None):
+    """Logits (B, K, H, W) of codes x (B,H,W) int64 and labels (B,) int64; sd maps keys to tensors or arrays;
+    layers: (mask_type, kernel, residual) per layer, default the reference's stack."""
     g = {k: torch.as_tensor(v).to(dtype) for k, v in sd.items()}
     x, label = torch.as_tensor(x), torch.as_tensor(label)
     h = F.embedding(x, g["embedding.weight"]).permute(0, 3, 1, 2)
     x_v = x_h = h
-    for i in range(n_layers):
+    for i, (mask, k, residual) in enumerate(_stack(n_layers, layers)):
         p = f"layers.{i}."
-        k = 7 if i == 0 else 3
         wv, wh = g[p + "vert_stack.weight"], g[p + "horiz_stack.weight"]
-        if i == 0:                                        # mask A (models.py:61-63)
+        if mask == "A":                                   # mask A (models.py:61-63)
             wv, wh = wv.clone(), wh.clone()
             wv[:, :, -1] = 0
             wh[:, :, :, -1] = 0
@@ -97,7 +141,7 @@ def prior_forward(sd, x, label, n_layers, dtype=torch.float32):
         v2h = F.conv2d(hv, g[p + "vert_to_horiz.weight"], g[p + "vert_to_horiz.bias"])
         out = _gate(v2h + hh + c)
         r = F.conv2d(out, g[p + "horiz_resid.weight"], g[p + "horiz_resid.bias"])
-        x_h = r + x_h if i > 0 else r
+        x_h = r + x_h if residual else r
         x_v = out_v
     y = F.relu(F.conv2d(x_h, g["output_conv.0.weight"], g["output_conv.0.bias"]))
     return F.conv2d(y, g["output_conv.2.weight"], g["output_conv.2.bias"])

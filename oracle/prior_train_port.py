@@ -1,7 +1,7 @@
 """The Gated PixelCNN prior restated differentiably with torch ops -- TEST INFRASTRUCTURE ONLY.
 
 ``prior_logits`` is the reference's GatedPixelCNN.forward (pixelcnn/models.py:121-130) on a dict of leaf tensors,
-with the reference's masking semantics: mask A zeroes the masked slices of layer 0's weights IN PLACE (through
+with the reference's masking semantics: mask A zeroes the masked slices of its layer's weights IN PLACE (through
 ``.data``) and then convolves with the full weight, so autograd gives the masked taps a (non-zero) gradient, as the
 reference's does.  (``oracle.prior_port.prior_forward`` masks a clone under no_grad, which would give them none.)
 ``prior_loss`` is the loss of the reference's ``gated_pixelcnn.py``.  Pinned against the unmodified reference by
@@ -11,6 +11,8 @@ oracle.make_prior_grad_golden`` writes.  The product never imports this module.
 import numpy as np
 import torch
 import torch.nn.functional as F
+
+from .prior_port import _stack
 
 # dot products of each gradient with this many seeded random tensors in the prior_grad_default fingerprint
 N_PROBES = 4
@@ -26,15 +28,15 @@ def _gate(t):
     return torch.tanh(a) * torch.sigmoid(b)
 
 
-def prior_logits(g, x, label, n_layers):
-    """Logits (B, K, H, W) of codes x (B,H,W) int64 and labels (B,) int64; g maps keys to (leaf) tensors."""
+def prior_logits(g, x, label, n_layers, layers=None):
+    """Logits (B, K, H, W) of codes x (B,H,W) int64 and labels (B,) int64; g maps keys to (leaf) tensors;
+    layers: (mask_type, kernel, residual) per layer, default the reference's stack."""
     h = F.embedding(x, g["embedding.weight"]).permute(0, 3, 1, 2)
     x_v = x_h = h
-    for i in range(n_layers):
+    for i, (mask, k, residual) in enumerate(_stack(n_layers, layers)):
         p = f"layers.{i}."
-        k = 7 if i == 0 else 3
         wv, wh = g[p + "vert_stack.weight"], g[p + "horiz_stack.weight"]
-        if i == 0:                                        # mask A (models.py:61-63): in place, on the parameter
+        if mask == "A":                                   # mask A (models.py:61-63): in place, on the parameter
             wv.data[:, :, -1].zero_()
             wh.data[:, :, :, -1].zero_()
         c = F.embedding(label, g[p + "class_cond_embedding.weight"])[:, :, None, None]
@@ -44,7 +46,7 @@ def prior_logits(g, x, label, n_layers):
         v2h = F.conv2d(hv, g[p + "vert_to_horiz.weight"], g[p + "vert_to_horiz.bias"])
         out = _gate(v2h + hh + c)
         r = F.conv2d(out, g[p + "horiz_resid.weight"], g[p + "horiz_resid.bias"])
-        x_h = r + x_h if i > 0 else r
+        x_h = r + x_h if residual else r
         x_v = out_v
     y = F.relu(F.conv2d(x_h, g["output_conv.0.weight"], g["output_conv.0.bias"]))
     return F.conv2d(y, g["output_conv.2.weight"], g["output_conv.2.bias"])

@@ -67,6 +67,7 @@ SIGNATURES = {
 }
 
 PRIOR_MAX_LAYERS = 32       # VQB_PRIOR_MAX_LAYERS
+PRIOR_MAX_KERNEL = 15       # VQB_PRIOR_MAX_KERNEL
 
 
 class PriorLayerWeights(C.Structure):

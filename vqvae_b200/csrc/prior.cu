@@ -1,7 +1,7 @@
 // prior.cu -- the Gated PixelCNN prior (pixelcnn/models.py of the reference), fp32 on CUDA cores (sm_90a).
 //
 // Activations are NHWC rows.  A buffer holds `ring` rows of a (B, ring, W, C) grid and row r lives in slot r % ring:
-// ring = H is a whole grid (the teacher-forced forward), ring = 1 or 2 the one or two rows the incremental sampler
+// ring = H is a whole grid (the teacher-forced forward), ring = 1 or gen_ring(H) the rows the incremental sampler
 // keeps.  Every output element is one fmaf chain over its inputs in a fixed order (taps, then input channels),
 // started from 0, then the bias: the value of an element does not depend on which positions share a block or on how
 // many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
@@ -365,10 +365,15 @@ __global__ void gate_kernel(const float *__restrict__ x, float *__restrict__ out
     }
 }
 
+// Rows of each layer's vertical output the sampler keeps: a layer l >= 1 with kernel k reads rows i - k/2 .. i of
+// layer l - 1's at row i.  The workspace does not see the kernels, so it holds the most any kernel reads; generate
+// uses the rows its own net reads (2 for the reference's 3x3 layers).
+int gen_ring(int H, int reach = VQB_PRIOR_MAX_KERNEL / 2 + 1) { return H < reach ? H : reach; }
+
 // workspace regions, in floats
 struct Ws {
     long long fwd_v, fwd_vh, fwd_x;               // forward: x0 | v[2] | vh | x[2]  (whole grids)
-    long long gen_x0, gen_v, gen_vh, gen_x, gen_lg;  // sampler: x0 | v[L] (2 rows) | vh[L] (1 row) | x[L] (1 row) | logits
+    long long gen_x0, gen_vh, gen_x, gen_lg, gen_v;  // sampler: x0 | vh[L] (1 row) | x[L] (1 row) | logits | v[L] (gen_ring)
     long long fwd_total, gen_total;
 };
 
@@ -380,11 +385,11 @@ Ws ws_layout(long long B, long long H, long long W, long long C, long long L, lo
     w.fwd_x = 5 * grid;
     w.fwd_total = 7 * grid;
     w.gen_x0 = 0;
-    w.gen_v = grid;
-    w.gen_vh = w.gen_v + L * B * 2 * W * C;
+    w.gen_vh = grid;
     w.gen_x = w.gen_vh + L * B * W * 2 * C;
     w.gen_lg = w.gen_x + L * B * W * C;
-    w.gen_total = w.gen_lg + B * K;
+    w.gen_v = w.gen_lg + B * K;                   // last: generate uses the first L * B * ring * W * C floats
+    w.gen_total = w.gen_v + L * B * gen_ring((int)H) * W * C;
     return w;
 }
 
@@ -474,20 +479,25 @@ extern "C" int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *l
     if (st) return st;
     if (!labels || !u || !codes || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
     if (workspace_bytes < vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    // Layer 0 must read only codes before (i, j): mask B reads row i and column j, a residual adds x_h at (i, j).
+    if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     const long long *lab = reinterpret_cast<const long long *>(labels);
     const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
     float *ws = static_cast<float *>(workspace);
-    const long long v_stride = (long long)B * 2 * W * n.C, vh_stride = (long long)B * W * 2 * n.C,
+    int reach = 1;
+    for (int l = 1; l < n.L; ++l) reach = max(reach, n.layer[l].kernel / 2 + 1);
+    const int ring = gen_ring(H, reach);
+    const long long v_stride = (long long)B * ring * W * n.C, vh_stride = (long long)B * W * 2 * n.C,
                     x_stride = (long long)B * W * n.C;
     const Act x0{ws + wl.gen_x0, H, n.C};
     for (int i = 0; i < H; ++i) {
         // row pass: every layer's vertical stack at row i (codes of rows < i are final)
         for (int l = 0; l < n.L; ++l) {
-            const Act vin = l == 0 ? x0 : Act{ws + wl.gen_v + (l - 1) * v_stride, 2, n.C};
+            const Act vin = l == 0 ? x0 : Act{ws + wl.gen_v + (l - 1) * v_stride, ring, n.C};
             vert_kernel<PF><<<blocks((long long)B * W, PF), NT, 0, s>>>(
-                n.layer[l], vin, Act{ws + wl.gen_v + l * v_stride, 2, n.C}, Act{ws + wl.gen_vh + l * vh_stride, 1, 2 * n.C},
-                lab, n.NC, B, H, W, i, 1, Act{});
+                n.layer[l], vin, Act{ws + wl.gen_v + l * v_stride, ring, n.C},
+                Act{ws + wl.gen_vh + l * vh_stride, 1, 2 * n.C}, lab, n.NC, B, H, W, i, 1, Act{});
         }
         for (int j = 0; j < W; ++j) {
             float *lg = step_logits ? step_logits + ((long long)i * W + j) * n.K : ws + wl.gen_lg;

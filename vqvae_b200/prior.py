@@ -16,16 +16,22 @@ Reference behaviour kept on purpose:
   P2  ``self.apply(weights_init)``: Xavier-uniform conv weights, zero biases, and one "Skipping initialization of"
       line per GatedMaskedConv2d (it matches 'Conv' by name but has no weight of its own)
   P3  mask A zeroes the last row of ``vert_stack.weight`` and the last column of ``horiz_stack.weight`` in the
-      caller's parameters.  Here that happens when layer 0's weights are (re)packed, i.e. once per change of the
-      parameter, so the packing cache and CUDA graphs around a forward stay valid
+      caller's parameters.  Here that happens when a mask-A layer's weights are (re)packed, i.e. once per change of
+      the parameter, so the packing cache and CUDA graphs around a forward stay valid
   P4  square grids only: the reference crops the vertical stack with the width and the horizontal one with the
       height, which fails for H != W; here that is a RuntimeError before any launch
+  P5  ``layers`` may be replaced by any GatedMaskedConv2d stack (odd kernels up to 15, either mask, with or without
+      residual), as the reference's forward walks whatever ``self.layers`` holds.  Every layer must have the model's
+      ``dim`` and layer 0's class count (the reference fails on such a model too, with a shape or index error); a
+      RuntimeError before any launch otherwise.  ``generate`` also needs layer 0 to be mask A without residual:
+      anything else reads the code being drawn, so the reference's one-forward-per-position loop is not causal in
+      raster order there, and the sampler refuses it (C ABI: VQB_ERR_UNSUPPORTED)
 """
 import torch
 import torch.nn as nn
 
 from . import ops
-from ._lib import C, PriorGrads, PriorLayerGrads, PriorLayerWeights, PriorNet
+from ._lib import PRIOR_MAX_KERNEL, C, PriorGrads, PriorLayerGrads, PriorLayerWeights, PriorNet
 from .modules import _packed, _packed_current
 
 HIDDEN = 512          # output_conv's hidden width
@@ -191,8 +197,23 @@ class GatedPixelCNN(nn.Module):
         )
         self.apply(weights_init)
 
+    def _check_layers(self):
+        """P5: the kernels take one channel count and one class count for the whole net."""
+        n_classes = self.layers[0].class_cond_embedding.num_embeddings if len(self.layers) else 1
+        for i, l in enumerate(self.layers):
+            dim, nc = l.horiz_resid.in_channels, l.class_cond_embedding.num_embeddings
+            kernel = l.vert_stack.kernel_size[1]
+            if dim != self.dim:
+                raise RuntimeError(f"GatedPixelCNN: layer {i} has {dim} channels, the model has dim={self.dim}")
+            if nc != n_classes:
+                raise RuntimeError(f"GatedPixelCNN: layer {i} has {nc} classes, layer 0 has {n_classes}")
+            if kernel > PRIOR_MAX_KERNEL:
+                raise RuntimeError(f"GatedPixelCNN: layer {i} has kernel {kernel}; the kernels take odd kernels up to "
+                                   f"{PRIOR_MAX_KERNEL}")
+
     def _net(self, keep):
         """(struct vqb_prior_net, its layer array); every tensor it points into is appended to `keep`."""
+        self._check_layers()
         layers = (PriorLayerWeights * len(self.layers))(*[l._weights(keep) for l in self.layers])
         o1, o2 = self.output_conv[0], self.output_conv[2]
         t = dict(embedding=_f32(self.embedding.weight), out1_w=_packed(o1.weight, ("prior", 1, 1)), out1_b=_f32(o1.bias),
@@ -222,6 +243,10 @@ class GatedPixelCNN(nn.Module):
         """generate() with given uniforms u (B,H,W) fp32: the code at (b,i,j) is the smallest k with u < CDF_k."""
         B, H, W = u.shape
         _square(H, W, "GatedPixelCNN.generate")
+        first = self.layers[0] if len(self.layers) else None
+        if first is not None and (first.mask_type != "A" or first.residual):
+            raise RuntimeError("GatedPixelCNN.generate: layer 0 must be mask A without residual (P5): this one reads "
+                               "the code being drawn, so the logits are not causal in raster order")
         ops._require_cuda(u, "GatedPixelCNN.generate uniforms")
         label = _labels(label, B, u.device, "GatedPixelCNN.generate")
         keep = []
