@@ -363,23 +363,39 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
         rc = vqb_encode_tmap_4d(&tout, dt, L.out, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
     }
-    const int stage = A_BYTES + L.N * 128;
-    const int fixed = kc2 * (A_BYTES + L.N2 * 128) + 8 * (2 * WG_MAX_STAGES + 1) + 1024;
-    int stages = (220 * 1024 - fixed) / stage;
-    if (stages > WG_MAX_STAGES) stages = WG_MAX_STAGES;
-    if (stages > maxk) stages = maxk;
-    if (stages < 1) return VQB_ERR_UNSUPPORTED;
-    q.stages = stages;
-    const int smem = stages * stage + fixed;
-    static int attr_max[64] = {0};      // per instantiation (slot below)
-    const int slot = (L.bf16 ? 32 : 0) + (L.N2 == 128 ? 16 : L.N2 == 64 ? 8 : 0) + (L.N == 16 ? 0 : L.N == 32 ? 1 : L.N == 64 ? 2 : L.N == 128 ? 3 : 4);
-    if (smem > attr_max[slot]) {
-        cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return (int)e;
-        attr_max[slot] = smem;
-    }
     const long long grid = (long long)q.tiles_x * q.tiles_y * tiles_n;
     if (grid <= 0 || grid > 0x7fffffffLL) return VQB_ERR_UNSUPPORTED;
+    const int stage = A_BYTES + L.N * 128;
+    const int fixed = kc2 * (A_BYTES + L.N2 * 128) + 8 * (2 * WG_MAX_STAGES + 1) + 1024;
+    auto ring = [&](int budget) {
+        const int st = (budget - fixed) / stage;
+        return st > WG_MAX_STAGES ? WG_MAX_STAGES : st > maxk ? maxk : st;
+    };
+    int stages = ring(220 * 1024);
+    if (stages < 1) return VQB_ERR_UNSUPPORTED;
+    static bool attr_set[64] = {false};      // per instantiation (slot below): every ring size fits in 220 KB
+    const int slot = (L.bf16 ? 32 : 0) + (L.N2 == 128 ? 16 : L.N2 == 64 ? 8 : 0) + (L.N == 16 ? 0 : L.N == 32 ? 1 : L.N == 64 ? 2 : L.N == 128 ? 3 : 4);
+    if (!attr_set[slot]) {
+        cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        if (e != cudaSuccess) return (int)e;
+        attr_set[slot] = true;
+    }
+    // More CTAs than SMs: a CTA spends its prologue, ring fill and epilogue with the tensor cores idle, and one per SM
+    // leaves them so.  Size the ring for two CTAs per SM (228 KB of shared memory, 1 KB of it reserved per CTA) when
+    // that keeps at least 3 stages and the registers allow it, so each CTA's k-steps cover the other's idle phases.
+    // The k-step order, and so every result bit, does not depend on the ring size.
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int shared = ring(113 * 1024);
+    if (grid * L.nph > sms && shared >= (maxk < 3 ? maxk : 3) && shared < stages) {
+        int per_sm = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, WG_THREADS, (size_t)(shared * stage + fixed)) ==
+                cudaSuccess && per_sm >= 2)
+            stages = shared;
+    }
+    q.stages = stages;
+    const int smem = stages * stage + fixed;
     if (cudaError_t le = vqb_launch(fn, dim3((unsigned)grid, (unsigned)L.nph), dim3(WG_THREADS), (size_t)smem, s, tin, tw, tw2, tout, q))
         return (int)le;
     VQB_COUNT_LAUNCH(1);
