@@ -209,18 +209,40 @@ __global__ void sum_partials_kernel(const double *__restrict__ partials, int n, 
 
 }  // namespace
 
-// workspace: [K floats code norms | pad to 256 B | VQ_MAX_CTAS doubles]
+// workspace: [Kpad floats code norms (+inf past K) | VQ_MAX_CTAS doubles SSE partials | Kpad / 128 floats per-block
+// maxima of the code norms | one counter of finished CTAs], Kpad = K rounded up to 256
 constexpr int VQ_MAX_CTAS = 2048;
 
+struct VqWorkspace {
+    float *bn;
+    double *partials;
+    float *bmax_part;
+    unsigned *done;
+};
+
+static size_t vq_kpad(int K) { return ((size_t)K + 255) / 256 * 256; }
+
+static VqWorkspace vq_workspace(void *ws, int K) {
+    unsigned char *p = reinterpret_cast<unsigned char *>(ws);
+    const size_t kpad = vq_kpad(K);
+    VqWorkspace w;
+    w.bn = reinterpret_cast<float *>(p);
+    w.partials = reinterpret_cast<double *>(p + kpad * sizeof(float));
+    w.bmax_part = reinterpret_cast<float *>(w.partials + VQ_MAX_CTAS);
+    w.done = reinterpret_cast<unsigned *>(w.bmax_part + kpad / 128);
+    return w;
+}
+
 size_t vq_exact_workspace_bytes(int K) {
-    return (((size_t)K * sizeof(float) + 255) / 256) * 256 + (size_t)VQ_MAX_CTAS * sizeof(double);
+    const size_t kpad = vq_kpad(K);
+    return kpad * sizeof(float) + (size_t)VQ_MAX_CTAS * sizeof(double) + kpad / 128 * sizeof(float) + 16;
 }
 
 int launch_vq_exact(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, int zq_bf16,
                     double *sse, int *hist, void *ws, cudaStream_t s) {
-    float *bn = reinterpret_cast<float *>(ws);
-    double *partials = reinterpret_cast<double *>(reinterpret_cast<unsigned char *>(ws) +
-                                                  (((size_t)K * sizeof(float) + 255) / 256) * 256);
+    const VqWorkspace w = vq_workspace(ws, K);
+    float *bn = w.bn;
+    double *partials = w.partials;
     cudaError_t e = cudaMemsetAsync(hist, 0, sizeof(int) * (size_t)K, s);
     if (e != cudaSuccess) return (int)e;
     code_norms_kernel<<<(K + 127) / 128, 128, 0, s>>>(E, K, D, bn);
@@ -255,92 +277,217 @@ int launch_vq_exact(const float *z, const float *E, long long N, int K, int D, l
 
 // ------------------------------------------------------------------------------------------------ tensor-core VQ (D = 64)
 // The same outputs as vq_exact_kernel, bit for bit, with the (N x K) distance work on Hopper tensor cores:
-//   1. per 128-row tile (z rows in shared memory, 128-byte swizzle) the codebook streams through in chunks of 128 codes;
-//      two warpgroups run wgmma m64n128k8 tf32 for the approximate scores s = ||e||^2 - 2 z.e, keep the running row
+//   1. per 128-row tile (z rows in shared memory, 128-byte swizzle) the codebook passes in chunks of 128 codes; two
+//      warpgroups run wgmma m64n128k8 tf32 for the approximate scores s = ||e||^2 - 2 z.e, keep the running row
 //      minimum and
 //   2. collect every code whose score lies within the TF32 error bound of the minimum so far
 //      (bound: 2^-6 ||z|| max||e|| + 2^-15 (||z||^2 + max||e||^2 + 2 ||z|| max||e||), far above the
 //      2 * 2^-10 sum|z||e| of TF32 operand rounding plus the fp32 rounding of the canonical distance);
-//   3. one thread per row re-scores its candidates in the canonical fp32 order of vq_exact_kernel and keeps the winner
-//      with the same tie / NaN rule.  A row whose list overflows, or whose scores or norms are not finite, is re-scored
-//      over all K codes: the result never depends on the approximation.
+//   3. two threads per row re-score its candidates in the canonical fp32 order of vq_exact_kernel and keep the winner
+//      with the same tie / NaN rule (a total order on (dist, k), so the split does not change the result).  A row whose
+//      list overflows, or whose scores or norms are not finite, is re-scored over all K codes: the result never depends
+//      on the approximation.
+//
+// Structure: one persistent CTA per SM, warp-specialised.  A producer warp loads z tiles (double-buffered, so the next
+// tile arrives during this one's re-scoring) and codebook chunks with their code norms by TMA into an mbarrier ring.
+// When the whole codebook fits in the ring (K <= 512 with the K-bin shared histogram beside it) it is loaded once per
+// CTA and stays; otherwise it streams through the ring continuously across tiles.  The two consumer warpgroups own 64
+// rows each and synchronise only through the ring and their own named barriers, so one warpgroup's epilogue runs while
+// the other's wgmma are in flight.  The norms of the codes (canonical order) and their maximum are computed once per
+// call by vq_prep_kernel; the row norms, the re-scoring and z_q all read z from the staged tile.  The SSE partials of
+// the CTAs are summed in CTA order by the last CTA to finish, so a call is two launches (prep, main) and gives a
+// bitwise-reproducible `sse`.
 namespace {
 
-constexpr int TC_ROWS = 128, TC_CODES = 128, TC_THREADS = 256, TC_CAP = 32;
-constexpr int TC_TILE = 128 * 128;                            // one [128][128 B] operand chunk
+constexpr int TC_ROWS = 128, TC_CODES = 128, TC_CAP = 24, TC_MAX_STAGES = 8;
+constexpr int TC_CONSUMERS = 256, TC_THREADS = TC_CONSUMERS + 32;   // two consumer warpgroups + the producer warp
+constexpr int TC_TILE = 128 * 128;                  // [128 rows][128 B]: 32 fp32 of K, 128-byte swizzle
+constexpr int TC_CHUNK = 2 * TC_TILE;               // a z tile or a codebook chunk: 128 rows x 64 fp32
+constexpr int TC_STAGE = TC_CHUNK + TC_CODES * 4;   // a chunk and its code norms
+constexpr int TC_HIST_SMEM = 1024;                  // histogram in shared memory up to this K
+constexpr int TC_BAR_ALL = 3;                       // named barrier of both consumer warpgroups (1, 2: one each)
 
-__device__ __forceinline__ void tc_stage_rows(uint32_t base, const float *src, long long row0, long long nrows, int tid) {
-    // rows of 64 fp32 -> two 128-byte-swizzled K chunks; rows past nrows are zero
-    for (int e = tid; e < 128 * 16; e += TC_THREADS) {
-        const int r = e >> 4, q = e & 15, chunk = q >> 3, j = q & 7;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row0 + r < nrows) v = __ldg(reinterpret_cast<const float4 *>(src + (size_t)(row0 + r) * 64) + q);
-        const uint32_t addr = base + (uint32_t)(chunk * TC_TILE + r * 128 + ((j ^ (r & 7)) << 4));
-        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-    }
+struct TcArgs {
+    const float *E, *bn, *bmax_part;
+    long long N;
+    int K, nch, stages, resident, nbpart, use_smem_hist, zq_bf16, dbg_cols;
+    long long *idx;
+    void *zq;
+    double *partials, *sse;
+    unsigned *done;
+    int *hist;
+    float *dbg;
+};
+
+// fp32 4q .. 4q+3 of row r of a [128][64] fp32 tile staged as two 128-byte-swizzled halves
+__device__ __forceinline__ float4 ld_tile4(const unsigned char *tile, int r, int q) {
+    return *reinterpret_cast<const float4 *>(tile + (q >> 3) * TC_TILE + r * 128 + (((q & 7) ^ (r & 7)) << 4));
 }
 
+// Code norms in the canonical order (quantizer.py:50; the arithmetic of code_norms_kernel), +inf for the padding codes
+// up to the grid's end, the per-block maxima over the real codes (NaN norms drop out: those rows are re-scored fully),
+// the zeroed histogram and the zeroed finished-CTA counter of vq_tc_kernel.
+__global__ void __launch_bounds__(128)
+vq_prep_kernel(const float *__restrict__ E, int K, float *__restrict__ bn, float *__restrict__ bmax_part,
+               int *__restrict__ hist, unsigned *__restrict__ done) {
+    __shared__ float wmax[4];
+    pdl_wait();                        // hist may still be read by the stream's earlier work
+    const int k = blockIdx.x * 128 + threadIdx.x;
+    float s = INFINITY, m = 0.f;
+    if (k < K) {
+        const float4 *e4 = reinterpret_cast<const float4 *>(E + (size_t)k * 64);
+        float4 v[16];
+#pragma unroll
+        for (int q = 0; q < 16; ++q) v[q] = __ldg(e4 + q);
+        s = 0.f;
+#pragma unroll
+        for (int q = 0; q < 16; ++q) {
+            s = __fadd_rn(s, __fmul_rn(v[q].x, v[q].x)); s = __fadd_rn(s, __fmul_rn(v[q].y, v[q].y));
+            s = __fadd_rn(s, __fmul_rn(v[q].z, v[q].z)); s = __fadd_rn(s, __fmul_rn(v[q].w, v[q].w));
+        }
+        m = fmaxf(m, s);
+        hist[k] = 0;
+    }
+    bn[k] = s;
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) bmax_part[blockIdx.x] = fmaxf(fmaxf(wmax[0], wmax[1]), fmaxf(wmax[2], wmax[3]));
+    if (k == 0) *done = 0u;
+}
+
+// DBG: also dump the approximate scores (vqb_debug_vq_scores_f32); a separate instantiation keeps the dump's address
+// arithmetic out of the release kernel's registers.
+template <bool DBG>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-vq_tc_kernel(const float *__restrict__ z, const float *__restrict__ E, const float *__restrict__ bn, long long N, int K,
-             int nchunks, long long *__restrict__ idx, void *__restrict__ zq, int zq_bf16, double *__restrict__ partials,
-             int *__restrict__ hist, float *__restrict__ dbg, int dbg_cols) {
+vq_tc_kernel(const __grid_constant__ CUtensorMap tma_z, const __grid_constant__ CUtensorMap tma_e,
+             const __grid_constant__ TcArgs p) {
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
     const uint32_t sbase = (raw + 1023u) & ~1023u;
     unsigned char *sm = smem_raw + (sbase - raw);
-    const uint32_t zt = sbase, et = sbase + 2 * TC_TILE;
-    float *bnc = reinterpret_cast<float *>(sm + 4 * TC_TILE);              // [TC_CODES]
-    float *thr = bnc + TC_CODES;                                           // [TC_ROWS] running row minimum
-    float *arow = thr + TC_ROWS;                                           // [TC_ROWS] canonical ||z||^2
-    int *cnt = reinterpret_cast<int *>(arow + TC_ROWS);                    // [TC_ROWS] candidates (> TC_CAP: full scan)
-    int *cand = cnt + TC_ROWS;                                             // [TC_ROWS][TC_CAP] candidate codes
-    float *cands = reinterpret_cast<float *>(cand + TC_ROWS * TC_CAP);     // [TC_ROWS][TC_CAP] their approximate scores
-    float *mg = cands + TC_ROWS * TC_CAP;                                  // [TC_ROWS] selection margin
+    const int S = p.stages;
+    // [z tile][z tile][S codebook chunks][S x 128 code norms][K histogram bins when use_smem_hist]
+    const uint32_t ring = sbase + 2 * TC_CHUNK;
+    const unsigned char *rings = sm + 2 * TC_CHUNK;
+    float *bnr = reinterpret_cast<float *>(sm + (size_t)(2 + S) * TC_CHUNK);
+    int *shist = reinterpret_cast<int *>(bnr + S * TC_CODES);
+    __shared__ __align__(8) uint64_t bars[2 * TC_MAX_STAGES + 4];
+    __shared__ float thr[TC_ROWS], arow[TC_ROWS], mg[TC_ROWS];     // running row minimum, canonical ||z||^2, margin
+    __shared__ int cnt[TC_ROWS], best_k[TC_ROWS];                    // candidates (> TC_CAP: full scan), winner
+    __shared__ int cand[TC_ROWS * TC_CAP];                           // candidate codes
+    __shared__ float cands[TC_ROWS * TC_CAP];                        // their approximate scores
     __shared__ float bmax_s;
-    __shared__ double red[TC_THREADS / 32];
+    __shared__ double red[TC_CONSUMERS / 32];
+    auto full = [&](int s) { return ptx::smem_u32(&bars[s]); };                     // chunk landed (TMA bytes)
+    auto empty = [&](int s) { return ptx::smem_u32(&bars[TC_MAX_STAGES + s]); };    // 8 consumer warps done with it
+    auto zfull = [&](int b) { return ptx::smem_u32(&bars[2 * TC_MAX_STAGES + b]); };
+    auto zempty = [&](int b) { return ptx::smem_u32(&bars[2 * TC_MAX_STAGES + 2 + b]); };   // both warpgroups done
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2, wl = warp & 3, cq = 2 * (lane & 3);
-    if (tid == 0) bmax_s = 0.f;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const long long ntiles = (p.N + TC_ROWS - 1) / TC_ROWS;
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), TC_CONSUMERS / 32); }
+        for (int b = 0; b < 2; ++b) { ptx::mbar_init(zfull(b), 1); ptx::mbar_init(zempty(b), 2); }
+        ptx::fence_mbar_init();
+        bmax_s = 0.f;
+    }
+    if (tid == TC_CONSUMERS) { ptx::prefetch_tmap(&tma_z); ptx::prefetch_tmap(&tma_e); }
+    if (p.use_smem_hist)
+        for (int k = tid; k < p.K; k += TC_THREADS) shist[k] = 0;
     __syncthreads();
+    // z, the code norms, and every output: a previous call's consumers (a graph replay's decoder) may still read z_q
+    pdl_wait();
+
+    if (warp == TC_CONSUMERS / 32) {   // ------------------------------------------------ producer
+        if (lane == 0) {
+            int rs = 0;                // ring slot and the number of times the ring has wrapped, continued across tiles
+            uint32_t wraps = 0;
+            int it = 0;
+            for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+                const int b = it & 1;
+                const int row0 = (int)(tile * TC_ROWS);
+                if (it >= 2) ptx::mbar_wait(zempty(b), (uint32_t)(((it >> 1) - 1) & 1));
+                ptx::mbar_expect_tx(zfull(b), (uint32_t)TC_CHUNK);
+                ptx::tma_load_2d(sbase + (uint32_t)(b * TC_CHUNK), &tma_z, zfull(b), 0, row0);
+                ptx::tma_load_2d(sbase + (uint32_t)(b * TC_CHUNK + TC_TILE), &tma_z, zfull(b), 32, row0);
+                if (p.resident && it > 0) continue;          // the whole codebook stays in the ring
+                for (int c = 0; c < p.nch; ++c) {
+                    const int s = rs;
+                    if (wraps > 0) ptx::mbar_wait(empty(s), (wraps - 1) & 1);
+                    if (++rs == S) { rs = 0; ++wraps; }
+                    ptx::mbar_expect_tx(full(s), (uint32_t)TC_STAGE);
+                    const uint32_t dst = ring + (uint32_t)(s * TC_CHUNK);
+                    ptx::tma_load_2d(dst, &tma_e, full(s), 0, c * TC_CODES);
+                    ptx::tma_load_2d(dst + TC_TILE, &tma_e, full(s), 32, c * TC_CODES);
+                    ptx::bulk_load_1d(ptx::smem_u32(bnr + s * TC_CODES), p.bn + (size_t)c * TC_CODES, TC_CODES * 4, full(s));
+                }
+            }
+        }
+        __syncwarp();
+        return;
+    }
+
+    // ------------------------------------------------------------------------------------ consumers
+    const int wgi = warp >> 2, wl = warp & 3, wt = tid & 127, cq = 2 * (lane & 3);
+    const uint32_t wg_bar = 1u + (uint32_t)wgi;
     {
         float m = 0.f;
-        for (int k = tid; k < K; k += TC_THREADS) m = fmaxf(m, __ldg(bn + k));      // NaN norms: rows re-scored fully below
+        for (int i = tid; i < p.nbpart; i += TC_CONSUMERS) m = fmaxf(m, __ldg(p.bmax_part + i));
+#pragma unroll
         for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
         if (lane == 0) atomicMax(reinterpret_cast<int *>(&bmax_s), __float_as_int(m));      // m >= 0: int order = float order
+        ptx::named_bar_sync(TC_BAR_ALL, TC_CONSUMERS);
     }
+    const float bmax = bmax_s;
+    // E row k, fp32 4q .. 4q+3: from the resident ring, or from L2
+    auto ld_code4 = [&](int k, int q) -> float4 {
+        if (p.resident) return ld_tile4(rings + (size_t)(k >> 7) * TC_CHUNK, k & 127, q);
+        return __ldg(reinterpret_cast<const float4 *>(p.E + (size_t)k * 64) + q);
+    };
+
     double my_sse = 0.0;
-    const long long ntiles = (N + TC_ROWS - 1) / TC_ROWS;
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    int rs = 0;                        // ring slot and its fill parity, as the producer steps them
+    uint32_t rpar = 0;
+    int it = 0;
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
         const long long r0 = tile * TC_ROWS;
-        __syncthreads();
-        tc_stage_rows(zt, z, r0, N, tid);
-        if (tid < TC_ROWS) {
-            float s = 0.f;                                                  // quantizer.py:49, canonical order
-            if (r0 + tid < N) {
-                const float *zr = z + (size_t)(r0 + tid) * 64;
-                for (int d = 0; d < 64; ++d) { const float v = __ldg(zr + d); s = __fadd_rn(s, __fmul_rn(v, v)); }
+        const int b = it & 1;
+        const uint32_t zt = sbase + (uint32_t)(b * TC_CHUNK);
+        const unsigned char *zs = sm + b * TC_CHUNK;
+        ptx::mbar_wait(zfull(b), (uint32_t)((it >> 1) & 1));
+        if (wt < 64) {                 // A_i (quantizer.py:49, canonical order) and the selection margin (see the header)
+            const int row = wgi * 64 + wt;
+            float s = 0.f;             // rows past N were zero-filled by the TMA: never written out
+#pragma unroll
+            for (int q = 0; q < 16; ++q) {
+                const float4 v = ld_tile4(zs, row, q);
+                s = __fadd_rn(s, __fmul_rn(v.x, v.x)); s = __fadd_rn(s, __fmul_rn(v.y, v.y));
+                s = __fadd_rn(s, __fmul_rn(v.z, v.z)); s = __fadd_rn(s, __fmul_rn(v.w, v.w));
             }
-            arow[tid] = s;
-            thr[tid] = INFINITY;
-            cnt[tid] = 0;
+            const float zn = sqrtf(s), en = sqrtf(bmax);
+            const float mgv = 0.015625f * zn * en + 3.0517578125e-5f * (s + bmax + 2.f * zn * en);
+            arow[row] = s;
+            thr[row] = INFINITY;
+            mg[row] = mgv;
+            cnt[row] = isfinite(mgv) ? 0 : TC_CAP + 1;     // not finite -> full re-scoring
         }
-        __syncthreads();
-        if (tid < TC_ROWS) {           // the row's selection margin (see the header); not finite -> full re-scoring
-            const float A = arow[tid], zn = sqrtf(A), en = sqrtf(bmax_s);
-            const float mgv = 0.015625f * zn * en + 3.0517578125e-5f * (A + bmax_s + 2.f * zn * en);
-            mg[tid] = mgv;
-            if (!isfinite(mgv)) cnt[tid] = TC_CAP + 1;
-        }
+        ptx::named_bar_sync(wg_bar, 128);
         // one sweep over the codebook: running row minimum of the approximate scores, and every code within the margin
         // of the minimum so far (codes that fall outside the final bound are dropped before re-scoring)
-        const int np = dbg ? dbg_cols / TC_CODES : nchunks;
-        for (int c = 0; c < np; ++c) {
+        for (int c = 0; c < p.nch; ++c) {
             const int k0 = c * TC_CODES;
-            __syncthreads();
-            tc_stage_rows(et, E, k0, K, tid);
-            if (tid < TC_CODES) bnc[tid] = k0 + tid < K ? __ldg(bn + k0 + tid) : INFINITY;
-            ptx::fence_proxy_async();
-            __syncthreads();
+            int s;
+            uint32_t par;
+            if (p.resident) { s = c; par = 0u; }
+            else {
+                s = rs; par = rpar;
+                if (++rs == S) { rs = 0; rpar ^= 1u; }
+            }
+            ptx::mbar_wait(full(s), par);
+            const uint32_t et = ring + (uint32_t)(s * TC_CHUNK);
+            const float *bnc = bnr + s * TC_CODES;
             float acc[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -357,7 +504,7 @@ vq_tc_kernel(const float *__restrict__ z, const float *__restrict__ E, const flo
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
-                const bool live = r0 + row < N;
+                const bool live = r0 + row < p.N;
                 float mn = INFINITY;
                 bool bad = false;
 #pragma unroll
@@ -367,8 +514,8 @@ vq_tc_kernel(const float *__restrict__ z, const float *__restrict__ E, const flo
                         const int col = 8 * j + cq + e;
                         const float sc = __fsub_rn(bnc[col], 2.f * acc[4 * j + 2 * h + e]);
                         acc[4 * j + 2 * h + e] = sc;
-                        if (dbg && live) dbg[(size_t)(r0 + row) * dbg_cols + k0 + col] = sc;
-                        if (k0 + col < K) { bad |= !(sc == sc); mn = fminf(mn, sc); }
+                        if (DBG && live) p.dbg[(size_t)(r0 + row) * p.dbg_cols + k0 + col] = sc;
+                        if (k0 + col < p.K) { bad |= !(sc == sc); mn = fminf(mn, sc); }
                     }
                 mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, 1));
                 mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, 2));
@@ -381,7 +528,7 @@ vq_tc_kernel(const float *__restrict__ z, const float *__restrict__ E, const flo
                         for (int e = 0; e < 2; ++e) {
                             const int col = 8 * j + cq + e;
                             const float sc = acc[4 * j + 2 * h + e];
-                            if (k0 + col < K && sc <= t) {
+                            if (k0 + col < p.K && sc <= t) {
                                 const int pos = atomicAdd(&cnt[row], 1);
                                 if (pos < TC_CAP) { cand[row * TC_CAP + pos] = k0 + col; cands[row * TC_CAP + pos] = sc; }
                             }
@@ -391,102 +538,166 @@ vq_tc_kernel(const float *__restrict__ z, const float *__restrict__ E, const flo
                 if ((lane & 3) == 0) thr[row] = rm;          // the row's four lanes read thr[row] above
                 if (bad) cnt[row] = TC_CAP + 1;
             }
+            __syncwarp();                                    // the warp's reads of the chunk and its norms are done
+            if (!p.resident && lane == 0) ptx::mbar_arrive(empty(s));
         }
-        __syncthreads();
+        ptx::named_bar_sync(wg_bar, 128);
         // canonical re-scoring of the candidates within the final bound (all K codes when the list overflowed or a score /
-        // norm was not finite)
-        if (tid < TC_ROWS && r0 + tid < N) {
-            const long long grow = r0 + tid;
-            const float *zr = z + (size_t)grow * 64;
-            const float A = arow[tid], t = thr[tid] + mg[tid];
-            const int nc = cnt[tid];
-            const bool full_scan = nc > TC_CAP || nc == 0;
-            const int n_try = full_scan ? K : nc;
-            float zv[64];
-#pragma unroll
-            for (int d = 0; d < 64; d += 4) {
-                const float4 v = __ldg(reinterpret_cast<const float4 *>(zr + d));
-                zv[d] = v.x; zv[d + 1] = v.y; zv[d + 2] = v.z; zv[d + 3] = v.w;
-            }
+        // norm was not finite): two threads per row, two independent dot-product chains per thread
+        {
+            const int row = wgi * 64 + (wt >> 1), half = wt & 1;
+            const long long grow = r0 + row;
             float bd = 0.f;
             int bk = -1;
-            for (int i = 0; i < n_try; ++i) {
-                if (!full_scan && cands[tid * TC_CAP + i] > t) continue;      // outside the final bound: cannot win
-                const int k = full_scan ? i : cand[tid * TC_CAP + i];
-                const float4 *er4 = reinterpret_cast<const float4 *>(E + (size_t)k * 64);
-                float m = 0.f;
+            if (grow < p.N) {
+                const float A = arow[row], t = thr[row] + mg[row];
+                const int nc = cnt[row];
+                const bool full_scan = nc > TC_CAP || nc == 0;
+                const int n_try = full_scan ? p.K : nc;
+                auto pick = [&](int i) -> int {          // -1: outside the final bound, cannot win
+                    if (full_scan) return i;
+                    return cands[row * TC_CAP + i] > t ? -1 : cand[row * TC_CAP + i];
+                };
+                for (int i = half; i < n_try; i += 4) {
+                    int ka = pick(i), kb = i + 2 < n_try ? pick(i + 2) : -1;
+                    if (ka < 0) { ka = kb; kb = -1; }
+                    if (ka < 0) continue;
+                    const int kb2 = kb >= 0 ? kb : ka;
+                    float ma = 0.f, mb = 0.f;
 #pragma unroll
-                for (int d = 0; d < 64; d += 4) {
-                    const float4 ev = __ldg(er4 + d / 4);
-                    m = __fmaf_rn(zv[d], ev.x, m); m = __fmaf_rn(zv[d + 1], ev.y, m);
-                    m = __fmaf_rn(zv[d + 2], ev.z, m); m = __fmaf_rn(zv[d + 3], ev.w, m);
+                    for (int q = 0; q < 16; ++q) {
+                        const float4 zv = ld_tile4(zs, row, q), ea = ld_code4(ka, q), eb = ld_code4(kb2, q);
+                        ma = __fmaf_rn(zv.x, ea.x, ma); mb = __fmaf_rn(zv.x, eb.x, mb);
+                        ma = __fmaf_rn(zv.y, ea.y, ma); mb = __fmaf_rn(zv.y, eb.y, mb);
+                        ma = __fmaf_rn(zv.z, ea.z, ma); mb = __fmaf_rn(zv.z, eb.z, mb);
+                        ma = __fmaf_rn(zv.w, ea.w, ma); mb = __fmaf_rn(zv.w, eb.w, mb);
+                    }
+                    const float da = __fsub_rn(__fadd_rn(A, __ldg(p.bn + ka)), __fmul_rn(2.0f, ma));   // quantizer.py:49-51
+                    if (bk < 0 || vq_better(da, ka, bd, bk)) { bd = da; bk = ka; }
+                    if (kb >= 0) {
+                        const float db = __fsub_rn(__fadd_rn(A, __ldg(p.bn + kb)), __fmul_rn(2.0f, mb));
+                        if (vq_better(db, kb, bd, bk)) { bd = db; bk = kb; }
+                    }
                 }
-                const float dist = __fsub_rn(__fadd_rn(A, __ldg(bn + k)), __fmul_rn(2.0f, m));   // quantizer.py:49-51
-                if (bk < 0 || vq_better(dist, k, bd, bk)) { bd = dist; bk = k; }
             }
-            const float *er = E + (size_t)bk * 64;
-            for (int d = 0; d < 64; d += 4) {
-                const float4 zv = __ldg(reinterpret_cast<const float4 *>(zr + d));
-                const float4 ev = __ldg(reinterpret_cast<const float4 *>(er + d));
-                float4 df, q;
+            const float od = __shfl_xor_sync(0xffffffffu, bd, 1);
+            const int ok = __shfl_xor_sync(0xffffffffu, bk, 1);
+            if (ok >= 0 && (bk < 0 || vq_better(od, ok, bd, bk))) { bd = od; bk = ok; }
+            if (half == 0 && grow < p.N) best_k[row] = bk;
+        }
+        ptx::named_bar_sync(wg_bar, 128);
+        // gather + straight-through + SSE + histogram from the staged tile: 16 threads per row, coalesced row stores
+        {
+            const int q = wt & 15;
+#pragma unroll 2
+            for (int pass = 0; pass < 8; ++pass) {
+                const int row = wgi * 64 + pass * 8 + (wt >> 4);
+                const long long grow = r0 + row;
+                if (grow >= p.N) continue;
+                const int k = best_k[row];
+                const float4 zv = ld_tile4(zs, row, q);
+                const float4 ev = ld_code4(k, q);
+                float4 df, o;
                 df.x = __fsub_rn(ev.x, zv.x); df.y = __fsub_rn(ev.y, zv.y);
                 df.z = __fsub_rn(ev.z, zv.z); df.w = __fsub_rn(ev.w, zv.w);
-                q.x = __fadd_rn(zv.x, df.x); q.y = __fadd_rn(zv.y, df.y);           // quantizer.py:67
-                q.z = __fadd_rn(zv.z, df.z); q.w = __fadd_rn(zv.w, df.w);
-                if (zq_bf16)
-                    *reinterpret_cast<uint2 *>(reinterpret_cast<__nv_bfloat16 *>(zq) + (size_t)grow * 64 + d) =
-                        make_uint2(pack_bf16(q.x, q.y), pack_bf16(q.z, q.w));
+                o.x = __fadd_rn(zv.x, df.x); o.y = __fadd_rn(zv.y, df.y);           // quantizer.py:67
+                o.z = __fadd_rn(zv.z, df.z); o.w = __fadd_rn(zv.w, df.w);
+                if (p.zq_bf16)
+                    *reinterpret_cast<uint2 *>(reinterpret_cast<__nv_bfloat16 *>(p.zq) + (size_t)grow * 64 + 4 * q) =
+                        make_uint2(pack_bf16(o.x, o.y), pack_bf16(o.z, o.w));
                 else
-                    *reinterpret_cast<float4 *>(reinterpret_cast<float *>(zq) + (size_t)grow * 64 + d) = q;
+                    *reinterpret_cast<float4 *>(reinterpret_cast<float *>(p.zq) + (size_t)grow * 64 + 4 * q) = o;
                 my_sse += (double)df.x * df.x + (double)df.y * df.y + (double)df.z * df.z + (double)df.w * df.w;
+                if (q == 0) {
+                    p.idx[grow] = k;
+                    if (p.use_smem_hist) atomicAdd(&shist[k], 1);
+                    else atomicAdd(&p.hist[k], 1);
+                }
             }
-            idx[grow] = bk;
-            atomicAdd(&hist[bk], 1);
         }
+        ptx::named_bar_sync(wg_bar, 128);            // the warpgroup is done with the z tile and the row state
+        if (wt == 0) ptx::mbar_arrive(zempty(b));
     }
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) my_sse += __shfl_xor_sync(0xffffffffu, my_sse, off);
     if (lane == 0) red[warp] = my_sse;
-    __syncthreads();
+    ptx::named_bar_sync(TC_BAR_ALL, TC_CONSUMERS);
+    if (p.use_smem_hist)
+        for (int k = tid; k < p.K; k += TC_CONSUMERS) {
+            const int c = shist[k];
+            if (c) atomicAdd(&p.hist[k], c);
+        }
     if (tid == 0) {
         double s = 0.0;
-        for (int w = 0; w < TC_THREADS / 32; ++w) s += red[w];
-        partials[blockIdx.x] = s;
+        for (int w = 0; w < TC_CONSUMERS / 32; ++w) s += red[w];
+        p.partials[blockIdx.x] = s;
+        __threadfence();
+        if (atomicAdd(p.done, 1u) == gridDim.x - 1) {      // the last CTA: sum the partials in CTA order
+            __threadfence();
+            double tot = 0.0;
+            for (unsigned i = 0; i < gridDim.x; ++i) tot += __ldcg(p.partials + i);
+            *p.sse = tot;
+        }
     }
 }
 
 }  // namespace
 
-bool vq_tc_supported(long long N, int K, int D) { return D == 64 && N >= 1 && K >= 1 && K <= (1 << 20); }
+bool vq_tc_supported(long long N, int K, int D) {
+    return D == 64 && N >= 1 && N <= 0x7fffffffLL - TC_ROWS && K >= 1 && K <= (1 << 20);
+}
 
 // dbg != null: also writes the approximate scores as (N, ceil(K / 256) * 256) floats (padding codes score +inf)
 int launch_vq_tc(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, int zq_bf16, double *sse,
                  int *hist, void *ws, float *dbg, cudaStream_t s) {
     if (!vq_tc_supported(N, K, D)) return VQB_ERR_UNSUPPORTED;
-    float *bn = reinterpret_cast<float *>(ws);
-    double *partials = reinterpret_cast<double *>(reinterpret_cast<unsigned char *>(ws) +
-                                                  (((size_t)K * sizeof(float) + 255) / 256) * 256);
-    cudaError_t e = cudaMemsetAsync(hist, 0, sizeof(int) * (size_t)K, s);
-    if (e != cudaSuccess) return (int)e;
-    code_norms_kernel<<<(K + 127) / 128, 128, 0, s>>>(E, K, D, bn);
-    const int smem = 4 * TC_TILE + (TC_CODES + 3 * TC_ROWS) * 4 + TC_ROWS * (1 + 2 * TC_CAP) * 4 + 1024;
-    static bool attr_set = false;
-    if (!attr_set) {
-        e = cudaFuncSetAttribute(vq_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    const VqWorkspace w = vq_workspace(ws, K);
+    const int kpad = (int)vq_kpad(K);
+    CUtensorMap tz, te;
+    int rc = vqb_encode_tmap_2d(&tz, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, z, 64, (uint64_t)N, 256, 32, TC_ROWS,
+                                CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = vqb_encode_tmap_2d(&te, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, E, 64, (uint64_t)K, 256, 32, TC_CODES,
+                            CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    auto *kernel = dbg ? vq_tc_kernel<true> : vq_tc_kernel<false>;
+    static int max_dyn[2] = {-1, -1};
+    int &md = max_dyn[dbg ? 1 : 0];
+    if (md < 0) {
+        cudaFuncAttributes fa;
+        cudaError_t e = cudaFuncGetAttributes(&fa, kernel);
         if (e != cudaSuccess) return (int)e;
-        attr_set = true;
+        const int m = 227 * 1024 - (int)fa.sharedSizeBytes;
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, m);
+        if (e != cudaSuccess) return (int)e;
+        md = m;
     }
+    TcArgs a = {};
+    a.E = E; a.bn = w.bn; a.bmax_part = w.bmax_part; a.N = N; a.K = K;
+    a.nch = dbg ? kpad / TC_CODES : (K + TC_CODES - 1) / TC_CODES;
+    a.nbpart = kpad / 128;
+    a.use_smem_hist = K <= TC_HIST_SMEM;
+    a.zq_bf16 = zq_bf16; a.dbg_cols = kpad;
+    a.idx = idx; a.zq = zq; a.partials = w.partials; a.sse = sse; a.done = w.done; a.hist = hist; a.dbg = dbg;
+    const int fixed = 1024 + 2 * TC_CHUNK + (a.use_smem_hist ? K * 4 : 0);
+    int stages = (md - fixed) / TC_STAGE;
+    if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
+    if (stages > a.nch) stages = a.nch;
+    if (stages < 1) return VQB_ERR_UNSUPPORTED;
+    a.stages = stages;
+    a.resident = a.nch <= stages;
+    const size_t smem = (size_t)fixed + (size_t)stages * TC_STAGE;
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const long long ntiles = (N + TC_ROWS - 1) / TC_ROWS;
-    long long grid = (long long)sms * 2;
+    long long grid = sms;
     if (grid > ntiles) grid = ntiles;
     if (grid > VQ_MAX_CTAS) grid = VQ_MAX_CTAS;
-    const int nchunks = (K + TC_CODES - 1) / TC_CODES;
-    const int dbg_cols = (K + 255) / 256 * 256;
-    vq_tc_kernel<<<(unsigned)grid, TC_THREADS, smem, s>>>(z, E, bn, N, K, nchunks, idx, zq, zq_bf16, partials, hist, dbg, dbg_cols);
-    sum_partials_kernel<<<1, 256, 0, s>>>(partials, (int)grid, sse);
-    VQB_COUNT_LAUNCH(3);
-    return vqb_cuda_status(cudaGetLastError());
+    cudaError_t e = vqb_launch(vq_prep_kernel, dim3((unsigned)(kpad / 128)), dim3(128), 0, s, E, K, w.bn, w.bmax_part, hist,
+                               w.done);
+    if (e != cudaSuccess) return (int)e;
+    e = vqb_launch(kernel, dim3((unsigned)grid), dim3(TC_THREADS), smem, s, tz, te, a);
+    VQB_COUNT_LAUNCH(2);
+    return vqb_cuda_status(e);
 }
