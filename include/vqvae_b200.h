@@ -77,8 +77,8 @@ unsigned long long vqb_launch_count(void);
  * nn.ConvTranspose2d weight (Cin,Cout,kh,kw) decoder.py:28-35   (transposed = 1)
  * -> `packed` holds Cout*Cin*kh*kw + 144*Cin floats (a larger buffer also does): the
  *    tap-major K-major rows [(r*kw+s)][co][ci] that every conv kernel reads; for a k4 s2
- *    transposed conv with Cout <= 4 the [9][16][Cin] form (3x3-neighbourhood +
- *    pixel-shuffle form of decoder.py:34-35) follows them.                        */
+ *    transposed conv with Cout <= 4 the [9][16][Cin] form follows them: per input
+ *    neighbour (dy, dx), the rows (sub-pixel phase, channel) of decoder.py:34-35.   */
 int vqb_pack_conv_weight_f32(const float *w, float *packed, int Cout, int Cin, int kh,
                              int kw, int transposed, void *stream);
 

@@ -11,7 +11,8 @@ pointers, which the caching allocator keeps mapped; only timing is read from the
 Beside each time: the modelled L2->SM bytes of the launch under two operand schemes -- "per-tap" (one 128-pixel A box
 per k-step, what wgconv_kernel loads) and "halo" (each tile's input halo once per chunk, the alternative) -- both with
 the N weight rows of every k-step, and the achieved bytes/s of each; the algorithmic FLOP/s; the card name and power
-limit.  Prints one JSON line.  Nothing is written to the repository tree.
+limit.  The output layer (convT to <= 4 channels) runs in scatter form, which loads each tile's halo once per chunk:
+both columns give that launch's bytes.  Prints one JSON line.  Nothing is written to the repository tree.
 """
 import argparse
 import json
@@ -70,8 +71,18 @@ def traffic(label, B):
         s = int(parts[2][parts[2].index("s") + 1:])
         h, w = (int(v) for v in parts[3].split("x"))
         w2 = 0
-        if transposed and s == 2 and cout <= 4:        # pixel-shuffle output layer: 3x3 neighbourhood, N = 16
-            N, nph, taps, step, ext, grid = 16, 1, 9, 1, 2, [(h, w)]
+        if transposed and s == 2 and cout <= 4:
+            # scatter-form output layer (convt_scatter_kernel): each tile's (TW + 2) x (TH + 2) halo once per chunk,
+            # the 64 gathered weight rows once per persistent CTA (two per SM of a 132-SM H100); both schemes alike
+            nc = (cin + ck - 1) // ck
+            tx = -(-w // 16)
+            tw = -(-w // tx)
+            ty = -(-h // (128 // (tw + 2) - 2))
+            th = -(-h // ty)
+            tiles = tx * ty * B
+            ctas = min(tiles, 2 * 132)
+            moved = tiles * nc * (tw + 2) * (th + 2) * 128 + ctas * nc * 64 * 128
+            return ctas, -(-tiles // ctas) * nc, moved, moved
         elif transposed and s == 2:                    # four sub-pixel phases of 2x2 taps
             N, nph, taps, step, ext, grid = _p2(max(cout, 16)), 4, 4, 1, 1, [(h, w)] * 4
         elif transposed or k == 3:

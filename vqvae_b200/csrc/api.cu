@@ -90,9 +90,10 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     const ConvGeom g = conv_geom(kh, kw, stride, pad, transposed, H, W);
     if (g.OH <= 0 || g.OW <= 0) return VQB_ERR_BAD_ARG;
 
-    // the two end layers: the output ConvTranspose2d (Cout <= 4) as one wgmma GEMM over the 3x3 input neighbourhood
-    // (N = 16 columns, pixel shuffle); the input conv (Cin = 3: K = 48 fp32 values per pixel straight from the NCHW
-    // image, HBM bound) and the fp32 mode on dedicated CUDA-core kernels (conv_edge.cu)
+    // the two end layers: the output ConvTranspose2d (Cout <= 4) as one wgmma GEMM per tile over its input pixels and
+    // their halo, summed into the pixel-shuffled output (wgconv.cu, scatter form); the input conv (Cin = 3: K = 48
+    // fp32 values per pixel straight from the NCHW image, HBM bound) and the fp32 mode on dedicated CUDA-core kernels
+    // (conv_edge.cu)
     if (kh == 4 && kw == 4 && stride == 2 && pad == 1 && !skip) {
         if (transposed && precision != VQB_FP32 && in_layout == VQB_NHWC && out_layout == VQB_NCHW &&
             convt_shuffle_supported(Cin, Cout)) {

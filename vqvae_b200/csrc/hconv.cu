@@ -6,8 +6,8 @@
 //   vqvae.py:16-17    Conv2d k1                 (fp32 output: z_e feeds the bit-exact VQ)
 //   decoder.py:28-29  ConvTranspose2d k3 s1 p1
 //   decoder.py:31-33  ConvTranspose2d k4 s2 p1  (four sub-pixel phases of 4 taps in one launch)
-//   decoder.py:34-35  ConvTranspose2d k4 s2 p1 to <= 4 channels (one 3x3-neighbourhood GEMM, N = 16, pixel-shuffle
-//                                                epilogue writing the NCHW fp32 module output)
+//   decoder.py:34-35  ConvTranspose2d k4 s2 p1 to <= 4 channels (scatter form: one GEMM over each tile's input pixels
+//                                                and halo, N = 64, neighbour sums writing the NCHW fp32 module output)
 //   residual.py:18-29 one ResidualLayer: 3x3 conv, ReLU and 1x1 conv chained inside one CTA per tile
 // A packed weight is the K-major layout the TF32 mode reads, in bf16: [kh*kw taps][Cout][Cin] (VQB_RES_W2: Cin zero
 // padded to 64), or [9 neighbour taps][16][Cin] for VQB_CONVT_K4S2_OUT.  The kernel reads the N rows of one k-step

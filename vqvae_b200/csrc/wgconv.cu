@@ -15,6 +15,8 @@
 //   * N2 > 0 (residual layer of the bf16 pipeline): the first GEMM's result is ReLU'd, rounded to bf16 and written
 //     to shared memory as the A operand of a second GEMM against an N2 x 64 weight tile loaded once, so
 //     out = act(skip + W2 . relu(W1 (*) r)) and the intermediate never leaves the SM.
+// The decoder's output layer (k4 s2 transposed conv to <= 4 channels) has its own persistent kernel at the end of this
+// file, convt_scatter_kernel: one GEMM per tile over the input pixels and their halo, read once per channel chunk.
 #include "ptx.cuh"
 #include "bf16_common.cuh"
 #include "wgconv.h"
@@ -33,7 +35,7 @@ struct WgParams {
     int B, ncols, mid_cols;
     int BW, BH, BN, tiles_x, tiles_y;
     int in_step, out_step, stages;
-    int relu, out_bf16, shuffle_cg;
+    int relu, out_bf16;
     int napps;                                // applications of a chained residual layer (whole-image tiles when > 1)
     int OHg[4], OWg[4], out_py[4], out_px[4], nsteps[4];
     long long out_sn, out_sh, out_sw, out_sc;
@@ -52,23 +54,6 @@ __device__ __forceinline__ void store_tile(const WgParams &p, const float *acc, 
         const int bw = row % p.BW, bh = (row / p.BW) % p.BH, bn = row / (p.BW * p.BH);
         const int gx = gx0 + bw, gy = gy0 + bh, n = n0 + bn;
         if (gx >= p.OWg[ph] || gy >= p.OHg[ph] || n >= p.B) continue;
-        if (p.shuffle_cg > 0) {
-            // k4 s2 transposed conv to a few channels: column = (sub-pixel phase, channel), fp32 NCHW output
-            float *out = reinterpret_cast<float *>(p.out);
-#pragma unroll
-            for (int j = 0; j < N / 8; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int c = 8 * j + cq + e;
-                    if (c >= p.ncols) continue;
-                    const int sp = c / p.shuffle_cg, co = c % p.shuffle_cg;
-                    float v = acc[4 * j + 2 * h + e] + (p.bias ? __ldg(p.bias + co) : 0.f);
-                    if (relu) v = fmaxf(v, 0.f);
-                    out[(long long)n * p.out_sn + (long long)(gy * 2 + (sp >> 1)) * p.out_sh +
-                        (long long)(gx * 2 + (sp & 1)) * p.out_sw + (long long)co * p.out_sc] = v;
-                }
-            continue;
-        }
         const long long ob = (long long)n * p.out_sn + (long long)(gy * p.out_step + p.out_py[ph]) * p.out_sh +
                              (long long)(gx * p.out_step + p.out_px[ph]) * p.out_sw;
 #pragma unroll
@@ -304,13 +289,13 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     if (!fn) return VQB_ERR_UNSUPPORTED;
     const int esz = L.bf16 ? 2 : 4, ck = 128 / esz;       // elements per 128-byte K chunk
     if (L.Cin % ck != 0 || L.w_inner % ck != 0) return VQB_ERR_UNSUPPORTED;
-    if (L.shuffle_cg == 0 && L.out_sc != 1) return VQB_ERR_UNSUPPORTED;
+    if (L.out_sc != 1) return VQB_ERR_UNSUPPORTED;
     WgParams q;
     memset(&q, 0, sizeof(q));
     q.bias = L.bias; q.skip = L.skip; q.out = L.out;
     q.B = L.B; q.ncols = L.ncols; q.mid_cols = L.ncols;
     q.in_step = L.in_step; q.out_step = L.out_step;
-    q.relu = L.relu; q.out_bf16 = L.out_bf16; q.shuffle_cg = L.shuffle_cg;
+    q.relu = L.relu; q.out_bf16 = L.out_bf16;
     q.napps = L.napps;
     if (L.napps < 1 || (L.napps > 1 && (L.N2 == 0 || L.Cin != L.N2 || L.skip != L.in))) return VQB_ERR_UNSUPPORTED;
     q.out_sn = L.out_sn; q.out_sh = L.out_sh; q.out_sw = L.out_sw; q.out_sc = L.out_sc;
@@ -474,24 +459,209 @@ int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void 
 }
 
 // ------------------------------------------------------------------------------------------------ output layer
-// decoder.py:34-35, ConvTranspose2d(Cin -> Cout <= 4, k4 s2 p1), NHWC in, NCHW fp32 out: one GEMM over the
-// 3x3 input neighbourhood with N = 16 columns (sub-pixel phase, channel) and a pixel-shuffle epilogue.
+// decoder.py:34-35, ConvTranspose2d(Cin -> Cout <= 4, k4 s2 p1), NHWC in, NCHW fp32 out, in scatter form.  Output
+// pixel (2 gy + py, 2 gx + px) takes input pixel (gy + dy, gx + dx) through kernel tap (py - 2 dy + 1, px - 2 dx + 1):
+// for each phase (py, px) the 2 x 2 neighbours dy = ky + py - 1, dx = kx + px - 1 (ky, kx in {0, 1}).  So every input
+// pixel p of a tile and its one-pixel halo is multiplied once by the 64 weight rows (phase, (ky, kx), co):
+//   Y[p][phase, k, co] = in[p] . w[tap of (phase, k)][phase, co]          (one m64n64 GEMM per warpgroup and chunk)
+// and the epilogue gathers
+//   out(2 gy + py, 2 gx + px, co) = act(Y[(gy + dy, gx + dx)][phase, k, co] summed over k = 0..3 in raster (dy, dx)
+//                                       order, + bias[co])
+// through shared memory.  The A operand is one 4-D TMA box {128 B of channels, TW + 2, TH + 2, 1} per chunk: the
+// tile's (TW + 2) x (TH + 2) halo pixels as plain rows (at most 128; TMA zero fills outside the image, which is the
+// padding).  Persistent CTAs: each gathers the 64 rows it needs from w_shuffle into shared memory once (in the 128-byte
+// swizzle wgmma reads, channels co >= Cout zero), then warp 8 streams the A boxes of the CTA's tiles through a ring
+// while warpgroups 0 and 1 run the GEMM and the epilogue.
 // w_shuffle: [9 taps (dy, dx)][16][Cin] (the region of vqb_pack_conv_weight_f32 at conv_pack_shuffle_offset, or
-// vqb_pack_conv_weight_bf16).
-bool convt_shuffle_supported(int Cin, int Cout) { return Cout >= 1 && Cout <= 4 && Cin % 32 == 0 && 9 * (Cin / 32) <= WG_MAX_STEPS; }
+// vqb_pack_conv_weight_bf16); row (py * 2 + px) * Cout + co of tap (dy + 1) * 3 + dx + 1.
+constexpr int SC_N = 64;                   // GEMM columns: 4 phases x 4 neighbours (ky, kx) x 4 channels
+constexpr int SC_BBYTES = SC_N * 128;      // one 128-byte channel chunk of the gathered weight
+constexpr int SC_ROW = 66;                 // staged floats per halo pixel: the 64 columns + 2 against bank conflicts
+constexpr int SC_STAGE_BYTES = 128 * SC_ROW * 4;
+constexpr int SC_MAX_STAGES = 4;
+constexpr int SC_THREADS = 288;            // warpgroups 0 and 1 (weight gather, GEMM, epilogue), warp 8 (TMA producer)
+
+struct ScParams {
+    const void *w;
+    const float *bias;
+    float *out;
+    int B, H, W, Cin, Cout, nc, ck, TW, TH, tiles_x, tiles_y, ntiles, stages, relu;
+    long long out_sn, out_sc, out_sh;
+};
+
+template <bool BF16>
+__global__ void __launch_bounds__(SC_THREADS, 2)
+convt_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant__ ScParams p) {
+    extern __shared__ unsigned char smem_raw[];
+    const uint32_t raw = ptx::smem_u32(smem_raw);
+    const uint32_t wres = (raw + 1023u) & ~1023u;                        // nc gathered weight chunks [64][128 B]
+    const uint32_t ring = wres + (uint32_t)(p.nc * SC_BBYTES);           // stages of one A box [128 px][128 B]
+    const uint32_t bars = ring + (uint32_t)(p.stages * A_BYTES);
+    float *const st = reinterpret_cast<float *>(smem_raw + (bars + 128u - raw));     // [128 px][SC_ROW]
+    auto full = [&](int s) { return bars + 8u * s; };
+    auto empty = [&](int s) { return bars + 8u * (SC_MAX_STAGES + s); };
+    const int S = p.stages, HW2 = p.TW + 2;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), 2); }
+        ptx::fence_mbar_init();
+    }
+    if (tid == 256) ptx::prefetch_tmap(&tma_in);
+    __syncthreads();
+    pdl_launch_dependents();
+
+    if (warp == 8) {
+        pdl_wait();                   // the activations come from the previous layer
+        if (lane == 0) {
+            const uint32_t abytes = (uint32_t)(HW2 * (p.TH + 2) * 128);
+            int g = 0;
+            for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+                const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, n = tile / (p.tiles_x * p.tiles_y);
+                for (int c = 0; c < p.nc; ++c, ++g) {
+                    const int s = g % S;
+                    if (g >= S) ptx::mbar_wait(empty(s), (uint32_t)((g / S - 1) & 1));
+                    ptx::mbar_expect_tx(full(s), abytes);
+                    ptx::tma_load_4d(ring + (uint32_t)(s * A_BYTES), &tma_in, full(s), c * p.ck, tx * p.TW - 1, ty * p.TH - 1, n);
+                }
+            }
+        }
+        return;
+    }
+
+    // gather the weight (it does not depend on the previous layer): row r = phase * 16 + k * 4 + co, 16-byte piece j
+    // of row r at j ^ (r & 7)
+    {
+        const size_t row_bytes = (size_t)p.Cin * (BF16 ? 2 : 4);
+        for (int i = tid; i < p.nc * SC_N * 8; i += 256) {
+            const int j = i & 7, r = (i >> 3) % SC_N, c = i / (8 * SC_N);
+            const int ph = r >> 4, k = (r >> 2) & 3, co = r & 3;
+            const int tap = ((k >> 1) + (ph >> 1)) * 3 + (k & 1) + (ph & 1);
+            uint4 v = make_uint4(0u, 0u, 0u, 0u);
+            if (co < p.Cout)
+                v = __ldg(reinterpret_cast<const uint4 *>(reinterpret_cast<const unsigned char *>(p.w) +
+                          (size_t)(tap * 16 + ph * p.Cout + co) * row_bytes + c * 128 + j * 16));
+            const uint32_t dst = wres + (uint32_t)(c * SC_BBYTES + r * 128 + ((j ^ (r & 7)) << 4));
+            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        }
+        ptx::fence_proxy_async();                      // generic-proxy writes -> visible to wgmma
+    }
+    float bias[4];
+#pragma unroll
+    for (int co = 0; co < 4; ++co) bias[co] = p.bias && co < p.Cout ? __ldg(p.bias + co) : 0.f;
+    pdl_wait();                       // `out` may still be read by the previous layer's consumers of it
+    const int wgi = warp >> 2, wl = warp & 3, cq = 2 * (lane & 3);
+    int g = 0;
+    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+        const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, n = tile / (p.tiles_x * p.tiles_y);
+        float acc[SC_N / 2];
+#pragma unroll
+        for (int i = 0; i < SC_N / 2; ++i) acc[i] = 0.f;
+        // first tile: the gathered weight is complete; later tiles: the previous epilogue has read the staging rows
+        ptx::named_bar_sync(1, 256);
+        for (int c = 0; c < p.nc; ++c, ++g) {
+            const int s = g % S;
+            ptx::mbar_wait(full(s), (uint32_t)((g / S) & 1));
+            const uint32_t a = ring + (uint32_t)(s * A_BYTES + wgi * 64 * 128), b = wres + (uint32_t)(c * SC_BBYTES);
+            wg::fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wg::mma<BF16, SC_N>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+            wg::commit();
+            wg::wait<0>();
+            wg::fence_regs<SC_N>(acc);
+            if (wl == 0 && lane == 0) ptx::mbar_arrive(empty(s));
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float *sr = st + (wgi * 64 + wl * 16 + (lane >> 2) + 8 * h) * SC_ROW + cq;
+#pragma unroll
+            for (int j = 0; j < SC_N / 8; ++j)
+                *reinterpret_cast<float2 *>(sr + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+        ptx::named_bar_sync(1, 256);
+        // lane = output column ox = 2 bx + px of the tile, warps over the output rows (co, by, py)
+        const int gx0 = tx * p.TW, gy0 = ty * p.TH, bx = lane >> 1, px = lane & 1;
+        float *out = p.out + (long long)n * p.out_sn + 2 * gx0 + lane;
+        const bool live = lane < 2 * p.TW && gx0 + bx < p.W;
+#pragma unroll
+        for (int co = 0; co < 4; ++co) {
+            if (co >= p.Cout || !live) break;
+            for (int r = warp; r < 2 * p.TH; r += 8) {
+                const int by = r >> 1, py = r & 1;
+                if (gy0 + by >= p.H) break;
+                // neighbour k = (ky, kx) of phase (py, px): halo row by + ky + py, halo column bx + kx + px
+                const float *s0 = st + ((by + py) * HW2 + bx + px) * SC_ROW + (py * 2 + px) * 16 + co;
+                float v = s0[0];
+                v += s0[SC_ROW + 4];
+                v += s0[HW2 * SC_ROW + 8];
+                v += s0[(HW2 + 1) * SC_ROW + 12];
+                v += bias[co];
+                if (p.relu) v = fmaxf(v, 0.f);
+                out[(long long)co * p.out_sc + (long long)(2 * (gy0 + by) + py) * p.out_sh] = v;
+            }
+        }
+    }
+}
+
+bool convt_shuffle_supported(int Cin, int Cout) { return Cout >= 1 && Cout <= 4 && Cin % 32 == 0 && Cin <= 256; }
 
 int launch_convt_shuffle_wg(int bf16, const void *in, const void *w_shuffle, const float *bias, float *out, int B, int Cin,
                             int H, int W, int Cout, int relu, cudaStream_t s) {
     if (!convt_shuffle_supported(Cin, Cout)) return VQB_ERR_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(w_shuffle)) & 15) return VQB_ERR_UNSUPPORTED;
-    WgLaunch L;
-    L.bf16 = bf16;
-    L.in = in; L.B = B; L.Cin = Cin; L.H = H; L.W = W;
-    L.w = w_shuffle; L.w_rows = 9LL * 16; L.w_inner = Cin;
-    L.N = 16; L.ncols = 4 * Cout; L.shuffle_cg = Cout;
-    L.bias = bias; L.out = out; L.relu = relu;
-    const int OH = 2 * H, OW = 2 * W;
-    L.out_sn = (long long)Cout * OH * OW; L.out_sc = (long long)OH * OW; L.out_sh = OW; L.out_sw = 1;
-    set_phase(L, 0, taps3x3(H, W), 16, bf16);
-    return launch_wgconv(L, s);
+    const int esz = bf16 ? 2 : 4, ck = 128 / esz;
+    if (Cin % ck != 0) return VQB_ERR_UNSUPPORTED;
+    ScParams q;
+    memset(&q, 0, sizeof(q));
+    q.w = w_shuffle; q.bias = bias; q.out = out; q.relu = relu;
+    q.B = B; q.H = H; q.W = W; q.Cin = Cin; q.Cout = Cout; q.nc = Cin / ck; q.ck = ck;
+    // tiles of at most 16 columns whose halo (TW + 2) x (TH + 2) fits 128 rows, split evenly over the image
+    q.tiles_x = (W + 15) / 16;
+    q.TW = (W + q.tiles_x - 1) / q.tiles_x;
+    const int th_max = 128 / (q.TW + 2) - 2;
+    q.tiles_y = (H + th_max - 1) / th_max;
+    q.TH = (H + q.tiles_y - 1) / q.tiles_y;
+    const long long ntiles = (long long)q.tiles_x * q.tiles_y * B;
+    if (ntiles <= 0 || ntiles > 0x7fffffffLL) return VQB_ERR_UNSUPPORTED;
+    q.ntiles = (int)ntiles;
+    q.out_sn = 4LL * Cout * H * W; q.out_sc = 4LL * H * W; q.out_sh = 2LL * W;
+
+    CUtensorMap tin;
+    const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t strides[3] = {(uint64_t)Cin * esz, (uint64_t)W * Cin * esz, (uint64_t)H * W * Cin * esz};
+    const uint32_t box[4] = {(uint32_t)ck, (uint32_t)(q.TW + 2), (uint32_t)(q.TH + 2), 1u};
+    const uint32_t es[4] = {1u, 1u, 1u, 1u};
+    const int rc = vqb_encode_tmap_4d(&tin, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, in,
+                                      dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+
+    // the gathered weight, the ring, the barriers and the staging rows: two CTAs per SM (113 KB each) when that keeps
+    // 2 stages, so one CTA's epilogue overlaps the other's GEMM; else one CTA with up to 4 stages
+    auto smem_for = [&](int stages) { return 1024 + q.nc * SC_BBYTES + stages * A_BYTES + 128 + SC_STAGE_BYTES; };
+    auto kernel = bf16 ? convt_scatter_kernel<true> : convt_scatter_kernel<false>;
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[bf16 ? 1 : 0]) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        if (e != cudaSuccess) return (int)e;
+        attr_set[bf16 ? 1 : 0] = true;
+    }
+    int dev = 0, sms = 132, per_sm = 1, occ = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int stages = SC_MAX_STAGES;
+    while (stages > 2 && smem_for(stages) > 113 * 1024) --stages;
+    if (smem_for(stages) <= 113 * 1024 && ntiles > sms &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, SC_THREADS, (size_t)smem_for(stages)) == cudaSuccess &&
+        occ >= 2) {
+        per_sm = 2;
+    } else {
+        stages = SC_MAX_STAGES;
+        while (stages > 1 && smem_for(stages) > 220 * 1024) --stages;
+    }
+    q.stages = stages;
+    const long long grid = ntiles < (long long)per_sm * sms ? ntiles : (long long)per_sm * sms;
+    if (cudaError_t le = vqb_launch(kernel, dim3((unsigned)grid), dim3(SC_THREADS), (size_t)smem_for(stages), s, tin, q))
+        return (int)le;
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
 }

@@ -27,7 +27,6 @@ struct WgLaunch {
     const void *skip = nullptr;           // same layout and type as out, may be null
     void *out = nullptr;
     int out_bf16 = 0, relu = 0;
-    int shuffle_cg = 0;                   // > 0: column c = (sub-pixel phase c / cg, channel c % cg), fp32 out
     int out_step = 1;
     long long out_sn = 0, out_sh = 0, out_sw = 0, out_sc = 1;    // element strides of out (and skip)
     int nph = 1;
