@@ -19,8 +19,8 @@
  *     SURVEY.md 8e): the opt-in shared-memory size of each kernel is configured once
  *     per process, on the device that is current at its first launch; calls may come
  *     from any host thread but are not re-entrant on the same workspace;
- *   - host pointers appear only in vqb_memcpy_async, the vqb_debug_* readers and the
- *     weight tables of the vqb_prior_* entry points;
+ *   - host pointers appear only in vqb_memcpy_async and the weight tables of the
+ *     vqb_prior_* entry points;
  *   - return value: 0 = success, >0 = cudaError_t, <0 = vqb_status below; no C++
  *     exception crosses the boundary;
  *   - activations between layers are NHWC ("pixel rows": (B*H*W, C) row-major); the
@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define VQB_ABI_VERSION 2
+#define VQB_ABI_VERSION 3
 
 enum vqb_status {
     VQB_OK = 0,
@@ -129,8 +129,8 @@ int vqb_conv2d_bf16(const void *in, const void *packed, const float *bias, void 
  * and tf32 modes).                                                                          */
 int vqb_conv_in_bf16(const float *x, const float *w_packed, const float *bias, void *out, int B,
                      int H, int W, int Cout, int relu, void *stream);
-/* VectorQuantizer core for the bf16 pipeline: as vqb_vq_forward_deferred_f32 (fp32 z, bit-exact
- * idx, deferred SSE) but zq is written as bf16 rows (N, D); D == 64 only.                    */
+/* VectorQuantizer core for the bf16 pipeline: as vqb_vq_forward_f32 (fp32 z, bit-exact idx,
+ * final sse) but zq is written as bf16 rows (N, D); D == 64 only.                            */
 int vqb_vq_forward_bf16zq_f32(const float *z, const float *codebook, int64_t N, int K, int D,
                               int64_t *idx, void *zq_bf16, double *sse, int32_t *hist,
                               void *workspace, size_t workspace_bytes, void *stream);
@@ -190,22 +190,11 @@ int vqb_vq_forward_f32(const float *z, const float *codebook, int64_t N, int K, 
                        int64_t *idx, float *zq, double *sse, int32_t *hist,
                        void *workspace, size_t workspace_bytes, void *stream);
 
-/* Deferred variant: identical outputs, except that `sse` is only final after
- * vqb_vq_reduce_sse_f32 has run on the same workspace (stream-ordered after this call).
- * The sm_90a kernels finish the SSE inside their own launch sequence, so `sse` is already
- * final here and vqb_vq_reduce_sse_f32 only validates its arguments; the pair stays so
- * that callers may run the scalar finisher on a side stream (vqvae.py:36 does not depend
- * on the loss terms of quantizer.py:63-64).                                            */
-int vqb_vq_forward_deferred_f32(const float *z, const float *codebook, int64_t N, int K, int D,
-                                int64_t *idx, float *zq, double *sse, int32_t *hist,
-                                void *workspace, size_t workspace_bytes, void *stream);
-int vqb_vq_reduce_sse_f32(const void *workspace, int64_t N, int K, int D, double *sse,
-                          void *stream);
-
 /* Kernel choice of vqb_vq_forward_f32: 0 = auto (see vqb_vq_forward_f32's dispatch),
- * 1 = always the exact FFMA kernel, 2 and 3 = require the wgmma kernel (TF32 candidate
- * selection + canonical fp32 re-scoring; D == 64, 1 <= K <= 2^20).  All produce
- * bit-identical idx / zq; the switch exists for tests and benchmarks.                 */
+ * 1 = always the exact FFMA kernel, 2 = require the wgmma kernel (TF32 candidate
+ * selection + canonical fp32 re-scoring; D == 64, 1 <= K <= 2^20); anything else is
+ * VQB_ERR_BAD_ARG.  All produce bit-identical idx / zq; the switch exists for tests
+ * and benchmarks.                                                                     */
 int vqb_set_vq_kernel(int which);
 
 /* Diagnostic twin of vqb_vq_forward_f32 (wgmma kernel, D == 64): additionally dumps the
@@ -245,12 +234,6 @@ int vqb_gather_rows_f32(const int64_t *idx, const float *codebook, int64_t N, in
 /* In-place ReLU over n floats: the nn.ReLU(True) of residual.py:19, which mutates
  * the caller's tensor when a ResidualLayer is called directly (SURVEY Q2).         */
 int vqb_relu_f32(float *x, int64_t n, void *stream);
-
-/* In-kernel timeline readers, kept for ABI version 2 compatibility: the sm_90a kernels record
- * no timelines, so these always return VQB_ERR_UNSUPPORTED.                              */
-int vqb_debug_read_trace(unsigned long long *dst, int n);
-int vqb_debug_read_trace_vq(unsigned long long *dst, int n);
-int vqb_debug_read_cta_times(unsigned long long *dst, int n);
 
 /* ---- layout changes at the module boundary (quantizer.py:45, :74) ---------------- */
 int vqb_nchw_to_nhwc_f32(const float *in, float *out, int B, int C, int H, int W, void *stream);

@@ -19,7 +19,7 @@ def _header_functions():
     return sorted(set(re.findall(r"\b(vqb_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_library_builds_loads_and_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_and_none_removed_in_abi_3():
     from vqvae_b200.build import build
     lib = ctypes.CDLL(build())
     names = _header_functions()
@@ -27,7 +27,10 @@ def test_library_builds_loads_and_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/vqvae_b200.h but not exported"
     lib.vqb_abi_version.restype = ctypes.c_int
-    assert lib.vqb_abi_version() == 2
+    assert lib.vqb_abi_version() == 3
+    for n in ("vqb_vq_forward_deferred_f32", "vqb_vq_reduce_sse_f32", "vqb_debug_read_trace", "vqb_debug_read_trace_vq",
+              "vqb_debug_read_cta_times"):      # removed in ABI version 3
+        assert not hasattr(lib, n), f"{n} is still exported"
     assert lib.vqb_diag_build() == 0          # the shipped library never reads the environment
     lib.vqb_error_string.restype = ctypes.c_char_p
     assert b"workspace" in lib.vqb_error_string(-3)
@@ -38,7 +41,7 @@ def test_ctypes_signature_table_matches_header():
     assert sorted(_lib.SIGNATURES) == _header_functions()
 
 
-def test_argument_validation_without_a_gpu():
+def test_abi_3_argument_validation_without_a_gpu():
     """Bad arguments are rejected before any CUDA call (safe on a CPU box)."""
     from vqvae_b200 import _lib
     lib = _lib.lib()
@@ -46,8 +49,6 @@ def test_argument_validation_without_a_gpu():
     assert lib.vqb_vq_forward_f32(None, None, 1, 1, 4, None, None, None, None, None, 0, None) == -1
     assert lib.vqb_set_vq_kernel(7) == -1
     assert lib.vqb_vq_workspace_bytes(1024, 512, 64) > 0
-    assert lib.vqb_vq_forward_deferred_f32(None, None, 1, 1, 4, None, None, None, None, None, 0, None) == -1
-    assert lib.vqb_vq_reduce_sse_f32(None, 1, 1, 4, None, None) == -1
     assert lib.vqb_residual_layer_f32(None, None, None, None, None, 1, 8, 8, 32, 32, 1, 1, None) == -1
     assert lib.vqb_residual_stack_f32(None, None, None, None, None, None, 1, 8, 8, 32, 32, 2, 1, None) == -1
     import ctypes
@@ -150,7 +151,7 @@ def test_bf16_pipeline_coverage(args, distinct_layers, covered):
     assert m._bf16_pipeline() is False           # other precisions never take the bf16 pipeline
 
 
-def test_new_entry_points_validate_arguments_without_a_gpu():
+def test_bf16_entry_points_and_vq_kernel_switch_validate_arguments():
     """bf16 pipeline entry points: bad arguments / unsupported shapes are rejected before any CUDA call."""
     from vqvae_b200 import _lib
     lib = _lib.lib()
@@ -170,7 +171,7 @@ def test_new_entry_points_validate_arguments_without_a_gpu():
     # the fp32-activation entry points refuse the bf16 enum instead of silently running TF32 (round-1 verdict)
     assert lib.vqb_conv2d_f32(p, p, None, None, p, 1, 64, 8, 8, 64, 3, 3, 1, 1, 0, 1, 1, 0, _lib.BF16, None) == -2
     assert lib.vqb_residual_layer_f32(p, p, p, p, p, 1, 8, 8, 32, 32, 1, _lib.BF16, None) == -2
-    assert lib.vqb_set_vq_kernel(3) == 0 and lib.vqb_set_vq_kernel(0) == 0
+    assert lib.vqb_set_vq_kernel(3) == -1 and lib.vqb_set_vq_kernel(2) == 0 and lib.vqb_set_vq_kernel(0) == 0
 
 
 def test_no_cpu_fallback():

@@ -22,8 +22,8 @@ def _run(kernel, z, E, **kw):
 
 
 def _check(z, E, **kw):
-    i_e, q_e, s_e, h_e = _run("exact", z, E, **kw)[:4]
-    i_t, q_t, s_t, h_t = _run("tc", z, E, **kw)[:4]
+    i_e, q_e, s_e, h_e = _run("exact", z, E, **kw)
+    i_t, q_t, s_t, h_t = _run("tc", z, E, **kw)
     assert torch.equal(i_t, i_e), int((i_t != i_e).sum())
     assert torch.equal(q_t.view(torch.int16 if q_t.dtype == torch.bfloat16 else torch.int32),
                        q_e.view(torch.int16 if q_e.dtype == torch.bfloat16 else torch.int32))
@@ -77,15 +77,14 @@ def test_nonfinite_rows():
 
 
 @pytest.mark.parametrize("K", [512, 1000])
-def test_bf16_zq_and_deferred_entry_points(K):
-    from vqvae_b200 import ops
+def test_bf16_zq_entry_point(K):
+    """The bf16-z_q call gives the fp32 call's idx, hist and sse bitwise, and its z_q rounded to bf16."""
     z, E = _normal(3000, K, 21, scale=0.5)
-    _check(z, E, defer=True, zq_dtype=torch.bfloat16)
+    _check(z, E, zq_dtype=torch.bfloat16)
     i0, q0, s0, h0 = _run("tc", z, E)
-    i1, q1, s1, h1, ws = _run("tc", z, E, defer=True)
-    ops.vq_reduce_sse(ws, z.shape[0], K, 64, s1)
-    torch.cuda.synchronize()
-    assert torch.equal(i0, i1) and torch.equal(q0, q1) and torch.equal(h0, h1) and s0.item() == s1.item()
+    i1, q1, s1, h1 = _run("tc", z, E, zq_dtype=torch.bfloat16)
+    assert torch.equal(i0, i1) and torch.equal(h0, h1) and s0.item() == s1.item()
+    assert torch.equal(q1.view(torch.int16), q0.to(torch.bfloat16).view(torch.int16))
 
 
 @pytest.mark.parametrize("K", [512, 1024])

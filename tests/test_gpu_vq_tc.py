@@ -103,27 +103,3 @@ def test_tc_kernel_large_n_matches_exact_kernel(K, kind):
     # oracle spot check on a slice
     o = cref.vq_rows(z[:4096], E)
     assert np.array_equal(i_t[:4096], o["idx"])
-
-
-@pytest.mark.parametrize("N,K,D,kernel", [(5000, 512, 64, "auto"), (777, 1000, 64, "auto"), (640, 512, 64, "exact"), (300, 96, 32, "auto")])
-def test_deferred_sse_reduction(N, K, D, kernel):
-    """vqb_vq_forward_deferred_f32 + vqb_vq_reduce_sse_f32 (the reduction may run later / on a side stream)
-    give exactly the outputs of vqb_vq_forward_f32, on the wgmma kernel and on the exact FFMA kernel."""
-    from vqvae_b200 import ops
-    rng = np.random.RandomState(N + K)
-    z = torch.from_numpy(rng.standard_normal((N, D)).astype(np.float32)).cuda()
-    E = torch.from_numpy((rng.standard_normal((K, D)) * 0.7).astype(np.float32)).cuda()
-    ops.set_vq_kernel(kernel)
-    try:
-        i0, q0, s0, h0 = ops.vq_forward(z, E)
-        i1, q1, s1, h1, ws = ops.vq_forward(z, E, defer=True)
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            ops.vq_reduce_sse(ws, N, K, D, s1)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-    finally:
-        ops.set_vq_kernel("auto")
-    assert torch.equal(i0, i1) and torch.equal(q0, q1) and torch.equal(h0, h1)
-    assert s0.item() == s1.item() and s0.item() > 0

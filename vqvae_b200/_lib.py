@@ -30,9 +30,7 @@ SIGNATURES = {
     "vqb_conv2d_f32": (_i, [_vp] * 5 + [_i] * 14 + [_vp]),
     "vqb_vq_workspace_bytes": (_sz, [_i64, _i, _i]),
     "vqb_vq_forward_f32": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "vqb_vq_forward_deferred_f32": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "vqb_memcpy_async": (_i, [_vp, _vp, _sz, _i, _vp]),
-    "vqb_vq_reduce_sse_f32": (_i, [_vp, _i64, _i, _i, _vp, _vp]),
     "vqb_vq_finish_f32": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _vp, _vp]),
     "vqb_vq_backward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _vp, _vp, _vp]),
     "vqb_onehot_f32": (_i, [_vp, _i64, _i, _vp, _vp]),
@@ -42,9 +40,6 @@ SIGNATURES = {
     "vqb_relu_f32": (_i, [_vp, _i64, _vp]),
     "vqb_launch_count": (C.c_ulonglong, []),
     "vqb_set_vq_kernel": (_i, [_i]),
-    "vqb_debug_read_trace": (_i, [_vp, _i]),
-    "vqb_debug_read_trace_vq": (_i, [_vp, _i]),
-    "vqb_debug_read_cta_times": (_i, [_vp, _i]),
     "vqb_residual_layer_f32": (_i, [_vp] * 5 + [_i] * 7 + [_vp]),
     "vqb_residual_stack_f32": (_i, [_vp] * 6 + [_i] * 7 + [_vp]),
     "vqb_conv_bf16_packed_bytes": (_sz, [_i, _i, _i]),
@@ -104,7 +99,7 @@ def lib():
             fn = getattr(handle, name)   # AttributeError if the symbol is missing
             fn.restype = res
             fn.argtypes = args
-        if handle.vqb_abi_version() != 2:
+        if handle.vqb_abi_version() != 3:
             raise RuntimeError("libvqvae_b200.so ABI version mismatch")
         _lib = handle
     return _lib

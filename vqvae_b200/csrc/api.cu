@@ -25,9 +25,9 @@ int vqb_pdl_enabled() {
 }
 
 unsigned long long g_vqb_launches = 0;
-static int g_vq_kernel = 0;   // 0 auto (tensor-core kernel when D == 64), 1 exact FFMA kernel, 2 / 3 tensor-core kernel
+static int g_vq_kernel = 0;   // 0 auto (tensor-core kernel when D == 64), 1 exact FFMA kernel, 2 tensor-core kernel
 extern "C" int vqb_set_vq_kernel(int which) {
-    if (which < 0 || which > 3) return VQB_ERR_BAD_ARG;
+    if (which < 0 || which > 2) return VQB_ERR_BAD_ARG;
     g_vq_kernel = which;
     return 0;
 }
@@ -192,7 +192,7 @@ static int vq_forward_impl(const float *z, const float *codebook, int64_t N, int
     if (N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
     if (D % 4 != 0) return VQB_ERR_UNSUPPORTED;
     const bool tc_ok = vq_tc_supported(N, K, D);
-    if (g_vq_kernel >= 2 && !tc_ok) return VQB_ERR_UNSUPPORTED;
+    if (g_vq_kernel == 2 && !tc_ok) return VQB_ERR_UNSUPPORTED;
     if (workspace_bytes < vqb_vq_workspace_bytes(N, K, D)) return VQB_ERR_WORKSPACE;
     const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(codebook) |
                          reinterpret_cast<uintptr_t>(zq) | reinterpret_cast<uintptr_t>(workspace);
@@ -210,21 +210,7 @@ extern "C" int vqb_vq_forward_f32(const float *z, const float *codebook, int64_t
     return vq_forward_impl(z, codebook, N, K, D, idx, zq, 0, sse, hist, workspace, workspace_bytes, stream);
 }
 
-// The exact kernel finishes the SSE inside its own launch sequence, so the deferred variant has nothing left
-// for vqb_vq_reduce_sse_f32 to do; both keep the contract of the header.
-extern "C" int vqb_vq_forward_deferred_f32(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx,
-                                           float *zq, double *sse, int32_t *hist, void *workspace,
-                                           size_t workspace_bytes, void *stream) {
-    return vq_forward_impl(z, codebook, N, K, D, idx, zq, 0, sse, hist, workspace, workspace_bytes, stream);
-}
-
-extern "C" int vqb_vq_reduce_sse_f32(const void *workspace, int64_t N, int K, int D, double *sse, void *stream) {
-    (void)stream;
-    if (!workspace || !sse || N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
-    return 0;
-}
-
-// VQB_BF16 pipeline: same contract as vqb_vq_forward_deferred_f32 (fp32 z in, bit-exact idx) but z_q leaves as bf16
+// VQB_BF16 pipeline: same contract as vqb_vq_forward_f32 (fp32 z in, bit-exact idx) but z_q leaves as bf16
 // rows for the decoder's first conv.
 extern "C" int vqb_vq_forward_bf16zq_f32(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx,
                                          void *zq_bf16, double *sse, int32_t *hist, void *workspace,
@@ -252,11 +238,6 @@ extern "C" int vqb_debug_vq_scores_f32(const float *z, const float *codebook, in
     return launch_vq_tc(z, codebook, N, K, D, reinterpret_cast<long long *>(idx), zq, 0, sse, hist, workspace, scores,
                         (cudaStream_t)stream);
 }
-
-// In-kernel timeline readers of ABI version 2: the sm_90a kernels record none, so they answer VQB_ERR_UNSUPPORTED.
-extern "C" int vqb_debug_read_trace(unsigned long long *, int) { return VQB_ERR_UNSUPPORTED; }
-extern "C" int vqb_debug_read_trace_vq(unsigned long long *, int) { return VQB_ERR_UNSUPPORTED; }
-extern "C" int vqb_debug_read_cta_times(unsigned long long *, int) { return VQB_ERR_UNSUPPORTED; }
 
 extern "C" int vqb_residual_layer_f32(const float *r, const float *w1_packed, const float *w2_packed, float *out,
                                       float *tmp, int B, int H, int W, int C, int Cmid, int relu_out, int precision,

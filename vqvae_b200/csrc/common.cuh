@@ -7,9 +7,9 @@
 
 #define VQB_MAX_TAPS 16
 
-// Experiment / diagnostic knobs (VQB_* environment variables, the work-skipping VQB_TC_FLAGS bits, in-kernel
-// timelines) exist only in a library built with -DVQB_DIAG=1 (VQB_DIAG=1 python -m vqvae_b200.build).  The release library never reads the environment: vqb_getenv() is a constant nullptr there and the
-// flag tests in the kernels fold away.
+// The environment knobs for experiments (VQB_PDL, VQB_MEMCPY_RUNTIME) are read only by a library built with
+// -DVQB_DIAG=1 (VQB_DIAG=1 python -m vqvae_b200.build).  The release library never reads the environment:
+// vqb_getenv() is a constant nullptr there.
 #ifndef VQB_DIAG
 #define VQB_DIAG 0
 #endif
@@ -87,21 +87,6 @@ static inline cudaError_t vqb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 b
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = vqb_pdl_enabled() ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-}
-// same, as thread-block clusters of `cluster` CTAs along x (the grid must be a multiple of it)
-template <typename... KArgs, typename... Args>
-static inline cudaError_t vqb_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
-                                             unsigned cluster, Args &&...args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = vqb_pdl_enabled() ? 2 : 1;
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 #endif

@@ -39,7 +39,7 @@ struct WgParams {
     int napps;                                // applications of a chained residual layer (whole-image tiles when > 1)
     int OHg[4], OWg[4], out_py[4], out_px[4], nsteps[4];
     long long out_sn, out_sh, out_sw, out_sc;
-    int4 steps[4][WG_MAX_STEPS];              // x = a_c0 | b_c0 << 16, y = dx, z = dy, w = w_row
+    int4 steps[4][WG_MAX_STEPS];              // x = c0, y = dx, z = dy, w = w_row
 };
 
 // Epilogue of one accumulator fragment (wgmma D layout, see wgmma.cuh) for the pixel rows of this thread.
@@ -150,8 +150,8 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
                     const int4 st = p.steps[ph][i];
                     const uint32_t dst = sbase + (uint32_t)(s * STAGE);
                     ptx::mbar_expect_tx(full(s), (uint32_t)STAGE);
-                    ptx::tma_load_4d(dst, src, full(s), st.x & 0xffff, gx0 * p.in_step + st.y, gy0 * p.in_step + st.z, n0);
-                    ptx::tma_load_2d(dst + A_BYTES, &tma_w, full(s), st.x >> 16, st.w);
+                    ptx::tma_load_4d(dst, src, full(s), st.x, gx0 * p.in_step + st.y, gy0 * p.in_step + st.z, n0);
+                    ptx::tma_load_2d(dst + A_BYTES, &tma_w, full(s), st.x, st.w);
                 }
             }
             __syncwarp();
@@ -306,7 +306,7 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
         q.nsteps[i] = L.nsteps[i];
         for (int t = 0; t < L.nsteps[i]; ++t) {
             const WgStep &st = L.steps[i][t];
-            q.steps[i][t] = make_int4(st.a_c0 | (st.b_c0 << 16), st.dx, st.dy, st.w_row);
+            q.steps[i][t] = make_int4(st.c0, st.dx, st.dy, st.w_row);
         }
         if (L.OWg[i] > maxw) maxw = L.OWg[i];
         if (L.OHg[i] > maxh) maxh = L.OHg[i];
@@ -400,7 +400,7 @@ static bool set_phase(WgLaunch &L, int i, const ConvPhase &ph, int rows_per_tap,
     for (int a = 0; a < (chunk_outer ? nc : ph.ntaps); ++a)
         for (int b = 0; b < (chunk_outer ? ph.ntaps : nc); ++b) {
             const int t = chunk_outer ? b : a, c0 = (chunk_outer ? a : b) * ck;
-            L.steps[i][n++] = WgStep{c0, c0, ph.tap_dx[t], ph.tap_dy[t], ph.tap_w[t] * rows_per_tap};
+            L.steps[i][n++] = WgStep{c0, ph.tap_dx[t], ph.tap_dy[t], ph.tap_w[t] * rows_per_tap};
         }
     L.nsteps[i] = n;
     return true;

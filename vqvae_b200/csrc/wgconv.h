@@ -4,9 +4,9 @@
 
 #define WG_MAX_STEPS 72        // k-steps per phase: taps x 128-byte channel chunks (e.g. 9 taps x 8 chunks)
 
-// One k-step: the A box starts at channel a_c0 of the input pixel shifted by (dy, dx); the B box is the N weight
-// rows starting at w_row, channel b_c0 within the row.
-struct WgStep { int a_c0, b_c0, dx, dy, w_row; };
+// One k-step over channels [c0, c0 + chunk): the A box is those channels of the input pixel shifted by (dy, dx); the
+// B box is the same channels of the N weight rows starting at w_row.
+struct WgStep { int c0, dx, dy, w_row; };
 
 struct WgLaunch {
     int bf16 = 0;                         // operands: 0 = fp32 activations read as TF32, 1 = bf16

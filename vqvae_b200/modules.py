@@ -482,23 +482,21 @@ class VQVAE(nn.Module):
         D = vq.e_dim
         group = self.process_group
         # The decoder does not depend on the loss / perplexity scalars (vqvae.py:36 vs quantizer.py:63-71), so
-        # the SSE reduction, the batch-sharded all-reduce (SURVEY 8e) and the scalar finisher run on a side
-        # stream and overlap the decoder; fork/join with events, so the whole forward stays capturable in one
-        # CUDA graph.
+        # the batch-sharded all-reduce of (sse, hist) (SURVEY 8e) and the scalar finisher run on a side stream
+        # and overlap the decoder; fork/join with events, so the whole forward stays capturable in one CUDA graph.
         n_rows = z_e.shape[0] * H * W
-        idx, zq, sse, hist, ws = ops.vq_forward(z_e.view(-1, D), vq._codebook(), defer=True,
-                                                zq_dtype=torch.bfloat16 if bf16 else torch.float32)
+        idx, zq, sse, hist = ops.vq_forward(z_e.view(-1, D), vq._codebook(),
+                                            zq_dtype=torch.bfloat16 if bf16 else torch.float32)
         main = torch.cuda.current_stream()
         if self._side_stream is None or self._side_stream.device != z_e.device:
             self._side_stream = torch.cuda.Stream(device=z_e.device)
         side = self._side_stream
         side.wait_stream(main)
         with torch.cuda.stream(side):
-            ops.vq_reduce_sse(ws, n_rows, vq.n_e, D, sse)
             embedding_loss, perplexity = vq._scalars(sse, hist, n_rows, group if self.sync_scalars else None)
             self.last_vq_stats = (hist, sse, n_rows)
             if not torch.cuda.is_current_stream_capturing():
-                for t in (ws, sse, hist, embedding_loss, perplexity):
+                for t in (sse, hist, embedding_loss, perplexity):
                     t.record_stream(side)
         x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16)  # :36
         main.wait_stream(side)

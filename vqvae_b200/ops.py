@@ -214,15 +214,14 @@ def residual_stack(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, n_layers, preci
     return out
 
 
-def vq_forward(z_rows, codebook, defer=False, zq_dtype=torch.float32):
+def vq_forward(z_rows, codebook, zq_dtype=torch.float32):
     """Fused VectorQuantizer core on (N,D) fp32 rows -> (idx int64 (N,), zq (N,D), sse f64 (1,),
-    hist int32 (K,)).  defer=True (vqb_vq_forward_deferred_f32) additionally returns the workspace:
-    `sse` is final only after vq_reduce_sse(ws, ...) has run (e.g. on a side stream).  zq_dtype=torch.bfloat16
-    (vqb_vq_forward_bf16zq_f32, D == 64, deferred only) writes z_q as bf16 rows for the bf16 pipeline."""
+    hist int32 (K,)); `sse` is final when the call returns.  zq_dtype=torch.bfloat16
+    (vqb_vq_forward_bf16zq_f32, D == 64) writes z_q as bf16 rows for the bf16 pipeline."""
     _require_cuda(z_rows, "z")
     bf16zq = zq_dtype == torch.bfloat16
-    if zq_dtype not in (torch.float32, torch.bfloat16) or (bf16zq and not defer):
-        raise ValueError("vq_forward: z_q is fp32, or bf16 rows with the deferred SSE (defer=True)")
+    if zq_dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError("vq_forward: z_q is fp32 or bf16 rows")
     N, D = z_rows.shape
     K = codebook.shape[0]
     dev = z_rows.device
@@ -233,21 +232,11 @@ def vq_forward(z_rows, codebook, defer=False, zq_dtype=torch.float32):
     ws_bytes = lib().vqb_vq_workspace_bytes(N, K, D)
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
     span = _Span(f"vq N={N} K={K} D={D}{' (bf16 zq)' if bf16zq else ''}")
-    if bf16zq:
-        fn = lib().vqb_vq_forward_bf16zq_f32
-    else:
-        fn = lib().vqb_vq_forward_deferred_f32 if defer else lib().vqb_vq_forward_f32
+    fn = lib().vqb_vq_forward_bf16zq_f32 if bf16zq else lib().vqb_vq_forward_f32
     check(fn(z_rows.data_ptr(), codebook.data_ptr(), N, K, D, idx.data_ptr(), zq.data_ptr(), sse.data_ptr(),
              hist.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "vq_forward")
     span.done()
-    if defer:
-        return idx, zq, sse, hist, ws
     return idx, zq, sse, hist
-
-
-def vq_reduce_sse(ws, N, K, D, sse):
-    """Completes `sse` after vq_forward(..., defer=True) (vqb_vq_reduce_sse_f32), on the current stream."""
-    check(lib().vqb_vq_reduce_sse_f32(ws.data_ptr(), N, K, D, sse.data_ptr(), _stream()), "vq_reduce_sse")
 
 
 def vq_finish(sse, hist, N, K, D, beta):
@@ -312,7 +301,7 @@ def relu_(x):
     return x
 
 
-VQ_KERNELS = {"auto": 0, "exact": 1, "tc": 2, "tc_r1": 3}
+VQ_KERNELS = {"auto": 0, "exact": 1, "tc": 2}
 
 
 def set_vq_kernel(name: str):
