@@ -235,6 +235,10 @@ int vqb_gather_rows_f32(const int64_t *idx, const float *codebook, int64_t N, in
  * the caller's tensor when a ResidualLayer is called directly (SURVEY Q2).         */
 int vqb_relu_f32(float *x, int64_t n, void *stream);
 
+/* Gradient through a ReLU from its kept output y: out = y > 0 ? g : 0 over n floats (out may be g).
+ * The backward of VQVAE.forward's ReLUs (residual.py:19,21,50, encoder.py:30,33, decoder.py:33). */
+int vqb_relu_backward_f32(const float *g, const float *y, float *out, int64_t n, void *stream);
+
 /* ---- layout changes at the module boundary (quantizer.py:45, :74) ---------------- */
 int vqb_nchw_to_nhwc_f32(const float *in, float *out, int B, int C, int H, int W, void *stream);
 int vqb_nhwc_to_nchw_f32(const float *in, float *out, int B, int C, int H, int W, void *stream);
@@ -243,6 +247,22 @@ int vqb_nhwc_to_nchw_f32(const float *in, float *out, int B, int C, int H, int W
  * kind 1 = host -> device, 2 = device -> host, 3 = device -> device.  Host buffers should be
  * pinned (the copy is only asynchronous then).                                          */
 int vqb_memcpy_async(void *dst, const void *src, size_t bytes, int kind, void *stream);
+
+/* ---- weight gradient of one convolution layer (training VQVAE.forward, main.py:74-79) ------------------
+ * dW (and dbias unless NULL) of the layer vqb_conv2d_f32 runs with the same geometry: `in` is the layer's
+ * input (B,Cin,H,W) in in_layout, g_out the gradient of its output (B,Cout,OH,OW) in gout_layout.  dW is
+ * written in the parameter's own layout, (Cout,Cin,kh,kw) or, transposed, (Cin,Cout,kh,kw); dbias (Cout).
+ * Both are OVERWRITTEN.  Any kernel size, stride, padding and channel counts.  fp32 on CUDA cores; the
+ * reduction over images and pixels runs in fixed chunks summed in a fixed order, with no atomics: two calls
+ * give bitwise-equal results.  A weight applied several times (a shared ResidualLayer) gets one reduction
+ * over all its applications when their inputs and output gradients are passed as one batch of n*B images.
+ * 2 launches, 3 for a transposed conv with a bias.  workspace: vqb_conv_wgrad_workspace_bytes bytes,
+ * enough with or without dbias (0 = bad geometry).                                                       */
+size_t vqb_conv_wgrad_workspace_bytes(int B, int Cin, int H, int W, int Cout, int kh, int kw, int stride,
+                                      int pad, int transposed);
+int vqb_conv_wgrad_f32(const float *in, const float *g_out, float *dW, float *dbias, int B, int Cin, int H,
+                       int W, int Cout, int kh, int kw, int stride, int pad, int transposed, int in_layout,
+                       int gout_layout, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- Gated PixelCNN prior, pixelcnn/models.py (inference, fp32 on CUDA cores) ----------------------------
  * The prior over VQ code grids: teacher-forced logits (GatedPixelCNN.forward, models.py:121-130) and the whole

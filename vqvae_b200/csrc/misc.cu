@@ -127,6 +127,13 @@ __global__ void relu_kernel(float *__restrict__ x, long long n) {
         x[i] = fmaxf(x[i], 0.f);
 }
 
+// out = y > 0 ? g : 0 (out may be g): the gradient through a ReLU whose output y was kept
+__global__ void relu_backward_kernel(const float *g, const float *__restrict__ y, float *out, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
+         i += (long long)gridDim.x * blockDim.x)
+        out[i] = __ldg(y + i) > 0.f ? g[i] : 0.f;
+}
+
 unsigned grid_for(long long total, int block) {
     long long g = (total + block - 1) / block;
     if (g > 148LL * 32) g = 148LL * 32;
@@ -213,6 +220,14 @@ extern "C" int vqb_relu_f32(float *x, int64_t n, void *stream) {
     if (!x || n < 0) return VQB_ERR_BAD_ARG;
     if (n == 0) return 0;
     relu_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(x, n);
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_relu_backward_f32(const float *g, const float *y, float *out, int64_t n, void *stream) {
+    if (!g || !y || !out || n < 0) return VQB_ERR_BAD_ARG;
+    if (n == 0) return 0;
+    relu_backward_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(g, y, out, n);
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }

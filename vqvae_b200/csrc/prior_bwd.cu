@@ -12,11 +12,11 @@
 // reproducible.  Weight gradients cover all kh*kw taps, mask A's included (the reference convolves with the full,
 // zeroed weight, so autograd gives those taps a gradient); dgrad reads the taps the forward kept.
 #include "prior.cuh"
+#include "wgrad_reduce.cuh"
 
 namespace {
 
 constexpr int BM = 64, BN = 64, BK = 16, GT = 256;       // CTA tile, k-step, threads (16 x 16, 4 x 4 outputs each)
-constexpr long long WG_CHUNK = 2048;                     // at most this many positions per wgrad partial
 
 struct Grid {                     // position n of a (B, H, W) grid
     int H, W;
@@ -236,50 +236,12 @@ __global__ void __launch_bounds__(GT) gemm_kernel(LA a, LB b, EP ep, int M, int 
         }
 }
 
-// ---- split-K reduction of the wgrad partials, into the parameters' layouts --------------------------------------
-// Job: partials [splits][M][cols] with cols = taps*Cin (+1 for the bias); column tap*Cin + ci -> w[m][ci][tap]
-// (the (Cout, Cin, kh, kw) layout with tap = r*kw + s), the ones column -> bias[m].
-struct RJob {
-    const float *part;
-    float *w, *bias;
-    int M, Cin, taps, cols, splits;
-};
-constexpr int MAX_JOBS = 5;
-struct RJobs {
-    RJob j[MAX_JOBS];
-};
-
-__global__ void reduce_kernel(RJobs jobs) {
-    const RJob J = jobs.j[blockIdx.y];
-    const long long total = (long long)J.M * J.cols, stride = total;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        float v = 0.f;
-        for (int z = 0; z < J.splits; ++z) v += J.part[z * stride + i];
-        const int m = (int)(i / J.cols), j = (int)(i % J.cols);
-        if (j >= J.taps * J.Cin) {
-            J.bias[m] = v;
-        } else {
-            const int tap = j / J.Cin, ci = j % J.Cin;
-            J.w[((long long)m * J.Cin + ci) * J.taps + tap] = v;
-        }
-    }
-}
-
 // ---- host side ---------------------------------------------------------------------------------------------------
 int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-struct Split {                    // wgrad reduction over K positions: `splits` chunks of `chunk` positions
-    int splits, chunk;
-};
+using Split = WgradSplit;         // wgrad reduction over K positions: `splits` chunks of `chunk` positions
 
-Split wsplit(int M, int N, long long K) {
-    const long long tiles = (long long)cdiv(M, BM) * cdiv(N, BN);
-    long long s = cdiv(2 * 132, tiles);                      // about two CTAs per SM
-    s = s > cdiv(K, WG_CHUNK) ? s : cdiv(K, WG_CHUNK);       // and short fmaf chains
-    s = s < cdiv(K, BK) ? s : cdiv(K, BK);
-    const int chunk = cdiv(cdiv(K, s), BK) * BK;
-    return {cdiv(K, chunk), chunk};
-}
+Split wsplit(int M, int N, long long K) { return wgrad_split(M, N, K, BM, BN, BK); }
 
 template <class LA, class LB, class EP>
 void gemm(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K, Split sp) {
@@ -377,7 +339,7 @@ void reduce(cudaStream_t st, const Phase &p, float *part, float *const (&w)[MAX_
         jobs.j[i] = RJob{part + j.off, w[i], b[i], j.M, j.Cin, j.taps, j.cols(), j.sp.splits};
         most = most > (long long)j.M * j.cols() ? most : (long long)j.M * j.cols();
     }
-    reduce_kernel<<<dim3(cdiv(most, NT) < 1024 ? cdiv(most, NT) : 1024, p.n), NT, 0, st>>>(jobs);
+    wgrad_reduce(st, jobs, p.n, most);
 }
 
 bool grads_ok(const vqb_prior_grads *g, int L) {

@@ -7,7 +7,10 @@ re-exports these classes).  The nn.Conv2d / nn.ConvTranspose2d / nn.Embedding ch
 are kept ONLY as parameter containers (identical init order => identical weights under
 the same torch seed, identical ``state_dict()``); their own ``forward`` is never used.
 Every ``forward`` here launches the hand-written sm_90a kernels through the C ABI
-(``include/vqvae_b200.h``).  Inference only: outputs carry no autograd graph.
+(``include/vqvae_b200.h``).  ``VQVAE.forward`` is differentiable in training mode (``_VQVAEFunction``: model.train(),
+grad enabled, a parameter or the image requiring grad), so the reference's ``main.py`` loop runs unchanged; in eval
+mode, under no_grad, and for the piecewise sub-module calls the outputs carry no autograd graph (unlike the
+reference, whose eval-mode outputs do).
 
 Reference semantics reproduced on purpose (SURVEY 3.3):
   Q1  ResidualStack applies ONE shared ResidualLayer n times (residual.py:44-45)
@@ -268,8 +271,9 @@ class Encoder(nn.Module):
         )
         self.conv_stack[0]._bf16_key = ("f32", False)      # bf16: vqb_conv_in_bf16 reads the fp32 packing
 
-    def _forward_nhwc(self, x, bf16=False):
-        """x: prepared NCHW fp32 CUDA tensor -> (NHWC activation, bf16 in the bf16 pipeline, B, H, W)."""
+    def _forward_nhwc(self, x, bf16=False, acts=None):
+        """x: prepared NCHW fp32 CUDA tensor -> (NHWC activation, bf16 in the bf16 pipeline, B, H, W).  `acts` (a
+        dict, training walk) receives the post-ReLU outputs of the three convs and the stack's output as "enc"."""
         B, _, H, W = x.shape
         cs = self.conv_stack
         if bf16:      # the 3-channel image has its own entry point: fp32 NCHW in, bf16 NHWC out
@@ -278,11 +282,16 @@ class Encoder(nn.Module):
             H, W = H // 2, W // 2
         else:
             h, H, W = _run_conv(cs[0], x, B, H, W, in_layout=NCHW, relu=True)
+        a1 = h
         h, H, W = _run_conv(cs[2], h, B, H, W, bf16, relu=True)
+        a2 = h
         # the only consumer of conv 4 is the stack, whose first op is ReLU (or, with an
         # empty stack, its final F.relu): fold that ReLU into this epilogue (Q2/Q3).
         h, H, W = _run_conv(cs[4], h, B, H, W, bf16, relu=True)
+        a3 = h
         h = cs[5]._apply_nhwc(h, B, H, W, bf16)
+        if acts is not None:
+            acts["enc"] = (a1, a2, a3, h)
         return h, B, H, W
 
     def forward(self, x):
@@ -305,12 +314,17 @@ class Decoder(nn.Module):
             nn.ConvTranspose2d(h_dim // 2, 3, kernel_size=kernel, stride=stride, padding=1),
         )
 
-    def _forward_from_nhwc(self, z, B, H, W, bf16=False):
-        """z: NHWC (B,H,W,in_dim), bf16 in the bf16 pipeline -> x_hat fp32 NCHW."""
+    def _forward_from_nhwc(self, z, B, H, W, bf16=False, acts=None):
+        """z: NHWC (B,H,W,in_dim), bf16 in the bf16 pipeline -> x_hat fp32 NCHW.  `acts` (a dict, training walk)
+        receives the stack's input and output and the last hidden activation as "dec"."""
         ics = self.inverse_conv_stack
         h, H, W = _run_conv(ics[0], z, B, H, W, bf16, relu=True)     # ReLU of the stack folded in (Q2/Q3)
+        d1 = h
         h = ics[1]._apply_nhwc(h, B, H, W, bf16)
+        d_out = h
         h, H, W = _run_conv(ics[2], h, B, H, W, bf16, relu=True)
+        if acts is not None:
+            acts["dec"] = (d1, d_out, h)
         return _run_conv(ics[4], h, B, H, W, bf16, out_layout=NCHW)[0]
 
     def forward(self, x):
@@ -410,6 +424,146 @@ class _PointwiseConv2d(nn.Conv2d):
         return _run_conv(self, x, B, H, W, in_layout=NCHW, out_layout=NCHW)[0]
 
 
+def _conv_dgrad(conv, g, B, H, W, prec, *, in_layout=NHWC, out_layout=NHWC, skip=None, out=None):
+    """Gradient of a conv container's input from `g`, the gradient of its (B, ., H, W) output: the adjoint conv
+    (Conv2d <-> ConvTranspose2d, same weight, stride and padding) on vqb_conv2d_f32, from the ("f32", not transposed)
+    packing, which is built the first time a backward needs it and refreshed by _packed like the forward's."""
+    transposed = isinstance(conv, nn.ConvTranspose2d)
+    kh, kw = conv.kernel_size
+    w = _packed(conv.weight, ("f32", not transposed))
+    return ops.conv2d(g, w, None, B=B, Cin=conv.out_channels, H=H, W=W, Cout=conv.in_channels, kh=kh, kw=kw,
+                      stride=conv.stride[0], pad=conv.padding[0], transposed=not transposed, in_layout=in_layout,
+                      out_layout=out_layout, skip=skip, precision=prec, out=out)
+
+
+def _conv_wgrad(conv, x, g, B, H, W, grads, *, in_layout=NHWC, gout_layout=NHWC):
+    """grads[id(param)] = the weight (and bias) gradient of a conv container from its (B, ., H, W) input `x` and
+    its output gradient `g` (vqb_conv_wgrad_f32)."""
+    kh, kw = conv.kernel_size
+    dW = torch.empty(conv.weight.shape, dtype=torch.float32, device=g.device)
+    db = torch.empty(conv.bias.shape, dtype=torch.float32, device=g.device) if conv.bias is not None else None
+    ops.conv_wgrad(x, g, dW, db, B=B, Cin=conv.in_channels, H=H, W=W, Cout=conv.out_channels, kh=kh, kw=kw,
+                   stride=conv.stride[0], pad=conv.padding[0], transposed=isinstance(conv, nn.ConvTranspose2d),
+                   in_layout=in_layout, gout_layout=gout_layout)
+    grads[id(conv.weight)] = dW
+    if db is not None:
+        grads[id(conv.bias)] = db
+
+
+def _stack_backward(stack, g, r0, out, B, H, W, prec, grads):
+    """Gradient of a ResidualStack's input r0 = relu(x) (NHWC) from g, the gradient of its output `out`; the stack's
+    weight gradients go to `grads`.  Per application r' = relu(r + W2.m), m = relu(W1 (*) r), with t = g' [r' > 0]
+    and g_m = (W2^T t) [m > 0]:  dW2 += t (x) m,  dW1 += g_m (x) r,  g_r = t + W1^T (*) g_m  (Q2: every mask is taken
+    from a kept post-ReLU activation).  The one-launch forward keeps r_1 .. r_{n-1} and every m on chip: they are
+    recomputed here by the per-application entry points.  The applications of one layer (Q1: all of them in the
+    reference's stack) take consecutive slots of the n-image-batch buffers, so each of its weights gets ONE wgrad
+    call, a single fixed-order reduction over all its applications."""
+    layers = list(stack.stack)
+    n = len(layers)
+    if n == 0:
+        return g
+    first = {}
+    for i, l in enumerate(layers):
+        first.setdefault(id(l), i)
+    order = sorted(range(n), key=lambda i: (first[id(layers[i])], i))
+    slot = {i: s for s, i in enumerate(order)}
+    groups = []                                     # (layer, first slot, end slot)
+    for s, i in enumerate(order):
+        if groups and groups[-1][0] is layers[i]:
+            groups[-1][2] = s + 1
+        else:
+            groups.append([layers[i], s, s + 1])
+    c1 = layers[0].res_block[1]
+    C, Cmid = c1.in_channels, c1.out_channels
+    f32 = dict(dtype=torch.float32, device=g.device)
+    R = torch.empty((n, B, H, W, C), **f32)         # application inputs r_0 .. r_{n-1}
+    M = torch.empty((n, B, H, W, Cmid), **f32)      # m_i
+    T = torch.empty((n, B, H, W, C), **f32)         # t_i
+    GM = torch.empty((n, B, H, W, Cmid), **f32)     # g_m of each application
+    R[slot[0]].copy_(r0)
+    for i in range(n - 1):
+        w1, w2 = (_packed(layers[i].res_block[k].weight, ("f32", False)) for k in (1, 3))
+        ops.residual_layer(R[slot[i]], w1, w2, B=B, H=H, W=W, C=C, Cmid=Cmid, relu_out=True, precision=prec,
+                           out=R[slot[i + 1]])
+    for l, s0, s1 in groups:
+        ops.conv2d(R[s0:s1], _packed(l.res_block[1].weight, ("f32", False)), None, B=(s1 - s0) * B, Cin=C, H=H, W=W,
+                   Cout=Cmid, kh=3, kw=3, stride=1, pad=1, relu=True, precision=prec, out=M[s0:s1])
+    for i in reversed(range(n)):
+        s, l = slot[i], layers[i]
+        ops.relu_backward(g, out if i == n - 1 else R[slot[i + 1]], out=T[s])
+        ops.relu_backward(_conv_dgrad(l.res_block[3], T[s], B, H, W, prec), M[s], out=GM[s])
+        g = _conv_dgrad(l.res_block[1], GM[s], B, H, W, prec, skip=T[s])
+    for l, s0, s1 in groups:
+        _conv_wgrad(l.res_block[3], M[s0:s1], T[s0:s1], (s1 - s0) * B, H, W, grads)
+        _conv_wgrad(l.res_block[1], R[s0:s1], GM[s0:s1], (s1 - s0) * B, H, W, grads)
+    return g
+
+
+class _VQVAEFunction(torch.autograd.Function):
+    """VQVAE.forward in training mode: inputs are the model, the image and every parameter in ``parameters()`` order
+    (a shared ResidualLayer once).  The forward is the inference walk (fp32 activations; the bf16 mode runs the TF32
+    kernels) keeping the activations it already produces; the backward runs every input gradient on the forward conv
+    kernels (vqb_conv2d_f32 with the transposed flag flipped), every conv weight gradient on vqb_conv_wgrad_f32 and
+    the VQ step on vqb_vq_backward_f32, and returns one gradient per parameter."""
+
+    @staticmethod
+    def forward(ctx, model, x, *params):
+        acts = {}
+        embedding_loss, x_hat, perplexity = model._walk(x, False, acts)
+        ctx.model, ctx.acts, ctx.prec = model, acts, _conv_precision()
+        # saved so that autograd raises, as it does for the reference, when the image or a parameter is modified in
+        # place between this forward and its backward (the backward reads the weights as they are then)
+        ctx.save_for_backward(x, *params)
+        ctx.mark_non_differentiable(perplexity)
+        return embedding_loss, x_hat, perplexity
+
+    @staticmethod
+    def backward(ctx, g_loss, g_xhat, _g_perp):
+        if ctx.acts is None:            # the first backward freed the saved activations
+            raise RuntimeError("VQVAE: backward through the same forward twice is not supported "
+                               "(its saved activations are freed by the first backward)")
+        ctx.saved_tensors                 # autograd's check that nothing saved was modified in place
+        model, a, prec = ctx.model, ctx.acts, ctx.prec
+        ctx.acts = None
+        enc, dec = model.encoder.conv_stack, model.decoder.inverse_conv_stack
+        vq = model.vector_quantization
+        x = a["x"]
+        B, _, H0, W0 = x.shape
+        H1, W1, H2, W2 = H0 // 2, W0 // 2, H0 // 4, W0 // 4
+        a1, a2, a3, e_out = a["enc"]
+        d1, d_out, d2 = a["dec"]
+        grads = {}
+        gx = ops._f32c(g_xhat)
+        # decoder, last layer first: convT 4 (NCHW out), ReLU, convT 2, the stack, convT 0 (its ReLU folded in)
+        _conv_wgrad(dec[4], d2, gx, B, H1, W1, grads, gout_layout=NCHW)
+        g = ops.relu_backward(_conv_dgrad(dec[4], gx, B, H0, W0, prec, in_layout=NCHW), d2)
+        _conv_wgrad(dec[2], d_out, g, B, H2, W2, grads)
+        g = _conv_dgrad(dec[2], g, B, H1, W1, prec)
+        g = _stack_backward(dec[1], g, d1, d_out, B, H2, W2, prec, grads)
+        g = ops.relu_backward(g, d1, out=g)
+        _conv_wgrad(dec[0], a["zq"], g, B, H2, W2, grads)
+        g = _conv_dgrad(dec[0], g, B, H2, W2, prec)
+        # the VQ step: straight-through to z_e plus the loss terms; the codebook gradient (float atomics)
+        dz, dE = ops.vq_backward(g.view(-1, vq.e_dim), g_loss, a["z_e"], a["codebook"], a["idx"], float(vq.beta))
+        grads[id(vq.embedding.weight)] = dE
+        pq = model.pre_quantization_conv
+        _conv_wgrad(pq, e_out, dz, B, H2, W2, grads)
+        g = _conv_dgrad(pq, dz, B, H2, W2, prec)
+        # encoder: the stack, then convs 4, 2, 0, each followed by a ReLU
+        g = _stack_backward(enc[5], g, a3, e_out, B, H2, W2, prec, grads)
+        g = ops.relu_backward(g, a3, out=g)
+        _conv_wgrad(enc[4], a2, g, B, H2, W2, grads)
+        g = _conv_dgrad(enc[4], g, B, H2, W2, prec)
+        g = ops.relu_backward(g, a2, out=g)
+        _conv_wgrad(enc[2], a1, g, B, H1, W1, grads)
+        g = _conv_dgrad(enc[2], g, B, H2, W2, prec)
+        g = ops.relu_backward(g, a1, out=g)
+        _conv_wgrad(enc[0], x, g, B, H0, W0, grads, in_layout=NCHW)
+        dx = _conv_dgrad(enc[0], g, B, H1, W1, prec, out_layout=NCHW) if ctx.needs_input_grad[1] else None
+        params = list(model.parameters())
+        return (None, dx) + tuple(grads[id(p)].to(p.dtype) for p in params)
+
+
 class VQVAE(nn.Module):
     """models/vqvae.py:10-44."""
 
@@ -466,18 +620,45 @@ class VQVAE(nn.Module):
         return all(ops.lib().vqb_conv_bf16_packed_bytes(key[1], c.out_channels, c.in_channels) != 0
                    for c, key in keys if key[0] == "bf16")
 
-    def _encode_rows(self, x, bf16=False):
+    def _encode_rows(self, x, bf16=False, acts=None):
         x = _prep_input(x, 3, "VQVAE")
         if x.shape[2] % 4 or x.shape[3] % 4:
             raise RuntimeError("VQVAE: image height and width must be divisible by 4 (Q11)")
-        h, B, H, W = self.encoder._forward_nhwc(x, bf16)
+        if acts is not None:
+            acts["x"] = x
+        h, B, H, W = self.encoder._forward_nhwc(x, bf16, acts)
         # NHWC (B,H,W,D) rows, fp32 in every mode: they feed the exact VQ
         z_e = _run_conv(self.pre_quantization_conv, h, B, H, W, bf16, out_f32=True)[0]
         return z_e, B, H, W
 
+    def _trains(self, x):
+        """Whether forward(x) takes the differentiable path (see forward)."""
+        return self.training and torch.is_grad_enabled() and \
+            (x.requires_grad or any(p.requires_grad for p in self.parameters()))
+
     def forward(self, x, verbose=False):
-        bf16 = self._bf16_pipeline()
-        z_e, B, H, W = self._encode_rows(x, bf16)                            # vqvae.py:31-33
+        """vqvae.py:29-44 -> (embedding_loss, x_hat, perplexity).  In training mode with grad enabled and a parameter
+        (or x) requiring grad, the outputs are differentiable (_VQVAEFunction): the same launches, so the same values,
+        as the eval-mode forward, which records no autograd graph."""
+        if self._trains(x):
+            if self.process_group is not None:
+                raise RuntimeError("VQVAE: training with process_group set is not supported (the loss gradient of a "
+                                   "batch-sharded forward would need an all-reduce)")
+            embedding_loss, x_hat, perplexity = _VQVAEFunction.apply(self, x, *self.parameters())
+        else:
+            embedding_loss, x_hat, perplexity = self._walk(x, self._bf16_pipeline())
+        if verbose:                                                          # :38-42 (Q8)
+            B, _, H, W = x.shape
+            print('original data shape:', x.shape)
+            print('encoded data shape:', torch.Size((B, self.vector_quantization.e_dim, H // 4, W // 4)))
+            print('recon data shape:', x_hat.shape)
+            assert False
+        return embedding_loss, x_hat, perplexity
+
+    def _walk(self, x, bf16, acts=None):
+        """The forward's launches -> (embedding_loss, x_hat, perplexity).  `acts` (a dict) receives the tensors the
+        training backward reads."""
+        z_e, B, H, W = self._encode_rows(x, bf16, acts)                      # vqvae.py:31-33
         vq = self.vector_quantization
         D = vq.e_dim
         group = self.process_group
@@ -485,7 +666,8 @@ class VQVAE(nn.Module):
         # the batch-sharded all-reduce of (sse, hist) (SURVEY 8e) and the scalar finisher run on a side stream
         # and overlap the decoder; fork/join with events, so the whole forward stays capturable in one CUDA graph.
         n_rows = z_e.shape[0] * H * W
-        idx, zq, sse, hist = ops.vq_forward(z_e.view(-1, D), vq._codebook(),
+        codebook = vq._codebook()
+        idx, zq, sse, hist = ops.vq_forward(z_e.view(-1, D), codebook,
                                             zq_dtype=torch.bfloat16 if bf16 else torch.float32)
         main = torch.cuda.current_stream()
         if self._side_stream is None or self._side_stream.device != z_e.device:
@@ -498,7 +680,7 @@ class VQVAE(nn.Module):
             if not torch.cuda.is_current_stream_capturing():
                 for t in (sse, hist, embedding_loss, perplexity):
                     t.record_stream(side)
-        x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16)  # :36
+        x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16, acts)  # :36
         main.wait_stream(side)
         if not torch.cuda.is_current_stream_capturing():
             # the two scalars were allocated in the side stream's pool and are consumed on the caller's stream: without this
@@ -506,11 +688,8 @@ class VQVAE(nn.Module):
             embedding_loss.record_stream(main)
             perplexity.record_stream(main)
         self.last_min_encoding_indices = idx.view(-1, 1)
-        if verbose:                                                          # :38-42 (Q8)
-            print('original data shape:', x.shape)
-            print('encoded data shape:', torch.Size((B, D, H, W)))
-            print('recon data shape:', x_hat.shape)
-            assert False
+        if acts is not None:
+            acts.update(z_e=z_e.view(-1, D), codebook=codebook, idx=idx, zq=zq)
         return embedding_loss, x_hat, perplexity
 
     def reduce_scalars(self):
@@ -524,11 +703,15 @@ class VQVAE(nn.Module):
 
     def repack(self):
         """Refresh every cached weight packing whose parameter changed (load_state_dict, optimizer step), IN PLACE
-        in the buffers earlier forwards -- and CUDA graphs captured around them -- already read.  A plain forward
-        does this by itself; HostPipeline calls it before replaying a captured graph."""
+        in the buffers earlier forwards -- and CUDA graphs captured around them -- already read: the forward's, and
+        the input-gradient packing of a training backward once one exists.  A plain forward (backward) does this by
+        itself; HostPipeline calls it before replaying a captured graph."""
         bf16 = self._bf16_pipeline()
         for conv in _convs(self):
-            _packed(conv.weight, _pack_key(conv, bf16))
+            fwd = _pack_key(conv, bf16)
+            _packed(conv.weight, fwd)
+            for key in [k for k in getattr(conv.weight, "_vqb_packed", {}) if k[0] == "f32" and k != fwd]:
+                _packed(conv.weight, key)           # a training backward's input-gradient packing, once it exists
 
     # ---- SURVEY 8(f) rank 1: the two halves callers use around the path ----------
     def encode(self, x):

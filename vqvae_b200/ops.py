@@ -84,16 +84,18 @@ def conv_out_hw(h, w, kh, kw, stride, pad, transposed):
 
 
 def conv2d(x, w_packed, bias, *, B, Cin, H, W, Cout, kh, kw, stride, pad, transposed=False,
-           in_layout=NHWC, out_layout=NHWC, relu=False, skip=None, precision=FP32):
+           in_layout=NHWC, out_layout=NHWC, relu=False, skip=None, precision=FP32, out=None):
     """One nn.Conv2d / nn.ConvTranspose2d forward (+bias, +skip, +ReLU) on raw buffers.
     `x` is any contiguous CUDA fp32 tensor holding the (B,Cin,H,W) activation in
-    `in_layout`; returns a new tensor in `out_layout` ((B,Cout,OH,OW) or (B,OH,OW,Cout))."""
+    `in_layout`; returns a new tensor in `out_layout` ((B,Cout,OH,OW) or (B,OH,OW,Cout)), or writes `out`
+    (a contiguous fp32 tensor of that many elements) when given."""
     _require_cuda(x, "input")
     oh, ow = conv_out_hw(H, W, kh, kw, stride, pad, transposed)
     if oh <= 0 or ow <= 0:
         raise RuntimeError(f"conv output size is non-positive ({oh}x{ow})")
     shape = (B, Cout, oh, ow) if out_layout == NCHW else (B, oh, ow, Cout)
-    out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
     span = _Span(f"conv{'T' if transposed else ''} {Cin}->{Cout} k{kh}s{stride} {H}x{W}"
                  f"{' +skip' if skip is not None else ''}")
     check(lib().vqb_conv2d_f32(
@@ -184,10 +186,11 @@ def residual_layer_bf16(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, relu_out):
     return out
 
 
-def residual_layer(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, relu_out, precision=FP32):
-    """out = act(r + W2.relu(W1 (*) r)) on NHWC buffers (vqb_residual_layer_f32)."""
+def residual_layer(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, relu_out, precision=FP32, out=None):
+    """out = act(r + W2.relu(W1 (*) r)) on NHWC buffers (vqb_residual_layer_f32), into `out` when given."""
     _require_cuda(r, "input")
-    out = torch.empty((B, H, W, C), dtype=torch.float32, device=r.device)
+    if out is None:
+        out = torch.empty((B, H, W, C), dtype=torch.float32, device=r.device)
     tmp = torch.empty((B, H, W, Cmid), dtype=torch.float32, device=r.device)
     span = _Span(f"res {C}->{Cmid}->{C} {H}x{W}")
     check(lib().vqb_residual_layer_f32(r.data_ptr(), w1_packed.data_ptr(), w2_packed.data_ptr(), out.data_ptr(),
@@ -299,6 +302,31 @@ def relu_(x):
     """In-place ReLU on a contiguous fp32 CUDA tensor (residual.py:19 side effect)."""
     check(lib().vqb_relu_f32(x.data_ptr(), x.numel(), _stream()), "relu_")
     return x
+
+
+def relu_backward(g, y, out=None):
+    """out = y > 0 ? g : 0 elementwise (vqb_relu_backward_f32); g, y contiguous fp32 of one size, `out` may be g."""
+    if out is None:
+        out = torch.empty_like(y)
+    check(lib().vqb_relu_backward_f32(g.data_ptr(), y.data_ptr(), out.data_ptr(), y.numel(), _stream()), "relu_backward")
+    return out
+
+
+def conv_wgrad(x, g_out, dW, dbias, *, B, Cin, H, W, Cout, kh, kw, stride, pad, transposed=False, in_layout=NHWC,
+               gout_layout=NHWC):
+    """Overwrite dW (the parameter's layout) and dbias (None: not computed) with the weight and bias gradient of one
+    conv layer from its input `x` and output gradient `g_out` (vqb_conv_wgrad_f32)."""
+    _require_cuda(x, "input")
+    n = lib().vqb_conv_wgrad_workspace_bytes(B, Cin, H, W, Cout, kh, kw, stride, pad, int(bool(transposed)))
+    if n == 0:
+        raise RuntimeError("conv_wgrad: bad geometry")
+    ws = torch.empty((n,), dtype=torch.uint8, device=x.device)
+    span = _Span(f"wgrad{'T' if transposed else ''} {Cin}->{Cout} k{kh}s{stride} {H}x{W} B={B}")
+    check(lib().vqb_conv_wgrad_f32(x.data_ptr(), g_out.data_ptr(), dW.data_ptr(),
+                                   dbias.data_ptr() if dbias is not None else None, B, Cin, H, W, Cout, kh, kw, stride,
+                                   pad, int(bool(transposed)), in_layout, gout_layout, ws.data_ptr(), n, _stream()),
+          "conv_wgrad")
+    span.done()
 
 
 VQ_KERNELS = {"auto": 0, "exact": 1, "tc": 2}
