@@ -63,15 +63,6 @@ extern "C" int vqb_device_info(int *sm_count, int *cc_major, int *cc_minor) {
     return 0;
 }
 
-static void set_strides(int layout, int C, int H, int W, long long &sn, long long &sh, long long &sw,
-                        long long &sc) {
-    if (layout == VQB_NCHW) {
-        sn = (long long)C * H * W; sc = (long long)H * W; sh = W; sw = 1;
-    } else {
-        sn = (long long)H * W * C; sh = (long long)W * C; sw = C; sc = 1;
-    }
-}
-
 extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const float *bias, const float *skip,
                               float *out, int B, int Cin, int H, int W, int Cout, int kh, int kw, int stride,
                               int pad, int transposed, int in_layout, int out_layout, int relu, int precision,
@@ -112,8 +103,8 @@ extern "C" int vqb_conv2d_f32(const float *in, const float *w_packed, const floa
     ConvLaunch p = {};
     p.in = in; p.w = w_packed; p.bias = bias; p.skip = skip; p.out = out;
     p.B = B; p.Cin = Cin; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu;
-    set_strides(in_layout, Cin, H, W, p.in_sn, p.in_sh, p.in_sw, p.in_sc);
-    set_strides(out_layout, Cout, g.OH, g.OW, p.out_sn, p.out_sh, p.out_sw, p.out_sc);
+    layout_strides(in_layout, Cin, H, W, p.in_sn, p.in_sh, p.in_sw, p.in_sc);
+    layout_strides(out_layout, Cout, g.OH, g.OW, p.out_sn, p.out_sh, p.out_sw, p.out_sc);
     auto run_ffma = [&](const ConvPhase &ph) {
         static_cast<ConvPhase &>(p) = ph;
         return Cout <= 4 ? launch_conv_small_cout(p, s) : launch_conv_ffma(p, s);

@@ -39,6 +39,16 @@ struct ConvPhase {
     int tap_w[VQB_MAX_TAPS], tap_dy[VQB_MAX_TAPS], tap_dx[VQB_MAX_TAPS];
 };
 
+// element strides (batch, row, column, channel) of a (B, C, H, W) activation stored in `layout` (VQB_NCHW or VQB_NHWC)
+static inline void layout_strides(int layout, int C, int H, int W, long long &sn, long long &sh, long long &sw,
+                                  long long &sc) {
+    if (layout == VQB_NCHW) {
+        sn = (long long)C * H * W; sc = (long long)H * W; sh = W; sw = 1;
+    } else {
+        sn = (long long)H * W * C; sh = (long long)W * C; sw = C; sc = 1;
+    }
+}
+
 ConvGeom conv_geom(int kh, int kw, int stride, int pad, int transposed, int H, int W);
 // phase i < g.nph of g; false when its output grid is empty
 bool conv_phase(const ConvGeom &g, int i, ConvPhase &ph);

@@ -7,21 +7,20 @@
 // Rows are X's channels and columns tap * Cy + cy, so the reduction writes dW in the parameter's own layout.  The bias
 // gradient sums g_out over its own grid: for a Conv2d it is a column of ones after the tap columns; a ConvTranspose2d
 // iterates over the input grid, so its bias is a second, one-column product with X = g_out.
-// Per CTA: a 64 x 64 tile of (rows x columns) over one chunk of positions, 16 positions per step staged in shared
-// memory (float4 loads along the channel dimension when it is contiguous), 4 x 4 outputs per thread, each one fmaf
-// chain in position order.  The chunk partials are summed in chunk order (wgrad_reduce.cuh): no atomics, so two calls
-// give bitwise-equal gradients.
-#include "wgrad_reduce.cuh"
+// The products run on the FFMA GEMM the prior's backward also uses (ffma_gemm.cuh), with X and the tap-shifted Y as
+// its operands: both stage four channels at a time with one float4 load when the channels are contiguous.  The
+// positions are split into fixed chunks whose partials are summed in chunk order: no atomics, so two calls give
+// bitwise-equal gradients.
+#include "ffma_gemm.cuh"
 
 namespace {
-
-constexpr int BM = 64, BN = 64, BK = 16, GT = 256;        // CTA tile, positions per step, threads (16 x 16, 4 x 4 each)
 
 struct Act {                       // a (B, C, H, W) activation addressed through element strides
     const float *p;
     int C, H, W;
     long long sn, sh, sw, sc;
     bool vec;                      // channels contiguous, C % 4 == 0, 16-byte aligned: float4 along the channels
+    __device__ __forceinline__ const float *at(long long b, int y, int x) const { return p + b * sn + y * sh + x * sw; }
 };
 
 struct Job {
@@ -33,129 +32,63 @@ struct Job {
     float *part;                   // [sp.splits][x.C][cols]
 };
 
-__device__ __forceinline__ void split_pos(long long p, int H, int W, long long &b, int &r, int &c) {
-    const long long hw = (long long)H * W;
-    b = p / hw;
-    const int rem = (int)(p - b * hw);
-    r = rem / W;
-    c = rem - r * W;
-}
-
-__global__ void __launch_bounds__(GT) wgrad_kernel(const Job J) {
-    __shared__ __align__(16) float Xs[BK][BM + 4];
-    __shared__ __align__(16) float Ys[BK][BN + 4];
-    const int tid = threadIdx.x, tm = tid / 16, tn = tid % 16;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-    const long long p_begin = (long long)blockIdx.z * J.sp.chunk;
-    const long long p_end = p_begin + J.sp.chunk < J.P ? p_begin + J.sp.chunk : J.P;
-    const Act &X = J.x, &Y = J.y;
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-    // Y's element (position p, column n): channel n % Cy of tap n / Cy at p's shifted position, or the ones column
-    auto y_at = [&](long long p, int n) -> float {
-        if (p >= p_end || n >= J.cols) return 0.f;
-        if (n >= J.ycols) return 1.f;
-        const int tap = n / Y.C, c = n - tap * Y.C, r = tap / J.kw, s = tap - r * J.kw;
-        long long b;
-        int oy, ox;
-        split_pos(p, X.H, X.W, b, oy, ox);
-        const int iy = oy * J.stride - J.pad + r, ix = ox * J.stride - J.pad + s;
-        if (iy < 0 || iy >= Y.H || ix < 0 || ix >= Y.W) return 0.f;
-        return __ldg(Y.p + b * Y.sn + iy * Y.sh + ix * Y.sw + c * Y.sc);
-    };
-
-    for (long long p0 = p_begin; p0 < p_end; p0 += BK) {
-        if (X.vec) {                                   // one float4 of channels per thread
-            const int kk = tid / 16, mm = (tid % 16) * 4, m = m0 + mm;
-            const long long p = p0 + kk;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p < p_end && m < X.C) {
-                long long b;
-                int yy, xx;
-                split_pos(p, X.H, X.W, b, yy, xx);
-                v = __ldg(reinterpret_cast<const float4 *>(X.p + b * X.sn + yy * X.sh + xx * X.sw + m));
-            }
-            *reinterpret_cast<float4 *>(&Xs[kk][mm]) = v;
-        } else {                                       // consecutive threads: consecutive addresses
-            const bool cfast = X.sc == 1;
-#pragma unroll
-            for (int q = 0; q < BM * BK / GT; ++q) {
-                const int e = tid + q * GT;
-                const int mm = cfast ? e % BM : e / BK, kk = cfast ? e / BM : e % BK, m = m0 + mm;
-                const long long p = p0 + kk;
-                float v = 0.f;
-                if (p < p_end && m < X.C) {
-                    long long b;
-                    int yy, xx;
-                    split_pos(p, X.H, X.W, b, yy, xx);
-                    v = __ldg(X.p + b * X.sn + yy * X.sh + xx * X.sw + m * X.sc);
-                }
-                Xs[kk][mm] = v;
-            }
-        }
-        if (Y.vec) {                                   // four consecutive columns of one tap per thread
-            const int kk = tid / 16, nn = (tid % 16) * 4, n = n0 + nn;
-            const long long p = p0 + kk;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (n + 3 < J.ycols) {
-                if (p < p_end) {
-                    const int tap = n / Y.C, c = n - tap * Y.C, r = tap / J.kw, s = tap - r * J.kw;
-                    long long b;
-                    int oy, ox;
-                    split_pos(p, X.H, X.W, b, oy, ox);
-                    const int iy = oy * J.stride - J.pad + r, ix = ox * J.stride - J.pad + s;
-                    if (iy >= 0 && iy < Y.H && ix >= 0 && ix < Y.W)
-                        v = __ldg(reinterpret_cast<const float4 *>(Y.p + b * Y.sn + iy * Y.sh + ix * Y.sw + c));
-                }
-            } else {
-                v = make_float4(y_at(p, n), y_at(p, n + 1), y_at(p, n + 2), y_at(p, n + 3));
-            }
-            *reinterpret_cast<float4 *>(&Ys[kk][nn]) = v;
-        } else {
-            const bool cfast = Y.sc == 1;
-#pragma unroll
-            for (int q = 0; q < BN * BK / GT; ++q) {
-                const int e = tid + q * GT;
-                const int nn = cfast ? e % BN : e / BK, kk = cfast ? e / BN : e % BK;
-                Ys[kk][nn] = y_at(p0 + kk, n0 + nn);
-            }
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < BK; ++kk) {
-            const float4 av = *reinterpret_cast<const float4 *>(&Xs[kk][tm * 4]);
-            const float4 bv = *reinterpret_cast<const float4 *>(&Ys[kk][tn * 4]);
-            const float ar[4] = {av.x, av.y, av.z, av.w}, br[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(ar[i], br[j], acc[i][j]);
-        }
-        __syncthreads();
+struct Pos {                       // position p of a (B, H, W) grid
+    long long b;
+    int y, x;
+    __device__ __forceinline__ Pos(long long p, int H, int W) {
+        const long long hw = (long long)H * W;
+        b = p / hw;
+        const int rem = (int)(p - b * hw);
+        y = rem / W;
+        x = rem - y * W;
     }
-    float *part = J.part + (long long)blockIdx.z * X.C * J.cols;
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int m = m0 + tm * 4 + i, n = n0 + tn * 4 + j;
-            if (m < X.C && n < J.cols) part[(long long)m * J.cols + n] = acc[i][j];
-        }
-}
+};
+
+// X as the A operand: row c = channel c, k = position p of X's grid
+struct XGrid {
+    Act x;
+    bool j_fast, vec;              // positions fast when the channels are not contiguous; vec: x.vec
+    __device__ __forceinline__ const float *at(long long p) const {
+        const Pos q(p, x.H, x.W);
+        return x.at(q.b, q.y, q.x);
+    }
+    __device__ __forceinline__ float operator()(int c, long long p) const { return __ldg(at(p) + c * x.sc); }
+    __device__ __forceinline__ float4 four(int c, long long p) const {
+        return __ldg(reinterpret_cast<const float4 *>(at(p) + c));
+    }
+};
+
+// Y at the taps as the B operand: k = position p = (b, oy, ox) of X's grid (H x W), column n = tap * C + c reads channel
+// c of Y at (oy * stride - pad + r, ox * stride - pad + s), tap = r * kw + s; 0 outside Y's grid
+struct YTap {
+    Act y;
+    int H, W, kw, stride, pad;
+    bool j_fast, vec;              // columns fast when the channels are contiguous; vec: y.vec (C % 4 == 0, so a group
+                                   // of four columns stays inside one tap)
+    // tap `tap` of position p in Y, or nullptr outside Y's grid
+    __device__ __forceinline__ const float *at(long long p, int tap) const {
+        const int r = tap / kw, s = tap - r * kw;
+        const Pos q(p, H, W);
+        const int iy = q.y * stride - pad + r, ix = q.x * stride - pad + s;
+        return iy < 0 || iy >= y.H || ix < 0 || ix >= y.W ? nullptr : y.at(q.b, iy, ix);
+    }
+    __device__ __forceinline__ float operator()(long long p, int n) const {
+        const int tap = n / y.C, c = n - tap * y.C;
+        const float *a = at(p, tap);
+        return a ? __ldg(a + c * y.sc) : 0.f;
+    }
+    __device__ __forceinline__ float4 four(long long p, int n) const {
+        const int tap = n / y.C, c = n - tap * y.C;
+        const float *a = at(p, tap);
+        return a ? __ldg(reinterpret_cast<const float4 *>(a + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+};
 
 // ---- host side ---------------------------------------------------------------------------------------------------
 Act act(const float *p, int layout, int C, int H, int W) {
     Act a;
     a.p = p; a.C = C; a.H = H; a.W = W;
-    if (layout == VQB_NCHW) {
-        a.sn = (long long)C * H * W; a.sc = (long long)H * W; a.sh = W; a.sw = 1;
-    } else {
-        a.sn = (long long)H * W * C; a.sh = (long long)W * C; a.sw = C; a.sc = 1;
-    }
+    layout_strides(layout, C, H, W, a.sn, a.sh, a.sw, a.sc);
     a.vec = a.sc == 1 && C % 4 == 0 && (reinterpret_cast<uintptr_t>(p) & 15) == 0;
     return a;
 }
@@ -235,8 +168,9 @@ extern "C" int vqb_conv_wgrad_f32(const float *in, const float *g_out, float *dW
         Job &j = jobs[i];
         j.part = part;
         part += job_floats(j);
-        const dim3 grid(wgrad_cdiv(j.x.C, BM), wgrad_cdiv(j.cols, BN), j.sp.splits);
-        wgrad_kernel<<<grid, GT, 0, st>>>(j);
+        const XGrid a{j.x, j.x.sc != 1, j.x.vec};
+        const WithOnes<YTap> b{YTap{j.y, j.x.H, j.x.W, j.kw, j.stride, j.pad, j.y.sc == 1, j.y.vec}, j.ycols};
+        gemm(st, a, b, Partial{j.part, j.x.C, j.cols}, j.x.C, j.cols, j.P, j.sp);
         // partial columns tap * Cy + cy -> dW[row][cy][tap]; the ones column -> dbias[row]
         rj.j[i] = RJob{j.part, dW, dbias, j.x.C, j.y.C, j.taps, j.cols, j.sp.splits};
         most = most > (long long)j.x.C * j.cols ? most : (long long)j.x.C * j.cols;

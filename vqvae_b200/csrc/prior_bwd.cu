@@ -1,22 +1,21 @@
 // prior_bwd.cu -- backward of the Gated PixelCNN prior (GatedPixelCNN.forward, pixelcnn/models.py:121-130), fp32 on
 // CUDA cores (sm_90a).
 //
-// Every gradient is a matrix product, run by one shared-memory tiled GEMM (`gemm_kernel`) whose operands are read
-// through small accessor structs: the activations the training forward saved (prior.cuh: Saved), NHWC grids read at a
-// tap's shifted position (im2col on the fly), the forward's packed weights, a one-hot of codes or labels.
+// Every gradient is a matrix product, run by the FFMA GEMM the conv weight gradients also use (ffma_gemm.cuh:
+// `gemm_kernel`).  This file gives it the prior's operands as accessor structs: the activations the training forward
+// saved (prior.cuh: Saved), NHWC grids read at a tap's shifted position (im2col on the fly), the forward's packed
+// weights, a one-hot of codes or labels; and the epilogues that apply the gates' and the ReLU's derivatives.
 //   dgrad: rows = positions, columns = input channels, reduction = kept taps x output channels
 //   wgrad: rows = output channels, columns = taps x input channels (+ a column of ones: the bias), reduction =
-//          positions, split into fixed chunks; the chunk partials are summed in chunk order by `reduce_kernel`, which
-//          also writes each gradient in its parameter's layout.
+//          positions, split into fixed chunks; the chunk partials are summed in chunk order by
+//          `wgrad_reduce_kernel`, which also writes each gradient in its parameter's layout.
 // Every output element is one fmaf chain in a fixed order and no float atomics are used, so the gradients are bitwise
 // reproducible.  Weight gradients cover all kh*kw taps, mask A's included (the reference convolves with the full,
 // zeroed weight, so autograd gives those taps a gradient); dgrad reads the taps the forward kept.
 #include "prior.cuh"
-#include "wgrad_reduce.cuh"
+#include "ffma_gemm.cuh"
 
 namespace {
-
-constexpr int BM = 64, BN = 64, BK = 16, GT = 256;       // CTA tile, k-step, threads (16 x 16, 4 x 4 outputs each)
 
 struct Grid {                     // position n of a (B, H, W) grid
     int H, W;
@@ -28,21 +27,7 @@ struct Grid {                     // position n of a (B, H, W) grid
     }
 };
 
-// ---- operand accessors: (i, j) -> float; j_fast: consecutive j are consecutive addresses -------------------------
-struct Mat {                      // p[i][j], row length ld
-    const float *p;
-    int ld;
-    static constexpr bool j_fast = true;
-    __device__ __forceinline__ float operator()(int i, int j) const { return __ldg(p + (long long)i * ld + j); }
-};
-
-struct MatT {                     // p[j][i]
-    const float *p;
-    int ld;
-    static constexpr bool j_fast = false;
-    __device__ __forceinline__ float operator()(int i, int j) const { return __ldg(p + (long long)j * ld + i); }
-};
-
+// ---- the prior's operand accessors (ffma_gemm.cuh: Mat, MatT, WithOnes) -----------------------------------------
 struct Nchw {                     // d_logits (B, K, H, W) as a (positions x K) matrix
     const float *p;
     int K, HW;
@@ -103,14 +88,6 @@ struct OneHot {                   // (m, n) -> 1 if the clamped index of positio
     int per, count;
     static constexpr bool j_fast = true;
     __device__ __forceinline__ float operator()(int m, int n) const { return clampi(idx[n / per], count) == m ? 1.f : 0.f; }
-};
-
-template <class L>
-struct WithOnes {                 // column `cols` of ones after the columns of b: the bias gradient's column
-    L b;
-    int cols;
-    static constexpr bool j_fast = L::j_fast;
-    __device__ __forceinline__ float operator()(int k, int n) const { return n < cols ? b(k, n) : 1.f; }
 };
 
 // ---- epilogues: (m, n, value) -----------------------------------------------------------------------------------
@@ -178,85 +155,15 @@ struct VertBack {
     }
 };
 
-struct Partial {                  // wgrad: chunk z's partial of element (m, n) of an (M x cols) gradient
-    float *part;
-    long long M, cols;
-    __device__ __forceinline__ void operator()(int m, int n, float v) const {
-        part[(long long)blockIdx.z * M * cols + (long long)m * cols + n] = v;
-    }
-};
-
-// ---- the GEMM: out(m, n) = sum over k in [z*chunk, min(K, (z+1)*chunk)) of A(m, k) * B(k, n), k ascending ----------
-template <class LA, class LB, class EP>
-__global__ void __launch_bounds__(GT) gemm_kernel(LA a, LB b, EP ep, int M, int N, int K, int chunk) {
-    __shared__ __align__(16) float As[BK][BM + 4];
-    __shared__ __align__(16) float Bs[BK][BN + 4];
-    const int tid = threadIdx.x, tm = tid / 16, tn = tid % 16;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-    const int k_begin = blockIdx.z * chunk, k_end = min(K, k_begin + chunk);
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-    for (int k0 = k_begin; k0 < k_end; k0 += BK) {
-#pragma unroll
-        for (int q = 0; q < BM * BK / GT; ++q) {
-            const int e = tid + q * GT;
-            const int mm = LA::j_fast ? e / BK : e % BM, kk = LA::j_fast ? e % BK : e / BM;
-            const int m = m0 + mm, k = k0 + kk;
-            As[kk][mm] = (m < M && k < k_end) ? a(m, k) : 0.f;
-        }
-#pragma unroll
-        for (int q = 0; q < BN * BK / GT; ++q) {
-            const int e = tid + q * GT;
-            const int nn = LB::j_fast ? e % BN : e / BK, kk = LB::j_fast ? e / BN : e % BK;
-            const int n = n0 + nn, k = k0 + kk;
-            Bs[kk][nn] = (n < N && k < k_end) ? b(k, n) : 0.f;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < BK; ++kk) {
-            const float4 av = *reinterpret_cast<const float4 *>(&As[kk][tm * 4]);
-            const float4 bv = *reinterpret_cast<const float4 *>(&Bs[kk][tn * 4]);
-            const float ar[4] = {av.x, av.y, av.z, av.w}, br[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(ar[i], br[j], acc[i][j]);
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int m = m0 + tm * 4 + i, n = n0 + tn * 4 + j;
-            if (m < M && n < N) ep(m, n, acc[i][j]);
-        }
-}
-
 // ---- host side ---------------------------------------------------------------------------------------------------
-int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
-
-using Split = WgradSplit;         // wgrad reduction over K positions: `splits` chunks of `chunk` positions
-
-Split wsplit(int M, int N, long long K) { return wgrad_split(M, N, K, BM, BN, BK); }
-
 template <class LA, class LB, class EP>
-void gemm(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K, Split sp) {
-    const dim3 grid(cdiv(M, BM), cdiv(N, BN), sp.splits);
-    gemm_kernel<LA, LB, EP><<<grid, GT, 0, st>>>(a, b, ep, M, N, K, sp.chunk);
-}
-
-template <class LA, class LB, class EP>
-void dgrad(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K) { gemm(st, a, b, ep, M, N, K, Split{1, K}); }
+void dgrad(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K) { gemm(st, a, b, ep, M, N, K, WgradSplit{1, K}); }
 
 // A wgrad job in the partial region: M x cols partials of a reduction over `npos` positions, at `off` floats.
 struct WJob {
     int M, Cin, taps;
     bool bias;
-    Split sp;
+    WgradSplit sp;
     long long off;
     int cols() const { return Cin * taps + (bias ? 1 : 0); }
     long long floats() const { return (long long)sp.splits * M * cols(); }
@@ -270,7 +177,7 @@ struct Phase {
     WJob &add(int M, int Cin, int taps, bool bias, long long npos) {
         WJob &j = job[n++];
         j.M = M; j.Cin = Cin; j.taps = taps; j.bias = bias;
-        j.sp = wsplit(M, j.cols(), npos);
+        j.sp = wgrad_split(M, j.cols(), npos, BM, BN, BK);
         j.off = floats;
         floats += j.floats();
         return j;
