@@ -355,6 +355,36 @@ int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *codes, const
                            const float *d_logits, const void *saved, const vqb_prior_grads *grads, void *workspace,
                            size_t workspace_bytes, void *stream);
 
+/* One layer and the gate on their own (GatedMaskedConv2d / GatedActivation called as modules).  The same rules as the
+ * net: fp32, no float atomics (two calls give bitwise-equal results), no host synchronisation, argument checks
+ * before any launch, and vqb_prior_layer_f32's shape limits.                                                    */
+/* GatedActivation's backward: x (outer, 2C, inner) and d_out (outer, C, inner) -> d_x (outer, 2C, inner).  One
+ * launch.                                                                                                        */
+int vqb_prior_gate_backward_f32(const float *x, const float *d_out, float *d_x, int64_t outer, int C, int64_t inner,
+                                void *stream);
+/* Bytes of a layer's `saved` on a (B, H, W) grid: 16*B*H*W*dim (0 = bad sizes).                                  */
+size_t vqb_prior_layer_train_saved_bytes(int B, int H, int W, int dim);
+/* vqb_prior_layer_f32 that also stores h_vert (bias included, class embedding not) and the horizontal gate's
+ * pre-activation in `saved`; vh is the same B*H*W*2*dim floats of scratch, free after the call.  out_v and out_h
+ * are bitwise vqb_prior_layer_f32's.  Two launches.                                                              */
+int vqb_prior_layer_forward_train_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                                      const int64_t *labels, int B, int H, int W, int dim, int n_classes,
+                                      float *out_v, float *out_h, float *vh, void *saved, size_t saved_bytes,
+                                      void *stream);
+/* Workspace of vqb_prior_layer_backward_f32 (0 = bad arguments).                                                 */
+size_t vqb_prior_layer_backward_workspace_bytes(const vqb_prior_layer_weights *layer, int B, int H, int W, int dim,
+                                                int n_classes);
+/* Gradients of one layer from d_out_v, d_out_h (B,H,W,dim) NHWC, the layer's inputs x_v, x_h and the `saved` of a
+ * vqb_prior_layer_forward_train_f32 call with the same layer and inputs: overwrites the nine gradients of `grads`
+ * (each in its parameter's layout, mask A's taps included) and d_x_v, d_x_h (B,H,W,dim) NHWC.  d_out_v == NULL is a
+ * zero gradient.  The body of one layer of vqb_prior_backward_f32, without layer 0's d_x_v + d_x_h fold (that is the
+ * net's embedding gradient): 10 launches.                                                                        */
+int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                                 const int64_t *labels, int B, int H, int W, int dim, int n_classes,
+                                 const float *d_out_v, const float *d_out_h, const void *saved,
+                                 const vqb_prior_layer_grads *grads, float *d_x_v, float *d_x_h, void *workspace,
+                                 size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -547,3 +547,34 @@ extern "C" int vqb_prior_forward_train_f32(const vqb_prior_net *net, const int64
     VQB_COUNT_LAUNCH(2 + 2 * n.L);
     return vqb_cuda_status(cudaGetLastError());
 }
+
+extern "C" size_t vqb_prior_layer_train_saved_bytes(int B, int H, int W, int dim) {
+    if (B <= 0 || H <= 0 || W <= 0 || dim <= 0) return 0;
+    return (size_t)LayerSaved{(long long)B * H * W, dim}.total() * sizeof(float);
+}
+
+// vqb_prior_layer_f32's two launches with the vertical and horizontal stores of the net's training forward switched
+// on: the same arithmetic, so bitwise the same outputs.
+extern "C" int vqb_prior_layer_forward_train_f32(const vqb_prior_layer_weights *layer, const float *x_v,
+                                                 const float *x_h, const int64_t *labels, int B, int H, int W, int dim,
+                                                 int n_classes, float *out_v, float *out_h, float *vh, void *saved,
+                                                 size_t saved_bytes, void *stream) {
+    if (!layer || !x_v || !x_h || !labels || !out_v || !out_h || !vh || !saved || B <= 0 || H <= 0 || W <= 0 || dim <= 0 ||
+        n_classes <= 0 || !layer_ok(*layer))
+        return VQB_ERR_BAD_ARG;
+    if (!dim_ok(dim)) return VQB_ERR_UNSUPPORTED;
+    if (saved_bytes < vqb_prior_layer_train_saved_bytes(B, H, W, dim)) return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *lab = reinterpret_cast<const long long *>(labels);
+    const long long n = (long long)B * H * W;
+    const LayerSaved sv{n, dim};
+    float *sp = static_cast<float *>(saved);
+    Act in_v{const_cast<float *>(x_v), H, dim}, in_h{const_cast<float *>(x_h), H, dim};
+    Act ov{out_v, H, dim}, oh{out_h, H, dim}, vha{vh, H, 2 * dim};
+    vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H,
+                                                 Act{sp + sv.hv(), H, 2 * dim});
+    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W,
+                                                  Act{sp + sv.ph(), H, 2 * dim});
+    VQB_COUNT_LAUNCH(2);
+    return vqb_cuda_status(cudaGetLastError());
+}

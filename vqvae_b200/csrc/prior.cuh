@@ -74,4 +74,13 @@ struct Saved {
     long long total() const { return hid() + N * HID; }
 };
 
+// What one layer's training forward (vqb_prior_layer_forward_train_f32) keeps, in floats, NHWC (2C) grids: hv and
+// ph as in Saved.
+struct LayerSaved {
+    long long N, C;
+    long long hv() const { return 0; }
+    long long ph() const { return 2 * N * C; }
+    long long total() const { return 4 * N * C; }
+};
+
 }  // namespace

@@ -195,14 +195,12 @@ Phase head_phase(const Net &n, long long npos) {
     return p;
 }
 
-Phase layer_phase(const Net &n, int l, long long npos) {
-    const vqb_prior_layer_weights &w = n.layer[l];
-    const int C = n.C;
+Phase layer_phase(const vqb_prior_layer_weights &w, int C, int NC, long long npos) {
     Phase p;
     p.add(C, C, 1, true, npos);
     p.add(2 * C, C, hcols(w), true, npos);
     p.add(2 * C, 2 * C, 1, true, npos);
-    p.add(n.NC, 2 * C, 1, false, npos);
+    p.add(NC, 2 * C, 1, false, npos);
     p.add(2 * C, C, vrows(w) * w.kernel, true, npos);
     return p;
 }
@@ -231,7 +229,7 @@ Bws bws_layout(const Net &n, long long npos) {
     const long long e = emb_phase(n, npos).floats;
     part = part > e ? part : e;
     for (int l = 0; l < n.L; ++l) {
-        const long long f = layer_phase(n, l, npos).floats;
+        const long long f = layer_phase(n.layer[l], n.C, n.NC, npos).floats;
         part = part > f ? part : f;
     }
     w.total = w.part + part;
@@ -249,15 +247,64 @@ void reduce(cudaStream_t st, const Phase &p, float *part, float *const (&w)[MAX_
     wgrad_reduce(st, jobs, p.n, most);
 }
 
+// One layer's backward: 10 launches.  xv, xh: the layer's inputs; hv, ph: h_vert and the horizontal gate's
+// pre-activation its training forward kept; ghi = d out_h, gvi = d out_v (nullptr: zero, as for the net's last
+// layer) -> gho = d x_h, gvo = d x_v (+ fold, the net's layer 0: x_v and x_h are both the embedding) and the nine
+// weight gradients of q.  work: 6 grids of scratch; part: the wgrad partials of layer_phase.
+void layer_backward(cudaStream_t st, const vqb_prior_layer_weights &w, const vqb_prior_layer_grads &q, int C, int NC,
+                    const long long *lab, Grid g, int npos, const float *xv, const float *xh, const float *hv,
+                    const float *ph, const float *ghi, const float *gvi, float *gho, float *gvo, const float *fold,
+                    float *work, float *part) {
+    const int C2 = 2 * C, half = w.kernel / 2, vr = vrows(w) - (w.mask_a ? 1 : 0), hc = hcols(w) - (w.mask_a ? 1 : 0);
+    const long long grid = (long long)npos * C;
+    float *dph = work, *dhv = dph + 2 * grid, *cls = dhv + 2 * grid;
+    const Phase p = layer_phase(w, C, NC, npos);
+    // out_h = horiz_resid(gate(pre_h)) [+ x_h]: d pre_h, then d x_h = [d out_h +] horiz_stack^T * d pre_h
+    dgrad(st, Mat{ghi, C}, WPacked{w.resid_w, C, C}, GateBack{dph, ph, C}, npos, C, C);
+    gemm(st, MatT{ghi, C}, WithOnes<Gated>{Gated{ph, C}, C}, Partial{part + p.job[0].off, C, C + 1}, C, C + 1,
+         npos, p.job[0].sp);
+    dgrad(st, Tap{dph, C2, hc, 0, half, -1, g}, WPacked{w.horiz_w, C, C2}, Store{gho, w.residual ? ghi : nullptr, C},
+          npos, C, hc * C2);
+    gemm(st, MatT{dph, C2}, WithOnes<Tap>{Tap{xh, C, hcols(w), 0, half, 1, g}, hcols(w) * C},
+         Partial{part + p.job[1].off, C2, p.job[1].cols()}, C2, p.job[1].cols(), npos, p.job[1].sp);
+    gemm(st, MatT{dph, C2}, WithOnes<Mat>{Mat{hv, C2}, C2}, Partial{part + p.job[2].off, C2, C2 + 1}, C2, C2 + 1,
+         npos, p.job[2].sp);
+    // d h_vert = W_v2h^T d pre_h + gate'(h_vert + class) * d out_v; class gradient; d x_v = vert_stack^T * d h_vert
+    dgrad(st, Mat{dph, C2}, WPacked{w.v2h_w, C2, C2},
+          VertBack{dhv, cls, hv, gvi, dph, w.class_emb, lab, C, g.H * g.W, NC}, npos, C2, C2);
+    gemm(st, OneHot{lab, g.H * g.W, NC}, Mat{cls, C2}, Partial{part + p.job[3].off, NC, C2}, NC, C2, npos,
+         p.job[3].sp);
+    gemm(st, MatT{dhv, C2}, WithOnes<Tap>{Tap{xv, C, w.kernel, half, half, 1, g}, vrows(w) * w.kernel * C},
+         Partial{part + p.job[4].off, C2, p.job[4].cols()}, C2, p.job[4].cols(), npos, p.job[4].sp);
+    dgrad(st, Tap{dhv, C2, w.kernel, half, half, -1, g}, WPacked{w.vert_w, C, C2}, Store{gvo, fold, C}, npos, C,
+          vr * w.kernel * C2);
+    reduce(st, p, part, {q.resid_w, q.horiz_w, q.v2h_w, q.class_emb, q.vert_w},
+           {q.resid_b, q.horiz_b, q.v2h_b, nullptr, q.vert_b});
+}
+
+// GatedActivation's backward: d x (outer, 2C, inner) from x and d out (outer, C, inner); one thread per output element
+__global__ void gate_backward_kernel(const float *__restrict__ x, const float *__restrict__ d_out,
+                                     float *__restrict__ d_x, long long outer, int C, long long inner) {
+    const long long total = outer * C * inner;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long o = i / ((long long)C * inner), rest = i % ((long long)C * inner);
+        const long long a = o * 2 * C * inner + rest, b = a + (long long)C * inner;
+        float da, dg;
+        gate_back(__ldg(x + a), __ldg(x + b), __ldg(d_out + i), da, dg);
+        d_x[a] = da;
+        d_x[b] = dg;
+    }
+}
+
+bool layer_grads_ok(const vqb_prior_layer_grads &q) {
+    return q.vert_w && q.vert_b && q.v2h_w && q.v2h_b && q.horiz_w && q.horiz_b && q.resid_w && q.resid_b && q.class_emb;
+}
+
 bool grads_ok(const vqb_prior_grads *g, int L) {
     if (!g || !g->layers || g->n_layers != L || !g->embedding || !g->out1_w || !g->out1_b || !g->out2_w || !g->out2_b)
         return false;
-    for (int l = 0; l < L; ++l) {
-        const vqb_prior_layer_grads &q = g->layers[l];
-        if (!q.vert_w || !q.vert_b || !q.v2h_w || !q.v2h_b || !q.horiz_w || !q.horiz_b || !q.resid_w || !q.resid_b ||
-            !q.class_emb)
-            return false;
-    }
+    for (int l = 0; l < L; ++l)
+        if (!layer_grads_ok(g->layers[l])) return false;
     return true;
 }
 
@@ -280,7 +327,7 @@ extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *c
         return VQB_ERR_BAD_ARG;
     if (workspace_bytes < vqb_prior_backward_workspace_bytes(net, B, H, W)) return VQB_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
-    const int npos = B * H * W, C = n.C, C2 = 2 * C, K = n.K;
+    const int npos = B * H * W, C = n.C, K = n.K;
     const long long grid = (long long)npos * C;
     const long long *lab = reinterpret_cast<const long long *>(labels);
     const Saved sv{npos, C, n.L};
@@ -310,36 +357,11 @@ extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *c
     // layers, last to first.  gh[cur] = d x_h^{l+1}, gv[cur] = d x_v^{l+1} (none for the last layer)
     int cur = 0;
     for (int l = n.L - 1; l >= 0; --l) {
-        const vqb_prior_layer_weights &w = n.layer[l];
-        const vqb_prior_layer_grads &q = grads->layers[l];
-        const int half = w.kernel / 2, vr = vrows(w) - (w.mask_a ? 1 : 0), hc = hcols(w) - (w.mask_a ? 1 : 0);
-        float *dph = ws + wl.work, *dhv = dph + 2 * grid, *cls = dhv + 2 * grid;
-        const float *ph = sp + sv.ph(l), *hv = sp + sv.hv(l), *xv = sp + sv.xv(l), *xh = sp + sv.xh(l);
-        const float *ghi = gh[cur], *gvi = l == n.L - 1 ? nullptr : gv[cur];
-        float *gho = gh[cur ^ 1], *gvo = gv[cur ^ 1];
-        const Phase p = layer_phase(n, l, npos);
-        // out_h = horiz_resid(gate(pre_h)) [+ x_h]: d pre_h, then d x_h = [d out_h +] horiz_stack^T * d pre_h
-        dgrad(st, Mat{ghi, C}, WPacked{w.resid_w, C, C}, GateBack{dph, ph, C}, npos, C, C);
-        gemm(st, MatT{ghi, C}, WithOnes<Gated>{Gated{ph, C}, C}, Partial{part + p.job[0].off, C, C + 1}, C, C + 1,
-             npos, p.job[0].sp);
-        dgrad(st, Tap{dph, C2, hc, 0, half, -1, g}, WPacked{w.horiz_w, C, C2}, Store{gho, w.residual ? ghi : nullptr, C},
-              npos, C, hc * C2);
-        gemm(st, MatT{dph, C2}, WithOnes<Tap>{Tap{xh, C, hcols(w), 0, half, 1, g}, hcols(w) * C},
-             Partial{part + p.job[1].off, C2, p.job[1].cols()}, C2, p.job[1].cols(), npos, p.job[1].sp);
-        gemm(st, MatT{dph, C2}, WithOnes<Mat>{Mat{hv, C2}, C2}, Partial{part + p.job[2].off, C2, C2 + 1}, C2, C2 + 1,
-             npos, p.job[2].sp);
-        // d h_vert = W_v2h^T d pre_h + gate'(h_vert + class) * d x_v^{l+1}; class gradient; d x_v = vert_stack^T * d h_vert
-        dgrad(st, Mat{dph, C2}, WPacked{w.v2h_w, C2, C2},
-              VertBack{dhv, cls, hv, gvi, dph, w.class_emb, lab, C, H * W, n.NC}, npos, C2, C2);
-        gemm(st, OneHot{lab, H * W, n.NC}, Mat{cls, C2}, Partial{part + p.job[3].off, n.NC, C2}, n.NC, C2, npos,
-             p.job[3].sp);
-        gemm(st, MatT{dhv, C2}, WithOnes<Tap>{Tap{xv, C, w.kernel, half, half, 1, g}, vrows(w) * w.kernel * C},
-             Partial{part + p.job[4].off, C2, p.job[4].cols()}, C2, p.job[4].cols(), npos, p.job[4].sp);
+        float *gho = gh[cur ^ 1];
         // layer 0: x_v and x_h are both the embedding, so d x_v^0 + d x_h^0 is its gradient per position
-        dgrad(st, Tap{dhv, C2, w.kernel, half, half, -1, g}, WPacked{w.vert_w, C, C2},
-              Store{gvo, l == 0 ? gho : nullptr, C}, npos, C, vr * w.kernel * C2);
-        reduce(st, p, part, {q.resid_w, q.horiz_w, q.v2h_w, q.class_emb, q.vert_w},
-               {q.resid_b, q.horiz_b, q.v2h_b, nullptr, q.vert_b});
+        layer_backward(st, n.layer[l], grads->layers[l], C, n.NC, lab, g, npos, sp + sv.xv(l), sp + sv.xh(l),
+                       sp + sv.hv(l), sp + sv.ph(l), gh[cur], l == n.L - 1 ? nullptr : gv[cur], gho, gv[cur ^ 1],
+                       l == 0 ? gho : nullptr, ws + wl.work, part);
         launches += 10;
         cur ^= 1;
     }
@@ -352,5 +374,43 @@ extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *c
         launches += 2;
     }
     VQB_COUNT_LAUNCH(launches);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_prior_gate_backward_f32(const float *x, const float *d_out, float *d_x, int64_t outer, int C,
+                                          int64_t inner, void *stream) {
+    if (!x || !d_out || !d_x || outer <= 0 || C <= 0 || inner <= 0) return VQB_ERR_BAD_ARG;
+    gate_backward_kernel<<<grid_for(outer * C * inner), NT, 0, (cudaStream_t)stream>>>(x, d_out, d_x, outer, C, inner);
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+// workspace of one layer's backward: the 6 grids of layer_backward's scratch, then its wgrad partials
+extern "C" size_t vqb_prior_layer_backward_workspace_bytes(const vqb_prior_layer_weights *layer, int B, int H, int W,
+                                                           int dim, int n_classes) {
+    if (!layer || !layer_ok(*layer) || B <= 0 || H <= 0 || W <= 0 || n_classes <= 0 || !dim_ok(dim)) return 0;
+    const long long npos = (long long)B * H * W;
+    return (size_t)(6 * npos * dim + layer_phase(*layer, dim, n_classes, npos).floats) * sizeof(float);
+}
+
+extern "C" int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                                           const int64_t *labels, int B, int H, int W, int dim, int n_classes,
+                                           const float *d_out_v, const float *d_out_h, const void *saved,
+                                           const vqb_prior_layer_grads *grads, float *d_x_v, float *d_x_h,
+                                           void *workspace, size_t workspace_bytes, void *stream) {
+    if (!layer || !x_v || !x_h || !labels || !d_out_h || !saved || !grads || !d_x_v || !d_x_h || !workspace ||
+        B <= 0 || H <= 0 || W <= 0 || dim <= 0 || n_classes <= 0 || !layer_ok(*layer) || !layer_grads_ok(*grads))
+        return VQB_ERR_BAD_ARG;
+    if (!dim_ok(dim)) return VQB_ERR_UNSUPPORTED;
+    if (workspace_bytes < vqb_prior_layer_backward_workspace_bytes(layer, B, H, W, dim, n_classes))
+        return VQB_ERR_WORKSPACE;
+    const int npos = B * H * W;
+    const LayerSaved sv{npos, dim};
+    const float *sp = static_cast<const float *>(saved);
+    float *ws = static_cast<float *>(workspace);
+    layer_backward((cudaStream_t)stream, *layer, *grads, dim, n_classes, reinterpret_cast<const long long *>(labels),
+                   Grid{H, W}, npos, x_v, x_h, sp + sv.hv(), sp + sv.ph(), d_out_h, d_out_v, d_x_h, d_x_v, nullptr, ws,
+                   ws + 6LL * npos * dim);
+    VQB_COUNT_LAUNCH(10);
     return vqb_cuda_status(cudaGetLastError());
 }

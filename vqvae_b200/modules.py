@@ -8,9 +8,11 @@ are kept ONLY as parameter containers (identical init order => identical weights
 the same torch seed, identical ``state_dict()``); their own ``forward`` is never used.
 Every ``forward`` here launches the hand-written sm_90a kernels through the C ABI
 (``include/vqvae_b200.h``).  ``VQVAE.forward`` is differentiable in training mode (``_VQVAEFunction``: model.train(),
-grad enabled, a parameter or the image requiring grad), so the reference's ``main.py`` loop runs unchanged; in eval
-mode, under no_grad, and for the piecewise sub-module calls the outputs carry no autograd graph (unlike the
-reference, whose eval-mode outputs do).
+grad enabled, a parameter or the image requiring grad), so the reference's ``main.py`` loop runs unchanged.  The
+sub-modules (Encoder, Decoder, ResidualStack, ResidualLayer, the pre-quantization conv) follow the same rule when
+called on their own, each through its own autograd Function whose backward is its slice of _VQVAEFunction.backward,
+so notebook-style piecewise walks train too.  In eval mode and under no_grad the outputs carry no autograd graph
+(unlike the reference, whose eval-mode outputs do).
 
 Reference semantics reproduced on purpose (SURVEY 3.3):
   Q1  ResidualStack applies ONE shared ResidualLayer n times (residual.py:44-45)
@@ -171,12 +173,23 @@ def _run_conv(conv, x, B, H, W, bf16=False, *, in_layout=NHWC, out_layout=NHWC, 
     return (y,) + ops.conv_out_hw(H, W, kh, kw, stride, pad, isinstance(conv, nn.ConvTranspose2d))
 
 
-def _prep_input(x, channels, what):
+def _trains(module, *inputs):
+    """Whether a call of `module` on `inputs` takes the differentiable path: training mode, grad enabled, and an input
+    or one of the module's parameters requiring grad (VQVAE.forward's rule, for every module of the family)."""
+    return module.training and torch.is_grad_enabled() and \
+        (any(x.requires_grad for x in inputs) or any(p.requires_grad for p in module.parameters()))
+
+
+def _check_input(x, channels, what):
     if x.dim() != 4:
         raise RuntimeError(f"{what}: expected a 4-D (B,C,H,W) tensor, got {tuple(x.shape)}")
     if x.shape[1] != channels:
         raise RuntimeError(f"{what}: expected {channels} input channels, got {x.shape[1]}")
     ops._require_cuda(x, what + " input")
+
+
+def _prep_input(x, channels, what):
+    _check_input(x, channels, what)
     x = x.detach()
     if x.dtype != torch.float32:
         x = x.float()
@@ -220,6 +233,8 @@ class ResidualLayer(nn.Module):
                                   precision=_conv_precision())
 
     def forward(self, x):
+        if _trains(self, x):
+            return _residual_train(self, [self], x, self.res_block[1].in_channels, "ResidualLayer")
         r, B, H, W = _prep_relu_input(x, self.res_block[1].in_channels, "ResidualLayer")
         return ops.nhwc_to_nchw(self._apply_nhwc(r, B, H, W, relu_out=False))
 
@@ -250,6 +265,8 @@ class ResidualStack(nn.Module):
 
     def forward(self, x):
         ch = self.stack[0].res_block[1].in_channels if len(self.stack) else x.shape[1]
+        if _trains(self, x):
+            return _residual_train(self, list(self.stack), x, ch, "ResidualStack")
         # an empty stack has no in-place ReLU: only its final F.relu, on a copy
         r, B, H, W = _prep_relu_input(x, ch, "ResidualStack", in_place=len(self.stack) > 0)
         return ops.nhwc_to_nchw(self._apply_nhwc(r, B, H, W))
@@ -295,6 +312,13 @@ class Encoder(nn.Module):
         return h, B, H, W
 
     def forward(self, x):
+        if _trains(self, x):
+            if x.dim() == 4 and (x.shape[2] % 4 or x.shape[3] % 4):
+                # the input gradients run the adjoint convs, which map the 2x-strided grids back onto exactly twice
+                # their size: an image side that is not a multiple of 4 has rows no adjoint reaches (Q11)
+                raise RuntimeError("Encoder: training needs an image height and width divisible by 4 (Q11); the "
+                                   "inference call (model.eval() or torch.no_grad()) takes any size")
+            return _EncoderFunction.apply(self, x, *self.parameters())
         x = _prep_input(x, self.conv_stack[0].in_channels, "Encoder")
         h, _, _, _ = self._forward_nhwc(x)
         return ops.nhwc_to_nchw(h)
@@ -328,6 +352,8 @@ class Decoder(nn.Module):
         return _run_conv(ics[4], h, B, H, W, bf16, out_layout=NCHW)[0]
 
     def forward(self, x):
+        if _trains(self, x):
+            return _DecoderFunction.apply(self, x, *self.parameters())
         x = _prep_input(x, self.inverse_conv_stack[0].in_channels, "Decoder")
         B, _, H, W = x.shape
         return self._forward_from_nhwc(ops.nchw_to_nhwc(x), B, H, W)
@@ -419,6 +445,8 @@ class _PointwiseConv2d(nn.Conv2d):
     """nn.Conv2d container whose forward runs vqb_conv2d_f32 (vqvae.py:16-17,33)."""
 
     def forward(self, x):
+        if _trains(self, x):
+            return _PointwiseFunction.apply(self, x, *self.parameters())
         x = _prep_input(x, self.in_channels, "pre_quantization_conv")
         B, _, H, W = x.shape
         return _run_conv(self, x, B, H, W, in_layout=NCHW, out_layout=NCHW)[0]
@@ -450,15 +478,15 @@ def _conv_wgrad(conv, x, g, B, H, W, grads, *, in_layout=NHWC, gout_layout=NHWC)
         grads[id(conv.bias)] = db
 
 
-def _stack_backward(stack, g, r0, out, B, H, W, prec, grads):
-    """Gradient of a ResidualStack's input r0 = relu(x) (NHWC) from g, the gradient of its output `out`; the stack's
-    weight gradients go to `grads`.  Per application r' = relu(r + W2.m), m = relu(W1 (*) r), with t = g' [r' > 0]
+def _stack_backward(layers, g, r0, out, B, H, W, prec, grads, relu_out=True):
+    """Gradient of a ResidualStack's input r0 = relu(x) (NHWC) from g, the gradient of its output `out`; the weight
+    gradients of its `layers` (the stack's list, or [layer] for a lone ResidualLayer, whose output has no final ReLU:
+    `relu_out` False) go to `grads`.  Per application r' = relu(r + W2.m), m = relu(W1 (*) r), with t = g' [r' > 0]
     and g_m = (W2^T t) [m > 0]:  dW2 += t (x) m,  dW1 += g_m (x) r,  g_r = t + W1^T (*) g_m  (Q2: every mask is taken
     from a kept post-ReLU activation).  The one-launch forward keeps r_1 .. r_{n-1} and every m on chip: they are
     recomputed here by the per-application entry points.  The applications of one layer (Q1: all of them in the
     reference's stack) take consecutive slots of the n-image-batch buffers, so each of its weights gets ONE wgrad
     call, a single fixed-order reduction over all its applications."""
-    layers = list(stack.stack)
     n = len(layers)
     if n == 0:
         return g
@@ -490,13 +518,213 @@ def _stack_backward(stack, g, r0, out, B, H, W, prec, grads):
                    Cout=Cmid, kh=3, kw=3, stride=1, pad=1, relu=True, precision=prec, out=M[s0:s1])
     for i in reversed(range(n)):
         s, l = slot[i], layers[i]
-        ops.relu_backward(g, out if i == n - 1 else R[slot[i + 1]], out=T[s])
+        if i == n - 1 and not relu_out:
+            T[s].copy_(g)
+        else:
+            ops.relu_backward(g, out if i == n - 1 else R[slot[i + 1]], out=T[s])
         ops.relu_backward(_conv_dgrad(l.res_block[3], T[s], B, H, W, prec), M[s], out=GM[s])
         g = _conv_dgrad(l.res_block[1], GM[s], B, H, W, prec, skip=T[s])
     for l, s0, s1 in groups:
         _conv_wgrad(l.res_block[3], M[s0:s1], T[s0:s1], (s1 - s0) * B, H, W, grads)
         _conv_wgrad(l.res_block[1], R[s0:s1], GM[s0:s1], (s1 - s0) * B, H, W, grads)
     return g
+
+
+def _decoder_backward(dec, gx, z, acts, B, H, W, prec, grads, out_layout=NHWC, need_dz=True):
+    """Gradient of a Decoder's (B, H, W) latent input z (NHWC) from gx, the fp32 NCHW gradient of its output, with the
+    activations `acts` ("dec") its training walk kept; weight gradients go to `grads`.  The input gradient is
+    returned in `out_layout` (None unless `need_dz`)."""
+    ics = dec.inverse_conv_stack
+    d1, d_out, d2 = acts
+    H1, W1 = 2 * H, 2 * W
+    # last layer first: convT 4 (NCHW out), ReLU, convT 2, the stack, convT 0 (its ReLU folded in)
+    _conv_wgrad(ics[4], d2, gx, B, H1, W1, grads, gout_layout=NCHW)
+    g = ops.relu_backward(_conv_dgrad(ics[4], gx, B, 2 * H1, 2 * W1, prec, in_layout=NCHW), d2)
+    _conv_wgrad(ics[2], d_out, g, B, H, W, grads)
+    g = _conv_dgrad(ics[2], g, B, H1, W1, prec)
+    g = _stack_backward(list(ics[1].stack), g, d1, d_out, B, H, W, prec, grads)
+    g = ops.relu_backward(g, d1, out=g)
+    _conv_wgrad(ics[0], z, g, B, H, W, grads)
+    return _conv_dgrad(ics[0], g, B, H, W, prec, out_layout=out_layout) if need_dz else None
+
+
+def _encoder_backward(enc, g, x, acts, prec, grads, need_dx):
+    """Gradient of an Encoder's image x (fp32 NCHW; None unless `need_dx`) from g, the NHWC gradient of its output,
+    with the activations `acts` ("enc") its training walk kept; weight gradients go to `grads`."""
+    cs = enc.conv_stack
+    a1, a2, a3, e_out = acts
+    B, _, H0, W0 = x.shape
+    if H0 % 4 or W0 % 4:                # the adjoints of the two strided convs map back onto exactly 2x their grids
+        raise RuntimeError("Encoder: the backward needs an image height and width divisible by 4 (Q11)")
+    H1, W1, H2, W2 = H0 // 2, W0 // 2, H0 // 4, W0 // 4
+    # the stack, then convs 4, 2, 0, each followed by a ReLU
+    g = _stack_backward(list(cs[5].stack), g, a3, e_out, B, H2, W2, prec, grads)
+    g = ops.relu_backward(g, a3, out=g)
+    _conv_wgrad(cs[4], a2, g, B, H2, W2, grads)
+    g = _conv_dgrad(cs[4], g, B, H2, W2, prec)
+    g = ops.relu_backward(g, a2, out=g)
+    _conv_wgrad(cs[2], a1, g, B, H1, W1, grads)
+    g = _conv_dgrad(cs[2], g, B, H2, W2, prec)
+    g = ops.relu_backward(g, a1, out=g)
+    _conv_wgrad(cs[0], x, g, B, H0, W0, grads, in_layout=NCHW)
+    return _conv_dgrad(cs[0], g, B, H1, W1, prec, out_layout=NCHW) if need_dx else None
+
+
+def _param_grads(module, grads):
+    """One gradient per parameter of `module`, in ``parameters()`` order and each parameter's dtype."""
+    return tuple(grads[id(p)].to(p.dtype) for p in module.parameters())
+
+
+class _ModuleFunction(torch.autograd.Function):
+    """What the sub-module Functions share: inputs are the module, its input and its parameters; the forward keeps its
+    saved activations on ctx (``ctx.acts``) and saves the input and parameters so that autograd raises, as for the
+    reference, when one is modified in place before the backward; a second backward raises."""
+
+    @staticmethod
+    def _open(ctx, what):
+        if ctx.acts is None:
+            raise RuntimeError(f"{what}: backward through the same forward twice is not supported "
+                               "(its saved activations are freed by the first backward)")
+        ctx.saved_tensors                 # autograd's check that nothing saved was modified in place
+        acts, ctx.acts = ctx.acts, None
+        return acts
+
+
+class _EncoderFunction(_ModuleFunction):
+    """Encoder.forward in training mode: the inference walk keeping a1, a2, a3 and the stack output."""
+
+    @staticmethod
+    def forward(ctx, enc, x, *params):
+        xp = _prep_input(x, enc.conv_stack[0].in_channels, "Encoder")
+        acts = {}
+        h, _, _, _ = enc._forward_nhwc(xp, False, acts)
+        ctx.module, ctx.acts, ctx.prec = enc, (xp, acts["enc"]), _conv_precision()
+        ctx.save_for_backward(x, *params)
+        return ops.nhwc_to_nchw(h)
+
+    @staticmethod
+    def backward(ctx, g):
+        xp, acts = _ModuleFunction._open(ctx, "Encoder")
+        grads = {}
+        dx = _encoder_backward(ctx.module, ops.nchw_to_nhwc(g), xp, acts, ctx.prec, grads, ctx.needs_input_grad[1])
+        return (None, dx) + _param_grads(ctx.module, grads)
+
+
+class _DecoderFunction(_ModuleFunction):
+    """Decoder.forward in training mode: the inference walk keeping its NHWC input, d1, d_out and d2."""
+
+    @staticmethod
+    def forward(ctx, dec, x, *params):
+        xp = _prep_input(x, dec.inverse_conv_stack[0].in_channels, "Decoder")
+        B, _, H, W = xp.shape
+        z = ops.nchw_to_nhwc(xp)
+        acts = {}
+        y = dec._forward_from_nhwc(z, B, H, W, acts=acts)
+        ctx.module, ctx.acts, ctx.prec = dec, (z, acts["dec"]), _conv_precision()
+        ctx.save_for_backward(x, *params)
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        z, acts = _ModuleFunction._open(ctx, "Decoder")
+        B, H, W, _ = z.shape
+        grads = {}
+        dz = _decoder_backward(ctx.module, ops._f32c(g), z, acts, B, H, W, ctx.prec, grads, out_layout=NCHW,
+                               need_dz=ctx.needs_input_grad[1])
+        return (None, dz) + _param_grads(ctx.module, grads)
+
+
+class _PointwiseFunction(_ModuleFunction):
+    """The pre-quantization conv in training mode: one dgrad and one wgrad, NCHW on both sides."""
+
+    @staticmethod
+    def forward(ctx, conv, x, *params):
+        xp = _prep_input(x, conv.in_channels, "pre_quantization_conv")
+        B, _, H, W = xp.shape
+        ctx.module, ctx.acts, ctx.prec = conv, xp, _conv_precision()
+        ctx.save_for_backward(x, *params)
+        return _run_conv(conv, xp, B, H, W, in_layout=NCHW, out_layout=NCHW)[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        xp = _ModuleFunction._open(ctx, "pre_quantization_conv")
+        B, _, H, W = xp.shape
+        g = ops._f32c(g)
+        grads = {}
+        _conv_wgrad(ctx.module, xp, g, B, H, W, grads, in_layout=NCHW, gout_layout=NCHW)
+        dx = _conv_dgrad(ctx.module, g, B, H, W, ctx.prec, in_layout=NCHW, out_layout=NCHW) \
+            if ctx.needs_input_grad[1] else None
+        return (None, dx) + _param_grads(ctx.module, grads)
+
+
+class _ReluInPlace(torch.autograd.Function):
+    """Q2 under autograd: nn.ReLU(True) rewrites the caller's tensor and is recorded on it (mark_dirty bumps its
+    version and routes its gradient through the mask, as torch's relu_ does)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        if x.is_contiguous() and x.dtype == torch.float32:
+            ops.relu_(x)
+        else:
+            x.copy_(ops.relu_(ops._f32c(x.detach()).clone()))
+        ctx.mark_dirty(x)
+        ctx.save_for_backward(x)
+        return x
+
+    @staticmethod
+    def backward(ctx, g):
+        y, = ctx.saved_tensors
+        return ops.relu_backward(ops._f32c(g), ops._f32c(y))
+
+
+class _ReluFunction(torch.autograd.Function):
+    """An empty ResidualStack in training mode: its final F.relu, on a copy (vqb_relu_f32 / vqb_relu_backward_f32)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        y = ops.relu_(ops._f32c(x.detach()).clone())
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        y, = ctx.saved_tensors
+        return ops.relu_backward(ops._f32c(g), y)
+
+
+class _StackFunction(_ModuleFunction):
+    """A ResidualStack (or a lone ResidualLayer) in training mode on r = relu(x), already taken in place: the inference
+    launches keeping r (NHWC) and the output; the backward is _stack_backward."""
+
+    @staticmethod
+    def forward(ctx, module, layers, relu_out, r, *params):
+        B, _, H, W = r.shape
+        rn = ops.nchw_to_nhwc(r)
+        out = module._apply_nhwc(rn, B, H, W) if relu_out else module._apply_nhwc(rn, B, H, W, relu_out=False)
+        ctx.module, ctx.layers, ctx.relu_out, ctx.acts, ctx.prec = module, layers, relu_out, (rn, out), _conv_precision()
+        ctx.save_for_backward(r, *params)
+        return ops.nhwc_to_nchw(out)
+
+    @staticmethod
+    def backward(ctx, g):
+        rn, out = _ModuleFunction._open(ctx, type(ctx.module).__name__)
+        B, H, W, _ = rn.shape
+        grads = {}
+        dr = _stack_backward(ctx.layers, ops.nchw_to_nhwc(g), rn, out, B, H, W, ctx.prec, grads, ctx.relu_out)
+        return (None, None, None, ops.nhwc_to_nchw(dr) if ctx.needs_input_grad[3] else None) + \
+            _param_grads(ctx.module, grads)
+
+
+def _residual_train(module, layers, x, channels, what):
+    """The differentiable call of a ResidualStack (layers = its list) or a ResidualLayer (layers = [itself]): the
+    in-place ReLU on the caller's x (Q2), then _StackFunction; an empty stack is its final ReLU only."""
+    _check_input(x, channels, what)
+    if not layers:
+        return _ReluFunction.apply(x)
+    if x.is_leaf and x.requires_grad:       # torch's own check, before the caller's tensor is touched
+        raise RuntimeError("a leaf Variable that requires grad is being used in an in-place operation.")
+    r = _ReluInPlace.apply(x)
+    return _StackFunction.apply(module, layers, isinstance(module, ResidualStack), r, *module.parameters())
 
 
 class _VQVAEFunction(torch.autograd.Function):
@@ -525,41 +753,19 @@ class _VQVAEFunction(torch.autograd.Function):
         ctx.saved_tensors                 # autograd's check that nothing saved was modified in place
         model, a, prec = ctx.model, ctx.acts, ctx.prec
         ctx.acts = None
-        enc, dec = model.encoder.conv_stack, model.decoder.inverse_conv_stack
         vq = model.vector_quantization
         x = a["x"]
         B, _, H0, W0 = x.shape
-        H1, W1, H2, W2 = H0 // 2, W0 // 2, H0 // 4, W0 // 4
-        a1, a2, a3, e_out = a["enc"]
-        d1, d_out, d2 = a["dec"]
+        H2, W2 = H0 // 4, W0 // 4
         grads = {}
-        gx = ops._f32c(g_xhat)
-        # decoder, last layer first: convT 4 (NCHW out), ReLU, convT 2, the stack, convT 0 (its ReLU folded in)
-        _conv_wgrad(dec[4], d2, gx, B, H1, W1, grads, gout_layout=NCHW)
-        g = ops.relu_backward(_conv_dgrad(dec[4], gx, B, H0, W0, prec, in_layout=NCHW), d2)
-        _conv_wgrad(dec[2], d_out, g, B, H2, W2, grads)
-        g = _conv_dgrad(dec[2], g, B, H1, W1, prec)
-        g = _stack_backward(dec[1], g, d1, d_out, B, H2, W2, prec, grads)
-        g = ops.relu_backward(g, d1, out=g)
-        _conv_wgrad(dec[0], a["zq"], g, B, H2, W2, grads)
-        g = _conv_dgrad(dec[0], g, B, H2, W2, prec)
+        g = _decoder_backward(model.decoder, ops._f32c(g_xhat), a["zq"], a["dec"], B, H2, W2, prec, grads)
         # the VQ step: straight-through to z_e plus the loss terms; the codebook gradient (float atomics)
         dz, dE = ops.vq_backward(g.view(-1, vq.e_dim), g_loss, a["z_e"], a["codebook"], a["idx"], float(vq.beta))
         grads[id(vq.embedding.weight)] = dE
         pq = model.pre_quantization_conv
-        _conv_wgrad(pq, e_out, dz, B, H2, W2, grads)
+        _conv_wgrad(pq, a["enc"][3], dz, B, H2, W2, grads)
         g = _conv_dgrad(pq, dz, B, H2, W2, prec)
-        # encoder: the stack, then convs 4, 2, 0, each followed by a ReLU
-        g = _stack_backward(enc[5], g, a3, e_out, B, H2, W2, prec, grads)
-        g = ops.relu_backward(g, a3, out=g)
-        _conv_wgrad(enc[4], a2, g, B, H2, W2, grads)
-        g = _conv_dgrad(enc[4], g, B, H2, W2, prec)
-        g = ops.relu_backward(g, a2, out=g)
-        _conv_wgrad(enc[2], a1, g, B, H1, W1, grads)
-        g = _conv_dgrad(enc[2], g, B, H2, W2, prec)
-        g = ops.relu_backward(g, a1, out=g)
-        _conv_wgrad(enc[0], x, g, B, H0, W0, grads, in_layout=NCHW)
-        dx = _conv_dgrad(enc[0], g, B, H1, W1, prec, out_layout=NCHW) if ctx.needs_input_grad[1] else None
+        dx = _encoder_backward(model.encoder, g, x, a["enc"], prec, grads, ctx.needs_input_grad[1])
         params = list(model.parameters())
         return (None, dx) + tuple(grads[id(p)].to(p.dtype) for p in params)
 
@@ -633,8 +839,7 @@ class VQVAE(nn.Module):
 
     def _trains(self, x):
         """Whether forward(x) takes the differentiable path (see forward)."""
-        return self.training and torch.is_grad_enabled() and \
-            (x.requires_grad or any(p.requires_grad for p in self.parameters()))
+        return _trains(self, x)
 
     def forward(self, x, verbose=False):
         """vqvae.py:29-44 -> (embedding_loss, x_hat, perplexity).  In training mode with grad enabled and a parameter

@@ -306,6 +306,8 @@ def relu_(x):
 
 def relu_backward(g, y, out=None):
     """out = y > 0 ? g : 0 elementwise (vqb_relu_backward_f32); g, y contiguous fp32 of one size, `out` may be g."""
+    if g.numel() != y.numel() or (out is not None and out.numel() != y.numel()):
+        raise RuntimeError(f"relu_backward: gradient {tuple(g.shape)} and activation {tuple(y.shape)} differ in size")
     if out is None:
         out = torch.empty_like(y)
     check(lib().vqb_relu_backward_f32(g.data_ptr(), y.data_ptr(), out.data_ptr(), y.numel(), _stream()), "relu_backward")
@@ -384,6 +386,18 @@ def prior_gate(x):
     return out
 
 
+def prior_gate_backward(x, d_out):
+    """d x of GatedActivation from its (B, 2C, ...) input and the (B, C, ...) gradient of its output
+    (vqb_prior_gate_backward_f32)."""
+    x, d_out = _f32c(x.detach()), _f32c(d_out)
+    c = x.shape[1] // 2
+    d_x = torch.empty_like(x)
+    if d_x.numel():
+        check(lib().vqb_prior_gate_backward_f32(x.data_ptr(), d_out.data_ptr(), d_x.data_ptr(), x.shape[0], c,
+                                                x[0, 0].numel(), _stream()), "prior_gate_backward")
+    return d_x
+
+
 def prior_layer(layer_w, x_v, x_h, labels, *, B, H, W, dim, n_classes):
     """One GatedMaskedConv2d on NHWC (B,H,W,dim) fp32 buffers -> (out_v, out_h) NHWC (vqb_prior_layer_f32)."""
     out_v = torch.empty((B, H, W, dim), dtype=torch.float32, device=x_v.device)
@@ -395,6 +409,45 @@ def prior_layer(layer_w, x_v, x_h, labels, *, B, H, W, dim, n_classes):
           "prior_layer")
     span.done()
     return out_v, out_h
+
+
+def prior_layer_forward_train(layer_w, x_v, x_h, labels, *, B, H, W, dim, n_classes):
+    """prior_layer that also keeps what its backward reads -> (out_v, out_h, saved), saved a uint8 buffer of
+    vqb_prior_layer_train_saved_bytes (vqb_prior_layer_forward_train_f32; the outputs are bitwise prior_layer's)."""
+    n = lib().vqb_prior_layer_train_saved_bytes(B, H, W, dim)
+    if n == 0:
+        raise RuntimeError("prior layer: bad sizes")
+    saved = torch.empty((n,), dtype=torch.uint8, device=x_v.device)
+    out_v = torch.empty((B, H, W, dim), dtype=torch.float32, device=x_v.device)
+    out_h = torch.empty_like(out_v)
+    vh = torch.empty((B, H, W, 2 * dim), dtype=torch.float32, device=x_v.device)
+    span = _Span(f"prior layer (train) dim={dim} {H}x{W}")
+    check(lib().vqb_prior_layer_forward_train_f32(_lib.C.byref(layer_w), x_v.data_ptr(), x_h.data_ptr(),
+                                                  labels.data_ptr(), B, H, W, dim, n_classes, out_v.data_ptr(),
+                                                  out_h.data_ptr(), vh.data_ptr(), saved.data_ptr(), saved.numel(),
+                                                  _stream()),
+          "prior_layer_forward_train")
+    span.done()
+    return out_v, out_h, saved
+
+
+def prior_layer_backward(layer_w, x_v, x_h, labels, d_out_v, d_out_h, saved, grads, *, B, H, W, dim, n_classes):
+    """One layer's gradients (vqb_prior_layer_backward_f32): the nine weight gradients into the tensors `grads` (a
+    PriorLayerGrads struct) points at -> (d_x_v, d_x_h) NHWC.  d_out_v None: a zero gradient."""
+    n = lib().vqb_prior_layer_backward_workspace_bytes(_lib.C.byref(layer_w), B, H, W, dim, n_classes)
+    if n == 0:
+        raise RuntimeError("prior layer backward: bad sizes")
+    ws = torch.empty((n,), dtype=torch.uint8, device=x_v.device)
+    d_x_v = torch.empty((B, H, W, dim), dtype=torch.float32, device=x_v.device)
+    d_x_h = torch.empty_like(d_x_v)
+    span = _Span(f"prior layer backward dim={dim} {H}x{W}")
+    check(lib().vqb_prior_layer_backward_f32(_lib.C.byref(layer_w), x_v.data_ptr(), x_h.data_ptr(), labels.data_ptr(),
+                                             B, H, W, dim, n_classes,
+                                             d_out_v.data_ptr() if d_out_v is not None else None, d_out_h.data_ptr(),
+                                             saved.data_ptr(), _lib.C.byref(grads), d_x_v.data_ptr(), d_x_h.data_ptr(),
+                                             ws.data_ptr(), n, _stream()), "prior_layer_backward")
+    span.done()
+    return d_x_v, d_x_h
 
 
 def _prior_workspace(net, B, H, W, dev):

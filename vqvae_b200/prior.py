@@ -10,7 +10,9 @@ whatever ``set_precision`` says.
 requires grad (``_PriorFunction``: the training forward keeps its activations, and the backward of
 ``csrc/prior_bwd.cu`` writes one gradient per parameter), so the reference's training loop runs unchanged.  Under
 ``torch.no_grad()`` it is the inference forward.  ``GatedMaskedConv2d`` and ``GatedActivation`` called on their own
-are inference only: their outputs carry no autograd graph.
+are differentiable too, under the same rule (grad enabled and an input or a parameter requiring grad):
+``_GatedLayerFunction`` runs the layer's training forward and single-layer backward (vqb_prior_layer_*_f32),
+``_GateFunction`` the gate and its backward.  Their outputs are bitwise the inference call's.
 
 Reference behaviour kept on purpose:
   P2  ``self.apply(weights_init)``: Xavier-uniform conv weights, zero biases, and one "Skipping initialization of"
@@ -71,17 +73,41 @@ def _labels(label, B, dev, what):
     return label.to(torch.int64).contiguous()
 
 
+def _grad_call(inputs, module=None):
+    """Whether a prior module's call is differentiable (GatedPixelCNN's rule): grad enabled and an input, or a
+    parameter of `module`, requiring grad."""
+    return torch.is_grad_enabled() and (any(x.requires_grad for x in inputs) or
+                                        (module is not None and any(p.requires_grad for p in module.parameters())))
+
+
+class _GateFunction(torch.autograd.Function):
+    """GatedActivation with a gradient: vqb_prior_gate_f32 forward, vqb_prior_gate_backward_f32 backward."""
+
+    @staticmethod
+    def forward(ctx, x):
+        ctx.save_for_backward(x)
+        return ops.prior_gate(x)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        x, = ctx.saved_tensors
+        return ops.prior_gate_backward(x, d_out)
+
+
 class GatedActivation(nn.Module):
-    """tanh(first half of the channels) * sigmoid(second half) (models.py:20-26).  Inference only: the output carries
-    no autograd graph (GatedPixelCNN.forward is the differentiable entry point)."""
+    """tanh(first half of the channels) * sigmoid(second half) (models.py:20-26).  Differentiable when grad is enabled
+    and x requires grad (_GateFunction), else the inference call."""
 
     def forward(self, x):
+        if _grad_call([x]):
+            return _GateFunction.apply(x)
         return ops.prior_gate(x)
 
 
 class GatedMaskedConv2d(nn.Module):
-    """One gated layer with a vertical and a horizontal stack (models.py:29-86).  Called on its own it is inference
-    only: the outputs carry no autograd graph (GatedPixelCNN.forward is the differentiable entry point)."""
+    """One gated layer with a vertical and a horizontal stack (models.py:29-86).  Differentiable with respect to x_v,
+    x_h and its nine parameters when grad is enabled and one of them requires grad (_GatedLayerFunction), else the
+    inference call."""
 
     def __init__(self, mask_type, dim, kernel, residual=True, n_classes=10):
         super().__init__()
@@ -130,6 +156,8 @@ class GatedMaskedConv2d(nn.Module):
         B, _, H, W = x_v.shape
         _square(H, W, "GatedMaskedConv2d")
         label = _labels(h, B, x_v.device, "GatedMaskedConv2d")
+        if _grad_call([x_v, x_h], self):
+            return _GatedLayerFunction.apply(self, x_v, x_h, label, *self.parameters())
         keep = []
         w = self._weights(keep)
         out_v, out_h = ops.prior_layer(w, ops.nchw_to_nhwc(x_v.detach()), ops.nchw_to_nhwc(x_h.detach()), label,
@@ -143,6 +171,48 @@ _LAYER_GRADS = dict(vert_w="vert_stack.weight", vert_b="vert_stack.bias", v2h_w=
                     resid_w="horiz_resid.weight", resid_b="horiz_resid.bias", class_emb="class_cond_embedding.weight")
 _NET_GRADS = dict(embedding="embedding.weight", out1_w="output_conv.0.weight", out1_b="output_conv.0.bias",
                   out2_w="output_conv.2.weight", out2_b="output_conv.2.bias")
+
+
+class _GatedLayerFunction(torch.autograd.Function):
+    """GatedMaskedConv2d.forward with gradients: inputs are the layer, x_v, x_h (NCHW), the labels and the layer's
+    parameters in ``parameters()`` order.  NCHW <-> NHWC at the boundary; the forward keeps x_v, x_h (NHWC) and
+    vqb_prior_layer_forward_train_f32's `saved`; the backward (vqb_prior_layer_backward_f32) returns the gradients of
+    x_v, x_h and every parameter, mask A's taps included.  The labels get none."""
+
+    @staticmethod
+    def forward(ctx, layer, x_v, x_h, label, *params):
+        B, dim, H, W = x_v.shape
+        keep = []
+        w = layer._weights(keep)
+        xv, xh = ops.nchw_to_nhwc(x_v.detach()), ops.nchw_to_nhwc(x_h.detach())
+        nc = layer.class_cond_embedding.num_embeddings
+        out_v, out_h, saved = ops.prior_layer_forward_train(w, xv, xh, label, B=B, H=H, W=W, dim=dim, n_classes=nc)
+        ctx.layer, ctx.w, ctx.keep, ctx.saved = layer, w, keep, (xv, xh, label, saved)
+        ctx.shape = (B, H, W, dim, nc)
+        ctx.save_for_backward(x_v, x_h, *params)
+        ctx.set_materialize_grads(False)
+        return ops.nhwc_to_nchw(out_v), ops.nhwc_to_nchw(out_h)
+
+    @staticmethod
+    def backward(ctx, g_v, g_h):
+        if ctx.saved is None:
+            raise RuntimeError("GatedMaskedConv2d: backward through the same forward twice is not supported "
+                               "(its saved activations are freed by the first backward)")
+        ctx.saved_tensors                 # autograd's check that nothing saved was modified in place
+        xv, xh, label, saved = ctx.saved
+        B, H, W, dim, nc = ctx.shape
+        if g_h is None:
+            g_h = torch.zeros((B, dim, H, W), dtype=torch.float32, device=xv.device)
+        dv = ops.nchw_to_nhwc(g_v) if g_v is not None else None
+        params = dict(ctx.layer.named_parameters())
+        grads = {k: torch.empty(p.shape, dtype=torch.float32, device=xv.device) for k, p in params.items()}
+        table = PriorLayerGrads(**{f: grads[k].data_ptr() for f, k in _LAYER_GRADS.items()})
+        d_x_v, d_x_h = ops.prior_layer_backward(ctx.w, xv, xh, label, dv, ops.nchw_to_nhwc(g_h), saved, table,
+                                                B=B, H=H, W=W, dim=dim, n_classes=nc)
+        ctx.saved = ctx.keep = None
+        need = ctx.needs_input_grad
+        return (None, ops.nhwc_to_nchw(d_x_v) if need[1] else None, ops.nhwc_to_nchw(d_x_h) if need[2] else None,
+                None) + tuple(grads[k].to(p.dtype) for k, p in params.items())
 
 
 class _PriorFunction(torch.autograd.Function):
