@@ -385,6 +385,28 @@ int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer, const flo
                                  const vqb_prior_layer_grads *grads, float *d_x_v, float *d_x_h, void *workspace,
                                  size_t workspace_bytes, void *stream);
 
+/* ---- Gated PixelCNN prior in TF32 (wgmma tensor cores) ---------------------------------------------------------
+ * The teacher-forced forward and the backward with every matrix product on a TF32 wgmma GEMM: each operand is
+ * rounded to TF32 (round to nearest, ties away from zero) as it is staged, products accumulate in fp32.  The one-hot
+ * sums of the class and code embedding gradients stay fp32.  Same arguments, shape limits and error codes as the fp32
+ * entry points (never an fp32 fall-back); `saved` has the same layout and size (vqb_prior_train_saved_bytes), and the
+ * backward the same workspace (vqb_prior_backward_workspace_bytes) and properties: every gradient overwritten in its
+ * parameter's layout, mask A's taps included; no float atomics (bitwise reproducible); no host synchronisation.
+ * generate stays fp32 (vqb_prior_generate_f32).                                                                    */
+/* Workspace of vqb_prior_forward_tf32: 4*B*H*W*(11*dim + 512) bytes (0 = bad sizes).                               */
+size_t vqb_prior_workspace_bytes_tf32(int B, int H, int W, int dim, int n_layers, int K);
+/* GatedPixelCNN.forward in TF32: 3 + 4*n_layers launches (embedding; per layer the vertical stack, vert_to_horiz with
+ * the vertical gate, the horizontal stack, the gate with horiz_resid; the head's two 1x1 convs).                   */
+int vqb_prior_forward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                           float *logits, void *workspace, size_t workspace_bytes, void *stream);
+/* vqb_prior_forward_tf32 keeping its activations in `saved`: the same launches, bitwise the same logits.           */
+int vqb_prior_forward_train_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                                 int W, float *logits, void *saved, size_t saved_bytes, void *stream);
+/* Gradients from a vqb_prior_forward_train_tf32 call's `saved`: 7 + 10*n_layers launches.                          */
+int vqb_prior_backward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                            const float *d_logits, const void *saved, const vqb_prior_grads *grads, void *workspace,
+                            size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

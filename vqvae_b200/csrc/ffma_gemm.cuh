@@ -86,6 +86,9 @@ struct Mat {                      // p[i][j], row length ld
     int ld;
     static constexpr bool j_fast = true;
     __device__ __forceinline__ float operator()(int i, int j) const { return __ldg(p + (long long)i * ld + j); }
+    // tc_gemm.cuh: 32 consecutive j of row i; a 32-wide k-step stays in a row when ld % 32 == 0
+    __device__ __forceinline__ const float *seg(int i, long long j0) const { return p + (long long)i * ld + j0; }
+    bool seg_ok() const { return ld % 32 == 0 && ((uintptr_t)p & 15) == 0; }
 };
 
 struct MatT {                     // p[j][i]

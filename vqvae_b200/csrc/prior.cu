@@ -260,13 +260,6 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
     head_positions(s, n, in, out, (long long)H * W, H, W, keep);
 }
 
-// embedding (models.py:122): x0[n] = E[clamp(codes[n])]
-__global__ void embed_kernel(const long long *__restrict__ codes, const float *__restrict__ E, long long N, int K,
-                             int C, float *__restrict__ x0) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < N * C; i += (long long)gridDim.x * blockDim.x)
-        x0[i] = __ldg(E + (long long)clampi(codes[i / C], K) * C + i % C);
-}
-
 // One sampling step at (i, j) for P images: every layer's horizontal stack, the head, the softmax and the inverse-CDF
 // draw.  The code goes to codes[b, i, j] and its embedding to x0[b, i, j], which later steps and row passes read.
 template <int P>

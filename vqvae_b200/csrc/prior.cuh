@@ -35,6 +35,13 @@ inline unsigned grid_for(long long total) {
     return (unsigned)(g > 148LL * 32 ? 148LL * 32 : (g < 1 ? 1 : g));
 }
 
+// embedding (models.py:122): x0[n] = E[clamp(codes[n])]
+__global__ void embed_kernel(const long long *__restrict__ codes, const float *__restrict__ E, long long N, int K,
+                             int C, float *__restrict__ x0) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < N * C; i += (long long)gridDim.x * blockDim.x)
+        x0[i] = __ldg(E + (long long)clampi(codes[i / C], K) * C + i % C);
+}
+
 inline bool layer_ok(const vqb_prior_layer_weights &w) {
     return w.vert_w && w.vert_b && w.v2h_w && w.v2h_b && w.horiz_w && w.horiz_b && w.resid_w && w.resid_b &&
            w.class_emb && w.kernel >= 1 && w.kernel <= VQB_PRIOR_MAX_KERNEL && (w.kernel & 1);

@@ -12,8 +12,14 @@
 // Every output element is one fmaf chain in a fixed order and no float atomics are used, so the gradients are bitwise
 // reproducible.  Weight gradients cover all kh*kw taps, mask A's included (the reference convolves with the full,
 // zeroed weight, so autograd gives those taps a gradient); dgrad reads the taps the forward kept.
+//
+// The TF32 mode (vqb_prior_*_tf32) runs the same products on the wgmma GEMM of tc_gemm.cuh, which takes the same
+// accessors and epilogues: the backward is this file's backward with `tc_gemm` in place of `gemm` (the one-hot sums of
+// the class and code embeddings stay on the FFMA GEMM), and the forward is written below as four products per layer
+// and two for the head, with the same Saved layout as the fp32 training forward.
 #include "prior.cuh"
 #include "ffma_gemm.cuh"
+#include "tc_gemm.cuh"
 
 namespace {
 
@@ -60,6 +66,17 @@ struct Tap {
         if (rr < 0 || rr >= grid.H || cc < 0 || cc >= grid.W) return 0.f;
         return __ldg(g + (((long long)b * grid.H + rr) * grid.W + cc) * C + c);
     }
+    // tc_gemm.cuh: columns j0 .. j0 + 31 at position n, one position decode (nullptr: the tap is outside the grid).
+    // C % 32 == 0 keeps a 32-wide k-step inside one tap.
+    __device__ __forceinline__ const float *seg(int n, long long j0) const {
+        const int j = (int)j0, tap = j / C, c = j - tap * C, tr = tap / cols, tc = tap - tr * cols;
+        int b, r, col;
+        grid.split(n, b, r, col);
+        const int rr = r + sgn * (tr - hr), cc = col + sgn * (tc - hc);
+        if (rr < 0 || rr >= grid.H || cc < 0 || cc >= grid.W) return nullptr;
+        return g + (((long long)b * grid.H + rr) * grid.W + cc) * C + c;
+    }
+    bool seg_ok() const { return C % 32 == 0 && ((uintptr_t)g & 15) == 0; }
 };
 
 struct Gated {                    // gate(pre) of a saved (positions x 2C) pre-activation: the gated layer's output
@@ -81,6 +98,12 @@ struct WPacked {
         const int tap = k / Cout, co = k - tap * Cout;
         return __ldg(p + ((long long)tap * Cin + ci) * Cout + co);
     }
+    // tc_gemm.cuh: rows k0 .. k0 + 31 of column ci, contiguous when Cout % 32 == 0
+    __device__ __forceinline__ const float *segT(long long k0, int ci) const {
+        const int k = (int)k0, tap = k / Cout, co = k - tap * Cout;
+        return p + ((long long)tap * Cin + ci) * Cout + co;
+    }
+    bool seg_ok() const { return Cout % 32 == 0 && ((uintptr_t)p & 15) == 0; }
 };
 
 struct OneHot {                   // (m, n) -> 1 if the clamped index of position n is m: idx[n / per]
@@ -155,9 +178,69 @@ struct VertBack {
     }
 };
 
+// ---- epilogues of the TF32 forward ------------------------------------------------------------------------------
+struct BiasStore {                // out[m][n] = v + bias[n] (+ add[m][n])
+    float *out;
+    const float *bias, *add;
+    int ld;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        const long long i = (long long)m * ld + n;
+        const float r = v + __ldg(bias + n);
+        out[i] = add ? r + __ldg(add + i) : r;
+    }
+};
+
+// v = (W_v2h h_vert)[m][n]: vh = v + bias + class (2C wide); for n < C also out_v = gate(h_vert + class)
+struct VertOut {
+    float *vh, *out_v;
+    const float *hv, *bias, *emb;
+    const long long *labels;
+    int C, HW, NC;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        const float *e = emb + (long long)clampi(labels[m / HW], NC) * 2 * C;
+        vh[(long long)m * 2 * C + n] = (v + __ldg(bias + n)) + __ldg(e + n);
+        if (n < C) {
+            const float *h = hv + (long long)m * 2 * C;
+            out_v[(long long)m * C + n] = gate(__ldg(h + n) + __ldg(e + n), __ldg(h + n + C) + __ldg(e + n + C));
+        }
+    }
+};
+
+struct ReluBias {                 // the head's hidden layer: out[m][n] = relu(v + bias[n])
+    float *out;
+    const float *bias;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        out[(long long)m * HID + n] = fmaxf(v + __ldg(bias + n), 0.f);
+    }
+};
+
+struct Logits {                   // logit n of position m into NCHW (B, K, H, W)
+    float *out;
+    const float *bias;
+    int K, HW;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        const int b = m / HW;
+        out[((long long)b * K + n) * HW + (m - b * HW)] = v + __ldg(bias + n);
+    }
+};
+
 // ---- host side ---------------------------------------------------------------------------------------------------
-template <class LA, class LB, class EP>
-void dgrad(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K) { gemm(st, a, b, ep, M, N, K, WgradSplit{1, K}); }
+struct Ffma {                     // the arithmetic of a product: fp32 FFMA (ffma_gemm.cuh) or TF32 wgmma (tc_gemm.cuh)
+    template <class LA, class LB, class EP>
+    static void run(cudaStream_t st, LA a, LB b, EP ep, int M, int N, long long K, WgradSplit sp) {
+        gemm(st, a, b, ep, M, N, K, sp);
+    }
+};
+
+struct Tf32 {
+    template <class LA, class LB, class EP>
+    static void run(cudaStream_t st, LA a, LB b, EP ep, int M, int N, long long K, WgradSplit sp) {
+        tc_gemm(st, a, b, ep, M, N, K, sp);
+    }
+};
+
+template <class G, class LA, class LB, class EP>
+void dgrad(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K) { G::run(st, a, b, ep, M, N, K, WgradSplit{1, K}); }
 
 // A wgrad job in the partial region: M x cols partials of a reduction over `npos` positions, at `off` floats.
 struct WJob {
@@ -251,6 +334,7 @@ void reduce(cudaStream_t st, const Phase &p, float *part, float *const (&w)[MAX_
 // pre-activation its training forward kept; ghi = d out_h, gvi = d out_v (nullptr: zero, as for the net's last
 // layer) -> gho = d x_h, gvo = d x_v (+ fold, the net's layer 0: x_v and x_h are both the embedding) and the nine
 // weight gradients of q.  work: 6 grids of scratch; part: the wgrad partials of layer_phase.
+template <class G>
 void layer_backward(cudaStream_t st, const vqb_prior_layer_weights &w, const vqb_prior_layer_grads &q, int C, int NC,
                     const long long *lab, Grid g, int npos, const float *xv, const float *xh, const float *hv,
                     const float *ph, const float *ghi, const float *gvi, float *gho, float *gvo, const float *fold,
@@ -260,24 +344,24 @@ void layer_backward(cudaStream_t st, const vqb_prior_layer_weights &w, const vqb
     float *dph = work, *dhv = dph + 2 * grid, *cls = dhv + 2 * grid;
     const Phase p = layer_phase(w, C, NC, npos);
     // out_h = horiz_resid(gate(pre_h)) [+ x_h]: d pre_h, then d x_h = [d out_h +] horiz_stack^T * d pre_h
-    dgrad(st, Mat{ghi, C}, WPacked{w.resid_w, C, C}, GateBack{dph, ph, C}, npos, C, C);
-    gemm(st, MatT{ghi, C}, WithOnes<Gated>{Gated{ph, C}, C}, Partial{part + p.job[0].off, C, C + 1}, C, C + 1,
-         npos, p.job[0].sp);
-    dgrad(st, Tap{dph, C2, hc, 0, half, -1, g}, WPacked{w.horiz_w, C, C2}, Store{gho, w.residual ? ghi : nullptr, C},
-          npos, C, hc * C2);
-    gemm(st, MatT{dph, C2}, WithOnes<Tap>{Tap{xh, C, hcols(w), 0, half, 1, g}, hcols(w) * C},
-         Partial{part + p.job[1].off, C2, p.job[1].cols()}, C2, p.job[1].cols(), npos, p.job[1].sp);
-    gemm(st, MatT{dph, C2}, WithOnes<Mat>{Mat{hv, C2}, C2}, Partial{part + p.job[2].off, C2, C2 + 1}, C2, C2 + 1,
-         npos, p.job[2].sp);
+    dgrad<G>(st, Mat{ghi, C}, WPacked{w.resid_w, C, C}, GateBack{dph, ph, C}, npos, C, C);
+    G::run(st, MatT{ghi, C}, WithOnes<Gated>{Gated{ph, C}, C}, Partial{part + p.job[0].off, C, C + 1}, C, C + 1,
+           npos, p.job[0].sp);
+    dgrad<G>(st, Tap{dph, C2, hc, 0, half, -1, g}, WPacked{w.horiz_w, C, C2},
+             Store{gho, w.residual ? ghi : nullptr, C}, npos, C, hc * C2);
+    G::run(st, MatT{dph, C2}, WithOnes<Tap>{Tap{xh, C, hcols(w), 0, half, 1, g}, hcols(w) * C},
+           Partial{part + p.job[1].off, C2, p.job[1].cols()}, C2, p.job[1].cols(), npos, p.job[1].sp);
+    G::run(st, MatT{dph, C2}, WithOnes<Mat>{Mat{hv, C2}, C2}, Partial{part + p.job[2].off, C2, C2 + 1}, C2, C2 + 1,
+           npos, p.job[2].sp);
     // d h_vert = W_v2h^T d pre_h + gate'(h_vert + class) * d out_v; class gradient; d x_v = vert_stack^T * d h_vert
-    dgrad(st, Mat{dph, C2}, WPacked{w.v2h_w, C2, C2},
-          VertBack{dhv, cls, hv, gvi, dph, w.class_emb, lab, C, g.H * g.W, NC}, npos, C2, C2);
+    dgrad<G>(st, Mat{dph, C2}, WPacked{w.v2h_w, C2, C2},
+             VertBack{dhv, cls, hv, gvi, dph, w.class_emb, lab, C, g.H * g.W, NC}, npos, C2, C2);
     gemm(st, OneHot{lab, g.H * g.W, NC}, Mat{cls, C2}, Partial{part + p.job[3].off, NC, C2}, NC, C2, npos,
          p.job[3].sp);
-    gemm(st, MatT{dhv, C2}, WithOnes<Tap>{Tap{xv, C, w.kernel, half, half, 1, g}, vrows(w) * w.kernel * C},
-         Partial{part + p.job[4].off, C2, p.job[4].cols()}, C2, p.job[4].cols(), npos, p.job[4].sp);
-    dgrad(st, Tap{dhv, C2, w.kernel, half, half, -1, g}, WPacked{w.vert_w, C, C2}, Store{gvo, fold, C}, npos, C,
-          vr * w.kernel * C2);
+    G::run(st, MatT{dhv, C2}, WithOnes<Tap>{Tap{xv, C, w.kernel, half, half, 1, g}, vrows(w) * w.kernel * C},
+           Partial{part + p.job[4].off, C2, p.job[4].cols()}, C2, p.job[4].cols(), npos, p.job[4].sp);
+    dgrad<G>(st, Tap{dhv, C2, w.kernel, half, half, -1, g}, WPacked{w.vert_w, C, C2}, Store{gvo, fold, C}, npos, C,
+             vr * w.kernel * C2);
     reduce(st, p, part, {q.resid_w, q.horiz_w, q.v2h_w, q.class_emb, q.vert_w},
            {q.resid_b, q.horiz_b, q.v2h_b, nullptr, q.vert_b});
 }
@@ -308,7 +392,97 @@ bool grads_ok(const vqb_prior_grads *g, int L) {
     return true;
 }
 
+// ---- the TF32 forward --------------------------------------------------------------------------------------------
+// Workspace of the inference call (vqb_prior_forward_tf32), in floats, with Saved's accessors: x_v and x_h ping-pong
+// between two grids each (layer 0 reads the embedding in grid 0 for both), one h_vert, pre_h and vh (2C), the hidden
+// layer (512).
+struct TcWs {
+    long long N, C;
+    long long xv(int l) const { return l == 0 ? 0 : (1 + ((l - 1) & 1)) * N * C; }
+    long long xh(int l) const { return l == 0 ? 0 : (3 + ((l - 1) & 1)) * N * C; }
+    long long hv(int) const { return 5 * N * C; }
+    long long ph(int) const { return 7 * N * C; }
+    long long vh() const { return 9 * N * C; }
+    long long hid() const { return 11 * N * C; }
+    long long total() const { return hid() + N * HID; }
+};
+
+// one TF32 product over all of K (positions x outputs)
+template <class LA, class LB, class EP>
+void tf32_product(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K) {
+    tc_gemm(st, a, b, ep, M, N, K, WgradSplit{1, K});
+}
+
+// GatedPixelCNN.forward in TF32, every activation at lay's offsets from sp: the embedding gather, per layer
+//   h_vert = vert_stack * x_v + b                      (kept taps)
+//   vh = v2h(h_vert) + b + class, out_v = gate(h_vert + class)
+//   pre_h = horiz_stack * x_h + b + vh                 (kept taps)
+//   out_h = horiz_resid(gate(pre_h)) + b [+ x_h]       (the gate computed as the operand is staged)
+// and the head hid = relu(W1 x_h + b1), logits = W2 hid + b2 (NCHW).  3 + 4*n_layers launches.
+template <class Lay>
+void forward_tf32(cudaStream_t st, const Net &n, const long long *codes, const long long *lab, int B, int H, int W,
+                  float *logits, float *sp, const Lay &lay) {
+    const int npos = B * H * W, C = n.C, C2 = 2 * C;
+    const Grid g{H, W};
+    embed_kernel<<<grid_for((long long)npos * C), NT, 0, st>>>(codes, n.emb, npos, n.K, C, sp + lay.xv(0));
+    float *vh = sp + lay.vh();
+    for (int l = 0; l < n.L; ++l) {
+        const vqb_prior_layer_weights &w = n.layer[l];
+        const int half = w.kernel / 2, vr = vrows(w) - (w.mask_a ? 1 : 0), hc = hcols(w) - (w.mask_a ? 1 : 0);
+        const float *xv = sp + lay.xv(l), *xh = sp + lay.xh(l);
+        float *hv = sp + lay.hv(l), *ph = sp + lay.ph(l);
+        tf32_product(st, Tap{xv, C, w.kernel, half, half, 1, g}, Mat{w.vert_w, C2}, BiasStore{hv, w.vert_b, nullptr, C2},
+                     npos, C2, vr * w.kernel * C);
+        tf32_product(st, Mat{hv, C2}, Mat{w.v2h_w, C2},
+                     VertOut{vh, sp + lay.xv(l + 1), hv, w.v2h_b, w.class_emb, lab, C, H * W, n.NC}, npos, C2, C2);
+        tf32_product(st, Tap{xh, C, hcols(w), 0, half, 1, g}, Mat{w.horiz_w, C2}, BiasStore{ph, w.horiz_b, vh, C2},
+                     npos, C2, hc * C);
+        tf32_product(st, Gated{ph, C}, Mat{w.resid_w, C},
+                     BiasStore{sp + lay.xh(l + 1), w.resid_b, w.residual ? xh : nullptr, C}, npos, C, C);
+    }
+    float *hid = sp + lay.hid();
+    tf32_product(st, Mat{sp + lay.xh(n.L), C}, Mat{n.w1, HID}, ReluBias{hid, n.b1}, npos, HID, C);
+    tf32_product(st, Mat{hid, HID}, Mat{n.w2, n.K}, Logits{logits, n.b2, n.K, H * W}, npos, n.K, HID);
+}
+
 }  // namespace
+
+extern "C" size_t vqb_prior_workspace_bytes_tf32(int B, int H, int W, int dim, int n_layers, int K) {
+    if (B <= 0 || H <= 0 || W <= 0 || dim <= 0 || n_layers <= 0 || K <= 0) return 0;
+    return (size_t)TcWs{(long long)B * H * W, dim}.total() * sizeof(float);
+}
+
+extern "C" int vqb_prior_forward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                      int H, int W, float *logits, void *workspace, size_t workspace_bytes,
+                                      void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!codes || !labels || !logits || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (workspace_bytes < vqb_prior_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    forward_tf32((cudaStream_t)stream, n, reinterpret_cast<const long long *>(codes),
+                 reinterpret_cast<const long long *>(labels), B, H, W, logits, static_cast<float *>(workspace),
+                 TcWs{(long long)B * H * W, n.C});
+    VQB_COUNT_LAUNCH(3 + 4 * n.L);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+// vqb_prior_forward_tf32's launches with every activation in the Saved layout of the fp32 training forward: the same
+// products on the same values, so bitwise the same logits.
+extern "C" int vqb_prior_forward_train_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                            int B, int H, int W, float *logits, void *saved, size_t saved_bytes,
+                                            void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!codes || !labels || !logits || !saved || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (saved_bytes < vqb_prior_train_saved_bytes(B, H, W, n.C, n.L)) return VQB_ERR_WORKSPACE;
+    forward_tf32((cudaStream_t)stream, n, reinterpret_cast<const long long *>(codes),
+                 reinterpret_cast<const long long *>(labels), B, H, W, logits, static_cast<float *>(saved),
+                 Saved{(long long)B * H * W, n.C, n.L});
+    VQB_COUNT_LAUNCH(3 + 4 * n.L);
+    return vqb_cuda_status(cudaGetLastError());
+}
 
 extern "C" size_t vqb_prior_backward_workspace_bytes(const vqb_prior_net *net, int B, int H, int W) {
     Net n;
@@ -316,10 +490,13 @@ extern "C" size_t vqb_prior_backward_workspace_bytes(const vqb_prior_net *net, i
     return (size_t)bws_layout(n, (long long)B * H * W).total * sizeof(float);
 }
 
-extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
-                                      int H, int W, const float *d_logits, const void *saved,
-                                      const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
-                                      void *stream) {
+namespace {
+
+// vqb_prior_backward_f32 (G = Ffma) and vqb_prior_backward_tf32 (G = Tf32): the same products, launches and workspace
+template <class G>
+int net_backward(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                 const float *d_logits, const void *saved, const vqb_prior_grads *grads, void *workspace,
+                 size_t workspace_bytes, void *stream) {
     Net n;
     const int st_ = net_from(net, n);
     if (st_) return st_;
@@ -344,13 +521,13 @@ extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *c
         float *dhid = ws + wl.work;
         const float *hid = sp + sv.hid(), *xL = sp + sv.xh(n.L);
         const Nchw dl{d_logits, K, H * W};
-        dgrad(st, dl, WPacked{n.w2, HID, K}, ReluBack{dhid, hid}, npos, HID, K);
+        dgrad<G>(st, dl, WPacked{n.w2, HID, K}, ReluBack{dhid, hid}, npos, HID, K);
         const Phase p = head_phase(n, npos);
-        gemm(st, NchwT{dl}, WithOnes<Mat>{Mat{hid, HID}, HID}, Partial{part + p.job[0].off, K, HID + 1}, K, HID + 1,
-             npos, p.job[0].sp);
-        gemm(st, MatT{dhid, HID}, WithOnes<Mat>{Mat{xL, C}, C}, Partial{part + p.job[1].off, HID, C + 1}, HID, C + 1,
-             npos, p.job[1].sp);
-        dgrad(st, Mat{dhid, HID}, WPacked{n.w1, C, HID}, Store{gh[0], nullptr, C}, npos, C, HID);
+        G::run(st, NchwT{dl}, WithOnes<Mat>{Mat{hid, HID}, HID}, Partial{part + p.job[0].off, K, HID + 1}, K,
+               HID + 1, npos, p.job[0].sp);
+        G::run(st, MatT{dhid, HID}, WithOnes<Mat>{Mat{xL, C}, C}, Partial{part + p.job[1].off, HID, C + 1}, HID,
+               C + 1, npos, p.job[1].sp);
+        dgrad<G>(st, Mat{dhid, HID}, WPacked{n.w1, C, HID}, Store{gh[0], nullptr, C}, npos, C, HID);
         reduce(st, p, part, {grads->out2_w, grads->out1_w}, {grads->out2_b, grads->out1_b});
         launches += 5;
     }
@@ -359,9 +536,9 @@ extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *c
     for (int l = n.L - 1; l >= 0; --l) {
         float *gho = gh[cur ^ 1];
         // layer 0: x_v and x_h are both the embedding, so d x_v^0 + d x_h^0 is its gradient per position
-        layer_backward(st, n.layer[l], grads->layers[l], C, n.NC, lab, g, npos, sp + sv.xv(l), sp + sv.xh(l),
-                       sp + sv.hv(l), sp + sv.ph(l), gh[cur], l == n.L - 1 ? nullptr : gv[cur], gho, gv[cur ^ 1],
-                       l == 0 ? gho : nullptr, ws + wl.work, part);
+        layer_backward<G>(st, n.layer[l], grads->layers[l], C, n.NC, lab, g, npos, sp + sv.xv(l), sp + sv.xh(l),
+                          sp + sv.hv(l), sp + sv.ph(l), gh[cur], l == n.L - 1 ? nullptr : gv[cur], gho, gv[cur ^ 1],
+                          l == 0 ? gho : nullptr, ws + wl.work, part);
         launches += 10;
         cur ^= 1;
     }
@@ -375,6 +552,22 @@ extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *c
     }
     VQB_COUNT_LAUNCH(launches);
     return vqb_cuda_status(cudaGetLastError());
+}
+
+}  // namespace
+
+extern "C" int vqb_prior_backward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                      int H, int W, const float *d_logits, const void *saved,
+                                      const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
+                                      void *stream) {
+    return net_backward<Ffma>(net, codes, labels, B, H, W, d_logits, saved, grads, workspace, workspace_bytes, stream);
+}
+
+extern "C" int vqb_prior_backward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                       int H, int W, const float *d_logits, const void *saved,
+                                       const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
+                                       void *stream) {
+    return net_backward<Tf32>(net, codes, labels, B, H, W, d_logits, saved, grads, workspace, workspace_bytes, stream);
 }
 
 extern "C" int vqb_prior_gate_backward_f32(const float *x, const float *d_out, float *d_x, int64_t outer, int C,
@@ -408,7 +601,7 @@ extern "C" int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer
     const LayerSaved sv{npos, dim};
     const float *sp = static_cast<const float *>(saved);
     float *ws = static_cast<float *>(workspace);
-    layer_backward((cudaStream_t)stream, *layer, *grads, dim, n_classes, reinterpret_cast<const long long *>(labels),
+    layer_backward<Ffma>((cudaStream_t)stream, *layer, *grads, dim, n_classes, reinterpret_cast<const long long *>(labels),
                    Grid{H, W}, npos, x_v, x_h, sp + sv.hv(), sp + sv.ph(), d_out_h, d_out_v, d_x_h, d_x_v, nullptr, ws,
                    ws + 6LL * npos * dim);
     VQB_COUNT_LAUNCH(10);

@@ -450,22 +450,35 @@ def prior_layer_backward(layer_w, x_v, x_h, labels, d_out_v, d_out_h, saved, gra
     return d_x_v, d_x_h
 
 
-def _prior_workspace(net, B, H, W, dev):
-    n = lib().vqb_prior_workspace_bytes(B, H, W, net.dim, net.n_layers, net.input_dim)
+def _prior_workspace(net, B, H, W, dev, size=None):
+    n = (size or lib().vqb_prior_workspace_bytes)(B, H, W, net.dim, net.n_layers, net.input_dim)
     if n == 0:
         raise RuntimeError("prior: bad sizes")
     return torch.empty((n,), dtype=torch.uint8, device=dev)
 
 
-def prior_forward(net, codes, labels):
-    """Teacher-forced logits (B, K, H, W) of int64 codes (B,H,W) and labels (B,) (vqb_prior_forward_f32)."""
+PRIOR_PRECISIONS = ("fp32", "tf32")
+
+
+def _prior_precision(precision):
+    """The C-ABI suffix of a prior precision: "fp32" -> "f32" (CUDA cores), "tf32" -> "tf32" (wgmma tensor cores)."""
+    if precision not in PRIOR_PRECISIONS:
+        raise ValueError(f"prior precision must be one of {PRIOR_PRECISIONS}, got {precision!r}")
+    return "f32" if precision == "fp32" else "tf32"
+
+
+def prior_forward(net, codes, labels, precision="fp32"):
+    """Teacher-forced logits (B, K, H, W) of int64 codes (B,H,W) and labels (B,) (vqb_prior_forward_f32, or
+    vqb_prior_forward_tf32 for precision="tf32")."""
+    sfx = _prior_precision(precision)
     B, H, W = codes.shape
     dev = codes.device
     logits = torch.empty((B, net.input_dim, H, W), dtype=torch.float32, device=dev)
-    ws = _prior_workspace(net, B, H, W, dev)
-    span = _Span(f"prior forward K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
-    check(lib().vqb_prior_forward_f32(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W,
-                                      logits.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "prior_forward")
+    ws = _prior_workspace(net, B, H, W, dev, lib().vqb_prior_workspace_bytes_tf32 if sfx == "tf32" else None)
+    span = _Span(f"prior forward ({precision}) K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(getattr(lib(), "vqb_prior_forward_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W,
+                                                      logits.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
+          "prior_forward")
     span.done()
     return logits
 
@@ -485,9 +498,11 @@ def prior_generate(net, labels, u, step_logits=None):
     return codes
 
 
-def prior_forward_train(net, codes, labels):
+def prior_forward_train(net, codes, labels, precision="fp32"):
     """prior_forward that also keeps the activations the backward needs: (logits, saved) with saved a uint8 buffer
-    of vqb_prior_train_saved_bytes (vqb_prior_forward_train_f32; the logits are bitwise prior_forward's)."""
+    of vqb_prior_train_saved_bytes (vqb_prior_forward_train_f32 / _tf32; the logits are bitwise prior_forward's in the
+    same precision)."""
+    sfx = _prior_precision(precision)
     B, H, W = codes.shape
     dev = codes.device
     n = lib().vqb_prior_train_saved_bytes(B, H, W, net.dim, net.n_layers)
@@ -495,24 +510,27 @@ def prior_forward_train(net, codes, labels):
         raise RuntimeError("prior: bad sizes")
     saved = torch.empty((n,), dtype=torch.uint8, device=dev)
     logits = torch.empty((B, net.input_dim, H, W), dtype=torch.float32, device=dev)
-    span = _Span(f"prior forward (train) K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
-    check(lib().vqb_prior_forward_train_f32(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W,
-                                            logits.data_ptr(), saved.data_ptr(), saved.numel(), _stream()),
+    span = _Span(f"prior forward (train, {precision}) K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(getattr(lib(), "vqb_prior_forward_train_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B,
+                                                            H, W, logits.data_ptr(), saved.data_ptr(), saved.numel(),
+                                                            _stream()),
           "prior_forward_train")
     span.done()
     return logits, saved
 
 
-def prior_backward(net, codes, labels, d_logits, saved, grads):
-    """Every parameter gradient of the prior (vqb_prior_backward_f32) into the tensors `grads` (a PriorGrads struct)
-    points at; d_logits (B, K, H, W) fp32 contiguous, saved from prior_forward_train on the same net and inputs."""
+def prior_backward(net, codes, labels, d_logits, saved, grads, precision="fp32"):
+    """Every parameter gradient of the prior (vqb_prior_backward_f32 / _tf32) into the tensors `grads` (a PriorGrads
+    struct) points at; d_logits (B, K, H, W) fp32 contiguous, saved from prior_forward_train on the same net and
+    inputs, in the same precision."""
+    sfx = _prior_precision(precision)
     B, H, W = codes.shape
     n = lib().vqb_prior_backward_workspace_bytes(_lib.C.byref(net), B, H, W)
     if n == 0:
         raise RuntimeError("prior backward: bad sizes")
     ws = torch.empty((n,), dtype=torch.uint8, device=codes.device)
-    span = _Span(f"prior backward K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
-    check(lib().vqb_prior_backward_f32(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W,
-                                       d_logits.data_ptr(), saved.data_ptr(), _lib.C.byref(grads), ws.data_ptr(),
-                                       ws.numel(), _stream()), "prior_backward")
+    span = _Span(f"prior backward ({precision}) K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(getattr(lib(), "vqb_prior_backward_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H,
+                                                       W, d_logits.data_ptr(), saved.data_ptr(), _lib.C.byref(grads),
+                                                       ws.data_ptr(), ws.numel(), _stream()), "prior_backward")
     span.done()

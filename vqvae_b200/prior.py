@@ -3,13 +3,17 @@
 Same class names, constructor signatures, attribute names and state-dict keys as the reference, so a state dict saved
 by its ``gated_pixelcnn.py`` loads unchanged and ``from pixelcnn.models import GatedPixelCNN`` (the top-level
 ``pixelcnn`` package re-exports these classes) drops in.  As in ``modules.py`` the nn.Conv2d / nn.Embedding children
-are parameter containers only: every forward runs the sm_90a kernels of ``csrc/prior.cu`` through the C ABI, in fp32
-whatever ``set_precision`` says.
+are parameter containers only: every forward runs the sm_90a kernels of ``csrc/prior.cu`` / ``csrc/prior_bwd.cu``
+through the C ABI, in the model's ``precision`` (fp32 by default) whatever ``set_precision`` says.
 
 ``GatedPixelCNN.forward`` is differentiable with respect to every parameter when grad is enabled and a parameter
 requires grad (``_PriorFunction``: the training forward keeps its activations, and the backward of
 ``csrc/prior_bwd.cu`` writes one gradient per parameter), so the reference's training loop runs unchanged.  Under
-``torch.no_grad()`` it is the inference forward.  ``GatedMaskedConv2d`` and ``GatedActivation`` called on their own
+``torch.no_grad()`` it is the inference forward.  ``GatedPixelCNN.precision`` (a plain attribute, not in the state
+dict) selects the arithmetic of ``forward``, inference and training alike: "fp32" (the default, CUDA cores) or
+"tf32" (every matrix product on the wgmma TF32 GEMM, operands rounded to TF32, fp32 accumulation; the one-hot
+embedding-gradient sums stay fp32).  ``generate``, ``GatedMaskedConv2d`` and ``GatedActivation`` stay fp32 in both
+modes, and ``set_precision`` does not affect the prior.  ``GatedMaskedConv2d`` and ``GatedActivation`` called on their own
 are differentiable too, under the same rule (grad enabled and an input or a parameter requiring grad):
 ``_GatedLayerFunction`` runs the layer's training forward and single-layer backward (vqb_prior_layer_*_f32),
 ``_GateFunction`` the gate and its backward.  Their outputs are bitwise the inference call's.
@@ -96,7 +100,7 @@ class _GateFunction(torch.autograd.Function):
 
 class GatedActivation(nn.Module):
     """tanh(first half of the channels) * sigmoid(second half) (models.py:20-26).  Differentiable when grad is enabled
-    and x requires grad (_GateFunction), else the inference call."""
+    and x requires grad (_GateFunction), else the inference call.  Always fp32."""
 
     def forward(self, x):
         if _grad_call([x]):
@@ -107,7 +111,7 @@ class GatedActivation(nn.Module):
 class GatedMaskedConv2d(nn.Module):
     """One gated layer with a vertical and a horizontal stack (models.py:29-86).  Differentiable with respect to x_v,
     x_h and its nine parameters when grad is enabled and one of them requires grad (_GatedLayerFunction), else the
-    inference call."""
+    inference call.  Always fp32 on its own (a model's ``precision`` applies to ``GatedPixelCNN.forward``)."""
 
     def __init__(self, mask_type, dim, kernel, residual=True, n_classes=10):
         super().__init__()
@@ -216,16 +220,17 @@ class _GatedLayerFunction(torch.autograd.Function):
 
 
 class _PriorFunction(torch.autograd.Function):
-    """GatedPixelCNN.forward with gradients: inputs are the model, codes, labels and every parameter in
-    ``parameters()`` order.  The forward keeps the activations vqb_prior_backward_f32 reads; the backward returns one
-    gradient per parameter in its shape and dtype, mask A's taps included (the reference's autograd gives them one)."""
+    """GatedPixelCNN.forward with gradients: inputs are the model, the precision, codes, labels and every parameter in
+    ``parameters()`` order.  The forward keeps the activations vqb_prior_backward_f32 (or _tf32) reads; the backward
+    runs in the precision the forward ran in and returns one gradient per parameter in its shape and dtype, mask A's
+    taps included (the reference's autograd gives them one)."""
 
     @staticmethod
-    def forward(ctx, model, codes, labels, *params):
+    def forward(ctx, model, precision, codes, labels, *params):
         keep = []
         net = model._net(keep)
-        logits, saved = ops.prior_forward_train(net, codes, labels)
-        ctx.model, ctx.net, ctx.keep, ctx.saved = model, net, keep, saved
+        logits, saved = ops.prior_forward_train(net, codes, labels, precision)
+        ctx.model, ctx.net, ctx.keep, ctx.saved, ctx.precision = model, net, keep, saved, precision
         ctx.save_for_backward(codes, labels)
         return logits
 
@@ -243,17 +248,22 @@ class _PriorFunction(torch.autograd.Function):
             for i in range(n_layers)])
         table = PriorGrads(layers=C.cast(layers, C.POINTER(PriorLayerGrads)), n_layers=n_layers,
                            **{f: grads[k].data_ptr() for f, k in _NET_GRADS.items()})
-        ops.prior_backward(ctx.net, codes, labels, _f32(d_logits), ctx.saved, table)
+        ops.prior_backward(ctx.net, codes, labels, _f32(d_logits), ctx.saved, table, ctx.precision)
         ctx.saved = ctx.keep = None
-        return (None, None, None) + tuple(grads[k].to(p.dtype) for k, p in params.items())
+        return (None, None, None, None) + tuple(grads[k].to(p.dtype) for k, p in params.items())
 
 
 class GatedPixelCNN(nn.Module):
     """Prior over code grids (models.py:89-143): layer 0 is a mask-A 7x7 layer without residual, the others mask-B
-    3x3 layers with residual, then a 1x1 -> ReLU -> 1x1 head to input_dim logits."""
+    3x3 layers with residual, then a 1x1 -> ReLU -> 1x1 head to input_dim logits.
+
+    ``precision``: "fp32" (default) or "tf32", the arithmetic of ``forward`` (see the module docstring).  A plain
+    attribute, so state dicts are the reference's; any other value raises ValueError from ``forward``.  ``generate``
+    is fp32 either way."""
 
     def __init__(self, input_dim=256, dim=64, n_layers=15, n_classes=10):
         super().__init__()
+        self.precision = "fp32"
         self.dim = dim
         self.embedding = nn.Embedding(input_dim, dim)
         self.layers = nn.ModuleList()
@@ -295,8 +305,11 @@ class GatedPixelCNN(nn.Module):
                         **{k: v.data_ptr() for k, v in t.items()})
 
     def forward(self, x, label):
-        """int64 codes (B,H,W) and labels (B,) -> fp32 logits (B, input_dim, H, W).  Differentiable with respect to
-        the parameters when grad is enabled and any parameter requires grad."""
+        """int64 codes (B,H,W) and labels (B,) -> fp32 logits (B, input_dim, H, W), in ``self.precision``.
+        Differentiable with respect to the parameters when grad is enabled and any parameter requires grad."""
+        precision = self.precision
+        if precision not in ops.PRIOR_PRECISIONS:
+            raise ValueError(f"GatedPixelCNN.precision must be one of {ops.PRIOR_PRECISIONS}, got {precision!r}")
         if x.dim() != 3:
             raise RuntimeError(f"GatedPixelCNN: expected codes of shape (B,H,W), got {tuple(x.shape)}")
         B, H, W = x.shape
@@ -305,12 +318,13 @@ class GatedPixelCNN(nn.Module):
         label = _labels(label, B, x.device, "GatedPixelCNN")
         x = x.detach().to(torch.int64).contiguous()
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            return _PriorFunction.apply(self, x, label, *self.parameters())
+            return _PriorFunction.apply(self, precision, x, label, *self.parameters())
         keep = []
-        return ops.prior_forward(self._net(keep), x, label)
+        return ops.prior_forward(self._net(keep), x, label, precision)
 
     def _sample(self, label, u, step_logits=None):
-        """generate() with given uniforms u (B,H,W) fp32: the code at (b,i,j) is the smallest k with u < CDF_k."""
+        """generate() with given uniforms u (B,H,W) fp32: the code at (b,i,j) is the smallest k with u < CDF_k.
+        fp32 whatever ``precision`` says."""
         B, H, W = u.shape
         _square(H, W, "GatedPixelCNN.generate")
         first = self.layers[0] if len(self.layers) else None
@@ -324,7 +338,8 @@ class GatedPixelCNN(nn.Module):
 
     def generate(self, label, shape=(8, 8), batch_size=64):
         """Sample (batch_size, *shape) int64 codes in raster order on the model's device.  Draws exactly one
-        torch.rand((batch_size, H, W)) from the current CUDA generator, so torch.manual_seed makes it reproducible."""
+        torch.rand((batch_size, H, W)) from the current CUDA generator, so torch.manual_seed makes it reproducible.
+        fp32 whatever ``precision`` says: the per-position step kernels are bound by latency, not by FLOPs."""
         H, W = shape
         _square(H, W, "GatedPixelCNN.generate")
         dev = next(self.parameters()).device
