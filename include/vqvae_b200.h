@@ -407,6 +407,65 @@ int vqb_prior_backward_tf32(const vqb_prior_net *net, const int64_t *codes, cons
                             const float *d_logits, const void *saved, const vqb_prior_grads *grads, void *workspace,
                             size_t workspace_bytes, void *stream);
 
+/* ---- optimizer step on device: Adam over many tensors, then every weight packing refreshed --------------------
+ * One training step's update of a parameter group is two calls, each normally ONE launch: vqb_adam_multi_f32 updates
+ * every parameter and its moments, then vqb_repack_multi rebuilds every packing read from those parameters and
+ * advances their step counters.  The descriptor arrays are HOST arrays, read during the call only; each launch carries
+ * its whole table as one by-value kernel parameter (needs a driver of the CUDA 12.1 line or newer), so both calls
+ * capture into a CUDA graph with no host-to-device copy, and a replay runs with the hyper-parameters and pointers of
+ * the capture.  A list longer than the per-launch capacity is split into several launches, in order.              */
+
+/* One parameter of vqb_adam_multi_f32: numel fp32 elements each of param, grad, exp_avg, exp_avg_sq and, with amsgrad,
+ * max_exp_avg_sq (NULL otherwise).  step: the device fp32 count of steps this parameter has taken (torch's
+ * state["step"]), read, not written: vqb_repack_multi advances it.                                                   */
+typedef struct vqb_adam_tensor {
+    float *param;
+    const float *grad;
+    float *exp_avg, *exp_avg_sq, *max_exp_avg_sq;
+    const float *step;
+    int64_t numel;
+} vqb_adam_tensor;
+
+/* Tensors per launch of vqb_adam_multi_f32 (480).                                                                     */
+int vqb_adam_capacity(void);
+/* torch.optim.Adam's update (weight decay as an L2 term on the grad, not decoupled), per element in fp32 in the order
+ * of torch's single-tensor Adam: g += wd*p; exp_avg lerps towards g by 1 - beta1; exp_avg_sq = exp_avg_sq*beta2 +
+ * (1 - beta2)*g*g; amsgrad max; denom = sqrt(v)/sqrt(bc2) + eps; p -= (lr/bc1)*exp_avg/denom, with bc_i = 1 - beta_i^t
+ * for t = step + 1 formed in double and rounded to fp32 once.  float4 accesses where a tensor's five pointers are
+ * 16-byte aligned.  No atomics: bitwise reproducible.  Hyper-parameters outside torch's ranges (lr, eps, weight_decay
+ * < 0, betas outside [0, 1)) are VQB_ERR_BAD_ARG.  ceil(n / vqb_adam_capacity()) launches (none for empty tensors). */
+int vqb_adam_multi_f32(const vqb_adam_tensor *tensors, int n, double lr, double beta1, double beta2, double eps,
+                       double weight_decay, int amsgrad, void *stream);
+
+/* The layouts of vqb_repack_multi: each writes one packing of the fp32 parameter `src` (as PyTorch stores it) into
+ * `dst`, as the single-packing entry point named writes it.                                                        */
+enum vqb_pack_layout {
+    VQB_PACK_F32 = 0,           /* K-major fp32 [kh*kw][Cout][Cin_pad] of a conv (transposed = 0) or transposed conv
+                                   (1), zero padded from Cin: vqb_pack_conv_weight_f32 (Cin_pad = Cin)              */
+    VQB_PACK_SHUFFLE_F32 = 1,   /* the [9][16][Cin] pixel-shuffle region of a k4 s2 transposed conv to Cout <= 4
+                                   channels (vqb_pack_conv_weight_f32 writes it after the K-major rows)             */
+    VQB_PACK_BF16 = 2,          /* VQB_PACK_F32 in bf16: vqb_pack_conv_weight_bf16                                 */
+    VQB_PACK_SHUFFLE_BF16 = 3,  /* VQB_PACK_SHUFFLE_F32 in bf16: vqb_pack_conv_weight_bf16, VQB_CONVT_K4S2_OUT     */
+    VQB_PACK_PRIOR_F32 = 4,     /* [(r*cols + s)*Cin + ci][co] over the kept taps r < rows, s < cols: vqb_prior_pack_f32 */
+    VQB_PACK_MASK_ZERO = 5      /* no packing: zeroes the taps r >= rows or s >= cols of the (Cout,Cin,kh,kw)
+                                   parameter `dst` itself (a mask-A layer's); `src` unused.  Those taps are read by
+                                   no packing of the same call                                                      */
+};
+
+typedef struct vqb_pack_desc {
+    void *dst;
+    const float *src;
+    int layout, Cout, Cin, Cin_pad, kh, kw, transposed, rows, cols;
+} vqb_pack_desc;
+
+/* Descriptors plus step counters per launch of vqb_repack_multi (480).                                              */
+int vqb_repack_capacity(void);
+/* Every packing of `descs`, then steps[i] += 1 for each of the n_steps device fp32 counters (issue it after the
+ * vqb_adam_multi_f32 calls that read them).  The descriptors must not write what another one reads.  Unknown layouts,
+ * NULL pointers, non-positive sizes, Cin_pad < Cin, rows / cols outside the kernel: VQB_ERR_BAD_ARG.
+ * ceil((n + n_steps) / vqb_repack_capacity()) launches.                                                             */
+int vqb_repack_multi(const vqb_pack_desc *descs, int n, float *const *steps, int n_steps, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

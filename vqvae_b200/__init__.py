@@ -9,6 +9,7 @@ from .modules import (Decoder, Encoder, ResidualLayer, ResidualStack, VectorQuan
 from .pipeline import HostPipeline, HostResult  # noqa: F401
 from .checkpoint import load_checkpoint, save_checkpoint  # noqa: F401
 from .prior import GatedPixelCNN  # noqa: F401
+from . import optim  # noqa: F401  (vqvae_b200.optim.Adam)
 
 __all__ = ["VQVAE", "VectorQuantizer", "Encoder", "Decoder", "ResidualLayer", "ResidualStack",
            "set_precision", "get_precision", "precision", "invalidate_packed", "packed_state", "HostPipeline",

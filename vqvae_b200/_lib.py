@@ -71,6 +71,10 @@ SIGNATURES = {
     "vqb_relu_backward_f32": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "vqb_conv_wgrad_workspace_bytes": (_sz, [_i] * 10),
     "vqb_conv_wgrad_f32": (_i, [_vp] * 4 + [_i] * 12 + [_vp, _sz, _vp]),
+    "vqb_adam_capacity": (_i, []),
+    "vqb_adam_multi_f32": (_i, [_vp, _i] + [C.c_double] * 5 + [_i, _vp]),
+    "vqb_repack_capacity": (_i, []),
+    "vqb_repack_multi": (_i, [_vp, _i, _vp, _i, _vp]),
 }
 
 PRIOR_MAX_LAYERS = 32       # VQB_PRIOR_MAX_LAYERS
@@ -99,6 +103,22 @@ class PriorGrads(C.Structure):
     """struct vqb_prior_grads"""
     _fields_ = [("layers", C.POINTER(PriorLayerGrads)), ("n_layers", _i), ("embedding", _vp), ("out1_w", _vp),
                 ("out1_b", _vp), ("out2_w", _vp), ("out2_b", _vp)]
+
+
+# enum vqb_pack_layout
+PACK_F32, PACK_SHUFFLE_F32, PACK_BF16, PACK_SHUFFLE_BF16, PACK_PRIOR_F32, PACK_MASK_ZERO = range(6)
+
+
+class AdamTensor(C.Structure):
+    """struct vqb_adam_tensor"""
+    _fields_ = [(n, _vp) for n in ("param", "grad", "exp_avg", "exp_avg_sq", "max_exp_avg_sq", "step")] + \
+        [("numel", _i64)]
+
+
+class PackDesc(C.Structure):
+    """struct vqb_pack_desc"""
+    _fields_ = [("dst", _vp), ("src", _vp)] + [(n, _i) for n in ("layout", "Cout", "Cin", "Cin_pad", "kh", "kw",
+                                                                 "transposed", "rows", "cols")]
 
 
 def lib():

@@ -2,45 +2,26 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "pack.cuh"
 
 namespace {
 
-// (Cout,Cin,kh,kw) or ConvTranspose (Cin,Cout,kh,kw)  ->  K-major rows [(r*kw+s)][co][ci] of Cin_pad >= Cin
-// channels, zero padded: the B operand of every conv kernel.  T = float or __nv_bfloat16 (rounded to nearest even).
+// the K-major packing of pack_kmajor_at.  T = float or __nv_bfloat16 (rounded to nearest even).
 template <typename T>
 __global__ void pack_weight_kernel(const float *__restrict__ w, T *__restrict__ out, int Cout, int Cin, int Cin_pad,
                                    int kh, int kw, int transposed) {
     const long long total = (long long)Cout * Cin_pad * kh * kw;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        const int ci = (int)(i % Cin_pad);
-        long long t = i / Cin_pad;
-        const int co = (int)(t % Cout);
-        const int tap = (int)(t / Cout);
-        const int r = tap / kw, s = tap % kw;
-        const long long src = transposed ? ((((long long)ci * Cout + co) * kh + r) * kw + s)
-                                         : ((((long long)co * Cin + ci) * kh + r) * kw + s);
-        out[i] = T(ci < Cin ? w[src] : 0.f);
-    }
+         i += (long long)gridDim.x * blockDim.x)
+        out[i] = T(pack_kmajor_at(w, i, Cout, Cin, Cin_pad, kh, kw, transposed));
 }
 
-// ConvTranspose2d k4 s2 p1 weight (Cin,Cout,4,4), Cout <= 4  ->  [9 neighbour taps (dy,dx)][16][Cin]:
-// row (py*2+px)*Cout+co of tap (dy,dx) holds W[ci][co][py-2dy+1][px-2dx+1] when that kernel index
-// exists (the neighbour contributes to that output phase), else 0.  Read by launch_convt_shuffle_wg (wgconv.cu).
+// the [9][16][Cin] pixel-shuffle packing of pack_shuffle_at
 template <typename T>
 __global__ void pack_convt_shuffle_kernel(const float *__restrict__ w, T *__restrict__ out, int Cout, int Cin) {
     const int total = 9 * 16 * Cin;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        const int ci = i % Cin, row = (i / Cin) % 16, tap = i / (16 * Cin);
-        const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-        float v = 0.f;
-        if (row < 4 * Cout) {
-            const int co = row % Cout, ph = row / Cout, py = ph >> 1, px = ph & 1;
-            const int kh = py - 2 * dy + 1, kw = px - 2 * dx + 1;
-            if (kh >= 0 && kh < 4 && kw >= 0 && kw < 4) v = w[(((size_t)ci * Cout + co) * 4 + kh) * 4 + kw];
-        }
-        out[i] = T(v);
-    }
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x)
+        out[i] = T(pack_shuffle_at(w, i, Cout, Cin));
 }
 
 // tiled transpose of the innermost two logical axes: in[b][R][Ccols] -> out[b][Ccols][R]

@@ -6,6 +6,7 @@
 // started from 0, then the bias: the value of an element does not depend on which positions share a block or on how
 // many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
 // sampler's logits are bitwise the forward's logits on the grid it produced.
+#include "pack.cuh"
 #include "prior.cuh"
 
 namespace {
@@ -335,17 +336,12 @@ __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act 
     }
 }
 
-// conv weight (Cout, Cin, kh, kw) -> [(r*cols + s)*Cin + ci][co] for the kept taps r < rows, s < cols
+// the kept-tap packing of pack_prior_at
 __global__ void pack_kernel(const float *__restrict__ w, float *__restrict__ out, int Cout, int Cin, int kh, int kw,
                             int rows, int cols) {
     const long long total = (long long)rows * cols * Cin * Cout;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int co = (int)(i % Cout);
-        const long long t = i / Cout;
-        const int ci = (int)(t % Cin), tap = (int)(t / Cin);
-        const int r = tap / cols, sc = tap % cols;
-        out[i] = w[(((long long)co * Cin + ci) * kh + r) * kw + sc];
-    }
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
+        out[i] = pack_prior_at(w, i, Cout, Cin, kh, kw, cols);
 }
 
 __global__ void gate_kernel(const float *__restrict__ x, float *__restrict__ out, long long outer, int C,

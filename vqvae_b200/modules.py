@@ -27,7 +27,7 @@ import contextlib
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import _lib, ops
 from .dist import reduce_vq_stats
 from ._lib import NCHW, NHWC, PRECISIONS, RES_W2
 
@@ -93,11 +93,43 @@ def _packed_current(param, key):
     return hit is not None and hit[0] == tag and tag[0] is not None
 
 
+def pack_spec(param, key):
+    """The one place a packing-cache key becomes a layout and its geometry, for the conv weight `param`:
+    ("f32", transposed), ("bf16", kind) (the residual 1x1's RES_W2 kind pads Cin to the kernels' 64) or
+    ("prior", rows, cols), the kept taps of a prior conv (vqvae_b200/prior.py).  Returns (pack, layouts):
+    pack(param, out) runs the key's single-packing entry point (refilling `out` when it has the right size) and returns
+    the buffer, or None for a bf16 shape the kernels do not cover; layouts is the same packing as vqb_repack_multi
+    descriptors, a list of (byte offset into that buffer, PackDesc fields), empty when there is no packing."""
+    kind = key[0]
+    if kind == "prior":
+        cout, cin, kh, kw = param.shape
+        f = dict(layout=_lib.PACK_PRIOR_F32, Cout=cout, Cin=cin, Cin_pad=cin, kh=kh, kw=kw, transposed=0,
+                 rows=key[1], cols=key[2])
+        return (lambda p, out: ops.prior_pack_weight(p, key[1], key[2], out=out)), [(0, f)]
+    transposed = bool(key[1]) if kind == "f32" else ops.KIND_GEOMETRY[key[1]][2]
+    cin, cout, kh, kw = param.shape if transposed else (param.shape[1], param.shape[0]) + tuple(param.shape[2:])
+    geo = dict(Cout=cout, Cin=cin, kh=kh, kw=kw, transposed=int(transposed), rows=0, cols=0)
+    if kind == "f32":
+        layouts = [(0, dict(geo, layout=_lib.PACK_F32, Cin_pad=cin))]
+        if transposed and kh == 4 and kw == 4 and cout <= 4:         # vqb_pack_conv_weight_f32 adds the shuffle form
+            layouts.append((4 * kh * kw * cout * cin, dict(geo, layout=_lib.PACK_SHUFFLE_F32, Cin_pad=cin)))
+        return (lambda p, out: ops.pack_conv_weight(p, key[1], out=out)), layouts
+    nbytes = ops.lib().vqb_conv_bf16_packed_bytes(key[1], cout, cin)
+    if nbytes == 0:
+        layouts = []
+    elif key[1] == _lib.CONVT_K4S2_OUT:
+        layouts = [(0, dict(geo, layout=_lib.PACK_SHUFFLE_BF16, Cin_pad=cin))]
+    else:                                                               # the padded channel count, from the byte size
+        layouts = [(0, dict(geo, layout=_lib.PACK_BF16, Cin_pad=nbytes // (2 * kh * kw * cout)))]
+    return (lambda p, out: ops.pack_conv_weight_bf16(p, key[1], out=out)), layouts
+
+
 def _packed(param, key):
-    """The packing `key` (see _pack_key) of a conv weight, cached ON the parameter object (so the cache dies with it).
-    When the parameter changes (load_state_dict, optimizer step, .to()) the SAME device buffer is repacked in place
-    whenever its size still fits, so CUDA graphs captured around a forward keep reading current weights after
-    ``repack`` (HostPipeline checks the tags before every replay)."""
+    """The packing `key` (see _pack_key, pack_spec) of a conv weight, cached ON the parameter object (so the cache
+    dies with it).  When the parameter changes (load_state_dict, optimizer step, .to()) the SAME device buffer is
+    repacked in place whenever its size still fits, so CUDA graphs captured around a forward keep reading current
+    weights after ``repack`` (HostPipeline checks the tags before every replay).  vqvae_b200.optim.Adam refreshes
+    every cached packing of the parameters it updates in the same buffers, and their tags with them."""
     cache = getattr(param, "_vqb_packed", None)
     if cache is None:
         cache = {}
@@ -107,11 +139,8 @@ def _packed(param, key):
         return hit[1]
     tag = _param_tag(param)
     old = hit[1] if hit is not None and hit[1] is not None and hit[1].device == param.device else None
-    if key[0] == "prior":            # ("prior", rows, cols): the kept taps of a prior conv (vqvae_b200/prior.py)
-        buf = ops.prior_pack_weight(param, key[1], key[2], out=old)
-    else:
-        pack = ops.pack_conv_weight if key[0] == "f32" else ops.pack_conv_weight_bf16
-        buf = pack(param, key[1], out=old)
+    pack, _ = pack_spec(param, key)
+    buf = pack(param, old)
     cache[key] = (tag, buf)
     return buf
 

@@ -534,3 +534,20 @@ def prior_backward(net, codes, labels, d_logits, saved, grads, precision="fp32")
                                                        W, d_logits.data_ptr(), saved.data_ptr(), _lib.C.byref(grads),
                                                        ws.data_ptr(), ws.numel(), _stream()), "prior_backward")
     span.done()
+
+
+# ---- optimizer step (vqb_adam_multi_f32 / vqb_repack_multi) -------------------------------------------------------
+def adam_multi(tensors, n, lr, beta1, beta2, eps, weight_decay, amsgrad):
+    """Adam over a ctypes array of n AdamTensor descriptors (device pointers; read during the call only)."""
+    span = _Span(f"adam x{n}")
+    check(lib().vqb_adam_multi_f32(tensors, n, float(lr), float(beta1), float(beta2), float(eps), float(weight_decay),
+                                   int(bool(amsgrad)), _stream()), "adam_multi")
+    span.done()
+
+
+def repack_multi(descs, n, steps, n_steps):
+    """Every packing of a ctypes array of n PackDesc descriptors, then +1 on each of the n_steps device fp32 step
+    counters of the ctypes pointer array `steps`."""
+    span = _Span(f"repack x{n}")
+    check(lib().vqb_repack_multi(descs, n, steps, n_steps, _stream()), "repack_multi")
+    span.done()

@@ -126,6 +126,16 @@ class GatedMaskedConv2d(nn.Module):
         self.horiz_stack = nn.Conv2d(dim, dim * 2, (1, half + 1), 1, (0, half))
         self.horiz_resid = nn.Conv2d(dim, dim, 1)
         self.gate = GatedActivation()
+        self._mark_mask_a()
+
+    def _mark_mask_a(self):
+        """A mask-A layer marks its two stacks' weights with the taps make_causal keeps, (rows, cols), so that
+        vqvae_b200.optim.Adam zeroes the others after each update.  Done when the layer is built, and again before each
+        packing (a parameter replaced or deep-copied since has lost the mark)."""
+        if self.mask_type == "A":
+            vs, hs = self.vert_stack, self.horiz_stack
+            vs.weight._vqb_mask_a = (vs.kernel_size[0] - 1, vs.kernel_size[1])
+            hs.weight._vqb_mask_a = (1, hs.kernel_size[1] - 1)
 
     def make_causal(self):
         """Zero the taps mask A excludes: the vertical stack's last row, the horizontal stack's last column."""
@@ -138,6 +148,7 @@ class GatedMaskedConv2d(nn.Module):
         vs, hs = self.vert_stack, self.horiz_stack
         vkey = ("prior", vs.kernel_size[0] - mask_a, vs.kernel_size[1])
         hkey = ("prior", 1, hs.kernel_size[1] - mask_a)
+        self._mark_mask_a()
         if mask_a and not (_packed_current(vs.weight, vkey) and _packed_current(hs.weight, hkey)):
             self.make_causal()          # P3: once per change of the parameters, right before they are packed
         t = dict(vert_w=_packed(vs.weight, vkey), vert_b=_f32(vs.bias),
