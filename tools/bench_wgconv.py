@@ -11,8 +11,9 @@ pointers, which the caching allocator keeps mapped; only timing is read from the
 Beside each time: the modelled L2->SM bytes of the launch under two operand schemes -- "per-tap" (one 128-pixel A box
 per k-step, what wgconv_kernel loads) and "halo" (each tile's input halo once per chunk, the alternative) -- both with
 the N weight rows of every k-step, and the achieved bytes/s of each; the algorithmic FLOP/s; the card name and power
-limit.  The output layer (convT to <= 4 channels) runs in scatter form, which loads each tile's halo once per chunk:
-both columns give that launch's bytes.  Prints one JSON line.  Nothing is written to the repository tree.
+limit.  The output layer (convT to <= 4 channels) runs in scatter form, which loads each tile's halo once per chunk,
+and so do the TF32 residual launches whose tiles hold whole images (res_scatter_kernel, which loads each tile once
+for all applications): both columns give those launches' bytes.  Prints one JSON line.  Nothing is written to the repository tree.
 """
 import argparse
 import json
@@ -61,6 +62,13 @@ def traffic(label, B):
             parts = [parts[0]] + parts[2:]
         c, cm, _ = (int(v) for v in parts[1].split("->"))
         h, w = (int(v) for v in parts[2].split("x"))
+        if not bf and cm == 32 and c in (64, 128) and w <= 16 and _p2(w) * _p2(h) <= 128:
+            # scatter form (res_scatter_kernel): the whole-image tile once, then per application 3 passes x nc chunks
+            # of 96 weight rows (one kernel row's taps), and the 1x1 weight once per CTA; both schemes alike
+            nc = c // 32
+            ctas = -(-B // (128 // (_p2(w) * _p2(h))))
+            moved = ctas * (nc * 128 * 128 + napps * 3 * nc * 96 * 128 + c * 128)
+            return ctas, napps * 3 * nc, moved, moved
         cin, N, nph, taps, step, ext = c, _p2(max(cm, 16)), 1, 9, 1, 2
         w2 = c * 128 * (1 if bf else max(cm // 32, 1))
         grid = [(h, w)]

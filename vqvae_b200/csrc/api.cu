@@ -259,7 +259,8 @@ extern "C" int vqb_residual_stack_f32(const float *r, const float *w1_packed, co
     if (precision < VQB_FP32 || precision > VQB_BF16) return VQB_ERR_BAD_ARG;
     if (precision == VQB_BF16) return VQB_ERR_UNSUPPORTED;
     if (n_layers > 1 && precision == VQB_TF32 && res_wg_supported(0, C, Cmid)) {
-        // all applications in ONE launch when a tile holds whole images (answers VQB_ERR_UNSUPPORTED otherwise)
+        // all applications in ONE launch when a tile holds whole images and Cmid = 32 (res_scatter_kernel; answers
+        // VQB_ERR_UNSUPPORTED otherwise)
         const int rc = launch_res_wg(0, r, w1_packed, w2_packed, out, B, H, W, C, Cmid, 1, n_layers, (cudaStream_t)stream);
         if (rc != VQB_ERR_UNSUPPORTED) return rc;
     }

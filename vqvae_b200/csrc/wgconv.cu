@@ -36,7 +36,6 @@ struct WgParams {
     int BW, BH, BN, tiles_x, tiles_y;
     int in_step, out_step, stages;
     int relu, out_bf16;
-    int napps;                                // applications of a chained residual layer (whole-image tiles when > 1)
     int OHg[4], OWg[4], out_py[4], out_px[4], nsteps[4];
     long long out_sn, out_sh, out_sw, out_sc;
     int4 steps[4][WG_MAX_STEPS];              // x = c0, y = dx, z = dy, w = w_row
@@ -72,7 +71,6 @@ __device__ __forceinline__ void store_tile(const WgParams &p, const float *acc, 
                 *reinterpret_cast<uint32_t *>(reinterpret_cast<__nv_bfloat16 *>(p.out) + ob + c) = pack_bf16(v0, v1);
             } else {
                 if (skip) {
-                    // plain load: with chained applications skip is `out`, written earlier by this kernel
                     const float2 sk = *reinterpret_cast<const float2 *>(reinterpret_cast<const float *>(skip) + ob + c);
                     v0 += sk.x; v1 += sk.y;
                 }
@@ -90,8 +88,7 @@ __host__ __device__ constexpr int chain_chunks() { return BF16 ? 1 : (N >= 32 ? 
 template <bool BF16, int N, int N2>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant__ CUtensorMap tma_w,
-              const __grid_constant__ CUtensorMap tma_w2, const __grid_constant__ CUtensorMap tma_out,
-              const __grid_constant__ WgParams p) {
+              const __grid_constant__ CUtensorMap tma_w2, const __grid_constant__ WgParams p) {
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
     const uint32_t sbase = (raw + 1023u) & ~1023u;
@@ -105,7 +102,6 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
     auto full = [&](int s) { return bars + 8u * s; };
     auto empty = [&](int s) { return bars + 8u * (WG_MAX_STAGES + s); };
     const uint32_t w2bar = bars + 8u * (2 * WG_MAX_STAGES);
-    constexpr int APP_BAR = 3, APP_THREADS = 32 + 256;       // producer warp + both consumer warpgroups
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ph = blockIdx.y;
@@ -124,7 +120,6 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
         ptx::prefetch_tmap(&tma_in);
         ptx::prefetch_tmap(&tma_w);
         if (N2 > 0) ptx::prefetch_tmap(&tma_w2);
-        if (p.napps > 1) ptx::prefetch_tmap(&tma_out);
     }
     __syncthreads();
     pdl_launch_dependents();           // the next layer may start its prologue
@@ -138,23 +133,16 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
             }
         }
         pdl_wait();                    // ... the activations do
-        int g = 0;                     // ring position, continued across applications
-        for (int app = 0; app < p.napps; ++app) {
-            // application app > 0 reads what app - 1 wrote to `out` (whole images per tile: no other CTA touches them)
-            if (app > 0) ptx::named_bar_sync(APP_BAR, APP_THREADS);
-            const CUtensorMap *src = app == 0 ? &tma_in : &tma_out;
-            if (lane == 0) {
-                for (int i = 0; i < nsteps; ++i, ++g) {
-                    const int s = g % S;
-                    if (g >= S) ptx::mbar_wait(empty(s), (uint32_t)((g / S - 1) & 1));
-                    const int4 st = p.steps[ph][i];
-                    const uint32_t dst = sbase + (uint32_t)(s * STAGE);
-                    ptx::mbar_expect_tx(full(s), (uint32_t)STAGE);
-                    ptx::tma_load_4d(dst, src, full(s), st.x, gx0 * p.in_step + st.y, gy0 * p.in_step + st.z, n0);
-                    ptx::tma_load_2d(dst + A_BYTES, &tma_w, full(s), st.x, st.w);
-                }
+        if (lane == 0) {
+            for (int i = 0; i < nsteps; ++i) {
+                const int s = i % S;
+                if (i >= S) ptx::mbar_wait(empty(s), (uint32_t)((i / S - 1) & 1));
+                const int4 st = p.steps[ph][i];
+                const uint32_t dst = sbase + (uint32_t)(s * STAGE);
+                ptx::mbar_expect_tx(full(s), (uint32_t)STAGE);
+                ptx::tma_load_4d(dst, &tma_in, full(s), st.x, gx0 * p.in_step + st.y, gy0 * p.in_step + st.z, n0);
+                ptx::tma_load_2d(dst + A_BYTES, &tma_w, full(s), st.x, st.w);
             }
-            __syncwarp();
         }
         return;
     }
@@ -162,79 +150,69 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
 
     pdl_wait();                        // skip / out may belong to the previous layer
     const int wgi = (warp >> 2) - 1;   // pixel rows 64 * wgi .. + 63 of the tile
-    int g = 0;
-    for (int app = 0; app < p.napps; ++app) {
-        const bool last = app + 1 == p.napps;
-        const void *skip = app == 0 ? p.skip : p.out;
-        const int relu = last ? p.relu : 1;
-        float acc[N / 2];
+    float acc[N / 2];
 #pragma unroll
-        for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-        for (int i = 0; i < nsteps; ++i, ++g) {
-            const int s = g % S;
-            ptx::mbar_wait(full(s), (uint32_t)((g / S) & 1));
-            const uint32_t a = sbase + (uint32_t)(s * STAGE) + (uint32_t)(wgi * 64 * 128), b = sbase + (uint32_t)(s * STAGE) + A_BYTES;
-            wg::fence();
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < nsteps; ++i) {
+        const int s = i % S;
+        ptx::mbar_wait(full(s), (uint32_t)((i / S) & 1));
+        const uint32_t a = sbase + (uint32_t)(s * STAGE) + (uint32_t)(wgi * 64 * 128), b = sbase + (uint32_t)(s * STAGE) + A_BYTES;
+        wg::fence();
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) wg::mma<BF16, N>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
-            wg::commit();
-            wg::wait<0>();
-            wg::fence_regs<N>(acc);
-            if ((warp & 3) == 0 && lane == 0) ptx::mbar_arrive(empty(s));
-        }
+        for (int kk = 0; kk < 4; ++kk) wg::mma<BF16, N>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs<N>(acc);
+        if ((warp & 3) == 0 && lane == 0) ptx::mbar_arrive(empty(s));
+    }
 
-        if constexpr (N2 == 0) {
-            store_tile<N>(p, acc, ph, wgi, gx0, gy0, n0, skip, relu);
-        } else {
-            // relu(first GEMM) -> rows of 128 bytes (64 bf16 / 32 fp32 channels per chunk), 128-byte swizzle: 16-byte
-            // piece j of row r sits at j ^ (r & 7)
-            const int wl = warp & 3, cq = 2 * (lane & 3);
+    if constexpr (N2 == 0) {
+        store_tile<N>(p, acc, ph, wgi, gx0, gy0, n0, p.skip, p.relu);
+    } else {
+        // relu(first GEMM) -> rows of 128 bytes (64 bf16 / 32 fp32 channels per chunk), 128-byte swizzle: 16-byte
+        // piece j of row r sits at j ^ (r & 7)
+        const int wl = warp & 3, cq = 2 * (lane & 3);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
-                const uint32_t rb = mid + (uint32_t)(row * 128);
-                if constexpr (BF16) {
+        for (int h = 0; h < 2; ++h) {
+            const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
+            const uint32_t rb = mid + (uint32_t)(row * 128);
+            if constexpr (BF16) {
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int c = 8 * j + cq;
-                        float v0 = 0.f, v1 = 0.f;
-                        if (j < N / 8 && c < p.mid_cols) { v0 = fmaxf(acc[4 * j + 2 * h], 0.f); v1 = fmaxf(acc[4 * j + 2 * h + 1], 0.f); }
-                        const uint32_t addr = rb + (uint32_t)(((j ^ (row & 7)) << 4) + cq * 2);
-                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16(v0, v1)) : "memory");
-                    }
-                } else {
+                for (int j = 0; j < 8; ++j) {
+                    const int c = 8 * j + cq;
+                    float v0 = 0.f, v1 = 0.f;
+                    if (j < N / 8 && c < p.mid_cols) { v0 = fmaxf(acc[4 * j + 2 * h], 0.f); v1 = fmaxf(acc[4 * j + 2 * h + 1], 0.f); }
+                    const uint32_t addr = rb + (uint32_t)(((j ^ (row & 7)) << 4) + cq * 2);
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16(v0, v1)) : "memory");
+                }
+            } else {
 #pragma unroll
-                    for (int j = 0; j < N / 8; ++j) {
-                        const int c = 8 * j + cq, piece = (c & 31) >> 2;
-                        const float v0 = fmaxf(acc[4 * j + 2 * h], 0.f), v1 = fmaxf(acc[4 * j + 2 * h + 1], 0.f);
-                        const uint32_t addr = rb + (uint32_t)((c >> 5) * A_BYTES) + (uint32_t)(((piece ^ (row & 7)) << 4) + (c & 3) * 4);
-                        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
-                    }
+                for (int j = 0; j < N / 8; ++j) {
+                    const int c = 8 * j + cq, piece = (c & 31) >> 2;
+                    const float v0 = fmaxf(acc[4 * j + 2 * h], 0.f), v1 = fmaxf(acc[4 * j + 2 * h + 1], 0.f);
+                    const uint32_t addr = rb + (uint32_t)((c >> 5) * A_BYTES) + (uint32_t)(((piece ^ (row & 7)) << 4) + (c & 3) * 4);
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
                 }
             }
-            ptx::fence_proxy_async();                        // generic-proxy writes -> visible to wgmma
-            ptx::named_bar_sync(1 + wgi, 128);               // this warpgroup's 64 rows are complete
-            ptx::mbar_wait(w2bar, 0);
-            float acc2[N2 > 0 ? N2 / 2 : 1];
-#pragma unroll
-            for (int i = 0; i < N2 / 2; ++i) acc2[i] = 0.f;
-            wg::fence();
-#pragma unroll
-            for (int c = 0; c < KC2; ++c) {
-                const uint32_t a = mid + (uint32_t)(c * A_BYTES + wgi * 64 * 128), b = w2s + (uint32_t)(c * N2 * 128);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk)
-                    wg::mma<BF16, N2>(acc2, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
-            }
-            wg::commit();
-            wg::wait<0>();
-            wg::fence_regs<N2>(acc2);
-            store_tile<N2>(p, acc2, ph, wgi, gx0, gy0, n0, skip, relu);
         }
-        if (!last) {
-            asm volatile("fence.proxy.async.global;" ::: "memory");      // these stores -> the next application's TMA reads
-            ptx::named_bar_sync(APP_BAR, APP_THREADS);
+        ptx::fence_proxy_async();                        // generic-proxy writes -> visible to wgmma
+        ptx::named_bar_sync(1 + wgi, 128);               // this warpgroup's 64 rows are complete
+        ptx::mbar_wait(w2bar, 0);
+        float acc2[N2 > 0 ? N2 / 2 : 1];
+#pragma unroll
+        for (int i = 0; i < N2 / 2; ++i) acc2[i] = 0.f;
+        wg::fence();
+#pragma unroll
+        for (int c = 0; c < KC2; ++c) {
+            const uint32_t a = mid + (uint32_t)(c * A_BYTES + wgi * 64 * 128), b = w2s + (uint32_t)(c * N2 * 128);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+                wg::mma<BF16, N2>(acc2, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
         }
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs<N2>(acc2);
+        store_tile<N2>(p, acc2, ph, wgi, gx0, gy0, n0, p.skip, p.relu);
     }
 }
 
@@ -244,7 +222,7 @@ int pow2_ceil(int x) {
     return p;
 }
 
-typedef void (*wg_fn)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, WgParams);
+typedef void (*wg_fn)(CUtensorMap, CUtensorMap, CUtensorMap, WgParams);
 
 template <bool BF16, int N2>
 wg_fn pick_n(int N) {
@@ -296,8 +274,6 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     q.B = L.B; q.ncols = L.ncols; q.mid_cols = L.ncols;
     q.in_step = L.in_step; q.out_step = L.out_step;
     q.relu = L.relu; q.out_bf16 = L.out_bf16;
-    q.napps = L.napps;
-    if (L.napps < 1 || (L.napps > 1 && (L.N2 == 0 || L.Cin != L.N2 || L.skip != L.in))) return VQB_ERR_UNSUPPORTED;
     q.out_sn = L.out_sn; q.out_sh = L.out_sh; q.out_sw = L.out_sw; q.out_sc = L.out_sc;
     int maxw = 0, maxh = 0, maxk = 1;
     for (int i = 0; i < L.nph; ++i) {
@@ -319,10 +295,9 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     q.tiles_x = (maxw + q.BW - 1) / q.BW;
     q.tiles_y = (maxh + q.BH - 1) / q.BH;
     const long long tiles_n = (L.B + q.BN - 1) / q.BN;
-    if (L.napps > 1 && (q.tiles_x != 1 || q.tiles_y != 1 || L.nph != 1)) return VQB_ERR_UNSUPPORTED;     // whole images per tile
 
     const CUtensorMapDataType dt = L.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    CUtensorMap tin, tw, tw2, tout;
+    CUtensorMap tin, tw, tw2;
     const uint64_t dims[4] = {(uint64_t)L.Cin, (uint64_t)L.W, (uint64_t)L.H, (uint64_t)L.B};
     const uint64_t strides[3] = {(uint64_t)L.Cin * esz, (uint64_t)L.W * L.Cin * esz, (uint64_t)L.H * L.W * L.Cin * esz};
     const uint32_t box[4] = {(uint32_t)ck, (uint32_t)(q.BW * L.in_step), (uint32_t)(q.BH * L.in_step), (uint32_t)q.BN};
@@ -333,7 +308,6 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
                             (uint32_t)L.N, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     tw2 = tw;
-    tout = tin;
     int kc2 = 0;
     if (L.N2 > 0) {
         if (L.ncols > 64 || L.w2_inner % ck != 0) return VQB_ERR_UNSUPPORTED;
@@ -342,10 +316,6 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
         q.mid_cols = L.ncols; q.ncols = L.N2;
         rc = vqb_encode_tmap_2d(&tw2, dt, L.w2, (uint64_t)L.w2_inner, (uint64_t)L.w2_rows, (uint64_t)L.w2_inner * esz, (uint32_t)ck,
                                 (uint32_t)L.N2, CU_TENSOR_MAP_SWIZZLE_128B);
-        if (rc) return rc;
-    }
-    if (L.napps > 1) {
-        rc = vqb_encode_tmap_4d(&tout, dt, L.out, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
     }
     const long long grid = (long long)q.tiles_x * q.tiles_y * tiles_n;
@@ -381,7 +351,7 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     }
     q.stages = stages;
     const int smem = stages * stage + fixed;
-    if (cudaError_t le = vqb_launch(fn, dim3((unsigned)grid, (unsigned)L.nph), dim3(WG_THREADS), (size_t)smem, s, tin, tw, tw2, tout, q))
+    if (cudaError_t le = vqb_launch(fn, dim3((unsigned)grid, (unsigned)L.nph), dim3(WG_THREADS), (size_t)smem, s, tin, tw, tw2, q))
         return (int)le;
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
@@ -432,27 +402,265 @@ int launch_conv_tc(WgLaunch &L, const ConvPhase *ph, int nph, int total_taps, bo
 }
 
 // ------------------------------------------------------------------------------------------------ residual layer
-// residual.py:18-29 on NHWC activations: per 128-pixel tile the 3x3 GEMM (C -> Cmid), ReLU, the 1x1 GEMM (Cmid -> C)
-// on the intermediate held in shared memory (fp32, or rounded to bf16), + r, ReLU.  In TF32 this is the arithmetic of
-// the two separate conv launches (same k-step order, same TF32 operands), in one launch.  napps > 1 (a ResidualStack
-// of one shared layer): whole images per tile, every application inside the same launch, the activation
-// round-tripping through `out` (L2) between them.
+// residual.py:18-29 on NHWC activations: the 3x3 GEMM (C -> Cmid), ReLU, the 1x1 GEMM (Cmid -> C) on the intermediate
+// held in shared memory (fp32, or rounded to bf16), + r, ReLU.  Two kernels:
+//   * res_scatter_kernel (TF32, Cmid = 32, a 128-pixel tile holds whole images): the 3x3 conv in scatter form, and
+//     every application of a ResidualStack in the same launch.  Per CTA the tile r_i is loaded once, one unshifted
+//     TMA box per 32-channel chunk, and stays in shared memory as the A operand.  Per kernel row dy (3 passes):
+//         Y[p][dx, co] = r_i[p] . w1[tap (dy, dx)][co]                       (m64n96, N = 3 taps x 32 channels)
+//     staged in shared memory; each consumer thread owns 16 (pixel, co) outputs of the intermediate and adds the
+//     neighbours' terms, m[q][co] = sum over t = 0..8 in raster order of Y[q + (dy, dx)][dx, co], dropping the
+//     neighbours outside the image (the zero padding).  Then relu(m) -> the 1x1 GEMM, + r_i (from the resident
+//     tile), ReLU.  Between applications the result overwrites the resident tile in place (pixels outside the image
+//     or past the batch as zero: the next application's padding); only the last application stores to `out`.
+//   * otherwise wgconv_kernel with N2 = C: per tile the 3x3 GEMM's k-steps (the two separate conv launches' order
+//     and operands in TF32), ReLU, the chained 1x1 GEMM.  One application per launch.
+// Which kernel runs depends only on (bf16, C, Cmid, H, W), so a stack and its layers one by one compute the same bits.
+constexpr int RS_MID = 32;                 // Cmid
+constexpr int RS_N = 3 * RS_MID;           // GEMM columns per pass: one kernel row's 3 taps x Cmid
+constexpr int RS_WBYTES = RS_N * 128;      // one pass's weight rows, one 128-byte channel chunk
+constexpr int RS_YS = RS_N + 8;            // staged floats per pixel: + 8 against bank conflicts of the fragment stores
+constexpr int RS_MAX_STAGES = 4;
+
+struct RsParams {
+    float *out;
+    int B, H, W, BW, BH, BN, napps, relu, stages;
+};
+
+template <int C>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant__ CUtensorMap tma_w1,
+                   const __grid_constant__ CUtensorMap tma_w2, const __grid_constant__ RsParams p) {
+    constexpr int NC = C / 32;
+    extern __shared__ unsigned char smem_raw[];
+    const uint32_t raw = ptx::smem_u32(smem_raw);
+    const uint32_t act = (raw + 1023u) & ~1023u;                  // NC chunks [128 px][128 B]: r_i, the A operand
+    const uint32_t ring = act + (uint32_t)(NC * A_BYTES);          // stages of one pass's w1 rows [96][128 B]
+    const uint32_t mid = ring + (uint32_t)(p.stages * RS_WBYTES);  // relu(m) [128 px][128 B]
+    const uint32_t w2s = mid + (uint32_t)A_BYTES;                  // w2 [C][128 B]
+    const uint32_t ysm = w2s + (uint32_t)(C * 128);                // Y [128 px][RS_YS] floats
+    const uint32_t bars = ysm + (uint32_t)(128 * RS_YS * 4);
+    float *const Y = reinterpret_cast<float *>(smem_raw + (ysm - raw));
+    auto full = [&](int s) { return bars + 8u * s; };
+    auto empty = [&](int s) { return bars + 8u * (RS_MAX_STAGES + s); };
+    const uint32_t abar = bars + 8u * (2 * RS_MAX_STAGES), w2bar = abar + 8u;
+    const int S = p.stages;
+    const int total = p.napps * 3 * NC;        // ring slots: application, pass (kernel row), chunk, innermost last
+    const int n0 = blockIdx.x * p.BN;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), 2); }
+        ptx::mbar_init(abar, 1);
+        ptx::mbar_init(w2bar, 1);
+        ptx::fence_mbar_init();
+    }
+    if (tid == 32) {
+        ptx::prefetch_tmap(&tma_in);
+        ptx::prefetch_tmap(&tma_w1);
+        ptx::prefetch_tmap(&tma_w2);
+    }
+    __syncthreads();
+    pdl_launch_dependents();
+
+    if (warp == 0) {
+        auto load_w1 = [&](int g) {
+            const int s = g % S;
+            ptx::mbar_expect_tx(full(s), (uint32_t)RS_WBYTES);
+            ptx::tma_load_2d(ring + (uint32_t)(s * RS_WBYTES), &tma_w1, full(s), (g % NC) * 32, ((g / NC) % 3) * RS_N);
+        };
+        const int pre = total < S ? total : S;
+        if (lane == 0) {               // weights do not depend on the previous layer
+            ptx::mbar_expect_tx(w2bar, (uint32_t)(C * 128));
+            ptx::tma_load_2d(w2s, &tma_w2, w2bar, 0, 0);
+            for (int g = 0; g < pre; ++g) load_w1(g);
+        }
+        pdl_wait();                    // ... the activations do
+        if (lane == 0) {
+            ptx::mbar_expect_tx(abar, (uint32_t)(NC * A_BYTES));
+            for (int c = 0; c < NC; ++c) ptx::tma_load_4d(act + (uint32_t)(c * A_BYTES), &tma_in, abar, c * 32, 0, 0, n0);
+            for (int g = pre; g < total; ++g) {
+                ptx::mbar_wait(empty(g % S), (uint32_t)((g / S - 1) & 1));
+                load_w1(g);
+            }
+        }
+        return;
+    }
+    if (warp < 4) return;
+
+    pdl_wait();                        // `out` may still be read by the previous layer
+    const int wgi = (warp >> 2) - 1, wl = warp & 3, cw = warp - 4, cq = 2 * (lane & 3);
+    const int lbw = __ffs(p.BW) - 1, lbh = __ffs(p.BH) - 1;
+    ptx::mbar_wait(abar, 0);
+    ptx::mbar_wait(w2bar, 0);
+    int g = 0;
+    for (int app = 0; app < p.napps; ++app) {
+        const bool last = app + 1 == p.napps;
+        float m[16];                   // intermediate channel `lane` of pixels 16 cw .. + 15, taps added in raster order
+#pragma unroll
+        for (int i = 0; i < 16; ++i) m[i] = 0.f;
+#pragma unroll 1
+        for (int r = 0; r < 3; ++r) {
+            float acc[RS_N / 2];       // the first k-step overwrites (scale-d 0): no register writes between the wgmma
+            for (int c = 0; c < NC; ++c, ++g) {
+                const int s = g % S;
+                ptx::mbar_wait(full(s), (uint32_t)((g / S) & 1));
+                const uint32_t a = act + (uint32_t)(c * A_BYTES + wgi * 64 * 128), b = ring + (uint32_t)(s * RS_WBYTES);
+                wg::fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) wg::mma<false, RS_N>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), (c | kk) != 0);
+                wg::commit();
+                wg::wait<0>();
+                wg::fence_regs<RS_N>(acc);
+                if (wl == 0 && lane == 0) ptx::mbar_arrive(empty(s));
+            }
+            ptx::named_bar_sync(1, 256);             // every thread has added the previous pass's terms
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float *yr = Y + (wgi * 64 + wl * 16 + (lane >> 2) + 8 * h) * RS_YS + cq;
+#pragma unroll
+                for (int j = 0; j < RS_N / 8; ++j)
+                    *reinterpret_cast<float2 *>(yr + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+            ptx::named_bar_sync(1, 256);             // Y of all 128 pixels is staged
+            const int dy = r - 1;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                // neighbours by (bn, bh, bw), never by flat row: no wrap into the next row or image.  A dropped term
+                // adds +0, which leaves m bitwise as it was (m starts at +0 and so is never -0).
+                const int q = cw * 16 + i, bw = q & (p.BW - 1), bh = (q >> lbw) & (p.BH - 1);
+                const bool row_in = bh + dy >= 0 && bh + dy < p.H;
+                const float *yq = Y + (row_in ? q + dy * p.BW : q) * RS_YS + lane;
+                const float t0 = row_in && bw > 0 ? yq[-RS_YS] : 0.f;
+                const float t1 = row_in ? yq[RS_MID] : 0.f;
+                const float t2 = row_in && bw + 1 < p.W ? yq[RS_YS + 2 * RS_MID] : 0.f;
+                m[i] += t0;
+                m[i] += t1;
+                m[i] += t2;
+            }
+        }
+        // relu(m) -> this warp's 16 rows of the mid tile (fp32, 128-byte swizzle: piece j of row r at j ^ (r & 7))
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int row = cw * 16 + i;
+            const uint32_t addr = mid + (uint32_t)(row * 128 + (((lane >> 2) ^ (row & 7)) << 4) + (lane & 3) * 4);
+            asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(fmaxf(m[i], 0.f)) : "memory");
+        }
+        ptx::fence_proxy_async();                    // generic-proxy writes -> visible to wgmma
+        ptx::named_bar_sync(2 + wgi, 128);           // this warpgroup's 64 rows are complete
+        float acc2[C / 2];
+        wg::fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+            wg::mma<false, C>(acc2, wg::desc_sw128(mid + (uint32_t)(wgi * 64 * 128) + 32u * kk), wg::desc_sw128(w2s + 32u * kk), kk != 0);
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs<C>(acc2);
+        // + r_i from the resident tile, ReLU, back into the resident tile as r_{i+1} (pixels outside the image or past
+        // the batch as zero: the next application's padding).  A warpgroup's GEMMs read only its own 64 rows of the
+        // tile, and each element is read and written by one thread.
+        const int relu = last ? p.relu : 1;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
+            const int bw = row & (p.BW - 1), bh = (row >> lbw) & (p.BH - 1), bn = row >> (lbw + lbh);
+            const bool live = bw < p.W && bh < p.H && n0 + bn < p.B;
+#pragma unroll
+            for (int j = 0; j < C / 8; ++j) {
+                const int c = 8 * j + cq;
+                const uint32_t addr = act + (uint32_t)((c >> 5) * A_BYTES + row * 128 + ((((c & 31) >> 2) ^ (row & 7)) << 4) + (c & 3) * 4);
+                float s0, s1;
+                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(s0), "=f"(s1) : "r"(addr) : "memory");
+                float v0 = acc2[4 * j + 2 * h] + s0, v1 = acc2[4 * j + 2 * h + 1] + s1;
+                if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                if (!live) { v0 = 0.f; v1 = 0.f; }
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
+            }
+        }
+        if (!last) {
+            ptx::fence_proxy_async();                // r_{i+1} -> the next application's wgmma
+            ptx::named_bar_sync(2 + wgi, 128);
+        }
+    }
+    // the last application's 16 rows of this warp (written by its own lanes) -> `out`, 16 bytes per lane
+    __syncwarp();
+    for (int e = lane; e < 16 * (C / 4); e += 32) {
+        const int row = wgi * 64 + wl * 16 + e / (C / 4), c = (e % (C / 4)) * 4;
+        const int bw = row & (p.BW - 1), bh = (row >> lbw) & (p.BH - 1), bn = row >> (lbw + lbh);
+        if (bw >= p.W || bh >= p.H || n0 + bn >= p.B) continue;
+        const uint32_t addr = act + (uint32_t)((c >> 5) * A_BYTES + row * 128 + ((((c & 31) >> 2) ^ (row & 7)) << 4));
+        float4 v;
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+        *reinterpret_cast<float4 *>(p.out + (((long long)(n0 + bn) * p.H + bh) * p.W + bw) * C + c) = v;
+    }
+}
+
+bool res_scatter_supported(int C, int Cmid, int H, int W) {
+    return (C == 64 || C == 128) && Cmid == RS_MID && H >= 1 && W >= 1 && W <= 16 && pow2_ceil(W) * pow2_ceil(H) <= 128;
+}
+
+// r, out: NHWC fp32 (B, H, W, C); w1: [9][32][C]; w2: [C][32]
+static int launch_res_scatter(const void *r, const void *w1, const void *w2, void *out, int B, int H, int W, int C,
+                              int relu_out, int napps, cudaStream_t s) {
+    RsParams q;
+    memset(&q, 0, sizeof(q));
+    q.out = static_cast<float *>(out);
+    q.B = B; q.H = H; q.W = W; q.napps = napps; q.relu = relu_out;
+    q.BW = pow2_ceil(W); q.BH = pow2_ceil(H); q.BN = 128 / (q.BW * q.BH);      // the tile launch_wgconv would pick
+    const int total = napps * 3 * (C / 32);
+    q.stages = total < RS_MAX_STAGES ? total : RS_MAX_STAGES;
+    const long long grid = ((long long)B + q.BN - 1) / q.BN;
+    if (grid > 0x7fffffffLL) return VQB_ERR_UNSUPPORTED;
+
+    const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    CUtensorMap tin, tw1, tw2;
+    const uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t strides[3] = {(uint64_t)C * 4, (uint64_t)W * C * 4, (uint64_t)H * W * C * 4};
+    const uint32_t box[4] = {32u, (uint32_t)q.BW, (uint32_t)q.BH, (uint32_t)q.BN};
+    const uint32_t es[4] = {1u, 1u, 1u, 1u};
+    int rc = vqb_encode_tmap_4d(&tin, dt, r, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = vqb_encode_tmap_2d(&tw1, dt, w1, (uint64_t)C, 9ull * RS_MID, (uint64_t)C * 4, 32u, (uint32_t)RS_N,
+                            CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = vqb_encode_tmap_2d(&tw2, dt, w2, (uint64_t)RS_MID, (uint64_t)C, (uint64_t)RS_MID * 4, 32u, (uint32_t)C,
+                            CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    const int smem = 1024 + (C / 32) * A_BYTES + q.stages * RS_WBYTES + A_BYTES + C * 128 + 128 * RS_YS * 4 +
+                     8 * (2 * RS_MAX_STAGES + 2);
+    auto kernel = C == 128 ? res_scatter_kernel<128> : res_scatter_kernel<64>;
+    static bool attr_set[2] = {false, false};
+    if (!attr_set[C == 128]) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        if (e != cudaSuccess) return (int)e;
+        attr_set[C == 128] = true;
+    }
+    if (cudaError_t le = vqb_launch(kernel, dim3((unsigned)grid), dim3(WG_THREADS), (size_t)smem, s, tin, tw1, tw2, q))
+        return (int)le;
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
 bool res_wg_supported(int bf16, int C, int Cmid) {
     return (C == 64 || C == 128) && (bf16 ? Cmid % 16 == 0 && Cmid >= 16 && Cmid <= 64 : Cmid == 32 || Cmid == 64);
 }
 
-// w1: [9][Cmid][C]; w2: [C][Cmid] (TF32) or [C][64] (bf16, Cmid zero padded to one chunk)
+// w1: [9][Cmid][C]; w2: [C][Cmid] (TF32) or [C][64] (bf16, Cmid zero padded to one chunk).  napps > 1 (a ResidualStack
+// of one shared layer) runs on res_scatter_kernel only and answers VQB_ERR_UNSUPPORTED elsewhere.
 int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void *out, int B, int H, int W, int C, int Cmid,
                   int relu_out, int napps, cudaStream_t s) {
-    if (!res_wg_supported(bf16, C, Cmid) || r == out) return VQB_ERR_UNSUPPORTED;
+    if (!res_wg_supported(bf16, C, Cmid) || r == out || napps < 1) return VQB_ERR_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(out)) & 15) return VQB_ERR_UNSUPPORTED;
+    if (!bf16 && res_scatter_supported(C, Cmid, H, W))
+        return launch_res_scatter(r, w1, w2, out, B, H, W, C, relu_out, napps, s);
+    if (napps > 1) return VQB_ERR_UNSUPPORTED;
     WgLaunch L;
     L.bf16 = bf16;
     L.in = r; L.B = B; L.Cin = C; L.H = H; L.W = W;
     L.w = w1; L.w_rows = 9LL * Cmid; L.w_inner = C;
     L.N = wg_gemm_cols(Cmid); L.ncols = Cmid;
     L.w2 = w2; L.w2_rows = C; L.w2_inner = bf16 ? 64 : Cmid; L.N2 = C;
-    L.skip = r; L.out = out; L.out_bf16 = bf16; L.relu = relu_out; L.napps = napps;
+    L.skip = r; L.out = out; L.out_bf16 = bf16; L.relu = relu_out;
     L.out_sn = (long long)H * W * C; L.out_sh = (long long)W * C; L.out_sw = C; L.out_sc = 1;
     set_phase(L, 0, taps3x3(H, W), Cmid, bf16);
     return launch_wgconv(L, s);

@@ -22,7 +22,6 @@ struct WgLaunch {
     long long w2_rows = 0;
     int w2_inner = 64;
     int N2 = 0;
-    int napps = 1;                        // > 1: that many chained applications (skip = in, whole-image tiles)
     const float *bias = nullptr;          // per output channel, may be null
     const void *skip = nullptr;           // same layout and type as out, may be null
     void *out = nullptr;
