@@ -1,4 +1,4 @@
-// ffma_gemm.cuh -- the fp32 CUDA-core GEMM of both backwards (internal; shared by prior_bwd.cu and conv_wgrad.cu),
+// ffma_gemm.cuh -- the fp32 CUDA-core GEMM of both backwards (internal; shared by prior_gemm.cu and conv_wgrad.cu),
 // the deterministic split of a weight gradient's reduction over positions, and the reduction of its chunk partials
 // into the parameter's layout.
 //

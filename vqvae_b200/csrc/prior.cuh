@@ -1,5 +1,5 @@
-// prior.cuh -- what the Gated PixelCNN's forward (prior.cu) and backward (prior_bwd.cu) share: shape limits, the
-// NHWC activation view, the host-side weight table and its argument checks, and the gate.
+// prior.cuh -- what the Gated PixelCNN's per-position kernels (prior.cu) and its matrix products (prior_gemm.cu) share:
+// shape limits, the NHWC activation view, the host-side weight table and its argument checks, and the gate.
 #pragma once
 #include "common.cuh"
 

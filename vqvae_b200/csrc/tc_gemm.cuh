@@ -1,6 +1,6 @@
 // tc_gemm.cuh -- the TF32 tensor-core GEMM (wgmma, sm_90a) behind the FFMA GEMM's interface (ffma_gemm.cuh): the same
 // operand accessors, epilogues and WgradSplit chunking, so a product written for `gemm` runs on tensor cores by
-// calling `tc_gemm` instead.  Internal; used by the prior's TF32 forward and backward (prior_bwd.cu).
+// calling `tc_gemm` instead.  Internal; used by the prior's TF32 forward and backward (prior_gemm.cu).
 //
 // tc_gemm_kernel computes out(m, n) = sum over k in chunk z of A(m, k) * B(k, n).  Per CTA: a 128-row tile, two
 // warpgroups of m64nBNk8 (BN = 64 or 128, chosen per call from N), k-steps of 32 floats.  Both operands are staged

@@ -3,12 +3,12 @@
 Same class names, constructor signatures, attribute names and state-dict keys as the reference, so a state dict saved
 by its ``gated_pixelcnn.py`` loads unchanged and ``from pixelcnn.models import GatedPixelCNN`` (the top-level
 ``pixelcnn`` package re-exports these classes) drops in.  As in ``modules.py`` the nn.Conv2d / nn.Embedding children
-are parameter containers only: every forward runs the sm_90a kernels of ``csrc/prior.cu`` / ``csrc/prior_bwd.cu``
+are parameter containers only: every forward runs the sm_90a kernels of ``csrc/prior.cu`` / ``csrc/prior_gemm.cu``
 through the C ABI, in the model's ``precision`` (fp32 by default) whatever ``set_precision`` says.
 
 ``GatedPixelCNN.forward`` is differentiable with respect to every parameter when grad is enabled and a parameter
 requires grad (``_PriorFunction``: the training forward keeps its activations, and the backward of
-``csrc/prior_bwd.cu`` writes one gradient per parameter), so the reference's training loop runs unchanged.  Under
+``csrc/prior_gemm.cu`` writes one gradient per parameter), so the reference's training loop runs unchanged.  Under
 ``torch.no_grad()`` it is the inference forward.  ``GatedPixelCNN.precision`` (a plain attribute, not in the state
 dict) selects the arithmetic of ``forward``, inference and training alike: "fp32" (the default, CUDA cores) or
 "tf32" (every matrix product on the wgmma TF32 GEMM, operands rounded to TF32, fp32 accumulation; the one-hot
