@@ -173,6 +173,30 @@ int vqb_residual_stack_f32(const float *r, const float *w1_packed, const float *
                            float *out, float *scratch, float *tmp, int B, int H, int W, int C,
                            int Cmid, int n_layers, int precision, void *stream);
 
+/* ---- the latent block of a VQVAE forward in one launch, TF32 only -------------------
+ * head: out0 = relu( conv(x) + head_bias ), the k3 s1 p1 layer that feeds the stack:
+ *   nn.Conv2d(Cin, C) (head_transposed = 0, encoder.py:35) or nn.ConvTranspose2d(Cin, C)
+ *   (head_transposed = 1, decoder.py:28); x NHWC (B,H,W,Cin), head_w_packed from
+ *   vqb_pack_conv_weight_f32; head_bias may be NULL.
+ * then the ResidualStack of vqb_residual_stack_f32 on out0 (n_layers >= 1, w1/w2 as there),
+ * then, when tail_cout > 0, the 1x1 conv C -> tail_cout of vqvae.py:16-17 (tail_w_packed
+ * from vqb_pack_conv_weight_f32, + tail_bias, may be NULL), whose output replaces the stack's.
+ * tail_w_packed must be NULL exactly when tail_cout == 0 (VQB_ERR_BAD_ARG otherwise).
+ * out: NHWC (B,H,W,C), or the (B*H*W, tail_cout) rows of z_e with the tail.
+ * Bitwise the separate calls (vqb_conv2d_f32 with VQB_TF32, vqb_residual_stack_f32 [,
+ * vqb_conv2d_f32 1x1]).  Shapes: those vqb_residual_stack_f32 runs in one launch (C in {64,
+ * 128}, Cmid = 32, whole images per 128-pixel tile), Cin % 32 == 0, Cin <= 256, tail_cout 0
+ * or 64; anything else, x == out or a pointer not 16-byte aligned returns VQB_ERR_UNSUPPORTED
+ * and launches nothing: run the separate calls then.
+ * vqb_latent_block_supported answers 1 for the shapes vqb_latent_block_tf32 takes, else 0
+ * (no CUDA call: callers ask before allocating the output).                               */
+int vqb_latent_block_tf32(const float *x, const float *head_w_packed, const float *head_bias,
+                          int head_transposed, const float *w1_packed, const float *w2_packed,
+                          int n_layers, const float *tail_w_packed, const float *tail_bias,
+                          int tail_cout, float *out, int B, int Cin, int H, int W, int C, int Cmid,
+                          void *stream);
+int vqb_latent_block_supported(int Cin, int H, int W, int C, int Cmid, int tail_cout);
+
 /* ---- VectorQuantizer.forward, quantizer.py:45-76 --------------------------------
  * z        (N, D) fp32 pixel rows (= z.permute(0,2,3,1).view(-1, e_dim), :45-46)
  * codebook (K, D) fp32 embedding.weight (:26)

@@ -13,7 +13,8 @@ per k-step, what wgconv_kernel loads) and "halo" (each tile's input halo once pe
 the N weight rows of every k-step, and the achieved bytes/s of each; the algorithmic FLOP/s; the card name and power
 limit.  The output layer (convT to <= 4 channels) runs in scatter form, which loads each tile's halo once per chunk,
 and so do the TF32 residual launches whose tiles hold whole images (res_scatter_kernel, which loads each tile once
-for all applications): both columns give those launches' bytes.  Prints one JSON line.  Nothing is written to the repository tree.
+for all applications): both columns give those launches' bytes.  A latent block (the k3 conv, the stack and the
+encoder's 1x1 conv in one res_scatter_kernel launch) adds its head conv's per-tap boxes and the tail's weight.  Prints one JSON line.  Nothing is written to the repository tree.
 """
 import argparse
 import json
@@ -28,7 +29,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 WGCONV_CALLS = {"vqb_conv2d_f32", "vqb_conv2d_bf16", "vqb_residual_layer_f32", "vqb_residual_stack_f32",
-                "vqb_residual_layer_bf16"}
+                "vqb_residual_layer_bf16", "vqb_latent_block_tf32"}
 
 
 def _card():
@@ -49,11 +50,20 @@ def _p2(x):
     return p
 
 
+def layers(label):
+    """The layer labels of one launch: a latent block's label ("res x2 128->32->128 8x8 +conv 128->128 k3s1 +conv
+    128->64 k1s1") names its stack and, after each "+", a conv at the stack's resolution."""
+    parts = label.split(" +")
+    hw = parts[0].split()[-1]
+    return [parts[0]] + [p + " " + hw for p in parts[1:]]
+
+
 def traffic(label, B):
     """(CTAs, k-steps per CTA, per-tap bytes, halo bytes) of one wgconv launch, from its ops label.  Tile shape as
     launch_wgconv picks it; 128-byte rows; weights: N rows per k-step (+ the chained 1x1 weight once per CTA)."""
     bf = label.startswith("bf16 ")
-    parts = (label[5:] if bf else label).split()
+    extra = [p.split() for p in layers(label)[1:]]
+    parts = (label[5:] if bf else label).split(" +")[0].split()
     ck = 64 if bf else 32
     napps = 1
     if parts[0] == "res":
@@ -68,7 +78,18 @@ def traffic(label, B):
             nc = c // 32
             ctas = -(-B // (128 // (_p2(w) * _p2(h))))
             moved = ctas * (nc * 128 * 128 + napps * 3 * nc * 96 * 128 + c * 128)
-            return ctas, napps * 3 * nc, moved, moved
+            ksteps = napps * 3 * nc
+            for conv in extra:
+                cin_, cout_ = (int(v) for v in conv[1].split("->"))
+                if conv[2] == "k3s1":
+                    # the head conv (latent block): the separate launch's per-tap A boxes and C weight rows per k-step,
+                    # in place of loading the tile
+                    moved += ctas * (9 * (cin_ // 32) * (128 * 128 + cout_ * 128) - nc * 128 * 128)
+                    ksteps += 9 * (cin_ // 32)
+                else:                              # the 1x1 tail: its weight once per CTA
+                    moved += ctas * cout_ * cin_ * 4
+                    ksteps += cin_ // 32
+            return ctas, ksteps, moved, moved
         cin, N, nph, taps, step, ext = c, _p2(max(cm, 16)), 1, 9, 1, 2
         w2 = c * 128 * (1 if bf else max(cm // 32, 1))
         grid = [(h, w)]
@@ -189,7 +210,7 @@ def main():
             for label, fn, cargs in record(model, x):
                 ms = time_call(fn, cargs, args.iters, args.reps)
                 ctas, ksteps, per_tap, halo = traffic(label, wl["batch"])
-                flops = bench.layer_model(label, wl["batch"], wl["K"], wl["D"])[0]
+                flops = sum(bench.layer_model(part, wl["batch"], wl["K"], wl["D"])[0] for part in layers(label))
                 rows.append(dict(launch=label, ms=round(ms, 5), ctas=ctas, ksteps_per_cta=ksteps,
                                  per_tap_MB=round(per_tap / 1e6, 1), halo_MB=round(halo / 1e6, 1),
                                  per_tap_TBps=round(per_tap / (ms * 1e-3) / 1e12, 2),

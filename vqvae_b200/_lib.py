@@ -15,6 +15,8 @@ _lib = None
 NCHW, NHWC = 0, 1
 FP32, TF32, BF16 = 0, 1, 2
 PRECISIONS = {"fp32": FP32, "tf32": TF32, "bf16": BF16}
+# enum vqb_status: the shape is outside what the kernels implement
+ERR_UNSUPPORTED = -2
 # enum vqb_conv_kind
 CONV_K1, CONV_K3, CONVT_K3, CONV_K4S2, CONVT_K4S2, CONVT_K4S2_OUT, RES_W2 = range(7)
 
@@ -42,6 +44,8 @@ SIGNATURES = {
     "vqb_set_vq_kernel": (_i, [_i]),
     "vqb_residual_layer_f32": (_i, [_vp] * 5 + [_i] * 7 + [_vp]),
     "vqb_residual_stack_f32": (_i, [_vp] * 6 + [_i] * 7 + [_vp]),
+    "vqb_latent_block_tf32": (_i, [_vp] * 3 + [_i] + [_vp] * 2 + [_i] + [_vp] * 2 + [_i, _vp] + [_i] * 6 + [_vp]),
+    "vqb_latent_block_supported": (_i, [_i] * 6),
     "vqb_conv_bf16_packed_bytes": (_sz, [_i, _i, _i]),
     "vqb_pack_conv_weight_bf16": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "vqb_conv2d_bf16": (_i, [_vp, _vp, _vp, _vp] + [_i] * 8 + [_vp]),

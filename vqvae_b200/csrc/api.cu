@@ -275,6 +275,23 @@ extern "C" int vqb_residual_stack_f32(const float *r, const float *w1_packed, co
     return 0;
 }
 
+extern "C" int vqb_latent_block_tf32(const float *x, const float *head_w_packed, const float *head_bias,
+                                     int head_transposed, const float *w1_packed, const float *w2_packed, int n_layers,
+                                     const float *tail_w_packed, const float *tail_bias, int tail_cout, float *out,
+                                     int B, int Cin, int H, int W, int C, int Cmid, void *stream) {
+    if (!x || !head_w_packed || !w1_packed || !w2_packed || !out) return VQB_ERR_BAD_ARG;
+    if (B <= 0 || Cin <= 0 || H <= 0 || W <= 0 || C <= 0 || Cmid <= 0 || n_layers < 1 || tail_cout < 0)
+        return VQB_ERR_BAD_ARG;
+    if (head_transposed != 0 && head_transposed != 1) return VQB_ERR_BAD_ARG;
+    if ((tail_w_packed != nullptr) != (tail_cout != 0)) return VQB_ERR_BAD_ARG;
+    return launch_latent_block(x, head_w_packed, head_bias, Cin, head_transposed, w1_packed, w2_packed, n_layers,
+                               tail_w_packed, tail_bias, tail_cout, out, B, H, W, C, Cmid, (cudaStream_t)stream);
+}
+
+extern "C" int vqb_latent_block_supported(int Cin, int H, int W, int C, int Cmid, int tail_cout) {
+    return Cin > 0 && H > 0 && W > 0 && tail_cout >= 0 && latent_block_supported(Cin, C, Cmid, H, W, tail_cout) ? 1 : 0;
+}
+
 // Thin stream-ordered copy for the host-buffer front end (vqvae_b200/pipeline.py): one ctypes call instead of
 // a torch stream context + Tensor.copy_ per transfer (the Python overhead per step was larger than the kernels).
 extern "C" int vqb_memcpy_async(void *dst, const void *src, size_t bytes, int kind, void *stream) {

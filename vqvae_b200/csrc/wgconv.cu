@@ -15,6 +15,8 @@
 //   * N2 > 0 (residual layer of the bf16 pipeline): the first GEMM's result is ReLU'd, rounded to bf16 and written
 //     to shared memory as the A operand of a second GEMM against an N2 x 64 weight tile loaded once, so
 //     out = act(skip + W2 . relu(W1 (*) r)) and the intermediate never leaves the SM.
+// The TF32 residual stack on whole-image tiles has its own kernel, res_scatter_kernel, which can also run the k3 conv
+// before the stack and the 1x1 conv after it in the same launch (the latent block of the inference forward).
 // The decoder's output layer (k4 s2 transposed conv to <= 4 channels) has its own persistent kernel at the end of this
 // file, convt_scatter_kernel: one GEMM per tile over the input pixels and their halo, read once per channel chunk.
 #include "ptx.cuh"
@@ -413,6 +415,14 @@ int launch_conv_tc(WgLaunch &L, const ConvPhase *ph, int nph, int total_taps, bo
 //     neighbours outside the image (the zero padding).  Then relu(m) -> the 1x1 GEMM, + r_i (from the resident
 //     tile), ReLU.  Between applications the result overwrites the resident tile in place (pixels outside the image
 //     or past the batch as zero: the next application's padding); only the last application stores to `out`.
+//     Two optional phases make it the whole latent block of a VQVAE inference forward (vqb_latent_block_tf32):
+//       - head: r_0 = relu(conv(x) + b) of the k3 s1 conv (or stride-1 transposed conv) that feeds the stack, C
+//         output channels, computed into the resident tile instead of loaded: wgconv_kernel's k-steps for that
+//         layer from the same builder (set_phase: tap outer, chunk inner; shifted 4-D boxes of x, zero filled;
+//         the same weight rows), accumulated from zero, then + bias and ReLU as store_tile does them.  So r_0 is
+//         bitwise the separate conv launch's output, and so is everything after it.
+//       - tail: z_e = r_n . Wpq^T + b (a 1x1 conv to TAIL_N channels, the k1 launch's 4 wgmma per 32-channel chunk
+//         in one chain from zero, then the bias), stored as fp32 NHWC rows instead of r_n.
 //   * otherwise wgconv_kernel with N2 = C: per tile the 3x3 GEMM's k-steps (the two separate conv launches' order
 //     and operands in TF32), ReLU, the chained 1x1 GEMM.  One application per launch.
 // Which kernel runs depends only on (bf16, C, Cmid, H, W), so a stack and its layers one by one compute the same bits.
@@ -420,45 +430,67 @@ constexpr int RS_MID = 32;                 // Cmid
 constexpr int RS_N = 3 * RS_MID;           // GEMM columns per pass: one kernel row's 3 taps x Cmid
 constexpr int RS_WBYTES = RS_N * 128;      // one pass's weight rows, one 128-byte channel chunk
 constexpr int RS_YS = RS_N + 8;            // staged floats per pixel: + 8 against bank conflicts of the fragment stores
-constexpr int RS_MAX_STAGES = 4;
+constexpr int RS_MAX_STAGES = 4;           // of the w1 ring, and of the head's ring
+constexpr int TAIL_N = 64;                 // output channels of the tail (the VQ's embedding dim)
 
 struct RsParams {
-    float *out;
+    float *out;                            // r_n, or z_e rows with a tail
+    const float *head_bias, *tail_bias;
     int B, H, W, BW, BH, BN, napps, relu, stages;
+    int head_steps, head_stages, tail;     // head_steps = 0: r_0 is loaded from tma_in
+    int4 head[WG_MAX_STEPS];               // the head's k-steps: x = c0, y = dx, z = dy, w = w_row
 };
 
+// Shared memory (1024-byte aligned, C = 128 / 64):
+//   act   NC chunks [128 px][128 B]                the resident tile r_i, the A operand          64 / 32 KB
+//   ring  S stages of one pass's w1 rows [96][128 B]                                           48 KB
+//   mid   relu(m) [128 px][128 B]                                                               16 KB
+//   Y     [128 px][RS_YS] floats                                                                52 KB
+//   w2s   w2 [C][128 B]                                                                         16 / 8 KB
+//   bars  full[4], empty[4], hfull[4], hempty[4], abar, w2bar, tbar
+// The head runs before any of ring .. w2s is used: its ring of head_stages x (A box [128 px][128 B] + C weight rows
+// [C][128 B]) starts at `ring` and may reach the end of w2s, so the stack's w1 and w2 loads wait until every head stage
+// is consumed.  The tail's weight [NC][TAIL_N][128 B] goes into the w1 ring once its last stage is consumed.
 template <int C>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant__ CUtensorMap tma_w1,
-                   const __grid_constant__ CUtensorMap tma_w2, const __grid_constant__ RsParams p) {
+                   const __grid_constant__ CUtensorMap tma_w2, const __grid_constant__ CUtensorMap tma_hw,
+                   const __grid_constant__ CUtensorMap tma_tw, const __grid_constant__ RsParams p) {
     constexpr int NC = C / 32;
+    constexpr int HSTAGE = A_BYTES + C * 128;
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
-    const uint32_t act = (raw + 1023u) & ~1023u;                  // NC chunks [128 px][128 B]: r_i, the A operand
-    const uint32_t ring = act + (uint32_t)(NC * A_BYTES);          // stages of one pass's w1 rows [96][128 B]
-    const uint32_t mid = ring + (uint32_t)(p.stages * RS_WBYTES);  // relu(m) [128 px][128 B]
-    const uint32_t w2s = mid + (uint32_t)A_BYTES;                  // w2 [C][128 B]
-    const uint32_t ysm = w2s + (uint32_t)(C * 128);                // Y [128 px][RS_YS] floats
-    const uint32_t bars = ysm + (uint32_t)(128 * RS_YS * 4);
+    const uint32_t act = (raw + 1023u) & ~1023u;
+    const uint32_t ring = act + (uint32_t)(NC * A_BYTES);
+    const uint32_t mid = ring + (uint32_t)(p.stages * RS_WBYTES);
+    const uint32_t ysm = mid + (uint32_t)A_BYTES;
+    const uint32_t w2s = ysm + (uint32_t)(128 * RS_YS * 4);
+    const uint32_t bars = w2s + (uint32_t)(C * 128);
     float *const Y = reinterpret_cast<float *>(smem_raw + (ysm - raw));
     auto full = [&](int s) { return bars + 8u * s; };
     auto empty = [&](int s) { return bars + 8u * (RS_MAX_STAGES + s); };
-    const uint32_t abar = bars + 8u * (2 * RS_MAX_STAGES), w2bar = abar + 8u;
-    const int S = p.stages;
+    auto hfull = [&](int s) { return bars + 8u * (2 * RS_MAX_STAGES + s); };
+    auto hempty = [&](int s) { return bars + 8u * (3 * RS_MAX_STAGES + s); };
+    const uint32_t abar = bars + 8u * (4 * RS_MAX_STAGES), w2bar = abar + 8u, tbar = abar + 16u;
+    const int S = p.stages, HS = p.head_stages, nh = p.head_steps;
     const int total = p.napps * 3 * NC;        // ring slots: application, pass (kernel row), chunk, innermost last
     const int n0 = blockIdx.x * p.BN;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
         for (int s = 0; s < S; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), 2); }
+        for (int s = 0; s < HS; ++s) { ptx::mbar_init(hfull(s), 1); ptx::mbar_init(hempty(s), 2); }
         ptx::mbar_init(abar, 1);
         ptx::mbar_init(w2bar, 1);
+        ptx::mbar_init(tbar, 1);
         ptx::fence_mbar_init();
     }
     if (tid == 32) {
         ptx::prefetch_tmap(&tma_in);
         ptx::prefetch_tmap(&tma_w1);
         ptx::prefetch_tmap(&tma_w2);
+        if (nh) ptx::prefetch_tmap(&tma_hw);
+        if (p.tail) ptx::prefetch_tmap(&tma_tw);
     }
     __syncthreads();
     pdl_launch_dependents();
@@ -469,19 +501,39 @@ res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_cons
             ptx::mbar_expect_tx(full(s), (uint32_t)RS_WBYTES);
             ptx::tma_load_2d(ring + (uint32_t)(s * RS_WBYTES), &tma_w1, full(s), (g % NC) * 32, ((g / NC) % 3) * RS_N);
         };
-        const int pre = total < S ? total : S;
-        if (lane == 0) {               // weights do not depend on the previous layer
+        auto load_weights = [&] {
             ptx::mbar_expect_tx(w2bar, (uint32_t)(C * 128));
             ptx::tma_load_2d(w2s, &tma_w2, w2bar, 0, 0);
-            for (int g = 0; g < pre; ++g) load_w1(g);
-        }
-        pdl_wait();                    // ... the activations do
+            for (int g = 0; g < S; ++g) load_w1(g);
+        };
+        if (lane == 0 && !nh) load_weights();      // weights do not depend on the previous layer
+        pdl_wait();                                // ... the activations do
         if (lane == 0) {
-            ptx::mbar_expect_tx(abar, (uint32_t)(NC * A_BYTES));
-            for (int c = 0; c < NC; ++c) ptx::tma_load_4d(act + (uint32_t)(c * A_BYTES), &tma_in, abar, c * 32, 0, 0, n0);
-            for (int g = pre; g < total; ++g) {
+            if (nh) {
+                for (int i = 0; i < nh; ++i) {
+                    const int s = i % HS;
+                    if (i >= HS) ptx::mbar_wait(hempty(s), (uint32_t)((i / HS - 1) & 1));
+                    const int4 st = p.head[i];
+                    const uint32_t dst = ring + (uint32_t)(s * HSTAGE);
+                    ptx::mbar_expect_tx(hfull(s), (uint32_t)HSTAGE);
+                    ptx::tma_load_4d(dst, &tma_in, hfull(s), st.x, st.y, st.z, n0);
+                    ptx::tma_load_2d(dst + A_BYTES, &tma_hw, hfull(s), st.x, st.w);
+                }
+                // the head's ring lies over the stack's weights: wait until its last stages are consumed
+                for (int i = nh > HS ? nh - HS : 0; i < nh; ++i) ptx::mbar_wait(hempty(i % HS), (uint32_t)((i / HS) & 1));
+                load_weights();
+            } else {
+                ptx::mbar_expect_tx(abar, (uint32_t)(NC * A_BYTES));
+                for (int c = 0; c < NC; ++c) ptx::tma_load_4d(act + (uint32_t)(c * A_BYTES), &tma_in, abar, c * 32, 0, 0, n0);
+            }
+            for (int g = S; g < total; ++g) {
                 ptx::mbar_wait(empty(g % S), (uint32_t)((g / S - 1) & 1));
                 load_w1(g);
+            }
+            if (p.tail) {              // into the w1 ring once its last stages are consumed
+                for (int g = total - S; g < total; ++g) ptx::mbar_wait(empty(g % S), (uint32_t)((g / S) & 1));
+                ptx::mbar_expect_tx(tbar, (uint32_t)(NC * TAIL_N * 128));
+                for (int c = 0; c < NC; ++c) ptx::tma_load_2d(ring + (uint32_t)(c * TAIL_N * 128), &tma_tw, tbar, c * 32, 0);
             }
         }
         return;
@@ -491,8 +543,51 @@ res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_cons
     pdl_wait();                        // `out` may still be read by the previous layer
     const int wgi = (warp >> 2) - 1, wl = warp & 3, cw = warp - 4, cq = 2 * (lane & 3);
     const int lbw = __ffs(p.BW) - 1, lbh = __ffs(p.BH) - 1;
-    ptx::mbar_wait(abar, 0);
-    ptx::mbar_wait(w2bar, 0);
+    // address in the resident tile of channels (c, c + 1) of tile row `row` (128-byte swizzle: piece j of row r at
+    // j ^ (r & 7))
+    auto act_addr = [&](int row, int c) {
+        return act + (uint32_t)((c >> 5) * A_BYTES + row * 128 + ((((c & 31) >> 2) ^ (row & 7)) << 4) + (c & 3) * 4);
+    };
+    auto live_row = [&](int row) {
+        const int bw = row & (p.BW - 1), bh = (row >> lbw) & (p.BH - 1), bn = row >> (lbw + lbh);
+        return bw < p.W && bh < p.H && n0 + bn < p.B;
+    };
+    if (nh) {
+        float acc[C / 2];
+#pragma unroll
+        for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
+        for (int i = 0; i < nh; ++i) {
+            const int s = i % HS;
+            ptx::mbar_wait(hfull(s), (uint32_t)((i / HS) & 1));
+            const uint32_t a = ring + (uint32_t)(s * HSTAGE + wgi * 64 * 128), b = ring + (uint32_t)(s * HSTAGE + A_BYTES);
+            wg::fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wg::mma<false, C>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+            wg::commit();
+            wg::wait<0>();
+            wg::fence_regs<C>(acc);
+            if (wl == 0 && lane == 0) ptx::mbar_arrive(hempty(s));
+        }
+        // relu(acc + bias) -> the resident tile as r_0, padding pixels as zero
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
+            const bool live = live_row(row);
+#pragma unroll
+            for (int j = 0; j < C / 8; ++j) {
+                const int c = 8 * j + cq;
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (p.head_bias) { v0 += __ldg(p.head_bias + c); v1 += __ldg(p.head_bias + c + 1); }
+                v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+                if (!live) { v0 = 0.f; v1 = 0.f; }
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(act_addr(row, c)), "f"(v0), "f"(v1) : "memory");
+            }
+        }
+        ptx::fence_proxy_async();                    // r_0 -> the first application's wgmma
+        ptx::named_bar_sync(2 + wgi, 128);
+    } else {
+        ptx::mbar_wait(abar, 0);
+    }
     int g = 0;
     for (int app = 0; app < p.napps; ++app) {
         const bool last = app + 1 == p.napps;
@@ -548,6 +643,7 @@ res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_cons
         }
         ptx::fence_proxy_async();                    // generic-proxy writes -> visible to wgmma
         ptx::named_bar_sync(2 + wgi, 128);           // this warpgroup's 64 rows are complete
+        if (app == 0) ptx::mbar_wait(w2bar, 0);
         float acc2[C / 2];
         wg::fence();
 #pragma unroll
@@ -563,12 +659,11 @@ res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_cons
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
-            const int bw = row & (p.BW - 1), bh = (row >> lbw) & (p.BH - 1), bn = row >> (lbw + lbh);
-            const bool live = bw < p.W && bh < p.H && n0 + bn < p.B;
+            const bool live = live_row(row);
 #pragma unroll
             for (int j = 0; j < C / 8; ++j) {
                 const int c = 8 * j + cq;
-                const uint32_t addr = act + (uint32_t)((c >> 5) * A_BYTES + row * 128 + ((((c & 31) >> 2) ^ (row & 7)) << 4) + (c & 3) * 4);
+                const uint32_t addr = act_addr(row, c);
                 float s0, s1;
                 asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(s0), "=f"(s1) : "r"(addr) : "memory");
                 float v0 = acc2[4 * j + 2 * h] + s0, v1 = acc2[4 * j + 2 * h + 1] + s1;
@@ -577,10 +672,42 @@ res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_cons
                 asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
             }
         }
-        if (!last) {
-            ptx::fence_proxy_async();                // r_{i+1} -> the next application's wgmma
+        if (!last || p.tail) {
+            ptx::fence_proxy_async();                // r_{i+1} -> the next application's (or the tail's) wgmma
             ptx::named_bar_sync(2 + wgi, 128);
         }
+    }
+    if (p.tail) {
+        // z_e = r_n . Wpq^T + b for this warpgroup's 64 rows -> fp32 NHWC rows
+        ptx::mbar_wait(tbar, 0);
+        float acc3[TAIL_N / 2];
+#pragma unroll
+        for (int i = 0; i < TAIL_N / 2; ++i) acc3[i] = 0.f;
+        wg::fence();
+#pragma unroll
+        for (int c = 0; c < NC; ++c) {
+            const uint32_t a = act + (uint32_t)(c * A_BYTES + wgi * 64 * 128), b = ring + (uint32_t)(c * TAIL_N * 128);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wg::mma<false, TAIL_N>(acc3, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+        }
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs<TAIL_N>(acc3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
+            const int bw = row & (p.BW - 1), bh = (row >> lbw) & (p.BH - 1), bn = row >> (lbw + lbh);
+            if (bw >= p.W || bh >= p.H || n0 + bn >= p.B) continue;
+            float *o = p.out + (((long long)(n0 + bn) * p.H + bh) * p.W + bw) * TAIL_N;
+#pragma unroll
+            for (int j = 0; j < TAIL_N / 8; ++j) {
+                const int c = 8 * j + cq;
+                float v0 = acc3[4 * j + 2 * h], v1 = acc3[4 * j + 2 * h + 1];
+                if (p.tail_bias) { v0 += __ldg(p.tail_bias + c); v1 += __ldg(p.tail_bias + c + 1); }
+                *reinterpret_cast<float2 *>(o + c) = make_float2(v0, v1);
+            }
+        }
+        return;
     }
     // the last application's 16 rows of this warp (written by its own lanes) -> `out`, 16 bytes per lane
     __syncwarp();
@@ -588,9 +715,8 @@ res_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_cons
         const int row = wgi * 64 + wl * 16 + e / (C / 4), c = (e % (C / 4)) * 4;
         const int bw = row & (p.BW - 1), bh = (row >> lbw) & (p.BH - 1), bn = row >> (lbw + lbh);
         if (bw >= p.W || bh >= p.H || n0 + bn >= p.B) continue;
-        const uint32_t addr = act + (uint32_t)((c >> 5) * A_BYTES + row * 128 + ((((c & 31) >> 2) ^ (row & 7)) << 4));
         float4 v;
-        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(act_addr(row, c)) : "memory");
         *reinterpret_cast<float4 *>(p.out + (((long long)(n0 + bn) * p.H + bh) * p.W + bw) * C + c) = v;
     }
 }
@@ -599,26 +725,36 @@ bool res_scatter_supported(int C, int Cmid, int H, int W) {
     return (C == 64 || C == 128) && Cmid == RS_MID && H >= 1 && W >= 1 && W <= 16 && pow2_ceil(W) * pow2_ceil(H) <= 128;
 }
 
-// r, out: NHWC fp32 (B, H, W, C); w1: [9][32][C]; w2: [C][32]
-static int launch_res_scatter(const void *r, const void *w1, const void *w2, void *out, int B, int H, int W, int C,
-                              int relu_out, int napps, cudaStream_t s) {
+// The conv that feeds the stack (x: NHWC fp32 (B, H, W, Cin); w: its vqb_pack_conv_weight_f32 rows [9][C][Cin]) and
+// the 1x1 conv after it (w: [TAIL_N][C]); null members: no such phase.
+struct RsHead { const void *x, *w; const float *bias; int Cin, transposed; };
+struct RsTail { const void *w; const float *bias; };
+
+// r, out: NHWC fp32 (B, H, W, C) (out: (B, H, W, TAIL_N) with a tail); w1: [9][32][C]; w2: [C][32].  With a head, r is
+// not read.
+static int launch_res_scatter(const RsHead &head, const RsTail &tail, const void *r, const void *w1, const void *w2,
+                              void *out, int B, int H, int W, int C, int relu_out, int napps, cudaStream_t s) {
     RsParams q;
     memset(&q, 0, sizeof(q));
     q.out = static_cast<float *>(out);
+    q.head_bias = head.bias; q.tail_bias = tail.bias; q.tail = tail.w != nullptr;
     q.B = B; q.H = H; q.W = W; q.napps = napps; q.relu = relu_out;
     q.BW = pow2_ceil(W); q.BH = pow2_ceil(H); q.BN = 128 / (q.BW * q.BH);      // the tile launch_wgconv would pick
     const int total = napps * 3 * (C / 32);
     q.stages = total < RS_MAX_STAGES ? total : RS_MAX_STAGES;
     const long long grid = ((long long)B + q.BN - 1) / q.BN;
     if (grid > 0x7fffffffLL) return VQB_ERR_UNSUPPORTED;
+    const int region = q.stages * RS_WBYTES + A_BYTES + 128 * RS_YS * 4 + C * 128;     // ring .. the end of w2s
+    if (q.tail && (C / 32) * TAIL_N * 128 > q.stages * RS_WBYTES) return VQB_ERR_UNSUPPORTED;
 
     const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    CUtensorMap tin, tw1, tw2;
-    const uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-    const uint64_t strides[3] = {(uint64_t)C * 4, (uint64_t)W * C * 4, (uint64_t)H * W * C * 4};
+    CUtensorMap tin, tw1, tw2, thw, ttw;
+    const int Cin = head.x ? head.Cin : C;
+    const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t strides[3] = {(uint64_t)Cin * 4, (uint64_t)W * Cin * 4, (uint64_t)H * W * Cin * 4};
     const uint32_t box[4] = {32u, (uint32_t)q.BW, (uint32_t)q.BH, (uint32_t)q.BN};
     const uint32_t es[4] = {1u, 1u, 1u, 1u};
-    int rc = vqb_encode_tmap_4d(&tin, dt, r, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
+    int rc = vqb_encode_tmap_4d(&tin, dt, head.x ? head.x : r, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     rc = vqb_encode_tmap_2d(&tw1, dt, w1, (uint64_t)C, 9ull * RS_MID, (uint64_t)C * 4, 32u, (uint32_t)RS_N,
                             CU_TENSOR_MAP_SWIZZLE_128B);
@@ -626,8 +762,32 @@ static int launch_res_scatter(const void *r, const void *w1, const void *w2, voi
     rc = vqb_encode_tmap_2d(&tw2, dt, w2, (uint64_t)RS_MID, (uint64_t)C, (uint64_t)RS_MID * 4, 32u, (uint32_t)C,
                             CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
-    const int smem = 1024 + (C / 32) * A_BYTES + q.stages * RS_WBYTES + A_BYTES + C * 128 + 128 * RS_YS * 4 +
-                     8 * (2 * RS_MAX_STAGES + 2);
+    thw = ttw = tw1;
+    if (head.x) {
+        // the k-steps of the separate launch of this conv (vqb_conv2d_f32 -> launch_conv_tc): the same builder
+        WgLaunch L;
+        L.bf16 = 0; L.Cin = Cin;
+        ConvPhase ph;
+        conv_phase(conv_geom(3, 3, 1, 1, head.transposed, H, W), 0, ph);
+        if (!set_phase(L, 0, ph, C, false)) return VQB_ERR_UNSUPPORTED;
+        q.head_steps = L.nsteps[0];
+        for (int i = 0; i < q.head_steps; ++i) {
+            const WgStep &st = L.steps[0][i];
+            q.head[i] = make_int4(st.c0, st.dx, st.dy, st.w_row);
+        }
+        const int hstage = A_BYTES + C * 128;
+        q.head_stages = region / hstage < RS_MAX_STAGES ? region / hstage : RS_MAX_STAGES;
+        if (q.head_stages > q.head_steps) q.head_stages = q.head_steps;
+        rc = vqb_encode_tmap_2d(&thw, dt, head.w, (uint64_t)Cin, 9ull * C, (uint64_t)Cin * 4, 32u, (uint32_t)C,
+                                CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+    }
+    if (q.tail) {
+        rc = vqb_encode_tmap_2d(&ttw, dt, tail.w, (uint64_t)C, (uint64_t)TAIL_N, (uint64_t)C * 4, 32u, (uint32_t)TAIL_N,
+                                CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+    }
+    const int smem = 1024 + (C / 32) * A_BYTES + region + 8 * (4 * RS_MAX_STAGES + 3);
     auto kernel = C == 128 ? res_scatter_kernel<128> : res_scatter_kernel<64>;
     static bool attr_set[2] = {false, false};
     if (!attr_set[C == 128]) {
@@ -635,10 +795,27 @@ static int launch_res_scatter(const void *r, const void *w1, const void *w2, voi
         if (e != cudaSuccess) return (int)e;
         attr_set[C == 128] = true;
     }
-    if (cudaError_t le = vqb_launch(kernel, dim3((unsigned)grid), dim3(WG_THREADS), (size_t)smem, s, tin, tw1, tw2, q))
+    if (cudaError_t le = vqb_launch(kernel, dim3((unsigned)grid), dim3(WG_THREADS), (size_t)smem, s, tin, tw1, tw2, thw,
+                                    ttw, q))
         return (int)le;
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
+}
+
+bool latent_block_supported(int Cin, int C, int Cmid, int H, int W, int tail_cout) {
+    return res_scatter_supported(C, Cmid, H, W) && Cin % 32 == 0 && 9 * (Cin / 32) <= WG_MAX_STEPS &&
+           (tail_cout == 0 || tail_cout == TAIL_N);
+}
+
+int launch_latent_block(const void *x, const void *head_w, const float *head_bias, int Cin, int transposed,
+                        const void *w1, const void *w2, int napps, const void *tail_w, const float *tail_bias,
+                        int tail_cout, void *out, int B, int H, int W, int C, int Cmid, cudaStream_t s) {
+    if (!latent_block_supported(Cin, C, Cmid, H, W, tail_cout) || (tail_w != nullptr) != (tail_cout != 0) || napps < 1 ||
+        x == out)
+        return VQB_ERR_UNSUPPORTED;
+    if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15) return VQB_ERR_UNSUPPORTED;
+    return launch_res_scatter(RsHead{x, head_w, head_bias, Cin, transposed}, RsTail{tail_w, tail_bias}, nullptr, w1, w2,
+                              out, B, H, W, C, 1, napps, s);
 }
 
 bool res_wg_supported(int bf16, int C, int Cmid) {
@@ -652,7 +829,7 @@ int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void 
     if (!res_wg_supported(bf16, C, Cmid) || r == out || napps < 1) return VQB_ERR_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(out)) & 15) return VQB_ERR_UNSUPPORTED;
     if (!bf16 && res_scatter_supported(C, Cmid, H, W))
-        return launch_res_scatter(r, w1, w2, out, B, H, W, C, relu_out, napps, s);
+        return launch_res_scatter(RsHead{}, RsTail{}, r, w1, w2, out, B, H, W, C, relu_out, napps, s);
     if (napps > 1) return VQB_ERR_UNSUPPORTED;
     WgLaunch L;
     L.bf16 = bf16;

@@ -46,6 +46,15 @@ int launch_conv_tc(WgLaunch &L, const ConvPhase *ph, int nph, int total_taps, bo
 bool res_wg_supported(int bf16, int C, int Cmid);
 int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void *out, int B, int H, int W, int C, int Cmid,
                   int relu_out, int napps, cudaStream_t s);
+// A stride-1 k3 conv (or transposed conv) Cin -> C with bias and ReLU, a ResidualStack of napps applications and, when
+// tail_cout > 0, the 1x1 conv tail_w (C -> tail_cout) with bias, in one launch (res_scatter_kernel): the separate
+// launches' bits.  out: (B, H, W, C) NHWC, or (B, H, W, tail_cout) with the tail.  Answers VQB_ERR_UNSUPPORTED,
+// launching nothing, when latent_block_supported fails (tail_cout = 0: no tail), tail_w is given without tail_cout or
+// the other way round, x == out, or a pointer is not 16-byte aligned.
+bool latent_block_supported(int Cin, int C, int Cmid, int H, int W, int tail_cout);
+int launch_latent_block(const void *x, const void *head_w, const float *head_bias, int Cin, int transposed,
+                        const void *w1, const void *w2, int napps, const void *tail_w, const float *tail_bias,
+                        int tail_cout, void *out, int B, int H, int W, int C, int Cmid, cudaStream_t s);
 bool convt_shuffle_supported(int Cin, int Cout);
 int launch_convt_shuffle_wg(int bf16, const void *in, const void *w_shuffle, const float *bias, float *out, int B, int Cin,
                             int H, int W, int Cout, int relu, cudaStream_t s);

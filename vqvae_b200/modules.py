@@ -301,6 +301,25 @@ class ResidualStack(nn.Module):
         return ops.nhwc_to_nchw(self._apply_nhwc(r, B, H, W))
 
 
+def _latent_block(head, stack, h, B, H, W, tail=None):
+    """VQVAE._walk's TF32 inference path: the k3 s1 conv `head` (its ReLU folded in), the ResidualStack `stack` and, given,
+    the 1x1 conv `tail` on NHWC h as one launch (ops.latent_block) -> the output of the last of them, bitwise the
+    separate launches.  None (nothing allocated or launched) when the stack is not the reference's [layer] * n
+    construction with n >= 1 or the library does not take the shapes (the tail's Cout included): the caller runs the
+    separate launches then."""
+    if len(stack.stack) == 0 or any(l is not stack.stack[0] for l in stack.stack):
+        return None
+    c1, c2 = stack.stack[0].res_block[1], stack.stack[0].res_block[3]
+    transposed = isinstance(head, nn.ConvTranspose2d)
+    return ops.latent_block(h, _packed(head.weight, _pack_key(head, False)), _bias(head),
+                            _packed(c1.weight, _pack_key(c1, False)), _packed(c2.weight, _pack_key(c2, False)),
+                            None if tail is None else _packed(tail.weight, _pack_key(tail, False)),
+                            None if tail is None else _bias(tail),
+                            B=B, Cin=head.in_channels, H=H, W=W, C=head.out_channels, Cmid=c1.out_channels,
+                            n_layers=len(stack.stack), transposed=transposed,
+                            tail_cout=0 if tail is None else tail.out_channels)
+
+
 class Encoder(nn.Module):
     """q_theta(z|x): models/encoder.py:9-43."""
 
@@ -317,9 +336,12 @@ class Encoder(nn.Module):
         )
         self.conv_stack[0]._bf16_key = ("f32", False)      # bf16: vqb_conv_in_bf16 reads the fp32 packing
 
-    def _forward_nhwc(self, x, bf16=False, acts=None):
+    def _forward_nhwc(self, x, bf16=False, acts=None, tail=None, fuse=False):
         """x: prepared NCHW fp32 CUDA tensor -> (NHWC activation, bf16 in the bf16 pipeline, B, H, W).  `acts` (a
-        dict, training walk) receives the post-ReLU outputs of the three convs and the stack's output as "enc"."""
+        dict, training walk) receives the post-ReLU outputs of the three convs and the stack's output as "enc".
+        `tail` (VQVAE's pre-quantization conv): applied to the stack's output, which makes the result z_e (fp32 in
+        every mode).  `fuse` (VQVAE._walk's TF32 inference path): conv 4, the stack and `tail` in one launch when
+        _latent_block takes them."""
         B, _, H, W = x.shape
         cs = self.conv_stack
         if bf16:      # the 3-channel image has its own entry point: fp32 NCHW in, bf16 NHWC out
@@ -331,6 +353,9 @@ class Encoder(nn.Module):
         a1 = h
         h, H, W = _run_conv(cs[2], h, B, H, W, bf16, relu=True)
         a2 = h
+        z = _latent_block(cs[4], cs[5], h, B, H, W, tail) if fuse else None      # k3 s1 p1: H, W unchanged
+        if z is not None:
+            return z, B, H, W
         # the only consumer of conv 4 is the stack, whose first op is ReLU (or, with an
         # empty stack, its final F.relu): fold that ReLU into this epilogue (Q2/Q3).
         h, H, W = _run_conv(cs[4], h, B, H, W, bf16, relu=True)
@@ -338,6 +363,8 @@ class Encoder(nn.Module):
         h = cs[5]._apply_nhwc(h, B, H, W, bf16)
         if acts is not None:
             acts["enc"] = (a1, a2, a3, h)
+        if tail is not None:
+            h = _run_conv(tail, h, B, H, W, bf16, out_f32=True)[0]
         return h, B, H, W
 
     def forward(self, x):
@@ -367,13 +394,16 @@ class Decoder(nn.Module):
             nn.ConvTranspose2d(h_dim // 2, 3, kernel_size=kernel, stride=stride, padding=1),
         )
 
-    def _forward_from_nhwc(self, z, B, H, W, bf16=False, acts=None):
+    def _forward_from_nhwc(self, z, B, H, W, bf16=False, acts=None, fuse=False):
         """z: NHWC (B,H,W,in_dim), bf16 in the bf16 pipeline -> x_hat fp32 NCHW.  `acts` (a dict, training walk)
-        receives the stack's input and output and the last hidden activation as "dec"."""
+        receives the stack's input and output and the last hidden activation as "dec".  `fuse` (VQVAE._walk's TF32
+        inference path): the first conv and the stack in one launch when _latent_block takes them."""
         ics = self.inverse_conv_stack
-        h, H, W = _run_conv(ics[0], z, B, H, W, bf16, relu=True)     # ReLU of the stack folded in (Q2/Q3)
-        d1 = h
-        h = ics[1]._apply_nhwc(h, B, H, W, bf16)
+        h = _latent_block(ics[0], ics[1], z, B, H, W) if fuse else None      # k3 s1 p1: H, W unchanged
+        if h is None:
+            h, H, W = _run_conv(ics[0], z, B, H, W, bf16, relu=True)     # ReLU of the stack folded in (Q2/Q3)
+            d1 = h
+            h = ics[1]._apply_nhwc(h, B, H, W, bf16)
         d_out = h
         h, H, W = _run_conv(ics[2], h, B, H, W, bf16, relu=True)
         if acts is not None:
@@ -855,16 +885,14 @@ class VQVAE(nn.Module):
         return all(ops.lib().vqb_conv_bf16_packed_bytes(key[1], c.out_channels, c.in_channels) != 0
                    for c, key in keys if key[0] == "bf16")
 
-    def _encode_rows(self, x, bf16=False, acts=None):
+    def _encode_rows(self, x, bf16=False, acts=None, fuse=False):
         x = _prep_input(x, 3, "VQVAE")
         if x.shape[2] % 4 or x.shape[3] % 4:
             raise RuntimeError("VQVAE: image height and width must be divisible by 4 (Q11)")
         if acts is not None:
             acts["x"] = x
-        h, B, H, W = self.encoder._forward_nhwc(x, bf16, acts)
         # NHWC (B,H,W,D) rows, fp32 in every mode: they feed the exact VQ
-        z_e = _run_conv(self.pre_quantization_conv, h, B, H, W, bf16, out_f32=True)[0]
-        return z_e, B, H, W
+        return self.encoder._forward_nhwc(x, bf16, acts, self.pre_quantization_conv, fuse)
 
     def _trains(self, x):
         """Whether forward(x) takes the differentiable path (see forward)."""
@@ -892,7 +920,11 @@ class VQVAE(nn.Module):
     def _walk(self, x, bf16, acts=None):
         """The forward's launches -> (embedding_loss, x_hat, perplexity).  `acts` (a dict) receives the tensors the
         training backward reads."""
-        z_e, B, H, W = self._encode_rows(x, bf16, acts)                      # vqvae.py:31-33
+        # Inference in TF32: each side's k3 conv, its ResidualStack and (encoder) the pre-quantization conv run as one
+        # launch where _latent_block takes the shape, bitwise the separate launches.  The training walk keeps those,
+        # since its backward reads the activations between them.
+        fuse = acts is None and not bf16 and _conv_precision() == PRECISIONS["tf32"]
+        z_e, B, H, W = self._encode_rows(x, bf16, acts, fuse)                # vqvae.py:31-33
         vq = self.vector_quantization
         D = vq.e_dim
         group = self.process_group
@@ -914,7 +946,7 @@ class VQVAE(nn.Module):
             if not torch.cuda.is_current_stream_capturing():
                 for t in (sse, hist, embedding_loss, perplexity):
                     t.record_stream(side)
-        x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16, acts)  # :36
+        x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16, acts, fuse)  # :36
         main.wait_stream(side)
         if not torch.cuda.is_current_stream_capturing():
             # the two scalars were allocated in the side stream's pool and are consumed on the caller's stream: without this

@@ -217,6 +217,33 @@ def residual_stack(r, w1_packed, w2_packed, *, B, H, W, C, Cmid, n_layers, preci
     return out
 
 
+def latent_block(x, head_w, head_bias, w1_packed, w2_packed, tail_w=None, tail_bias=None, *, B, Cin, H, W, C, Cmid,
+                 n_layers, transposed, tail_cout=0):
+    """relu(k3 s1 conv or transposed conv of NHWC x + head_bias), the ResidualStack of residual_stack and, given
+    tail_w, the 1x1 conv to tail_cout channels + tail_bias, as ONE TF32 launch (vqb_latent_block_tf32), bitwise the
+    separate calls.  Returns the NHWC stack output, or the tail's (B, H, W, tail_cout) rows; None (nothing allocated or
+    launched) for a shape the launch does not take."""
+    _require_cuda(x, "input")
+    if (tail_w is None) != (tail_cout == 0):
+        raise ValueError("latent_block: tail_w and tail_cout > 0 go together")
+    if not lib().vqb_latent_block_supported(Cin, H, W, C, Cmid, tail_cout):
+        return None
+    out = torch.empty((B, H, W, tail_cout or C), dtype=torch.float32, device=x.device)
+    conv = f"+conv{'T' if transposed else ''} {Cin}->{C} k3s1"
+    tail = "" if tail_w is None else f" +conv {C}->{tail_cout} k1s1"
+    span = _Span(f"res x{n_layers} {C}->{Cmid}->{C} {H}x{W} {conv}{tail}")
+    rc = lib().vqb_latent_block_tf32(x.data_ptr(), head_w.data_ptr(), head_bias.data_ptr() if head_bias is not None else None,
+                                     int(bool(transposed)), w1_packed.data_ptr(), w2_packed.data_ptr(), n_layers,
+                                     tail_w.data_ptr() if tail_w is not None else None,
+                                     tail_bias.data_ptr() if tail_bias is not None else None, tail_cout, out.data_ptr(),
+                                     B, Cin, H, W, C, Cmid, _stream())
+    if rc == _lib.ERR_UNSUPPORTED:      # a supported shape declined only for aliasing or alignment
+        return None
+    check(rc, "latent_block")
+    span.done()
+    return out
+
+
 def vq_forward(z_rows, codebook, zq_dtype=torch.float32):
     """Fused VectorQuantizer core on (N,D) fp32 rows -> (idx int64 (N,), zq (N,D), sse f64 (1,),
     hist int32 (K,)); `sse` is final when the call returns.  zq_dtype=torch.bfloat16
