@@ -197,6 +197,25 @@ int vqb_latent_block_tf32(const float *x, const float *head_w_packed, const floa
                           void *stream);
 int vqb_latent_block_supported(int Cin, int H, int W, int C, int Cmid, int tail_cout);
 
+/* ---- the decoder's last two layers in one launch, TF32 only -------------------------
+ * h = relu( convT(d_out) + convt_bias ), the k4 s2 p1 nn.ConvTranspose2d(Cin, C) of
+ *   decoder.py:31-33 on d_out NHWC (B,H,W,Cin),
+ * x_hat = act( convT(h) + out_bias ), the k4 s2 p1 nn.ConvTranspose2d(C, Cout) of
+ *   decoder.py:34-35, act = ReLU iff relu_out; x_hat fp32 NCHW (B,Cout,4H,4W).
+ * Both weights packed by vqb_pack_conv_weight_f32; the biases may be NULL.  h_out: NULL, or
+ * NHWC (B,2H,2W,C), which then receives h.  Bitwise the separate calls (vqb_conv2d_f32 with
+ * VQB_TF32, NHWC out with ReLU, then NHWC in, NCHW out).  Shapes: C == 64, 1 <= Cout <= 4,
+ * Cin % 32 == 0, Cin <= 256, whole latent images per 128-pixel tile (pow2(W) <= 16 and
+ * pow2(W) * pow2(H) <= 128); anything else, d_out aliasing an output or a pointer not
+ * 16-byte aligned returns VQB_ERR_UNSUPPORTED and launches nothing: run the separate calls
+ * then.  vqb_decoder_tail_supported answers 1 for the shapes vqb_decoder_tail_tf32 takes,
+ * else 0 (no CUDA call).                                                                  */
+int vqb_decoder_tail_tf32(const float *d_out, const float *convt_w_packed, const float *convt_bias,
+                          const float *out_w_packed, const float *out_bias, float *h_out,
+                          float *x_hat, int B, int Cin, int H, int W, int C, int Cout,
+                          int relu_out, void *stream);
+int vqb_decoder_tail_supported(int Cin, int H, int W, int C, int Cout);
+
 /* ---- VectorQuantizer.forward, quantizer.py:45-76 --------------------------------
  * z        (N, D) fp32 pixel rows (= z.permute(0,2,3,1).view(-1, e_dim), :45-46)
  * codebook (K, D) fp32 embedding.weight (:26)

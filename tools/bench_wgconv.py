@@ -14,7 +14,10 @@ the N weight rows of every k-step, and the achieved bytes/s of each; the algorit
 limit.  The output layer (convT to <= 4 channels) runs in scatter form, which loads each tile's halo once per chunk,
 and so do the TF32 residual launches whose tiles hold whole images (res_scatter_kernel, which loads each tile once
 for all applications): both columns give those launches' bytes.  A latent block (the k3 conv, the stack and the
-encoder's 1x1 conv in one res_scatter_kernel launch) adds its head conv's per-tap boxes and the tail's weight.  Prints one JSON line.  Nothing is written to the repository tree.
+encoder's 1x1 conv in one res_scatter_kernel launch) adds its head conv's per-tap boxes and the tail's weight.  The
+decoder tail (the k4 s2 transposed conv and the output layer in one wgconv_kernel launch) is the transposed conv's
+traffic with one CTA per tile for all four phases, plus the output layer's gathered weight once per CTA: its input h
+stays in shared memory.  Prints one JSON line.  Nothing is written to the repository tree.
 """
 import argparse
 import json
@@ -29,7 +32,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 WGCONV_CALLS = {"vqb_conv2d_f32", "vqb_conv2d_bf16", "vqb_residual_layer_f32", "vqb_residual_stack_f32",
-                "vqb_residual_layer_bf16", "vqb_latent_block_tf32"}
+                "vqb_residual_layer_bf16", "vqb_latent_block_tf32", "vqb_decoder_tail_tf32"}
 
 
 def _card():
@@ -52,9 +55,14 @@ def _p2(x):
 
 def layers(label):
     """The layer labels of one launch: a latent block's label ("res x2 128->32->128 8x8 +conv 128->128 k3s1 +conv
-    128->64 k1s1") names its stack and, after each "+", a conv at the stack's resolution."""
+    128->64 k1s1") names its stack and, after each "+", a conv at the stack's resolution; a decoder tail's ("convT
+    128->64 k4s2 8x8 +convT 64->3 k4s2") names the k4 s2 transposed conv and the output layer, which runs at that
+    conv's output resolution."""
     parts = label.split(" +")
     hw = parts[0].split()[-1]
+    if parts[0].split()[0] == "convT" and parts[0].split()[2] == "k4s2":
+        h, w = (int(v) for v in hw.split("x"))
+        hw = f"{2 * h}x{2 * w}"
     return [parts[0]] + [p + " " + hw for p in parts[1:]]
 
 
@@ -131,7 +139,15 @@ def traffic(label, B):
     wbytes = ctas * (napps * a * N * 128 + w2)
     per_tap = ctas * napps * a * 128 * 128 + wbytes
     halo = ctas * napps * halo_px * nc * 128 + wbytes
-    return ctas, napps * a, per_tap, halo
+    ksteps = napps * a
+    if extra:
+        # decoder tail: one CTA per tile runs the four phases, then gathers the output layer's 64 live weight rows per
+        # 32-channel chunk of h once; h itself never leaves shared memory
+        ctas //= nph
+        ksteps *= nph
+        per_tap += ctas * (cout // 32) * 64 * 128
+        halo += ctas * (cout // 32) * 64 * 128
+    return ctas, ksteps, per_tap, halo
 
 
 def record(model, x):

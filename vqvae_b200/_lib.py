@@ -46,6 +46,8 @@ SIGNATURES = {
     "vqb_residual_stack_f32": (_i, [_vp] * 6 + [_i] * 7 + [_vp]),
     "vqb_latent_block_tf32": (_i, [_vp] * 3 + [_i] + [_vp] * 2 + [_i] + [_vp] * 2 + [_i, _vp] + [_i] * 6 + [_vp]),
     "vqb_latent_block_supported": (_i, [_i] * 6),
+    "vqb_decoder_tail_tf32": (_i, [_vp] * 7 + [_i] * 7 + [_vp]),
+    "vqb_decoder_tail_supported": (_i, [_i] * 5),
     "vqb_conv_bf16_packed_bytes": (_sz, [_i, _i, _i]),
     "vqb_pack_conv_weight_bf16": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "vqb_conv2d_bf16": (_i, [_vp, _vp, _vp, _vp] + [_i] * 8 + [_vp]),

@@ -292,6 +292,20 @@ extern "C" int vqb_latent_block_supported(int Cin, int H, int W, int C, int Cmid
     return Cin > 0 && H > 0 && W > 0 && tail_cout >= 0 && latent_block_supported(Cin, C, Cmid, H, W, tail_cout) ? 1 : 0;
 }
 
+extern "C" int vqb_decoder_tail_tf32(const float *d_out, const float *convt_w_packed, const float *convt_bias,
+                                     const float *out_w_packed, const float *out_bias, float *h_out, float *x_hat, int B,
+                                     int Cin, int H, int W, int C, int Cout, int relu_out, void *stream) {
+    if (!d_out || !convt_w_packed || !out_w_packed || !x_hat) return VQB_ERR_BAD_ARG;
+    if (B <= 0 || Cin <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return VQB_ERR_BAD_ARG;
+    if (relu_out != 0 && relu_out != 1) return VQB_ERR_BAD_ARG;
+    return launch_decoder_tail(d_out, convt_w_packed, convt_bias, out_w_packed, out_bias, h_out, x_hat, B, Cin, H, W, C,
+                               Cout, relu_out, (cudaStream_t)stream);
+}
+
+extern "C" int vqb_decoder_tail_supported(int Cin, int H, int W, int C, int Cout) {
+    return decoder_tail_supported(Cin, H, W, C, Cout) ? 1 : 0;
+}
+
 // Thin stream-ordered copy for the host-buffer front end (vqvae_b200/pipeline.py): one ctypes call instead of
 // a torch stream context + Tensor.copy_ per transfer (the Python overhead per step was larger than the kernels).
 extern "C" int vqb_memcpy_async(void *dst, const void *src, size_t bytes, int kind, void *stream) {

@@ -15,6 +15,8 @@
 //   * N2 > 0 (residual layer of the bf16 pipeline): the first GEMM's result is ReLU'd, rounded to bf16 and written
 //     to shared memory as the A operand of a second GEMM against an N2 x 64 weight tile loaded once, so
 //     out = act(skip + W2 . relu(W1 (*) r)) and the intermediate never leaves the SM.
+//   * TAIL (TF32, N = 64, the decoder's k4 s2 transposed conv on whole-image tiles): the CTA runs all four phases
+//     itself, keeps h = relu(convT + b) of its images in shared memory and chains the output layer on it (below).
 // The TF32 residual stack on whole-image tiles has its own kernel, res_scatter_kernel, which can also run the k3 conv
 // before the stack and the 1x1 conv after it in the same launch (the latent block of the inference forward).
 // The decoder's output layer (k4 s2 transposed conv to <= 4 channels) has its own persistent kernel at the end of this
@@ -41,7 +43,39 @@ struct WgParams {
     int OHg[4], OWg[4], out_py[4], out_px[4], nsteps[4];
     long long out_sn, out_sh, out_sw, out_sc;
     int4 steps[4][WG_MAX_STEPS];              // x = c0, y = dx, z = dy, w = w_row
+    // TAIL: the output layer (w_shuffle rows as convt_scatter_kernel reads them, bias may be null) -> x_hat NCHW fp32;
+    // `out` is h (NHWC) or null
+    const void *tail_w;
+    const float *tail_bias;
+    float *tail_out;
+    int tail_cout, tail_relu;
 };
+
+// The output layer's weight in scatter form (see convt_scatter_kernel): 64 GEMM columns (phase, neighbour (ky, kx),
+// co), gathered once per CTA.
+constexpr int SC_N = 64;                   // GEMM columns: 4 phases x 4 neighbours (ky, kx) x 4 channels
+constexpr int SC_BBYTES = SC_N * 128;      // one 128-byte channel chunk of the gathered weight
+
+// Gather the output layer's 64 live weight rows from w_shuffle ([9 taps (dy, dx)][16][Cin], row (py * 2 + px) * Cout
+// + co of tap (dy + 1) * 3 + dx + 1) into nc chunks [64][128 B] at wres, by 256 threads (t = 0..255): row r = phase *
+// 16 + k * 4 + co in the 128-byte swizzle wgmma reads (16-byte piece j of row r at j ^ (r & 7)), channels co >= Cout
+// zero.  Ends with the proxy fence; the caller's barrier makes the rows complete.
+template <bool BF16>
+__device__ __forceinline__ void gather_shuffle_weight(uint32_t wres, const void *w, int Cin, int Cout, int nc, int t) {
+    const size_t row_bytes = (size_t)Cin * (BF16 ? 2 : 4);
+    for (int i = t; i < nc * SC_N * 8; i += 256) {
+        const int j = i & 7, r = (i >> 3) % SC_N, c = i / (8 * SC_N);
+        const int ph = r >> 4, k = (r >> 2) & 3, co = r & 3;
+        const int tap = ((k >> 1) + (ph >> 1)) * 3 + (k & 1) + (ph & 1);
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (co < Cout)
+            v = __ldg(reinterpret_cast<const uint4 *>(reinterpret_cast<const unsigned char *>(w) +
+                      (size_t)(tap * 16 + ph * Cout + co) * row_bytes + c * 128 + j * 16));
+        const uint32_t dst = wres + (uint32_t)(c * SC_BBYTES + r * 128 + ((j ^ (r & 7)) << 4));
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+    }
+    ptx::fence_proxy_async();                      // generic-proxy writes -> visible to wgmma
+}
 
 // Epilogue of one accumulator fragment (wgmma D layout, see wgmma.cuh) for the pixel rows of this thread.
 template <int N>
@@ -87,31 +121,48 @@ __device__ __forceinline__ void store_tile(const WgParams &p, const float *acc, 
 template <bool BF16, int N>
 __host__ __device__ constexpr int chain_chunks() { return BF16 ? 1 : (N >= 32 ? N / 32 : 1); }
 
-template <bool BF16, int N, int N2>
+// TAIL: h of the tile's images stays in shared memory as the A operand of the output layer's GEMM.  Each of the 4 phases
+// runs the k-steps of the per-phase launch (the same table, ring and chain), then its epilogue (+ bias, ReLU, in
+// store_tile's order) writes the values to h (and to `out` when given).  h: KC2 = 2 chunks [4 x 128 rows][128 B] of 32
+// channels, 128-byte swizzle, rows in tile raster order (image, 2 BH, 2 BW), so every 64-row block is 1024-byte aligned
+// and warpgroup wgi's phase rows all land in h rows 256 wgi .. + 255.  Then, per 64-row block, the output layer's
+//   Y[q][phase, k, co] = h[q] . w_out[tap of (phase, k)][phase, co]      (m64n64, chunk outer, from zero)
+// as in convt_scatter_kernel, and Y overwrites the block's h rows in place (the block's GEMM has read them): columns
+// 0..31 in the chunk 0 row, 32..63 in the chunk 1 row, word w of the 32 at (w + 2 q) mod 32 against bank conflicts.
+// Finally x_hat(2 gy + py, 2 gx + px, co) = sum over k in raster (ky, kx) order of Y[(gy + ky + py - 1, gx + kx + px
+// - 1)][phase, k, co] (+0 for a neighbour outside the image, the term of convt_scatter_kernel's zero-filled halo row),
+// + bias, optional ReLU.  So h and x_hat are bitwise the two separate launches'.
+// Shared memory (1024-byte aligned): ring S x (A box + 64 weight rows) | h 128 KB | gathered output weight 16 KB | bars.
+constexpr int TAIL_PHASE_ROWS = 4 * 128;   // h rows per tile: 4 phases x 128 pixels
+
+template <bool BF16, int N, int N2, bool TAIL = false>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant__ CUtensorMap tma_w,
               const __grid_constant__ CUtensorMap tma_w2, const __grid_constant__ WgParams p) {
+    static_assert(!TAIL || (!BF16 && N == SC_N && N2 == 0), "TAIL: TF32, 64 channels of h, no second GEMM");
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = ptx::smem_u32(smem_raw);
     const uint32_t sbase = (raw + 1023u) & ~1023u;
     constexpr int STAGE = A_BYTES + N * 128;
     constexpr int KC2 = chain_chunks<BF16, N>();
+    constexpr int HCHUNK = TAIL_PHASE_ROWS * 128;      // TAIL: one 32-channel chunk of h
     const int S = p.stages;
     // N2 > 0: KC2 intermediate tiles [128 px][128 B], then the KC2 W2 tiles [N2][128 B]
+    // TAIL: KC2 chunks of h, then the KC2 chunks of the gathered output weight [64][128 B]
     const uint32_t mid = sbase + (uint32_t)(S * STAGE);
-    const uint32_t w2s = mid + (uint32_t)(KC2 * A_BYTES);
-    const uint32_t bars = mid + (N2 > 0 ? (uint32_t)(KC2 * (A_BYTES + N2 * 128)) : 0u);
+    const uint32_t w2s = mid + (uint32_t)(KC2 * (TAIL ? HCHUNK : A_BYTES));
+    const uint32_t bars = mid + (N2 > 0 ? (uint32_t)(KC2 * (A_BYTES + N2 * 128))
+                                 : TAIL ? (uint32_t)(KC2 * (HCHUNK + SC_BBYTES)) : 0u);
     auto full = [&](int s) { return bars + 8u * s; };
     auto empty = [&](int s) { return bars + 8u * (WG_MAX_STAGES + s); };
     const uint32_t w2bar = bars + 8u * (2 * WG_MAX_STAGES);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int ph = blockIdx.y;
+    const int ph0 = TAIL ? 0 : blockIdx.y, nph = TAIL ? 4 : 1;      // the phases this CTA runs
     int tile = blockIdx.x;
     const int tx = tile % p.tiles_x; tile /= p.tiles_x;
     const int ty = tile % p.tiles_y; tile /= p.tiles_y;
     const int gx0 = tx * p.BW, gy0 = ty * p.BH, n0 = tile * p.BN;
-    const int nsteps = p.nsteps[ph];
 
     if (tid == 0) {
         for (int s = 0; s < S; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), 2); }
@@ -136,40 +187,130 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
         }
         pdl_wait();                    // ... the activations do
         if (lane == 0) {
-            for (int i = 0; i < nsteps; ++i) {
-                const int s = i % S;
-                if (i >= S) ptx::mbar_wait(empty(s), (uint32_t)((i / S - 1) & 1));
-                const int4 st = p.steps[ph][i];
-                const uint32_t dst = sbase + (uint32_t)(s * STAGE);
-                ptx::mbar_expect_tx(full(s), (uint32_t)STAGE);
-                ptx::tma_load_4d(dst, &tma_in, full(s), st.x, gx0 * p.in_step + st.y, gy0 * p.in_step + st.z, n0);
-                ptx::tma_load_2d(dst + A_BYTES, &tma_w, full(s), st.x, st.w);
-            }
+            int g = 0;                 // ring slot counter over the CTA's phases
+            for (int ph = ph0; ph < ph0 + nph; ++ph)
+                for (int i = 0; i < p.nsteps[ph]; ++i, ++g) {
+                    const int s = g % S;
+                    if (g >= S) ptx::mbar_wait(empty(s), (uint32_t)((g / S - 1) & 1));
+                    const int4 st = p.steps[ph][i];
+                    const uint32_t dst = sbase + (uint32_t)(s * STAGE);
+                    ptx::mbar_expect_tx(full(s), (uint32_t)STAGE);
+                    ptx::tma_load_4d(dst, &tma_in, full(s), st.x, gx0 * p.in_step + st.y, gy0 * p.in_step + st.z, n0);
+                    ptx::tma_load_2d(dst + A_BYTES, &tma_w, full(s), st.x, st.w);
+                }
         }
         return;
     }
     if (warp < 4) return;
 
+    // TAIL: the output weight does not depend on the previous layer
+    if constexpr (TAIL) gather_shuffle_weight<false>(w2s, p.tail_w, N, p.tail_cout, KC2, tid - 128);
     pdl_wait();                        // skip / out may belong to the previous layer
     const int wgi = (warp >> 2) - 1;   // pixel rows 64 * wgi .. + 63 of the tile
     float acc[N / 2];
+    int g = 0;
+    for (int ph = ph0; ph < ph0 + nph; ++ph) {
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-    for (int i = 0; i < nsteps; ++i) {
-        const int s = i % S;
-        ptx::mbar_wait(full(s), (uint32_t)((i / S) & 1));
-        const uint32_t a = sbase + (uint32_t)(s * STAGE) + (uint32_t)(wgi * 64 * 128), b = sbase + (uint32_t)(s * STAGE) + A_BYTES;
-        wg::fence();
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+        for (int i = 0; i < p.nsteps[ph]; ++i, ++g) {
+            const int s = g % S;
+            ptx::mbar_wait(full(s), (uint32_t)((g / S) & 1));
+            const uint32_t a = sbase + (uint32_t)(s * STAGE) + (uint32_t)(wgi * 64 * 128), b = sbase + (uint32_t)(s * STAGE) + A_BYTES;
+            wg::fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wg::mma<BF16, N>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
-        wg::commit();
-        wg::wait<0>();
-        wg::fence_regs<N>(acc);
-        if ((warp & 3) == 0 && lane == 0) ptx::mbar_arrive(empty(s));
+            for (int kk = 0; kk < 4; ++kk) wg::mma<BF16, N>(acc, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+            wg::commit();
+            wg::wait<0>();
+            wg::fence_regs<N>(acc);
+            if ((warp & 3) == 0 && lane == 0) ptx::mbar_arrive(empty(s));
+        }
+        if constexpr (TAIL) {
+            // + bias, ReLU (store_tile's order) -> h in shared memory, and to `out` when given
+            const int wl = warp & 3, cq = 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = wgi * 64 + wl * 16 + (lane >> 2) + 8 * h;
+                const int bw = row % p.BW, bh = (row / p.BW) % p.BH, bn = row / (p.BW * p.BH);
+                const int hr = (bn * 2 * p.BH + 2 * bh + p.out_py[ph]) * 2 * p.BW + 2 * bw + p.out_px[ph];
+                const bool live = gx0 + bw < p.OWg[ph] && gy0 + bh < p.OHg[ph] && n0 + bn < p.B;
+                float *o = reinterpret_cast<float *>(p.out) + (long long)(n0 + bn) * p.out_sn +
+                           (long long)((gy0 + bh) * p.out_step + p.out_py[ph]) * p.out_sh +
+                           (long long)((gx0 + bw) * p.out_step + p.out_px[ph]) * p.out_sw;
+#pragma unroll
+                for (int j = 0; j < N / 8; ++j) {
+                    const int c = 8 * j + cq;
+                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    if (p.bias) { v0 += __ldg(p.bias + c); v1 += __ldg(p.bias + c + 1); }
+                    if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                    const uint32_t addr = mid + (uint32_t)((c >> 5) * HCHUNK + hr * 128 + ((((c & 31) >> 2) ^ (hr & 7)) << 4) + (c & 3) * 4);
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
+                    if (p.out && live) *reinterpret_cast<float2 *>(o + c) = make_float2(v0, v1);
+                }
+            }
+        }
     }
 
-    if constexpr (N2 == 0) {
-        store_tile<N>(p, acc, ph, wgi, gx0, gy0, n0, p.skip, p.relu);
+    if constexpr (TAIL) {
+        ptx::fence_proxy_async();                        // h (generic-proxy writes) -> visible to wgmma
+        ptx::named_bar_sync(1, 256);                     // h and the gathered output weight are complete
+        const int wl = warp & 3, cq = 2 * (lane & 3);
+        for (int blk = 4 * wgi; blk < 4 * wgi + 4; ++blk) {
+            float y[SC_N / 2];
+#pragma unroll
+            for (int i = 0; i < SC_N / 2; ++i) y[i] = 0.f;
+            wg::fence();
+#pragma unroll
+            for (int c = 0; c < KC2; ++c) {
+                const uint32_t a = mid + (uint32_t)(c * HCHUNK + blk * 64 * 128), b = w2s + (uint32_t)(c * SC_BBYTES);
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) wg::mma<false, SC_N>(y, wg::desc_sw128(a + 32u * kk), wg::desc_sw128(b + 32u * kk), 1u);
+            }
+            wg::commit();
+            wg::wait<0>();
+            wg::fence_regs<SC_N>(y);
+            ptx::named_bar_sync(2 + wgi, 128);           // the whole warpgroup's GEMM has read the block's h rows
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int q = blk * 64 + wl * 16 + (lane >> 2) + 8 * h;
+#pragma unroll
+                for (int j = 0; j < SC_N / 8; ++j) {
+                    const int c = 8 * j + cq;
+                    const uint32_t addr = mid + (uint32_t)((c >> 5) * HCHUNK + q * 128 + (((c & 31) + 2 * q) & 31) * 4);
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(y[4 * j + 2 * h]), "f"(y[4 * j + 2 * h + 1]) : "memory");
+                }
+            }
+        }
+        ptx::named_bar_sync(1, 256);                     // Y of the whole tile is staged
+        // one output pixel per thread and step, (image, co, oy, ox) with ox fastest: coalesced NCHW rows
+        const int H = p.OHg[0], W = p.OWg[0];            // the latent: every phase of the k4 s2 p1 layer is H x W
+        const int lw = __ffs(4 * p.BW) - 1, lh = __ffs(4 * p.BH) - 1, Cout = p.tail_cout;
+        const float *const ys = reinterpret_cast<const float *>(smem_raw + (mid - raw));
+        auto yat = [&](int q, int col) {                 // Y[q][col]
+            return ys[(col >> 5) * (HCHUNK / 4) + q * 32 + (((col & 31) + 2 * q) & 31)];
+        };
+        const int total = (p.BN * Cout) << (lw + lh);
+        for (int e = tid - 128; e < total; e += 256) {
+            const int ox = e & (4 * p.BW - 1), oy = (e >> lw) & (4 * p.BH - 1), co = (e >> (lw + lh)) % Cout;
+            const int bn = (e >> (lw + lh)) / Cout;
+            if (ox >= 4 * W || oy >= 4 * H || n0 + bn >= p.B) continue;
+            const int gy = oy >> 1, py = oy & 1, gx = ox >> 1, px = ox & 1;
+            const int base = bn * 4 * p.BH * p.BW, col = (py * 2 + px) * 16 + co;
+            float t[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int hy = gy + (k >> 1) + py - 1, hx = gx + (k & 1) + px - 1;
+                t[k] = hy >= 0 && hy < 2 * H && hx >= 0 && hx < 2 * W ? yat(base + hy * 2 * p.BW + hx, col + 4 * k) : 0.f;
+            }
+            float v = t[0];
+            v += t[1];
+            v += t[2];
+            v += t[3];
+            v += p.tail_bias ? __ldg(p.tail_bias + co) : 0.f;
+            if (p.tail_relu) v = fmaxf(v, 0.f);
+            p.tail_out[(long long)(n0 + bn) * Cout * 16 * H * W + (long long)co * 16 * H * W + oy * 4 * W + ox] = v;
+        }
+    } else if constexpr (N2 == 0) {
+        store_tile<N>(p, acc, ph0, wgi, gx0, gy0, n0, p.skip, p.relu);
     } else {
         // relu(first GEMM) -> rows of 128 bytes (64 bf16 / 32 fp32 channels per chunk), 128-byte swizzle: 16-byte
         // piece j of row r sits at j ^ (r & 7)
@@ -214,7 +355,7 @@ wgconv_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_constant_
         wg::commit();
         wg::wait<0>();
         wg::fence_regs<N2>(acc2);
-        store_tile<N2>(p, acc2, ph, wgi, gx0, gy0, n0, p.skip, p.relu);
+        store_tile<N2>(p, acc2, ph0, wgi, gx0, gy0, n0, p.skip, p.relu);
     }
 }
 
@@ -265,7 +406,11 @@ int wg_gemm_cols(int ncols) {
 
 int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     if (L.nph < 1 || L.nph > 4 || wg_gemm_cols(L.N) != L.N || L.ncols > L.N) return VQB_ERR_UNSUPPORTED;
-    const wg_fn fn = pick(L.bf16, L.N, L.N2);
+    const bool tail = L.tail_out != nullptr;
+    if (tail && (L.bf16 || L.N != SC_N || L.ncols != SC_N || L.N2 != 0 || L.nph != 4 || L.out_step != 2 ||
+                 L.tail_cout < 1 || L.tail_cout > 4))
+        return VQB_ERR_UNSUPPORTED;
+    const wg_fn fn = tail ? wgconv_kernel<false, SC_N, 0, true> : pick(L.bf16, L.N, L.N2);
     if (!fn) return VQB_ERR_UNSUPPORTED;
     const int esz = L.bf16 ? 2 : 4, ck = 128 / esz;       // elements per 128-byte K chunk
     if (L.Cin % ck != 0 || L.w_inner % ck != 0) return VQB_ERR_UNSUPPORTED;
@@ -277,6 +422,8 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     q.in_step = L.in_step; q.out_step = L.out_step;
     q.relu = L.relu; q.out_bf16 = L.out_bf16;
     q.out_sn = L.out_sn; q.out_sh = L.out_sh; q.out_sw = L.out_sw; q.out_sc = L.out_sc;
+    q.tail_w = L.tail_w; q.tail_bias = L.tail_bias; q.tail_out = L.tail_out; q.tail_cout = L.tail_cout;
+    q.tail_relu = L.tail_relu;
     int maxw = 0, maxh = 0, maxk = 1;
     for (int i = 0; i < L.nph; ++i) {
         if (L.nsteps[i] > WG_MAX_STEPS) return VQB_ERR_UNSUPPORTED;
@@ -297,6 +444,11 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     q.tiles_x = (maxw + q.BW - 1) / q.BW;
     q.tiles_y = (maxh + q.BH - 1) / q.BH;
     const long long tiles_n = (L.B + q.BN - 1) / q.BN;
+    if (tail) {      // whole images per tile, and every phase over the same H x W grid
+        if (q.tiles_x != 1 || q.tiles_y != 1) return VQB_ERR_UNSUPPORTED;
+        for (int i = 0; i < 4; ++i)
+            if (L.OHg[i] != maxh || L.OWg[i] != maxw) return VQB_ERR_UNSUPPORTED;
+    }
 
     const CUtensorMapDataType dt = L.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
     CUtensorMap tin, tw, tw2;
@@ -323,7 +475,8 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     const long long grid = (long long)q.tiles_x * q.tiles_y * tiles_n;
     if (grid <= 0 || grid > 0x7fffffffLL) return VQB_ERR_UNSUPPORTED;
     const int stage = A_BYTES + L.N * 128;
-    const int fixed = kc2 * (A_BYTES + L.N2 * 128) + 8 * (2 * WG_MAX_STAGES + 1) + 1024;
+    const int fixed = (tail ? (SC_N / 32) * (TAIL_PHASE_ROWS * 128 + SC_BBYTES) : kc2 * (A_BYTES + L.N2 * 128)) +
+                      8 * (2 * WG_MAX_STAGES + 1) + 1024;
     auto ring = [&](int budget) {
         const int st = (budget - fixed) / stage;
         return st > WG_MAX_STAGES ? WG_MAX_STAGES : st > maxk ? maxk : st;
@@ -331,7 +484,7 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     int stages = ring(220 * 1024);
     if (stages < 1) return VQB_ERR_UNSUPPORTED;
     static bool attr_set[64] = {false};      // per instantiation (slot below): every ring size fits in 220 KB
-    const int slot = (L.bf16 ? 32 : 0) + (L.N2 == 128 ? 16 : L.N2 == 64 ? 8 : 0) + (L.N == 16 ? 0 : L.N == 32 ? 1 : L.N == 64 ? 2 : L.N == 128 ? 3 : 4);
+    const int slot = tail ? 24 : (L.bf16 ? 32 : 0) + (L.N2 == 128 ? 16 : L.N2 == 64 ? 8 : 0) + (L.N == 16 ? 0 : L.N == 32 ? 1 : L.N == 64 ? 2 : L.N == 128 ? 3 : 4);
     if (!attr_set[slot]) {
         cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
         if (e != cudaSuccess) return (int)e;
@@ -345,7 +498,7 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int shared = ring(113 * 1024);
-    if (grid * L.nph > sms && shared >= (maxk < 3 ? maxk : 3) && shared < stages) {
+    if (!tail && grid * L.nph > sms && shared >= (maxk < 3 ? maxk : 3) && shared < stages) {
         int per_sm = 0;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, WG_THREADS, (size_t)(shared * stage + fixed)) ==
                 cudaSuccess && per_sm >= 2)
@@ -353,7 +506,8 @@ int launch_wgconv(const WgLaunch &L, cudaStream_t s) {
     }
     q.stages = stages;
     const int smem = stages * stage + fixed;
-    if (cudaError_t le = vqb_launch(fn, dim3((unsigned)grid, (unsigned)L.nph), dim3(WG_THREADS), (size_t)smem, s, tin, tw, tw2, q))
+    if (cudaError_t le = vqb_launch(fn, dim3((unsigned)grid, tail ? 1u : (unsigned)L.nph), dim3(WG_THREADS), (size_t)smem, s,
+                                    tin, tw, tw2, q))
         return (int)le;
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
@@ -859,8 +1013,6 @@ int launch_res_wg(int bf16, const void *r, const void *w1, const void *w2, void 
 // while warpgroups 0 and 1 run the GEMM and the epilogue.
 // w_shuffle: [9 taps (dy, dx)][16][Cin] (the region of vqb_pack_conv_weight_f32 at conv_pack_shuffle_offset, or
 // vqb_pack_conv_weight_bf16); row (py * 2 + px) * Cout + co of tap (dy + 1) * 3 + dx + 1.
-constexpr int SC_N = 64;                   // GEMM columns: 4 phases x 4 neighbours (ky, kx) x 4 channels
-constexpr int SC_BBYTES = SC_N * 128;      // one 128-byte channel chunk of the gathered weight
 constexpr int SC_ROW = 66;                 // staged floats per halo pixel: the 64 columns + 2 against bank conflicts
 constexpr int SC_STAGE_BYTES = 128 * SC_ROW * 4;
 constexpr int SC_MAX_STAGES = 4;
@@ -914,23 +1066,8 @@ convt_scatter_kernel(const __grid_constant__ CUtensorMap tma_in, const __grid_co
         return;
     }
 
-    // gather the weight (it does not depend on the previous layer): row r = phase * 16 + k * 4 + co, 16-byte piece j
-    // of row r at j ^ (r & 7)
-    {
-        const size_t row_bytes = (size_t)p.Cin * (BF16 ? 2 : 4);
-        for (int i = tid; i < p.nc * SC_N * 8; i += 256) {
-            const int j = i & 7, r = (i >> 3) % SC_N, c = i / (8 * SC_N);
-            const int ph = r >> 4, k = (r >> 2) & 3, co = r & 3;
-            const int tap = ((k >> 1) + (ph >> 1)) * 3 + (k & 1) + (ph & 1);
-            uint4 v = make_uint4(0u, 0u, 0u, 0u);
-            if (co < p.Cout)
-                v = __ldg(reinterpret_cast<const uint4 *>(reinterpret_cast<const unsigned char *>(p.w) +
-                          (size_t)(tap * 16 + ph * p.Cout + co) * row_bytes + c * 128 + j * 16));
-            const uint32_t dst = wres + (uint32_t)(c * SC_BBYTES + r * 128 + ((j ^ (r & 7)) << 4));
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-        }
-        ptx::fence_proxy_async();                      // generic-proxy writes -> visible to wgmma
-    }
+    // gather the weight (it does not depend on the previous layer)
+    gather_shuffle_weight<BF16>(wres, p.w, p.Cin, p.Cout, p.nc, tid);
     float bias[4];
 #pragma unroll
     for (int co = 0; co < 4; ++co) bias[co] = p.bias && co < p.Cout ? __ldg(p.bias + co) : 0.f;
@@ -1049,4 +1186,34 @@ int launch_convt_shuffle_wg(int bf16, const void *in, const void *w_shuffle, con
         return (int)le;
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------------ decoder tail
+// decoder.py:32-35 from d_out: the k4 s2 transposed conv Cin -> 64 with ReLU and the output layer 64 -> Cout <= 4 as one
+// wgconv_kernel launch in TAIL mode (see above the kernel), one CTA per whole-image tile.
+bool decoder_tail_supported(int Cin, int H, int W, int C, int Cout) {
+    return C == SC_N && Cout >= 1 && Cout <= 4 && Cin % 32 == 0 && Cin >= 32 && Cin <= 256 && H >= 1 && W >= 1 &&
+           W <= 16 && pow2_ceil(W) * pow2_ceil(H) <= 128;
+}
+
+int launch_decoder_tail(const void *d_out, const void *convt_w, const float *convt_bias, const void *out_w,
+                        const float *out_bias, void *h_out, float *x_hat, int B, int Cin, int H, int W, int C, int Cout,
+                        int relu_out, cudaStream_t s) {
+    if (!decoder_tail_supported(Cin, H, W, C, Cout) || d_out == h_out || d_out == x_hat) return VQB_ERR_UNSUPPORTED;
+    if ((reinterpret_cast<uintptr_t>(d_out) | reinterpret_cast<uintptr_t>(h_out) | reinterpret_cast<uintptr_t>(x_hat) |
+         reinterpret_cast<uintptr_t>(convt_w) | reinterpret_cast<uintptr_t>(out_w)) & 15)
+        return VQB_ERR_UNSUPPORTED;
+    // the separate launch of the transposed conv (vqb_conv2d_f32 -> launch_conv_tc): the same phases and k-steps
+    const ConvGeom g = conv_geom(4, 4, 2, 1, 1, H, W);
+    ConvPhase phases[4];
+    for (int i = 0; i < 4; ++i)
+        if (!conv_phase(g, i, phases[i])) return VQB_ERR_UNSUPPORTED;
+    WgLaunch L;
+    L.in = d_out; L.B = B; L.Cin = Cin; L.H = H; L.W = W;
+    L.w = convt_w; L.ncols = C;
+    L.bias = convt_bias; L.out = h_out; L.relu = 1;
+    layout_strides(VQB_NHWC, C, g.OH, g.OW, L.out_sn, L.out_sh, L.out_sw, L.out_sc);
+    L.tail_w = static_cast<const float *>(out_w) + conv_pack_shuffle_offset(Cout, C, 4, 4);
+    L.tail_bias = out_bias; L.tail_out = x_hat; L.tail_cout = Cout; L.tail_relu = relu_out;
+    return launch_conv_tc(L, phases, 4, 16, false, s);
 }

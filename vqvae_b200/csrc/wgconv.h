@@ -32,6 +32,13 @@ struct WgLaunch {
     int OHg[4] = {0, 0, 0, 0}, OWg[4] = {0, 0, 0, 0}, out_py[4] = {0, 0, 0, 0}, out_px[4] = {0, 0, 0, 0};
     int nsteps[4] = {0, 0, 0, 0};
     WgStep steps[4][WG_MAX_STEPS];
+    // the decoder's output layer chained on whole-image tiles of this k4 s2 transposed conv (N = 64, TF32, 4 phases):
+    // x_hat NCHW (B, tail_cout, 2 OH, 2 OW) from w_shuffle rows (vqb_pack_conv_weight_f32's shuffle region); out
+    // (h) may then be null.  tail_out = null: no tail.
+    const void *tail_w = nullptr;
+    const float *tail_bias = nullptr;
+    float *tail_out = nullptr;
+    int tail_cout = 0, tail_relu = 0;
 };
 
 int launch_wgconv(const WgLaunch &L, cudaStream_t s);
@@ -55,6 +62,15 @@ bool latent_block_supported(int Cin, int C, int Cmid, int H, int W, int tail_cou
 int launch_latent_block(const void *x, const void *head_w, const float *head_bias, int Cin, int transposed,
                         const void *w1, const void *w2, int napps, const void *tail_w, const float *tail_bias,
                         int tail_cout, void *out, int B, int H, int W, int C, int Cmid, cudaStream_t s);
+// The decoder's k4 s2 transposed conv Cin -> C (bias, ReLU) and the output layer C -> Cout (k4 s2 transposed, + bias,
+// optional ReLU) in one launch (wgconv_kernel in TAIL mode): x_hat NCHW (B, Cout, 4H, 4W) and, when h_out is not
+// null, h NHWC (B, 2H, 2W, C), bitwise the two separate launches.  w: vqb_pack_conv_weight_f32 packings of both
+// layers.  Answers VQB_ERR_UNSUPPORTED, launching nothing, when decoder_tail_supported fails, d_out aliases an
+// output or a pointer is not 16-byte aligned.
+bool decoder_tail_supported(int Cin, int H, int W, int C, int Cout);
+int launch_decoder_tail(const void *d_out, const void *convt_w, const float *convt_bias, const void *out_w,
+                        const float *out_bias, void *h_out, float *x_hat, int B, int Cin, int H, int W, int C, int Cout,
+                        int relu_out, cudaStream_t s);
 bool convt_shuffle_supported(int Cin, int Cout);
 int launch_convt_shuffle_wg(int bf16, const void *in, const void *w_shuffle, const float *bias, float *out, int B, int Cin,
                             int H, int W, int Cout, int relu, cudaStream_t s);

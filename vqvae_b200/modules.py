@@ -320,6 +320,16 @@ def _latent_block(head, stack, h, B, H, W, tail=None):
                             tail_cout=0 if tail is None else tail.out_channels)
 
 
+def _decoder_tail(convt, out, d_out, B, H, W, keep_h):
+    """VQVAE._walk's TF32 path: the k4 s2 transposed conv `convt` (its ReLU folded in) and the output layer `out` on
+    NHWC d_out as one launch (ops.decoder_tail) -> (x_hat NCHW, h NHWC if keep_h else None), bitwise the separate
+    launches.  None (nothing allocated or launched) when the library does not take the shapes: the caller runs the
+    separate launches then."""
+    return ops.decoder_tail(d_out, _packed(convt.weight, _pack_key(convt, False)), _bias(convt),
+                            _packed(out.weight, _pack_key(out, False)), _bias(out), B=B, Cin=convt.in_channels, H=H,
+                            W=W, C=convt.out_channels, Cout=out.out_channels, keep_h=keep_h)
+
+
 class Encoder(nn.Module):
     """q_theta(z|x): models/encoder.py:9-43."""
 
@@ -394,10 +404,11 @@ class Decoder(nn.Module):
             nn.ConvTranspose2d(h_dim // 2, 3, kernel_size=kernel, stride=stride, padding=1),
         )
 
-    def _forward_from_nhwc(self, z, B, H, W, bf16=False, acts=None, fuse=False):
+    def _forward_from_nhwc(self, z, B, H, W, bf16=False, acts=None, fuse=False, fuse_tail=False):
         """z: NHWC (B,H,W,in_dim), bf16 in the bf16 pipeline -> x_hat fp32 NCHW.  `acts` (a dict, training walk)
         receives the stack's input and output and the last hidden activation as "dec".  `fuse` (VQVAE._walk's TF32
-        inference path): the first conv and the stack in one launch when _latent_block takes them."""
+        inference path): the first conv and the stack in one launch when _latent_block takes them.  `fuse_tail`
+        (VQVAE._walk in TF32, both walks): the last two layers in one launch when _decoder_tail takes them."""
         ics = self.inverse_conv_stack
         h = _latent_block(ics[0], ics[1], z, B, H, W) if fuse else None      # k3 s1 p1: H, W unchanged
         if h is None:
@@ -405,10 +416,15 @@ class Decoder(nn.Module):
             d1 = h
             h = ics[1]._apply_nhwc(h, B, H, W, bf16)
         d_out = h
-        h, H, W = _run_conv(ics[2], h, B, H, W, bf16, relu=True)
+        tail = _decoder_tail(ics[2], ics[4], d_out, B, H, W, acts is not None) if fuse_tail else None
+        if tail is not None:
+            x_hat, h = tail
+        else:
+            h, H, W = _run_conv(ics[2], h, B, H, W, bf16, relu=True)
+            x_hat = _run_conv(ics[4], h, B, H, W, bf16, out_layout=NCHW)[0]
         if acts is not None:
             acts["dec"] = (d1, d_out, h)
-        return _run_conv(ics[4], h, B, H, W, bf16, out_layout=NCHW)[0]
+        return x_hat
 
     def forward(self, x):
         if _trains(self, x):
@@ -922,8 +938,10 @@ class VQVAE(nn.Module):
         training backward reads."""
         # Inference in TF32: each side's k3 conv, its ResidualStack and (encoder) the pre-quantization conv run as one
         # launch where _latent_block takes the shape, bitwise the separate launches.  The training walk keeps those,
-        # since its backward reads the activations between them.
-        fuse = acts is None and not bf16 and _conv_precision() == PRECISIONS["tf32"]
+        # since its backward reads the activations between them.  The decoder's last two layers run as one launch in
+        # both walks: it can also store the hidden activation the backward reads.
+        tf32 = not bf16 and _conv_precision() == PRECISIONS["tf32"]
+        fuse = acts is None and tf32
         z_e, B, H, W = self._encode_rows(x, bf16, acts, fuse)                # vqvae.py:31-33
         vq = self.vector_quantization
         D = vq.e_dim
@@ -946,7 +964,7 @@ class VQVAE(nn.Module):
             if not torch.cuda.is_current_stream_capturing():
                 for t in (sse, hist, embedding_loss, perplexity):
                     t.record_stream(side)
-        x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16, acts, fuse)  # :36
+        x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16, acts, fuse, tf32)  # :36
         main.wait_stream(side)
         if not torch.cuda.is_current_stream_capturing():
             # the two scalars were allocated in the side stream's pool and are consumed on the caller's stream: without this

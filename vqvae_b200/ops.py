@@ -244,6 +244,29 @@ def latent_block(x, head_w, head_bias, w1_packed, w2_packed, tail_w=None, tail_b
     return out
 
 
+def decoder_tail(d_out, convt_w, convt_bias, out_w, out_bias, *, B, Cin, H, W, C, Cout, relu_out=False, keep_h=False):
+    """relu(k4 s2 transposed conv of NHWC d_out + convt_bias) -> h, then the k4 s2 transposed conv of h to Cout channels +
+    out_bias (ReLU'd if relu_out), as ONE TF32 launch (vqb_decoder_tail_tf32), bitwise the separate calls.  Returns
+    (x_hat NCHW (B, Cout, 4H, 4W), h NHWC (B, 2H, 2W, C) if keep_h else None); None (nothing allocated or launched) for a
+    shape the launch does not take."""
+    _require_cuda(d_out, "input")
+    if not lib().vqb_decoder_tail_supported(Cin, H, W, C, Cout):
+        return None
+    x_hat = torch.empty((B, Cout, 4 * H, 4 * W), dtype=torch.float32, device=d_out.device)
+    h = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float32, device=d_out.device) if keep_h else None
+    span = _Span(f"convT {Cin}->{C} k4s2 {H}x{W} +convT {C}->{Cout} k4s2")
+    rc = lib().vqb_decoder_tail_tf32(d_out.data_ptr(), convt_w.data_ptr(),
+                                     convt_bias.data_ptr() if convt_bias is not None else None, out_w.data_ptr(),
+                                     out_bias.data_ptr() if out_bias is not None else None,
+                                     h.data_ptr() if h is not None else None, x_hat.data_ptr(), B, Cin, H, W, C, Cout,
+                                     int(bool(relu_out)), _stream())
+    if rc == _lib.ERR_UNSUPPORTED:      # a supported shape declined only for aliasing or alignment
+        return None
+    check(rc, "decoder_tail")
+    span.done()
+    return x_hat, h
+
+
 def vq_forward(z_rows, codebook, zq_dtype=torch.float32):
     """Fused VectorQuantizer core on (N,D) fp32 rows -> (idx int64 (N,), zq (N,D), sse f64 (1,),
     hist int32 (K,)); `sse` is final when the call returns.  zq_dtype=torch.bfloat16
