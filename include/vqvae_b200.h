@@ -363,6 +363,27 @@ int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *codes, const 
 int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, int B, int H, int W,
                            int64_t *codes, float *step_logits, void *workspace, size_t workspace_bytes,
                            void *stream);
+/* Workspace of vqb_prior_complete_f32 for any n_given: at least vqb_prior_workspace_bytes, plus every layer's
+ * vertical output as a whole grid, 4*n_layers*B*H*W*dim bytes (0 = bad sizes).                               */
+size_t vqb_prior_complete_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K);
+/* GatedPixelCNN completion: the raster positions p = i*W + j < n_given of every image are given, the rest are
+ * sampled as vqb_prior_generate_f32 samples them.  given (B,H,W) int64: codes[b,p] = given[b,p] for p < n_given,
+ * as given (out-of-range values included; the kernels clamp them where they embed them); given[b,p] for
+ * p >= n_given is never read.  Code (b,p) for p >= n_given is the smallest k with u[b,p] < CDF_k of that step's
+ * logits, which are bitwise vqb_prior_forward_f32's logits at p on the returned codes (clamped); so with the same
+ * u, completing a prefix of vqb_prior_generate_f32's output returns that output bitwise.  u at p < n_given is
+ * not read; step_logits (NULL or (B,H,W,input_dim)) is written only at p >= n_given.
+ * With i0 = n_given / W and j0 = n_given % W: one launch copies the given codes and embeds them; if i0 > 0, one
+ * launch per layer computes its vertical output on rows [0, i0); rows i0 .. H-1 then run as in generate, with, in
+ * row i0 when j0 > 0, one launch per layer of horizontal stacks over columns [0, j0) before the steps from j0.
+ * 0 < n_given < H*W: 1 + n_layers*[i0 > 0] + n_layers*(H - i0) + n_layers*[j0 > 0] + (H*W - n_given) launches;
+ * n_given = 0 is vqb_prior_generate_f32 (its launches and codes); n_given = H*W is the copy alone.
+ * workspace: n_given < W needs vqb_prior_workspace_bytes (generate's rings), n_given >= W
+ * vqb_prior_complete_workspace_bytes (whole-grid vertical outputs).  VQB_ERR_BAD_ARG for n_given outside
+ * [0, H*W]; VQB_ERR_UNSUPPORTED, before any launch, for a layer 0 generate refuses.  No host synchronisation.  */
+int vqb_prior_complete_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, const int64_t *given,
+                           int64_t n_given, int B, int H, int W, int64_t *codes, float *step_logits,
+                           void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- Gated PixelCNN prior, training (fp32 on CUDA cores) ------------------------------------------------------
  * The forward keeps its activations in `saved`; the backward turns d_logits into the gradient of every parameter.

@@ -3,7 +3,9 @@
   python tools/bench_prior.py [--iters N]
 
 Reports generate() for the reference's CIFAR settings (B=100, 8x8, K=512, dim=64, 15 layers, labels arange(10) x 10)
-and for the cfg3 latent (B=16, 64x64, K=1024), eagerly and as a CUDA-graph replay; the teacher-forced forward at
+and for the cfg3 latent (B=16, 64x64, K=1024), eagerly and as a CUDA-graph replay; complete() of the same two
+shapes with the top half of each grid given (n_given = 32 and 2048), the same ways, with launches per call and the
+ratio of its graph replay to generate's ("vs_generate_graph"); the teacher-forced forward at
 B=32, 8x8; algorithmic FLOPs of the incremental schedule and of the reference's one-forward-per-position schedule;
 and the unmodified reference's GatedPixelCNN.generate in stock PyTorch eager on the same GPU ("kind": "reference",
 from the copy oracle/prior_ref.py makes in oracle/_ref; without that copy the torch restatement
@@ -88,6 +90,33 @@ def bench_generate(m, B, S, iters, graph=True):
     return out
 
 
+def bench_complete(m, B, S, n_given, iters, ref_ms=None):
+    """complete() of B grids of SxS from their first n_given positions: eager (a fresh torch.rand per call, as the public
+    method draws) and as a CUDA-graph replay of _complete, with launches per call; ref_ms: generate's time at the same
+    shape, for the ratio."""
+    from vqvae_b200 import ops
+    labels = (torch.arange(10, device="cuda").repeat((B + 9) // 10))[:B]
+    x = torch.randint(0, m.embedding.num_embeddings, (B, S, S), device="cuda")
+    m.complete(x, labels, n_given)
+    n0 = ops.launch_count()
+    m.complete(x, labels, n_given)
+    launches = ops.launch_count() - n0
+    eager = _time(lambda: m.complete(x, labels, n_given), iters)
+    out = dict(B=B, grid=S, n_given=n_given, eager_ms=eager, launches=launches,
+               samples_per_s_eager=B / eager * 1e3)
+    u = torch.rand((B, S, S), device="cuda")
+    m._complete(labels, u, x, n_given)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        m._complete(labels, u, x, n_given)
+    ms = _time(g.replay, iters)
+    out.update(graph_ms=ms, samples_per_s_graph=B / ms * 1e3)
+    if ref_ms is not None:
+        out["vs_generate_graph"] = ms / ref_ms
+    return out
+
+
 def _reference(m, labels, shape, B, rows=None):
     """(callable, kind) sampling with the reference: its own GatedPixelCNN ("reference", the verbatim copy made by
     oracle.prior_ref.build_prior_ref) holding m's weights, or the torch restatement ("port") when the copy is absent.
@@ -131,6 +160,7 @@ def main():
         res["generate_8x8"] = bench_generate(m, 100, 8, a.iters)
         res["generate_8x8"]["flops_incremental"], res["generate_8x8"]["flops_reference_schedule"] = \
             (f * 100 for f in flops(8, 8, 512, 64, 15))
+        res["complete_8x8"] = bench_complete(m, 100, 8, 32, a.iters, res["generate_8x8"]["graph_ms"])
         x = torch.randint(0, 512, (32, 8, 8), device="cuda")
         lab = torch.arange(32, device="cuda") % 10
         res["forward_8x8_B32_ms"] = _time(lambda: m(x, lab), a.iters)
@@ -143,6 +173,8 @@ def main():
         res["generate_64x64"] = bench_generate(m3, 16, 64, max(1, a.iters // 2))
         res["generate_64x64"]["flops_incremental"], res["generate_64x64"]["flops_reference_schedule"] = \
             (f * 16 for f in flops(64, 64, 1024, 64, 15))
+        res["complete_64x64"] = bench_complete(m3, 16, 64, 64 * 32, max(1, a.iters // 2),
+                                               res["generate_64x64"]["graph_ms"])
         lab16 = torch.arange(10, device="cuda").repeat(2)[:16]
         row_fn, kind = _reference(m3, lab16, (64, 64), 16, rows=1)
         row = _time(row_fn, 1)

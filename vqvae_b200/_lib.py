@@ -61,6 +61,8 @@ SIGNATURES = {
     "vqb_prior_layer_f32": (_i, [_vp] * 4 + [_i] * 5 + [_vp] * 4),
     "vqb_prior_forward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
     "vqb_prior_generate_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
+    "vqb_prior_complete_workspace_bytes": (_sz, [_i] * 6),
+    "vqb_prior_complete_f32": (_i, [_vp] * 4 + [_i64] + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
     "vqb_prior_train_saved_bytes": (_sz, [_i] * 5),
     "vqb_prior_forward_train_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
     "vqb_prior_backward_workspace_bytes": (_sz, [_vp] + [_i] * 3),

@@ -1,10 +1,10 @@
 // prior.cu -- the Gated PixelCNN prior (pixelcnn/models.py of the reference), fp32 on CUDA cores (sm_90a).
 //
 // Activations are NHWC rows.  A buffer holds `ring` rows of a (B, ring, W, C) grid and row r lives in slot r % ring:
-// ring = H is a whole grid (the teacher-forced forward), ring = 1 or gen_ring(H) the rows the incremental sampler
-// keeps.  Every output element is one fmaf chain over its inputs in a fixed order (taps, then input channels),
-// started from 0, then the bias: the value of an element does not depend on which positions share a block or on how
-// many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
+// ring = H is a whole grid (the teacher-forced forward, and completion's vertical outputs), ring = 1 or gen_ring(H)
+// the rows the incremental sampler keeps.  Every output element is one fmaf chain over its inputs in a fixed order
+// (taps, then input channels), started from 0, then the bias: the value of an element does not depend on which
+// positions share a block or on how many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
 // sampler's logits are bitwise the forward's logits on the grid it produced.
 #include "pack.cuh"
 #include "prior.cuh"
@@ -73,7 +73,8 @@ __device__ __forceinline__ int horiz_cols(const vqb_prior_layer_weights &w) { re
 
 // Vertical stack of one layer at the P positions of the block (models.py:69-72, :77):
 //   h_vert = vert_stack(x_v) ; out_v = gate(h_vert + emb[label]) ; vh = vert_to_horiz(h_vert) + emb[label]
-// keep.p != nullptr (the training forward) also stores h_vert there for the backward.
+// keep.p != nullptr (the training forward) also stores h_vert there for the backward.  vh.p == nullptr skips vh
+// (completion's prefix rows, whose horizontal stacks never run).
 template <int P>
 __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &out_v,
                                const Act &vh, int H, int W, const Act &keep) {
@@ -108,6 +109,7 @@ __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, con
         const float *e = w.class_emb + (long long)s.lab[p] * C2;
         out_v.at(s.b[p], s.r[p], s.c[p], W)[c] = gate(s.pre[c * P + p] + __ldg(e + c), s.pre[(c + C) * P + p] + __ldg(e + c + C));
     }
+    if (!vh.p) return;
 #pragma unroll
     for (int q = 0; q < 2; ++q)
 #pragma unroll
@@ -211,17 +213,19 @@ __device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, float *c
     }
 }
 
-// Slots of a block over the positions [row0, row0 + nrows) x [0, W) of all B images, position-major in (b, row, col).
+// Slots of a block over the positions [row0, row0 + nrows) x [col0, col0 + ncols) of all B images, position-major in
+// (b, row, col).
 template <int P>
-__device__ void set_slots(Smem<P> &s, int B, int row0, int nrows, int W, const long long *labels, int NC) {
+__device__ void set_slots(Smem<P> &s, int B, int row0, int nrows, int col0, int ncols, const long long *labels,
+                          int NC) {
     if (threadIdx.x < P) {
         const int p = threadIdx.x;
         const long long g = (long long)blockIdx.x * P + p;
-        const long long per = (long long)nrows * W;
+        const long long per = (long long)nrows * ncols;
         if (g < B * per) {
             s.b[p] = (int)(g / per);
-            s.r[p] = row0 + (int)((g % per) / W);
-            s.c[p] = (int)(g % W);
+            s.r[p] = row0 + (int)((g % per) / ncols);
+            s.c[p] = col0 + (int)(g % ncols);
             s.lab[p] = clampi(labels[s.b[p]], NC);
         } else {
             s.b[p] = -1; s.r[p] = 0; s.c[p] = 0; s.lab[p] = 0;
@@ -235,15 +239,17 @@ __global__ void __launch_bounds__(NT) vert_kernel(vqb_prior_layer_weights w, Act
                                                   const long long *labels, int NC, int B, int H, int W, int row0,
                                                   int nrows, Act keep) {
     __shared__ __align__(16) Smem<P> s;
-    set_slots(s, B, row0, nrows, W, labels, NC);
+    set_slots(s, B, row0, nrows, 0, W, labels, NC);
     vert_positions(s, w, in, out_v, vh, H, W, keep);
 }
 
+// over rows [row0, row0 + nrows) x columns [col0, col0 + ncols)
 template <int P>
 __global__ void __launch_bounds__(NT) horiz_kernel(vqb_prior_layer_weights w, Act in, Act vh, Act out_h,
-                                                   const long long *labels, int NC, int B, int H, int W, Act keep) {
+                                                   const long long *labels, int NC, int B, int H, int W, int row0,
+                                                   int nrows, int col0, int ncols, Act keep) {
     __shared__ __align__(16) Smem<P> s;
-    set_slots(s, B, 0, H, W, labels, NC);
+    set_slots(s, B, row0, nrows, col0, ncols, labels, NC);
     horiz_positions(s, w, in, vh, out_h, H, W, keep);
 }
 
@@ -253,7 +259,7 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
                                                   float *logits, Act keep) {
     __shared__ __align__(16) Smem<P> s;
     __shared__ float *out[P];
-    set_slots(s, B, 0, H, W, labels, n.NC);
+    set_slots(s, B, 0, H, 0, W, labels, n.NC);
     if (threadIdx.x < P) {
         const int p = threadIdx.x;
         out[p] = s.b[p] >= 0 ? logits + (long long)s.b[p] * n.K * H * W + (long long)s.r[p] * W + s.c[p] : nullptr;
@@ -336,6 +342,20 @@ __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act 
     }
 }
 
+// Completion's given prefix: codes[b, p] = given[b, p] as given and x0[b, p] = E[clamp(given[b, p])] (embed_kernel's
+// clamp) for the raster positions p < n of every image; positions >= n are not read.
+__global__ void given_kernel(const long long *__restrict__ given, const float *__restrict__ E, int B, long long HW,
+                             long long n, int K, int C, float *__restrict__ x0, long long *__restrict__ codes) {
+    const long long total = (long long)B * n * C;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long q = i / C, pos = q / n * HW + q % n;
+        const int c = (int)(i % C);
+        const long long code = given[pos];
+        x0[pos * C + c] = __ldg(E + (long long)clampi(code, K) * C + c);
+        if (c == 0) codes[pos] = code;
+    }
+}
+
 // the kept-tap packing of pack_prior_at
 __global__ void pack_kernel(const float *__restrict__ w, float *__restrict__ out, int Cout, int Cin, int kh, int kw,
                             int rows, int cols) {
@@ -364,6 +384,7 @@ struct Ws {
     long long fwd_v, fwd_vh, fwd_x;               // forward: x0 | v[2] | vh | x[2]  (whole grids)
     long long gen_x0, gen_vh, gen_x, gen_lg, gen_v;  // sampler: x0 | vh[L] (1 row) | x[L] (1 row) | logits | v[L] (gen_ring)
     long long fwd_total, gen_total;
+    long long comp_total;                         // completion: the sampler's regions with v[L] whole grids (ring = H)
 };
 
 Ws ws_layout(long long B, long long H, long long W, long long C, long long L, long long K) {
@@ -379,6 +400,7 @@ Ws ws_layout(long long B, long long H, long long W, long long C, long long L, lo
     w.gen_lg = w.gen_x + L * B * W * C;
     w.gen_v = w.gen_lg + B * K;                   // last: generate uses the first L * B * ring * W * C floats
     w.gen_total = w.gen_v + L * B * gen_ring((int)H) * W * C;
+    w.comp_total = w.gen_v + L * grid;
     return w;
 }
 
@@ -386,6 +408,58 @@ constexpr int PF = 8;             // positions per block of the whole-grid kerne
 constexpr int PS = 4;             // images per block of the sampling step
 
 unsigned blocks(long long positions, int P) { return (unsigned)((positions + P - 1) / P); }
+
+// The sampler of generate and complete, from raster position n_given = i0*W + j0 on (generate: n_given = 0).  The
+// positions before it are final and their embeddings are in x0.  When i0 > 0, every layer's vertical output is first
+// computed for rows [0, i0) in one launch per layer, into whole-grid rings (ring = H: the completion workspace) that
+// the later row passes read; those rows' vh and horizontal stacks have no reader and are not computed.  Then rows
+// i0 .. H-1 as generate runs them: per row one vertical pass per layer, then one step per position.  In row i0 with
+// j0 > 0, one horizontal launch per layer over columns [0, j0) first fills the one-row x[l] that the step at (i0, j0)
+// reads.  Every value is the fmaf chain generate computes at that position, so the logits are bitwise generate's.
+// Launches: L*[i0 > 0] + L*(H - i0) + L*[j0 > 0] + (H*W - n_given).
+void sample_from(const Net &n, const long long *lab, const float *u, int B, int H, int W, long long n_given,
+                 long long *codes, float *step_logits, float *ws, cudaStream_t s) {
+    const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
+    const int i0 = (int)(n_given / W), j0 = (int)(n_given % W);
+    int reach = 1;
+    for (int l = 1; l < n.L; ++l) reach = max(reach, n.layer[l].kernel / 2 + 1);
+    const int ring = i0 > 0 ? H : gen_ring(H, reach);
+    const long long v_stride = (long long)B * ring * W * n.C, vh_stride = (long long)B * W * 2 * n.C,
+                    x_stride = (long long)B * W * n.C;
+    const Act x0{ws + wl.gen_x0, H, n.C};
+    const auto v = [&](int l) { return Act{ws + wl.gen_v + l * v_stride, ring, n.C}; };
+    const auto vh = [&](int l) { return Act{ws + wl.gen_vh + l * vh_stride, 1, 2 * n.C}; };
+    const auto x = [&](int l) { return Act{ws + wl.gen_x + l * x_stride, 1, n.C}; };
+    unsigned long long launches = 0;
+    if (i0 > 0) {
+        for (int l = 0; l < n.L; ++l)
+            vert_kernel<PF><<<blocks((long long)B * i0 * W, PF), NT, 0, s>>>(
+                n.layer[l], l == 0 ? x0 : v(l - 1), v(l), Act{}, lab, n.NC, B, H, W, 0, i0, Act{});
+        launches += n.L;
+    }
+    for (int i = i0; i < H; ++i) {
+        // row pass: every layer's vertical stack at row i (codes of rows < i are final)
+        for (int l = 0; l < n.L; ++l)
+            vert_kernel<PF><<<blocks((long long)B * W, PF), NT, 0, s>>>(n.layer[l], l == 0 ? x0 : v(l - 1), v(l),
+                                                                        vh(l), lab, n.NC, B, H, W, i, 1, Act{});
+        launches += n.L;
+        const int jstart = i == i0 ? j0 : 0;
+        if (jstart > 0) {
+            for (int l = 0; l < n.L; ++l)
+                horiz_kernel<PF><<<blocks((long long)B * jstart, PF), NT, 0, s>>>(
+                    n.layer[l], l == 0 ? x0 : x(l - 1), vh(l), x(l), lab, n.NC, B, H, W, i, 1, 0, jstart, Act{});
+            launches += n.L;
+        }
+        for (int j = jstart; j < W; ++j) {
+            float *lg = step_logits ? step_logits + ((long long)i * W + j) * n.K : ws + wl.gen_lg;
+            const long long img = step_logits ? (long long)H * W * n.K : n.K;
+            step_kernel<PS><<<blocks(B, PS), NT, 0, s>>>(n, x0, x(0), vh(0), vh_stride, x_stride, lab, u, B, H, W, i,
+                                                         j, lg, img, codes);
+        }
+        launches += W - jstart;
+    }
+    VQB_COUNT_LAUNCH(launches);
+}
 
 }  // namespace
 
@@ -426,7 +500,8 @@ extern "C" int vqb_prior_layer_f32(const vqb_prior_layer_weights *layer, const f
     Act in_v{const_cast<float *>(x_v), H, dim}, in_h{const_cast<float *>(x_h), H, dim};
     Act ov{out_v, H, dim}, oh{out_h, H, dim}, vha{vh, H, 2 * dim};
     vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H, Act{});
-    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W, Act{});
+    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W, 0, H, 0, W,
+                                                  Act{});
     VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -453,7 +528,8 @@ extern "C" int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *co
         const Act vin = l == 0 ? x0 : v[(l - 1) & 1], xin = l == 0 ? x0 : x[(l - 1) & 1];
         vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H,
                                                         Act{});
-        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W, Act{});
+        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W, 0, H, 0,
+                                                         W, Act{});
     }
     head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, x[(n.L - 1) & 1], lab, B, H, W, logits, Act{});
     VQB_COUNT_LAUNCH(2 + 2 * n.L);
@@ -470,33 +546,43 @@ extern "C" int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *l
     if (workspace_bytes < vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
     // Layer 0 must read only codes before (i, j): mask B reads row i and column j, a residual adds x_h at (i, j).
     if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
+    sample_from(n, reinterpret_cast<const long long *>(labels), u, B, H, W, 0, reinterpret_cast<long long *>(codes),
+                step_logits, static_cast<float *>(workspace), (cudaStream_t)stream);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_prior_complete_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K) {
+    const size_t base = vqb_prior_workspace_bytes(B, H, W, dim, n_layers, K);
+    if (!base) return 0;
+    const size_t comp = (size_t)ws_layout(B, H, W, dim, n_layers, K).comp_total * sizeof(float);
+    return comp > base ? comp : base;
+}
+
+extern "C" int vqb_prior_complete_f32(const vqb_prior_net *net, const int64_t *labels, const float *u,
+                                      const int64_t *given, int64_t n_given, int B, int H, int W, int64_t *codes,
+                                      float *step_logits, void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!labels || !u || !given || !codes || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    const long long HW = (long long)H * W;
+    if (n_given < 0 || n_given > HW) return VQB_ERR_BAD_ARG;
+    // a prefix shorter than a row keeps generate's rings (and its workspace); a longer one whole grids
+    const size_t need = n_given < W ? vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)
+                                    : vqb_prior_complete_workspace_bytes(B, H, W, n.C, n.L, n.K);
+    if (workspace_bytes < need) return VQB_ERR_WORKSPACE;
+    if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
-    const long long *lab = reinterpret_cast<const long long *>(labels);
-    const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
     float *ws = static_cast<float *>(workspace);
-    int reach = 1;
-    for (int l = 1; l < n.L; ++l) reach = max(reach, n.layer[l].kernel / 2 + 1);
-    const int ring = gen_ring(H, reach);
-    const long long v_stride = (long long)B * ring * W * n.C, vh_stride = (long long)B * W * 2 * n.C,
-                    x_stride = (long long)B * W * n.C;
-    const Act x0{ws + wl.gen_x0, H, n.C};
-    for (int i = 0; i < H; ++i) {
-        // row pass: every layer's vertical stack at row i (codes of rows < i are final)
-        for (int l = 0; l < n.L; ++l) {
-            const Act vin = l == 0 ? x0 : Act{ws + wl.gen_v + (l - 1) * v_stride, ring, n.C};
-            vert_kernel<PF><<<blocks((long long)B * W, PF), NT, 0, s>>>(
-                n.layer[l], vin, Act{ws + wl.gen_v + l * v_stride, ring, n.C},
-                Act{ws + wl.gen_vh + l * vh_stride, 1, 2 * n.C}, lab, n.NC, B, H, W, i, 1, Act{});
-        }
-        for (int j = 0; j < W; ++j) {
-            float *lg = step_logits ? step_logits + ((long long)i * W + j) * n.K : ws + wl.gen_lg;
-            const long long img = step_logits ? (long long)H * W * n.K : n.K;
-            step_kernel<PS><<<blocks(B, PS), NT, 0, s>>>(n, x0, Act{ws + wl.gen_x, 1, n.C}, Act{ws + wl.gen_vh, 1, 2 * n.C},
-                                                         vh_stride, x_stride, lab, u, B, H, W, i, j, lg, img,
-                                                         reinterpret_cast<long long *>(codes));
-        }
+    long long *out = reinterpret_cast<long long *>(codes);
+    if (n_given > 0) {
+        float *x0 = ws + ws_layout(B, H, W, n.C, n.L, n.K).gen_x0;
+        given_kernel<<<grid_for((long long)B * n_given * n.C), NT, 0, s>>>(
+            reinterpret_cast<const long long *>(given), net->embedding, B, HW, n_given, n.K, n.C, x0, out);
+        VQB_COUNT_LAUNCH(1);
     }
-    VQB_COUNT_LAUNCH((unsigned long long)H * (n.L + W));
+    if (n_given < HW)
+        sample_from(n, reinterpret_cast<const long long *>(labels), u, B, H, W, n_given, out, step_logits, ws, s);
     return vqb_cuda_status(cudaGetLastError());
 }
 
@@ -528,8 +614,8 @@ extern "C" int vqb_prior_forward_train_f32(const vqb_prior_net *net, const int64
                                                         Act{sp + sv.xv(l + 1), H, n.C}, vh, lab, n.NC, B, H, W, 0, H,
                                                         Act{sp + sv.hv(l), H, 2 * n.C});
         horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xh(l), H, n.C}, vh,
-                                                         Act{sp + sv.xh(l + 1), H, n.C}, lab, n.NC, B, H, W,
-                                                         Act{sp + sv.ph(l), H, 2 * n.C});
+                                                         Act{sp + sv.xh(l + 1), H, n.C}, lab, n.NC, B, H, W, 0,
+                                                         H, 0, W, Act{sp + sv.ph(l), H, 2 * n.C});
     }
     head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, Act{sp + sv.xh(n.L), H, n.C}, lab, B, H, W, logits,
                                                     Act{sp + sv.hid(), H, HID});
@@ -562,7 +648,7 @@ extern "C" int vqb_prior_layer_forward_train_f32(const vqb_prior_layer_weights *
     Act ov{out_v, H, dim}, oh{out_h, H, dim}, vha{vh, H, 2 * dim};
     vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H,
                                                  Act{sp + sv.hv(), H, 2 * dim});
-    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W,
+    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W, 0, H, 0, W,
                                                   Act{sp + sv.ph(), H, 2 * dim});
     VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());

@@ -548,6 +548,23 @@ def prior_generate(net, labels, u, step_logits=None):
     return codes
 
 
+def prior_complete(net, labels, u, given, n_given, step_logits=None):
+    """The sampling loop from raster position n_given on (vqb_prior_complete_f32): int64 codes (B,H,W) whose positions
+    < n_given are the int64 `given` (B,H,W) and the rest are drawn with the uniforms u (B,H,W).  step_logits: None,
+    or a (B,H,W,K) fp32 tensor receiving the logits of every step (positions >= n_given)."""
+    B, H, W = u.shape
+    dev = u.device
+    codes = torch.empty((B, H, W), dtype=torch.int64, device=dev)
+    ws = _prior_workspace(net, B, H, W, dev, None if n_given < W else lib().vqb_prior_complete_workspace_bytes)
+    span = _Span(f"prior complete K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W} n_given={n_given}")
+    check(lib().vqb_prior_complete_f32(_lib.C.byref(net), labels.data_ptr(), u.data_ptr(), given.data_ptr(), n_given,
+                                       B, H, W, codes.data_ptr(),
+                                       step_logits.data_ptr() if step_logits is not None else None, ws.data_ptr(),
+                                       ws.numel(), _stream()), "prior_complete")
+    span.done()
+    return codes
+
+
 def prior_forward_train(net, codes, labels, precision="fp32"):
     """prior_forward that also keeps the activations the backward needs: (logits, saved) with saved a uint8 buffer
     of vqb_prior_train_saved_bytes (vqb_prior_forward_train_f32 / _tf32; the logits are bitwise prior_forward's in the

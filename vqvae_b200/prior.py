@@ -12,9 +12,9 @@ requires grad (``_PriorFunction``: the training forward keeps its activations, a
 ``torch.no_grad()`` it is the inference forward.  ``GatedPixelCNN.precision`` (a plain attribute, not in the state
 dict) selects the arithmetic of ``forward``, inference and training alike: "fp32" (the default, CUDA cores) or
 "tf32" (every matrix product on the wgmma TF32 GEMM, operands rounded to TF32, fp32 accumulation; the one-hot
-embedding-gradient sums stay fp32).  ``generate``, ``GatedMaskedConv2d`` and ``GatedActivation`` stay fp32 in both
-modes, and ``set_precision`` does not affect the prior.  ``GatedMaskedConv2d`` and ``GatedActivation`` called on their own
-are differentiable too, under the same rule (grad enabled and an input or a parameter requiring grad):
+embedding-gradient sums stay fp32).  ``generate``, ``complete``, ``GatedMaskedConv2d`` and ``GatedActivation`` stay
+fp32 in both modes, and ``set_precision`` does not affect the prior.  ``GatedMaskedConv2d`` and ``GatedActivation``
+called on their own are differentiable too, under the same rule (grad enabled and an input or a parameter requiring grad):
 ``_GatedLayerFunction`` runs the layer's training forward and single-layer backward (vqb_prior_layer_*_f32),
 ``_GateFunction`` the gate and its backward.  Their outputs are bitwise the inference call's.
 
@@ -29,10 +29,12 @@ Reference behaviour kept on purpose:
   P5  ``layers`` may be replaced by any GatedMaskedConv2d stack (odd kernels up to 15, either mask, with or without
       residual), as the reference's forward walks whatever ``self.layers`` holds.  Every layer must have the model's
       ``dim`` and layer 0's class count (the reference fails on such a model too, with a shape or index error); a
-      RuntimeError before any launch otherwise.  ``generate`` also needs layer 0 to be mask A without residual:
-      anything else reads the code being drawn, so the reference's one-forward-per-position loop is not causal in
-      raster order there, and the sampler refuses it (C ABI: VQB_ERR_UNSUPPORTED)
+      RuntimeError before any launch otherwise.  ``generate`` and ``complete`` also need layer 0 to be mask A without
+      residual: anything else reads the code being drawn, so the reference's one-forward-per-position loop is not
+      causal in raster order there, and the sampler refuses it (C ABI: VQB_ERR_UNSUPPORTED)
 """
+import operator
+
 import torch
 import torch.nn as nn
 
@@ -270,7 +272,7 @@ class GatedPixelCNN(nn.Module):
 
     ``precision``: "fp32" (default) or "tf32", the arithmetic of ``forward`` (see the module docstring).  A plain
     attribute, so state dicts are the reference's; any other value raises ValueError from ``forward``.  ``generate``
-    is fp32 either way."""
+    and ``complete`` are fp32 either way."""
 
     def __init__(self, input_dim=256, dim=64, n_layers=15, n_classes=10):
         super().__init__()
@@ -333,15 +335,19 @@ class GatedPixelCNN(nn.Module):
         keep = []
         return ops.prior_forward(self._net(keep), x, label, precision)
 
+    def _check_causal(self, what):
+        """P5: the sampler needs a layer 0 that reads only the codes before the one being drawn."""
+        first = self.layers[0] if len(self.layers) else None
+        if first is not None and (first.mask_type != "A" or first.residual):
+            raise RuntimeError(f"{what}: layer 0 must be mask A without residual (P5): this one reads "
+                               "the code being drawn, so the logits are not causal in raster order")
+
     def _sample(self, label, u, step_logits=None):
         """generate() with given uniforms u (B,H,W) fp32: the code at (b,i,j) is the smallest k with u < CDF_k.
         fp32 whatever ``precision`` says."""
         B, H, W = u.shape
         _square(H, W, "GatedPixelCNN.generate")
-        first = self.layers[0] if len(self.layers) else None
-        if first is not None and (first.mask_type != "A" or first.residual):
-            raise RuntimeError("GatedPixelCNN.generate: layer 0 must be mask A without residual (P5): this one reads "
-                               "the code being drawn, so the logits are not causal in raster order")
+        self._check_causal("GatedPixelCNN.generate")
         ops._require_cuda(u, "GatedPixelCNN.generate uniforms")
         label = _labels(label, B, u.device, "GatedPixelCNN.generate")
         keep = []
@@ -357,3 +363,48 @@ class GatedPixelCNN(nn.Module):
         ops._require_cuda(torch.empty(0, device=dev), "GatedPixelCNN parameters")
         u = torch.rand((batch_size, H, W), device=dev)
         return self._sample(label, u)
+
+    def _given(self, x, label, n_given):
+        """complete()'s host-side checks, in order, before any CUDA check or launch: the codes' rank, n_given (an
+        int, ValueError outside [0, H*W]), a square grid, layer 0 (P5), the label count.  Returns n_given."""
+        n_given = operator.index(n_given)
+        if x.dim() != 3:
+            raise RuntimeError(f"GatedPixelCNN.complete: expected codes of shape (B,H,W), got {tuple(x.shape)}")
+        B, H, W = x.shape
+        if not 0 <= n_given <= H * W:
+            raise ValueError(f"GatedPixelCNN.complete: n_given must be in [0, H*W] = [0, {H * W}], got {n_given}")
+        _square(H, W, "GatedPixelCNN.complete")
+        self._check_causal("GatedPixelCNN.complete")
+        n = (label if torch.is_tensor(label) else torch.as_tensor(label)).numel()
+        if n != B:
+            raise RuntimeError(f"GatedPixelCNN.complete: expected {B} labels, got {n}")
+        return n_given
+
+    def _complete(self, label, u, x, n_given, step_logits=None):
+        """complete() with given uniforms u (B,H,W) fp32: positions p = i*W + j < n_given are x's codes as given,
+        the code at each later (b,i,j) is the smallest k with u < CDF_k of that step's logits.  step_logits: None or
+        (B,H,W,K) fp32, written at the positions >= n_given only.  fp32 whatever ``precision`` says."""
+        n_given = self._given(x, label, n_given)
+        B, H, W = x.shape
+        if tuple(u.shape) != (B, H, W):
+            raise RuntimeError(f"GatedPixelCNN.complete: uniforms of shape {tuple(u.shape)} for codes {(B, H, W)}")
+        ops._require_cuda(x, "GatedPixelCNN.complete codes")
+        ops._require_cuda(u, "GatedPixelCNN.complete uniforms")
+        label = _labels(label, B, x.device, "GatedPixelCNN.complete")
+        x = x.detach().to(torch.int64).contiguous()
+        if n_given == H * W:                # nothing to sample: no packing, no launch
+            return x.clone()
+        keep = []
+        return ops.prior_complete(self._net(keep), label, _f32(u), x, n_given, step_logits)
+
+    def complete(self, x, label, n_given):
+        """Complete the code grids x (B,H,W) from their first n_given positions in raster order (p = i*W + j):
+        positions < n_given are returned as x holds them, the rest are sampled as generate() samples them, each
+        conditioned on everything before it; x's values there are never read.  A new int64 (B,H,W) tensor; x is not
+        modified.  Draws exactly one torch.rand((B, H, W)) from the current CUDA generator whatever n_given is, so
+        after the same torch.manual_seed, completing any prefix of generate()'s output returns that output.
+        n_given = 0 is generate(); the restrictions are generate()'s (square grids, P5, fp32)."""
+        n_given = self._given(x, label, n_given)
+        ops._require_cuda(x, "GatedPixelCNN.complete codes")
+        u = torch.rand(tuple(x.shape), device=x.device)
+        return self._complete(label, u, x, n_given)
