@@ -384,6 +384,32 @@ size_t vqb_prior_complete_workspace_bytes(int B, int H, int W, int dim, int n_la
 int vqb_prior_complete_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, const int64_t *given,
                            int64_t n_given, int B, int H, int W, int64_t *codes, float *step_logits,
                            void *workspace, size_t workspace_bytes, void *stream);
+/* The draw's knobs, one set for the whole batch.  With z = l / T in fp32 (saturated to +-FLT_MAX) and fkey the
+ * order-preserving map from fp32 to uint32, the kept set is S = {k : fkey(z_k) >= t}, t = max(t_k, t_p):
+ *   t_k  the largest t with at least top_k codes kept (ties at the threshold are kept);
+ *   t_p  the largest t whose kept codes hold at least top_p of the tempered softmax expf(z - max) / sum.
+ * top_k = 0 (or K) and top_p = 1 turn their truncation off; temperature 1, top_k 0, top_p 1 is generate's draw.   */
+typedef struct vqb_prior_sampling {
+    float temperature;                        /* finite, > 0 */
+    int top_k;                                /* 0 (off) .. input_dim */
+    float top_p;                              /* (0, 1]; 1 is off */
+} vqb_prior_sampling;
+/* Workspace of vqb_prior_sample_f32 from raster position n_given: at least what vqb_prior_complete_f32 needs there,
+ * plus 256*ceil(input_dim/32) + 4 bytes per image for the kept-set search and log_prob (0 = bad sizes or n_given outside [0, H*W]). */
+size_t vqb_prior_sample_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K, int64_t n_given);
+/* vqb_prior_complete_f32 (n_given = 0: vqb_prior_generate_f32) drawing each code from the softmax of that step's
+ * tempered logits truncated to S: the smallest k in S with u < CDF_k, CDF the fp32 running sum over S of
+ * q_k = expf(z_k - max) / sum over S, in generate's order (the last k in S with q_k > 0 if rounding leaves u above
+ * the total).  sampling NULL, or knobs off, is complete's draw: the same codes and step logits, bit for bit.
+ * log_prob: NULL, or (B) fp32 receiving, per image, the compensated (Kahan) fp32 sum in raster order over the
+ * sampled positions of l_code - max(l) - logf(sum expf(l - max(l))), the model's untempered, untruncated
+ * log-probability (0 when n_given = H*W).  step_logits stay the raw logits.  given may be NULL when n_given = 0.  The same launches as
+ * vqb_prior_complete_f32 for this n_given, no host synchronisation, the knobs passed as kernel arguments.
+ * VQB_ERR_BAD_ARG for a knob outside its range, VQB_ERR_UNSUPPORTED for a layer 0 generate refuses, both before
+ * any launch.                                                                                                    */
+int vqb_prior_sample_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, const int64_t *given,
+                         int64_t n_given, int B, int H, int W, const vqb_prior_sampling *sampling, int64_t *codes,
+                         float *log_prob, float *step_logits, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- Gated PixelCNN prior, training (fp32 on CUDA cores) ------------------------------------------------------
  * The forward keeps its activations in `saved`; the backward turns d_logits into the gradient of every parameter.

@@ -63,6 +63,8 @@ SIGNATURES = {
     "vqb_prior_generate_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
     "vqb_prior_complete_workspace_bytes": (_sz, [_i] * 6),
     "vqb_prior_complete_f32": (_i, [_vp] * 4 + [_i64] + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
+    "vqb_prior_sample_workspace_bytes": (_sz, [_i] * 6 + [_i64]),
+    "vqb_prior_sample_f32": (_i, [_vp] * 4 + [_i64] + [_i] * 3 + [_vp] * 5 + [_sz, _vp]),
     "vqb_prior_train_saved_bytes": (_sz, [_i] * 5),
     "vqb_prior_forward_train_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
     "vqb_prior_backward_workspace_bytes": (_sz, [_vp] + [_i] * 3),
@@ -99,6 +101,11 @@ class PriorNet(C.Structure):
     """struct vqb_prior_net"""
     _fields_ = [("layers", C.POINTER(PriorLayerWeights)), ("n_layers", _i), ("embedding", _vp), ("out1_w", _vp),
                 ("out1_b", _vp), ("out2_w", _vp), ("out2_b", _vp), ("input_dim", _i), ("dim", _i), ("n_classes", _i)]
+
+
+class PriorSampling(C.Structure):
+    """struct vqb_prior_sampling"""
+    _fields_ = [("temperature", _f), ("top_k", _i), ("top_p", _f)]
 
 
 class PriorLayerGrads(C.Structure):

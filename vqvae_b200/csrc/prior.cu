@@ -6,6 +6,8 @@
 // (taps, then input channels), started from 0, then the bias: the value of an element does not depend on which
 // positions share a block or on how many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
 // sampler's logits are bitwise the forward's logits on the grid it produced.
+#include <cfloat>
+
 #include "pack.cuh"
 #include "prior.cuh"
 
@@ -267,13 +269,51 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
     head_positions(s, n, in, out, (long long)H * W, H, W, keep);
 }
 
+// The draw's knobs (vqb_prior_sampling, checked by the entry point) and its extra outputs.  Samp{} is generate's draw
+// from the plain softmax.
+struct Samp {
+    float T = 1.f;                // temperature
+    int top_k = 0;                // 0 or >= K: no top-k truncation
+    float top_p = 1.f;            // >= 1: no nucleus truncation
+    float *scratch = nullptr;     // the kept-set search's keys and probabilities: search_floats(1, K) per image
+    float *log_prob = nullptr;    // (B) sum of log p_model(code) over the sampled steps, or nullptr
+    float *log_c = nullptr;       // (B) the compensation of log_prob's Kahan sum
+};
+
+// floats of the draw's scratch for B images: per image, per lane of the draw's warp, ceil(K/32) keys and as many
+// probabilities, interleaved by lane so that each warp access is one contiguous 128-byte line; then B floats of
+// log_prob's compensation
+long long search_floats(long long B, long long K) { return B * 64 * ((K + 31) / 32) + B; }
+
+// order-preserving map from fp32 to uint32: a < b  <=>  fkey(a) < fkey(b) (-0 below +0)
+__device__ __forceinline__ unsigned fkey(float z) {
+    const unsigned v = __float_as_uint(z);
+    return (v & 0x80000000u) ? ~v : (v | 0x80000000u);
+}
+
+// z = l / T in fp32, saturated to the finite range so that max(z) - z stays defined for tiny T; l itself at T = 1
+__device__ __forceinline__ float tempered(float l, float T) {
+    return T == 1.f ? l : fminf(fmaxf(l / T, -FLT_MAX), FLT_MAX);
+}
+
+// Warp sums (xor butterfly: every lane ends with the same value, since each pairwise fp32 add is commutative)
+__device__ __forceinline__ float warp_sum(float v) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
 // One sampling step at (i, j) for P images: every layer's horizontal stack, the head, the softmax and the inverse-CDF
 // draw.  The code goes to codes[b, i, j] and its embedding to x0[b, i, j], which later steps and row passes read.
+// `first`: the first sampled step of the call, which writes log_prob instead of adding to it.
 template <int P>
 __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act vh0, long long vh_stride,
                                                   long long x_stride, const long long *labels, const float *u, int B,
                                                   int H, int W, int i, int j, float *logits, long long logit_img,
-                                                  long long *codes) {
+                                                  long long *codes, Samp sp, bool first) {
     __shared__ __align__(16) Smem<P> s;
     __shared__ float *out[P];
     if (threadIdx.x < P) {
@@ -293,25 +333,65 @@ __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act 
     }
     head_positions(s, n, Act{xrow0.p + (n.L - 1) * x_stride, 1, n.C}, out, 1, H, W, Act{});
     __syncthreads();
-    // softmax + inverse CDF, one warp per image: lane L owns logits [L*cs, L*cs + cs); the CDF is the fp32 running sum
-    // of p_k = expf(l_k - max) / sum, over the lanes' chunk sums scanned in lane order and then within the chunk.
+    // softmax + inverse CDF, one warp per image: lane L owns logits [L*cs, L*cs + cs).  z = l / T; the kept set is
+    // S = {k : fkey(z_k) >= t} (t = 0: every code); the CDF is the fp32 running sum of q_k = expf(z_k - max) / sum_S
+    // over k in S, over the lanes' chunk sums scanned in lane order and then within the chunk.  With the default knobs
+    // this is the plain softmax's arithmetic, bit for bit.
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
     const int K = n.K;
+    const bool by_k = sp.top_k > 0 && sp.top_k < K, by_p = sp.top_p < 1.f;
     for (int p = warp; p < P; p += NT / 32) {
         if (s.b[p] < 0) continue;
         const int b = s.b[p];
         const float *lg = out[p];
         const int cs = (K + 31) / 32, k0 = min(K, lane * cs), k1 = min(K, k0 + cs);
         float m = -INFINITY;
-        for (int k = k0; k < k1; ++k) m = fmaxf(m, lg[k]);
-        for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        for (int k = k0; k < k1; ++k) m = fmaxf(m, tempered(lg[k], sp.T));
+        m = warp_max(m);
         float sum = 0.f;
-        for (int k = k0; k < k1; ++k) sum += expf(lg[k] - m);
-        for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        for (int k = k0; k < k1; ++k) sum += expf(tempered(lg[k], sp.T) - m);
+        sum = warp_sum(sum);
+        unsigned t = 0;
+        float sum_s = sum;
+        if (by_k || by_p) {
+            // t = max(t_k, t_p), each the largest threshold whose kept set still has top_k codes / top_p of the
+            // tempered softmax's mass, found bit by bit from the MSB: 32 sweeps over the cached keys and probabilities
+            unsigned *key = reinterpret_cast<unsigned *>(sp.scratch + (long long)b * 64 * cs) + lane;
+            float *prob = sp.scratch + (long long)b * 64 * cs + 32 * cs + lane;
+            for (int k = k0; k < k1; ++k) {
+                const float z = tempered(lg[k], sp.T);
+                key[(k - k0) * 32] = fkey(z);
+                prob[(k - k0) * 32] = expf(z - m) / sum;
+            }
+            unsigned t_k = 0, t_p = 0;
+            for (int bit = 31; bit >= 0; --bit) {
+                const unsigned ck = t_k | 1u << bit, cp = t_p | 1u << bit;
+                int cnt = 0;
+                float mass = 0.f;
+                for (int q = 0; q < k1 - k0; ++q) {
+                    const unsigned kq = key[q * 32];
+                    if (by_k) cnt += kq >= ck;
+                    if (by_p && kq >= cp) mass += prob[q * 32];
+                }
+                for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+                mass = warp_sum(mass);
+                if (by_k && cnt >= sp.top_k) t_k = ck;
+                if (by_p && mass >= sp.top_p) t_p = cp;
+            }
+            t = max(t_k, t_p);
+            sum_s = 0.f;
+            for (int k = k0; k < k1; ++k) {
+                const float z = tempered(lg[k], sp.T);
+                if (fkey(z) >= t) sum_s += expf(z - m);
+            }
+            sum_s = warp_sum(sum_s);
+        }
         float part = 0.f;
         int last = -1;
         for (int k = k0; k < k1; ++k) {
-            const float pk = expf(lg[k] - m) / sum;
+            const float z = tempered(lg[k], sp.T);
+            if (fkey(z) < t) continue;
+            const float pk = expf(z - m) / sum_s;
             part += pk;
             if (pk > 0.f) last = k;
         }
@@ -325,27 +405,53 @@ __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act 
         const float uu = u[((long long)b * H + i) * W + j];
         int hit = -1;
         for (int k = k0; k < k1; ++k) {
-            cdf += expf(lg[k] - m) / sum;
+            const float z = tempered(lg[k], sp.T);
+            if (fkey(z) < t) continue;
+            cdf += expf(z - m) / sum_s;
             if (uu < cdf) { hit = k; break; }
         }
         const unsigned found = __ballot_sync(0xffffffffu, hit >= 0);
         int code;
         if (found) {
             code = __shfl_sync(0xffffffffu, hit, __ffs(found) - 1);
-        } else {                    // u above the rounded total: the last code with non-zero probability
+        } else {                    // u above the rounded total: the last kept code with non-zero probability
             for (int o = 16; o; o >>= 1) last = max(last, __shfl_xor_sync(0xffffffffu, last, o));
             code = last < 0 ? K - 1 : last;
         }
         if (lane == 0) codes[((long long)b * H + i) * W + j] = code;
+        if (sp.log_prob) {          // log p_model(code): the raw logits' softmax, the draw's max and sum when T = 1
+            float ml = m, suml = sum;
+            if (sp.T != 1.f) {
+                ml = -INFINITY;
+                for (int k = k0; k < k1; ++k) ml = fmaxf(ml, lg[k]);
+                ml = warp_max(ml);
+                suml = 0.f;
+                for (int k = k0; k < k1; ++k) suml += expf(lg[k] - ml);
+                suml = warp_sum(suml);
+            }
+            if (lane == 0) {        // compensated fp32 sum in raster order: 4096 near-equal terms stay accurate
+                const float lp = (lg[code] - ml) - logf(suml);
+                if (first) {
+                    sp.log_prob[b] = lp;
+                    sp.log_c[b] = 0.f;
+                } else {
+                    const float acc = sp.log_prob[b], y = lp - sp.log_c[b], t = acc + y;
+                    sp.log_c[b] = (t - acc) - y;
+                    sp.log_prob[b] = t;
+                }
+            }
+        }
         float *x = x0.at(b, i, j, W);
         for (int c = lane; c < n.C; c += 32) x[c] = __ldg(n.emb + (long long)code * n.C + c);
     }
 }
 
 // Completion's given prefix: codes[b, p] = given[b, p] as given and x0[b, p] = E[clamp(given[b, p])] (embed_kernel's
-// clamp) for the raster positions p < n of every image; positions >= n are not read.
+// clamp) for the raster positions p < n of every image; positions >= n are not read.  zero: nullptr, or the (B)
+// log_prob of a call that samples nothing (n = HW), set to 0 here since no step writes it.
 __global__ void given_kernel(const long long *__restrict__ given, const float *__restrict__ E, int B, long long HW,
-                             long long n, int K, int C, float *__restrict__ x0, long long *__restrict__ codes) {
+                             long long n, int K, int C, float *__restrict__ x0, long long *__restrict__ codes,
+                             float *__restrict__ zero) {
     const long long total = (long long)B * n * C;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const long long q = i / C, pos = q / n * HW + q % n;
@@ -354,6 +460,9 @@ __global__ void given_kernel(const long long *__restrict__ given, const float *_
         x0[pos * C + c] = __ldg(E + (long long)clampi(code, K) * C + c);
         if (c == 0) codes[pos] = code;
     }
+    if (zero)
+        for (long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (long long)gridDim.x * blockDim.x)
+            zero[b] = 0.f;
 }
 
 // the kept-tap packing of pack_prior_at
@@ -416,9 +525,9 @@ unsigned blocks(long long positions, int P) { return (unsigned)((positions + P -
 // i0 .. H-1 as generate runs them: per row one vertical pass per layer, then one step per position.  In row i0 with
 // j0 > 0, one horizontal launch per layer over columns [0, j0) first fills the one-row x[l] that the step at (i0, j0)
 // reads.  Every value is the fmaf chain generate computes at that position, so the logits are bitwise generate's.
-// Launches: L*[i0 > 0] + L*(H - i0) + L*[j0 > 0] + (H*W - n_given).
+// Launches: L*[i0 > 0] + L*(H - i0) + L*[j0 > 0] + (H*W - n_given).  sp: the draw's knobs, the same for every step.
 void sample_from(const Net &n, const long long *lab, const float *u, int B, int H, int W, long long n_given,
-                 long long *codes, float *step_logits, float *ws, cudaStream_t s) {
+                 const Samp &sp, long long *codes, float *step_logits, float *ws, cudaStream_t s) {
     const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
     const int i0 = (int)(n_given / W), j0 = (int)(n_given % W);
     int reach = 1;
@@ -454,11 +563,39 @@ void sample_from(const Net &n, const long long *lab, const float *u, int B, int 
             float *lg = step_logits ? step_logits + ((long long)i * W + j) * n.K : ws + wl.gen_lg;
             const long long img = step_logits ? (long long)H * W * n.K : n.K;
             step_kernel<PS><<<blocks(B, PS), NT, 0, s>>>(n, x0, x(0), vh(0), vh_stride, x_stride, lab, u, B, H, W, i,
-                                                         j, lg, img, codes);
+                                                         j, lg, img, codes, sp, (long long)i * W + j == n_given);
         }
         launches += W - jstart;
     }
     VQB_COUNT_LAUNCH(launches);
+}
+
+// generate's, complete's and sample's body after their argument checks: the given prefix (n_given > 0), then the
+// sampler from n_given on.
+void sample_call(const Net &n, const int64_t *labels, const float *u, const int64_t *given, long long n_given, int B,
+                 int H, int W, const Samp &sp, int64_t *codes, float *step_logits, void *workspace, cudaStream_t s) {
+    const long long HW = (long long)H * W;
+    float *ws = static_cast<float *>(workspace);
+    long long *out = reinterpret_cast<long long *>(codes);
+    if (n_given > 0) {
+        given_kernel<<<grid_for((long long)B * n_given * n.C), NT, 0, s>>>(
+            reinterpret_cast<const long long *>(given), n.emb, B, HW, n_given, n.K, n.C,
+            ws + ws_layout(B, H, W, n.C, n.L, n.K).gen_x0, out, n_given == HW ? sp.log_prob : nullptr);
+        VQB_COUNT_LAUNCH(1);
+    }
+    if (n_given < HW)
+        sample_from(n, reinterpret_cast<const long long *>(labels), u, B, H, W, n_given, sp, out, step_logits, ws, s);
+}
+
+// Floats of the sampler's regions from raster position n_given: a prefix shorter than a row keeps generate's rings,
+// a longer one every layer's vertical output as a whole grid.  The kept-set search's scratch follows them.
+long long ring_floats(const Ws &w, long long W, long long n_given) { return n_given < W ? w.gen_total : w.comp_total; }
+
+// bytes a sampler call from n_given needs: generate's workspace at least, so one buffer also serves the forward
+size_t sampler_bytes(int B, int H, int W, int dim, int n_layers, int K, long long n_given, bool search) {
+    const size_t base = vqb_prior_workspace_bytes(B, H, W, dim, n_layers, K);
+    const long long f = ring_floats(ws_layout(B, H, W, dim, n_layers, K), W, n_given) + (search ? search_floats(B, K) : 0);
+    return (size_t)f * sizeof(float) > base ? (size_t)f * sizeof(float) : base;
 }
 
 }  // namespace
@@ -546,8 +683,7 @@ extern "C" int vqb_prior_generate_f32(const vqb_prior_net *net, const int64_t *l
     if (workspace_bytes < vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
     // Layer 0 must read only codes before (i, j): mask B reads row i and column j, a residual adds x_h at (i, j).
     if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
-    sample_from(n, reinterpret_cast<const long long *>(labels), u, B, H, W, 0, reinterpret_cast<long long *>(codes),
-                step_logits, static_cast<float *>(workspace), (cudaStream_t)stream);
+    sample_call(n, labels, u, nullptr, 0, B, H, W, Samp{}, codes, step_logits, workspace, (cudaStream_t)stream);
     return vqb_cuda_status(cudaGetLastError());
 }
 
@@ -567,22 +703,41 @@ extern "C" int vqb_prior_complete_f32(const vqb_prior_net *net, const int64_t *l
     if (!labels || !u || !given || !codes || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
     const long long HW = (long long)H * W;
     if (n_given < 0 || n_given > HW) return VQB_ERR_BAD_ARG;
-    // a prefix shorter than a row keeps generate's rings (and its workspace); a longer one whole grids
-    const size_t need = n_given < W ? vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)
-                                    : vqb_prior_complete_workspace_bytes(B, H, W, n.C, n.L, n.K);
-    if (workspace_bytes < need) return VQB_ERR_WORKSPACE;
+    if (workspace_bytes < sampler_bytes(B, H, W, n.C, n.L, n.K, n_given, false)) return VQB_ERR_WORKSPACE;
     if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
-    cudaStream_t s = (cudaStream_t)stream;
-    float *ws = static_cast<float *>(workspace);
-    long long *out = reinterpret_cast<long long *>(codes);
-    if (n_given > 0) {
-        float *x0 = ws + ws_layout(B, H, W, n.C, n.L, n.K).gen_x0;
-        given_kernel<<<grid_for((long long)B * n_given * n.C), NT, 0, s>>>(
-            reinterpret_cast<const long long *>(given), net->embedding, B, HW, n_given, n.K, n.C, x0, out);
-        VQB_COUNT_LAUNCH(1);
+    sample_call(n, labels, u, given, n_given, B, H, W, Samp{}, codes, step_logits, workspace, (cudaStream_t)stream);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_prior_sample_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K,
+                                                   int64_t n_given) {
+    if (!vqb_prior_workspace_bytes(B, H, W, dim, n_layers, K) || n_given < 0 || n_given > (long long)H * W) return 0;
+    return sampler_bytes(B, H, W, dim, n_layers, K, n_given, true);
+}
+
+extern "C" int vqb_prior_sample_f32(const vqb_prior_net *net, const int64_t *labels, const float *u,
+                                    const int64_t *given, int64_t n_given, int B, int H, int W,
+                                    const vqb_prior_sampling *sampling, int64_t *codes, float *log_prob,
+                                    float *step_logits, void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!labels || !u || !codes || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (n_given < 0 || n_given > (long long)H * W || (n_given > 0 && !given)) return VQB_ERR_BAD_ARG;
+    Samp sp;
+    if (sampling) {
+        sp.T = sampling->temperature;
+        sp.top_k = sampling->top_k;
+        sp.top_p = sampling->top_p;
     }
-    if (n_given < HW)
-        sample_from(n, reinterpret_cast<const long long *>(labels), u, B, H, W, n_given, out, step_logits, ws, s);
+    if (!(sp.T > 0.f && sp.T <= FLT_MAX) || sp.top_k < 0 || sp.top_k > n.K || !(sp.top_p > 0.f && sp.top_p <= 1.f))
+        return VQB_ERR_BAD_ARG;
+    if (workspace_bytes < vqb_prior_sample_workspace_bytes(B, H, W, n.C, n.L, n.K, n_given)) return VQB_ERR_WORKSPACE;
+    if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
+    sp.scratch = static_cast<float *>(workspace) + ring_floats(ws_layout(B, H, W, n.C, n.L, n.K), W, n_given);
+    sp.log_prob = log_prob;
+    sp.log_c = sp.scratch + search_floats(B, n.K) - B;
+    sample_call(n, labels, u, given, n_given, B, H, W, sp, codes, step_logits, workspace, (cudaStream_t)stream);
     return vqb_cuda_status(cudaGetLastError());
 }
 

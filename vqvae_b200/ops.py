@@ -500,8 +500,8 @@ def prior_layer_backward(layer_w, x_v, x_h, labels, d_out_v, d_out_h, saved, gra
     return d_x_v, d_x_h
 
 
-def _prior_workspace(net, B, H, W, dev, size=None):
-    n = (size or lib().vqb_prior_workspace_bytes)(B, H, W, net.dim, net.n_layers, net.input_dim)
+def _prior_workspace(net, B, H, W, dev, size=None, *extra):
+    n = (size or lib().vqb_prior_workspace_bytes)(B, H, W, net.dim, net.n_layers, net.input_dim, *extra)
     if n == 0:
         raise RuntimeError("prior: bad sizes")
     return torch.empty((n,), dtype=torch.uint8, device=dev)
@@ -555,7 +555,7 @@ def prior_complete(net, labels, u, given, n_given, step_logits=None):
     B, H, W = u.shape
     dev = u.device
     codes = torch.empty((B, H, W), dtype=torch.int64, device=dev)
-    ws = _prior_workspace(net, B, H, W, dev, None if n_given < W else lib().vqb_prior_complete_workspace_bytes)
+    ws = _prior_workspace(net, B, H, W, dev, lib().vqb_prior_sample_workspace_bytes, n_given)
     span = _Span(f"prior complete K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W} n_given={n_given}")
     check(lib().vqb_prior_complete_f32(_lib.C.byref(net), labels.data_ptr(), u.data_ptr(), given.data_ptr(), n_given,
                                        B, H, W, codes.data_ptr(),
@@ -563,6 +563,26 @@ def prior_complete(net, labels, u, given, n_given, step_logits=None):
                                        ws.numel(), _stream()), "prior_complete")
     span.done()
     return codes
+
+
+def prior_sample(net, labels, u, given, n_given, sampling, step_logits=None):
+    """prior_complete drawing from the tempered, truncated softmax that `sampling` (a PriorSampling struct) sets
+    (vqb_prior_sample_f32) -> (codes (B,H,W) int64, log_prob (B,) fp32: the model's log-probability of the sampled
+    positions).  given: None when n_given = 0."""
+    B, H, W = u.shape
+    dev = u.device
+    codes = torch.empty((B, H, W), dtype=torch.int64, device=dev)
+    log_prob = torch.empty((B,), dtype=torch.float32, device=dev)
+    ws = _prior_workspace(net, B, H, W, dev, lib().vqb_prior_sample_workspace_bytes, n_given)
+    span = _Span(f"prior sample K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W} n_given={n_given} "
+                 f"T={sampling.temperature:g} top_k={sampling.top_k} top_p={sampling.top_p:g}")
+    check(lib().vqb_prior_sample_f32(_lib.C.byref(net), labels.data_ptr(), u.data_ptr(),
+                                     given.data_ptr() if given is not None else None, n_given, B, H, W,
+                                     _lib.C.byref(sampling), codes.data_ptr(), log_prob.data_ptr(),
+                                     step_logits.data_ptr() if step_logits is not None else None, ws.data_ptr(),
+                                     ws.numel(), _stream()), "prior_sample")
+    span.done()
+    return codes, log_prob
 
 
 def prior_forward_train(net, codes, labels, precision="fp32"):

@@ -12,9 +12,10 @@ requires grad (``_PriorFunction``: the training forward keeps its activations, a
 ``torch.no_grad()`` it is the inference forward.  ``GatedPixelCNN.precision`` (a plain attribute, not in the state
 dict) selects the arithmetic of ``forward``, inference and training alike: "fp32" (the default, CUDA cores) or
 "tf32" (every matrix product on the wgmma TF32 GEMM, operands rounded to TF32, fp32 accumulation; the one-hot
-embedding-gradient sums stay fp32).  ``generate``, ``complete``, ``GatedMaskedConv2d`` and ``GatedActivation`` stay
-fp32 in both modes, and ``set_precision`` does not affect the prior.  ``GatedMaskedConv2d`` and ``GatedActivation``
-called on their own are differentiable too, under the same rule (grad enabled and an input or a parameter requiring grad):
+embedding-gradient sums stay fp32).  ``generate``, ``complete``, ``sample``, ``sample_completion``,
+``GatedMaskedConv2d`` and ``GatedActivation`` stay fp32 in both modes, and ``set_precision`` does not affect the
+prior.  ``GatedMaskedConv2d`` and ``GatedActivation`` called on their own are differentiable too, under the same rule
+(grad enabled and an input or a parameter requiring grad):
 ``_GatedLayerFunction`` runs the layer's training forward and single-layer backward (vqb_prior_layer_*_f32),
 ``_GateFunction`` the gate and its backward.  Their outputs are bitwise the inference call's.
 
@@ -33,13 +34,15 @@ Reference behaviour kept on purpose:
       residual: anything else reads the code being drawn, so the reference's one-forward-per-position loop is not
       causal in raster order there, and the sampler refuses it (C ABI: VQB_ERR_UNSUPPORTED)
 """
+import math
+import numbers
 import operator
 
 import torch
 import torch.nn as nn
 
 from . import ops
-from ._lib import PRIOR_MAX_KERNEL, C, PriorGrads, PriorLayerGrads, PriorLayerWeights, PriorNet
+from ._lib import PRIOR_MAX_KERNEL, C, PriorGrads, PriorLayerGrads, PriorLayerWeights, PriorNet, PriorSampling
 from .modules import _packed, _packed_current
 
 HIDDEN = 512          # output_conv's hidden width
@@ -408,3 +411,84 @@ class GatedPixelCNN(nn.Module):
         ops._require_cuda(x, "GatedPixelCNN.complete codes")
         u = torch.rand(tuple(x.shape), device=x.device)
         return self._complete(label, u, x, n_given)
+
+    def _knobs(self, temperature, top_k, top_p, what):
+        """The sampling knobs' checks (ValueError), as the C ABI sees them (fp32 temperature and top_p) ->
+        PriorSampling; top_k None is 0 and top_p None is 1 (off)."""
+        K = self.embedding.num_embeddings
+        if isinstance(temperature, bool) or not isinstance(temperature, numbers.Real):
+            raise ValueError(f"{what}: temperature must be a real number, got {temperature!r}")
+        t32 = C.c_float(temperature).value
+        if not (math.isfinite(t32) and t32 > 0):
+            raise ValueError(f"{what}: temperature must be finite and > 0 in fp32, got {temperature!r}")
+        if top_k is not None and (isinstance(top_k, bool) or not isinstance(top_k, numbers.Integral)
+                                  or not 1 <= top_k <= K):
+            raise ValueError(f"{what}: top_k must be None or an int in [1, {K}], got {top_k!r}")
+        if top_p is not None:
+            if isinstance(top_p, bool) or not isinstance(top_p, numbers.Real):
+                raise ValueError(f"{what}: top_p must be None or a float in (0, 1], got {top_p!r}")
+            p32 = C.c_float(top_p).value
+            if not (0 < p32 <= 1 and 0 < top_p <= 1):
+                raise ValueError(f"{what}: top_p must be None or a float in (0, 1] (fp32), got {top_p!r}")
+        return PriorSampling(temperature=t32, top_k=0 if top_k is None else int(top_k),
+                             top_p=1.0 if top_p is None else C.c_float(top_p).value)
+
+    def _sample_with(self, label, u, x, n_given, temperature, top_k, top_p, step_logits=None):
+        """sample() / sample_completion() with given uniforms u (B,H,W) fp32 -> (codes, log_prob).  x: the codes
+        whose first n_given raster positions are kept (None with n_given = 0).  step_logits: None or (B,H,W,K) fp32,
+        the raw logits of every sampled step.  fp32 whatever ``precision`` says."""
+        what = "GatedPixelCNN.sample" if x is None else "GatedPixelCNN.sample_completion"
+        if x is None:
+            if u.dim() != 3:
+                raise RuntimeError(f"{what}: expected uniforms of shape (B,H,W), got {tuple(u.shape)}")
+            if n_given != 0:
+                raise ValueError(f"{what}: n_given must be 0 without codes, got {n_given!r}")
+            B, H, W = u.shape
+            _square(H, W, what)
+            self._check_causal(what)
+        else:
+            n_given = self._given(x, label, n_given)
+            B, H, W = x.shape
+            if tuple(u.shape) != (B, H, W):
+                raise RuntimeError(f"{what}: uniforms of shape {tuple(u.shape)} for codes {(B, H, W)}")
+        sampling = self._knobs(temperature, top_k, top_p, what)
+        if x is not None:
+            ops._require_cuda(x, what + " codes")
+        ops._require_cuda(u, what + " uniforms")
+        label = _labels(label, B, u.device, what)
+        if x is not None:
+            x = x.detach().to(torch.int64).contiguous()
+            if n_given == H * W:            # nothing to sample: no packing, no launch
+                return x.clone(), torch.zeros((B,), dtype=torch.float32, device=x.device)
+        keep = []
+        return ops.prior_sample(self._net(keep), label, _f32(u), x, n_given, sampling, step_logits)
+
+    def sample(self, label, shape=(8, 8), batch_size=64, *, temperature=1.0, top_k=None, top_p=None):
+        """generate() with control over the draw -> (codes (batch_size, H, W) int64, log_prob (batch_size,) fp32).
+        Each code is drawn from the softmax of that step's logits divided by `temperature`, restricted to the top_k
+        codes (ties at the threshold kept) and to the smallest top set holding top_p of the tempered probability
+        (nucleus sampling), then renormalized; None turns a truncation off.  log_prob is the sum over the grid of the
+        model's own log-probability of each sampled code (untempered, untruncated softmax), for ranking samples.
+        Draws exactly one torch.rand((batch_size, H, W)), so with the default knobs and the same seed the codes are
+        generate()'s.  ValueError for a knob out of range; the other restrictions are generate()'s (square grids,
+        P5, fp32, one set of knobs for the batch)."""
+        H, W = shape
+        what = "GatedPixelCNN.sample"
+        _square(H, W, what)
+        self._check_causal(what)
+        self._knobs(temperature, top_k, top_p, what)
+        dev = next(self.parameters()).device
+        ops._require_cuda(torch.empty(0, device=dev), "GatedPixelCNN parameters")
+        u = torch.rand((batch_size, H, W), device=dev)
+        return self._sample_with(label, u, None, 0, temperature, top_k, top_p)
+
+    def sample_completion(self, x, label, n_given, *, temperature=1.0, top_k=None, top_p=None):
+        """complete() with sample()'s knobs -> (codes (B,H,W) int64, log_prob (B,) fp32).  log_prob sums the
+        model's log-probability over the sampled positions only (0 when n_given = H*W).  Draws exactly one
+        torch.rand((B, H, W)), so with the default knobs and the same seed the codes are complete()'s."""
+        what = "GatedPixelCNN.sample_completion"
+        n_given = self._given(x, label, n_given)
+        self._knobs(temperature, top_k, top_p, what)
+        ops._require_cuda(x, what + " codes")
+        u = torch.rand(tuple(x.shape), device=x.device)
+        return self._sample_with(label, u, x, n_given, temperature, top_k, top_p)
