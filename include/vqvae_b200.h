@@ -497,6 +497,33 @@ int vqb_prior_backward_tf32(const vqb_prior_net *net, const int64_t *codes, cons
                             const float *d_logits, const void *saved, const vqb_prior_grads *grads, void *workspace,
                             size_t workspace_bytes, void *stream);
 
+/* ---- Gated PixelCNN prior: log-likelihood of given code grids (fp32 and TF32) -----------------------------------
+ * With l = the logits vqb_prior_forward_f32 (or _tf32) computes on codes and labels, and c = codes clamped to
+ * [0, input_dim - 1], the term of position p = i*W + j of image b is
+ *   lp[b, p] = (l_c - M) - logf(S),  M = max_k l_k,  S = sum_k expf(l_k - M)      (l at b, p; a fixed-order sum)
+ * The logits are never written to memory: the layers are the forward's launches (bitwise the same activations), the
+ * head's logits, bitwise the forward's, are reduced on chip to a running (M, S, l_c) per position, and one finish
+ * launch combines them.  pos_log_prob: NULL or (B, H, W) fp32 receiving every lp; log_prob: NULL or (B) fp32
+ * receiving, per image, the compensated (Kahan) fp32 sum of lp over p >= n_given in raster order (0 when
+ * n_given = H*W), vqb_prior_sample_f32's sum.  At least one of them non-NULL, n_given in [0, H*W]: VQB_ERR_BAD_ARG
+ * otherwise.  Shape limits and the other checks are vqb_prior_forward_*'s; any layer 0 is taken (with a layer 0 that
+ * reads the code it scores, the sum is the reference's cross-entropy, not a likelihood).  Deterministic (no float
+ * atomics; two calls are bitwise equal), no host synchronisation.
+ * Launches: fp32 3 + 2*n_layers (embedding, two per layer, head, finish); TF32 4 + 4*n_layers (embedding, four per
+ * layer, the hidden layer, head, finish).                                                                         */
+/* vqb_prior_workspace_bytes + 12*B*H*W bytes (0 = bad sizes).                                                      */
+size_t vqb_prior_log_prob_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K);
+/* vqb_prior_workspace_bytes_tf32 + 12*B*H*W*splits bytes (0 = bad sizes): the TF32 head splits the K codes over
+ * `splits` CTAs per 128 positions, from the shape only.  With T = ceil(K / BN) tiles of BN = (K <= 64 ? 64 : 128)
+ * codes and s = min(T, max(1, ceil(264 / ceil(B*H*W / 128)))): splits = ceil(T / ceil(T / s)).                   */
+size_t vqb_prior_log_prob_workspace_bytes_tf32(int B, int H, int W, int dim, int n_layers, int K);
+int vqb_prior_log_prob_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int64_t n_given,
+                           int B, int H, int W, float *log_prob, float *pos_log_prob, void *workspace,
+                           size_t workspace_bytes, void *stream);
+int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int64_t n_given,
+                            int B, int H, int W, float *log_prob, float *pos_log_prob, void *workspace,
+                            size_t workspace_bytes, void *stream);
+
 /* ---- optimizer step on device: Adam over many tensors, then every weight packing refreshed --------------------
  * One training step's update of a parameter group is two calls, each normally ONE launch: vqb_adam_multi_f32 updates
  * every parameter and its moments, then vqb_repack_multi rebuilds every packing read from those parameters and

@@ -180,12 +180,45 @@ __device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, co
     }
 }
 
-// output_conv (models.py:107-111): logits = W2 . relu(W1 . x_h + b1) + b2 at the P positions of the block.
-// Logit k of slot p goes to out[p] + k * kstride.  keep.p != nullptr (the training forward) also stores the hidden
-// layer there.
+// Where head_positions sends logit k of slot p: sink(p, k, value), each (p, k) once, by thread k % NT, in increasing
+// k per thread.  ToHbm stores it at out[p] + k * kstride (the forward's and the sampler's logits); Lse reduces it.
 template <int P>
-__device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, float *const (&out)[P], long long kstride,
-                               int H, int W, const Act &keep) {
+struct ToHbm {
+    float *const *out;
+    long long kstride;
+    __device__ __forceinline__ void operator()(int p, int k, float v) const { out[p][k * kstride] = v; }
+};
+
+// A running log-sum-exp per slot over the logits this thread sees, and the logit of the slot's target code (the
+// thread that sees it stores it in t[p], shared memory)
+template <int P>
+struct Lse {
+    float m[P], s[P];
+    int tgt[P];
+    float *t;
+    __device__ __forceinline__ void operator()(int p, int k, float v) {
+        if (v > m[p]) {
+            s[p] = s[p] * expf(m[p] - v) + 1.f;
+            m[p] = v;
+        } else {
+            s[p] += expf(v - m[p]);
+        }
+        if (k == tgt[p]) t[p] = v;
+    }
+};
+
+// (m, s) <- the log-sum-exp pair of the union of (m, s) and (m2, s2); an empty pair (-INFINITY, 0) changes nothing
+__device__ __forceinline__ void lse_merge(float &m, float &s, float m2, float s2) {
+    const float M = fmaxf(m, m2);
+    if (M == -INFINITY) return;
+    s = s * expf(m - M) + s2 * expf(m2 - M);
+    m = M;
+}
+
+// output_conv (models.py:107-111): logits = W2 . relu(W1 . x_h + b1) + b2 at the P positions of the block, each
+// handed to `sink`.  keep.p != nullptr (the training forward) also stores the hidden layer there.
+template <int P, class Sink>
+__device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, Sink &sink, int H, int W, const Act &keep) {
     const int C = n.C, tid = threadIdx.x;
     __syncthreads();
     load_tap(s, in, 0, 0, H, W);
@@ -211,7 +244,7 @@ __device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, float *c
         if (k < n.K)
 #pragma unroll
             for (int p = 0; p < P; ++p)
-                if (s.b[p] >= 0) out[p][k * kstride] = acc[0][p] + __ldg(n.b2 + k);
+                if (s.b[p] >= 0) sink(p, k, acc[0][p] + __ldg(n.b2 + k));
     }
 }
 
@@ -266,7 +299,53 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
         const int p = threadIdx.x;
         out[p] = s.b[p] >= 0 ? logits + (long long)s.b[p] * n.K * H * W + (long long)s.r[p] * W + s.c[p] : nullptr;
     }
-    head_positions(s, n, in, out, (long long)H * W, H, W, keep);
+    ToHbm<P> sink{out, (long long)H * W};
+    head_positions(s, n, in, sink, H, W, keep);
+}
+
+// head_kernel's logits reduced on chip: each position's one partial (M, S, l_t) (prior.cuh) over all K codes, its
+// target the clamped code codes[b, i, j].  A block owns all K logits of its P positions: each thread keeps a running
+// log-sum-exp per slot over its codes k = tid (mod NT), then the warps' pairs are merged by xor butterflies and the
+// eight warps' in warp order.
+template <int P>
+__global__ void __launch_bounds__(NT) lse_head_kernel(Net n, Act in, const long long *labels, const long long *codes,
+                                                      int B, int H, int W, float *part) {
+    __shared__ __align__(16) Smem<P> s;
+    __shared__ float t[P], wm[NT / 32][P], wsum[NT / 32][P];
+    set_slots(s, B, 0, H, 0, W, labels, n.NC);
+    Lse<P> sink;
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        sink.m[p] = -INFINITY;
+        sink.s[p] = 0.f;
+        sink.tgt[p] = s.b[p] >= 0 ? clampi(codes[((long long)s.b[p] * H + s.r[p]) * W + s.c[p]], n.K) : -1;
+    }
+    sink.t = t;
+    head_positions(s, n, in, sink, H, W, Act{});
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        float m = sink.m[p], sm = sink.s[p];
+        for (int o = 16; o; o >>= 1) {
+            const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, sm, o);
+            lse_merge(m, sm, m2, s2);
+        }
+        if (lane == 0) {
+            wm[warp][p] = m;
+            wsum[warp][p] = sm;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < P) {
+        const int p = threadIdx.x;
+        if (s.b[p] < 0) return;
+        float m = wm[0][p], sm = wsum[0][p];
+        for (int w = 1; w < NT / 32; ++w) lse_merge(m, sm, wm[w][p], wsum[w][p]);
+        float *q = part + (((long long)s.b[p] * H + s.r[p]) * W + s.c[p]) * 3;
+        q[0] = m;
+        q[1] = sm;
+        q[2] = t[p];
+    }
 }
 
 // The draw's knobs (vqb_prior_sampling, checked by the entry point) and its extra outputs.  Samp{} is generate's draw
@@ -331,7 +410,8 @@ __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act 
         horiz_positions(s, n.layer[l], in, vh, o, H, W, Act{});
         __syncthreads();
     }
-    head_positions(s, n, Act{xrow0.p + (n.L - 1) * x_stride, 1, n.C}, out, 1, H, W, Act{});
+    ToHbm<P> sink{out, 1};
+    head_positions(s, n, Act{xrow0.p + (n.L - 1) * x_stride, 1, n.C}, sink, H, W, Act{});
     __syncthreads();
     // softmax + inverse CDF, one warp per image: lane L owns logits [L*cs, L*cs + cs).  z = l / T; the kept set is
     // S = {k : fkey(z_k) >= t} (t = 0: every code); the CDF is the fp32 running sum of q_k = expf(z_k - max) / sum_S
@@ -643,6 +723,31 @@ extern "C" int vqb_prior_layer_f32(const vqb_prior_layer_weights *layer, const f
     return vqb_cuda_status(cudaGetLastError());
 }
 
+namespace {
+
+// The teacher-forced forward up to the head, in the workspace's ping-pong grids: the embedding, then per layer the
+// vertical and the horizontal stack over every position.  Returns x_h of the last layer.  1 + 2*L launches.
+Act forward_layers(const Net &n, const long long *codes, const long long *lab, int B, int H, int W, float *ws,
+                   cudaStream_t s) {
+    const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
+    const long long npos = (long long)B * H * W, grid = npos * n.C;
+    Act x0{ws, H, n.C}, vh{ws + wl.fwd_vh, H, 2 * n.C};
+    Act v[2] = {{ws + wl.fwd_v, H, n.C}, {ws + wl.fwd_v + grid, H, n.C}};
+    Act x[2] = {{ws + wl.fwd_x, H, n.C}, {ws + wl.fwd_x + grid, H, n.C}};
+    embed_kernel<<<grid_for(grid), NT, 0, s>>>(codes, n.emb, npos, n.K, n.C, x0.p);
+    for (int l = 0; l < n.L; ++l) {
+        const Act vin = l == 0 ? x0 : v[(l - 1) & 1], xin = l == 0 ? x0 : x[(l - 1) & 1];
+        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H,
+                                                        Act{});
+        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W, 0, H, 0,
+                                                         W, Act{});
+    }
+    VQB_COUNT_LAUNCH(1 + 2 * n.L);
+    return x[(n.L - 1) & 1];
+}
+
+}  // namespace
+
 extern "C" int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
                                      int H, int W, float *logits, void *workspace, size_t workspace_bytes,
                                      void *stream) {
@@ -653,23 +758,36 @@ extern "C" int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *co
     if (workspace_bytes < vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
     cudaStream_t s = (cudaStream_t)stream;
     const long long *lab = reinterpret_cast<const long long *>(labels);
-    const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
+    const Act xL = forward_layers(n, reinterpret_cast<const long long *>(codes), lab, B, H, W,
+                                  static_cast<float *>(workspace), s);
+    head_kernel<PF><<<blocks((long long)B * H * W, PF), NT, 0, s>>>(n, xL, lab, B, H, W, logits, Act{});
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_prior_log_prob_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K) {
+    const size_t base = vqb_prior_workspace_bytes(B, H, W, dim, n_layers, K);
+    if (!base) return 0;
+    return base + (size_t)B * H * W * 3 * sizeof(float);
+}
+
+// The forward's layer walk, then lse_head_kernel in place of head_kernel (the same logits, reduced on chip: one
+// partial per position, after the forward's workspace) and the finish.  3 + 2*n_layers launches.
+extern "C" int vqb_prior_log_prob_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                      int64_t n_given, int B, int H, int W, float *log_prob, float *pos_log_prob,
+                                      void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = log_prob_args(net, n, codes, labels, n_given, B, H, W, log_prob, pos_log_prob, workspace);
+    if (st) return st;
+    if (workspace_bytes < vqb_prior_log_prob_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *lab = reinterpret_cast<const long long *>(labels), *cd = reinterpret_cast<const long long *>(codes);
     float *ws = static_cast<float *>(workspace);
-    const long long npos = (long long)B * H * W, grid = npos * n.C;
-    Act x0{ws, H, n.C}, vh{ws + wl.fwd_vh, H, 2 * n.C};
-    Act v[2] = {{ws + wl.fwd_v, H, n.C}, {ws + wl.fwd_v + grid, H, n.C}};
-    Act x[2] = {{ws + wl.fwd_x, H, n.C}, {ws + wl.fwd_x + grid, H, n.C}};
-    embed_kernel<<<grid_for(grid), NT, 0, s>>>(reinterpret_cast<const long long *>(codes), net->embedding, npos, n.K,
-                                               n.C, x0.p);
-    for (int l = 0; l < n.L; ++l) {
-        const Act vin = l == 0 ? x0 : v[(l - 1) & 1], xin = l == 0 ? x0 : x[(l - 1) & 1];
-        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H,
-                                                        Act{});
-        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W, 0, H, 0,
-                                                         W, Act{});
-    }
-    head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, x[(n.L - 1) & 1], lab, B, H, W, logits, Act{});
-    VQB_COUNT_LAUNCH(2 + 2 * n.L);
+    float *part = ws + vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K) / sizeof(float);
+    const Act xL = forward_layers(n, cd, lab, B, H, W, ws, s);
+    lse_head_kernel<PF><<<blocks((long long)B * H * W, PF), NT, 0, s>>>(n, xL, lab, cd, B, H, W, part);
+    log_prob_finish_kernel<<<B, NT, 0, s>>>(part, 1, (long long)H * W, n_given, log_prob, pos_log_prob);
+    VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());
 }
 

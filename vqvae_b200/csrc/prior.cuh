@@ -63,6 +63,66 @@ inline int net_from(const vqb_prior_net *net, Net &n) {
     return 0;
 }
 
+// ---- log_prob (vqb_prior_log_prob_*): what both precisions' heads hand to one finish launch ----------------------
+// The head of either precision reduces each position's logits, N range by N range, to one partial (M, S, l_t):
+// M the range's largest logit, S the sum of expf(l - M) over the range, l_t the logit of the position's clamped code
+// (-INFINITY when the code lies outside the range).  Partials of position g (g = (b*H + i)*W + j) are
+// part[(g*splits + z)*3 + {0, 1, 2}] for ranges z = 0 .. splits-1.
+
+// lp = (l_t - M) - logf(S) with M = max_z M_z, S = sum over z in order of S_z * expf(M_z - M), l_t = max_z l_t_z
+__device__ __forceinline__ float lp_of(const float *q, int splits) {
+    float M = -INFINITY, lt = -INFINITY;
+    for (int z = 0; z < splits; ++z) {
+        M = fmaxf(M, q[3 * z]);
+        lt = fmaxf(lt, q[3 * z + 2]);
+    }
+    float S = 0.f;
+    for (int z = 0; z < splits; ++z) S += q[3 * z + 1] * expf(q[3 * z] - M);
+    return (lt - M) - logf(S);
+}
+
+// One block per image: every position's lp into pos (if non-null), and into log_prob[b] (if non-null) the
+// compensated fp32 sum of lp over the raster positions p >= n_given, in raster order, with the sampler's Kahan step
+// (prior.cu: step_kernel), so 4096 near-equal terms stay accurate and the result does not depend on the launch.
+__global__ void __launch_bounds__(NT) log_prob_finish_kernel(const float *__restrict__ part, int splits, long long HW,
+                                                              long long n_given, float *__restrict__ log_prob,
+                                                              float *__restrict__ pos) {
+    __shared__ float lp[NT];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    float acc = 0.f, comp = 0.f;
+    for (long long p0 = 0; p0 < HW; p0 += NT) {
+        const long long p = p0 + tid;
+        if (p < HW) {
+            const float v = lp_of(part + ((long long)b * HW + p) * splits * 3, splits);
+            lp[tid] = v;
+            if (pos) pos[(long long)b * HW + p] = v;
+        }
+        __syncthreads();
+        if (tid == 0 && log_prob) {
+            const int n = (int)(HW - p0 < NT ? HW - p0 : NT);
+            for (int q = 0; q < n; ++q) {
+                if (p0 + q < n_given) continue;
+                const float y = lp[q] - comp, t = acc + y;
+                comp = (t - acc) - y;
+                acc = t;
+            }
+        }
+        __syncthreads();
+    }
+    if (tid == 0 && log_prob) log_prob[b] = acc;
+}
+
+// The C entry points' checks shared by both precisions, in their order; fills n.
+inline int log_prob_args(const vqb_prior_net *net, Net &n, const int64_t *codes, const int64_t *labels,
+                         int64_t n_given, int B, int H, int W, const float *log_prob, const float *pos,
+                         const void *workspace) {
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!codes || !labels || !workspace || (!log_prob && !pos) || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (n_given < 0 || n_given > (long long)H * W) return VQB_ERR_BAD_ARG;
+    return 0;
+}
+
 // Activations the training forward keeps for the backward, in floats; N = B*H*W positions, all NHWC grids:
 //   xv[l], l = 0..L   input of layer l's vertical stack (xv[0] the embedding, also x_h of layer 0); xv[L] unused
 //   xh[l], l = 1..L   input of layer l's horizontal stack (xh[L] the head's input)

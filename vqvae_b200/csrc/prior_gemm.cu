@@ -16,7 +16,8 @@
 // The TF32 mode (vqb_prior_*_tf32) runs the same products on the wgmma GEMM of tc_gemm.cuh, which takes the same
 // accessors and epilogues: the backward is this file's backward with `tc_gemm` in place of `gemm` (the one-hot sums of
 // the class and code embeddings stay on the FFMA GEMM), and the forward is written below as four products per layer
-// and two for the head, with the same Saved layout as the fp32 training forward.  The fp32 forward stays on prior.cu's
+// and two for the head, with the same Saved layout as the fp32 training forward.  log_prob in TF32 runs that forward
+// up to the head's hidden layer and reduces the logits on chip (`tc_lse_kernel`).  The fp32 forward stays on prior.cu's
 // per-position kernels: on the FFMA GEMM it is faster on large grids but slower on the reference's 8x8 default
 // (DESIGN §8.1).
 #include "prior.cuh"
@@ -417,10 +418,10 @@ struct TcWs {
 //   vh = v2h(h_vert) + b + class, out_v = gate(h_vert + class)
 //   pre_h = horiz_stack * x_h + b + vh                 (kept taps)
 //   out_h = horiz_resid(gate(pre_h)) + b [+ x_h]       (the gate computed as the operand is staged)
-// and the head hid = relu(W1 x_h + b1), logits = W2 hid + b2 (NCHW).  3 + 4*n_layers launches.
+// and the head's hidden layer hid = relu(W1 x_h + b1), left at lay.hid().  2 + 4*n_layers launches.
 template <class Lay>
-void forward_tf32(cudaStream_t st, const Net &n, const long long *codes, const long long *lab, int B, int H, int W,
-                  float *logits, float *sp, const Lay &lay) {
+void forward_hid_tf32(cudaStream_t st, const Net &n, const long long *codes, const long long *lab, int B, int H, int W,
+                      float *sp, const Lay &lay) {
     const int npos = B * H * W, C = n.C, C2 = 2 * C;
     const Grid g{H, W};
     embed_kernel<<<grid_for((long long)npos * C), NT, 0, st>>>(codes, n.emb, npos, n.K, C, sp + lay.xv(0));
@@ -439,9 +440,113 @@ void forward_tf32(cudaStream_t st, const Net &n, const long long *codes, const l
         product<Tf32>(st, Gated{ph, C}, Mat{w.resid_w, C},
                       BiasStore{sp + lay.xh(l + 1), w.resid_b, w.residual ? xh : nullptr, C}, npos, C, C);
     }
-    float *hid = sp + lay.hid();
-    product<Tf32>(st, Mat{sp + lay.xh(n.L), C}, Mat{n.w1, HID}, ReluBias{hid, n.b1}, npos, HID, C);
-    product<Tf32>(st, Mat{hid, HID}, Mat{n.w2, n.K}, Logits{logits, n.b2, n.K, H * W}, npos, n.K, HID);
+    product<Tf32>(st, Mat{sp + lay.xh(n.L), C}, Mat{n.w1, HID}, ReluBias{sp + lay.hid(), n.b1}, npos, HID, C);
+}
+
+// GatedPixelCNN.forward in TF32: forward_hid_tf32, then logits = W2 hid + b2 (NCHW).  3 + 4*n_layers launches.
+template <class Lay>
+void forward_tf32(cudaStream_t st, const Net &n, const long long *codes, const long long *lab, int B, int H, int W,
+                  float *logits, float *sp, const Lay &lay) {
+    forward_hid_tf32(st, n, codes, lab, B, H, W, sp, lay);
+    product<Tf32>(st, Mat{sp + lay.hid(), HID}, Mat{n.w2, n.K}, Logits{logits, n.b2, n.K, H * W}, B * H * W, n.K, HID);
+}
+
+// ---- log_prob in TF32 ----------------------------------------------------------------------------------------------
+// The logits product of forward_tf32 with its epilogue replaced by a running log-sum-exp: CTA (x, y) takes the
+// 128-position tile x and the N tiles [y*per, min((y+1)*per, tiles)) of the K codes, in order.  Each N tile is
+// tc_tile's product (the forward's staging, k order and BN), plus the bias: bitwise the forward's logits.  A row's
+// BN logits sit on the four lanes of a quad (wgmma's accumulator layout), so each row's tile max and sum of exp are
+// quad shuffles; the running (m, s) of a row is rescaled to the new max tile by tile, and the logit at the row's
+// clamped code is kept.  One partial (prior.cuh) per position and CTA column y; no logit goes to memory.
+template <int BN, class LA, class LB>
+__global__ void __launch_bounds__(TC_T) tc_lse_kernel(LA a, LB b, const float *__restrict__ bias,
+                                                      const long long *__restrict__ codes, int M, int N, int K,
+                                                      int per, int a_mode, int b_mode, float *__restrict__ part) {
+    extern __shared__ unsigned char tc_smem[];
+    const uint32_t base = (ptx::smem_u32(tc_smem) + 1023u) & ~1023u;
+    const int tid = threadIdx.x, wgi = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int m0 = blockIdx.x * TC_BM, splits = gridDim.y;
+    const int t0 = blockIdx.y * per, t1 = min((N + BN - 1) / BN, t0 + per);
+    const int row = m0 + wgi * 64 + warp * 16 + (lane >> 2);
+    float m[2] = {-INFINITY, -INFINITY}, s[2] = {0.f, 0.f}, lt[2] = {-INFINITY, -INFINITY};
+    int tgt[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) tgt[h] = row + 8 * h < M ? clampi(codes[row + 8 * h], N) : -1;
+    float acc[BN / 2];
+    for (int t = t0; t < t1; ++t) {
+        const int n0 = t * BN;
+        __syncthreads();                                // the previous tile's last stage is read by both warpgroups
+        tc_tile<BN>(acc, a, b, base, m0, M, n0, N, 0, K, a_mode, b_mode);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float mt = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = n0 + 8 * j + 2 * (lane & 3) + e;
+                    float &v = acc[4 * j + 2 * h + e];
+                    if (n < N) {
+                        v = v + __ldg(bias + n);
+                        mt = fmaxf(mt, v);
+                        if (n == tgt[h]) lt[h] = v;
+                    }
+                }
+            mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+            mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+            const float Mn = fmaxf(m[h], mt);
+            float st = 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                    if (n0 + 8 * j + 2 * (lane & 3) + e < N) st += expf(acc[4 * j + 2 * h + e] - Mn);
+            st += __shfl_xor_sync(0xffffffffu, st, 1);
+            st += __shfl_xor_sync(0xffffffffu, st, 2);
+            s[h] = s[h] * expf(m[h] - Mn) + st;
+            m[h] = Mn;
+        }
+    }
+    // the target logit sits on one lane of the quad (or none, outside this CTA's N tiles)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        lt[h] = fmaxf(lt[h], __shfl_xor_sync(0xffffffffu, lt[h], 1));
+        lt[h] = fmaxf(lt[h], __shfl_xor_sync(0xffffffffu, lt[h], 2));
+        const int r = row + 8 * h;
+        if ((lane & 3) == 0 && r < M) {
+            float *q = part + ((long long)r * splits + blockIdx.y) * 3;
+            q[0] = m[h];
+            q[1] = s[h];
+            q[2] = lt[h];
+        }
+    }
+}
+
+// N ranges of tc_lse_kernel over npos positions and K codes: enough CTAs for about two per SM of an H100 (132 SMs,
+// a constant: the split, and with it the result's bits, depends on the shape only), at most one N tile per range.
+// per: N tiles per range.
+int lse_splits(long long npos, int K, int *per = nullptr) {
+    const int tiles = wgrad_cdiv(K, tc_bn(K)), ptiles = wgrad_cdiv(npos, TC_BM);
+    int splits = wgrad_cdiv(2 * 132, ptiles);
+    splits = splits < 1 ? 1 : (splits > tiles ? tiles : splits);
+    const int p = wgrad_cdiv(tiles, splits);
+    if (per) *per = p;
+    return wgrad_cdiv(tiles, p);                    // no empty range
+}
+
+template <int BN, class LA, class LB>
+void tc_lse_launch(cudaStream_t st, const LA &a, const LB &b, const float *bias, const long long *codes, int M, int N,
+                   int K, float *part) {
+    static bool attr_set = false;                   // if this fails, so does the launch, and the caller reports it
+    if (!attr_set)
+        attr_set = cudaFuncSetAttribute(tc_lse_kernel<BN, LA, LB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        TcTile<BN>::SMEM) == cudaSuccess;
+    int per;
+    const int splits = lse_splits(M, N, &per);
+    int a_mode, b_mode;
+    tc_modes(a, b, N, K, WgradSplit{1, K}, a_mode, b_mode);
+    tc_lse_kernel<BN, LA, LB><<<dim3(wgrad_cdiv(M, TC_BM), splits), TC_T, TcTile<BN>::SMEM, st>>>(
+        a, b, bias, codes, M, N, K, per, a_mode, b_mode, part);
 }
 
 }  // namespace
@@ -480,6 +585,37 @@ extern "C" int vqb_prior_forward_train_tf32(const vqb_prior_net *net, const int6
                  reinterpret_cast<const long long *>(labels), B, H, W, logits, static_cast<float *>(saved),
                  Saved{(long long)B * H * W, n.C, n.L});
     VQB_COUNT_LAUNCH(3 + 4 * n.L);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_prior_log_prob_workspace_bytes_tf32(int B, int H, int W, int dim, int n_layers, int K) {
+    const size_t base = vqb_prior_workspace_bytes_tf32(B, H, W, dim, n_layers, K);
+    if (!base) return 0;
+    const long long npos = (long long)B * H * W;
+    return base + (size_t)npos * lse_splits(npos, K) * 3 * sizeof(float);
+}
+
+// forward_tf32 up to hid (the same launches and values), then tc_lse_kernel in place of the logits product, and the
+// finish.  4 + 4*n_layers launches.
+extern "C" int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                       int64_t n_given, int B, int H, int W, float *log_prob, float *pos_log_prob,
+                                       void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = log_prob_args(net, n, codes, labels, n_given, B, H, W, log_prob, pos_log_prob, workspace);
+    if (st) return st;
+    if (workspace_bytes < vqb_prior_log_prob_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *cd = reinterpret_cast<const long long *>(codes);
+    const int npos = B * H * W;
+    const TcWs lay{npos, n.C};
+    float *sp = static_cast<float *>(workspace), *part = sp + lay.total();
+    forward_hid_tf32(s, n, cd, reinterpret_cast<const long long *>(labels), B, H, W, sp, lay);
+    const Mat a{sp + lay.hid(), HID}, b{n.w2, n.K};
+    if (tc_bn(n.K) == 64) tc_lse_launch<64>(s, a, b, n.b2, cd, npos, n.K, HID, part);
+    else tc_lse_launch<128>(s, a, b, n.b2, cd, npos, n.K, HID, part);
+    log_prob_finish_kernel<<<B, NT, 0, s>>>(part, lse_splits(npos, n.K), (long long)H * W, n_given, log_prob,
+                                            pos_log_prob);
+    VQB_COUNT_LAUNCH(4 + 4 * n.L);
     return vqb_cuda_status(cudaGetLastError());
 }
 

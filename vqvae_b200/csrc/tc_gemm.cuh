@@ -5,7 +5,9 @@
 // tc_gemm_kernel computes out(m, n) = sum over k in chunk z of A(m, k) * B(k, n).  Per CTA: a 128-row tile, two
 // warpgroups of m64nBNk8 (BN = 64 or 128, chosen per call from N), k-steps of 32 floats.  Both operands are staged
 // K-major into 128-byte swizzled shared-memory rows, A as [m][k] and B as [n][k], through registers: each thread loads
-// the next k-step while the tensor cores run the current one, then writes it to the other of two stages.
+// the next k-step while the tensor cores run the current one, then writes it to the other of two stages.  That k-loop
+// is `tc_tile`, which prior_gemm.cu's log_prob head (`tc_lse_kernel`) also runs, tile after tile, with the staging
+// modes `tc_modes` and the tile width `tc_bn` choose here: its products are bitwise this kernel's.
 //
 // Staging.  An operand accessor may offer 32 consecutive k of one row as a pointer (A: `seg(i, k0)`, contiguous along
 // j; B: `segT(k0, j)`, contiguous along i), or nullptr for a row of zeros (a tap outside the grid).  When the product's
@@ -149,20 +151,18 @@ struct Stager {
     }
 };
 
-template <int BN, class LA, class LB, class EP>
-__global__ void __launch_bounds__(TC_T) tc_gemm_kernel(LA a, LB b, EP ep, int M, int N, long long K, int chunk,
-                                                       int a_mode, int b_mode) {
+// The (128 x BN) tile at rows m0, columns n0 of the product over k in [k_begin, k_begin + kc), into acc in wgmma's
+// accumulator layout (wgmma.cuh), staged through the two stages at `base` (TcTile<BN>).  Every thread of the CTA
+// calls it.  On return no wgmma of this thread is in flight, but the other warpgroup may still read the stage of the
+// last k-step: a caller that runs the loop again first waits for the whole CTA.
+template <int BN, class LA, class LB>
+__device__ __forceinline__ void tc_tile(float (&acc)[BN / 2], const LA &a, const LB &b, uint32_t base, int m0, int M,
+                                        int n0, int N, long long k_begin, int kc, int a_mode, int b_mode) {
     using T = TcTile<BN>;
-    extern __shared__ unsigned char tc_smem[];
-    const uint32_t base = (ptx::smem_u32(tc_smem) + 1023u) & ~1023u;
-    const int tid = threadIdx.x, wgi = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
-    const int m0 = blockIdx.x * TC_BM, n0 = blockIdx.y * BN;
-    const long long k_begin = (long long)blockIdx.z * chunk;
-    const int kc = (int)min((long long)chunk, K - k_begin);     // this chunk's k, counted in 32 bits
+    const int wgi = threadIdx.x >> 7;
     const int steps = (kc + TC_BK - 1) / TC_BK;
     Stager<false, TC_BM, LA> sa;
     Stager<true, BN, LB> sb;
-    float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     // k-step s of both operands into stage s % 2
@@ -197,6 +197,19 @@ __global__ void __launch_bounds__(TC_T) tc_gemm_kernel(LA a, LB b, EP ep, int M,
         wg::wait<0>();
         wg::fence_regs<BN>(acc);
     }
+}
+
+template <int BN, class LA, class LB, class EP>
+__global__ void __launch_bounds__(TC_T) tc_gemm_kernel(LA a, LB b, EP ep, int M, int N, long long K, int chunk,
+                                                       int a_mode, int b_mode) {
+    extern __shared__ unsigned char tc_smem[];
+    const uint32_t base = (ptx::smem_u32(tc_smem) + 1023u) & ~1023u;
+    const int tid = threadIdx.x, wgi = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int m0 = blockIdx.x * TC_BM, n0 = blockIdx.y * BN;
+    const long long k_begin = (long long)blockIdx.z * chunk;
+    const int kc = (int)min((long long)chunk, K - k_begin);     // this chunk's k, counted in 32 bits
+    float acc[BN / 2];
+    tc_tile<BN>(acc, a, b, base, m0, M, n0, N, k_begin, kc, a_mode, b_mode);
     // wgmma's accumulator layout (wgmma.cuh): row 16*warp + lane/4 (+8), columns 8j + 2*(lane%4) + {0,1}
     const int row = m0 + wgi * 64 + warp * 16 + (lane >> 2);
 #pragma unroll
@@ -221,11 +234,11 @@ void tc_launch(cudaStream_t st, const LA &a, const LB &b, const EP &ep, int M, i
     tc_gemm_kernel<BN, LA, LB, EP><<<grid, TC_T, TcTile<BN>::SMEM, st>>>(a, b, ep, M, N, K, sp.chunk, a_mode, b_mode);
 }
 
-// one launch: the (M x N) product over K, chunk z of sp on blockIdx.z (as `gemm`)
-template <class LA, class LB, class EP>
-void tc_gemm(cudaStream_t st, LA a, LB b, EP ep, int M, int N, long long K, WgradSplit sp) {
+// How tc_tile stages each operand of a product over K in chunks of sp.chunk
+template <class LA, class LB>
+void tc_modes(const LA &a, const LB &b, int N, long long K, WgradSplit sp, int &a_mode, int &b_mode) {
     const bool whole = K % TC_BK == 0 && sp.chunk % TC_BK == 0;     // no k-step leaves a row of 32
-    int a_mode = BY_VALUE, b_mode = BY_VALUE;
+    a_mode = b_mode = BY_VALUE;
     if constexpr (has_seg<LA>)
         if (whole && a.seg_ok()) a_mode = ALONG_K;
     if constexpr (has_segT<LB>)
@@ -233,7 +246,17 @@ void tc_gemm(cudaStream_t st, LA a, LB b, EP ep, int M, int N, long long K, Wgra
     // (never a WithOnes operand: its N = cols + 1 is odd, as cols is a multiple of 32)
     if constexpr (has_seg<LB>)
         if (N % 4 == 0 && b.seg_ok()) b_mode = ALONG_N;
-    if (N <= 64) tc_launch<64>(st, a, b, ep, M, N, K, sp, a_mode, b_mode);
+}
+
+// the tile width of a product with N columns
+inline int tc_bn(int N) { return N <= 64 ? 64 : 128; }
+
+// one launch: the (M x N) product over K, chunk z of sp on blockIdx.z (as `gemm`)
+template <class LA, class LB, class EP>
+void tc_gemm(cudaStream_t st, LA a, LB b, EP ep, int M, int N, long long K, WgradSplit sp) {
+    int a_mode, b_mode;
+    tc_modes(a, b, N, K, sp, a_mode, b_mode);
+    if (tc_bn(N) == 64) tc_launch<64>(st, a, b, ep, M, N, K, sp, a_mode, b_mode);
     else tc_launch<128>(st, a, b, ep, M, N, K, sp, a_mode, b_mode);
 }
 

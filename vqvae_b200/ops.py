@@ -533,6 +533,27 @@ def prior_forward(net, codes, labels, precision="fp32"):
     return logits
 
 
+def prior_log_prob(net, codes, labels, n_given, precision="fp32", per_position=False):
+    """log softmax of the teacher-forced logits at each int64 code of codes (B,H,W) (clamped to [0, K-1]), without
+    writing the logits (vqb_prior_log_prob_f32, or _tf32 for precision="tf32") -> per_position=False: (B,) fp32, the
+    compensated sum over the raster positions >= n_given; per_position=True: the (B,H,W) fp32 map of every term."""
+    sfx = _prior_precision(precision)
+    B, H, W = codes.shape
+    dev = codes.device
+    ws = _prior_workspace(net, B, H, W, dev, getattr(lib(), "vqb_prior_log_prob_workspace_bytes" +
+                                                     ("_tf32" if sfx == "tf32" else "")))
+    out = torch.empty((B, H, W) if per_position else (B,), dtype=torch.float32, device=dev)
+    span = _Span(f"prior log_prob ({precision}) K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W} "
+                 f"n_given={n_given}")
+    check(getattr(lib(), "vqb_prior_log_prob_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), n_given,
+                                                       B, H, W, None if per_position else out.data_ptr(),
+                                                       out.data_ptr() if per_position else None, ws.data_ptr(),
+                                                       ws.numel(), _stream()),
+          "prior_log_prob")
+    span.done()
+    return out
+
+
 def prior_generate(net, labels, u, step_logits=None):
     """The whole sampling loop (vqb_prior_generate_f32): int64 codes (B,H,W) drawn with the uniforms u (B,H,W).
     step_logits: None, or a (B,H,W,K) fp32 tensor receiving the logits of every step."""

@@ -10,7 +10,7 @@ through the C ABI, in the model's ``precision`` (fp32 by default) whatever ``set
 requires grad (``_PriorFunction``: the training forward keeps its activations, and the backward of
 ``csrc/prior_gemm.cu`` writes one gradient per parameter), so the reference's training loop runs unchanged.  Under
 ``torch.no_grad()`` it is the inference forward.  ``GatedPixelCNN.precision`` (a plain attribute, not in the state
-dict) selects the arithmetic of ``forward``, inference and training alike: "fp32" (the default, CUDA cores) or
+dict) selects the arithmetic of ``forward`` (inference and training alike) and of ``log_prob``: "fp32" (the default, CUDA cores) or
 "tf32" (every matrix product on the wgmma TF32 GEMM, operands rounded to TF32, fp32 accumulation; the one-hot
 embedding-gradient sums stay fp32).  ``generate``, ``complete``, ``sample``, ``sample_completion``,
 ``GatedMaskedConv2d`` and ``GatedActivation`` stay fp32 in both modes, and ``set_precision`` does not affect the
@@ -337,6 +337,62 @@ class GatedPixelCNN(nn.Module):
             return _PriorFunction.apply(self, precision, x, label, *self.parameters())
         keep = []
         return ops.prior_forward(self._net(keep), x, label, precision)
+
+    def _log_prob_args(self, x, label, n_given, per_position):
+        """log_prob()'s host-side checks, in order, before any CUDA check or launch: the precision, n_given (an int),
+        the codes' rank, n_given in [0, H*W], per_position only with n_given = 0, a square grid, the layers (P5),
+        the label count (ValueError for the arguments, RuntimeError for the shapes, as forward and complete)."""
+        what = "GatedPixelCNN.log_prob"
+        if self.precision not in ops.PRIOR_PRECISIONS:
+            raise ValueError(f"GatedPixelCNN.precision must be one of {ops.PRIOR_PRECISIONS}, got {self.precision!r}")
+        if isinstance(n_given, bool) or not isinstance(n_given, numbers.Integral):
+            raise ValueError(f"{what}: n_given must be an int, got {n_given!r}")
+        if x.dim() != 3:
+            raise RuntimeError(f"{what}: expected codes of shape (B,H,W), got {tuple(x.shape)}")
+        B, H, W = x.shape
+        if not 0 <= n_given <= H * W:
+            raise ValueError(f"{what}: n_given must be in [0, H*W] = [0, {H * W}], got {n_given}")
+        if per_position and n_given != 0:
+            raise ValueError(f"{what}: per_position=True scores every position; n_given must be 0, got {n_given}")
+        _square(H, W, what)
+        self._check_layers()
+        n = (label if torch.is_tensor(label) else torch.as_tensor(label)).numel()
+        if n != B:
+            raise RuntimeError(f"{what}: expected {B} labels, got {n}")
+        return int(n_given)
+
+    def _log_prob(self, x, label, n_given=0, per_position=False):
+        """log_prob() as a graph-capturable call: the same checks and result, and for int64 contiguous codes and
+        labels on the device no copy of either, so a CUDA graph captured around it reads x and label in place."""
+        n_given = self._log_prob_args(x, label, n_given, per_position)
+        B, H, W = x.shape
+        ops._require_cuda(x, "GatedPixelCNN.log_prob codes")
+        label = _labels(label, B, x.device, "GatedPixelCNN.log_prob")
+        x = x.detach().to(torch.int64).contiguous()
+        if n_given == H * W:                # nothing to score: no packing, no launch
+            return torch.zeros((B,), dtype=torch.float32, device=x.device)
+        keep = []
+        return ops.prior_log_prob(self._net(keep), x, label, n_given, self.precision, per_position)
+
+    def log_prob(self, x, label, *, n_given=0, per_position=False):
+        """Log-likelihood of given code grids: int64 codes x (B,H,W) and labels (B,) (as forward takes them) ->
+        fp32 (B,), entry b the sum over raster positions p = i*W + j >= n_given of
+        log_softmax(forward(x, label)[b, :, i, j])[x[b, i, j]], in the model's ``precision``.  per_position=True
+        returns the (B,H,W) fp32 map of every position's term instead (n_given must then be 0).  The first n_given
+        positions are context, not scored, as in sample_completion; n_given = H*W gives zeros without a launch.
+
+        -log_prob(x, label).sum() / x.numel() is the reference's validation loss (nn.CrossEntropyLoss on forward's
+        logits), without writing the B*K*H*W logits: each position's logits are reduced on chip and the per-image
+        sums are compensated fp32 sums in raster order, deterministic.  Codes outside [0, K-1] are clamped, as the
+        embedding clamps them, and scored as the clamped code (torch's cross-entropy would raise).  Any layer stack
+        forward takes is taken; with a layer 0 that reads the code it scores (not mask A without residual, P5) the
+        result is the reference loop's cross-entropy, not a likelihood.
+
+        Never differentiable: it runs the inference kernels even with grad enabled and parameters requiring grad,
+        keeps no training activations, and returns a tensor without grad.  Train with forward plus the
+        cross-entropy.  ValueError for a bad precision, n_given or per_position with n_given != 0; RuntimeError for
+        forward's shape, layer (P5), label and device checks; every host-side check runs before any CUDA check."""
+        return self._log_prob(x, label, n_given, per_position)
 
     def _check_causal(self, what):
         """P5: the sampler needs a layer 0 that reads only the codes before the one being drawn."""
