@@ -263,6 +263,32 @@ int vqb_vq_backward_f32(const float *g_zq, const float *g_loss, const float *z, 
 int vqb_vq_finish_f32(const double *sse, const int32_t *hist, int64_t N, int K, int D,
                       float beta, float *loss, float *perplexity, void *stream);
 
+/* ---- exponential-moving-average codebook (VectorQuantizer(decay=...), van den Oord et al. 2017, A.1) ----
+ * One update from the rows z (N,D) fp32 that vqb_vq_forward_f32 quantized, their codes idx (N) int64 (clamped to
+ * [0, K-1]) and its hist (K) int32 (n_k):
+ *   cluster_size N_k <- decay N_k + (1-decay) n_k        embed_sum m_k <- decay m_k + (1-decay) s_k
+ *   n = sum_k N_k,   codebook e_k <- m_k / ((N_k + eps) / (n + K eps) * n)          (all three in place, fp32)
+ * s_k = sum of the rows of code k in a fixed order: by ascending row index, in consecutive segments of 256 rows, each
+ * one fp32 add chain, the segment partials added in segment order; the result bits depend on (z, idx) only.  Five
+ * launches, no float atomics, no host synchronisation.  decay in [0, 1), eps finite and > 0 and NULL pointers:
+ * VQB_ERR_BAD_ARG; D % 4 != 0: VQB_ERR_UNSUPPORTED; both before any launch.  z, embed_sum, codebook and the
+ * workspace (vqb_vq_ema_workspace_bytes(N,K,D) bytes, 0 for a shape it refuses) 16-byte aligned.              */
+size_t vqb_vq_ema_workspace_bytes(int64_t N, int K, int D);
+int vqb_vq_ema_update_f32(const float *z, const int64_t *idx, const int32_t *hist, int64_t N, int K,
+                          int D, float decay, float eps, float *cluster_size, float *embed_sum,
+                          float *codebook, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Backward of the EMA quantizer, whose loss is the commitment term alone (the codebook gets no gradient):
+ *   dz (N,D) = g_zq + g_loss * 2 beta/(N D) * (z - zq)
+ * zq = the forward's fp32 z_q rows (not the codebook, which the update has overwritten).  g_zq / g_loss may be
+ * NULL (= zero).  One launch, no atomics.  D % 4 == 0, 16-byte aligned pointers.                              */
+int vqb_vq_commit_backward_f32(const float *g_zq, const float *g_loss, const float *z, const float *zq,
+                               int64_t N, int D, float beta, float *dz, void *stream);
+
+/* vqb_vq_finish_f32 for the EMA quantizer: loss = beta * sse/(N*D) (fp32), the same perplexity.             */
+int vqb_vq_finish_ema_f32(const double *sse, const int32_t *hist, int64_t N, int K, int D,
+                          float beta, float *loss, float *perplexity, void *stream);
+
 /* Dense one-hot min_encodings (N,K) fp32 for direct VectorQuantizer.forward callers
  * (quantizer.py:55-57,76); VQVAE.forward discards it (vqvae.py:34) so it is never
  * built on that path.                                                             */

@@ -35,6 +35,10 @@ SIGNATURES = {
     "vqb_memcpy_async": (_i, [_vp, _vp, _sz, _i, _vp]),
     "vqb_vq_finish_f32": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _vp, _vp]),
     "vqb_vq_backward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _vp, _vp, _vp]),
+    "vqb_vq_ema_workspace_bytes": (_sz, [_i64, _i, _i]),
+    "vqb_vq_ema_update_f32": (_i, [_vp, _vp, _vp, _i64, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "vqb_vq_commit_backward_f32": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _f, _vp, _vp]),
+    "vqb_vq_finish_ema_f32": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _vp, _vp]),
     "vqb_onehot_f32": (_i, [_vp, _i64, _i, _vp, _vp]),
     "vqb_gather_rows_f32": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vqb_nchw_to_nhwc_f32": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),

@@ -24,9 +24,16 @@ def load_checkpoint(path, device="cuda"):
     missing = [k for k in _HP_KEYS if k not in hp]
     if missing:
         raise KeyError(f"{path}: hyperparameters lack {missing}")
+    ema = data.get("vq_ema")
+    kw = {} if ema is None else dict(ema_decay=ema["decay"], ema_eps=ema["eps"])
     model = VQVAE(hp["n_hiddens"], hp["n_residual_hiddens"], hp["n_residual_layers"], hp["n_embeddings"],
-                  hp["embedding_dim"], hp["beta"])
+                  hp["embedding_dim"], hp["beta"], **kw)
     model.load_state_dict(data["model"])          # 23 keys incl. the aliased stack.1.* (SURVEY Q1)
+    if ema is not None:                           # the EMA buffers travel beside "model" (save_checkpoint)
+        vq = model.vector_quantization
+        with torch.no_grad():
+            vq.ema_cluster_size.copy_(ema["cluster_size"])
+            vq.ema_embed_sum.copy_(ema["embed_sum"])
     model = model.to(device).eval()
     if torch.device(device).type == "cuda":
         with torch.cuda.device(torch.device(device)):
@@ -35,5 +42,17 @@ def load_checkpoint(path, device="cuda"):
 
 
 def save_checkpoint(model, results, hyperparameters, path):
-    """Write the reference's checkpoint format (utils.py:106-115) so its notebook / load_model can read the file."""
-    torch.save({"model": model.state_dict(), "results": results, "hyperparameters": hyperparameters}, path)
+    """Write the reference's checkpoint format (utils.py:106-115) so its notebook / load_model can read the file.
+    A model with an EMA codebook (``ema_decay``) keeps ``model`` to the reference's keys, so that ``load_model`` still
+    loads it strictly, and adds ``"vq_ema": {decay, eps, cluster_size, embed_sum}``; load_checkpoint rebuilds the
+    EMA model from it."""
+    sd = model.state_dict()
+    data = {"model": sd, "results": results, "hyperparameters": hyperparameters}
+    vq = model.vector_quantization
+    if vq.decay is not None:
+        prefix = "vector_quantization."
+        for k in vq._EMA_KEYS:
+            del sd[prefix + k]
+        data["vq_ema"] = {"decay": vq.decay, "eps": vq.eps, "cluster_size": vq.ema_cluster_size.detach().cpu(),
+                          "embed_sum": vq.ema_embed_sum.detach().cpu()}
+    torch.save(data, path)

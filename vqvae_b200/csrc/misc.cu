@@ -42,7 +42,9 @@ __global__ void transpose_kernel(const float *__restrict__ in, float *__restrict
     }
 }
 
-// quantizer.py:63-64 and :70-71 in fp32, like the reference's scalar ops
+// quantizer.py:63-64 and :70-71 in fp32, like the reference's scalar ops.  COMMIT_ONLY (the EMA codebook): the loss is
+// the commitment term beta * mse alone.
+template <bool COMMIT_ONLY>
 __global__ void vq_finish_kernel(const double *__restrict__ sse, const int *__restrict__ hist, long long N,
                                  int K, int D, float beta, float *__restrict__ loss, float *__restrict__ perp) {
     __shared__ float sh[256];
@@ -59,7 +61,7 @@ __global__ void vq_finish_kernel(const double *__restrict__ sse, const int *__re
     }
     if (threadIdx.x == 0) {
         const float mse = (float)(*sse / ((double)N * (double)D));
-        *loss = __fadd_rn(mse, __fmul_rn(beta, mse));
+        *loss = COMMIT_ONLY ? __fmul_rn(beta, mse) : __fadd_rn(mse, __fmul_rn(beta, mse));
         *perp = expf(-sh[0]);
     }
 }
@@ -172,7 +174,15 @@ extern "C" int vqb_nhwc_to_nchw_f32(const float *in, float *out, int B, int C, i
 extern "C" int vqb_vq_finish_f32(const double *sse, const int32_t *hist, int64_t N, int K, int D, float beta,
                                  float *loss, float *perplexity, void *stream) {
     if (!sse || !hist || !loss || !perplexity || N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
-    vq_finish_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(sse, hist, N, K, D, beta, loss, perplexity);
+    vq_finish_kernel<false><<<1, 256, 0, (cudaStream_t)stream>>>(sse, hist, N, K, D, beta, loss, perplexity);
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_vq_finish_ema_f32(const double *sse, const int32_t *hist, int64_t N, int K, int D, float beta,
+                                     float *loss, float *perplexity, void *stream) {
+    if (!sse || !hist || !loss || !perplexity || N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
+    vq_finish_kernel<true><<<1, 256, 0, (cudaStream_t)stream>>>(sse, hist, N, K, D, beta, loss, perplexity);
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }

@@ -23,6 +23,7 @@ Reference semantics reproduced on purpose (SURVEY 3.3):
   Q8  verbose=True prints three shapes and then ``assert False``
 """
 import contextlib
+import math
 
 import torch
 import torch.nn as nn
@@ -436,36 +437,105 @@ class Decoder(nn.Module):
 
 class _VQFunction(torch.autograd.Function):
     """Training-mode VectorQuantizer core (SURVEY 8f rank 3): the fused forward kernel plus vqb_vq_backward_f32 --
-    straight-through gradient to z, commitment / codebook gradients scatter-added by index (quantizer.py:63-67)."""
+    straight-through gradient to z, commitment / codebook gradients scatter-added by index (quantizer.py:63-67).
+    With an EMA codebook (`vq.decay` set) the loss is the commitment term alone, `update` runs the EMA update right
+    after the VQ kernel, and the backward is vqb_vq_commit_backward_f32 on the forward's own z_q rows: the codebook is
+    neither saved (the update rewrites it in place) nor given a gradient."""
 
     @staticmethod
-    def forward(ctx, z_rows, codebook, beta):
+    def forward(ctx, z_rows, codebook, beta, vq, update):
         z_rows, codebook = z_rows.detach().contiguous(), codebook.detach().contiguous()
         idx, zq, sse, hist = ops.vq_forward(z_rows, codebook)
         N, D = z_rows.shape
-        loss, perp = ops.vq_finish(sse, hist, N, codebook.shape[0], D, beta)
-        ctx.save_for_backward(z_rows, codebook, idx)
-        ctx.beta = beta
+        ctx.beta, ctx.ema = beta, vq.decay is not None
+        if ctx.ema:
+            loss, perp = ops.vq_finish_ema(sse, hist, N, codebook.shape[0], D, beta)
+            if update:
+                vq._ema_update(z_rows, idx, hist)
+            ctx.save_for_backward(z_rows, zq)
+        else:
+            loss, perp = ops.vq_finish(sse, hist, N, codebook.shape[0], D, beta)
+            ctx.save_for_backward(z_rows, codebook, idx)
         ctx.mark_non_differentiable(perp, idx)
         return loss, zq, perp, idx
 
     @staticmethod
     def backward(ctx, g_loss, g_zq, _g_perp, _g_idx):
+        if ctx.ema:
+            z_rows, zq = ctx.saved_tensors
+            return ops.vq_commit_backward(g_zq, g_loss, z_rows, zq, ctx.beta), None, None, None, None
         z_rows, codebook, idx = ctx.saved_tensors
         dz, dE = ops.vq_backward(g_zq, g_loss, z_rows, codebook, idx, ctx.beta)
-        return dz, dE, None
+        return dz, dE, None, None, None
+
+
+def _check_ema(decay, eps):
+    """ValueError unless decay is None or in [0, 1) and eps is finite and > 0."""
+    if decay is not None:
+        try:
+            d = float(decay)
+        except (TypeError, ValueError):
+            raise ValueError(f"decay must be None or a number in [0, 1), got {decay!r}") from None
+        if not 0.0 <= d < 1.0:
+            raise ValueError(f"decay must be None or a number in [0, 1), got {decay!r}")
+    try:
+        e = float(eps)
+    except (TypeError, ValueError):
+        raise ValueError(f"eps must be a finite number > 0, got {eps!r}") from None
+    if not (math.isfinite(e) and e > 0.0):
+        raise ValueError(f"eps must be a finite number > 0, got {eps!r}")
 
 
 class VectorQuantizer(nn.Module):
-    """Discretisation bottleneck: models/quantizer.py:10-76."""
+    """Discretisation bottleneck: models/quantizer.py:10-76.
 
-    def __init__(self, n_e, e_dim, beta):
+    ``decay`` (keyword only, default None = the reference's module): learn the codebook by exponential moving averages
+    (van den Oord et al. 2017, appendix A.1) instead of by gradient.  ``embedding.weight`` then takes no gradient, two
+    fp32 buffers hold the averages -- ``ema_cluster_size`` N (K,) and ``ema_embed_sum`` m (K, D), initialised as if
+    each code had been assigned one vector equal to itself (N = 1, m = e) -- and every differentiable call in training
+    mode (grad enabled, z requiring grad) updates N, m and the codebook in place (vqb_vq_ema_update_f32):
+    N <- decay N + (1-decay) n_k,  m <- decay m + (1-decay) s_k,  e = m / ((N + eps) / (n + K eps) * n).  The loss is
+    the commitment term beta * mse((sg[z_q], z)) on every path."""
+
+    def __init__(self, n_e, e_dim, beta, *, decay=None, eps=1e-5):
+        _check_ema(decay, eps)
         super().__init__()
         self.n_e = n_e
         self.e_dim = e_dim
         self.beta = beta
+        self.decay = None if decay is None else float(decay)
+        self.eps = float(eps)
         self.embedding = nn.Embedding(self.n_e, self.e_dim)
         self.embedding.weight.data.uniform_(-1.0 / self.n_e, 1.0 / self.n_e)
+        if self.decay is not None:
+            self.embedding.weight.requires_grad_(False)
+            self.register_buffer("ema_cluster_size", torch.ones(self.n_e))
+            self.register_buffer("ema_embed_sum", self.embedding.weight.detach().clone())
+
+    _EMA_KEYS = ("ema_cluster_size", "ema_embed_sum")
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                              error_msgs):
+        """A state dict without the EMA buffers (a reference checkpoint, a decay=None model) loads into an EMA model:
+        the buffers restart from the loaded codebook (N = 1, m = e)."""
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                                      error_msgs)
+        w = state_dict.get(prefix + "embedding.weight")
+        keys = [prefix + k for k in self._EMA_KEYS]
+        if self.decay is None or w is None or not all(k in missing_keys for k in keys):
+            return
+        with torch.no_grad():
+            self.ema_cluster_size.fill_(1.0)
+            self.ema_embed_sum.copy_(w)
+        for k in keys:
+            missing_keys.remove(k)
+
+    def _ema_update(self, rows, idx, hist):
+        """One EMA update of N, m and the codebook from the rows the VQ kernel just quantized; bumps their version
+        counters as an optimizer step does."""
+        w = self.embedding.weight
+        ops.vq_ema_update(rows, idx, hist, self.decay, self.eps, self.ema_cluster_size, self.ema_embed_sum, w.detach())
+        torch.autograd.graph.increment_version([w, self.ema_cluster_size, self.ema_embed_sum])
 
     def _codebook(self):
         w = self.embedding.weight.detach()
@@ -483,7 +553,8 @@ class VectorQuantizer(nn.Module):
             # split), so the global row count is n_local * world_size: no host sync needed
             hist, sse = reduce_vq_stats(hist, sse, group)
             n_total = n_total * torch.distributed.get_world_size(group)
-        return ops.vq_finish(sse, hist, n_total, self.n_e, self.e_dim, self.beta)
+        finish = ops.vq_finish if self.decay is None else ops.vq_finish_ema
+        return finish(sse, hist, n_total, self.n_e, self.e_dim, self.beta)
 
     def _quantize_rows(self, rows, group=None):
         """rows (N, e_dim) fp32 CUDA -> (loss, zq_rows, perplexity, idx (N,))."""
@@ -499,7 +570,8 @@ class VectorQuantizer(nn.Module):
         ops._require_cuda(z, "VectorQuantizer input")
         B, D, H, W = z.shape
         rows = z.float().permute(0, 2, 3, 1).contiguous().view(-1, D)                   # quantizer.py:45-46
-        loss, zq, perp, idx = _VQFunction.apply(rows, self.embedding.weight.float(), float(self.beta))
+        update = self.training and self.decay is not None and z.requires_grad
+        loss, zq, perp, idx = _VQFunction.apply(rows, self.embedding.weight.float(), float(self.beta), self, update)
         z_q = zq.view(B, H, W, D).permute(0, 3, 1, 2).contiguous()                      # :74
         return loss, z_q, perp, ops.onehot(idx, self.n_e), idx.view(-1, 1)
 
@@ -815,7 +887,11 @@ class _VQVAEFunction(torch.autograd.Function):
         embedding_loss, x_hat, perplexity = model._walk(x, False, acts)
         ctx.model, ctx.acts, ctx.prec = model, acts, _conv_precision()
         # saved so that autograd raises, as it does for the reference, when the image or a parameter is modified in
-        # place between this forward and its backward (the backward reads the weights as they are then)
+        # place between this forward and its backward (the backward reads the weights as they are then).  An EMA
+        # codebook is not: the forward's own update rewrites it, and the backward does not read it.
+        vq = model.vector_quantization
+        if vq.decay is not None:
+            params = [p for p in params if p is not vq.embedding.weight]
         ctx.save_for_backward(x, *params)
         ctx.mark_non_differentiable(perplexity)
         return embedding_loss, x_hat, perplexity
@@ -834,26 +910,33 @@ class _VQVAEFunction(torch.autograd.Function):
         H2, W2 = H0 // 4, W0 // 4
         grads = {}
         g = _decoder_backward(model.decoder, ops._f32c(g_xhat), a["zq"], a["dec"], B, H2, W2, prec, grads)
-        # the VQ step: straight-through to z_e plus the loss terms; the codebook gradient (float atomics)
-        dz, dE = ops.vq_backward(g.view(-1, vq.e_dim), g_loss, a["z_e"], a["codebook"], a["idx"], float(vq.beta))
+        if vq.decay is None:
+            # the VQ step: straight-through to z_e plus the loss terms; the codebook gradient (float atomics)
+            dz, dE = ops.vq_backward(g.view(-1, vq.e_dim), g_loss, a["z_e"], a["codebook"], a["idx"], float(vq.beta))
+        else:
+            # EMA codebook: the commitment term only, from the forward's z_q rows; no codebook gradient
+            dz, dE = ops.vq_commit_backward(g.view(-1, vq.e_dim), g_loss, a["z_e"], a["zq"], float(vq.beta)), None
         grads[id(vq.embedding.weight)] = dE
         pq = model.pre_quantization_conv
         _conv_wgrad(pq, a["enc"][3], dz, B, H2, W2, grads)
         g = _conv_dgrad(pq, dz, B, H2, W2, prec)
         dx = _encoder_backward(model.encoder, g, x, a["enc"], prec, grads, ctx.needs_input_grad[1])
         params = list(model.parameters())
-        return (None, dx) + tuple(grads[id(p)].to(p.dtype) for p in params)
+        return (None, dx) + tuple(None if grads[id(p)] is None else grads[id(p)].to(p.dtype) for p in params)
 
 
 class VQVAE(nn.Module):
     """models/vqvae.py:10-44."""
 
     def __init__(self, h_dim, res_h_dim, n_res_layers, n_embeddings, embedding_dim, beta,
-                 save_img_embedding_map=False):
+                 save_img_embedding_map=False, *, ema_decay=None, ema_eps=1e-5):
+        """``ema_decay`` / ``ema_eps``: the quantizer's ``decay`` / ``eps`` (VectorQuantizer): None keeps the reference's
+        gradient-trained codebook."""
+        _check_ema(ema_decay, ema_eps)
         super().__init__()
         self.encoder = Encoder(3, h_dim, n_res_layers, res_h_dim)
         self.pre_quantization_conv = _PointwiseConv2d(h_dim, embedding_dim, kernel_size=1, stride=1)
-        self.vector_quantization = VectorQuantizer(n_embeddings, embedding_dim, beta)
+        self.vector_quantization = VectorQuantizer(n_embeddings, embedding_dim, beta, decay=ema_decay, eps=ema_eps)
         self.decoder = Decoder(embedding_dim, h_dim, n_res_layers, res_h_dim)
         if save_img_embedding_map:
             self.img_to_embedding_map = {i: [] for i in range(n_embeddings)}
@@ -958,11 +1041,15 @@ class VQVAE(nn.Module):
             self._side_stream = torch.cuda.Stream(device=z_e.device)
         side = self._side_stream
         side.wait_stream(main)
+        # A training call of an EMA model updates the codebook there too: the decoder reads z_q, not the codebook.
+        ema = acts is not None and vq.decay is not None
         with torch.cuda.stream(side):
             embedding_loss, perplexity = vq._scalars(sse, hist, n_rows, group if self.sync_scalars else None)
             self.last_vq_stats = (hist, sse, n_rows)
+            if ema:
+                vq._ema_update(z_e.view(-1, D), idx, hist)
             if not torch.cuda.is_current_stream_capturing():
-                for t in (sse, hist, embedding_loss, perplexity):
+                for t in (sse, hist, embedding_loss, perplexity) + ((z_e, idx) if ema else ()):
                     t.record_stream(side)
         x_hat = self.decoder._forward_from_nhwc(zq.view(B, H, W, D), B, H, W, bf16, acts, fuse, tf32)  # :36
         main.wait_stream(side)

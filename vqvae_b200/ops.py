@@ -315,6 +315,48 @@ def vq_backward(g_zq, g_loss, z_rows, codebook, idx, beta):
     return dz, dE
 
 
+def vq_finish_ema(sse, hist, N, K, D, beta):
+    """(loss, perplexity) of the EMA quantizer: loss = beta * mse, the commitment term alone (vqb_vq_finish_ema_f32)."""
+    out = torch.empty((2,), dtype=torch.float32, device=hist.device)
+    check(lib().vqb_vq_finish_ema_f32(sse.data_ptr(), hist.data_ptr(), N, K, D, float(beta),
+                                      out.data_ptr(), out.data_ptr() + 4, _stream()), "vq_finish_ema")
+    return out[0], out[1]
+
+
+def vq_commit_backward(g_zq, g_loss, z_rows, zq_rows, beta):
+    """dz (N,D) of the EMA quantizer from the forward's fp32 z_q rows (vqb_vq_commit_backward_f32); g_zq / g_loss may
+    be None."""
+    _require_cuda(z_rows, "z")
+    N, D = z_rows.shape
+    dz = torch.empty_like(z_rows)
+    gz = _f32c(g_zq) if g_zq is not None else None
+    gl = _f32c(g_loss).reshape(1) if g_loss is not None else None
+    check(lib().vqb_vq_commit_backward_f32(gz.data_ptr() if gz is not None else None,
+                                           gl.data_ptr() if gl is not None else None, z_rows.data_ptr(),
+                                           zq_rows.data_ptr(), N, D, float(beta), dz.data_ptr(), _stream()),
+          "vq_commit_backward")
+    return dz
+
+
+def vq_ema_update(z_rows, idx, hist, decay, eps, cluster_size, embed_sum, codebook):
+    """One EMA codebook update in place (vqb_vq_ema_update_f32): cluster_size (K,), embed_sum (K,D) and codebook
+    (K,D), fp32 contiguous CUDA tensors, from the rows z_rows (N,D) the VQ kernel quantized, their codes idx (N,) and
+    its hist (K,).  Version counters are the caller's to bump."""
+    _require_cuda(z_rows, "z")
+    N, D = z_rows.shape
+    K = codebook.shape[0]
+    for t in (cluster_size, embed_sum, codebook):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.device != z_rows.device:
+            raise RuntimeError("vq_ema_update: the EMA state and the codebook must be contiguous fp32 on z's device")
+    ws_bytes = lib().vqb_vq_ema_workspace_bytes(N, K, D)
+    ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=z_rows.device)
+    span = _Span(f"vq_ema N={N} K={K} D={D}")
+    check(lib().vqb_vq_ema_update_f32(z_rows.data_ptr(), idx.data_ptr(), hist.data_ptr(), N, K, D, float(decay),
+                                      float(eps), cluster_size.data_ptr(), embed_sum.data_ptr(), codebook.data_ptr(),
+                                      ws.data_ptr(), ws_bytes, _stream()), "vq_ema_update")
+    span.done()
+
+
 def onehot(idx, K):
     N = idx.numel()
     out = torch.empty((N, K), dtype=torch.float32, device=idx.device)
