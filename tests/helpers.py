@@ -1,6 +1,8 @@
 """Shared helpers of the parity tests (test infrastructure; may import oracle/)."""
 import json
 import os
+import subprocess
+import sys
 
 import numpy as np
 
@@ -61,3 +63,51 @@ def assert_zq_matches(g, zq_nchw, E=None):
         assert np.array_equal(zq_nchw, want, equal_nan=True)
     else:
         assert hashlib.sha256(zq_nchw.tobytes()).hexdigest() == str(g["z_q_sha256"])
+
+
+_CONV_PROFILE_SCRIPT = """
+import json, sys
+import torch
+from torch.profiler import ProfilerActivity, profile
+from vqvae_b200 import ops
+from vqvae_b200._lib import TF32
+out = []
+for B, Cin, H, W, Cout, k, s, p, t, il, ol, relu, skip in json.loads(sys.argv[1]):
+    oh, ow = ops.conv_out_hw(H, W, k, k, s, p, t)
+    x = torch.rand((B * Cin * H * W,), device="cuda")
+    w = ops.pack_conv_weight(torch.randn((Cin, Cout, k, k) if t else (Cout, Cin, k, k), device="cuda") * 0.05, t)
+    b = torch.rand((Cout,), device="cuda")
+    sk = torch.rand((B, oh, ow, Cout), device="cuda") if skip else None
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        ops.conv2d(x, w, b, B=B, Cin=Cin, H=H, W=W, Cout=Cout, kh=k, kw=k, stride=s, pad=p, transposed=t,
+                   in_layout=il, out_layout=ol, relu=relu, skip=sk, precision=TF32)
+        torch.cuda.synchronize()
+    out.append([e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA])
+print(json.dumps(out))
+"""
+
+
+def tf32_conv_kernels(cases):
+    """The CUDA kernel names torch.profiler records for one vqb_conv2d_f32 call in TF32 mode per case (B, Cin, H, W,
+    Cout, k, stride, pad, transposed, in_layout, out_layout, relu, skip), read in a fresh interpreter so that nothing
+    earlier tests did to the process's profiling state plays a part."""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    run = subprocess.run([sys.executable, "-c", _CONV_PROFILE_SCRIPT, json.dumps([list(c) for c in cases])], cwd=root,
+                         capture_output=True, text=True, timeout=600)
+    assert run.returncode == 0, run.stderr[-3000:]
+    return [[n for n in names if not n.startswith("Memcpy") and not n.startswith("Memset")]
+            for names in json.loads(run.stdout.strip().splitlines()[-1])]
+
+
+def tf32_conv_kernel(case):
+    """The kernel a TF32 vqb_conv2d_f32 call of `case` must run on, by name: the input conv (Cin = 3) its CUDA-core
+    kernel in every mode, the k4 s2 transposed output conv to <= 4 channels in NCHW the scatter-form wgmma kernel,
+    every other layer the wgmma convolution."""
+    from vqvae_b200._lib import NCHW
+    B, Cin, H, W, Cout, k, s, p, t, il, ol, relu, skip = case
+    if Cin == 3 and k == 4 and s == 2 and not t:
+        return "conv_in_k4s2_kernel"
+    if t and k == 4 and s == 2 and Cout <= 4 and ol == NCHW:
+        return "convt_scatter_kernel"
+    return "wgconv_kernel"

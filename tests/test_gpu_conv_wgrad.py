@@ -19,6 +19,14 @@ CASES = {
     "convt_k4s2_nchw_gout_bias": (1, 3, 32, 8, 8, 3, 4, 2, 1, NHWC, NCHW, True, 0),
     "ones_column_in_last_group": (0, 4, 3, 9, 9, 8, 3, 1, 1, NHWC, NHWC, True, 0),
     "conv1x1_no_bias": (0, 2, 16, 5, 5, 8, 1, 1, 0, NHWC, NHWC, False, 0),
+    # the position split under test: cfg3's input conv on 256 x 256 NCHW images, 32 768 positions staged element by
+    # element over hundreds of chunks; 3 * 7 * 9 = 189 positions, not a multiple of the 16-position k-step, so the
+    # last chunk is short; the output layer's bias as a second product over a 128 x 128 NCHW output gradient; the
+    # residual W1 at 64 x 64 latents over n * B = 4 images
+    "cfg3_input_k4s2_256": (0, 2, 3, 256, 256, 64, 4, 2, 1, NCHW, NHWC, True, 0),
+    "short_last_chunk_3x7x9": (0, 3, 16, 7, 9, 32, 3, 1, 1, NHWC, NHWC, True, 0),
+    "convt_k4s2_out_128_nchw_gout_bias": (1, 2, 64, 64, 64, 3, 4, 2, 1, NHWC, NCHW, True, 0),
+    "residual_w1_64x64_4_images": (0, 4, 128, 64, 64, 32, 3, 1, 1, NHWC, NHWC, False, 0),
 }
 
 

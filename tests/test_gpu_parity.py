@@ -11,7 +11,7 @@ import torch
 
 from oracle import cref
 from tests.helpers import (MODEL_CASES, VQ_CASES, assert_zq_matches, build_model, expected_zq, load_golden,
-                           make_vq_inputs, model_case_inputs)
+                           make_vq_inputs, model_case_inputs, tf32_conv_kernel, tf32_conv_kernels)
 
 pytestmark = pytest.mark.gpu
 
@@ -171,6 +171,23 @@ TC_CONV_CASES = [
     (5, 3, 16, 16, 64, 4, 2, 1, False, 0, 1, True, False),     # 20 warps: the last CTA is half empty
     (2, 3, 32, 32, 128, 4, 2, 1, False, 0, 1, True, False),    # Cout=128: four channel groups, full CTAs
     (3, 3, 6, 8, 64, 4, 2, 1, False, 0, 1, True, False),       # 36 pixels: one CTA of 4 warps, 4 live lanes in 2 of them
+    # The input gradients of the training backward: each the adjoint conv of a layer (modules._conv_dgrad: same weight,
+    # the transposed flag flipped), at 16 x 16 latents (two 16 x 8 tiles per image, a tile edge inside every image)
+    # and at ragged 12 x 20 latents (2 x 2 tiles per image, the right and bottom ones partly empty)
+    (3, 128, 16, 16, 32, 1, 1, 0, True, 1, 1, False, False),   # residual W2 adjoint: a transposed 1x1
+    (3, 128, 12, 20, 32, 1, 1, 0, True, 1, 1, False, False),
+    (3, 32, 16, 16, 128, 3, 1, 1, True, 1, 1, False, True),    # residual W1 adjoint: transposed k3 + skip
+    (3, 32, 12, 20, 128, 3, 1, 1, True, 1, 1, False, True),
+    (3, 64, 16, 16, 128, 1, 1, 0, True, 1, 1, False, False),   # pre-quantization conv adjoint
+    (3, 64, 12, 20, 128, 1, 1, 0, True, 1, 1, False, False),
+    (3, 128, 16, 16, 128, 3, 1, 1, True, 1, 1, False, False),  # encoder conv 4 adjoint
+    (3, 128, 12, 20, 128, 3, 1, 1, True, 1, 1, False, False),
+    (3, 128, 16, 16, 64, 3, 1, 1, False, 1, 1, False, False),  # decoder convT 0 adjoint
+    (3, 128, 12, 20, 64, 3, 1, 1, False, 1, 1, False, False),
+    (3, 64, 32, 32, 128, 4, 2, 1, False, 1, 1, False, False),  # decoder convT 2 adjoint: 32 x 32 -> 16 x 16
+    (3, 64, 24, 40, 128, 4, 2, 1, False, 1, 1, False, False),  # 24 x 40 -> 12 x 20
+    (2, 128, 64, 64, 64, 4, 2, 1, True, 1, 1, False, False),   # encoder conv 2 adjoint at 256 x 256 images: 64 x 64
+                                                               # -> 128 x 128, 256 CTAs, the two-CTA-per-SM ring
 ]
 
 
@@ -252,11 +269,22 @@ def test_tf32_full_size_properties_cfg2():
     print("cfg2 full size tf32: flips vs fp32 %.4f %%" % (100 * flips))
 
 
+@pytest.fixture(scope="module")
+def tc_kernels():
+    """case -> the CUDA kernels one TF32 call of each TC_CONV_CASES case ran, from torch.profiler."""
+    return dict(zip(TC_CONV_CASES, tf32_conv_kernels(TC_CONV_CASES)))
+
+
 @pytest.mark.parametrize("case", TC_CONV_CASES)
-def test_tc_conv_layers_vs_oracle(case):
+def test_tc_conv_layers_vs_oracle(case, tc_kernels):
+    """Within the TF32 tolerance of the oracle, and on the kernel the layer is meant to run: vqb_conv2d_f32 runs a
+    shape the wgmma launcher declines on the FFMA kernels, which pass every TF32 tolerance, so the profiler's kernel
+    names are checked (one launch is not enough: a stride-1 FFMA fallback is one launch too)."""
     from vqvae_b200._lib import TF32
     rng = np.random.RandomState(abs(hash(case)) % (2 ** 31))
     _conv_case(rng, *case, precision=TF32, atol=4e-3, rtol=2e-3)
+    names, want = tc_kernels[case], tf32_conv_kernel(case)
+    assert len(names) == 1 and want in names[0], (want, names)
 
 
 def test_tc_model_forward_tf32_tolerance():

@@ -16,6 +16,7 @@ from oracle.piecewise_port import PRIOR_LAYER_KEYS, gate, gated_layer, residual_
 from oracle.prior_train_port import fingerprint, leaf_params
 from oracle.vqvae_train_port import train_loss, vqvae_train_forward
 from oracle.weights import make_images, make_state_dict
+from tests.vqvae_masked import dec64, enc64, masked_relu, nchw64, res64, stack_masks
 
 pytestmark = pytest.mark.gpu
 
@@ -106,21 +107,22 @@ def test_notebook_walk_trains_every_parameter(name):
     assert vs_fused <= 1e-5
 
 
-def _module_cases(m, B, S):
-    """(name, module, input shape, fp64 function of (input, params dict)) for every VQ-VAE module alone."""
+def _module_cases(m, B, H, W):
+    """(name, module, input shape, fp64 function of (input, params dict)) for every VQ-VAE module alone, on H x W
+    images (H / 4 x W / 4 latents)."""
     e, d = "encoder.conv_stack.", "decoder.inverse_conv_stack."
     n = m.encoder.conv_stack[5].n_res_layers
     pq = m.pre_quantization_conv
-    H = S // 4
     h, emb = pq.in_channels, pq.out_channels
+    lat = (H // 4, W // 4)
     return [
-        ("encoder", m.encoder, (B, 3, S, S), lambda x, p: torch_port.encoder(x, p, n, p=e)),
-        ("decoder", m.decoder, (B, emb, H, H), lambda x, p: torch_port.decoder(x, p, n, p=d)),
-        ("pre_quantization_conv", pq, (B, h, H, H),
+        ("encoder", m.encoder, (B, 3, H, W), lambda x, p: torch_port.encoder(x, p, n, p=e)),
+        ("decoder", m.decoder, (B, emb) + lat, lambda x, p: torch_port.decoder(x, p, n, p=d)),
+        ("pre_quantization_conv", pq, (B, h) + lat,
          lambda x, p: F.conv2d(x, p["pre_quantization_conv.weight"], p["pre_quantization_conv.bias"])),
-        ("residual_layer", m.encoder.conv_stack[5].stack[0], (B, h, H, H),
+        ("residual_layer", m.encoder.conv_stack[5].stack[0], (B, h) + lat,
          lambda x, p: residual_layer(x, p[e + "5.stack.0.res_block.1.weight"], p[e + "5.stack.0.res_block.3.weight"])),
-        ("residual_stack", m.decoder.inverse_conv_stack[1], (B, h, H, H),
+        ("residual_stack", m.decoder.inverse_conv_stack[1], (B, h) + lat,
          lambda x, p: residual_stack(x, [(p[d + "1.stack.0.res_block.1.weight"],
                                           p[d + "1.stack.0.res_block.3.weight"])] * n)),
     ]
@@ -156,13 +158,19 @@ def _module_fp64(m, sd, fn, mod, x, G):
     return out
 
 
+# 32 x 32: every latent image inside one 128-pixel tile.  64 x 64: 16 x 16 latents, two tiles per image.  48 x 80:
+# 12 x 20 latents, ragged tiles on both axes and H != W in every call.
+IMAGE_SIZES = [(32, 32), (64, 64), (48, 80)]
+
+
 def test_every_vqvae_module_alone_matches_fp64_in_every_mode():
     import vqvae_b200
     c, sd, m, _ = _setup("cifar_default")
-    B, S = 4, 32
+    B = 4
     gen = torch.Generator().manual_seed(5)
     report = {}
-    for name, mod, shape, fn in _module_cases(m, B, S):
+    for (H, W), (name, mod, shape, fn) in [(hw, case) for hw in IMAGE_SIZES for case in _module_cases(m, B, *hw)]:
+        name = f"{name} {H}x{W}"
         x = torch.randn(shape, generator=gen).cuda()
         with torch.no_grad():
             mod.eval()
@@ -192,49 +200,6 @@ def test_every_vqvae_module_alone_matches_fp64_in_every_mode():
             assert max(per.values()) <= 1e-5, (name, per)
 
 
-def _res64(x, w1, w2, n, relu, final):
-    """residual.py with every ReLU given: n applications of one layer, then the stack's ReLU if `final`."""
-    for _ in range(n):
-        r = relu(x)
-        x = r + F.conv2d(relu(F.conv2d(r, w1, None, 1, 1)), w2)
-    return relu(x) if final else x
-
-
-def _enc64(x, p, n, relu, e="encoder.conv_stack."):
-    h = relu(F.conv2d(x, p[e + "0.weight"], p[e + "0.bias"], 2, 1))
-    h = relu(F.conv2d(h, p[e + "2.weight"], p[e + "2.bias"], 2, 1))
-    h = F.conv2d(h, p[e + "4.weight"], p[e + "4.bias"], 1, 1)
-    return _res64(h, p[e + "5.stack.0.res_block.1.weight"], p[e + "5.stack.0.res_block.3.weight"], n, relu, True)
-
-
-def _dec64(z, p, n, relu, d="decoder.inverse_conv_stack."):
-    h = F.conv_transpose2d(z, p[d + "0.weight"], p[d + "0.bias"], 1, 1)
-    h = _res64(h, p[d + "1.stack.0.res_block.1.weight"], p[d + "1.stack.0.res_block.3.weight"], n, relu, True)
-    h = relu(F.conv_transpose2d(h, p[d + "2.weight"], p[d + "2.bias"], 2, 1))
-    return F.conv_transpose2d(h, p[d + "4.weight"], p[d + "4.bias"], 2, 1)
-
-
-def _stack_masks(layer, r0, out, n, relu_out=True):
-    """The ReLU masks a TF32 stack backward reads, in the order the restatement applies its ReLUs: each application's
-    input r_i > 0 and m_i = relu(W1 (*) r_i) > 0, recomputed from r0 (NHWC) as _stack_backward does, then out > 0."""
-    from vqvae_b200 import ops
-    from vqvae_b200._lib import TF32
-    from vqvae_b200.modules import _packed
-    c1, c2 = layer.res_block[1], layer.res_block[3]
-    w1, w2 = _packed(c1.weight, ("f32", False)), _packed(c2.weight, ("f32", False))
-    B, H, W, C = r0.shape
-    masks, r = [], r0
-    for i in range(n):
-        m = ops.conv2d(r, w1, None, B=B, Cin=C, H=H, W=W, Cout=c1.out_channels, kh=3, kw=3, stride=1, pad=1,
-                       relu=True, precision=TF32)
-        masks += [r > 0, m > 0]
-        if i < n - 1:
-            r = ops.residual_layer(r, w1, w2, B=B, H=H, W=W, C=C, Cmid=c1.out_channels, relu_out=True, precision=TF32)
-    if relu_out:
-        masks.append(out > 0)
-    return masks
-
-
 def test_tf32_modules_match_fp64_at_the_gpu_masks():
     """Each VQ-VAE module alone in TF32 mode against fp64 autograd of the restatement whose ReLU masks are the ones
     the GPU's forward produced (the masks its backward reads): the TF32 error of the backward's own arithmetic, without
@@ -242,10 +207,10 @@ def test_tf32_modules_match_fp64_at_the_gpu_masks():
     import vqvae_b200
     from vqvae_b200 import ops
     c, sd, m, _ = _setup("cifar_default")
-    B, S, n = 4, 32, m.encoder.conv_stack[5].n_res_layers
+    B, n = 4, m.encoder.conv_stack[5].n_res_layers
     gen = torch.Generator().manual_seed(12)
     report = {}
-    for name, mod, shape, _ in _module_cases(m, B, S):
+    for (H, W), (name, mod, shape, _) in [(hw, case) for hw in IMAGE_SIZES for case in _module_cases(m, B, *hw)]:
         x = torch.randn(shape, generator=gen).cuda()
         with vqvae_b200.precision("tf32"):
             with torch.no_grad():
@@ -256,14 +221,14 @@ def test_tf32_modules_match_fp64_at_the_gpu_masks():
                     acts = {}
                     mod._forward_nhwc(x, False, acts)
                     a1, a2, a3, e_out = acts["enc"]
-                    masks = [a1 > 0, a2 > 0] + _stack_masks(mod.conv_stack[5].stack[0], a3, e_out, n)
-                    fn = lambda t, p, relu: _enc64(t, p, n, relu)                                  # noqa: E731
+                    masks = [a1 > 0, a2 > 0] + stack_masks(mod.conv_stack[5].stack[0], a3, e_out, n)
+                    fn = lambda t, p, relu: enc64(t, p, n, relu)                                   # noqa: E731
                 elif name == "decoder":
                     acts = {}
-                    mod._forward_from_nhwc(ops.nchw_to_nhwc(x), B, S // 4, S // 4, acts=acts)
+                    mod._forward_from_nhwc(ops.nchw_to_nhwc(x), B, H // 4, W // 4, acts=acts)
                     d1, d_out, d2 = acts["dec"]
-                    masks = _stack_masks(mod.inverse_conv_stack[1].stack[0], d1, d_out, n) + [d2 > 0]
-                    fn = lambda t, p, relu: _dec64(t, p, n, relu)                                  # noqa: E731
+                    masks = stack_masks(mod.inverse_conv_stack[1].stack[0], d1, d_out, n) + [d2 > 0]
+                    fn = lambda t, p, relu: dec64(t, p, n, relu)                                   # noqa: E731
                 elif name == "pre_quantization_conv":
                     masks = []
                     fn = lambda t, p, relu: F.conv2d(t, p["pre_quantization_conv.weight"],        # noqa: E731
@@ -272,19 +237,18 @@ def test_tf32_modules_match_fp64_at_the_gpu_masks():
                     layer = mod if name == "residual_layer" else mod.stack[0]
                     pre = _module_prefix(m, layer) + ".res_block."
                     out = ops.nchw_to_nhwc(mod(x.clone()))
-                    masks = _stack_masks(layer, ops.nchw_to_nhwc(torch.relu(x)), out, 1 if name == "residual_layer"
-                                         else n, relu_out=name != "residual_layer")
+                    masks = stack_masks(layer, ops.nchw_to_nhwc(torch.relu(x)), out, 1 if name == "residual_layer"
+                                        else n, relu_out=name != "residual_layer")
                     k = 1 if name == "residual_layer" else n
-                    fn = lambda t, p, relu, pre=pre, k=k, f=name != "residual_layer": _res64(     # noqa: E731
+                    fn = lambda t, p, relu, pre=pre, k=k, f=name != "residual_layer": res64(      # noqa: E731
                         t, p[pre + "1.weight"], p[pre + "3.weight"], k, relu, f)
             _, got = _run_module(mod, x, G)
-        it = iter([t.permute(0, 3, 1, 2).double().cpu() for t in masks])       # every mask is NHWC
-        relu = lambda t: t * next(it)                                                               # noqa: E731
+        relu, done = masked_relu(nchw64(masks))                    # every mask is NHWC
         fn64 = lambda t, p: fn(t, p, relu)                                                          # noqa: E731
         want = _module_fp64(m, sd, fn64, mod, x, G)
-        assert next(it, None) is None, name                         # every mask used once
-        report[name] = {k: _rel(got[k], want[k]) for k in want}
-        print(f"{name} tf32 at the GPU's masks:", " ".join(f"{k}={v:.1e}" for k, v in report[name].items()))
+        assert done(), (name, H, W)                                 # every mask used once
+        report[(name, H, W)] = per = {k: _rel(got[k], want[k]) for k in want}
+        print(f"{name} {H}x{W} tf32 at the GPU's masks:", " ".join(f"{k}={v:.1e}" for k, v in per.items()))
     for name, per in report.items():
         assert per["input"] <= 5e-3, (name, per)
         assert max(per.values()) <= 1e-2, (name, per)
@@ -459,7 +423,7 @@ def test_eval_and_no_grad_calls_keep_their_launches():
         out = mod(*[a.clone() for a in args])
         return ops.launch_count() - n0, out
 
-    for name, mod, shape, _ in _module_cases(m, 4, 32):
+    for name, mod, shape, _ in _module_cases(m, 4, 32, 32):
         xi = torch.randn(shape, device="cuda")
         with torch.no_grad():
             count(mod, xi)                       # packs the weights
@@ -546,7 +510,7 @@ def test_launch_counts_per_module(mode):
     from vqvae_b200 import ops
     c, sd, m, x = _setup("cifar_default")
     layer, x_v, x_h, h = _gated("B", 3, True, 64, 6, 11)
-    cases = [(name, mod, (torch.randn(shape, device="cuda"),)) for name, mod, shape, _ in _module_cases(m, 4, 32)]
+    cases = [(name, mod, (torch.randn(shape, device="cuda"),)) for name, mod, shape, _ in _module_cases(m, 4, 32, 32)]
     cases += [("empty_stack", ResidualStack(128, 128, 32, 0).cuda().train(), (torch.randn((4, 128, 8, 8), device="cuda"),)),
               ("gated_layer", layer, (x_v, x_h, h)),
               ("gated_activation", GatedActivation(), (torch.randn((2, 64, 6, 6), device="cuda"),))]

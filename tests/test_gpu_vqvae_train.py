@@ -169,17 +169,31 @@ def test_eval_mode_with_grad_enabled_is_unchanged():
     assert all(torch.equal(a, b) for a, b in zip(out, ref))
 
 
-def test_conv_gradients_are_deterministic_eagerly_and_in_a_cuda_graph():
-    c, sd, m, x = _setup("cifar_default")
+def _two_eager_steps(name, codebook_bar):
+    """Two training steps of a MODEL_CASES case -> (model, image, the first step's gradients); the conv gradients of
+    the two are bitwise equal, the codebook's (float atomics) within codebook_bar of its max |g|."""
+    c, sd, m, x = _setup(name)
     xc = x.cuda()
     runs = []
     for _ in range(2):
         _step(m, xc)
         runs.append(_grads(m))
     emb = "vector_quantization.embedding.weight"
-    assert all(torch.equal(runs[0][k], runs[1][k]) for k in runs[0] if k != emb)
+    assert all(torch.equal(runs[0][k], runs[1][k]) for k in runs[0] if k != emb), name
     e0, e1 = runs[0][emb], runs[1][emb]
-    assert float((e0 - e1).abs().max()) <= 1e-6 * float(e0.abs().max())
+    assert float((e0 - e1).abs().max()) <= codebook_bar * float(e0.abs().max()), name
+    return m, xc, runs[0]
+
+
+def test_conv_gradients_are_deterministic_eagerly_and_in_a_cuda_graph():
+    """Two eager steps give bitwise-equal conv gradients, at cifar_default and at cfg3_s256 (B = 2 at 256 x 256: the
+    multi-wave adjoint grids and the input conv's weight gradient over 32 768 positions); a CUDA-graph replay of the
+    cifar_default step gives them too."""
+    # the codebook gradient is summed with float atomics: cfg3_s256 adds 8192 rows into 1024 codes (1.2e-6 of max |g|
+    # between two steps, measured on an H100)
+    _two_eager_steps("cfg3_s256", 1e-5)
+    m, xc, first = _two_eager_steps("cifar_default", 1e-6)
+    emb = "vector_quantization.embedding.weight"
 
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -195,7 +209,7 @@ def test_conv_gradients_are_deterministic_eagerly_and_in_a_cuda_graph():
         p.grad.fill_(float("nan"))
     graph.replay()
     torch.cuda.synchronize()
-    assert all(torch.equal(p.grad, runs[0][k]) for k, p in m.named_parameters() if k != emb)
+    assert all(torch.equal(p.grad, first[k]) for k, p in m.named_parameters() if k != emb)
 
 
 @pytest.mark.parametrize("mode,bar", [("fp32", 1e-4), ("tf32", 1e-2)])

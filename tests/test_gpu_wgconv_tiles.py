@@ -1,9 +1,10 @@
 """Tile edges of the wgmma convolution (wgconv.cu), where each k-step's A box is the tile's input shifted by a tap and
 zero filled outside the image: taps that reach into neighbouring tiles on all four sides, ragged right / bottom tiles
 with stride-2 taps, several small images per tile (zero padding between images and past the batch), chained residual
-applications that read the previous application's output back, and the widest shapes the launcher takes (8 chunks,
-N = 256).  The model's layers reach none of these.  Held to the C oracle at the TF32 / bf16 tolerances of the existing
-layer tests.  Needs an H100 (``-m gpu``).
+applications that read the previous application's output back, the widest shapes the launcher takes (8 chunks,
+N = 256), and the training backward's adjoint convs over interior tiles.  The model's forward layers reach none of
+these.  Held to the C oracle at the TF32 / bf16 tolerances of the existing layer tests; every TF32 case is checked by
+kernel name, through the profiler, to run on the wgmma kernel.  Needs an H100 (``-m gpu``).
 """
 import numpy as np
 import pytest
@@ -42,11 +43,28 @@ TF32_CASES = [
     (6, 64, 4, 4, 64, 3, 1, False),       # 8 images per tile, 6 in the batch
     (5, 32, 6, 6, 32, 4, 2, False),       # stride 2, 3 x 3 outputs, 8 images per tile
     (1, 256, 16, 16, 256, 3, 1, False),   # 8 chunks x 9 taps, N = 256
+    # adjoint convs of the training backward (modules._conv_dgrad) with an interior tile: 3 x 3 tiles of 16 x 8
+    (2, 32, 24, 40, 128, 3, 1, True),     # residual W1's adjoint: transposed k3, 1 chunk, N = 128
+    (2, 128, 24, 40, 128, 3, 1, True),    # encoder conv 4's adjoint: transposed k3, 4 chunks
+    (2, 128, 20, 36, 32, 1, 1, True),     # residual W2's adjoint: transposed 1x1 over 3 x 3 tiles, ragged on both axes
 ]
 
 
+def _pad(k):
+    return 0 if k == 1 else 1
+
+
+@pytest.fixture(scope="module")
+def tf32_kernels():
+    """case -> the CUDA kernels one call of each TF32_CASES case ran, from torch.profiler."""
+    from tests.helpers import tf32_conv_kernels
+    from vqvae_b200._lib import NHWC
+    calls = [(B, Cin, H, W, Cout, k, s, _pad(k), t, NHWC, NHWC, True, False) for B, Cin, H, W, Cout, k, s, t in TF32_CASES]
+    return dict(zip(TF32_CASES, tf32_conv_kernels(calls)))
+
+
 @pytest.mark.parametrize("case", TF32_CASES)
-def test_tf32_tile_edge_layers_vs_oracle(case):
+def test_tf32_tile_edge_layers_vs_oracle(case, tf32_kernels):
     from vqvae_b200 import ops
     from vqvae_b200._lib import NHWC, TF32
     B, Cin, H, W, Cout, k, stride, transposed = case
@@ -54,10 +72,12 @@ def test_tf32_tile_edge_layers_vs_oracle(case):
     wp = ops.pack_conv_weight(_cuda(w), transposed)
     l0 = ops.launch_count()
     y = ops.conv2d(_cuda(x.transpose(0, 2, 3, 1)), wp, _cuda(b), B=B, Cin=Cin,
-                   H=H, W=W, Cout=Cout, kh=k, kw=k, stride=stride, pad=1, transposed=transposed, in_layout=NHWC,
+                   H=H, W=W, Cout=Cout, kh=k, kw=k, stride=stride, pad=_pad(k), transposed=transposed, in_layout=NHWC,
                    out_layout=NHWC, relu=True, precision=TF32)
-    assert ops.launch_count() - l0 == 1           # one wgmma launch, not the CUDA-core kernels
+    assert ops.launch_count() - l0 == 1
     np.testing.assert_allclose(y.cpu().numpy().transpose(0, 3, 1, 2), ref, atol=4e-3, rtol=2e-3)
+    names = tf32_kernels[case]                    # the wgmma kernel, not the CUDA-core fallback
+    assert len(names) == 1 and "wgconv_kernel" in names[0], names
 
 
 BF16_CASES = [
