@@ -278,6 +278,21 @@ int vqb_vq_ema_update_f32(const float *z, const int64_t *idx, const int32_t *his
                           int D, float decay, float eps, float *cluster_size, float *embed_sum,
                           float *codebook, void *workspace, size_t workspace_bytes, void *stream);
 
+/* Dead-code restart, run after vqb_vq_ema_update_f32 on the same rows z (N,D) fp32 and state, with uniforms u (N)
+ * fp32 in [0, 1) and a threshold t:
+ *   dead codes k_0 < k_1 < ... < k_{M-1}: cluster_size N_k < t (strict; a NaN N_k is not dead)
+ *   rows r_0, r_1, ...: the rows ordered by (u_i, i) ascending (uniform sampling without replacement)
+ *   for j < R = min(M, N):  codebook e_{k_j} <- z_{r_j},  embed_sum m_{k_j} <- fl(t z_{r_j}),  N_{k_j} <- t
+ *   *n_restarted (int32, device) <- R;  every other element keeps its bits.
+ * Twelve launches, no float atomics, no host synchronisation; with no dead code every kernel after the first returns
+ * at once.  NULL pointers, N, K or D <= 0, t not finite or <= 0: VQB_ERR_BAD_ARG; D % 4 != 0, K > 8192 or
+ * N > 2^32 - 1: VQB_ERR_UNSUPPORTED; a workspace shorter than vqb_vq_ema_restart_workspace_bytes(N,K) (0 for a shape
+ * it refuses): VQB_ERR_WORKSPACE; all before any launch.  z, embed_sum, codebook and the workspace 16-byte aligned. */
+size_t vqb_vq_ema_restart_workspace_bytes(int64_t N, int K);
+int vqb_vq_ema_restart_f32(const float *z, const float *u, int64_t N, int K, int D, float threshold,
+                           float *cluster_size, float *embed_sum, float *codebook, int32_t *n_restarted,
+                           void *workspace, size_t workspace_bytes, void *stream);
+
 /* Backward of the EMA quantizer, whose loss is the commitment term alone (the codebook gets no gradient):
  *   dz (N,D) = g_zq + g_loss * 2 beta/(N D) * (z - zq)
  * zq = the forward's fp32 z_q rows (not the codebook, which the update has overwritten).  g_zq / g_loss may be

@@ -34,6 +34,7 @@ def load_checkpoint(path, device="cuda"):
         with torch.no_grad():
             vq.ema_cluster_size.copy_(ema["cluster_size"])
             vq.ema_embed_sum.copy_(ema["embed_sum"])
+        vq.dead_code_threshold = ema.get("dead_code_threshold")
     model = model.to(device).eval()
     if torch.device(device).type == "cuda":
         with torch.cuda.device(torch.device(device)):
@@ -44,8 +45,8 @@ def load_checkpoint(path, device="cuda"):
 def save_checkpoint(model, results, hyperparameters, path):
     """Write the reference's checkpoint format (utils.py:106-115) so its notebook / load_model can read the file.
     A model with an EMA codebook (``ema_decay``) keeps ``model`` to the reference's keys, so that ``load_model`` still
-    loads it strictly, and adds ``"vq_ema": {decay, eps, cluster_size, embed_sum}``; load_checkpoint rebuilds the
-    EMA model from it."""
+    loads it strictly, and adds ``"vq_ema": {decay, eps, cluster_size, embed_sum}``, plus ``dead_code_threshold`` when
+    restarts are on; load_checkpoint rebuilds the EMA model from it."""
     sd = model.state_dict()
     data = {"model": sd, "results": results, "hyperparameters": hyperparameters}
     vq = model.vector_quantization
@@ -55,4 +56,6 @@ def save_checkpoint(model, results, hyperparameters, path):
             del sd[prefix + k]
         data["vq_ema"] = {"decay": vq.decay, "eps": vq.eps, "cluster_size": vq.ema_cluster_size.detach().cpu(),
                           "embed_sum": vq.ema_embed_sum.detach().cpu()}
+        if vq.dead_code_threshold is not None:
+            data["vq_ema"]["dead_code_threshold"] = vq.dead_code_threshold
     torch.save(data, path)

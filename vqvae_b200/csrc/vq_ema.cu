@@ -1,5 +1,6 @@
 // vq_ema.cu -- exponential-moving-average codebook update of a VectorQuantizer (van den Oord et al. 2017, app. A.1),
-// with per-code row sums in a fixed order, and the backward / loss finisher of the EMA model (commitment term only).
+// with per-code row sums in a fixed order, the backward / loss finisher of the EMA model (commitment term only), and
+// the dead-code restarts that may follow an update (see "dead-code restarts" below).
 //
 // One update, from the rows z (N, D) the VQ kernel quantized, their codes idx (clamped to [0, K-1]) and its hist:
 //   N_k <- g N_k + (1-g) hist_k,   m_k <- g m_k + (1-g) s_k,   n = sum_k N_k,
@@ -288,6 +289,204 @@ int sm_count() {
     return sms;
 }
 
+// ---- dead-code restarts (vqb_vq_ema_restart_f32), run after an update --------------------------------------------
+// From the rows z (N, D) the update consumed, uniforms u (N) in [0, 1) and a threshold t:
+//   dead codes k_0 < k_1 < ... < k_{M-1}: N_k < t (strict, so a NaN N_k is not dead)
+//   rows r_0, r_1, ...: the rows ordered by (u_i, i) ascending -- uniform sampling without replacement
+//   for j < R = min(M, N):  e_{k_j} <- z_{r_j},  m_{k_j} <- fl(t z_{r_j}),  N_{k_j} <- t;   *n_restarted = R
+// Row i's key is (bits of u_i) << 32 | i.  For u >= 0 the bit order is the value order, and the row index makes every
+// key unique, so the R rows are the R smallest keys and their order is the keys' order.
+//
+// Twelve launches, no host synchronisation, no float atomics; every kernel after the first returns at once when R = 0:
+//   1      rs_compact  one CTA: the dead flags in code order -> dead list, M, *n_restarted; counts zeroed
+//   2..9   rs_digits   pass p: counts of digit p (8 bits, from the top) over the keys whose digits 0..p-1 are those of
+//                      T, the R-th smallest key (every CTA derives them from passes 0..p-1); integer atomics only
+//   10     rs_collect  the R keys <= T into a list (integer atomics pick the slots: the set is fixed, not the order)
+//   11     rs_rank     each listed key's rank j among the R: the count of listed keys below it, one CTA per (256 keys,
+//                      chunk of RS_RANK_CHUNK keys), the chunk counts added with integer atomics -- a sort, R^2 compares
+//                      spread over the GPU
+//   12     rs_assign   one thread per (listed key, float4 column): the copies into e, m and N of code k_j
+constexpr int RS_MAX_K = 8192;                       // one CTA compacts the flags (8 per thread); R^2 rank compares
+constexpr long long RS_MAX_N = 0xFFFFFFFFLL;         // the row index fills the key's low 32 bits; counts fit unsigned
+constexpr int RS_THREADS = 256, RS_PASSES = 8, RS_COMPACT_THREADS = 1024, RS_RANK_CHUNK = 1024;
+
+struct RestartPlan {
+    size_t off_meta, off_dead, off_digits, off_keys, off_rank, total;
+};
+
+RestartPlan restart_plan(int K) {
+    RestartPlan p{};
+    size_t o = 0;
+    p.off_meta = o;   o = align16(o + 2 * sizeof(int));                                  // M, the collect counter
+    p.off_dead = o;   o = align16(o + sizeof(int) * (size_t)K);
+    p.off_digits = o; o = align16(o + sizeof(unsigned) * RS_PASSES * 256);
+    p.off_keys = o;   o = align16(o + sizeof(unsigned long long) * (size_t)K);
+    p.off_rank = o;   o = align16(o + sizeof(int) * (size_t)K);
+    p.total = o;
+    return p;
+}
+
+__device__ __forceinline__ unsigned long long rs_key(const float *u, long long i) {
+    return ((unsigned long long)__float_as_uint(__ldg(u + i)) << 32) | (unsigned long long)i;
+}
+
+__device__ __forceinline__ long long rs_count(const int *meta, long long N) {
+    return (long long)meta[0] < N ? (long long)meta[0] : N;
+}
+
+// The digits 0..npass-1 of T, the R-th smallest key, from the counts of those passes (every thread of the CTA calls
+// it; blockDim.x == 256, one digit per thread).  After all eight passes this is T itself.
+__device__ unsigned long long rs_prefix(const unsigned *digits, int npass, long long R) {
+    __shared__ unsigned long long s_prefix;
+    __shared__ long long s_rank;
+    __shared__ unsigned s_warp[RS_THREADS / 32];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    if (t == 0) { s_prefix = 0ULL; s_rank = R; }
+    __syncthreads();
+    for (int q = 0; q < npass; ++q) {
+        const long long rank = s_rank;              // 1-based rank of T among the keys matching the digits so far
+        const unsigned c = digits[q * 256 + t];
+        unsigned incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        for (int w = 0; w < warp; ++w) incl += s_warp[w];
+        const long long before = (long long)incl - c;
+        if (before < rank && rank <= (long long)incl) {    // exactly one digit holds the rank
+            s_prefix |= (unsigned long long)t << (56 - 8 * q);
+            s_rank = rank - before;
+        }
+        __syncthreads();
+    }
+    return s_prefix;
+}
+
+__global__ void __launch_bounds__(RS_COMPACT_THREADS) rs_compact(const float *__restrict__ cluster_size, int K,
+                                                                 long long N, float thr, int *__restrict__ meta,
+                                                                 int *__restrict__ dead, unsigned *__restrict__ digits,
+                                                                 int *__restrict__ rank, int *__restrict__ n_restarted) {
+    __shared__ int s_warp[RS_COMPACT_THREADS / 32];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    for (int i = t; i < RS_PASSES * 256; i += RS_COMPACT_THREADS) digits[i] = 0u;
+    for (int i = t; i < K; i += RS_COMPACT_THREADS) rank[i] = 0;
+    if (t == 0) meta[1] = 0;
+    const int per = (K + RS_COMPACT_THREADS - 1) / RS_COMPACT_THREADS;    // <= 8 codes per thread, in code order
+    const int k0 = t * per;
+    unsigned flags = 0u;
+    for (int q = 0; q < per; ++q)
+        if (k0 + q < K && cluster_size[k0 + q] < thr) flags |= 1u << q;
+    const int cnt = __popc(flags);
+    int incl = cnt;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    int pos = incl - cnt, M = 0;
+    for (int w = 0; w < RS_COMPACT_THREADS / 32; ++w) {
+        if (w < warp) pos += s_warp[w];
+        M += s_warp[w];
+    }
+    for (int q = 0; q < per; ++q)
+        if (flags >> q & 1u) dead[pos++] = k0 + q;
+    if (t == 0) {
+        meta[0] = M;
+        n_restarted[0] = (int)((long long)M < N ? (long long)M : N);
+    }
+}
+
+__global__ void __launch_bounds__(RS_THREADS) rs_digits(const float *__restrict__ u, long long N,
+                                                        const int *__restrict__ meta, unsigned *digits, int pass) {
+    __shared__ unsigned h[256];
+    const long long R = rs_count(meta, N);
+    if (R == 0) return;
+    const unsigned long long prefix = rs_prefix(digits, pass, R);
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    h[t] = 0u;
+    __syncthreads();
+    const int shift = 56 - 8 * pass;
+    const unsigned long long high = pass == 0 ? 0ULL : ~0ULL << (shift + 8);
+    for (long long i0 = (long long)blockIdx.x * RS_THREADS + warp * 32; i0 < N; i0 += (long long)gridDim.x * RS_THREADS) {
+        const long long i = i0 + lane;
+        int d = -1;
+        if (i < N) {
+            const unsigned long long key = rs_key(u, i);
+            if ((key & high) == prefix) d = (int)(key >> shift) & 255;
+        }
+        const unsigned peers = __match_any_sync(0xffffffffu, d);
+        if (d >= 0 && lane == __ffs(peers) - 1) atomicAdd(h + d, (unsigned)__popc(peers));
+    }
+    __syncthreads();
+    if (h[t]) atomicAdd(digits + pass * 256 + t, h[t]);
+}
+
+__global__ void __launch_bounds__(RS_THREADS) rs_collect(const float *__restrict__ u, long long N, int *meta,
+                                                         const unsigned *__restrict__ digits,
+                                                         unsigned long long *__restrict__ keys) {
+    const long long R = rs_count(meta, N);
+    if (R == 0) return;
+    const unsigned long long T = rs_prefix(digits, RS_PASSES, R);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned *counter = reinterpret_cast<unsigned *>(meta + 1);
+    for (long long i0 = (long long)blockIdx.x * RS_THREADS + warp * 32; i0 < N; i0 += (long long)gridDim.x * RS_THREADS) {
+        const long long i = i0 + lane;
+        const unsigned long long key = i < N ? rs_key(u, i) : ~0ULL;
+        const bool take = i < N && key <= T;
+        const unsigned b = __ballot_sync(0xffffffffu, take);
+        unsigned slot = 0u;
+        if (lane == 0 && b) slot = atomicAdd(counter, (unsigned)__popc(b));
+        slot = __shfl_sync(0xffffffffu, slot, 0);
+        if (take) keys[slot + __popc(b & ((1u << lane) - 1u))] = key;
+    }
+}
+
+// rank[q] += the number of listed keys in chunk blockIdx.y below key q (keys are unique: the ranks are 0..R-1)
+__global__ void __launch_bounds__(RS_THREADS) rs_rank(const int *__restrict__ meta, long long N,
+                                                      const unsigned long long *__restrict__ keys, int *rank) {
+    __shared__ unsigned long long s_key[RS_RANK_CHUNK];
+    const long long R = rs_count(meta, N);
+    const long long c0 = (long long)blockIdx.y * RS_RANK_CHUNK, q0 = (long long)blockIdx.x * RS_THREADS;
+    if (c0 >= R || q0 >= R) return;
+    const int cn = R - c0 < RS_RANK_CHUNK ? (int)(R - c0) : RS_RANK_CHUNK;
+    for (int i = threadIdx.x; i < cn; i += RS_THREADS) s_key[i] = keys[c0 + i];
+    __syncthreads();
+    const long long q = q0 + threadIdx.x;
+    if (q >= R) return;
+    const unsigned long long key = keys[q];
+    int below = 0;
+#pragma unroll 8
+    for (int i = 0; i < cn; ++i) below += s_key[i] < key;
+    if (below) atomicAdd(rank + q, below);
+}
+
+__global__ void __launch_bounds__(RS_THREADS) rs_assign(const float *__restrict__ z, long long N, int D, float thr,
+                                                        const int *__restrict__ meta, const int *__restrict__ dead,
+                                                        const unsigned long long *__restrict__ keys,
+                                                        const int *__restrict__ rank, float *__restrict__ cluster_size,
+                                                        float *__restrict__ embed_sum, float *__restrict__ codebook) {
+    const long long R = rs_count(meta, N);
+    if (R == 0) return;
+    const int d4 = D / 4;
+    const float4 *z4 = reinterpret_cast<const float4 *>(z);
+    for (long long g = (long long)blockIdx.x * RS_THREADS + threadIdx.x; g < R * d4; g += (long long)gridDim.x * RS_THREADS) {
+        const long long q = g / d4;
+        const int c = (int)(g - q * d4);
+        const long long k = dead[rank[q]];
+        const long long r = (long long)(keys[q] & 0xFFFFFFFFULL);
+        const float4 v = __ldg(z4 + r * d4 + c);
+        reinterpret_cast<float4 *>(codebook)[k * d4 + c] = v;
+        reinterpret_cast<float4 *>(embed_sum)[k * d4 + c] =
+            make_float4(__fmul_rn(thr, v.x), __fmul_rn(thr, v.y), __fmul_rn(thr, v.z), __fmul_rn(thr, v.w));
+        if (c == 0) cluster_size[k] = thr;
+    }
+}
+
 }  // namespace
 
 extern "C" size_t vqb_vq_ema_workspace_bytes(int64_t N, int K, int D) {
@@ -327,6 +526,50 @@ extern "C" int vqb_vq_ema_update_f32(const float *z, const int64_t *idx, const i
     ema_finish<<<(unsigned)fin, EMA_THREADS, 0, s>>>(K, D, p.nchunks, base, part, nnew, decay, eps, cluster_size,
                                                      embed_sum, codebook);
     VQB_COUNT_LAUNCH(5);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_vq_ema_restart_workspace_bytes(int64_t N, int K) {
+    if (N <= 0 || K <= 0 || K > RS_MAX_K || N > RS_MAX_N) return 0;
+    return restart_plan(K).total;
+}
+
+extern "C" int vqb_vq_ema_restart_f32(const float *z, const float *u, int64_t N, int K, int D, float threshold,
+                                      float *cluster_size, float *embed_sum, float *codebook, int32_t *n_restarted,
+                                      void *workspace, size_t workspace_bytes, void *stream) {
+    if (!z || !u || !cluster_size || !embed_sum || !codebook || !n_restarted || !workspace) return VQB_ERR_BAD_ARG;
+    if (N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
+    if (!(threshold > 0.f && threshold <= 3.4028235e38f)) return VQB_ERR_BAD_ARG;
+    if (D % 4 != 0 || K > RS_MAX_K || N > RS_MAX_N) return VQB_ERR_UNSUPPORTED;
+    const RestartPlan p = restart_plan(K);
+    if (workspace_bytes < p.total) return VQB_ERR_WORKSPACE;
+    const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(embed_sum) |
+                         reinterpret_cast<uintptr_t>(codebook) | reinterpret_cast<uintptr_t>(workspace);
+    if (al & 15) return VQB_ERR_ALIGNMENT;
+    const long long rmax = (long long)K < N ? (long long)K : N;
+    char *ws = static_cast<char *>(workspace);
+    int *meta = reinterpret_cast<int *>(ws + p.off_meta);
+    int *dead = reinterpret_cast<int *>(ws + p.off_dead);
+    unsigned *digits = reinterpret_cast<unsigned *>(ws + p.off_digits);
+    unsigned long long *keys = reinterpret_cast<unsigned long long *>(ws + p.off_keys);
+    int *rank = reinterpret_cast<int *>(ws + p.off_rank);
+    cudaStream_t s = (cudaStream_t)stream;
+    const int sms = sm_count();
+    long long scan = (N + RS_THREADS - 1) / RS_THREADS;
+    if (scan > 4LL * sms) scan = 4LL * sms;
+    long long asg = (rmax * (D / 4) + RS_THREADS - 1) / RS_THREADS;
+    if (asg > 4LL * sms) asg = 4LL * sms;
+    rs_compact<<<1, RS_COMPACT_THREADS, 0, s>>>(cluster_size, K, N, threshold, meta, dead, digits, rank,
+                                                 n_restarted);
+    for (int pass = 0; pass < RS_PASSES; ++pass)
+        rs_digits<<<(unsigned)scan, RS_THREADS, 0, s>>>(u, N, meta, digits, pass);
+    rs_collect<<<(unsigned)scan, RS_THREADS, 0, s>>>(u, N, meta, digits, keys);
+    const dim3 rank_grid((unsigned)((rmax + RS_THREADS - 1) / RS_THREADS),
+                         (unsigned)((rmax + RS_RANK_CHUNK - 1) / RS_RANK_CHUNK));
+    rs_rank<<<rank_grid, RS_THREADS, 0, s>>>(meta, N, keys, rank);
+    rs_assign<<<(unsigned)asg, RS_THREADS, 0, s>>>(z, N, D, threshold, meta, dead, keys, rank, cluster_size,
+                                                   embed_sum, codebook);
+    VQB_COUNT_LAUNCH(4 + RS_PASSES);
     return vqb_cuda_status(cudaGetLastError());
 }
 

@@ -24,6 +24,7 @@ Reference semantics reproduced on purpose (SURVEY 3.3):
 """
 import contextlib
 import math
+import numbers
 
 import torch
 import torch.nn as nn
@@ -495,7 +496,14 @@ class VectorQuantizer(nn.Module):
     each code had been assigned one vector equal to itself (N = 1, m = e) -- and every differentiable call in training
     mode (grad enabled, z requiring grad) updates N, m and the codebook in place (vqb_vq_ema_update_f32):
     N <- decay N + (1-decay) n_k,  m <- decay m + (1-decay) s_k,  e = m / ((N + eps) / (n + K eps) * n).  The loss is
-    the commitment term beta * mse((sg[z_q], z)) on every path."""
+    the commitment term beta * mse((sg[z_q], z)) on every path.
+
+    ``dead_code_threshold`` (attribute, default None = off; EMA codebooks of at most 8192 codes): after each update,
+    every code whose N fell below it moves onto a row of the batch just quantized, drawn uniformly without replacement
+    from one ``torch.rand`` per update (vqb_vq_ema_restart_f32): e <- z_row, m <- t z_row, N <- t.  ``last_restarts``,
+    a device int32 (1,) tensor written in place, holds how many codes the last update restarted."""
+
+    _MAX_RESTART_CODES = 8192
 
     def __init__(self, n_e, e_dim, beta, *, decay=None, eps=1e-5):
         _check_ema(decay, eps)
@@ -505,14 +513,37 @@ class VectorQuantizer(nn.Module):
         self.beta = beta
         self.decay = None if decay is None else float(decay)
         self.eps = float(eps)
+        self._dead_code_threshold = None
         self.embedding = nn.Embedding(self.n_e, self.e_dim)
         self.embedding.weight.data.uniform_(-1.0 / self.n_e, 1.0 / self.n_e)
         if self.decay is not None:
             self.embedding.weight.requires_grad_(False)
             self.register_buffer("ema_cluster_size", torch.ones(self.n_e))
             self.register_buffer("ema_embed_sum", self.embedding.weight.detach().clone())
+            self.register_buffer("last_restarts", torch.zeros(1, dtype=torch.int32), persistent=False)
+        else:
+            self.last_restarts = None
 
     _EMA_KEYS = ("ema_cluster_size", "ema_embed_sum")
+
+    @property
+    def dead_code_threshold(self):
+        """None (no restarts) or the cluster size t below which an EMA code is restarted after each update."""
+        return self._dead_code_threshold
+
+    @dead_code_threshold.setter
+    def dead_code_threshold(self, value):
+        if value is None:
+            self._dead_code_threshold = None
+            return
+        if isinstance(value, bool) or not isinstance(value, numbers.Real) or not math.isfinite(value) or value <= 0:
+            raise ValueError(f"dead_code_threshold must be None or a finite number > 0, got {value!r}")
+        if self.decay is None:
+            raise ValueError("dead_code_threshold needs an EMA codebook (decay=...): the gradient-trained codebook "
+                             "has no cluster sizes")
+        if self.n_e > self._MAX_RESTART_CODES:
+            raise ValueError(f"dead_code_threshold supports at most {self._MAX_RESTART_CODES} codes, not {self.n_e}")
+        self._dead_code_threshold = float(value)
 
     def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
                               error_msgs):
@@ -532,9 +563,14 @@ class VectorQuantizer(nn.Module):
 
     def _ema_update(self, rows, idx, hist):
         """One EMA update of N, m and the codebook from the rows the VQ kernel just quantized; bumps their version
-        counters as an optimizer step does."""
+        counters as an optimizer step does.  With a dead_code_threshold, the restart follows on the same stream, its
+        uniforms drawn whether or not any code is dead, so the RNG stream does not depend on the data."""
         w = self.embedding.weight
         ops.vq_ema_update(rows, idx, hist, self.decay, self.eps, self.ema_cluster_size, self.ema_embed_sum, w.detach())
+        if self._dead_code_threshold is not None:
+            u = torch.rand((rows.shape[0],), device=rows.device)
+            ops.vq_ema_restart(rows, u, self._dead_code_threshold, self.ema_cluster_size, self.ema_embed_sum,
+                               w.detach(), self.last_restarts)
         torch.autograd.graph.increment_version([w, self.ema_cluster_size, self.ema_embed_sum])
 
     def _codebook(self):

@@ -357,6 +357,28 @@ def vq_ema_update(z_rows, idx, hist, decay, eps, cluster_size, embed_sum, codebo
     span.done()
 
 
+def vq_ema_restart(z_rows, u, threshold, cluster_size, embed_sum, codebook, n_restarted):
+    """Dead-code restart in place after an EMA update (vqb_vq_ema_restart_f32): every code with cluster_size < threshold
+    moves onto a row of z_rows (N,D), the rows taken by ascending (u, row index) from the uniforms u (N,) fp32;
+    n_restarted (1,) int32 receives the count.  Same tensor requirements as vq_ema_update."""
+    _require_cuda(z_rows, "z")
+    N, D = z_rows.shape
+    K = codebook.shape[0]
+    for t in (cluster_size, embed_sum, codebook, u):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.device != z_rows.device:
+            raise RuntimeError("vq_ema_restart: the EMA state, the codebook and u must be contiguous fp32 on z's device")
+    if u.numel() != N or n_restarted.dtype != torch.int32 or n_restarted.numel() != 1 or \
+            n_restarted.device != z_rows.device:
+        raise RuntimeError("vq_ema_restart: u must hold N values and n_restarted be one int32 on z's device")
+    ws_bytes = lib().vqb_vq_ema_restart_workspace_bytes(N, K)
+    ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=z_rows.device)
+    span = _Span(f"vq_ema_restart N={N} K={K} D={D}")
+    check(lib().vqb_vq_ema_restart_f32(z_rows.data_ptr(), u.data_ptr(), N, K, D, float(threshold),
+                                       cluster_size.data_ptr(), embed_sum.data_ptr(), codebook.data_ptr(),
+                                       n_restarted.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "vq_ema_restart")
+    span.done()
+
+
 def onehot(idx, K):
     N = idx.numel()
     out = torch.empty((N, K), dtype=torch.float32, device=idx.device)
