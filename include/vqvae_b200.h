@@ -293,6 +293,24 @@ int vqb_vq_ema_restart_f32(const float *z, const float *u, int64_t N, int K, int
                            float *cluster_size, float *embed_sum, float *codebook, int32_t *n_restarted,
                            void *workspace, size_t workspace_bytes, void *stream);
 
+/* k-means initialisation of a codebook (K, D) fp32 from rows z (N, D) fp32, N >= K, with uniforms u (N) fp32 in [0, 1):
+ *   seed: code j <- the row of rank j when the rows are ordered by (u_i, i) ascending (vqb_vq_ema_restart_f32's
+ *         sampling without replacement, with every code dead), copied exactly
+ *   then iters Lloyd steps, t = 0 .. iters-1:  idx and sse[t] from vqb_vq_forward_f32 on the current codebook (the
+ *         canonical fp32 distances; sse[t] is the inertia before step t); n_k and s_k as vqb_vq_ema_update_f32 forms
+ *         them; e_k <- fl(s_k / (float)n_k) where n_k > 0 (a code no row picks keeps its bits)
+ * sse: iters doubles, may be NULL iff iters == 0.  Non-finite rows are used as they are: a row holding a NaN takes
+ * code 0 (NaN wins the argmin), whose centroid then turns NaN and takes every row -- the call cannot check for one
+ * without a host synchronisation.  12 + iters * (v + 5) launches, v = vqb_vq_forward_f32's launches for the shape (2 on
+ * the tensor-core kernel, 3 on the exact kernel); no float atomics, no host synchronisation, CUDA-graph capturable.
+ * NULL pointers, N, K or D <= 0, N < K, iters < 0: VQB_ERR_BAD_ARG; D % 4 != 0, K > 8192, N > 2^32 - 1, or a shape the
+ * VQ dispatch refuses when iters > 0: VQB_ERR_UNSUPPORTED; a workspace shorter than
+ * vqb_vq_kmeans_workspace_bytes(N,K,D) (0 for a shape it refuses): VQB_ERR_WORKSPACE; all before any launch.
+ * z, codebook and the workspace 16-byte aligned.                                                                  */
+size_t vqb_vq_kmeans_workspace_bytes(int64_t N, int K, int D);
+int vqb_vq_kmeans_f32(const float *z, const float *u, int64_t N, int K, int D, int iters, float *codebook,
+                      double *sse, void *workspace, size_t workspace_bytes, void *stream);
+
 /* Backward of the EMA quantizer, whose loss is the commitment term alone (the codebook gets no gradient):
  *   dz (N,D) = g_zq + g_loss * 2 beta/(N D) * (z - zq)
  * zq = the forward's fp32 z_q rows (not the codebook, which the update has overwritten).  g_zq / g_loss may be

@@ -39,6 +39,8 @@ SIGNATURES = {
     "vqb_vq_ema_update_f32": (_i, [_vp, _vp, _vp, _i64, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _sz, _vp]),
     "vqb_vq_ema_restart_workspace_bytes": (_sz, [_i64, _i]),
     "vqb_vq_ema_restart_f32": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "vqb_vq_kmeans_workspace_bytes": (_sz, [_i64, _i, _i]),
+    "vqb_vq_kmeans_f32": (_i, [_vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "vqb_vq_commit_backward_f32": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _f, _vp, _vp]),
     "vqb_vq_finish_ema_f32": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _vp, _vp]),
     "vqb_onehot_f32": (_i, [_vp, _i64, _i, _vp, _vp]),

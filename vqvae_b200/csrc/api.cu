@@ -12,6 +12,7 @@ int launch_convt_out_k4s2(const float *x, const float *wp, const float *bias, fl
                           int Cout, int relu, cudaStream_t s);
 #include "wgconv.h"
 bool vq_tc_supported(long long N, int K, int D);
+bool vq_exact_supported(int K, int D);
 int launch_vq_tc(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, int zq_bf16, double *sse,
                  int *hist, void *ws, float *dbg, cudaStream_t s);
 
@@ -177,13 +178,23 @@ extern "C" size_t vqb_vq_workspace_bytes(int64_t N, int K, int D) {
     return vq_exact_workspace_bytes(K);
 }
 
+// The shape checks of vqb_vq_forward_f32's dispatch under the current vqb_set_vq_kernel choice, answered before it
+// launches anything (vq_ema.cu's k-means asks them before its first launch).
+int vq_forward_check(long long N, int K, int D) {
+    if (N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
+    if (D % 4 != 0) return VQB_ERR_UNSUPPORTED;
+    const bool tc = vq_tc_supported(N, K, D);
+    if (g_vq_kernel == 2 && !tc) return VQB_ERR_UNSUPPORTED;
+    if ((!tc || g_vq_kernel == 1) && !vq_exact_supported(K, D)) return VQB_ERR_UNSUPPORTED;
+    return 0;
+}
+
 static int vq_forward_impl(const float *z, const float *codebook, int64_t N, int K, int D, int64_t *idx, void *zq,
                            int zq_bf16, double *sse, int32_t *hist, void *workspace, size_t workspace_bytes, void *stream) {
     if (!z || !codebook || !idx || !zq || !sse || !hist || !workspace) return VQB_ERR_BAD_ARG;
-    if (N <= 0 || K <= 0 || D <= 0) return VQB_ERR_BAD_ARG;
-    if (D % 4 != 0) return VQB_ERR_UNSUPPORTED;
+    const int rc = vq_forward_check(N, K, D);
+    if (rc != 0) return rc;
     const bool tc_ok = vq_tc_supported(N, K, D);
-    if (g_vq_kernel == 2 && !tc_ok) return VQB_ERR_UNSUPPORTED;
     if (workspace_bytes < vqb_vq_workspace_bytes(N, K, D)) return VQB_ERR_WORKSPACE;
     const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(codebook) |
                          reinterpret_cast<uintptr_t>(zq) | reinterpret_cast<uintptr_t>(workspace);

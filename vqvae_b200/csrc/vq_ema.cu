@@ -1,6 +1,7 @@
 // vq_ema.cu -- exponential-moving-average codebook update of a VectorQuantizer (van den Oord et al. 2017, app. A.1),
 // with per-code row sums in a fixed order, the backward / loss finisher of the EMA model (commitment term only), and
-// the dead-code restarts that may follow an update (see "dead-code restarts" below).
+// the dead-code restarts that may follow an update (see "dead-code restarts" below), and the k-means initialisation
+// that is built from both (see "k-means" at the end).
 //
 // One update, from the rows z (N, D) the VQ kernel quantized, their codes idx (clamped to [0, K-1]) and its hist:
 //   N_k <- g N_k + (1-g) hist_k,   m_k <- g m_k + (1-g) s_k,   n = sum_k N_k,
@@ -20,6 +21,8 @@
 // A segment's partial lives in slot floor(cb_k / S) + k + j (cb_k = first sorted position of code k, j = segment
 // number): strictly increasing in (k, j), so slots are unique and fewer than N / S + K + 1.
 #include "common.cuh"
+
+int vq_forward_check(long long N, int K, int D);      // api.cu: the VQ dispatch's shape checks
 
 namespace {
 
@@ -71,10 +74,12 @@ __global__ void __launch_bounds__(32) ema_count(const long long *__restrict__ id
     __shared__ unsigned sc[EMA_KTILE];
     const int lane = threadIdx.x;
     const long long c = blockIdx.x;
-    // side jobs, grid-stride: N_k' for the finisher's n, and the scan's tile flags (+ its tile counter) zeroed
+    // side jobs, grid-stride: N_k' for the finisher's n (unless nnew is NULL: k-means has no N, and then hist,
+    // cluster_size and decay are not read), and the scan's tile flags (+ its tile counter) zeroed
     const float omg = 1.0f - decay;
-    for (long long k = c * 32 + lane; k < K; k += (long long)gridDim.x * 32)
-        nnew[k] = __fadd_rn(__fmul_rn(decay, cluster_size[k]), __fmul_rn(omg, (float)hist[k]));
+    if (nnew)
+        for (long long k = c * 32 + lane; k < K; k += (long long)gridDim.x * 32)
+            nnew[k] = __fadd_rn(__fmul_rn(decay, cluster_size[k]), __fmul_rn(omg, (float)hist[k]));
     for (long long t = c * 32 + lane; t <= ntiles; t += (long long)gridDim.x * 32) status[t] = 0ULL;
     const long long r0 = c * rows_per_chunk;
     const long long r1 = r0 + rows_per_chunk < N ? r0 + rows_per_chunk : N;
@@ -189,6 +194,14 @@ __device__ __forceinline__ float4 add4(float4 a, float4 b) {
     return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
 }
 
+// column c (a float4) of s_k: code k's nseg segment partials from slot s0 on, added in segment order
+__device__ __forceinline__ float4 code_sum(const float *part, long long s0, long long nseg, int d4, int c) {
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 8
+    for (long long j = 0; j < nseg; ++j) s = add4(s, reinterpret_cast<const float4 *>(part)[(s0 + j) * d4 + c]);
+    return s;
+}
+
 // lanes per code / segment: D/4 float4 columns, at most one CTA's worth (wider rows loop over their columns)
 __host__ __device__ __forceinline__ int group_lanes(int D) { return D / 4 < EMA_THREADS ? D / 4 : EMA_THREADS; }
 
@@ -249,9 +262,7 @@ __global__ void __launch_bounds__(EMA_THREADS) ema_finish(int K, int D, long lon
         code_span(base, nchunks, k, cb, cnt);
         const long long s0 = seg_slot(cb, k), nseg = (cnt + EMA_SEG - 1) / EMA_SEG;
         for (int c = lane; c < d4; c += L) {
-            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 8
-            for (long long j = 0; j < nseg; ++j) s = add4(s, reinterpret_cast<const float4 *>(part)[(s0 + j) * d4 + c]);
+            const float4 s = code_sum(part, s0, nseg, d4, c);
             float4 *m4 = reinterpret_cast<float4 *>(embed_sum) + (long long)k * d4 + c;
             float4 m = *m4;
             m.x = __fadd_rn(__fmul_rn(decay, m.x), __fmul_rn(omg, s.x));
@@ -287,6 +298,44 @@ int sm_count() {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     return sms;
+}
+
+struct EmaBuffers {
+    unsigned *cnt;
+    long long *base;
+    unsigned long long *status;
+    long long *rows;
+    float *part, *nnew;
+};
+
+EmaBuffers ema_buffers(void *workspace, const EmaPlan &p) {
+    char *ws = static_cast<char *>(workspace);
+    return EmaBuffers{reinterpret_cast<unsigned *>(ws + p.off_cnt), reinterpret_cast<long long *>(ws + p.off_base),
+                      reinterpret_cast<unsigned long long *>(ws + p.off_status),
+                      reinterpret_cast<long long *>(ws + p.off_rows), reinterpret_cast<float *>(ws + p.off_part),
+                      reinterpret_cast<float *>(ws + p.off_nnew)};
+}
+
+// Launches 1..4 of the update: the counting sort of the rows by code and the segment partials of s_k.  nnew NULL: no
+// N_k' (hist, cluster_size and decay unused).
+void ema_sums(const EmaPlan &p, const EmaBuffers &b, const float *z, const long long *idx, const int *hist,
+              const float *cluster_size, float decay, float *nnew, long long N, int K, int D, cudaStream_t s) {
+    const int G = EMA_THREADS / group_lanes(D);
+    ema_count<<<(unsigned)p.nchunks, 32, 0, s>>>(idx, hist, cluster_size, N, K, p.rows_per_chunk, p.nchunks, decay,
+                                                 b.cnt, nnew, b.status, p.ntiles);
+    ema_scan<<<(unsigned)p.ntiles, EMA_SCAN_THREADS, 0, s>>>(b.cnt, p.M, b.base, b.status, p.ntiles);
+    ema_scatter<<<(unsigned)p.nchunks, 32, 0, s>>>(idx, N, K, p.rows_per_chunk, p.nchunks, b.base, b.rows);
+    ema_partial<<<(unsigned)((p.nslots + G - 1) / G), EMA_THREADS, 0, s>>>(z, K, D, p.nchunks, b.base, b.rows,
+                                                                           p.nslots, b.part);
+    VQB_COUNT_LAUNCH(4);
+}
+
+// CTAs of a per-code finisher (ema_finish, km_finish)
+unsigned finish_grid(int K, int D) {
+    const int G = EMA_THREADS / group_lanes(D);
+    long long fin = ((long long)K + G - 1) / G;
+    if (fin > 2LL * sm_count()) fin = 2LL * sm_count();
+    return (unsigned)fin;
 }
 
 // ---- dead-code restarts (vqb_vq_ema_restart_f32), run after an update --------------------------------------------
@@ -365,15 +414,22 @@ __device__ unsigned long long rs_prefix(const unsigned *digits, int npass, long 
     return s_prefix;
 }
 
+// the selection's counters zeroed by one CTA of RS_COMPACT_THREADS threads: the digit counts, the ranks, the collect
+// counter meta[1]
+__device__ __forceinline__ void rs_clear(int *meta, unsigned *digits, int *rank, int K) {
+    const int t = threadIdx.x;
+    for (int i = t; i < RS_PASSES * 256; i += RS_COMPACT_THREADS) digits[i] = 0u;
+    for (int i = t; i < K; i += RS_COMPACT_THREADS) rank[i] = 0;
+    if (t == 0) meta[1] = 0;
+}
+
 __global__ void __launch_bounds__(RS_COMPACT_THREADS) rs_compact(const float *__restrict__ cluster_size, int K,
                                                                  long long N, float thr, int *__restrict__ meta,
                                                                  int *__restrict__ dead, unsigned *__restrict__ digits,
                                                                  int *__restrict__ rank, int *__restrict__ n_restarted) {
     __shared__ int s_warp[RS_COMPACT_THREADS / 32];
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    for (int i = t; i < RS_PASSES * 256; i += RS_COMPACT_THREADS) digits[i] = 0u;
-    for (int i = t; i < K; i += RS_COMPACT_THREADS) rank[i] = 0;
-    if (t == 0) meta[1] = 0;
+    rs_clear(meta, digits, rank, K);
     const int per = (K + RS_COMPACT_THREADS - 1) / RS_COMPACT_THREADS;    // <= 8 codes per thread, in code order
     const int k0 = t * per;
     unsigned flags = 0u;
@@ -487,6 +543,101 @@ __global__ void __launch_bounds__(RS_THREADS) rs_assign(const float *__restrict_
     }
 }
 
+// Launches 2..11 of the restart: the R = min(meta[0], N) smallest keys of u listed in `keys`, rank[q] the rank of
+// keys[q] among them (R <= rmax, which sizes the rank grid).
+void restart_select(const float *u, long long N, long long rmax, int *meta, unsigned *digits, unsigned long long *keys,
+                    int *rank, cudaStream_t s) {
+    long long scan = (N + RS_THREADS - 1) / RS_THREADS;
+    if (scan > 4LL * sm_count()) scan = 4LL * sm_count();
+    for (int pass = 0; pass < RS_PASSES; ++pass)
+        rs_digits<<<(unsigned)scan, RS_THREADS, 0, s>>>(u, N, meta, digits, pass);
+    rs_collect<<<(unsigned)scan, RS_THREADS, 0, s>>>(u, N, meta, digits, keys);
+    const dim3 rank_grid((unsigned)((rmax + RS_THREADS - 1) / RS_THREADS),
+                         (unsigned)((rmax + RS_RANK_CHUNK - 1) / RS_RANK_CHUNK));
+    rs_rank<<<rank_grid, RS_THREADS, 0, s>>>(meta, N, keys, rank);
+    VQB_COUNT_LAUNCH(RS_PASSES + 2);
+}
+
+// ---- k-means initialisation (vqb_vq_kmeans_f32) -------------------------------------------------------------------
+// From rows z (N, D), N >= K, and uniforms u (N):
+//   seed   code j <- the row of rank j by (u_i, i): the restart's selection with every code dead (12 launches)
+//   iters  Lloyd steps, each: the VQ dispatch -> idx, sse[t]; the update's counting sort and segment partials; then
+//          km_finish: e_k <- fl(s_k / (float)n_k) where n_k > 0 (an empty code keeps its bits)
+// The sums are the update's (same kernels, same order), so the bits depend on (z, u) only.
+
+// launch 1 of the seed: every code dead (meta[0] = K) and the selection's counters zeroed
+__global__ void __launch_bounds__(RS_COMPACT_THREADS) km_all_dead(int K, int *__restrict__ meta,
+                                                                  unsigned *__restrict__ digits, int *__restrict__ rank) {
+    rs_clear(meta, digits, rank, K);
+    if (threadIdx.x == 0) meta[0] = K;
+}
+
+// launch 12 of the seed: one thread per (listed key, float4 column), code rank[q] <- its row
+__global__ void __launch_bounds__(RS_THREADS) km_seed(const float *__restrict__ z, int K, int D,
+                                                      const unsigned long long *__restrict__ keys,
+                                                      const int *__restrict__ rank, float *__restrict__ codebook) {
+    const int d4 = D / 4;
+    const float4 *z4 = reinterpret_cast<const float4 *>(z);
+    for (long long g = (long long)blockIdx.x * RS_THREADS + threadIdx.x; g < (long long)K * d4;
+         g += (long long)gridDim.x * RS_THREADS) {
+        const long long q = g / d4;
+        const int c = (int)(g - q * d4);
+        const long long r = (long long)(keys[q] & 0xFFFFFFFFULL);
+        reinterpret_cast<float4 *>(codebook)[(long long)rank[q] * d4 + c] = __ldg(z4 + r * d4 + c);
+    }
+}
+
+// the last launch of a Lloyd step: per code, s_k as ema_finish sums it, then the centroid
+__global__ void __launch_bounds__(EMA_THREADS) km_finish(int K, int D, long long nchunks,
+                                                         const long long *__restrict__ base,
+                                                         const float *__restrict__ part, float *__restrict__ codebook) {
+    const int L = group_lanes(D), G = EMA_THREADS / L, d4 = D / 4;
+    const int g = threadIdx.x / L, lane = threadIdx.x - g * L;
+    if (g >= G) return;
+    for (int k = blockIdx.x * G + g; k < K; k += gridDim.x * G) {
+        long long cb, n;
+        code_span(base, nchunks, k, cb, n);
+        if (n == 0) continue;
+        const float nk = (float)n;
+        const long long s0 = seg_slot(cb, k), nseg = (n + EMA_SEG - 1) / EMA_SEG;
+        for (int c = lane; c < d4; c += L) {
+            const float4 sk = code_sum(part, s0, nseg, d4, c);
+            reinterpret_cast<float4 *>(codebook)[(long long)k * d4 + c] =
+                make_float4(__fdiv_rn(sk.x, nk), __fdiv_rn(sk.y, nk), __fdiv_rn(sk.z, nk), __fdiv_rn(sk.w, nk));
+        }
+    }
+}
+
+// workspace: the restart's selection, the update's sort and partials, the VQ call's own workspace, idx (N), hist (K)
+// and the z_q rows (N, D) the VQ call writes and nobody reads
+struct KmeansPlan {
+    RestartPlan rs;
+    EmaPlan ema;
+    size_t off_ema, off_vq, vq_bytes, off_idx, off_hist, off_zq, total;
+};
+
+KmeansPlan kmeans_plan(long long N, int K, int D) {
+    KmeansPlan p{};
+    p.rs = restart_plan(K);
+    p.ema = ema_plan(N, K, D);
+    p.vq_bytes = vqb_vq_workspace_bytes(N, K, D);
+    size_t o = align16(p.rs.total);
+    p.off_ema = o;  o = align16(o + p.ema.total);
+    p.off_vq = o;   o = align16(o + p.vq_bytes);
+    p.off_idx = o;  o = align16(o + sizeof(long long) * (size_t)N);
+    p.off_hist = o; o = align16(o + sizeof(int) * (size_t)K);
+    p.off_zq = o;   o = align16(o + sizeof(float) * (size_t)N * (size_t)D);
+    p.total = o;
+    return p;
+}
+
+// VQB_OK, or the code vqb_vq_kmeans_f32 returns for the shape (the VQ dispatch's own checks when it runs a step)
+int kmeans_shape_check(long long N, int K, int D, int iters) {
+    if (N <= 0 || K <= 0 || D <= 0 || N < K || iters < 0) return VQB_ERR_BAD_ARG;
+    if (D % 4 != 0 || K > RS_MAX_K || N > RS_MAX_N) return VQB_ERR_UNSUPPORTED;
+    return iters > 0 ? vq_forward_check(N, K, D) : VQB_OK;
+}
+
 }  // namespace
 
 extern "C" size_t vqb_vq_ema_workspace_bytes(int64_t N, int K, int D) {
@@ -506,26 +657,12 @@ extern "C" int vqb_vq_ema_update_f32(const float *z, const int64_t *idx, const i
     const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(embed_sum) |
                          reinterpret_cast<uintptr_t>(codebook) | reinterpret_cast<uintptr_t>(workspace);
     if (al & 15) return VQB_ERR_ALIGNMENT;
-    char *ws = static_cast<char *>(workspace);
-    unsigned *cnt = reinterpret_cast<unsigned *>(ws + p.off_cnt);
-    long long *base = reinterpret_cast<long long *>(ws + p.off_base);
-    unsigned long long *status = reinterpret_cast<unsigned long long *>(ws + p.off_status);
-    long long *rows = reinterpret_cast<long long *>(ws + p.off_rows);
-    float *part = reinterpret_cast<float *>(ws + p.off_part);
-    float *nnew = reinterpret_cast<float *>(ws + p.off_nnew);
-    const long long *ip = reinterpret_cast<const long long *>(idx);
+    const EmaBuffers b = ema_buffers(workspace, p);
     cudaStream_t s = (cudaStream_t)stream;
-    const int G = EMA_THREADS / group_lanes(D);
-    long long fin = ((long long)K + G - 1) / G;
-    if (fin > 2LL * sm_count()) fin = 2LL * sm_count();
-    ema_count<<<(unsigned)p.nchunks, 32, 0, s>>>(ip, hist, cluster_size, N, K, p.rows_per_chunk, p.nchunks, decay, cnt,
-                                                 nnew, status, p.ntiles);
-    ema_scan<<<(unsigned)p.ntiles, EMA_SCAN_THREADS, 0, s>>>(cnt, p.M, base, status, p.ntiles);
-    ema_scatter<<<(unsigned)p.nchunks, 32, 0, s>>>(ip, N, K, p.rows_per_chunk, p.nchunks, base, rows);
-    ema_partial<<<(unsigned)((p.nslots + G - 1) / G), EMA_THREADS, 0, s>>>(z, K, D, p.nchunks, base, rows, p.nslots, part);
-    ema_finish<<<(unsigned)fin, EMA_THREADS, 0, s>>>(K, D, p.nchunks, base, part, nnew, decay, eps, cluster_size,
-                                                     embed_sum, codebook);
-    VQB_COUNT_LAUNCH(5);
+    ema_sums(p, b, z, reinterpret_cast<const long long *>(idx), hist, cluster_size, decay, b.nnew, N, K, D, s);
+    ema_finish<<<finish_grid(K, D), EMA_THREADS, 0, s>>>(K, D, p.nchunks, b.base, b.part, b.nnew, decay, eps,
+                                                         cluster_size, embed_sum, codebook);
+    VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }
 
@@ -554,22 +691,55 @@ extern "C" int vqb_vq_ema_restart_f32(const float *z, const float *u, int64_t N,
     unsigned long long *keys = reinterpret_cast<unsigned long long *>(ws + p.off_keys);
     int *rank = reinterpret_cast<int *>(ws + p.off_rank);
     cudaStream_t s = (cudaStream_t)stream;
-    const int sms = sm_count();
-    long long scan = (N + RS_THREADS - 1) / RS_THREADS;
-    if (scan > 4LL * sms) scan = 4LL * sms;
     long long asg = (rmax * (D / 4) + RS_THREADS - 1) / RS_THREADS;
-    if (asg > 4LL * sms) asg = 4LL * sms;
+    if (asg > 4LL * sm_count()) asg = 4LL * sm_count();
     rs_compact<<<1, RS_COMPACT_THREADS, 0, s>>>(cluster_size, K, N, threshold, meta, dead, digits, rank,
                                                  n_restarted);
-    for (int pass = 0; pass < RS_PASSES; ++pass)
-        rs_digits<<<(unsigned)scan, RS_THREADS, 0, s>>>(u, N, meta, digits, pass);
-    rs_collect<<<(unsigned)scan, RS_THREADS, 0, s>>>(u, N, meta, digits, keys);
-    const dim3 rank_grid((unsigned)((rmax + RS_THREADS - 1) / RS_THREADS),
-                         (unsigned)((rmax + RS_RANK_CHUNK - 1) / RS_RANK_CHUNK));
-    rs_rank<<<rank_grid, RS_THREADS, 0, s>>>(meta, N, keys, rank);
+    restart_select(u, N, rmax, meta, digits, keys, rank, s);
     rs_assign<<<(unsigned)asg, RS_THREADS, 0, s>>>(z, N, D, threshold, meta, dead, keys, rank, cluster_size,
                                                    embed_sum, codebook);
-    VQB_COUNT_LAUNCH(4 + RS_PASSES);
+    VQB_COUNT_LAUNCH(2);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_vq_kmeans_workspace_bytes(int64_t N, int K, int D) {
+    if (kmeans_shape_check(N, K, D, 0) != VQB_OK) return 0;
+    return kmeans_plan(N, K, D).total;
+}
+
+extern "C" int vqb_vq_kmeans_f32(const float *z, const float *u, int64_t N, int K, int D, int iters, float *codebook,
+                                 double *sse, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!z || !u || !codebook || !workspace || (iters > 0 && !sse)) return VQB_ERR_BAD_ARG;
+    const int rc = kmeans_shape_check(N, K, D, iters);
+    if (rc != VQB_OK) return rc;
+    const KmeansPlan p = kmeans_plan(N, K, D);
+    if (workspace_bytes < p.total) return VQB_ERR_WORKSPACE;
+    const uintptr_t al = reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(codebook) |
+                         reinterpret_cast<uintptr_t>(workspace);
+    if (al & 15) return VQB_ERR_ALIGNMENT;
+    char *ws = static_cast<char *>(workspace);
+    int *meta = reinterpret_cast<int *>(ws + p.rs.off_meta);
+    unsigned *digits = reinterpret_cast<unsigned *>(ws + p.rs.off_digits);
+    unsigned long long *keys = reinterpret_cast<unsigned long long *>(ws + p.rs.off_keys);
+    int *rank = reinterpret_cast<int *>(ws + p.rs.off_rank);
+    const EmaBuffers b = ema_buffers(ws + p.off_ema, p.ema);
+    int64_t *idx = reinterpret_cast<int64_t *>(ws + p.off_idx);
+    int32_t *hist = reinterpret_cast<int32_t *>(ws + p.off_hist);
+    float *zq = reinterpret_cast<float *>(ws + p.off_zq);
+    cudaStream_t s = (cudaStream_t)stream;
+    long long seed = ((long long)K * (D / 4) + RS_THREADS - 1) / RS_THREADS;
+    if (seed > 4LL * sm_count()) seed = 4LL * sm_count();
+    km_all_dead<<<1, RS_COMPACT_THREADS, 0, s>>>(K, meta, digits, rank);
+    restart_select(u, N, K, meta, digits, keys, rank, s);
+    km_seed<<<(unsigned)seed, RS_THREADS, 0, s>>>(z, K, D, keys, rank, codebook);
+    VQB_COUNT_LAUNCH(2);
+    for (int t = 0; t < iters; ++t) {
+        const int e = vqb_vq_forward_f32(z, codebook, N, K, D, idx, zq, sse + t, hist, ws + p.off_vq, p.vq_bytes, stream);
+        if (e != VQB_OK) return e;
+        ema_sums(p.ema, b, z, reinterpret_cast<const long long *>(idx), nullptr, nullptr, 0.f, nullptr, N, K, D, s);
+        km_finish<<<finish_grid(K, D), EMA_THREADS, 0, s>>>(K, D, p.ema.nchunks, b.base, b.part, codebook);
+        VQB_COUNT_LAUNCH(1);
+    }
     return vqb_cuda_status(cudaGetLastError());
 }
 

@@ -238,6 +238,21 @@ size_t vq_exact_workspace_bytes(int K) {
     return kpad * sizeof(float) + (size_t)VQ_MAX_CTAS * sizeof(double) + kpad / 128 * sizeof(float) + 16;
 }
 
+constexpr size_t VQ_EXACT_MAX_DYN = 227 * 1024 - 1024;   // 227 KB per CTA minus static smem
+
+// dynamic shared memory of vq_exact_kernel: its tiles, plus the code histogram when that fits
+static size_t vq_exact_smem(int K, int D, int &use_smem_hist) {
+    const size_t base = ((size_t)D * (VR + VPAD) + (size_t)D * (VC + VPAD) + VR + VC) * sizeof(float) +
+                        VR * sizeof(int);
+    use_smem_hist = (base + (size_t)K * sizeof(int) <= 200 * 1024) ? 1 : 0;
+    return base + (use_smem_hist ? (size_t)K * sizeof(int) : 0);
+}
+
+bool vq_exact_supported(int K, int D) {
+    int use_smem_hist;
+    return vq_exact_smem(K, D, use_smem_hist) <= VQ_EXACT_MAX_DYN;
+}
+
 int launch_vq_exact(const float *z, const float *E, long long N, int K, int D, long long *idx, void *zq, int zq_bf16,
                     double *sse, int *hist, void *ws, cudaStream_t s) {
     const VqWorkspace w = vq_workspace(ws, K);
@@ -246,15 +261,12 @@ int launch_vq_exact(const float *z, const float *E, long long N, int K, int D, l
     cudaError_t e = cudaMemsetAsync(hist, 0, sizeof(int) * (size_t)K, s);
     if (e != cudaSuccess) return (int)e;
     code_norms_kernel<<<(K + 127) / 128, 128, 0, s>>>(E, K, D, bn);
-    const size_t base = ((size_t)D * (VR + VPAD) + (size_t)D * (VC + VPAD) + VR + VC) * sizeof(float) +
-                        VR * sizeof(int);
-    const int use_smem_hist = (base + (size_t)K * sizeof(int) <= 200 * 1024) ? 1 : 0;
-    const size_t smem = base + (use_smem_hist ? (size_t)K * sizeof(int) : 0);
-    constexpr size_t kMaxDyn = 227 * 1024 - 1024;   // 227 KB per CTA minus static smem
-    if (smem > kMaxDyn) return VQB_ERR_UNSUPPORTED;
+    int use_smem_hist;
+    const size_t smem = vq_exact_smem(K, D, use_smem_hist);
+    if (smem > VQ_EXACT_MAX_DYN) return VQB_ERR_UNSUPPORTED;
     static bool attr_set = false;
     if (!attr_set) {
-        e = cudaFuncSetAttribute(vq_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDyn);
+        e = cudaFuncSetAttribute(vq_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VQ_EXACT_MAX_DYN);
         if (e != cudaSuccess) return (int)e;
         attr_set = true;
     }

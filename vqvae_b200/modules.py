@@ -573,6 +573,53 @@ class VectorQuantizer(nn.Module):
                                w.detach(), self.last_restarts)
         torch.autograd.graph.increment_version([w, self.ema_cluster_size, self.ema_embed_sum])
 
+    def init_codebook_kmeans(self, z, iters=10):
+        """Fit the codebook to one batch by k-means, in place (vqb_vq_kmeans_f32).  z is (B, e_dim, H, W) fp32 CUDA, what
+        forward takes; its rows, in forward's order, are the data.  The K codes start on K distinct rows drawn uniformly
+        without replacement (one ``torch.rand((B*H*W,))`` from the current generator); each of the `iters` Lloyd steps
+        then assigns every row to its nearest code by forward's fp32 distances and moves every code that took a row to
+        their mean (a code that took none stays).  iters=0 only seeds.  Returns the sum of squared distances before each
+        step, a float64 (iters,) device tensor that the library never reads back.
+
+        Records no autograd graph and leaves ``training`` as it is; the codebook's version counter moves, as after an
+        optimizer step.  An EMA codebook's averages restart from the new codebook (N = 1, m = e).  A row holding a NaN
+        takes over the codebook: finding one would need a host synchronisation, so the call does not look."""
+        self._check_kmeans(iters)
+        _check_input(z, self.e_dim, "VectorQuantizer")
+        self._check_kmeans_rows(z.shape[0] * z.shape[2] * z.shape[3])
+        with torch.no_grad():
+            z = _prep_input(z, self.e_dim, "VectorQuantizer")
+            return self._kmeans_rows(ops.nchw_to_nhwc(z).view(-1, self.e_dim), iters)
+
+    def _check_kmeans(self, iters):
+        """init_codebook_kmeans's checks of its arguments, then (_check_kmeans_rows) of the batch, made before anything
+        is allocated or launched."""
+        if isinstance(iters, bool) or not isinstance(iters, numbers.Integral) or iters < 0:
+            raise ValueError(f"iters must be an int >= 0, got {iters!r}")
+        if self.n_e > self._MAX_RESTART_CODES:
+            raise ValueError(f"init_codebook_kmeans supports at most {self._MAX_RESTART_CODES} codes, not {self.n_e}")
+        if self.e_dim % 4:
+            raise ValueError(f"init_codebook_kmeans needs e_dim % 4 == 0, not {self.e_dim}")
+
+    def _check_kmeans_rows(self, n_rows):
+        if n_rows < self.n_e:
+            raise ValueError(f"init_codebook_kmeans needs at least one row per code: {n_rows} rows, {self.n_e} codes")
+        ops._require_cuda(self.embedding.weight, "VectorQuantizer codebook")
+
+    def _kmeans_rows(self, rows, iters):
+        """init_codebook_kmeans on checked (N, e_dim) fp32 rows, under no_grad."""
+        w = self.embedding.weight
+        cb = self._codebook()
+        sse = ops.vq_kmeans(rows, torch.rand((rows.shape[0],), device=rows.device), int(iters), cb)
+        if cb.data_ptr() == w.data_ptr():
+            torch.autograd.graph.increment_version([w])          # the kernels wrote it in place
+        else:
+            w.copy_(cb)
+        if self.decay is not None:                               # as _load_from_state_dict restarts them
+            self.ema_cluster_size.fill_(1.0)
+            self.ema_embed_sum.copy_(w)
+        return sse
+
     def _codebook(self):
         w = self.embedding.weight.detach()
         if w.dtype != torch.float32:
@@ -1098,6 +1145,18 @@ class VQVAE(nn.Module):
         if acts is not None:
             acts.update(z_e=z_e.view(-1, D), codebook=codebook, idx=idx, zq=zq)
         return embedding_loss, x_hat, perplexity
+
+    def init_codebook_kmeans(self, x, iters=10):
+        """VectorQuantizer.init_codebook_kmeans on the z_e rows of the images x, from the encoder walk that forward
+        quantizes (in the active precision, the bf16 pipeline included).  Call it on the first batch before training;
+        an optimizer built earlier keeps its moments of the codebook.  Returns the (iters,) float64 device SSE."""
+        vq = self.vector_quantization
+        vq._check_kmeans(iters)
+        _check_input(x, 3, "VQVAE")
+        vq._check_kmeans_rows(x.shape[0] * (x.shape[2] // 4) * (x.shape[3] // 4))
+        with torch.no_grad():
+            z_e, _, _, _ = self._encode_rows(x, self._bf16_pipeline())
+            return vq._kmeans_rows(z_e.view(-1, vq.e_dim), iters)
 
     def reduce_scalars(self):
         """(embedding_loss, perplexity) over the WHOLE sharded batch from the statistics of the last forward: the one

@@ -379,6 +379,29 @@ def vq_ema_restart(z_rows, u, threshold, cluster_size, embed_sum, codebook, n_re
     span.done()
 
 
+def vq_kmeans(z_rows, u, iters, codebook):
+    """k-means fit of codebook (K,D), a contiguous fp32 CUDA tensor, in place (vqb_vq_kmeans_f32): seeded with the rows
+    of z_rows (N,D) ranked 0..K-1 by ascending (u, row index) from the uniforms u (N,) fp32, then `iters` Lloyd steps.
+    Returns sse, a float64 (iters,) device tensor: the inertia before each step.  Version counters are the caller's to
+    bump."""
+    _require_cuda(z_rows, "z")
+    N, D = z_rows.shape
+    K = codebook.shape[0]
+    for t in (codebook, u):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.device != z_rows.device:
+            raise RuntimeError("vq_kmeans: the codebook and u must be contiguous fp32 on z's device")
+    if u.numel() != N:
+        raise RuntimeError("vq_kmeans: u must hold N values")
+    sse = torch.empty((iters,), dtype=torch.float64, device=z_rows.device)
+    ws_bytes = lib().vqb_vq_kmeans_workspace_bytes(N, K, D)
+    ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=z_rows.device)
+    span = _Span(f"vq_kmeans N={N} K={K} D={D} iters={iters}")
+    check(lib().vqb_vq_kmeans_f32(z_rows.data_ptr(), u.data_ptr(), N, K, D, iters, codebook.data_ptr(),
+                                  sse.data_ptr() if iters else None, ws.data_ptr(), ws_bytes, _stream()), "vq_kmeans")
+    span.done()
+    return sse
+
+
 def onehot(idx, K):
     N = idx.numel()
     out = torch.empty((N, K), dtype=torch.float32, device=idx.device)
