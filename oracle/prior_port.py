@@ -47,6 +47,11 @@ PRIOR_SHAPE_CASES = {
     # residual on layer 0 (teacher-forced only: the sampler refuses it)
     "resid0": dict(K=37, dim=32, n_layers=2, n_classes=3, size=5, batch=2, wseed=56, xseed=57,
                    layers=[["A", 5, True], B3], parts=["forward", "backward"]),
+    # 2523 positions, not a multiple of 32: every weight gradient in 5 to 79 position chunks, the last one ragged (27
+    # to 475 positions) and ending in a short k-step; K = 300: three 128-wide N tiles of logits, the last 44 wide,
+    # and a 300-deep head dgrad ending in a short k-step
+    "chunks": dict(K=300, dim=64, n_layers=3, n_classes=10, size=29, batch=3, wseed=60, xseed=61,
+                   layers=[A7, B3, B3], parts=["forward", "backward"]),
     # the cfg3 latent with the reference's stack: the sampler's vertical rings over 64 rows
     "cfg3_sampler": dict(K=1024, dim=64, n_layers=15, n_classes=10, size=64, batch=2, wseed=58, xseed=59,
                          layers=[A7] + [B3] * 14, parts=["sampler"]),

@@ -1,5 +1,6 @@
 """CPU checks of the Gated PixelCNN prior's TF32 mode: the `precision` attribute, the TF32 entry points' declarations
-and argument checks, and the rounding helper of the emulated-TF32 restatement."""
+and argument checks, and the emulated-TF32 restatement's helpers: its roundings, its evaluation at given activations,
+and the decoder of the training forward's saved activations."""
 import ctypes
 import os
 import re
@@ -7,7 +8,8 @@ import re
 import pytest
 import torch
 
-from tests.prior_tf32_port import tf32_round
+from tests.prior_tf32_port import (decode_saved, encode_saved, prior_logits_tf32, saved_offsets, saved_points,
+                                   tf32_round, tf32_truncate)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PAIRS = [("vqb_prior_forward_tf32", "vqb_prior_forward_f32"),
@@ -119,3 +121,57 @@ def test_tf32_rounding_of_chosen_bit_patterns():
     d = tf32_round(x.double())
     assert d.dtype == torch.float64 and torch.equal(d.float().view(torch.int32), want.view(torch.int32))
     assert int((tf32_round(torch.randn(1000)).view(torch.int32) & 0x1FFF).abs().sum()) == 0
+
+
+def test_truncation_clears_the_low_13_bits():
+    x = torch.tensor([0x3F801FFF, 0xBF803FFF - (1 << 32), 0x00001FFF], dtype=torch.int64).to(torch.int32)
+    got = tf32_truncate(x.view(torch.float32).double()).float().view(torch.int32)
+    assert got.tolist() == [0x3F800000, 0xBF802000 - (1 << 32), 0]
+
+
+@pytest.mark.parametrize("kind", ["ce", "random"])
+@pytest.mark.parametrize("name", ["prior_ragged", "kernels", "resid0", "single3", "narrow"])
+def test_restatement_at_its_own_activations_is_the_plain_restatement(name, kind):
+    """With `at` set to the activations it records itself, the straight-through evaluation changes no value and no
+    gradient: logits and every gradient as without `at`."""
+    from oracle.prior_port import PRIOR_CASES, PRIOR_SHAPE_CASES, make_prior_inputs, make_prior_state_dict
+    from oracle.prior_train_port import leaf_params, prior_loss
+    c = PRIOR_CASES.get(name) or PRIOR_SHAPE_CASES[name]
+    sd = make_prior_state_dict(c["K"], c["dim"], c["n_layers"], c["n_classes"], c["wseed"], c.get("layers"))
+    codes, labels, _ = make_prior_inputs(c)
+    x, lab = torch.from_numpy(codes), torch.from_numpy(labels)
+    up = torch.randn((c["batch"], c["K"], c["size"], c["size"]), generator=torch.Generator().manual_seed(3),
+                     dtype=torch.float64)
+    runs = []
+    for at in (None, "own"):
+        record = {}
+        with torch.enable_grad():
+            g = leaf_params(sd, torch.float64)
+            if at == "own":
+                prior_logits_tf32(leaf_params(sd, torch.float64), x, lab, c["n_layers"], c.get("layers"),
+                                  record=record)
+                at, record = record, {}
+            lg = prior_logits_tf32(g, x, lab, c["n_layers"], c.get("layers"), at=at, record=record)
+            (prior_loss(lg, x) if kind == "ce" else (lg * up).sum()).backward()
+        assert list(record) == saved_points(c["n_layers"])
+        runs.append((lg.detach(), {k: v.grad for k, v in g.items()}))
+    (l0, g0), (l1, g1) = runs
+    assert float((l1 - l0).abs().max()) <= 1e-12 * float(l0.abs().max())
+    for k in g0:
+        assert float((g1[k] - g0[k]).abs().max()) <= 1e-12 * max(float(g0[k].abs().max()), 1e-300), k
+
+
+@pytest.mark.parametrize("B,H,W,dim,L", [(3, 5, 5, 32, 4), (1, 1, 1, 32, 1), (2, 6, 6, 96, 3), (3, 29, 29, 64, 3)])
+def test_saved_decoder_round_trips_and_spans_the_library_buffer(B, H, W, dim, L):
+    """Grids written at their offsets come back unchanged (no two overlap), the one grid left unnamed is the 2*dim
+    scratch between a layer's launches, and the length is vqb_prior_train_saved_bytes."""
+    from vqvae_b200 import _lib
+    off, total = saved_offsets(B, H, W, dim, L)
+    assert 4 * total == _lib.lib().vqb_prior_train_saved_bytes(B, H, W, dim, L)
+    gen = torch.Generator().manual_seed(L)
+    grids = {k: torch.randn((B, c, H, W), generator=gen).double() for k, (_, c) in off.items()}
+    buf = encode_saved(grids, B, H, W, dim, L)
+    assert buf.numel() == total and int(buf.isnan().sum()) == 2 * B * H * W * dim
+    got = decode_saved(buf.view(torch.uint8), B, H, W, dim, L)
+    assert set(got) == set(grids) >= set(saved_points(L)) | {"xv0"}
+    assert all(got[k].dtype == torch.float64 and torch.equal(got[k], grids[k]) for k in grids)
