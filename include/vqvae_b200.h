@@ -583,6 +583,55 @@ int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *codes, cons
                             int B, int H, int W, float *log_prob, float *pos_log_prob, void *workspace,
                             size_t workspace_bytes, void *stream);
 
+/* ---- Gated PixelCNN prior: the training cross-entropy without the logits (fp32 and TF32) -------------------------
+ * The reference's loss, nn.CrossEntropyLoss(reduction)(logits.permute(0, 2, 3, 1).reshape(-1, K), codes.reshape(-1)),
+ * with the logits of vqb_prior_forward_f32 (or _tf32) and codes clamped to [0, input_dim - 1], and its gradient with
+ * respect to every parameter, without storing the B*K*H*W logits or their gradient.
+ * Forward: vqb_prior_log_prob_*'s layer walk and head, then the finish.  The per-position loss is -lp[b, p] of
+ * vqb_prior_log_prob_* bitwise; VQB_PRIOR_CE_SUM is their sum in fp64 (thread t of one 1024-thread block adds
+ * positions t, t + 1024, ... in order, then a pairwise tree over the threads), rounded to fp32 once, and
+ * VQB_PRIOR_CE_MEAN that fp64 sum over B*H*W, rounded once.  With `saved` non-NULL the walk is the training forward's
+ * (vqb_prior_forward_train_*): `saved` receives bitwise that call's activations, then each position's (M, logf(S)).
+ * Backward: the head's products per chunk of P = min(4096, B*H*W) positions in raster order: the chunk's logits are
+ * recomputed (bitwise the forward's) and turned into d_l[n, k] = g_n * (expf((l_k - M) - logf(S)) - [k = c_n]) in a
+ * P x K buffer (g_n = d_loss[n] for VQB_PRIOR_CE_NONE, d_loss[0] / (B*H*W) for MEAN, d_loss[0] for SUM), which feed
+ * d_hidden and the output_conv.2 gradient; the chunks' output_conv.2 partials are added in chunk order.  The rest is
+ * vqb_prior_backward_*'s, with the embedding gradient's position chunks bounded in number.  No buffer grows with
+ * B*H*W*K.  Checks and limits are vqb_prior_forward_*'s, plus the reduction (VQB_ERR_BAD_ARG); any layer 0 is taken.
+ * Deterministic (no float atomics; two calls are bitwise equal), no host synchronisation.
+ * Launches, forward: fp32 3 + 2*n_layers, TF32 4 + 4*n_layers, one more for MEAN and SUM; backward, both
+ * precisions: 5 + 10*n_layers + 3*ceil(B*H*W / 4096).                                                            */
+#define VQB_PRIOR_CE_NONE 0     /* loss (B, H, W) */
+#define VQB_PRIOR_CE_MEAN 1     /* loss (1): the mean over B*H*W positions */
+#define VQB_PRIOR_CE_SUM 2      /* loss (1): the sum */
+/* Bytes of the forward's `saved`: vqb_prior_train_saved_bytes + 8*B*H*W (0 = bad sizes).                           */
+size_t vqb_prior_ce_saved_bytes(int B, int H, int W, int dim, int n_layers);
+/* Forward workspace (0 = bad sizes).  train = 0 (saved NULL): vqb_prior_log_prob_workspace_bytes(_tf32) + 4*B*H*W;
+ * train = 1: 4*B*H*W*(3*splits + 1), splits 1 in fp32 and vqb_prior_log_prob_workspace_bytes_tf32's in TF32.     */
+size_t vqb_prior_ce_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K, int train);
+size_t vqb_prior_ce_workspace_bytes_tf32(int B, int H, int W, int dim, int n_layers, int K, int train);
+/* loss: (B, H, W) fp32 for VQB_PRIOR_CE_NONE, one fp32 otherwise.  saved: NULL (inference), or
+ * vqb_prior_ce_saved_bytes for the backward.                                                                      */
+int vqb_prior_ce_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                             int W, int reduction, float *loss, void *saved, size_t saved_bytes, void *workspace,
+                             size_t workspace_bytes, void *stream);
+int vqb_prior_ce_forward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                              int W, int reduction, float *loss, void *saved, size_t saved_bytes, void *workspace,
+                              size_t workspace_bytes, void *stream);
+/* Backward workspace, both precisions (0 = bad arguments): vqb_prior_backward_workspace_bytes's regions without the
+ * output_conv.2 partials and with at most ceil(264 / tiles) embedding-gradient chunks, plus 4*P*K bytes for d_l and
+ * 4*s*K*513 for the output_conv.2 partials, s the chunks of a 513-column gradient over P positions (ffma_gemm.cuh). */
+size_t vqb_prior_ce_backward_workspace_bytes(const vqb_prior_net *net, int B, int H, int W);
+/* Every parameter gradient (overwritten, as vqb_prior_backward_*) from d_loss, the upstream gradient in device memory
+ * ((B, H, W) fp32 for VQB_PRIOR_CE_NONE, one fp32 otherwise), and the `saved` of a vqb_prior_ce_forward_* call with
+ * the same net, inputs, reduction and precision.                                                                  */
+int vqb_prior_ce_backward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                              int W, int reduction, const float *d_loss, const void *saved,
+                              const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes, void *stream);
+int vqb_prior_ce_backward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                               int W, int reduction, const float *d_loss, const void *saved,
+                               const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- optimizer step on device: Adam over many tensors, then every weight packing refreshed --------------------
  * One training step's update of a parameter group is two calls, each normally ONE launch: vqb_adam_multi_f32 updates
  * every parameter and its moments, then vqb_repack_multi rebuilds every packing read from those parameters and

@@ -90,6 +90,14 @@ SIGNATURES = {
     "vqb_prior_log_prob_workspace_bytes_tf32": (_sz, [_i] * 6),
     "vqb_prior_log_prob_f32": (_i, [_vp] * 3 + [_i64] + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
     "vqb_prior_log_prob_tf32": (_i, [_vp] * 3 + [_i64] + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
+    "vqb_prior_ce_saved_bytes": (_sz, [_i] * 5),
+    "vqb_prior_ce_workspace_bytes": (_sz, [_i] * 7),
+    "vqb_prior_ce_workspace_bytes_tf32": (_sz, [_i] * 7),
+    "vqb_prior_ce_forward_f32": (_i, [_vp] * 3 + [_i] * 4 + [_vp, _vp, _sz, _vp, _sz, _vp]),
+    "vqb_prior_ce_forward_tf32": (_i, [_vp] * 3 + [_i] * 4 + [_vp, _vp, _sz, _vp, _sz, _vp]),
+    "vqb_prior_ce_backward_workspace_bytes": (_sz, [_vp] + [_i] * 3),
+    "vqb_prior_ce_backward_f32": (_i, [_vp] * 3 + [_i] * 4 + [_vp] * 4 + [_sz, _vp]),
+    "vqb_prior_ce_backward_tf32": (_i, [_vp] * 3 + [_i] * 4 + [_vp] * 4 + [_sz, _vp]),
     "vqb_relu_backward_f32": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "vqb_conv_wgrad_workspace_bytes": (_sz, [_i] * 10),
     "vqb_conv_wgrad_f32": (_i, [_vp] * 4 + [_i] * 12 + [_vp, _sz, _vp]),

@@ -307,9 +307,10 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
 // target the clamped code codes[b, i, j].  A block owns all K logits of its P positions: each thread keeps a running
 // log-sum-exp per slot over its codes k = tid (mod NT), then the warps' pairs are merged by xor butterflies and the
 // eight warps' in warp order.
+// keep.p != nullptr (the cross-entropy's training forward) also stores the hidden layer there, as head_kernel does.
 template <int P>
 __global__ void __launch_bounds__(NT) lse_head_kernel(Net n, Act in, const long long *labels, const long long *codes,
-                                                      int B, int H, int W, float *part) {
+                                                      int B, int H, int W, float *part, Act keep) {
     __shared__ __align__(16) Smem<P> s;
     __shared__ float t[P], wm[NT / 32][P], wsum[NT / 32][P];
     set_slots(s, B, 0, H, 0, W, labels, n.NC);
@@ -321,7 +322,7 @@ __global__ void __launch_bounds__(NT) lse_head_kernel(Net n, Act in, const long 
         sink.tgt[p] = s.b[p] >= 0 ? clampi(codes[((long long)s.b[p] * H + s.r[p]) * W + s.c[p]], n.K) : -1;
     }
     sink.t = t;
-    head_positions(s, n, in, sink, H, W, Act{});
+    head_positions(s, n, in, sink, H, W, keep);
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
 #pragma unroll
     for (int p = 0; p < P; ++p) {
@@ -746,6 +747,26 @@ Act forward_layers(const Net &n, const long long *codes, const long long *lab, i
     return x[(n.L - 1) & 1];
 }
 
+// The training forward's walk up to the head: the same kernels as forward_layers, every activation into the Saved
+// layout at sp (the three stores the backward needs switched on).  Returns x_h of the last layer.  1 + 2*L launches.
+Act train_layers(const Net &n, const long long *codes, const long long *lab, int B, int H, int W, float *sp,
+                 cudaStream_t s) {
+    const long long npos = (long long)B * H * W;
+    const Saved sv{npos, n.C, n.L};
+    const Act vh{sp + sv.vh(), H, 2 * n.C};
+    embed_kernel<<<grid_for(npos * n.C), NT, 0, s>>>(codes, n.emb, npos, n.K, n.C, sp + sv.xv(0));
+    for (int l = 0; l < n.L; ++l) {
+        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xv(l), H, n.C},
+                                                        Act{sp + sv.xv(l + 1), H, n.C}, vh, lab, n.NC, B, H, W, 0, H,
+                                                        Act{sp + sv.hv(l), H, 2 * n.C});
+        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xh(l), H, n.C}, vh,
+                                                         Act{sp + sv.xh(l + 1), H, n.C}, lab, n.NC, B, H, W, 0,
+                                                         H, 0, W, Act{sp + sv.ph(l), H, 2 * n.C});
+    }
+    VQB_COUNT_LAUNCH(1 + 2 * n.L);
+    return Act{sp + sv.xh(n.L), H, n.C};
+}
+
 }  // namespace
 
 extern "C" int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
@@ -785,7 +806,7 @@ extern "C" int vqb_prior_log_prob_f32(const vqb_prior_net *net, const int64_t *c
     float *ws = static_cast<float *>(workspace);
     float *part = ws + vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K) / sizeof(float);
     const Act xL = forward_layers(n, cd, lab, B, H, W, ws, s);
-    lse_head_kernel<PF><<<blocks((long long)B * H * W, PF), NT, 0, s>>>(n, xL, lab, cd, B, H, W, part);
+    lse_head_kernel<PF><<<blocks((long long)B * H * W, PF), NT, 0, s>>>(n, xL, lab, cd, B, H, W, part, Act{});
     log_prob_finish_kernel<<<B, NT, 0, s>>>(part, 1, (long long)H * W, n_given, log_prob, pos_log_prob);
     VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());
@@ -879,20 +900,53 @@ extern "C" int vqb_prior_forward_train_f32(const vqb_prior_net *net, const int64
     const long long npos = (long long)B * H * W;
     const Saved sv{npos, n.C, n.L};
     float *sp = static_cast<float *>(saved);
-    const Act vh{sp + sv.vh(), H, 2 * n.C};
-    embed_kernel<<<grid_for(npos * n.C), NT, 0, s>>>(reinterpret_cast<const long long *>(codes), net->embedding, npos,
-                                                     n.K, n.C, sp + sv.xv(0));
-    for (int l = 0; l < n.L; ++l) {
-        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xv(l), H, n.C},
-                                                        Act{sp + sv.xv(l + 1), H, n.C}, vh, lab, n.NC, B, H, W, 0, H,
-                                                        Act{sp + sv.hv(l), H, 2 * n.C});
-        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xh(l), H, n.C}, vh,
-                                                         Act{sp + sv.xh(l + 1), H, n.C}, lab, n.NC, B, H, W, 0,
-                                                         H, 0, W, Act{sp + sv.ph(l), H, 2 * n.C});
-    }
+    train_layers(n, reinterpret_cast<const long long *>(codes), lab, B, H, W, sp, s);
     head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, Act{sp + sv.xh(n.L), H, n.C}, lab, B, H, W, logits,
                                                     Act{sp + sv.hid(), H, HID});
-    VQB_COUNT_LAUNCH(2 + 2 * n.L);
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" size_t vqb_prior_ce_saved_bytes(int B, int H, int W, int dim, int n_layers) {
+    if (B <= 0 || H <= 0 || W <= 0 || dim <= 0 || n_layers <= 0) return 0;
+    return (size_t)ce_saved_floats(Saved{(long long)B * H * W, dim, n_layers}) * sizeof(float);
+}
+
+extern "C" size_t vqb_prior_ce_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K, int train) {
+    const size_t base = vqb_prior_log_prob_workspace_bytes(B, H, W, dim, n_layers, K);
+    if (!base) return 0;
+    const size_t npos = (size_t)B * H * W;
+    return (train ? 3 * npos * sizeof(float) : base) + npos * sizeof(float);
+}
+
+// log_prob's launches with the finish of the cross-entropy; with `saved`, train_layers in place of forward_layers and
+// the hidden layer kept, so that `saved` is bitwise vqb_prior_forward_train_f32's.  Workspace: the forward's (saved
+// NULL), then one partial per position, then the per-position losses of MEAN and SUM.
+extern "C" int vqb_prior_ce_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                        int H, int W, int reduction, float *loss, void *saved, size_t saved_bytes,
+                                        void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = ce_args(net, n, codes, labels, B, H, W, reduction, loss, workspace);
+    if (st) return st;
+    if (saved && saved_bytes < vqb_prior_ce_saved_bytes(B, H, W, n.C, n.L)) return VQB_ERR_WORKSPACE;
+    if (workspace_bytes < vqb_prior_ce_workspace_bytes(B, H, W, n.C, n.L, n.K, saved != nullptr))
+        return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *lab = reinterpret_cast<const long long *>(labels), *cd = reinterpret_cast<const long long *>(codes);
+    const long long npos = (long long)B * H * W;
+    const Saved sv{npos, n.C, n.L};
+    float *ws = static_cast<float *>(workspace), *sp = static_cast<float *>(saved);
+    float *part = ws + (saved ? 0 : vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K) / sizeof(float));
+    Act xL, keep{};
+    if (saved) {
+        xL = train_layers(n, cd, lab, B, H, W, sp, s);
+        keep = Act{sp + sv.hid(), H, HID};
+    } else {
+        xL = forward_layers(n, cd, lab, B, H, W, ws, s);
+    }
+    lse_head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, xL, lab, cd, B, H, W, part, keep);
+    VQB_COUNT_LAUNCH(1 + ce_finish(s, part, 1, npos, reduction, loss, saved ? sp + sv.total() : nullptr,
+                                   part + 3 * npos));
     return vqb_cuda_status(cudaGetLastError());
 }
 

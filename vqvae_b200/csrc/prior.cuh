@@ -69,8 +69,9 @@ inline int net_from(const vqb_prior_net *net, Net &n) {
 // (-INFINITY when the code lies outside the range).  Partials of position g (g = (b*H + i)*W + j) are
 // part[(g*splits + z)*3 + {0, 1, 2}] for ranges z = 0 .. splits-1.
 
-// lp = (l_t - M) - logf(S) with M = max_z M_z, S = sum over z in order of S_z * expf(M_z - M), l_t = max_z l_t_z
-__device__ __forceinline__ float lp_of(const float *q, int splits) {
+// lp = (l_t - M) - logf(S) with M = max_z M_z, S = sum over z in order of S_z * expf(M_z - M), l_t = max_z l_t_z.
+// lse: nullptr, or where (M, logf(S)) go (the cross-entropy's backward reads softmax_k = expf((l_k - M) - logf(S)))
+__device__ __forceinline__ float lp_of(const float *q, int splits, float *lse = nullptr) {
     float M = -INFINITY, lt = -INFINITY;
     for (int z = 0; z < splits; ++z) {
         M = fmaxf(M, q[3 * z]);
@@ -78,7 +79,12 @@ __device__ __forceinline__ float lp_of(const float *q, int splits) {
     }
     float S = 0.f;
     for (int z = 0; z < splits; ++z) S += q[3 * z + 1] * expf(q[3 * z] - M);
-    return (lt - M) - logf(S);
+    const float ls = logf(S);
+    if (lse) {
+        lse[0] = M;
+        lse[1] = ls;
+    }
+    return (lt - M) - ls;
 }
 
 // One block per image: every position's lp into pos (if non-null), and into log_prob[b] (if non-null) the
@@ -123,6 +129,54 @@ inline int log_prob_args(const vqb_prior_net *net, Net &n, const int64_t *codes,
     return 0;
 }
 
+// ---- the cross-entropy (vqb_prior_ce_*): log_prob's head partials, then the loss ----------------------------------
+// Every position g's loss -lp (lp_of: bitwise -log_prob's term) into loss[g], and (M, logf(S)) into lse[2g], lse[2g+1]
+// (lse == nullptr: not kept)
+__global__ void __launch_bounds__(NT) ce_finish_kernel(const float *__restrict__ part, int splits, long long npos,
+                                                       float *__restrict__ loss, float *__restrict__ lse) {
+    for (long long g = (long long)blockIdx.x * NT + threadIdx.x; g < npos; g += (long long)gridDim.x * NT)
+        loss[g] = -lp_of(part + g * splits * 3, splits, lse ? lse + 2 * g : nullptr);
+}
+
+// One block: *out = (sum of loss[0 .. npos)) / div, rounded to fp32 once.  The sum is fp64 in a fixed order: thread t
+// adds positions t, t + CE_RT, t + 2*CE_RT, ... in turn, then the threads' sums meet in a pairwise tree.
+constexpr int CE_RT = 1024;
+__global__ void __launch_bounds__(CE_RT) ce_total_kernel(const float *__restrict__ loss, long long npos, double div,
+                                                         float *__restrict__ out) {
+    __shared__ double s[CE_RT];
+    double a = 0.0;
+    for (long long g = threadIdx.x; g < npos; g += CE_RT) a += loss[g];
+    s[threadIdx.x] = a;
+    __syncthreads();
+    for (int h = CE_RT / 2; h > 0; h >>= 1) {
+        if (threadIdx.x < h) s[threadIdx.x] += s[threadIdx.x + h];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *out = (float)(s[0] / div);
+}
+
+// The finish of both precisions' forwards: reduction "none" writes the per-position loss to out, "mean" and "sum" to
+// `scratch` and then the scalar to out.  1 or 2 launches, returned.
+inline int ce_finish(cudaStream_t st, const float *part, int splits, long long npos, int reduction, float *out,
+                     float *lse, float *scratch) {
+    float *loss = reduction == VQB_PRIOR_CE_NONE ? out : scratch;
+    ce_finish_kernel<<<grid_for(npos), NT, 0, st>>>(part, splits, npos, loss, lse);
+    if (reduction == VQB_PRIOR_CE_NONE) return 1;
+    ce_total_kernel<<<1, CE_RT, 0, st>>>(loss, npos, reduction == VQB_PRIOR_CE_MEAN ? (double)npos : 1.0, out);
+    return 2;
+}
+
+// The cross-entropy entry points' checks shared by both precisions and directions, in their order; fills n.
+inline int ce_args(const vqb_prior_net *net, Net &n, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                   int reduction, const float *loss, const void *workspace) {
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!codes || !labels || !loss || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    if (reduction != VQB_PRIOR_CE_NONE && reduction != VQB_PRIOR_CE_MEAN && reduction != VQB_PRIOR_CE_SUM)
+        return VQB_ERR_BAD_ARG;
+    return 0;
+}
+
 // Activations the training forward keeps for the backward, in floats; N = B*H*W positions, all NHWC grids:
 //   xv[l], l = 0..L   input of layer l's vertical stack (xv[0] the embedding, also x_h of layer 0); xv[L] unused
 //   xh[l], l = 1..L   input of layer l's horizontal stack (xh[L] the head's input)
@@ -140,6 +194,9 @@ struct Saved {
     long long hid() const { return (6 * L + 3) * N * C; }
     long long total() const { return hid() + N * HID; }
 };
+
+// The cross-entropy forward's `saved`: Saved, then each position's (M, logf(S)) at total() (ce_finish_kernel's lse)
+inline long long ce_saved_floats(const Saved &sv) { return sv.total() + 2 * sv.N; }
 
 // What one layer's training forward (vqb_prior_layer_forward_train_f32) keeps, in floats, NHWC (2C) grids: hv and
 // ph as in Saved.

@@ -181,6 +181,36 @@ struct VertBack {
     }
 };
 
+// Partial, added to what the earlier chunks of positions left there (first: the first chunk, which stores)
+struct PartialAdd {
+    float *part;
+    long long M, cols;
+    bool first;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        float &o = part[(long long)blockIdx.z * M * cols + (long long)m * cols + n];
+        o = first ? v : o + v;
+    }
+};
+
+// The cross-entropy's d_logits of row m of a chunk of positions starting at c0, from logit n without its bias:
+// l = v + bias (bitwise the forward's logit), d = g * (expf((l - M) - logS) - [n = c]), into out[m][n] (ld K).
+// g = d_loss[p * gstride] * scale; (M, logS) from lse[2p] (ce_finish_kernel); c the clamped code of position p.
+struct CeGrad {
+    float *out;
+    const float *bias, *lse, *d_loss;
+    const long long *codes;
+    float scale;
+    int K, gstride;
+    long long c0;
+    __device__ __forceinline__ void operator()(int m, int n, float v) const {
+        const long long p = c0 + m;
+        const float l = v + __ldg(bias + n);
+        const float q = expf((l - __ldg(lse + 2 * p)) - __ldg(lse + 2 * p + 1));
+        const float g = __ldg(d_loss + p * gstride) * scale;
+        out[(long long)m * K + n] = g * (n == clampi(codes[p], K) ? q - 1.f : q);
+    }
+};
+
 // ---- epilogues of the TF32 forward ------------------------------------------------------------------------------
 struct BiasStore {                // out[m][n] = v + bias[n] (+ add[m][n])
     float *out;
@@ -248,6 +278,16 @@ void product(cudaStream_t st, LA a, LB b, EP ep, int M, int N, int K) {
     G::run(st, a, b, ep, M, N, K, WgradSplit{1, K});
 }
 
+// The split of a reduction over npos positions whose partials must not grow with npos: about two CTAs per SM over
+// the gradient's tiles, never more chunks than that
+WgradSplit bounded_split(int M, int N, long long npos) {
+    const long long tiles = (long long)wgrad_cdiv(M, BM) * wgrad_cdiv(N, BN);
+    long long s = wgrad_cdiv(2 * 132, tiles);
+    s = s < wgrad_cdiv(npos, BK) ? s : wgrad_cdiv(npos, BK);
+    const int chunk = wgrad_cdiv(wgrad_cdiv(npos, s), BK) * BK;
+    return {wgrad_cdiv(npos, chunk), chunk};
+}
+
 // A wgrad job in the partial region: M x cols partials of a reduction over `npos` positions, at `off` floats.
 struct WJob {
     int M, Cin, taps;
@@ -263,10 +303,10 @@ struct Phase {
     WJob job[MAX_JOBS];
     int n = 0;
     long long floats = 0;
-    WJob &add(int M, int Cin, int taps, bool bias, long long npos) {
+    WJob &add(int M, int Cin, int taps, bool bias, long long npos, bool bounded = false) {
         WJob &j = job[n++];
         j.M = M; j.Cin = Cin; j.taps = taps; j.bias = bias;
-        j.sp = wgrad_split(M, j.cols(), npos, BM, BN, BK);
+        j.sp = bounded ? bounded_split(M, j.cols(), npos) : wgrad_split(M, j.cols(), npos, BM, BN, BK);
         j.off = floats;
         floats += j.floats();
         return j;
@@ -276,10 +316,19 @@ struct Phase {
 int vrows(const vqb_prior_layer_weights &w) { return w.kernel / 2 + 1; }     // vert_stack (k/2 + 1, k)
 int hcols(const vqb_prior_layer_weights &w) { return w.kernel / 2 + 1; }     // horiz_stack (1, k/2 + 1)
 
-// the wgrad jobs of the head (dW2, dW1), of layer l (resid, horiz, v2h, class, vert) and of the embedding
-Phase head_phase(const Net &n, long long npos) {
+// Positions per chunk of the cross-entropy's head backward (the d_logits buffer holds CE_CHUNK x K floats)
+constexpr long long CE_CHUNK = 4096;
+long long ce_rows(long long npos) { return npos < CE_CHUNK ? npos : CE_CHUNK; }
+
+// The split of the cross-entropy's output_conv.2 gradient within one chunk of positions; its partials are added
+// chunk after chunk (PartialAdd), so they do not grow with the positions either
+WgradSplit ce_w2_split(const Net &n, long long npos) { return wgrad_split(n.K, HID + 1, ce_rows(npos), BM, BN, BK); }
+
+// the wgrad jobs of the head (dW2, dW1; the cross-entropy's dW1 only), of layer l (resid, horiz, v2h, class, vert)
+// and of the embedding (the cross-entropy's on bounded_split)
+Phase head_phase(const Net &n, long long npos, bool ce = false) {
     Phase p;
-    p.add(n.K, HID, 1, true, npos);
+    if (!ce) p.add(n.K, HID, 1, true, npos);
     p.add(HID, n.C, 1, true, npos);
     return p;
 }
@@ -294,19 +343,20 @@ Phase layer_phase(const vqb_prior_layer_weights &w, int C, int NC, long long npo
     return p;
 }
 
-Phase emb_phase(const Net &n, long long npos) {
+Phase emb_phase(const Net &n, long long npos, bool ce = false) {
     Phase p;
-    p.add(n.K, n.C, 1, false, npos);
+    p.add(n.K, n.C, 1, false, npos, ce);
     return p;
 }
 
 // workspace regions, in floats: d x_h (2 grids), d x_v (2 grids), the head's d_hidden or a layer's d pre_h, d h_vert
-// and class gradient (union), then the wgrad partials of the largest phase
+// and class gradient (union), then the wgrad partials of the largest phase; the cross-entropy's (ce) then adds one
+// chunk of d_logits (dl, ce_rows x K) and the output_conv.2 partials (acc)
 struct Bws {
-    long long gh, gv, work, part, total;
+    long long gh, gv, work, part, dl, acc, total;
 };
 
-Bws bws_layout(const Net &n, long long npos) {
+Bws bws_layout(const Net &n, long long npos, bool ce = false) {
     Bws w;
     const long long grid = npos * n.C;
     w.gh = 0;
@@ -314,14 +364,16 @@ Bws bws_layout(const Net &n, long long npos) {
     w.work = 4 * grid;
     const long long head = npos * HID, layer = 6 * grid;
     w.part = w.work + (head > layer ? head : layer);
-    long long part = head_phase(n, npos).floats;
-    const long long e = emb_phase(n, npos).floats;
+    long long part = head_phase(n, npos, ce).floats;
+    const long long e = emb_phase(n, npos, ce).floats;
     part = part > e ? part : e;
     for (int l = 0; l < n.L; ++l) {
         const long long f = layer_phase(n.layer[l], n.C, n.NC, npos).floats;
         part = part > f ? part : f;
     }
-    w.total = w.part + part;
+    w.dl = w.part + part;
+    w.acc = w.dl + (ce ? ce_rows(npos) * n.K : 0);
+    w.total = w.acc + (ce ? (long long)ce_w2_split(n, npos).splits * n.K * (HID + 1) : 0);
     return w;
 }
 
@@ -619,6 +671,50 @@ extern "C" int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *
     return vqb_cuda_status(cudaGetLastError());
 }
 
+extern "C" size_t vqb_prior_ce_workspace_bytes_tf32(int B, int H, int W, int dim, int n_layers, int K, int train) {
+    const size_t base = vqb_prior_log_prob_workspace_bytes_tf32(B, H, W, dim, n_layers, K);
+    if (!base) return 0;
+    const long long npos = (long long)B * H * W;
+    return (train ? (size_t)npos * lse_splits(npos, K) * 3 * sizeof(float) : base) + (size_t)npos * sizeof(float);
+}
+
+// vqb_prior_log_prob_tf32's launches with the finish of the cross-entropy; with `saved`, every activation in the Saved
+// layout (forward_train_tf32's walk up to the hidden layer, so `saved` is bitwise its).  Workspace: the inference
+// forward's (saved NULL), then the head's partials, then the per-position losses of MEAN and SUM.
+extern "C" int vqb_prior_ce_forward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                         int H, int W, int reduction, float *loss, void *saved, size_t saved_bytes,
+                                         void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = ce_args(net, n, codes, labels, B, H, W, reduction, loss, workspace);
+    if (st) return st;
+    if (saved && saved_bytes < vqb_prior_ce_saved_bytes(B, H, W, n.C, n.L)) return VQB_ERR_WORKSPACE;
+    if (workspace_bytes < vqb_prior_ce_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K, saved != nullptr))
+        return VQB_ERR_WORKSPACE;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long *cd = reinterpret_cast<const long long *>(codes), *lab = reinterpret_cast<const long long *>(labels);
+    const int npos = B * H * W;
+    float *ws = static_cast<float *>(workspace), *sp = static_cast<float *>(saved), *part, *hid;
+    if (saved) {
+        const Saved lay{npos, n.C, n.L};
+        forward_hid_tf32(s, n, cd, lab, B, H, W, sp, lay);
+        hid = sp + lay.hid();
+        part = ws;
+    } else {
+        const TcWs lay{npos, n.C};
+        forward_hid_tf32(s, n, cd, lab, B, H, W, ws, lay);
+        hid = ws + lay.hid();
+        part = ws + lay.total();
+    }
+    const Mat a{hid, HID}, b{n.w2, n.K};
+    if (tc_bn(n.K) == 64) tc_lse_launch<64>(s, a, b, n.b2, cd, npos, n.K, HID, part);
+    else tc_lse_launch<128>(s, a, b, n.b2, cd, npos, n.K, HID, part);
+    const int splits = lse_splits(npos, n.K);
+    VQB_COUNT_LAUNCH(3 + 4 * n.L + ce_finish(s, part, splits, npos, reduction, loss,
+                                             saved ? sp + Saved{npos, n.C, n.L}.total() : nullptr,
+                                             part + (long long)npos * splits * 3));
+    return vqb_cuda_status(cudaGetLastError());
+}
+
 extern "C" size_t vqb_prior_backward_workspace_bytes(const vqb_prior_net *net, int B, int H, int W) {
     Net n;
     if (net_from(net, n) || B <= 0 || H <= 0 || W <= 0) return 0;
@@ -626,6 +722,34 @@ extern "C" size_t vqb_prior_backward_workspace_bytes(const vqb_prior_net *net, i
 }
 
 namespace {
+
+// The layers, last to first, from d x_h of the last layer in gh[0] (wl's regions), then the embedding (ce: on the
+// cross-entropy's bounded split).  Returns the launches: 10*L + 2.
+template <class G>
+unsigned long long body_backward(cudaStream_t st, const Net &n, const long long *codes, const long long *lab, Grid g,
+                                 int npos, const float *sp, const vqb_prior_grads *grads, float *ws, const Bws &wl,
+                                 bool ce) {
+    const int C = n.C;
+    const long long grid = (long long)npos * C;
+    const Saved sv{npos, C, n.L};
+    float *gh[2] = {ws + wl.gh, ws + wl.gh + grid}, *gv[2] = {ws + wl.gv, ws + wl.gv + grid};
+    float *part = ws + wl.part;
+    // gh[cur] = d x_h^{l+1}, gv[cur] = d x_v^{l+1} (none for the last layer)
+    int cur = 0;
+    for (int l = n.L - 1; l >= 0; --l) {
+        float *gho = gh[cur ^ 1];
+        // layer 0: x_v and x_h are both the embedding, so d x_v^0 + d x_h^0 is its gradient per position
+        layer_backward<G>(st, n.layer[l], grads->layers[l], C, n.NC, lab, g, npos, sp + sv.xv(l), sp + sv.xh(l),
+                          sp + sv.hv(l), sp + sv.ph(l), gh[cur], l == n.L - 1 ? nullptr : gv[cur], gho, gv[cur ^ 1],
+                          l == 0 ? gho : nullptr, ws + wl.work, part);
+        cur ^= 1;
+    }
+    // embedding: the per-position gradient summed by (clamped) code
+    const Phase p = emb_phase(n, npos, ce);
+    gemm(st, OneHot{codes, 1, n.K}, Mat{gv[cur], C}, Partial{part + p.job[0].off, n.K, C}, n.K, C, npos, p.job[0].sp);
+    reduce(st, p, part, {grads->embedding}, {nullptr});
+    return 10ULL * n.L + 2;
+}
 
 // vqb_prior_backward_f32 (G = Ffma) and vqb_prior_backward_tf32 (G = Tf32): the same products, launches and workspace
 template <class G>
@@ -640,15 +764,12 @@ int net_backward(const vqb_prior_net *net, const int64_t *codes, const int64_t *
     if (workspace_bytes < vqb_prior_backward_workspace_bytes(net, B, H, W)) return VQB_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
     const int npos = B * H * W, C = n.C, K = n.K;
-    const long long grid = (long long)npos * C;
     const long long *lab = reinterpret_cast<const long long *>(labels);
     const Saved sv{npos, C, n.L};
     const float *sp = static_cast<const float *>(saved);
     float *ws = static_cast<float *>(workspace);
     const Bws wl = bws_layout(n, npos);
-    float *gh[2] = {ws + wl.gh, ws + wl.gh + grid}, *gv[2] = {ws + wl.gv, ws + wl.gv + grid};
     float *part = ws + wl.part;
-    const Grid g{H, W};
     unsigned long long launches = 0;
 
     // head: d_hidden = relu' * (W2^T d_logits); dW2, db2; dW1, db1; d x_h^L = W1^T d_hidden
@@ -662,29 +783,64 @@ int net_backward(const vqb_prior_net *net, const int64_t *codes, const int64_t *
                HID + 1, npos, p.job[0].sp);
         G::run(st, MatT{dhid, HID}, WithOnes<Mat>{Mat{xL, C}, C}, Partial{part + p.job[1].off, HID, C + 1}, HID,
                C + 1, npos, p.job[1].sp);
-        product<G>(st, Mat{dhid, HID}, WPacked{n.w1, C, HID}, Store{gh[0], nullptr, C}, npos, C, HID);
+        product<G>(st, Mat{dhid, HID}, WPacked{n.w1, C, HID}, Store{ws + wl.gh, nullptr, C}, npos, C, HID);
         reduce(st, p, part, {grads->out2_w, grads->out1_w}, {grads->out2_b, grads->out1_b});
         launches += 5;
     }
-    // layers, last to first.  gh[cur] = d x_h^{l+1}, gv[cur] = d x_v^{l+1} (none for the last layer)
-    int cur = 0;
-    for (int l = n.L - 1; l >= 0; --l) {
-        float *gho = gh[cur ^ 1];
-        // layer 0: x_v and x_h are both the embedding, so d x_v^0 + d x_h^0 is its gradient per position
-        layer_backward<G>(st, n.layer[l], grads->layers[l], C, n.NC, lab, g, npos, sp + sv.xv(l), sp + sv.xh(l),
-                          sp + sv.hv(l), sp + sv.ph(l), gh[cur], l == n.L - 1 ? nullptr : gv[cur], gho, gv[cur ^ 1],
-                          l == 0 ? gho : nullptr, ws + wl.work, part);
-        launches += 10;
-        cur ^= 1;
+    launches += body_backward<G>(st, n, reinterpret_cast<const long long *>(codes), lab, Grid{H, W}, npos, sp, grads,
+                                 ws, wl, false);
+    VQB_COUNT_LAUNCH(launches);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+// vqb_prior_ce_backward_f32 (G = Ffma) and _tf32 (G = Tf32): net_backward with the head's d_logits made per chunk of
+// ce_rows positions.  Per chunk: the logits product of the forward (Mat hid x Mat W2, one k chunk: bitwise the
+// forward's logits) with the CeGrad epilogue into dl; d_hidden = relu' * (dl W2^T); dW2, db2 partials added to acc.
+// Then dW1, db1 and d x_h^L over all positions, one reduce for both head gradients, and body_backward.
+template <class G>
+int ce_backward(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                int reduction, const float *d_loss, const void *saved, const vqb_prior_grads *grads, void *workspace,
+                size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st_ = ce_args(net, n, codes, labels, B, H, W, reduction, d_loss, workspace);
+    if (st_) return st_;
+    if (!saved || !grads_ok(grads, n.L)) return VQB_ERR_BAD_ARG;
+    if (workspace_bytes < vqb_prior_ce_backward_workspace_bytes(net, B, H, W)) return VQB_ERR_WORKSPACE;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int npos = B * H * W, C = n.C, K = n.K;
+    const long long *cd = reinterpret_cast<const long long *>(codes);
+    const Saved sv{npos, C, n.L};
+    const float *sp = static_cast<const float *>(saved);
+    float *ws = static_cast<float *>(workspace);
+    const Bws wl = bws_layout(n, npos, true);
+    float *part = ws + wl.part, *dl = ws + wl.dl, *acc = ws + wl.acc, *dhid = ws + wl.work;
+    const float *hid = sp + sv.hid(), *xL = sp + sv.xh(n.L), *lse = sp + sv.total();
+    const int rows = (int)ce_rows(npos);
+    const WgradSplit s2 = ce_w2_split(n, npos);
+    const float scale = reduction == VQB_PRIOR_CE_MEAN ? (float)(1.0 / npos) : 1.f;
+    const int gstride = reduction == VQB_PRIOR_CE_NONE ? 1 : 0;
+    unsigned long long launches = 0;
+    for (int c0 = 0; c0 < npos; c0 += rows) {
+        const int P = npos - c0 < rows ? npos - c0 : rows;
+        const float *hc = hid + (long long)c0 * HID;
+        product<G>(st, Mat{hc, HID}, Mat{n.w2, K}, CeGrad{dl, n.b2, lse, d_loss, cd, scale, K, gstride, c0}, P, K,
+                   HID);
+        product<G>(st, Mat{dl, K}, WPacked{n.w2, HID, K}, ReluBack{dhid + (long long)c0 * HID, hc}, P, HID, K);
+        G::run(st, MatT{dl, K}, WithOnes<Mat>{Mat{hc, HID}, HID}, PartialAdd{acc, K, HID + 1, c0 == 0}, K, HID + 1, P,
+               s2);
+        launches += 3;
     }
-    // embedding: the per-position gradient summed by (clamped) code
-    {
-        const Phase p = emb_phase(n, npos);
-        gemm(st, OneHot{reinterpret_cast<const long long *>(codes), 1, K}, Mat{gv[cur], C},
-             Partial{part + p.job[0].off, K, C}, K, C, npos, p.job[0].sp);
-        reduce(st, p, part, {grads->embedding}, {nullptr});
-        launches += 2;
-    }
+    const Phase p = head_phase(n, npos, true);
+    G::run(st, MatT{dhid, HID}, WithOnes<Mat>{Mat{xL, C}, C}, Partial{part + p.job[0].off, HID, C + 1}, HID, C + 1,
+           npos, p.job[0].sp);
+    product<G>(st, Mat{dhid, HID}, WPacked{n.w1, C, HID}, Store{ws + wl.gh, nullptr, C}, npos, C, HID);
+    RJobs jobs;
+    jobs.j[0] = RJob{acc, grads->out2_w, grads->out2_b, K, HID, 1, HID + 1, s2.splits};
+    jobs.j[1] = RJob{part + p.job[0].off, grads->out1_w, grads->out1_b, HID, C, 1, C + 1, p.job[0].sp.splits};
+    const long long w2 = (long long)K * (HID + 1), w1 = (long long)HID * (C + 1);
+    wgrad_reduce(st, jobs, 2, w2 > w1 ? w2 : w1);
+    launches += 3 + body_backward<G>(st, n, cd, reinterpret_cast<const long long *>(labels), Grid{H, W}, npos, sp,
+                                     grads, ws, wl, true);
     VQB_COUNT_LAUNCH(launches);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -703,6 +859,28 @@ extern "C" int vqb_prior_backward_tf32(const vqb_prior_net *net, const int64_t *
                                        const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
                                        void *stream) {
     return net_backward<Tf32>(net, codes, labels, B, H, W, d_logits, saved, grads, workspace, workspace_bytes, stream);
+}
+
+extern "C" size_t vqb_prior_ce_backward_workspace_bytes(const vqb_prior_net *net, int B, int H, int W) {
+    Net n;
+    if (net_from(net, n) || B <= 0 || H <= 0 || W <= 0) return 0;
+    return (size_t)bws_layout(n, (long long)B * H * W, true).total * sizeof(float);
+}
+
+extern "C" int vqb_prior_ce_backward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                         int H, int W, int reduction, const float *d_loss, const void *saved,
+                                         const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
+                                         void *stream) {
+    return ce_backward<Ffma>(net, codes, labels, B, H, W, reduction, d_loss, saved, grads, workspace, workspace_bytes,
+                             stream);
+}
+
+extern "C" int vqb_prior_ce_backward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                          int H, int W, int reduction, const float *d_loss, const void *saved,
+                                          const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
+                                          void *stream) {
+    return ce_backward<Tf32>(net, codes, labels, B, H, W, reduction, d_loss, saved, grads, workspace, workspace_bytes,
+                             stream);
 }
 
 extern "C" int vqb_prior_gate_backward_f32(const float *x, const float *d_out, float *d_x, int64_t outer, int C,

@@ -641,6 +641,65 @@ def prior_log_prob(net, codes, labels, n_given, precision="fp32", per_position=F
     return out
 
 
+PRIOR_CE_REDUCTIONS = ("none", "mean", "sum")      # VQB_PRIOR_CE_NONE, _MEAN, _SUM
+
+
+def _prior_ce_reduction(reduction):
+    if reduction not in PRIOR_CE_REDUCTIONS:
+        raise ValueError(f"reduction must be one of {PRIOR_CE_REDUCTIONS}, got {reduction!r}")
+    return PRIOR_CE_REDUCTIONS.index(reduction)
+
+
+def prior_ce_forward(net, codes, labels, reduction, precision="fp32", train=False):
+    """The cross-entropy of the teacher-forced logits at int64 codes (B,H,W) (clamped to [0, K-1]) without writing the
+    logits (vqb_prior_ce_forward_f32, or _tf32 for precision="tf32") -> (loss, saved): loss (B,H,W) fp32 for
+    reduction="none", a 0-d fp32 tensor otherwise; saved None, or with train=True the uint8 buffer of
+    vqb_prior_ce_saved_bytes that prior_ce_backward reads."""
+    sfx = _prior_precision(precision)
+    r = _prior_ce_reduction(reduction)
+    B, H, W = codes.shape
+    dev = codes.device
+    saved = None
+    if train:
+        n = lib().vqb_prior_ce_saved_bytes(B, H, W, net.dim, net.n_layers)
+        if n == 0:
+            raise RuntimeError("prior: bad sizes")
+        saved = torch.empty((n,), dtype=torch.uint8, device=dev)
+    ws = _prior_workspace(net, B, H, W, dev, getattr(lib(), "vqb_prior_ce_workspace_bytes" +
+                                                     ("_tf32" if sfx == "tf32" else "")), int(train))
+    loss = torch.empty((B, H, W) if r == 0 else (), dtype=torch.float32, device=dev)
+    span = _Span(f"prior cross_entropy ({precision}, {reduction}) K={net.input_dim} dim={net.dim} L={net.n_layers} "
+                 f"{H}x{W}")
+    check(getattr(lib(), "vqb_prior_ce_forward_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H,
+                                                         W, r, loss.data_ptr(),
+                                                         saved.data_ptr() if saved is not None else None,
+                                                         saved.numel() if saved is not None else 0, ws.data_ptr(),
+                                                         ws.numel(), _stream()),
+          "prior_ce_forward")
+    span.done()
+    return loss, saved
+
+
+def prior_ce_backward(net, codes, labels, reduction, d_loss, saved, grads, precision="fp32"):
+    """Every parameter gradient of the prior's cross-entropy (vqb_prior_ce_backward_f32 / _tf32) into the tensors
+    `grads` (a PriorGrads struct) points at; d_loss fp32 contiguous on the device, (B,H,W) for reduction="none" and
+    one element otherwise, saved from prior_ce_forward(train=True) on the same net, inputs and reduction."""
+    sfx = _prior_precision(precision)
+    r = _prior_ce_reduction(reduction)
+    B, H, W = codes.shape
+    n = lib().vqb_prior_ce_backward_workspace_bytes(_lib.C.byref(net), B, H, W)
+    if n == 0:
+        raise RuntimeError("prior backward: bad sizes")
+    ws = torch.empty((n,), dtype=torch.uint8, device=codes.device)
+    span = _Span(f"prior cross_entropy backward ({precision}, {reduction}) K={net.input_dim} dim={net.dim} "
+                 f"L={net.n_layers} {H}x{W}")
+    check(getattr(lib(), "vqb_prior_ce_backward_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B,
+                                                          H, W, r, d_loss.data_ptr(), saved.data_ptr(),
+                                                          _lib.C.byref(grads), ws.data_ptr(), ws.numel(), _stream()),
+          "prior_ce_backward")
+    span.done()
+
+
 def prior_generate(net, labels, u, step_logits=None):
     """The whole sampling loop (vqb_prior_generate_f32): int64 codes (B,H,W) drawn with the uniforms u (B,H,W).
     step_logits: None, or a (B,H,W,K) fp32 tensor receiving the logits of every step."""

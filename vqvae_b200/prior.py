@@ -256,17 +256,52 @@ class _PriorFunction(torch.autograd.Function):
             raise RuntimeError("GatedPixelCNN: backward through the same forward twice is not supported "
                                "(its saved activations are freed by the first backward)")
         codes, labels = ctx.saved_tensors
-        params = dict(ctx.model.named_parameters())
-        grads = {k: torch.empty(p.shape, dtype=torch.float32, device=codes.device) for k, p in params.items()}
-        n_layers = len(ctx.model.layers)
-        layers = (PriorLayerGrads * n_layers)(*[
-            PriorLayerGrads(**{f: grads[f"layers.{i}.{k}"].data_ptr() for f, k in _LAYER_GRADS.items()})
-            for i in range(n_layers)])
-        table = PriorGrads(layers=C.cast(layers, C.POINTER(PriorLayerGrads)), n_layers=n_layers,
-                           **{f: grads[k].data_ptr() for f, k in _NET_GRADS.items()})
+        params, grads, table, _layers = _grad_table(ctx.model, codes.device)
         ops.prior_backward(ctx.net, codes, labels, _f32(d_logits), ctx.saved, table, ctx.precision)
         ctx.saved = ctx.keep = None
         return (None, None, None, None) + tuple(grads[k].to(p.dtype) for k, p in params.items())
+
+
+def _grad_table(model, dev):
+    """(parameters by name, an empty fp32 gradient per parameter, the PriorGrads struct pointing at them, its layer
+    array, which must outlive the backward call)."""
+    params = dict(model.named_parameters())
+    grads = {k: torch.empty(p.shape, dtype=torch.float32, device=dev) for k, p in params.items()}
+    n_layers = len(model.layers)
+    layers = (PriorLayerGrads * n_layers)(*[
+        PriorLayerGrads(**{f: grads[f"layers.{i}.{k}"].data_ptr() for f, k in _LAYER_GRADS.items()})
+        for i in range(n_layers)])
+    table = PriorGrads(layers=C.cast(layers, C.POINTER(PriorLayerGrads)), n_layers=n_layers,
+                       **{f: grads[k].data_ptr() for f, k in _NET_GRADS.items()})
+    return params, grads, table, layers
+
+
+class _PriorCEFunction(torch.autograd.Function):
+    """GatedPixelCNN.cross_entropy with gradients: inputs are the model, the precision, the reduction, codes, labels
+    and every parameter in ``parameters()`` order.  The forward keeps the training activations and each position's
+    log-sum-exp (vqb_prior_ce_forward_*), not the logits; the backward (vqb_prior_ce_backward_*, in the forward's
+    precision) recomputes the logits chunk by chunk and returns one gradient per parameter, as _PriorFunction does."""
+
+    @staticmethod
+    def forward(ctx, model, precision, reduction, codes, labels, *params):
+        keep = []
+        net = model._net(keep)
+        loss, saved = ops.prior_ce_forward(net, codes, labels, reduction, precision, train=True)
+        ctx.model, ctx.net, ctx.keep, ctx.saved = model, net, keep, saved
+        ctx.precision, ctx.reduction = precision, reduction
+        ctx.save_for_backward(codes, labels)
+        return loss
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        if ctx.saved is None:           # the first backward freed the saved activations
+            raise RuntimeError("GatedPixelCNN.cross_entropy: backward through the same call twice is not supported "
+                               "(its saved activations are freed by the first backward)")
+        codes, labels = ctx.saved_tensors
+        params, grads, table, _layers = _grad_table(ctx.model, codes.device)
+        ops.prior_ce_backward(ctx.net, codes, labels, ctx.reduction, _f32(d_loss), ctx.saved, table, ctx.precision)
+        ctx.saved = ctx.keep = None
+        return (None,) * 5 + tuple(grads[k].to(p.dtype) for k, p in params.items())
 
 
 class GatedPixelCNN(nn.Module):
@@ -390,9 +425,49 @@ class GatedPixelCNN(nn.Module):
 
         Never differentiable: it runs the inference kernels even with grad enabled and parameters requiring grad,
         keeps no training activations, and returns a tensor without grad.  Train with forward plus the
-        cross-entropy.  ValueError for a bad precision, n_given or per_position with n_given != 0; RuntimeError for
+        cross-entropy.  cross_entropy() is that training loss without the logits, and differentiable.  ValueError for a bad precision, n_given or per_position with n_given != 0; RuntimeError for
         forward's shape, layer (P5), label and device checks; every host-side check runs before any CUDA check."""
         return self._log_prob(x, label, n_given, per_position)
+
+    def cross_entropy(self, x, label, *, reduction="mean"):
+        """The reference's training loss without the B*K*H*W logits: int64 codes x (B,H,W) and labels (B,) (as forward
+        takes them) -> the value of nn.CrossEntropyLoss(reduction=reduction)(forward(x, label).permute(0, 2, 3, 1)
+        .reshape(-1, K), x.reshape(-1)), in the model's ``precision``: a 0-d fp32 tensor for reduction "mean" (over
+        B*H*W) or "sum", the (B,H,W) fp32 map for "none".  The "none" values are bitwise -log_prob(x, label,
+        per_position=True) in the same precision; "sum" and "mean" add them in fp64 in a fixed order (DESIGN §8.3).
+
+        Differentiable with respect to every parameter under forward's rule (grad enabled and a parameter requiring
+        grad): the call keeps the training activations and each position's log-sum-exp, and the backward recomputes
+        the logits a chunk of positions at a time, so neither the logits nor their gradient is ever stored whole.
+        Otherwise it runs the inference kernels and returns the same bits without a graph.  The upstream gradient is
+        read on the device (no host synchronisation), so the loss, its backward and vqvae_b200.optim.Adam.step()
+        capture into one CUDA graph; a second backward through the same call raises.
+
+        Codes outside [0, K-1] are clamped, as the embedding clamps them, and scored and differentiated as the clamped
+        code (torch's cross-entropy would raise).  No weight, ignore_index or label_smoothing.  Any layer stack
+        forward takes is taken.  ValueError for a bad precision or reduction; RuntimeError for forward's shape,
+        layer (P5), label and device checks; every host-side check runs before any CUDA check."""
+        what = "GatedPixelCNN.cross_entropy"
+        precision = self.precision
+        if precision not in ops.PRIOR_PRECISIONS:
+            raise ValueError(f"GatedPixelCNN.precision must be one of {ops.PRIOR_PRECISIONS}, got {precision!r}")
+        if not isinstance(reduction, str) or reduction not in ops.PRIOR_CE_REDUCTIONS:
+            raise ValueError(f"{what}: reduction must be one of {ops.PRIOR_CE_REDUCTIONS}, got {reduction!r}")
+        if x.dim() != 3:
+            raise RuntimeError(f"{what}: expected codes of shape (B,H,W), got {tuple(x.shape)}")
+        B, H, W = x.shape
+        _square(H, W, what)
+        self._check_layers()
+        n = (label if torch.is_tensor(label) else torch.as_tensor(label)).numel()
+        if n != B:
+            raise RuntimeError(f"{what}: expected {B} labels, got {n}")
+        ops._require_cuda(x, what + " codes")
+        label = _labels(label, B, x.device, what)
+        x = x.detach().to(torch.int64).contiguous()
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            return _PriorCEFunction.apply(self, precision, reduction, x, label, *self.parameters())
+        keep = []
+        return ops.prior_ce_forward(self._net(keep), x, label, reduction, precision)[0]
 
     def _check_causal(self, what):
         """P5: the sampler needs a layer 0 that reads only the codes before the one being drawn."""
