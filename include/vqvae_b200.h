@@ -369,7 +369,7 @@ int vqb_conv_wgrad_f32(const float *in, const float *g_out, float *dW, float *db
 /* ---- Gated PixelCNN prior, pixelcnn/models.py (inference, fp32 on CUDA cores) ----------------------------
  * The prior over VQ code grids: teacher-forced logits (GatedPixelCNN.forward, models.py:121-130) and the whole
  * sampling loop (GatedPixelCNN.generate, :132-143) in one call.  Activations are NHWC rows.  Shapes: dim % 32 == 0
- * and dim <= 256, 1 <= input_dim (K) <= 8192, 1 <= n_layers <= VQB_PRIOR_MAX_LAYERS, odd kernel <= 15, any
+ * and dim <= 1024 (the reference script's dim = img_dim**2 up to 32x32 latents), 1 <= input_dim (K) <= 8192, 1 <= n_layers <= VQB_PRIOR_MAX_LAYERS, odd kernel <= 15, any
  * n_classes; other dims return VQB_ERR_UNSUPPORTED.  Out-of-range codes and labels are clamped to the nearest
  * valid row in the kernels (as vqb_gather_rows_f32 does): a host-side range check would need a device sync.
  * The weight tables below are HOST structs holding device pointers; they are read during the call only.     */
@@ -520,7 +520,9 @@ int vqb_prior_layer_forward_train_f32(const vqb_prior_layer_weights *layer, cons
                                       const int64_t *labels, int B, int H, int W, int dim, int n_classes,
                                       float *out_v, float *out_h, float *vh, void *saved, size_t saved_bytes,
                                       void *stream);
-/* Workspace of vqb_prior_layer_backward_f32 (0 = bad arguments).                                                 */
+/* Workspace of vqb_prior_layer_backward_f32 (0 = bad arguments).  This pair keeps the dim <= 256 limit it was
+ * published with (VQB_ERR_UNSUPPORTED / 0 above it); vqb_prior_layer_backward_wide_* below take every dim the net
+ * takes.                                                                                                        */
 size_t vqb_prior_layer_backward_workspace_bytes(const vqb_prior_layer_weights *layer, int B, int H, int W, int dim,
                                                 int n_classes);
 /* Gradients of one layer from d_out_v, d_out_h (B,H,W,dim) NHWC, the layer's inputs x_v, x_h and the `saved` of a
@@ -533,6 +535,15 @@ int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer, const flo
                                  const float *d_out_v, const float *d_out_h, const void *saved,
                                  const vqb_prior_layer_grads *grads, float *d_x_v, float *d_x_h, void *workspace,
                                  size_t workspace_bytes, void *stream);
+/* vqb_prior_layer_backward_workspace_bytes / vqb_prior_layer_backward_f32 for dim % 32 == 0 up to 1024: the same
+ * arguments, checks, launches and bits.                                                                         */
+size_t vqb_prior_layer_backward_wide_workspace_bytes(const vqb_prior_layer_weights *layer, int B, int H, int W,
+                                                     int dim, int n_classes);
+int vqb_prior_layer_backward_wide_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                                      const int64_t *labels, int B, int H, int W, int dim, int n_classes,
+                                      const float *d_out_v, const float *d_out_h, const void *saved,
+                                      const vqb_prior_layer_grads *grads, float *d_x_v, float *d_x_h, void *workspace,
+                                      size_t workspace_bytes, void *stream);
 
 /* ---- Gated PixelCNN prior in TF32 (wgmma tensor cores) ---------------------------------------------------------
  * The teacher-forced forward and the backward with every matrix product on a TF32 wgmma GEMM: each operand is

@@ -82,6 +82,8 @@ SIGNATURES = {
     "vqb_prior_layer_forward_train_f32": (_i, [_vp] * 4 + [_i] * 5 + [_vp] * 4 + [_sz, _vp]),
     "vqb_prior_layer_backward_workspace_bytes": (_sz, [_vp] + [_i] * 5),
     "vqb_prior_layer_backward_f32": (_i, [_vp] * 4 + [_i] * 5 + [_vp] * 7 + [_sz, _vp]),
+    "vqb_prior_layer_backward_wide_workspace_bytes": (_sz, [_vp] + [_i] * 5),
+    "vqb_prior_layer_backward_wide_f32": (_i, [_vp] * 4 + [_i] * 5 + [_vp] * 7 + [_sz, _vp]),
     "vqb_prior_workspace_bytes_tf32": (_sz, [_i] * 6),
     "vqb_prior_forward_tf32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
     "vqb_prior_forward_train_tf32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),

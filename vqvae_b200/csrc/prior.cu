@@ -7,19 +7,35 @@
 // positions share a block or on how many do.  The forward's kernels and the sampler's position step call the same device functions below, so the
 // sampler's logits are bitwise the forward's logits on the grid it produced.
 #include <cfloat>
+#include <type_traits>
 
 #include "pack.cuh"
 #include "prior.cuh"
 
 namespace {
 
-// one block's positions: image, row, column and clamped label of each of its P slots (b < 0: slot unused)
-template <int P>
+// one block's positions: image, row, column and clamped label of each of its P slots (b < 0: slot unused).  Q: output
+// channels per thread of the 2*dim-wide products, so the block holds dim <= Q*NT/2 channels; Q = 2 is dim <= MAXC.
+template <int P, int Q = 2>
 struct Smem {
-    float x[MAXC * P];            // [ci][p]: one tap of the input, or the gated activations
-    float pre[HID * P];           // [c][p]: pre-activations (2*dim) or the head's hidden layer (512)
+    static constexpr int CAP = Q * NT / 2;
+    float x[CAP * P];             // [ci][p]: one tap of the input, or the gated activations
+    float pre[(Q * NT > HID ? Q * NT : HID) * P];  // [c][p]: pre-activations (2*dim) or the head's hidden layer (512)
     int b[P], r[P], c[P], lab[P];
 };
+
+// The block's Smem: static shared memory for the dim <= MAXC kernels, dynamic (above 48 KB, opted in by `wide_attr`)
+// for the wide ones
+template <int P, int Q>
+__device__ __forceinline__ Smem<P, Q> &block_smem() {
+    if constexpr (Q == 2) {
+        __shared__ __align__(16) Smem<P, Q> s;
+        return s;
+    } else {
+        extern __shared__ __align__(16) unsigned char wide_smem[];
+        return *reinterpret_cast<Smem<P, Q> *>(wide_smem);
+    }
+}
 
 template <int P>
 __device__ __forceinline__ void load_vec(float (&v)[P], const float *s) {
@@ -56,8 +72,8 @@ __device__ __forceinline__ void mac(float (&acc)[Q][P], const float *xs, const f
 }
 
 // x[ci][p] = in at (b, r + dy, c + dx) of slot p, 0 outside the grid or for an unused slot
-template <int P>
-__device__ __forceinline__ void load_tap(Smem<P> &s, const Act &in, int dy, int dx, int H, int W) {
+template <int P, int Q>
+__device__ __forceinline__ void load_tap(Smem<P, Q> &s, const Act &in, int dy, int dx, int H, int W) {
     const int C = in.C;
     for (int i = threadIdx.x; i < P * C; i += NT) {
         const int p = i / C, ci = i % C;
@@ -77,13 +93,13 @@ __device__ __forceinline__ int horiz_cols(const vqb_prior_layer_weights &w) { re
 //   h_vert = vert_stack(x_v) ; out_v = gate(h_vert + emb[label]) ; vh = vert_to_horiz(h_vert) + emb[label]
 // keep.p != nullptr (the training forward) also stores h_vert there for the backward.  vh.p == nullptr skips vh
 // (completion's prefix rows, whose horizontal stacks never run).
-template <int P>
-__device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &out_v,
+template <int P, int Q>
+__device__ void vert_positions(Smem<P, Q> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &out_v,
                                const Act &vh, int H, int W, const Act &keep) {
     const int C = in.C, C2 = 2 * C, tid = threadIdx.x;
-    float acc[2][P];
+    float acc[Q][P];
 #pragma unroll
-    for (int q = 0; q < 2; ++q)
+    for (int q = 0; q < Q; ++q)
 #pragma unroll
         for (int p = 0; p < P; ++p) acc[q][p] = 0.f;
     const int rows = vert_rows(w), k = w.kernel, half = k / 2;
@@ -92,10 +108,10 @@ __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, con
             __syncthreads();
             load_tap(s, in, tr - half, tc - half, H, W);
             __syncthreads();
-            mac<P, 2>(acc, s.x, w.vert_w + (long long)(tr * k + tc) * C * C2, C, C2, 0);
+            mac<P, Q>(acc, s.x, w.vert_w + (long long)(tr * k + tc) * C * C2, C, C2, 0);
         }
 #pragma unroll
-    for (int q = 0; q < 2; ++q) {
+    for (int q = 0; q < Q; ++q) {
         const int c = tid + q * NT;
         if (c < C2)
 #pragma unroll
@@ -113,12 +129,12 @@ __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, con
     }
     if (!vh.p) return;
 #pragma unroll
-    for (int q = 0; q < 2; ++q)
+    for (int q = 0; q < Q; ++q)
 #pragma unroll
         for (int p = 0; p < P; ++p) acc[q][p] = 0.f;
-    mac<P, 2>(acc, s.pre, w.v2h_w, C2, C2, 0);
+    mac<P, Q>(acc, s.pre, w.v2h_w, C2, C2, 0);
 #pragma unroll
-    for (int q = 0; q < 2; ++q) {
+    for (int q = 0; q < Q; ++q) {
         const int c = tid + q * NT;
         if (c >= C2) continue;
 #pragma unroll
@@ -133,13 +149,13 @@ __device__ void vert_positions(Smem<P> &s, const vqb_prior_layer_weights &w, con
 //   out = gate(horiz_stack(x_h) + vh) ; out_h = horiz_resid(out) [+ x_h]
 // The forward's per-layer kernel and the sampler's position step both run this.  keep.p != nullptr (the training
 // forward) also stores the gate's pre-activation there.
-template <int P>
-__device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &vh,
+template <int P, int Q>
+__device__ void horiz_positions(Smem<P, Q> &s, const vqb_prior_layer_weights &w, const Act &in, const Act &vh,
                                 const Act &out_h, int H, int W, const Act &keep) {
     const int C = in.C, C2 = 2 * C, tid = threadIdx.x;
-    float acc[2][P];
+    float acc[Q][P];
 #pragma unroll
-    for (int q = 0; q < 2; ++q)
+    for (int q = 0; q < Q; ++q)
 #pragma unroll
         for (int p = 0; p < P; ++p) acc[q][p] = 0.f;
     const int cols = horiz_cols(w), half = w.kernel / 2;
@@ -147,10 +163,10 @@ __device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, co
         __syncthreads();
         load_tap(s, in, 0, tc - half, H, W);
         __syncthreads();
-        mac<P, 2>(acc, s.x, w.horiz_w + (long long)tc * C * C2, C, C2, 0);
+        mac<P, Q>(acc, s.x, w.horiz_w + (long long)tc * C * C2, C, C2, 0);
     }
 #pragma unroll
-    for (int q = 0; q < 2; ++q) {
+    for (int q = 0; q < Q; ++q) {
         const int c = tid + q * NT;
         if (c >= C2) continue;
 #pragma unroll
@@ -165,17 +181,23 @@ __device__ void horiz_positions(Smem<P> &s, const vqb_prior_layer_weights &w, co
         s.x[c * P + p] = gate(s.pre[c * P + p], s.pre[(c + C) * P + p]);
     }
     __syncthreads();
-    float r[1][P];
+    constexpr int R = (Q + 1) / 2;                  // output channels per thread of the dim-wide product
+    float r[R][P];
 #pragma unroll
-    for (int p = 0; p < P; ++p) r[0][p] = 0.f;
-    mac<P, 1>(r, s.x, w.resid_w, C, C, 0);
-    if (tid < C) {
+    for (int q = 0; q < R; ++q)
+#pragma unroll
+        for (int p = 0; p < P; ++p) r[q][p] = 0.f;
+    mac<P, R>(r, s.x, w.resid_w, C, C, 0);
+#pragma unroll
+    for (int q = 0; q < R; ++q) {
+        const int c = tid + q * NT;
+        if (c >= C) continue;
 #pragma unroll
         for (int p = 0; p < P; ++p) {
             if (s.b[p] < 0) continue;
-            float v = r[0][p] + __ldg(w.resid_b + tid);
-            if (w.residual) v = v + in.at(s.b[p], s.r[p], s.c[p], W)[tid];
-            out_h.at(s.b[p], s.r[p], s.c[p], W)[tid] = v;
+            float v = r[q][p] + __ldg(w.resid_b + c);
+            if (w.residual) v = v + in.at(s.b[p], s.r[p], s.c[p], W)[c];
+            out_h.at(s.b[p], s.r[p], s.c[p], W)[c] = v;
         }
     }
 }
@@ -217,8 +239,8 @@ __device__ __forceinline__ void lse_merge(float &m, float &s, float m2, float s2
 
 // output_conv (models.py:107-111): logits = W2 . relu(W1 . x_h + b1) + b2 at the P positions of the block, each
 // handed to `sink`.  keep.p != nullptr (the training forward) also stores the hidden layer there.
-template <int P, class Sink>
-__device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, Sink &sink, int H, int W, const Act &keep) {
+template <int P, int Q, class Sink>
+__device__ void head_positions(Smem<P, Q> &s, const Net &n, const Act &in, Sink &sink, int H, int W, const Act &keep) {
     const int C = n.C, tid = threadIdx.x;
     __syncthreads();
     load_tap(s, in, 0, 0, H, W);
@@ -250,8 +272,8 @@ __device__ void head_positions(Smem<P> &s, const Net &n, const Act &in, Sink &si
 
 // Slots of a block over the positions [row0, row0 + nrows) x [col0, col0 + ncols) of all B images, position-major in
 // (b, row, col).
-template <int P>
-__device__ void set_slots(Smem<P> &s, int B, int row0, int nrows, int col0, int ncols, const long long *labels,
+template <int P, int Q>
+__device__ void set_slots(Smem<P, Q> &s, int B, int row0, int nrows, int col0, int ncols, const long long *labels,
                           int NC) {
     if (threadIdx.x < P) {
         const int p = threadIdx.x;
@@ -269,30 +291,30 @@ __device__ void set_slots(Smem<P> &s, int B, int row0, int nrows, int col0, int 
     __syncthreads();
 }
 
-template <int P>
+template <int P, int Q = 2>
 __global__ void __launch_bounds__(NT) vert_kernel(vqb_prior_layer_weights w, Act in, Act out_v, Act vh,
                                                   const long long *labels, int NC, int B, int H, int W, int row0,
                                                   int nrows, Act keep) {
-    __shared__ __align__(16) Smem<P> s;
+    Smem<P, Q> &s = block_smem<P, Q>();
     set_slots(s, B, row0, nrows, 0, W, labels, NC);
     vert_positions(s, w, in, out_v, vh, H, W, keep);
 }
 
 // over rows [row0, row0 + nrows) x columns [col0, col0 + ncols)
-template <int P>
+template <int P, int Q = 2>
 __global__ void __launch_bounds__(NT) horiz_kernel(vqb_prior_layer_weights w, Act in, Act vh, Act out_h,
                                                    const long long *labels, int NC, int B, int H, int W, int row0,
                                                    int nrows, int col0, int ncols, Act keep) {
-    __shared__ __align__(16) Smem<P> s;
+    Smem<P, Q> &s = block_smem<P, Q>();
     set_slots(s, B, row0, nrows, col0, ncols, labels, NC);
     horiz_positions(s, w, in, vh, out_h, H, W, keep);
 }
 
 // logits NCHW (B, K, H, W)
-template <int P>
+template <int P, int Q = 2>
 __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long *labels, int B, int H, int W,
                                                   float *logits, Act keep) {
-    __shared__ __align__(16) Smem<P> s;
+    Smem<P, Q> &s = block_smem<P, Q>();
     __shared__ float *out[P];
     set_slots(s, B, 0, H, 0, W, labels, n.NC);
     if (threadIdx.x < P) {
@@ -308,10 +330,10 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
 // log-sum-exp per slot over its codes k = tid (mod NT), then the warps' pairs are merged by xor butterflies and the
 // eight warps' in warp order.
 // keep.p != nullptr (the cross-entropy's training forward) also stores the hidden layer there, as head_kernel does.
-template <int P>
+template <int P, int Q = 2>
 __global__ void __launch_bounds__(NT) lse_head_kernel(Net n, Act in, const long long *labels, const long long *codes,
                                                       int B, int H, int W, float *part, Act keep) {
-    __shared__ __align__(16) Smem<P> s;
+    Smem<P, Q> &s = block_smem<P, Q>();
     __shared__ float t[P], wm[NT / 32][P], wsum[NT / 32][P];
     set_slots(s, B, 0, H, 0, W, labels, n.NC);
     Lse<P> sink;
@@ -389,12 +411,12 @@ __device__ __forceinline__ float warp_max(float v) {
 // One sampling step at (i, j) for P images: every layer's horizontal stack, the head, the softmax and the inverse-CDF
 // draw.  The code goes to codes[b, i, j] and its embedding to x0[b, i, j], which later steps and row passes read.
 // `first`: the first sampled step of the call, which writes log_prob instead of adding to it.
-template <int P>
+template <int P, int Q = 2>
 __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act vh0, long long vh_stride,
                                                   long long x_stride, const long long *labels, const float *u, int B,
                                                   int H, int W, int i, int j, float *logits, long long logit_img,
                                                   long long *codes, Samp sp, bool first) {
-    __shared__ __align__(16) Smem<P> s;
+    Smem<P, Q> &s = block_smem<P, Q>();
     __shared__ float *out[P];
     if (threadIdx.x < P) {
         const int p = threadIdx.x, b = blockIdx.x * P + p;
@@ -596,8 +618,82 @@ Ws ws_layout(long long B, long long H, long long W, long long C, long long L, lo
 
 constexpr int PF = 8;             // positions per block of the whole-grid kernels and the row pass
 constexpr int PS = 4;             // images per block of the sampling step
+constexpr int PF_WIDE = 8;        // the same for dim > MAXC (DESIGN §8.4)
+constexpr int PS_WIDE = 4;
 
 unsigned blocks(long long positions, int P) { return (unsigned)((positions + P - 1) / P); }
+
+// Output channels per thread of the 2*dim-wide products: 2 up to dim = MAXC (the original instantiations), else
+// ceil(2*dim / NT), 3 .. 8
+int q_of(int C) { return 2 * C <= 2 * NT ? 2 : (2 * C + NT - 1) / NT; }
+
+// f(std::integral_constant<int, q_of(C)>{}): the per-position kernels' instantiation for dim C
+template <int Q = 2, class F>
+void by_q(int C, F &&f) {
+    if constexpr (Q < 2 * MAXC_WIDE / NT) {
+        if (q_of(C) != Q) return by_q<Q + 1>(C, f);
+    }
+    f(std::integral_constant<int, Q>{});
+}
+
+template <int Q> constexpr int pf() { return Q == 2 ? PF : PF_WIDE; }
+template <int Q> constexpr int ps() { return Q == 2 ? PS : PS_WIDE; }
+
+// Dynamic shared memory of kernel Kern, an instantiation on Smem<P, Q>: none for Q = 2; else sizeof(Smem<P, Q>),
+// opted in once (above 48 KB, at most 227 KB per block).  If the opt-in fails, so does the launch, and the caller
+// reports it.
+template <auto Kern, int P, int Q>
+size_t smem_of() {
+    if constexpr (Q == 2) {
+        return 0;
+    } else {
+        constexpr size_t bytes = sizeof(Smem<P, Q>);
+        static_assert(bytes + 1024 <= 227 * 1024, "Smem<P, Q> exceeds the H100's shared memory per block");
+        static bool attr_set = false;
+        if (!attr_set)
+            attr_set = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess;
+        return bytes;
+    }
+}
+
+// The per-position kernels' launches at dim = in.C's instantiation (vert_kernel's and horiz_kernel's over rows
+// [row0, row0 + nrows) x columns [col0, col0 + ncols) of B images; the heads over every position)
+void launch_vert(cudaStream_t s, const vqb_prior_layer_weights &w, const Act &in, const Act &out_v, const Act &vh,
+                 const long long *lab, int NC, int B, int H, int W, int row0, int nrows, const Act &keep) {
+    by_q(in.C, [&](auto q) {
+        constexpr int Q = decltype(q)::value, P = pf<Q>();
+        vert_kernel<P, Q><<<blocks((long long)B * nrows * W, P), NT, smem_of<vert_kernel<P, Q>, P, Q>(), s>>>(
+            w, in, out_v, vh, lab, NC, B, H, W, row0, nrows, keep);
+    });
+}
+
+void launch_horiz(cudaStream_t s, const vqb_prior_layer_weights &w, const Act &in, const Act &vh, const Act &out_h,
+                  const long long *lab, int NC, int B, int H, int W, int row0, int nrows, int col0, int ncols,
+                  const Act &keep) {
+    by_q(in.C, [&](auto q) {
+        constexpr int Q = decltype(q)::value, P = pf<Q>();
+        horiz_kernel<P, Q><<<blocks((long long)B * nrows * ncols, P), NT, smem_of<horiz_kernel<P, Q>, P, Q>(), s>>>(
+            w, in, vh, out_h, lab, NC, B, H, W, row0, nrows, col0, ncols, keep);
+    });
+}
+
+void launch_head(cudaStream_t s, const Net &n, const Act &in, const long long *lab, int B, int H, int W, float *logits,
+                 const Act &keep) {
+    by_q(n.C, [&](auto q) {
+        constexpr int Q = decltype(q)::value, P = pf<Q>();
+        head_kernel<P, Q><<<blocks((long long)B * H * W, P), NT, smem_of<head_kernel<P, Q>, P, Q>(), s>>>(
+            n, in, lab, B, H, W, logits, keep);
+    });
+}
+
+void launch_lse_head(cudaStream_t s, const Net &n, const Act &in, const long long *lab, const long long *codes, int B,
+                     int H, int W, float *part, const Act &keep) {
+    by_q(n.C, [&](auto q) {
+        constexpr int Q = decltype(q)::value, P = pf<Q>();
+        lse_head_kernel<P, Q><<<blocks((long long)B * H * W, P), NT, smem_of<lse_head_kernel<P, Q>, P, Q>(), s>>>(
+            n, in, lab, codes, B, H, W, part, keep);
+    });
+}
 
 // The sampler of generate and complete, from raster position n_given = i0*W + j0 on (generate: n_given = 0).  The
 // positions before it are final and their embeddings are in x0.  When i0 > 0, every layer's vertical output is first
@@ -623,28 +719,30 @@ void sample_from(const Net &n, const long long *lab, const float *u, int B, int 
     unsigned long long launches = 0;
     if (i0 > 0) {
         for (int l = 0; l < n.L; ++l)
-            vert_kernel<PF><<<blocks((long long)B * i0 * W, PF), NT, 0, s>>>(
-                n.layer[l], l == 0 ? x0 : v(l - 1), v(l), Act{}, lab, n.NC, B, H, W, 0, i0, Act{});
+            launch_vert(s, n.layer[l], l == 0 ? x0 : v(l - 1), v(l), Act{}, lab, n.NC, B, H, W, 0, i0, Act{});
         launches += n.L;
     }
     for (int i = i0; i < H; ++i) {
         // row pass: every layer's vertical stack at row i (codes of rows < i are final)
         for (int l = 0; l < n.L; ++l)
-            vert_kernel<PF><<<blocks((long long)B * W, PF), NT, 0, s>>>(n.layer[l], l == 0 ? x0 : v(l - 1), v(l),
-                                                                        vh(l), lab, n.NC, B, H, W, i, 1, Act{});
+            launch_vert(s, n.layer[l], l == 0 ? x0 : v(l - 1), v(l), vh(l), lab, n.NC, B, H, W, i, 1, Act{});
         launches += n.L;
         const int jstart = i == i0 ? j0 : 0;
         if (jstart > 0) {
             for (int l = 0; l < n.L; ++l)
-                horiz_kernel<PF><<<blocks((long long)B * jstart, PF), NT, 0, s>>>(
-                    n.layer[l], l == 0 ? x0 : x(l - 1), vh(l), x(l), lab, n.NC, B, H, W, i, 1, 0, jstart, Act{});
+                launch_horiz(s, n.layer[l], l == 0 ? x0 : x(l - 1), vh(l), x(l), lab, n.NC, B, H, W, i, 1, 0, jstart,
+                             Act{});
             launches += n.L;
         }
         for (int j = jstart; j < W; ++j) {
             float *lg = step_logits ? step_logits + ((long long)i * W + j) * n.K : ws + wl.gen_lg;
             const long long img = step_logits ? (long long)H * W * n.K : n.K;
-            step_kernel<PS><<<blocks(B, PS), NT, 0, s>>>(n, x0, x(0), vh(0), vh_stride, x_stride, lab, u, B, H, W, i,
-                                                         j, lg, img, codes, sp, (long long)i * W + j == n_given);
+            const bool first = (long long)i * W + j == n_given;
+            by_q(n.C, [&](auto q) {
+                constexpr int Q = decltype(q)::value, P = ps<Q>();
+                step_kernel<P, Q><<<blocks(B, P), NT, smem_of<step_kernel<P, Q>, P, Q>(), s>>>(
+                    n, x0, x(0), vh(0), vh_stride, x_stride, lab, u, B, H, W, i, j, lg, img, codes, sp, first);
+            });
         }
         launches += W - jstart;
     }
@@ -714,12 +812,10 @@ extern "C" int vqb_prior_layer_f32(const vqb_prior_layer_weights *layer, const f
     if (!dim_ok(dim)) return VQB_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     const long long *lab = reinterpret_cast<const long long *>(labels);
-    const long long n = (long long)B * H * W;
     Act in_v{const_cast<float *>(x_v), H, dim}, in_h{const_cast<float *>(x_h), H, dim};
     Act ov{out_v, H, dim}, oh{out_h, H, dim}, vha{vh, H, 2 * dim};
-    vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H, Act{});
-    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W, 0, H, 0, W,
-                                                  Act{});
+    launch_vert(s, *layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H, Act{});
+    launch_horiz(s, *layer, in_h, vha, oh, lab, n_classes, B, H, W, 0, H, 0, W, Act{});
     VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -738,10 +834,8 @@ Act forward_layers(const Net &n, const long long *codes, const long long *lab, i
     embed_kernel<<<grid_for(grid), NT, 0, s>>>(codes, n.emb, npos, n.K, n.C, x0.p);
     for (int l = 0; l < n.L; ++l) {
         const Act vin = l == 0 ? x0 : v[(l - 1) & 1], xin = l == 0 ? x0 : x[(l - 1) & 1];
-        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H,
-                                                        Act{});
-        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W, 0, H, 0,
-                                                         W, Act{});
+        launch_vert(s, n.layer[l], vin, v[l & 1], vh, lab, n.NC, B, H, W, 0, H, Act{});
+        launch_horiz(s, n.layer[l], xin, vh, x[l & 1], lab, n.NC, B, H, W, 0, H, 0, W, Act{});
     }
     VQB_COUNT_LAUNCH(1 + 2 * n.L);
     return x[(n.L - 1) & 1];
@@ -756,12 +850,10 @@ Act train_layers(const Net &n, const long long *codes, const long long *lab, int
     const Act vh{sp + sv.vh(), H, 2 * n.C};
     embed_kernel<<<grid_for(npos * n.C), NT, 0, s>>>(codes, n.emb, npos, n.K, n.C, sp + sv.xv(0));
     for (int l = 0; l < n.L; ++l) {
-        vert_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xv(l), H, n.C},
-                                                        Act{sp + sv.xv(l + 1), H, n.C}, vh, lab, n.NC, B, H, W, 0, H,
-                                                        Act{sp + sv.hv(l), H, 2 * n.C});
-        horiz_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n.layer[l], Act{sp + sv.xh(l), H, n.C}, vh,
-                                                         Act{sp + sv.xh(l + 1), H, n.C}, lab, n.NC, B, H, W, 0,
-                                                         H, 0, W, Act{sp + sv.ph(l), H, 2 * n.C});
+        launch_vert(s, n.layer[l], Act{sp + sv.xv(l), H, n.C}, Act{sp + sv.xv(l + 1), H, n.C}, vh, lab, n.NC, B, H,
+                    W, 0, H, Act{sp + sv.hv(l), H, 2 * n.C});
+        launch_horiz(s, n.layer[l], Act{sp + sv.xh(l), H, n.C}, vh, Act{sp + sv.xh(l + 1), H, n.C}, lab, n.NC, B, H,
+                     W, 0, H, 0, W, Act{sp + sv.ph(l), H, 2 * n.C});
     }
     VQB_COUNT_LAUNCH(1 + 2 * n.L);
     return Act{sp + sv.xh(n.L), H, n.C};
@@ -781,7 +873,7 @@ extern "C" int vqb_prior_forward_f32(const vqb_prior_net *net, const int64_t *co
     const long long *lab = reinterpret_cast<const long long *>(labels);
     const Act xL = forward_layers(n, reinterpret_cast<const long long *>(codes), lab, B, H, W,
                                   static_cast<float *>(workspace), s);
-    head_kernel<PF><<<blocks((long long)B * H * W, PF), NT, 0, s>>>(n, xL, lab, B, H, W, logits, Act{});
+    launch_head(s, n, xL, lab, B, H, W, logits, Act{});
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -806,7 +898,7 @@ extern "C" int vqb_prior_log_prob_f32(const vqb_prior_net *net, const int64_t *c
     float *ws = static_cast<float *>(workspace);
     float *part = ws + vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K) / sizeof(float);
     const Act xL = forward_layers(n, cd, lab, B, H, W, ws, s);
-    lse_head_kernel<PF><<<blocks((long long)B * H * W, PF), NT, 0, s>>>(n, xL, lab, cd, B, H, W, part, Act{});
+    launch_lse_head(s, n, xL, lab, cd, B, H, W, part, Act{});
     log_prob_finish_kernel<<<B, NT, 0, s>>>(part, 1, (long long)H * W, n_given, log_prob, pos_log_prob);
     VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());
@@ -901,8 +993,7 @@ extern "C" int vqb_prior_forward_train_f32(const vqb_prior_net *net, const int64
     const Saved sv{npos, n.C, n.L};
     float *sp = static_cast<float *>(saved);
     train_layers(n, reinterpret_cast<const long long *>(codes), lab, B, H, W, sp, s);
-    head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, Act{sp + sv.xh(n.L), H, n.C}, lab, B, H, W, logits,
-                                                    Act{sp + sv.hid(), H, HID});
+    launch_head(s, n, Act{sp + sv.xh(n.L), H, n.C}, lab, B, H, W, logits, Act{sp + sv.hid(), H, HID});
     VQB_COUNT_LAUNCH(1);
     return vqb_cuda_status(cudaGetLastError());
 }
@@ -944,7 +1035,7 @@ extern "C" int vqb_prior_ce_forward_f32(const vqb_prior_net *net, const int64_t 
     } else {
         xL = forward_layers(n, cd, lab, B, H, W, ws, s);
     }
-    lse_head_kernel<PF><<<blocks(npos, PF), NT, 0, s>>>(n, xL, lab, cd, B, H, W, part, keep);
+    launch_lse_head(s, n, xL, lab, cd, B, H, W, part, keep);
     VQB_COUNT_LAUNCH(1 + ce_finish(s, part, 1, npos, reduction, loss, saved ? sp + sv.total() : nullptr,
                                    part + 3 * npos));
     return vqb_cuda_status(cudaGetLastError());
@@ -968,15 +1059,12 @@ extern "C" int vqb_prior_layer_forward_train_f32(const vqb_prior_layer_weights *
     if (saved_bytes < vqb_prior_layer_train_saved_bytes(B, H, W, dim)) return VQB_ERR_WORKSPACE;
     cudaStream_t s = (cudaStream_t)stream;
     const long long *lab = reinterpret_cast<const long long *>(labels);
-    const long long n = (long long)B * H * W;
-    const LayerSaved sv{n, dim};
+    const LayerSaved sv{(long long)B * H * W, dim};
     float *sp = static_cast<float *>(saved);
     Act in_v{const_cast<float *>(x_v), H, dim}, in_h{const_cast<float *>(x_h), H, dim};
     Act ov{out_v, H, dim}, oh{out_h, H, dim}, vha{vh, H, 2 * dim};
-    vert_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H,
-                                                 Act{sp + sv.hv(), H, 2 * dim});
-    horiz_kernel<PF><<<blocks(n, PF), NT, 0, s>>>(*layer, in_h, vha, oh, lab, n_classes, B, H, W, 0, H, 0, W,
-                                                  Act{sp + sv.ph(), H, 2 * dim});
+    launch_vert(s, *layer, in_v, ov, vha, lab, n_classes, B, H, W, 0, H, Act{sp + sv.hv(), H, 2 * dim});
+    launch_horiz(s, *layer, in_h, vha, oh, lab, n_classes, B, H, W, 0, H, 0, W, Act{sp + sv.ph(), H, 2 * dim});
     VQB_COUNT_LAUNCH(2);
     return vqb_cuda_status(cudaGetLastError());
 }

@@ -6,7 +6,8 @@
 namespace {
 
 constexpr int NT = 256;           // threads of every prior kernel
-constexpr int MAXC = 256;         // dim <= 256, dim % 32 == 0
+constexpr int MAXC = 256;         // dim <= 256: the per-position kernels' original instantiations (prior.cu)
+constexpr int MAXC_WIDE = 1024;   // dim <= 1024, dim % 32 == 0: every dim the prior accepts
 constexpr int HID = 512;          // output_conv.0: dim -> 512 (models.py:109)
 constexpr int MAXK = 8192;
 
@@ -47,7 +48,7 @@ inline bool layer_ok(const vqb_prior_layer_weights &w) {
            w.class_emb && w.kernel >= 1 && w.kernel <= VQB_PRIOR_MAX_KERNEL && (w.kernel & 1);
 }
 
-inline bool dim_ok(int C) { return C % 32 == 0 && C <= MAXC; }
+inline bool dim_ok(int C) { return C % 32 == 0 && C <= MAXC_WIDE; }
 
 inline int net_from(const vqb_prior_net *net, Net &n) {
     if (!net || !net->layers || !net->embedding || !net->out1_w || !net->out1_b || !net->out2_w || !net->out2_b)

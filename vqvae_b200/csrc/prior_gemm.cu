@@ -891,25 +891,27 @@ extern "C" int vqb_prior_gate_backward_f32(const float *x, const float *d_out, f
     return vqb_cuda_status(cudaGetLastError());
 }
 
-// workspace of one layer's backward: the 6 grids of layer_backward's scratch, then its wgrad partials
-extern "C" size_t vqb_prior_layer_backward_workspace_bytes(const vqb_prior_layer_weights *layer, int B, int H, int W,
-                                                           int dim, int n_classes) {
-    if (!layer || !layer_ok(*layer) || B <= 0 || H <= 0 || W <= 0 || n_classes <= 0 || !dim_ok(dim)) return 0;
+namespace {
+
+// One layer's backward for dims up to maxc (MAXC: the ABI-3 pair vqb_prior_layer_backward_*, which has always
+// refused dim > 256; MAXC_WIDE: vqb_prior_layer_backward_wide_*).  Workspace: the 6 grids of layer_backward's
+// scratch, then its wgrad partials (0 = bad arguments).
+size_t layer_backward_ws(int maxc, const vqb_prior_layer_weights *layer, int B, int H, int W, int dim, int n_classes) {
+    if (!layer || !layer_ok(*layer) || B <= 0 || H <= 0 || W <= 0 || n_classes <= 0 || !dim_ok(dim) || dim > maxc)
+        return 0;
     const long long npos = (long long)B * H * W;
     return (size_t)(6 * npos * dim + layer_phase(*layer, dim, n_classes, npos).floats) * sizeof(float);
 }
 
-extern "C" int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
-                                           const int64_t *labels, int B, int H, int W, int dim, int n_classes,
-                                           const float *d_out_v, const float *d_out_h, const void *saved,
-                                           const vqb_prior_layer_grads *grads, float *d_x_v, float *d_x_h,
-                                           void *workspace, size_t workspace_bytes, void *stream) {
+int layer_backward_call(int maxc, const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                        const int64_t *labels, int B, int H, int W, int dim, int n_classes, const float *d_out_v,
+                        const float *d_out_h, const void *saved, const vqb_prior_layer_grads *grads, float *d_x_v,
+                        float *d_x_h, void *workspace, size_t workspace_bytes, void *stream) {
     if (!layer || !x_v || !x_h || !labels || !d_out_h || !saved || !grads || !d_x_v || !d_x_h || !workspace ||
         B <= 0 || H <= 0 || W <= 0 || dim <= 0 || n_classes <= 0 || !layer_ok(*layer) || !layer_grads_ok(*grads))
         return VQB_ERR_BAD_ARG;
-    if (!dim_ok(dim)) return VQB_ERR_UNSUPPORTED;
-    if (workspace_bytes < vqb_prior_layer_backward_workspace_bytes(layer, B, H, W, dim, n_classes))
-        return VQB_ERR_WORKSPACE;
+    if (!dim_ok(dim) || dim > maxc) return VQB_ERR_UNSUPPORTED;
+    if (workspace_bytes < layer_backward_ws(maxc, layer, B, H, W, dim, n_classes)) return VQB_ERR_WORKSPACE;
     const int npos = B * H * W;
     const LayerSaved sv{npos, dim};
     const float *sp = static_cast<const float *>(saved);
@@ -919,4 +921,34 @@ extern "C" int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer
                    ws + 6LL * npos * dim);
     VQB_COUNT_LAUNCH(10);
     return vqb_cuda_status(cudaGetLastError());
+}
+
+}  // namespace
+
+extern "C" size_t vqb_prior_layer_backward_workspace_bytes(const vqb_prior_layer_weights *layer, int B, int H, int W,
+                                                           int dim, int n_classes) {
+    return layer_backward_ws(MAXC, layer, B, H, W, dim, n_classes);
+}
+
+extern "C" int vqb_prior_layer_backward_f32(const vqb_prior_layer_weights *layer, const float *x_v, const float *x_h,
+                                           const int64_t *labels, int B, int H, int W, int dim, int n_classes,
+                                           const float *d_out_v, const float *d_out_h, const void *saved,
+                                           const vqb_prior_layer_grads *grads, float *d_x_v, float *d_x_h,
+                                           void *workspace, size_t workspace_bytes, void *stream) {
+    return layer_backward_call(MAXC, layer, x_v, x_h, labels, B, H, W, dim, n_classes, d_out_v, d_out_h, saved, grads,
+                               d_x_v, d_x_h, workspace, workspace_bytes, stream);
+}
+
+extern "C" size_t vqb_prior_layer_backward_wide_workspace_bytes(const vqb_prior_layer_weights *layer, int B, int H,
+                                                                int W, int dim, int n_classes) {
+    return layer_backward_ws(MAXC_WIDE, layer, B, H, W, dim, n_classes);
+}
+
+extern "C" int vqb_prior_layer_backward_wide_f32(const vqb_prior_layer_weights *layer, const float *x_v,
+                                                const float *x_h, const int64_t *labels, int B, int H, int W, int dim,
+                                                int n_classes, const float *d_out_v, const float *d_out_h,
+                                                const void *saved, const vqb_prior_layer_grads *grads, float *d_x_v,
+                                                float *d_x_h, void *workspace, size_t workspace_bytes, void *stream) {
+    return layer_backward_call(MAXC_WIDE, layer, x_v, x_h, labels, B, H, W, dim, n_classes, d_out_v, d_out_h, saved,
+                               grads, d_x_v, d_x_h, workspace, workspace_bytes, stream);
 }

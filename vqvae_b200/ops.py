@@ -569,20 +569,21 @@ def prior_layer_forward_train(layer_w, x_v, x_h, labels, *, B, H, W, dim, n_clas
 
 
 def prior_layer_backward(layer_w, x_v, x_h, labels, d_out_v, d_out_h, saved, grads, *, B, H, W, dim, n_classes):
-    """One layer's gradients (vqb_prior_layer_backward_f32): the nine weight gradients into the tensors `grads` (a
+    """One layer's gradients (vqb_prior_layer_backward_wide_f32, any dim the prior takes): the nine weight gradients into the tensors `grads` (a
     PriorLayerGrads struct) points at -> (d_x_v, d_x_h) NHWC.  d_out_v None: a zero gradient."""
-    n = lib().vqb_prior_layer_backward_workspace_bytes(_lib.C.byref(layer_w), B, H, W, dim, n_classes)
+    n = lib().vqb_prior_layer_backward_wide_workspace_bytes(_lib.C.byref(layer_w), B, H, W, dim, n_classes)
     if n == 0:
         raise RuntimeError("prior layer backward: bad sizes")
     ws = torch.empty((n,), dtype=torch.uint8, device=x_v.device)
     d_x_v = torch.empty((B, H, W, dim), dtype=torch.float32, device=x_v.device)
     d_x_h = torch.empty_like(d_x_v)
     span = _Span(f"prior layer backward dim={dim} {H}x{W}")
-    check(lib().vqb_prior_layer_backward_f32(_lib.C.byref(layer_w), x_v.data_ptr(), x_h.data_ptr(), labels.data_ptr(),
-                                             B, H, W, dim, n_classes,
-                                             d_out_v.data_ptr() if d_out_v is not None else None, d_out_h.data_ptr(),
-                                             saved.data_ptr(), _lib.C.byref(grads), d_x_v.data_ptr(), d_x_h.data_ptr(),
-                                             ws.data_ptr(), n, _stream()), "prior_layer_backward")
+    check(lib().vqb_prior_layer_backward_wide_f32(_lib.C.byref(layer_w), x_v.data_ptr(), x_h.data_ptr(),
+                                                  labels.data_ptr(), B, H, W, dim, n_classes,
+                                                  d_out_v.data_ptr() if d_out_v is not None else None,
+                                                  d_out_h.data_ptr(), saved.data_ptr(), _lib.C.byref(grads),
+                                                  d_x_v.data_ptr(), d_x_h.data_ptr(), ws.data_ptr(), n, _stream()),
+          "prior_layer_backward")
     span.done()
     return d_x_v, d_x_h
 

@@ -33,6 +33,9 @@ Reference behaviour kept on purpose:
       RuntimeError before any launch otherwise.  ``generate`` and ``complete`` also need layer 0 to be mask A without
       residual: anything else reads the code being drawn, so the reference's one-forward-per-position loop is not
       causal in raster order there, and the sampler refuses it (C ABI: VQB_ERR_UNSUPPORTED)
+
+Limits: dim % 32 == 0 and dim <= 1024, so gated_pixelcnn.py's GatedPixelCNN(K, img_dim**2, n_layers) runs for
+latents up to 32x32; the library refuses any other dim before any launch (VQB_ERR_UNSUPPORTED, a RuntimeError).
 """
 import math
 import numbers
@@ -196,8 +199,8 @@ _NET_GRADS = dict(embedding="embedding.weight", out1_w="output_conv.0.weight", o
 class _GatedLayerFunction(torch.autograd.Function):
     """GatedMaskedConv2d.forward with gradients: inputs are the layer, x_v, x_h (NCHW), the labels and the layer's
     parameters in ``parameters()`` order.  NCHW <-> NHWC at the boundary; the forward keeps x_v, x_h (NHWC) and
-    vqb_prior_layer_forward_train_f32's `saved`; the backward (vqb_prior_layer_backward_f32) returns the gradients of
-    x_v, x_h and every parameter, mask A's taps included.  The labels get none."""
+    vqb_prior_layer_forward_train_f32's `saved`; the backward (vqb_prior_layer_backward_wide_f32) returns the gradients
+    of x_v, x_h and every parameter, mask A's taps included.  The labels get none."""
 
     @staticmethod
     def forward(ctx, layer, x_v, x_h, label, *params):
