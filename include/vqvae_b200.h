@@ -469,6 +469,20 @@ size_t vqb_prior_sample_workspace_bytes(int B, int H, int W, int dim, int n_laye
 int vqb_prior_sample_f32(const vqb_prior_net *net, const int64_t *labels, const float *u, const int64_t *given,
                          int64_t n_given, int B, int H, int W, const vqb_prior_sampling *sampling, int64_t *codes,
                          float *log_prob, float *step_logits, void *workspace, size_t workspace_bytes, void *stream);
+/* vqb_prior_sample_f32 with one prefix length per image: n_given (B) int64 on the device, never read on the host, so
+ * a captured graph follows new values written there.  Each value is clamped to [0, H*W], as codes and labels are.
+ * Image b's codes, log_prob[b] and step logits are bitwise those of vqb_prior_sample_f32 on image b alone with
+ * n_given = clamp(n_given[b]) and the same u and knobs (log_prob[b] = 0 when that is H*W); step_logits are written
+ * at image b's positions >= n_given[b] only.  sampling NULL is complete's draw (the ragged complete), log_prob may
+ * be NULL, given may not.  Schedule: one launch copies and embeds every image's given prefix, then generate's
+ * row passes and steps, each step skipping the images that have that position given: 1 + H*(n_layers + W) launches
+ * whatever the values.  workspace: vqb_prior_sample_workspace_bytes(..., n_given = 0) (generate's rings and the
+ * draw's scratch).  VQB_ERR_BAD_ARG for a NULL given or n_given and for vqb_prior_sample_f32's other bad
+ * arguments; VQB_ERR_UNSUPPORTED for a layer 0 generate refuses; both before any launch.                        */
+int vqb_prior_sample_ragged_f32(const vqb_prior_net *net, const int64_t *labels, const float *u,
+                                const int64_t *given, const int64_t *n_given, int B, int H, int W,
+                                const vqb_prior_sampling *sampling, int64_t *codes, float *log_prob,
+                                float *step_logits, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- Gated PixelCNN prior, training (fp32 on CUDA cores) ------------------------------------------------------
  * The forward keeps its activations in `saved`; the backward turns d_logits into the gradient of every parameter.
@@ -593,6 +607,17 @@ int vqb_prior_log_prob_f32(const vqb_prior_net *net, const int64_t *codes, const
 int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int64_t n_given,
                             int B, int H, int W, float *log_prob, float *pos_log_prob, void *workspace,
                             size_t workspace_bytes, void *stream);
+/* log_prob with one prefix length per image: n_given (B) int64 on the device (never read on the host, each value
+ * clamped to [0, H*W]); log_prob[b] is bitwise entry b of vqb_prior_log_prob_* on the same inputs with the scalar
+ * n_given = clamp(n_given[b]).
+ * No per-position output.  The same launches and workspace as vqb_prior_log_prob_* in the same precision;
+ * VQB_ERR_BAD_ARG for a NULL log_prob or n_given and for their other bad arguments.                              */
+int vqb_prior_log_prob_ragged_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                  const int64_t *n_given, int B, int H, int W, float *log_prob, void *workspace,
+                                  size_t workspace_bytes, void *stream);
+int vqb_prior_log_prob_ragged_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                   const int64_t *n_given, int B, int H, int W, float *log_prob, void *workspace,
+                                   size_t workspace_bytes, void *stream);
 
 /* ---- Gated PixelCNN prior: the training cross-entropy without the logits (fp32 and TF32) -------------------------
  * The reference's loss, nn.CrossEntropyLoss(reduction)(logits.permute(0, 2, 3, 1).reshape(-1, K), codes.reshape(-1)),

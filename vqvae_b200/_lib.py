@@ -73,6 +73,7 @@ SIGNATURES = {
     "vqb_prior_complete_f32": (_i, [_vp] * 4 + [_i64] + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
     "vqb_prior_sample_workspace_bytes": (_sz, [_i] * 6 + [_i64]),
     "vqb_prior_sample_f32": (_i, [_vp] * 4 + [_i64] + [_i] * 3 + [_vp] * 5 + [_sz, _vp]),
+    "vqb_prior_sample_ragged_f32": (_i, [_vp] * 5 + [_i] * 3 + [_vp] * 5 + [_sz, _vp]),
     "vqb_prior_train_saved_bytes": (_sz, [_i] * 5),
     "vqb_prior_forward_train_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp, _sz, _vp]),
     "vqb_prior_backward_workspace_bytes": (_sz, [_vp] + [_i] * 3),
@@ -92,6 +93,8 @@ SIGNATURES = {
     "vqb_prior_log_prob_workspace_bytes_tf32": (_sz, [_i] * 6),
     "vqb_prior_log_prob_f32": (_i, [_vp] * 3 + [_i64] + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
     "vqb_prior_log_prob_tf32": (_i, [_vp] * 3 + [_i64] + [_i] * 3 + [_vp] * 3 + [_sz, _vp]),
+    "vqb_prior_log_prob_ragged_f32": (_i, [_vp] * 4 + [_i] * 3 + [_vp] * 2 + [_sz, _vp]),
+    "vqb_prior_log_prob_ragged_tf32": (_i, [_vp] * 4 + [_i] * 3 + [_vp] * 2 + [_sz, _vp]),
     "vqb_prior_ce_saved_bytes": (_sz, [_i] * 5),
     "vqb_prior_ce_workspace_bytes": (_sz, [_i] * 7),
     "vqb_prior_ce_workspace_bytes_tf32": (_sz, [_i] * 7),

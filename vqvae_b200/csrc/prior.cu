@@ -411,27 +411,48 @@ __device__ __forceinline__ float warp_max(float v) {
 // One sampling step at (i, j) for P images: every layer's horizontal stack, the head, the softmax and the inverse-CDF
 // draw.  The code goes to codes[b, i, j] and its embedding to x0[b, i, j], which later steps and row passes read.
 // `first`: the first sampled step of the call, which writes log_prob instead of adding to it.
-template <int P, int Q = 2>
+// RAGGED: image b keeps its raster positions p < g_b = clamp_given(ragged[b], H*W) as given (`first` is not read).
+// In a row it has given whole the step does nothing for it; at a given position of its first free row it runs only
+// the horizontal stacks, which the row's later steps read; from p = g_b on it is the step above, first at p = g_b.
+template <int P, int Q = 2, bool RAGGED = false>
 __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act vh0, long long vh_stride,
                                                   long long x_stride, const long long *labels, const float *u, int B,
                                                   int H, int W, int i, int j, float *logits, long long logit_img,
-                                                  long long *codes, Samp sp, bool first) {
+                                                  long long *codes, Samp sp, bool first, const long long *ragged) {
     Smem<P, Q> &s = block_smem<P, Q>();
     __shared__ float *out[P];
+    const long long HW = (long long)H * W, at = (long long)i * W + j;
     if (threadIdx.x < P) {
         const int p = threadIdx.x, b = blockIdx.x * P + p;
         s.b[p] = b < B ? b : -1;
+        if constexpr (RAGGED)
+            if (b < B && (long long)(i + 1) * W <= clamp_given(ragged[b], HW)) s.b[p] = -1;
         s.r[p] = i; s.c[p] = j;
         s.lab[p] = b < B ? clampi(labels[b], n.NC) : 0;
         out[p] = b < B ? logits + (long long)b * logit_img : nullptr;
     }
     __syncthreads();
+    if constexpr (RAGGED) {
+        bool live = false;
+#pragma unroll
+        for (int p = 0; p < P; ++p) live |= s.b[p] >= 0;
+        if (!live) return;
+    }
     for (int l = 0; l < n.L; ++l) {
         const Act in = l == 0 ? x0 : Act{xrow0.p + (l - 1) * x_stride, 1, n.C};
         const Act vh{vh0.p + l * vh_stride, 1, 2 * n.C};
         const Act o{xrow0.p + l * x_stride, 1, n.C};
         horiz_positions(s, n.layer[l], in, vh, o, H, W, Act{});
         __syncthreads();
+    }
+    if constexpr (RAGGED) {         // given positions: no head, no draw
+        if (threadIdx.x < P && s.b[threadIdx.x] >= 0 && at < clamp_given(ragged[s.b[threadIdx.x]], HW))
+            s.b[threadIdx.x] = -1;
+        __syncthreads();
+        bool live = false;
+#pragma unroll
+        for (int p = 0; p < P; ++p) live |= s.b[p] >= 0;
+        if (!live) return;
     }
     ToHbm<P> sink{out, 1};
     head_positions(s, n, Act{xrow0.p + (n.L - 1) * x_stride, 1, n.C}, sink, H, W, Act{});
@@ -534,6 +555,7 @@ __global__ void __launch_bounds__(NT) step_kernel(Net n, Act x0, Act xrow0, Act 
             }
             if (lane == 0) {        // compensated fp32 sum in raster order: 4096 near-equal terms stay accurate
                 const float lp = (lg[code] - ml) - logf(suml);
+                if constexpr (RAGGED) first = at == clamp_given(ragged[b], HW);
                 if (first) {
                     sp.log_prob[b] = lp;
                     sp.log_c[b] = 0.f;
@@ -566,6 +588,25 @@ __global__ void given_kernel(const long long *__restrict__ given, const float *_
     if (zero)
         for (long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (long long)gridDim.x * blockDim.x)
             zero[b] = 0.f;
+}
+
+// given_kernel with image b's own bound g_b = clamp_given(n_given[b], HW), over every position of the grid; zero:
+// nullptr, or the (B) log_prob, set to 0 for the images with nothing to sample (g_b = HW).
+__global__ void given_ragged_kernel(const long long *__restrict__ given, const long long *__restrict__ n_given,
+                                    const float *__restrict__ E, int B, long long HW, int K, int C,
+                                    float *__restrict__ x0, long long *__restrict__ codes, float *__restrict__ zero) {
+    const long long total = (long long)B * HW * C;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long pos = i / C;
+        if (pos % HW >= clamp_given(n_given[pos / HW], HW)) continue;
+        const int c = (int)(i % C);
+        const long long code = given[pos];
+        x0[pos * C + c] = __ldg(E + (long long)clampi(code, K) * C + c);
+        if (c == 0) codes[pos] = code;
+    }
+    if (zero)
+        for (long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x; b < B; b += (long long)gridDim.x * blockDim.x)
+            if (clamp_given(n_given[b], HW) == HW) zero[b] = 0.f;
 }
 
 // the kept-tap packing of pack_prior_at
@@ -703,8 +744,11 @@ void launch_lse_head(cudaStream_t s, const Net &n, const Act &in, const long lon
 // j0 > 0, one horizontal launch per layer over columns [0, j0) first fills the one-row x[l] that the step at (i0, j0)
 // reads.  Every value is the fmaf chain generate computes at that position, so the logits are bitwise generate's.
 // Launches: L*[i0 > 0] + L*(H - i0) + L*[j0 > 0] + (H*W - n_given).  sp: the draw's knobs, the same for every step.
+// ragged (with n_given = 0): the (B) per-image prefix lengths on the device, which the steps read (step_kernel's
+// RAGGED instantiation); the schedule is generate's, H*(L + W) launches whatever their values.
 void sample_from(const Net &n, const long long *lab, const float *u, int B, int H, int W, long long n_given,
-                 const Samp &sp, long long *codes, float *step_logits, float *ws, cudaStream_t s) {
+                 const Samp &sp, long long *codes, float *step_logits, float *ws, cudaStream_t s,
+                 const long long *ragged = nullptr) {
     const Ws wl = ws_layout(B, H, W, n.C, n.L, n.K);
     const int i0 = (int)(n_given / W), j0 = (int)(n_given % W);
     int reach = 1;
@@ -740,8 +784,14 @@ void sample_from(const Net &n, const long long *lab, const float *u, int B, int 
             const bool first = (long long)i * W + j == n_given;
             by_q(n.C, [&](auto q) {
                 constexpr int Q = decltype(q)::value, P = ps<Q>();
-                step_kernel<P, Q><<<blocks(B, P), NT, smem_of<step_kernel<P, Q>, P, Q>(), s>>>(
-                    n, x0, x(0), vh(0), vh_stride, x_stride, lab, u, B, H, W, i, j, lg, img, codes, sp, first);
+                if (ragged)
+                    step_kernel<P, Q, true><<<blocks(B, P), NT, smem_of<step_kernel<P, Q, true>, P, Q>(), s>>>(
+                        n, x0, x(0), vh(0), vh_stride, x_stride, lab, u, B, H, W, i, j, lg, img, codes, sp, false,
+                        ragged);
+                else
+                    step_kernel<P, Q><<<blocks(B, P), NT, smem_of<step_kernel<P, Q>, P, Q>(), s>>>(
+                        n, x0, x(0), vh(0), vh_stride, x_stride, lab, u, B, H, W, i, j, lg, img, codes, sp, first,
+                        nullptr);
             });
         }
         launches += W - jstart;
@@ -764,6 +814,32 @@ void sample_call(const Net &n, const int64_t *labels, const float *u, const int6
     }
     if (n_given < HW)
         sample_from(n, reinterpret_cast<const long long *>(labels), u, B, H, W, n_given, sp, out, step_logits, ws, s);
+}
+
+// The ragged sampler's body after its argument checks: every image's given prefix in one launch, then generate's
+// schedule with each step deciding per image.  1 + H*(L + W) launches.
+void sample_ragged_call(const Net &n, const int64_t *labels, const float *u, const int64_t *given,
+                        const int64_t *n_given, int B, int H, int W, const Samp &sp, int64_t *codes,
+                        float *step_logits, void *workspace, cudaStream_t s) {
+    const long long HW = (long long)H * W;
+    float *ws = static_cast<float *>(workspace);
+    long long *out = reinterpret_cast<long long *>(codes);
+    const long long *ng = reinterpret_cast<const long long *>(n_given);
+    given_ragged_kernel<<<grid_for((long long)B * HW * n.C), NT, 0, s>>>(
+        reinterpret_cast<const long long *>(given), ng, n.emb, B, HW, n.K, n.C,
+        ws + ws_layout(B, H, W, n.C, n.L, n.K).gen_x0, out, sp.log_prob);
+    VQB_COUNT_LAUNCH(1);
+    sample_from(n, reinterpret_cast<const long long *>(labels), u, B, H, W, 0, sp, out, step_logits, ws, s, ng);
+}
+
+// The draw's knobs of a sampling entry point (NULL: the defaults) into sp; false for a knob outside its range
+bool knobs_from(const vqb_prior_sampling *sampling, int K, Samp &sp) {
+    if (sampling) {
+        sp.T = sampling->temperature;
+        sp.top_k = sampling->top_k;
+        sp.top_p = sampling->top_p;
+    }
+    return sp.T > 0.f && sp.T <= FLT_MAX && sp.top_k >= 0 && sp.top_k <= K && sp.top_p > 0.f && sp.top_p <= 1.f;
 }
 
 // Floats of the sampler's regions from raster position n_given: a prefix shorter than a row keeps generate's rings,
@@ -884,8 +960,28 @@ extern "C" size_t vqb_prior_log_prob_workspace_bytes(int B, int H, int W, int di
     return base + (size_t)B * H * W * 3 * sizeof(float);
 }
 
-// The forward's layer walk, then lse_head_kernel in place of head_kernel (the same logits, reduced on chip: one
-// partial per position, after the forward's workspace) and the finish.  3 + 2*n_layers launches.
+namespace {
+
+// log_prob's launches after the checks: the forward's layer walk, then lse_head_kernel in place of head_kernel (the
+// same logits, reduced on chip: one partial per position, after the forward's workspace) and the finish, which reads
+// n_given or, with ragged != nullptr, image b's own ragged[b].  3 + 2*n_layers launches.
+void log_prob_f32(const Net &n, const int64_t *codes, const int64_t *labels, int64_t n_given, const int64_t *ragged,
+                  int B, int H, int W, float *log_prob, float *pos_log_prob, void *workspace, cudaStream_t s) {
+    const long long *lab = reinterpret_cast<const long long *>(labels), *cd = reinterpret_cast<const long long *>(codes);
+    float *ws = static_cast<float *>(workspace);
+    float *part = ws + vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K) / sizeof(float);
+    const Act xL = forward_layers(n, cd, lab, B, H, W, ws, s);
+    launch_lse_head(s, n, xL, lab, cd, B, H, W, part, Act{});
+    if (ragged)
+        log_prob_finish_kernel<true><<<B, NT, 0, s>>>(part, 1, (long long)H * W, 0, log_prob, pos_log_prob,
+                                                      reinterpret_cast<const long long *>(ragged));
+    else
+        log_prob_finish_kernel<<<B, NT, 0, s>>>(part, 1, (long long)H * W, n_given, log_prob, pos_log_prob);
+    VQB_COUNT_LAUNCH(2);
+}
+
+}  // namespace
+
 extern "C" int vqb_prior_log_prob_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
                                       int64_t n_given, int B, int H, int W, float *log_prob, float *pos_log_prob,
                                       void *workspace, size_t workspace_bytes, void *stream) {
@@ -893,14 +989,18 @@ extern "C" int vqb_prior_log_prob_f32(const vqb_prior_net *net, const int64_t *c
     const int st = log_prob_args(net, n, codes, labels, n_given, B, H, W, log_prob, pos_log_prob, workspace);
     if (st) return st;
     if (workspace_bytes < vqb_prior_log_prob_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
-    cudaStream_t s = (cudaStream_t)stream;
-    const long long *lab = reinterpret_cast<const long long *>(labels), *cd = reinterpret_cast<const long long *>(codes);
-    float *ws = static_cast<float *>(workspace);
-    float *part = ws + vqb_prior_workspace_bytes(B, H, W, n.C, n.L, n.K) / sizeof(float);
-    const Act xL = forward_layers(n, cd, lab, B, H, W, ws, s);
-    launch_lse_head(s, n, xL, lab, cd, B, H, W, part, Act{});
-    log_prob_finish_kernel<<<B, NT, 0, s>>>(part, 1, (long long)H * W, n_given, log_prob, pos_log_prob);
-    VQB_COUNT_LAUNCH(2);
+    log_prob_f32(n, codes, labels, n_given, nullptr, B, H, W, log_prob, pos_log_prob, workspace, (cudaStream_t)stream);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_prior_log_prob_ragged_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                             const int64_t *n_given, int B, int H, int W, float *log_prob,
+                                             void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = log_prob_ragged_args(net, n, codes, labels, n_given, B, H, W, log_prob, workspace);
+    if (st) return st;
+    if (workspace_bytes < vqb_prior_log_prob_workspace_bytes(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    log_prob_f32(n, codes, labels, 0, n_given, B, H, W, log_prob, nullptr, workspace, (cudaStream_t)stream);
     return vqb_cuda_status(cudaGetLastError());
 }
 
@@ -956,19 +1056,35 @@ extern "C" int vqb_prior_sample_f32(const vqb_prior_net *net, const int64_t *lab
     if (!labels || !u || !codes || !workspace || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
     if (n_given < 0 || n_given > (long long)H * W || (n_given > 0 && !given)) return VQB_ERR_BAD_ARG;
     Samp sp;
-    if (sampling) {
-        sp.T = sampling->temperature;
-        sp.top_k = sampling->top_k;
-        sp.top_p = sampling->top_p;
-    }
-    if (!(sp.T > 0.f && sp.T <= FLT_MAX) || sp.top_k < 0 || sp.top_k > n.K || !(sp.top_p > 0.f && sp.top_p <= 1.f))
-        return VQB_ERR_BAD_ARG;
+    if (!knobs_from(sampling, n.K, sp)) return VQB_ERR_BAD_ARG;
     if (workspace_bytes < vqb_prior_sample_workspace_bytes(B, H, W, n.C, n.L, n.K, n_given)) return VQB_ERR_WORKSPACE;
     if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
     sp.scratch = static_cast<float *>(workspace) + ring_floats(ws_layout(B, H, W, n.C, n.L, n.K), W, n_given);
     sp.log_prob = log_prob;
     sp.log_c = sp.scratch + search_floats(B, n.K) - B;
     sample_call(n, labels, u, given, n_given, B, H, W, sp, codes, step_logits, workspace, (cudaStream_t)stream);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+// vqb_prior_sample_f32's checks with a device n_given; generate's rings and the search's scratch after them
+extern "C" int vqb_prior_sample_ragged_f32(const vqb_prior_net *net, const int64_t *labels, const float *u,
+                                           const int64_t *given, const int64_t *n_given, int B, int H, int W,
+                                           const vqb_prior_sampling *sampling, int64_t *codes, float *log_prob,
+                                           float *step_logits, void *workspace, size_t workspace_bytes,
+                                           void *stream) {
+    Net n;
+    const int st = net_from(net, n);
+    if (st) return st;
+    if (!labels || !u || !given || !n_given || !codes || !workspace || B <= 0 || H <= 0 || W <= 0)
+        return VQB_ERR_BAD_ARG;
+    Samp sp;
+    if (!knobs_from(sampling, n.K, sp)) return VQB_ERR_BAD_ARG;
+    if (workspace_bytes < vqb_prior_sample_workspace_bytes(B, H, W, n.C, n.L, n.K, 0)) return VQB_ERR_WORKSPACE;
+    if (!n.layer[0].mask_a || n.layer[0].residual) return VQB_ERR_UNSUPPORTED;
+    sp.scratch = static_cast<float *>(workspace) + ring_floats(ws_layout(B, H, W, n.C, n.L, n.K), W, 0);
+    sp.log_prob = log_prob;
+    sp.log_c = sp.scratch + search_floats(B, n.K) - B;
+    sample_ragged_call(n, labels, u, given, n_given, B, H, W, sp, codes, step_logits, workspace, (cudaStream_t)stream);
     return vqb_cuda_status(cudaGetLastError());
 }
 

@@ -31,6 +31,9 @@ __device__ __forceinline__ float gate(float a, float g) {      // GatedActivatio
 
 __device__ __forceinline__ int clampi(long long v, int n) { return v < 0 ? 0 : (v >= n ? n - 1 : (int)v); }
 
+// A per-image prefix length (the ragged entry points' n_given[b]) clamped to [0, HW], as codes and labels are clamped
+__device__ __forceinline__ long long clamp_given(long long v, long long HW) { return v < 0 ? 0 : (v > HW ? HW : v); }
+
 inline unsigned grid_for(long long total) {
     long long g = (total + NT - 1) / NT;
     return (unsigned)(g > 148LL * 32 ? 148LL * 32 : (g < 1 ? 1 : g));
@@ -91,11 +94,15 @@ __device__ __forceinline__ float lp_of(const float *q, int splits, float *lse = 
 // One block per image: every position's lp into pos (if non-null), and into log_prob[b] (if non-null) the
 // compensated fp32 sum of lp over the raster positions p >= n_given, in raster order, with the sampler's Kahan step
 // (prior.cu: step_kernel), so 4096 near-equal terms stay accurate and the result does not depend on the launch.
+// RAGGED: image b's own n_given is clamp_given(ragged[b], HW) (the scalar n_given is not read).
+template <bool RAGGED = false>
 __global__ void __launch_bounds__(NT) log_prob_finish_kernel(const float *__restrict__ part, int splits, long long HW,
                                                               long long n_given, float *__restrict__ log_prob,
-                                                              float *__restrict__ pos) {
+                                                              float *__restrict__ pos,
+                                                              const long long *__restrict__ ragged = nullptr) {
     __shared__ float lp[NT];
     const int b = blockIdx.x, tid = threadIdx.x;
+    if constexpr (RAGGED) n_given = clamp_given(ragged[b], HW);
     float acc = 0.f, comp = 0.f;
     for (long long p0 = 0; p0 < HW; p0 += NT) {
         const long long p = p0 + tid;
@@ -128,6 +135,15 @@ inline int log_prob_args(const vqb_prior_net *net, Net &n, const int64_t *codes,
     if (!codes || !labels || !workspace || (!log_prob && !pos) || B <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
     if (n_given < 0 || n_given > (long long)H * W) return VQB_ERR_BAD_ARG;
     return 0;
+}
+
+// The ragged entry points' checks (vqb_prior_log_prob_ragged_*): log_prob_args with log_prob required, then n_given
+inline int log_prob_ragged_args(const vqb_prior_net *net, Net &n, const int64_t *codes, const int64_t *labels,
+                                const int64_t *n_given, int B, int H, int W, const float *log_prob,
+                                const void *workspace) {
+    const int st = log_prob_args(net, n, codes, labels, 0, B, H, W, log_prob, nullptr, workspace);
+    if (st) return st;
+    return n_given ? 0 : VQB_ERR_BAD_ARG;
 }
 
 // ---- the cross-entropy (vqb_prior_ce_*): log_prob's head partials, then the loss ----------------------------------

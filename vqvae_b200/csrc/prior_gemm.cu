@@ -647,16 +647,13 @@ extern "C" size_t vqb_prior_log_prob_workspace_bytes_tf32(int B, int H, int W, i
     return base + (size_t)npos * lse_splits(npos, K) * 3 * sizeof(float);
 }
 
-// forward_tf32 up to hid (the same launches and values), then tc_lse_kernel in place of the logits product, and the
-// finish.  4 + 4*n_layers launches.
-extern "C" int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
-                                       int64_t n_given, int B, int H, int W, float *log_prob, float *pos_log_prob,
-                                       void *workspace, size_t workspace_bytes, void *stream) {
-    Net n;
-    const int st = log_prob_args(net, n, codes, labels, n_given, B, H, W, log_prob, pos_log_prob, workspace);
-    if (st) return st;
-    if (workspace_bytes < vqb_prior_log_prob_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
-    cudaStream_t s = (cudaStream_t)stream;
+namespace {
+
+// log_prob's launches after the checks: forward_tf32 up to hid (the same launches and values), then tc_lse_kernel in
+// place of the logits product, and the finish, which reads n_given or, with ragged != nullptr, image b's own
+// ragged[b].  4 + 4*n_layers launches.
+void log_prob_tf32(const Net &n, const int64_t *codes, const int64_t *labels, int64_t n_given, const int64_t *ragged,
+                   int B, int H, int W, float *log_prob, float *pos_log_prob, void *workspace, cudaStream_t s) {
     const long long *cd = reinterpret_cast<const long long *>(codes);
     const int npos = B * H * W;
     const TcWs lay{npos, n.C};
@@ -665,9 +662,36 @@ extern "C" int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *
     const Mat a{sp + lay.hid(), HID}, b{n.w2, n.K};
     if (tc_bn(n.K) == 64) tc_lse_launch<64>(s, a, b, n.b2, cd, npos, n.K, HID, part);
     else tc_lse_launch<128>(s, a, b, n.b2, cd, npos, n.K, HID, part);
-    log_prob_finish_kernel<<<B, NT, 0, s>>>(part, lse_splits(npos, n.K), (long long)H * W, n_given, log_prob,
-                                            pos_log_prob);
+    if (ragged)
+        log_prob_finish_kernel<true><<<B, NT, 0, s>>>(part, lse_splits(npos, n.K), (long long)H * W, 0, log_prob,
+                                                      pos_log_prob, reinterpret_cast<const long long *>(ragged));
+    else
+        log_prob_finish_kernel<<<B, NT, 0, s>>>(part, lse_splits(npos, n.K), (long long)H * W, n_given, log_prob,
+                                                pos_log_prob);
     VQB_COUNT_LAUNCH(4 + 4 * n.L);
+}
+
+}  // namespace
+
+extern "C" int vqb_prior_log_prob_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                       int64_t n_given, int B, int H, int W, float *log_prob, float *pos_log_prob,
+                                       void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = log_prob_args(net, n, codes, labels, n_given, B, H, W, log_prob, pos_log_prob, workspace);
+    if (st) return st;
+    if (workspace_bytes < vqb_prior_log_prob_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    log_prob_tf32(n, codes, labels, n_given, nullptr, B, H, W, log_prob, pos_log_prob, workspace, (cudaStream_t)stream);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_prior_log_prob_ragged_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                              const int64_t *n_given, int B, int H, int W, float *log_prob,
+                                              void *workspace, size_t workspace_bytes, void *stream) {
+    Net n;
+    const int st = log_prob_ragged_args(net, n, codes, labels, n_given, B, H, W, log_prob, workspace);
+    if (st) return st;
+    if (workspace_bytes < vqb_prior_log_prob_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K)) return VQB_ERR_WORKSPACE;
+    log_prob_tf32(n, codes, labels, 0, n_given, B, H, W, log_prob, nullptr, workspace, (cudaStream_t)stream);
     return vqb_cuda_status(cudaGetLastError());
 }
 

@@ -642,6 +642,24 @@ def prior_log_prob(net, codes, labels, n_given, precision="fp32", per_position=F
     return out
 
 
+def prior_log_prob_ragged(net, codes, labels, n_given, precision="fp32"):
+    """prior_log_prob with one prefix length per image, n_given int64 (B,) on the device (vqb_prior_log_prob_ragged_f32
+    / _tf32) -> (B,) fp32, entry b the compensated sum over the raster positions >= n_given[b] (clamped to [0, H*W])."""
+    sfx = _prior_precision(precision)
+    B, H, W = codes.shape
+    dev = codes.device
+    ws = _prior_workspace(net, B, H, W, dev, getattr(lib(), "vqb_prior_log_prob_workspace_bytes" +
+                                                     ("_tf32" if sfx == "tf32" else "")))
+    out = torch.empty((B,), dtype=torch.float32, device=dev)
+    span = _Span(f"prior log_prob ragged ({precision}) K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}")
+    check(getattr(lib(), "vqb_prior_log_prob_ragged_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(),
+                                                              n_given.data_ptr(), B, H, W, out.data_ptr(),
+                                                              ws.data_ptr(), ws.numel(), _stream()),
+          "prior_log_prob_ragged")
+    span.done()
+    return out
+
+
 PRIOR_CE_REDUCTIONS = ("none", "mean", "sum")      # VQB_PRIOR_CE_NONE, _MEAN, _SUM
 
 
@@ -751,6 +769,28 @@ def prior_sample(net, labels, u, given, n_given, sampling, step_logits=None):
                                      ws.numel(), _stream()), "prior_sample")
     span.done()
     return codes, log_prob
+
+
+def prior_sample_ragged(net, labels, u, given, n_given, sampling=None, step_logits=None, log_prob=True):
+    """prior_sample with one prefix length per image (vqb_prior_sample_ragged_f32): n_given int64 (B,) on the device,
+    never read here; given the int64 codes (B,H,W) whose positions < n_given[b] image b keeps.  sampling None is
+    complete's draw.  -> (codes (B,H,W) int64, log_prob (B,) fp32, or None with log_prob=False)."""
+    B, H, W = u.shape
+    dev = u.device
+    codes = torch.empty((B, H, W), dtype=torch.int64, device=dev)
+    lp = torch.empty((B,), dtype=torch.float32, device=dev) if log_prob else None
+    ws = _prior_workspace(net, B, H, W, dev, lib().vqb_prior_sample_workspace_bytes, 0)
+    knobs = "" if sampling is None else \
+        f" T={sampling.temperature:g} top_k={sampling.top_k} top_p={sampling.top_p:g}"
+    span = _Span(f"prior sample ragged K={net.input_dim} dim={net.dim} L={net.n_layers} {H}x{W}{knobs}")
+    check(lib().vqb_prior_sample_ragged_f32(_lib.C.byref(net), labels.data_ptr(), u.data_ptr(), given.data_ptr(),
+                                            n_given.data_ptr(), B, H, W,
+                                            _lib.C.byref(sampling) if sampling is not None else None,
+                                            codes.data_ptr(), lp.data_ptr() if lp is not None else None,
+                                            step_logits.data_ptr() if step_logits is not None else None,
+                                            ws.data_ptr(), ws.numel(), _stream()), "prior_sample_ragged")
+    span.done()
+    return codes, lp
 
 
 def prior_forward_train(net, codes, labels, precision="fp32"):

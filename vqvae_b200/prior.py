@@ -85,6 +85,35 @@ def _labels(label, B, dev, what):
     return label.to(torch.int64).contiguous()
 
 
+def _per_image(n_given):
+    """Whether n_given gives one prefix length per image (a 1-D tensor, a list or a tuple) rather than one for the
+    batch (an int or a 0-d tensor)."""
+    return isinstance(n_given, (list, tuple)) or (torch.is_tensor(n_given) and n_given.dim() != 0)
+
+
+def _ragged(n_given, x, what):
+    """A per-image n_given for the codes x (B,H,W) -> int64 (B,) on x's device.  A tensor must be 1-D with B entries of
+    an integer dtype, on x's device; its values are never read on the host (the kernels clamp them to [0, H*W]), and an
+    int64 contiguous one is used in place.  A list or tuple must hold B ints in [0, H*W], checked here.  ValueError
+    for the shape, dtype, length or a value; RuntimeError for the device."""
+    B, H, W = x.shape
+    if torch.is_tensor(n_given):
+        if n_given.dim() != 1 or n_given.numel() != B:
+            raise ValueError(f"{what}: a per-image n_given must be a 1-D tensor of {B} entries, got shape "
+                             f"{tuple(n_given.shape)}")
+        if n_given.dtype == torch.bool or n_given.is_floating_point() or n_given.is_complex():
+            raise ValueError(f"{what}: a per-image n_given must have an integer dtype, got {n_given.dtype}")
+        if n_given.device != x.device:
+            raise RuntimeError(f"{what}: n_given is on {n_given.device}, the codes on {x.device}")
+        return n_given.to(torch.int64).contiguous()
+    if len(n_given) != B:
+        raise ValueError(f"{what}: a per-image n_given must have {B} entries, got {len(n_given)}")
+    for v in n_given:
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral) or not 0 <= v <= H * W:
+            raise ValueError(f"{what}: every n_given must be an int in [0, H*W] = [0, {H * W}], got {v!r}")
+    return torch.tensor([int(v) for v in n_given], dtype=torch.int64, device=x.device)
+
+
 def _grad_call(inputs, module=None):
     """Whether a prior module's call is differentiable (GatedPixelCNN's rule): grad enabled and an input, or a
     parameter of `module`, requiring grad."""
@@ -379,25 +408,33 @@ class GatedPixelCNN(nn.Module):
     def _log_prob_args(self, x, label, n_given, per_position):
         """log_prob()'s host-side checks, in order, before any CUDA check or launch: the precision, n_given (an int),
         the codes' rank, n_given in [0, H*W], per_position only with n_given = 0, a square grid, the layers (P5),
-        the label count (ValueError for the arguments, RuntimeError for the shapes, as forward and complete)."""
+        the label count (ValueError for the arguments, RuntimeError for the shapes, as forward and complete).  A
+        per-image n_given is checked by _ragged and returned as an int64 device tensor."""
         what = "GatedPixelCNN.log_prob"
         if self.precision not in ops.PRIOR_PRECISIONS:
             raise ValueError(f"GatedPixelCNN.precision must be one of {ops.PRIOR_PRECISIONS}, got {self.precision!r}")
-        if isinstance(n_given, bool) or not isinstance(n_given, numbers.Integral):
+        ragged = _per_image(n_given)
+        if not ragged and (isinstance(n_given, bool) or not isinstance(n_given, numbers.Integral)):
             raise ValueError(f"{what}: n_given must be an int, got {n_given!r}")
+        if ragged and per_position:
+            raise ValueError(f"{what}: per_position=True scores every position; n_given must be 0, got a per-image "
+                             "n_given")
         if x.dim() != 3:
             raise RuntimeError(f"{what}: expected codes of shape (B,H,W), got {tuple(x.shape)}")
         B, H, W = x.shape
-        if not 0 <= n_given <= H * W:
-            raise ValueError(f"{what}: n_given must be in [0, H*W] = [0, {H * W}], got {n_given}")
-        if per_position and n_given != 0:
-            raise ValueError(f"{what}: per_position=True scores every position; n_given must be 0, got {n_given}")
+        if ragged:
+            n_given = _ragged(n_given, x, what)
+        else:
+            if not 0 <= n_given <= H * W:
+                raise ValueError(f"{what}: n_given must be in [0, H*W] = [0, {H * W}], got {n_given}")
+            if per_position and n_given != 0:
+                raise ValueError(f"{what}: per_position=True scores every position; n_given must be 0, got {n_given}")
         _square(H, W, what)
         self._check_layers()
         n = (label if torch.is_tensor(label) else torch.as_tensor(label)).numel()
         if n != B:
             raise RuntimeError(f"{what}: expected {B} labels, got {n}")
-        return int(n_given)
+        return n_given if ragged else int(n_given)
 
     def _log_prob(self, x, label, n_given=0, per_position=False):
         """log_prob() as a graph-capturable call: the same checks and result, and for int64 contiguous codes and
@@ -407,9 +444,11 @@ class GatedPixelCNN(nn.Module):
         ops._require_cuda(x, "GatedPixelCNN.log_prob codes")
         label = _labels(label, B, x.device, "GatedPixelCNN.log_prob")
         x = x.detach().to(torch.int64).contiguous()
+        keep = []
+        if torch.is_tensor(n_given):
+            return ops.prior_log_prob_ragged(self._net(keep), x, label, n_given, self.precision)
         if n_given == H * W:                # nothing to score: no packing, no launch
             return torch.zeros((B,), dtype=torch.float32, device=x.device)
-        keep = []
         return ops.prior_log_prob(self._net(keep), x, label, n_given, self.precision, per_position)
 
     def log_prob(self, x, label, *, n_given=0, per_position=False):
@@ -418,6 +457,14 @@ class GatedPixelCNN(nn.Module):
         log_softmax(forward(x, label)[b, :, i, j])[x[b, i, j]], in the model's ``precision``.  per_position=True
         returns the (B,H,W) fp32 map of every position's term instead (n_given must then be 0).  The first n_given
         positions are context, not scored, as in sample_completion; n_given = H*W gives zeros without a launch.
+
+        n_given may also be per image: a 1-D integer tensor of B entries on x's device, or a list or tuple of B ints
+        in [0, H*W].  Entry b is then the sum over image b's positions >= n_given[b], bitwise entry b of the scalar
+        call on the same batch with n_given = n_given[b], in either precision (in fp32 also the call on image b
+        alone), in one call with the scalar call's launches.  A
+        tensor is never read on the host (no synchronisation: a captured graph follows new values written into it),
+        and its values are clamped to [0, H*W] as codes are clamped; a list's values are checked (ValueError).
+        per_position=True takes no per-image n_given (ValueError).  A 0-d tensor is not an int here (ValueError).
 
         -log_prob(x, label).sum() / x.numel() is the reference's validation loss (nn.CrossEntropyLoss on forward's
         logits), without writing the B*K*H*W logits: each position's logits are reduced on chip and the per-image
@@ -503,12 +550,17 @@ class GatedPixelCNN(nn.Module):
 
     def _given(self, x, label, n_given):
         """complete()'s host-side checks, in order, before any CUDA check or launch: the codes' rank, n_given (an
-        int, ValueError outside [0, H*W]), a square grid, layer 0 (P5), the label count.  Returns n_given."""
-        n_given = operator.index(n_given)
+        int, ValueError outside [0, H*W]), a square grid, layer 0 (P5), the label count.  Returns n_given: an int, or
+        a per-image n_given as an int64 device tensor (_ragged's checks)."""
+        ragged = _per_image(n_given)
+        if not ragged:
+            n_given = operator.index(n_given)
         if x.dim() != 3:
             raise RuntimeError(f"GatedPixelCNN.complete: expected codes of shape (B,H,W), got {tuple(x.shape)}")
         B, H, W = x.shape
-        if not 0 <= n_given <= H * W:
+        if ragged:
+            n_given = _ragged(n_given, x, "GatedPixelCNN.complete")
+        elif not 0 <= n_given <= H * W:
             raise ValueError(f"GatedPixelCNN.complete: n_given must be in [0, H*W] = [0, {H * W}], got {n_given}")
         _square(H, W, "GatedPixelCNN.complete")
         self._check_causal("GatedPixelCNN.complete")
@@ -529,9 +581,12 @@ class GatedPixelCNN(nn.Module):
         ops._require_cuda(u, "GatedPixelCNN.complete uniforms")
         label = _labels(label, B, x.device, "GatedPixelCNN.complete")
         x = x.detach().to(torch.int64).contiguous()
+        keep = []
+        if torch.is_tensor(n_given):
+            return ops.prior_sample_ragged(self._net(keep), label, _f32(u), x, n_given, None, step_logits,
+                                           log_prob=False)[0]
         if n_given == H * W:                # nothing to sample: no packing, no launch
             return x.clone()
-        keep = []
         return ops.prior_complete(self._net(keep), label, _f32(u), x, n_given, step_logits)
 
     def complete(self, x, label, n_given):
@@ -540,7 +595,16 @@ class GatedPixelCNN(nn.Module):
         conditioned on everything before it; x's values there are never read.  A new int64 (B,H,W) tensor; x is not
         modified.  Draws exactly one torch.rand((B, H, W)) from the current CUDA generator whatever n_given is, so
         after the same torch.manual_seed, completing any prefix of generate()'s output returns that output.
-        n_given = 0 is generate(); the restrictions are generate()'s (square grids, P5, fp32)."""
+        n_given = 0 is generate(); the restrictions are generate()'s (square grids, P5, fp32).
+
+        n_given may also be per image: a 1-D integer tensor of B entries on x's device, or a list or tuple of B ints
+        in [0, H*W].  Image b then keeps its positions < n_given[b] and is bitwise what complete() returns for image b
+        alone with n_given = n_given[b] and the same uniforms.  One call runs generate()'s schedule, 1 + H*(L + W)
+        launches for L layers whatever the values, each step skipping the images that have that position given.  A
+        tensor is never read on the host (no synchronisation: a graph captured around _complete follows new values
+        written into it), and its values are clamped to [0, H*W] as codes are clamped; a list's values are checked
+        (ValueError).  An int or a 0-d integer tensor is one n_given for the batch, as before; a 1-D tensor of one
+        entry takes the per-image path, with the same bits and its own launch count."""
         n_given = self._given(x, label, n_given)
         ops._require_cuda(x, "GatedPixelCNN.complete codes")
         u = torch.rand(tuple(x.shape), device=x.device)
@@ -575,7 +639,7 @@ class GatedPixelCNN(nn.Module):
         if x is None:
             if u.dim() != 3:
                 raise RuntimeError(f"{what}: expected uniforms of shape (B,H,W), got {tuple(u.shape)}")
-            if n_given != 0:
+            if _per_image(n_given) or n_given != 0:
                 raise ValueError(f"{what}: n_given must be 0 without codes, got {n_given!r}")
             B, H, W = u.shape
             _square(H, W, what)
@@ -590,11 +654,13 @@ class GatedPixelCNN(nn.Module):
             ops._require_cuda(x, what + " codes")
         ops._require_cuda(u, what + " uniforms")
         label = _labels(label, B, u.device, what)
+        keep = []
         if x is not None:
             x = x.detach().to(torch.int64).contiguous()
+            if torch.is_tensor(n_given):
+                return ops.prior_sample_ragged(self._net(keep), label, _f32(u), x, n_given, sampling, step_logits)
             if n_given == H * W:            # nothing to sample: no packing, no launch
                 return x.clone(), torch.zeros((B,), dtype=torch.float32, device=x.device)
-        keep = []
         return ops.prior_sample(self._net(keep), label, _f32(u), x, n_given, sampling, step_logits)
 
     def sample(self, label, shape=(8, 8), batch_size=64, *, temperature=1.0, top_k=None, top_p=None):
@@ -619,7 +685,9 @@ class GatedPixelCNN(nn.Module):
     def sample_completion(self, x, label, n_given, *, temperature=1.0, top_k=None, top_p=None):
         """complete() with sample()'s knobs -> (codes (B,H,W) int64, log_prob (B,) fp32).  log_prob sums the
         model's log-probability over the sampled positions only (0 when n_given = H*W).  Draws exactly one
-        torch.rand((B, H, W)), so with the default knobs and the same seed the codes are complete()'s."""
+        torch.rand((B, H, W)), so with the default knobs and the same seed the codes are complete()'s.  n_given may be
+        per image, as complete() takes it: log_prob[b] then sums over image b's sampled positions only (0 when
+        n_given[b] = H*W), and codes, log_prob and step logits are bitwise the scalar call's on image b alone."""
         what = "GatedPixelCNN.sample_completion"
         n_given = self._given(x, label, n_given)
         self._knobs(temperature, top_k, top_p, what)
