@@ -344,6 +344,11 @@ int vqb_relu_backward_f32(const float *g, const float *y, float *out, int64_t n,
 /* ---- layout changes at the module boundary (quantizer.py:45, :74) ---------------- */
 int vqb_nchw_to_nhwc_f32(const float *in, float *out, int B, int C, int H, int W, void *stream);
 int vqb_nhwc_to_nchw_f32(const float *in, float *out, int B, int C, int H, int W, void *stream);
+/* The same changes between C real channels and Cp >= C stored ones (a standalone GatedMaskedConv2d at a dim the prior
+ * kernels run padded, VQB_PACK_PRIOR_PAD_F32): NCHW (B,C,H,W) -> NHWC (B,H,W,Cp) with channels C..Cp-1 zero, and
+ * NHWC (B,H,W,Cp) -> NCHW (B,C,H,W) reading channels 0..C-1 only.  One launch each.                              */
+int vqb_nchw_to_nhwc_pad_f32(const float *in, float *out, int B, int C, int Cp, int H, int W, void *stream);
+int vqb_nhwc_to_nchw_unpad_f32(const float *in, float *out, int B, int C, int Cp, int H, int W, void *stream);
 
 /* Stream-ordered copy used by the host-buffer streaming front end (vqvae_b200.HostPipeline):
  * kind 1 = host -> device, 2 = device -> host, 3 = device -> device.  Host buffers should be
@@ -708,9 +713,24 @@ enum vqb_pack_layout {
     VQB_PACK_BF16 = 2,          /* VQB_PACK_F32 in bf16: vqb_pack_conv_weight_bf16                                 */
     VQB_PACK_SHUFFLE_BF16 = 3,  /* VQB_PACK_SHUFFLE_F32 in bf16: vqb_pack_conv_weight_bf16, VQB_CONVT_K4S2_OUT     */
     VQB_PACK_PRIOR_F32 = 4,     /* [(r*cols + s)*Cin + ci][co] over the kept taps r < rows, s < cols: vqb_prior_pack_f32 */
-    VQB_PACK_MASK_ZERO = 5      /* no packing: zeroes the taps r >= rows or s >= cols of the (Cout,Cin,kh,kw)
+    VQB_PACK_MASK_ZERO = 5,     /* no packing: zeroes the taps r >= rows or s >= cols of the (Cout,Cin,kh,kw)
                                    parameter `dst` itself (a mask-A layer's); `src` unused.  Those taps are read by
                                    no packing of the same call                                                      */
+    /* The prior at a dim the kernels do not take (dim % 32 != 0): GatedPixelCNN runs them at Cp = roundup(dim, 32)
+     * channels on zero-padded copies of its parameters.  These three layouts take the padded channel count Cp in
+     * Cin_pad and say which axes pad in `transposed` = kout + 4*kin, one kind per axis (Cout, Cin):
+     *   0  the axis is not padded (output_conv's 512 and K axes, an embedding's rows);
+     *   1  a dim-wide axis: n = dim real channels, then Cp - dim zeros (width Cp);
+     *   2  a gate axis of n = 2*dim channels, padded per half: [dim real, Cp - dim zeros | dim real, Cp - dim zeros]
+     *      (width 2*Cp), because the kernels pair channel c with channel c + Cp.
+     * A padded width below the real one, a kind outside 0..2, an odd gate axis or no padded axis: VQB_ERR_BAD_ARG.
+     * A bias is Cout = its length, Cin = 1; an embedding (rows, cols) is Cout = rows, Cin = cols; both kh = kw = 1. */
+    VQB_PACK_PRIOR_PAD_F32,     /* (6) VQB_PACK_PRIOR_F32 at the padded widths: [(r*cols + s)*Cin' + ci'][co'], zero
+                                   at every padding channel; what vqb_prior_pack_f32 makes of the padded weight     */
+    VQB_PACK_PAD_F32,           /* (7) the parameter in its own layout (Cout, Cin, kh, kw) at the padded widths
+                                   (Cout', Cin', kh, kw), zero at every padding channel                             */
+    VQB_PACK_UNPAD_F32          /* (8) the inverse of VQB_PACK_PAD_F32, for gradients: `dst` (Cout, Cin, kh, kw)
+                                   receives the real entries of the padded `src` (Cout', Cin', kh, kw)              */
 };
 
 typedef struct vqb_pack_desc {
@@ -722,7 +742,8 @@ typedef struct vqb_pack_desc {
 /* Descriptors plus step counters per launch of vqb_repack_multi (480).                                              */
 int vqb_repack_capacity(void);
 /* Every packing of `descs`, then steps[i] += 1 for each of the n_steps device fp32 counters (issue it after the
- * vqb_adam_multi_f32 calls that read them).  The descriptors must not write what another one reads.  Unknown layouts,
+ * vqb_adam_multi_f32 calls that read them).  A single packing is one descriptor and no counters; so is a gradient's
+ * VQB_PACK_UNPAD_F32 copy.  The descriptors must not write what another one reads.  Unknown layouts,
  * NULL pointers, non-positive sizes, Cin_pad < Cin, rows / cols outside the kernel: VQB_ERR_BAD_ARG.
  * ceil((n + n_steps) / vqb_repack_capacity()) launches.                                                             */
 int vqb_repack_multi(const vqb_pack_desc *descs, int n, float *const *steps, int n_steps, void *stream);

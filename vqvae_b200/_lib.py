@@ -47,6 +47,8 @@ SIGNATURES = {
     "vqb_gather_rows_f32": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp]),
     "vqb_nchw_to_nhwc_f32": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "vqb_nhwc_to_nchw_f32": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "vqb_nchw_to_nhwc_pad_f32": (_i, [_vp, _vp] + [_i] * 5 + [_vp]),
+    "vqb_nhwc_to_nchw_unpad_f32": (_i, [_vp, _vp] + [_i] * 5 + [_vp]),
     "vqb_relu_f32": (_i, [_vp, _i64, _vp]),
     "vqb_launch_count": (C.c_ulonglong, []),
     "vqb_set_vq_kernel": (_i, [_i]),
@@ -147,6 +149,7 @@ class PriorGrads(C.Structure):
 
 # enum vqb_pack_layout
 PACK_F32, PACK_SHUFFLE_F32, PACK_BF16, PACK_SHUFFLE_BF16, PACK_PRIOR_F32, PACK_MASK_ZERO = range(6)
+PACK_PRIOR_PAD_F32, PACK_PAD_F32, PACK_UNPAD_F32 = range(6, 9)
 
 
 class AdamTensor(C.Structure):

@@ -42,6 +42,27 @@ __global__ void transpose_kernel(const float *__restrict__ in, float *__restrict
     }
 }
 
+// transpose_kernel between strided rows: in[b][R][ldi] (columns c < Cc read) -> out[b][Cc][ldo], rows R..ldo-1 of
+// the output written as zeros.  The channel padding of vqb_nchw_to_nhwc_pad_f32 (ldo = Cp) and the unpadding of
+// vqb_nhwc_to_nchw_unpad_f32 (ldi = Cp).
+__global__ void transpose_pad_kernel(const float *__restrict__ in, float *__restrict__ out, int R, int Cc, int ldi,
+                                     int ldo) {
+    __shared__ float tile[32][33];
+    const long long b = blockIdx.z;
+    const float *src = in + b * (long long)R * ldi;
+    float *dst = out + b * (long long)Cc * ldo;
+    const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+    for (int j = threadIdx.y; j < 32; j += 8) {
+        const int r = r0 + j, c = c0 + threadIdx.x;
+        if (r < R && c < Cc) tile[j][threadIdx.x] = src[(long long)r * ldi + c];
+    }
+    __syncthreads();
+    for (int j = threadIdx.y; j < 32; j += 8) {
+        const int c = c0 + j, r = r0 + threadIdx.x;
+        if (r < ldo && c < Cc) dst[(long long)c * ldo + r] = r < R ? tile[threadIdx.x][j] : 0.f;
+    }
+}
+
 // quantizer.py:63-64 and :70-71 in fp32, like the reference's scalar ops.  COMMIT_ONLY (the EMA codebook): the loss is
 // the commitment term beta * mse alone.
 template <bool COMMIT_ONLY>
@@ -169,6 +190,28 @@ extern "C" int vqb_nchw_to_nhwc_f32(const float *in, float *out, int B, int C, i
 extern "C" int vqb_nhwc_to_nchw_f32(const float *in, float *out, int B, int C, int H, int W, void *stream) {
     if (!in || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
     return transpose_launch(in, out, B, H * W, C, (cudaStream_t)stream);  // [HW][C] -> [C][HW]
+}
+
+static int transpose_pad_launch(const float *in, float *out, int Bt, int R, int Cc, int ldi, int ldo,
+                                cudaStream_t s) {
+    if (Bt > 65535) return VQB_ERR_UNSUPPORTED;
+    dim3 grid((Cc + 31) / 32, ((R > ldo ? R : ldo) + 31) / 32, Bt), block(32, 8);
+    if (grid.y > 65535) return VQB_ERR_UNSUPPORTED;
+    transpose_pad_kernel<<<grid, block, 0, s>>>(in, out, R, Cc, ldi, ldo);
+    VQB_COUNT_LAUNCH(1);
+    return vqb_cuda_status(cudaGetLastError());
+}
+
+extern "C" int vqb_nchw_to_nhwc_pad_f32(const float *in, float *out, int B, int C, int Cp, int H, int W,
+                                        void *stream) {
+    if (!in || !out || B <= 0 || C <= 0 || Cp < C || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    return transpose_pad_launch(in, out, B, C, H * W, H * W, Cp, (cudaStream_t)stream);  // [C][HW] -> [HW][Cp]
+}
+
+extern "C" int vqb_nhwc_to_nchw_unpad_f32(const float *in, float *out, int B, int C, int Cp, int H, int W,
+                                          void *stream) {
+    if (!in || !out || B <= 0 || C <= 0 || Cp < C || H <= 0 || W <= 0) return VQB_ERR_BAD_ARG;
+    return transpose_pad_launch(in, out, B, H * W, C, Cp, H * W, (cudaStream_t)stream);  // [HW][Cp] -> [C][HW]
 }
 
 extern "C" int vqb_vq_finish_f32(const double *sse, const int32_t *hist, int64_t N, int K, int D, float beta,

@@ -131,6 +131,13 @@ __host__ __device__ long long job_elems(const Job &j) {
         case VQB_PACK_SHUFFLE_BF16: return 9LL * 16 * j.Cin;
         case VQB_PACK_PRIOR_F32: return (long long)j.rows * j.cols * j.Cin * j.Cout;
         case VQB_PACK_MASK_ZERO: return (long long)j.Cout * j.Cin * j.kh * j.kw;
+        case VQB_PACK_PRIOR_PAD_F32:      // Cin_pad = Cp, transposed = kout + 4*kin (vqb_pack_layout)
+            return (long long)j.rows * j.cols * pad_width(j.Cin, j.transposed >> 2, j.Cin_pad) *
+                   pad_width(j.Cout, j.transposed & 3, j.Cin_pad);
+        case VQB_PACK_PAD_F32:
+            return (long long)pad_width(j.Cout, j.transposed & 3, j.Cin_pad) *
+                   pad_width(j.Cin, j.transposed >> 2, j.Cin_pad) * j.kh * j.kw;
+        case VQB_PACK_UNPAD_F32: return (long long)j.Cout * j.Cin * j.kh * j.kw;
         default: return 1;                // STEP_JOB
     }
 }
@@ -164,6 +171,18 @@ __global__ void __launch_bounds__(NT) repack_kernel(const __grid_constant__ Repa
                     if (r >= j.rows || s >= j.cols) static_cast<float *>(j.dst)[i] = 0.f;
                     break;
                 }
+                case VQB_PACK_PRIOR_PAD_F32:
+                    static_cast<float *>(j.dst)[i] = pack_prior_pad_at(j.src, i, j.Cout, j.Cin, j.kh, j.kw, j.cols,
+                                                                       j.Cin_pad, j.transposed & 3, j.transposed >> 2);
+                    break;
+                case VQB_PACK_PAD_F32:
+                    static_cast<float *>(j.dst)[i] = pack_pad_at(j.src, i, j.Cout, j.Cin, j.kh * j.kw, j.Cin_pad,
+                                                                 j.transposed & 3, j.transposed >> 2);
+                    break;
+                case VQB_PACK_UNPAD_F32:
+                    static_cast<float *>(j.dst)[i] = unpad_at(j.src, i, j.Cout, j.Cin, j.kh * j.kw, j.Cin_pad,
+                                                              j.transposed & 3, j.transposed >> 2);
+                    break;
                 default:                      // STEP_JOB: nothing in this launch reads the counter
                     *static_cast<float *>(j.dst) += 1.f;
                     break;
@@ -182,6 +201,19 @@ bool bad_hyper(double lr, double beta1, double beta2, double eps, double wd) {
            !(wd >= 0.0);
 }
 
+// the padded layouts' geometry (vqb_pack_layout): Cin_pad = Cp > 0, transposed = kout + 4*kin with kinds 0..2, at
+// least one padded axis, a gate axis even, and no real channel count above its padded half
+bool bad_axis(int n, int kind, int cp) {
+    if (kind == 0) return false;
+    return (kind == 2 && n % 2 != 0) || n / kind > cp;
+}
+
+bool bad_padding(const vqb_pack_desc &d) {
+    const int kout = d.transposed & 3, kin = d.transposed >> 2;
+    return !d.src || d.Cin_pad <= 0 || d.transposed < 1 || d.transposed > 10 || kout > 2 || kin > 2 ||
+           bad_axis(d.Cout, kout, d.Cin_pad) || bad_axis(d.Cin, kin, d.Cin_pad);
+}
+
 bool bad_desc(const vqb_pack_desc &d) {
     if (!d.dst || d.Cout <= 0 || d.Cin <= 0 || d.kh <= 0 || d.kw <= 0) return true;
     switch (d.layout) {
@@ -193,6 +225,11 @@ bool bad_desc(const vqb_pack_desc &d) {
         case VQB_PACK_MASK_ZERO:
             return (d.layout == VQB_PACK_PRIOR_F32 && !d.src) || d.rows < 0 || d.cols < 0 || d.rows > d.kh ||
                    d.cols > d.kw;
+        case VQB_PACK_PRIOR_PAD_F32:
+            if (d.rows < 0 || d.cols < 0 || d.rows > d.kh || d.cols > d.kw) return true;
+            return bad_padding(d);
+        case VQB_PACK_PAD_F32:
+        case VQB_PACK_UNPAD_F32: return bad_padding(d);
         default: return true;
     }
 }

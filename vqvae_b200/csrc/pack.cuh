@@ -42,3 +42,54 @@ __device__ __forceinline__ float pack_prior_at(const float *__restrict__ w, long
     const int r = tap / cols, sc = tap % cols;
     return w[(((long long)co * Cin + ci) * kh + r) * kw + sc];
 }
+
+// The padded prior layouts (VQB_PACK_PRIOR_PAD_F32, _PAD_F32, _UNPAD_F32): a channel axis of n real channels and kind
+// 0 (not padded), 1 (dim-wide: n -> cp) or 2 (a gate axis: 2*dim -> 2*cp, padded per half).
+__host__ __device__ __forceinline__ int pad_width(int n, int kind, int cp) { return kind == 0 ? n : kind * cp; }
+
+// real channel -> its padded index
+__device__ __forceinline__ int pad_index(int c, int n, int kind, int cp) {
+    if (kind == 0) return c;
+    const int d = n / kind;
+    return (c / d) * cp + c % d;
+}
+
+// padded index -> its real channel, or -1 for a padding channel
+__device__ __forceinline__ int pad_real(int c, int n, int kind, int cp) {
+    if (kind == 0) return c;
+    const int d = n / kind, r = c % cp;
+    return r < d ? (c / cp) * d + r : -1;
+}
+
+// VQB_PACK_PRIOR_PAD_F32: pack_prior_at of the zero-padded weight.  i < rows*cols*Cin'*Cout'.
+__device__ __forceinline__ float pack_prior_pad_at(const float *__restrict__ w, long long i, int Cout, int Cin, int kh,
+                                                   int kw, int cols, int cp, int kout, int kin) {
+    const int coutp = pad_width(Cout, kout, cp), cinp = pad_width(Cin, kin, cp);
+    const int co = pad_real((int)(i % coutp), Cout, kout, cp);
+    const long long t = i / coutp;
+    const int ci = pad_real((int)(t % cinp), Cin, kin, cp), tap = (int)(t / cinp);
+    if (co < 0 || ci < 0) return 0.f;
+    const int r = tap / cols, sc = tap % cols;
+    return w[(((long long)co * Cin + ci) * kh + r) * kw + sc];
+}
+
+// VQB_PACK_PAD_F32: (Cout, Cin, khw) -> (Cout', Cin', khw), zero at the padding.  i < Cout'*Cin'*khw.
+__device__ __forceinline__ float pack_pad_at(const float *__restrict__ w, long long i, int Cout, int Cin, int khw,
+                                             int cp, int kout, int kin) {
+    const int cinp = pad_width(Cin, kin, cp);
+    const int tap = (int)(i % khw);
+    const long long t = i / khw;
+    const int ci = pad_real((int)(t % cinp), Cin, kin, cp), co = pad_real((int)(t / cinp), Cout, kout, cp);
+    if (co < 0 || ci < 0) return 0.f;
+    return w[((long long)co * Cin + ci) * khw + tap];
+}
+
+// VQB_PACK_UNPAD_F32: element i < Cout*Cin*khw of (Cout, Cin, khw), read from the padded (Cout', Cin', khw).
+__device__ __forceinline__ float unpad_at(const float *__restrict__ w, long long i, int Cout, int Cin, int khw, int cp,
+                                          int kout, int kin) {
+    const int cinp = pad_width(Cin, kin, cp);
+    const int tap = (int)(i % khw);
+    const long long t = i / khw;
+    const int ci = pad_index((int)(t % Cin), Cin, kin, cp), co = pad_index((int)(t / Cin), Cout, kout, cp);
+    return w[((long long)co * cinp + ci) * khw + tap];
+}

@@ -95,14 +95,41 @@ def _packed_current(param, key):
     return hit is not None and hit[0] == tag and tag[0] is not None
 
 
+def pad_geometry(shape, cp, kout, kin):
+    """The PackDesc geometry of a prior parameter of `shape` at Cp channels (the padded layouts of vqb_pack_layout):
+    Cp in Cin_pad and the axis kinds in `transposed` = kout + 4*kin.  A 1-D parameter is (Cout, 1), a 2-D one
+    (Cout, Cin), a conv weight (Cout, Cin, kh, kw)."""
+    shape = tuple(shape)
+    kh, kw = shape[2:4] if len(shape) == 4 else (1, 1)
+    return dict(Cout=shape[0], Cin=shape[1] if len(shape) > 1 else 1, Cin_pad=cp, kh=kh, kw=kw,
+                transposed=kout + 4 * kin)
+
+
 def pack_spec(param, key):
     """The one place a packing-cache key becomes a layout and its geometry, for the conv weight `param`:
     ("f32", transposed), ("bf16", kind) (the residual 1x1's RES_W2 kind pads Cin to the kernels' 64) or
     ("prior", rows, cols), the kept taps of a prior conv (vqvae_b200/prior.py).  Returns (pack, layouts):
     pack(param, out) runs the key's single-packing entry point (refilling `out` when it has the right size) and returns
     the buffer, or None for a bf16 shape the kernels do not cover; layouts is the same packing as vqb_repack_multi
-    descriptors, a list of (byte offset into that buffer, PackDesc fields), empty when there is no packing."""
+    descriptors, a list of (byte offset into that buffer, PackDesc fields), empty when there is no packing.
+
+    A prior at a dim the kernels do not take runs them at Cp channels on zero-padded copies (DESIGN §8.5), under two
+    more keys: ("prior_pad", rows, cols, Cp, kout, kin), the ("prior", rows, cols) packing of the padded conv weight,
+    and ("pad", Cp, kout, kin), any prior parameter (bias, embedding, conv weight) in its own layout at the padded
+    widths; kout and kin are the kinds of its first two axes (vqb_pack_layout: 0 kept, 1 dim-wide, 2 a gate axis
+    padded per half).  Both are filled by one vqb_repack_multi descriptor, padding included."""
     kind = key[0]
+    if kind in ("prior_pad", "pad"):
+        cp, kout, kin = key[-3:]
+        g = pad_geometry(param.shape, cp, kout, kin)
+        coutp, cinp = ops.pad_width(g["Cout"], kout, cp), ops.pad_width(g["Cin"], kin, cp)
+        if kind == "prior_pad":
+            f = dict(g, layout=_lib.PACK_PRIOR_PAD_F32, rows=key[1], cols=key[2])
+            n = key[1] * key[2] * cinp * coutp
+        else:
+            f = dict(g, layout=_lib.PACK_PAD_F32, rows=0, cols=0)
+            n = coutp * cinp * g["kh"] * g["kw"]
+        return (lambda p, out: ops.pack_one(p, f, n, out=out)), [(0, f)]
     if kind == "prior":
         cout, cin, kh, kw = param.shape
         f = dict(layout=_lib.PACK_PRIOR_F32, Cout=cout, Cin=cin, Cin_pad=cin, kh=kh, kw=kw, transposed=0,

@@ -435,6 +435,29 @@ def nhwc_to_nchw(x):
     return out
 
 
+def nchw_to_nhwc_pad(x, cp):
+    """nchw_to_nhwc with the channels zero-padded to cp (vqb_nchw_to_nhwc_pad_f32); nchw_to_nhwc itself at cp = C."""
+    _require_cuda(x, "input")
+    x = _f32c(x)
+    B, C, H, W = x.shape
+    if cp == C:
+        return nchw_to_nhwc(x)
+    out = torch.empty((B, H, W, cp), dtype=torch.float32, device=x.device)
+    check(lib().vqb_nchw_to_nhwc_pad_f32(x.data_ptr(), out.data_ptr(), B, C, cp, H, W, _stream()), "nchw_to_nhwc_pad")
+    return out
+
+
+def nhwc_to_nchw_unpad(x, c):
+    """nhwc_to_nchw of the first c channels of x (B,H,W,Cp) (vqb_nhwc_to_nchw_unpad_f32); nhwc_to_nchw at c = Cp."""
+    B, H, W, cp = x.shape
+    if cp == c:
+        return nhwc_to_nchw(x)
+    out = torch.empty((B, c, H, W), dtype=torch.float32, device=x.device)
+    check(lib().vqb_nhwc_to_nchw_unpad_f32(x.data_ptr(), out.data_ptr(), B, c, cp, H, W, _stream()),
+          "nhwc_to_nchw_unpad")
+    return out
+
+
 def relu_(x):
     """In-place ReLU on a contiguous fp32 CUDA tensor (residual.py:19 side effect)."""
     check(lib().vqb_relu_f32(x.data_ptr(), x.numel(), _stream()), "relu_")
@@ -846,3 +869,22 @@ def repack_multi(descs, n, steps, n_steps):
     span = _Span(f"repack x{n}")
     check(lib().vqb_repack_multi(descs, n, steps, n_steps, _stream()), "repack_multi")
     span.done()
+
+
+def pad_width(n, kind, cp):
+    """Width at Cp channels of an axis of n real channels and kind 0 (kept), 1 (dim-wide) or 2 (a gate axis, padded
+    per half): vqb_pack_layout's padded layouts."""
+    return kind * cp if kind else n
+
+
+def pack_one(w, fields, n, out=None):
+    """One packing of the fp32 CUDA parameter w into n fp32 elements, described by the PackDesc fields `fields`
+    (layout and geometry), through vqb_repack_multi with one descriptor; `out` is refilled when it has that size."""
+    _require_cuda(w, "weight")
+    w = _f32c(w.detach())
+    n = max(n, 1)
+    if out is None or out.numel() != n or out.dtype != torch.float32 or out.device != w.device:
+        out = torch.empty((n,), dtype=torch.float32, device=w.device)
+    desc = (_lib.PackDesc * 1)(_lib.PackDesc(dst=out.data_ptr(), src=w.data_ptr(), **fields))
+    repack_multi(desc, 1, None, 0)
+    return out

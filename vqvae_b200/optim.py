@@ -35,6 +35,10 @@ def _layout_bytes(off, f):
         n = f["kh"] * f["kw"] * f["Cout"] * f["Cin_pad"]
     elif layout in (_lib.PACK_SHUFFLE_F32, _lib.PACK_SHUFFLE_BF16):
         n = 9 * 16 * f["Cin"]
+    elif layout in (_lib.PACK_PRIOR_PAD_F32, _lib.PACK_PAD_F32):    # Cp in Cin_pad, the axis kinds in transposed
+        cp, kout, kin = f["Cin_pad"], f["transposed"] & 3, f["transposed"] >> 2
+        n = ops.pad_width(f["Cout"], kout, cp) * ops.pad_width(f["Cin"], kin, cp) * \
+            (f["rows"] * f["cols"] if layout == _lib.PACK_PRIOR_PAD_F32 else f["kh"] * f["kw"])
     else:
         n = f["rows"] * f["cols"] * f["Cin"] * f["Cout"]
     return off + n * (2 if layout in (_lib.PACK_BF16, _lib.PACK_SHUFFLE_BF16) else 4)

@@ -34,8 +34,12 @@ Reference behaviour kept on purpose:
       residual: anything else reads the code being drawn, so the reference's one-forward-per-position loop is not
       causal in raster order there, and the sampler refuses it (C ABI: VQB_ERR_UNSUPPORTED)
 
-Limits: dim % 32 == 0 and dim <= 1024, so gated_pixelcnn.py's GatedPixelCNN(K, img_dim**2, n_layers) runs for
-latents up to 32x32; the library refuses any other dim before any launch (VQB_ERR_UNSUPPORTED, a RuntimeError).
+Limits: any dim from 1 to 1024, so gated_pixelcnn.py's GatedPixelCNN(K, img_dim**2, n_layers) runs for every latent
+grid up to 32x32.  The library's kernels take dim % 32 == 0 only; at any other dim the module runs them at
+Cp = roundup(dim, 32) channels on zero-padded packings of its parameters, each gate axis padded per half, and copies
+the real entries of the Cp-shaped gradients back (DESIGN §8.5).  Results are bitwise those of GatedPixelCNN(K, Cp) with
+the zero-padded weights; state dicts stay the reference's at dim.  A dim above 1024 raises a RuntimeError before any
+launch (at a multiple of 32, the library's VQB_ERR_UNSUPPORTED).
 """
 import math
 import numbers
@@ -45,8 +49,9 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from ._lib import PRIOR_MAX_KERNEL, C, PriorGrads, PriorLayerGrads, PriorLayerWeights, PriorNet, PriorSampling
-from .modules import _packed, _packed_current
+from ._lib import (PACK_UNPAD_F32, PRIOR_MAX_KERNEL, C, PackDesc, PriorGrads, PriorLayerGrads, PriorLayerWeights,
+                   PriorNet, PriorSampling)
+from .modules import _packed, _packed_current, pad_geometry
 
 HIDDEN = 512          # output_conv's hidden width
 
@@ -121,6 +126,82 @@ def _grad_call(inputs, module=None):
                                         (module is not None and any(p.requires_grad for p in module.parameters())))
 
 
+MAX_DIM = 1024        # the widest prior the kernels run (dim % 32 == 0 up to it; any other dim padded up to it)
+
+# The kinds of a prior parameter's first two axes at a padded dim (vqb_pack_layout): 1 a dim-wide axis, padded at its
+# end, 2 a gate axis of 2*dim channels, padded per half (the kernels pair channel c with c + Cp), 0 not padded.  Every
+# parameter not listed (output_conv.0.bias, output_conv.2) is the same at every Cp.
+_PAD_KINDS = {"vert_stack.weight": (2, 1), "vert_stack.bias": (2, 0), "vert_to_horiz.weight": (2, 2),
+              "vert_to_horiz.bias": (2, 0), "horiz_stack.weight": (2, 1), "horiz_stack.bias": (2, 0),
+              "horiz_resid.weight": (1, 1), "horiz_resid.bias": (1, 0), "class_cond_embedding.weight": (0, 2),
+              "embedding.weight": (0, 1), "output_conv.0.weight": (0, 1)}
+
+
+def _kinds(name):
+    """_PAD_KINDS of a parameter named as in GatedPixelCNN or GatedMaskedConv2d.named_parameters()."""
+    if name.startswith("layers."):
+        name = name.split(".", 2)[2]
+    return _PAD_KINDS.get(name, (0, 0))
+
+
+def _padded_dim(dim):
+    """The channel count the kernels run a dim-wide prior at: dim when they take it (dim % 32 == 0), else
+    roundup(dim, 32), on zero-padded packings of the parameters (DESIGN §8.5).  RuntimeError, before any packing or
+    launch, for a dim above MAX_DIM that would need padding."""
+    cp = -(-dim // 32) * 32
+    if cp != dim and dim > MAX_DIM:
+        raise RuntimeError(f"GatedPixelCNN: dim {dim} is above the {MAX_DIM} channels the prior kernels run")
+    return cp
+
+
+def _conv_key(cp, dim, name, rows=1, cols=1):
+    """Packing-cache key of the prior conv weight `name` (a _PAD_KINDS entry) keeping taps rows x cols, at Cp."""
+    return ("prior", rows, cols) if cp == dim else ("prior_pad", rows, cols, cp) + _PAD_KINDS[name]
+
+
+def _vector(p, cp, dim, name):
+    """A bias or embedding as the kernels read it: the parameter itself (fp32, contiguous), or at a padded dim its
+    zero-padded copy, cached and refreshed like a weight packing."""
+    return _f32(p) if cp == dim else _packed(p, ("pad", cp) + _PAD_KINDS[name])
+
+
+class _Grads:
+    """One fp32 gradient per parameter of `module` (a GatedPixelCNN or a GatedMaskedConv2d of channel count `dim`) and
+    the tensors the backward kernels write them into.  At a padded dim those are Cp-shaped buffers for the padded
+    parameters, and finish() copies their real entries into the gradients in one vqb_repack_multi launch
+    (VQB_PACK_UNPAD_F32), with no host synchronisation; otherwise the gradients themselves."""
+
+    def __init__(self, module, dev, dim):
+        cp = _padded_dim(dim)
+        self.params = dict(module.named_parameters())
+        self.grads = {k: torch.empty(p.shape, dtype=torch.float32, device=dev) for k, p in self.params.items()}
+        self.out = dict(self.grads)
+        descs = []
+        for k, p in self.params.items():
+            kout, kin = _kinds(k)
+            if cp == dim or not (kout or kin):
+                continue
+            g = pad_geometry(p.shape, cp, kout, kin)
+            shape = list(p.shape)
+            shape[0] = ops.pad_width(shape[0], kout, cp)
+            if len(shape) > 1:
+                shape[1] = ops.pad_width(shape[1], kin, cp)
+            self.out[k] = torch.empty(shape, dtype=torch.float32, device=dev)
+            descs.append(PackDesc(dst=self.grads[k].data_ptr(), src=self.out[k].data_ptr(), layout=PACK_UNPAD_F32,
+                                  rows=0, cols=0, **g))
+        self.descs = (PackDesc * len(descs))(*descs) if descs else None
+
+    def ptr(self, name):
+        return self.out[name].data_ptr()
+
+    def finish(self):
+        """The gradients in parameters() order, each in its parameter's dtype."""
+        if self.descs is not None:
+            ops.repack_multi(self.descs, len(self.descs), None, 0)
+        self.out = None
+        return tuple(self.grads[k].to(p.dtype) for k, p in self.params.items())
+
+
 class _GateFunction(torch.autograd.Function):
     """GatedActivation with a gradient: vqb_prior_gate_f32 forward, vqb_prior_gate_backward_f32 backward."""
 
@@ -180,19 +261,25 @@ class GatedMaskedConv2d(nn.Module):
         self.horiz_stack.weight.data[:, :, :, -1].zero_()
 
     def _weights(self, keep):
-        """struct vqb_prior_layer_weights of this layer; tensors it points into are appended to `keep`."""
+        """struct vqb_prior_layer_weights of this layer; tensors it points into are appended to `keep`.  At a dim the
+        kernels do not take, the packings of the zero-padded layer at _padded_dim(dim) channels (DESIGN §8.5)."""
+        dim = self.horiz_resid.in_channels
+        cp = _padded_dim(dim)
         mask_a = self.mask_type == "A"
         vs, hs = self.vert_stack, self.horiz_stack
-        vkey = ("prior", vs.kernel_size[0] - mask_a, vs.kernel_size[1])
-        hkey = ("prior", 1, hs.kernel_size[1] - mask_a)
+        vkey = _conv_key(cp, dim, "vert_stack.weight", vs.kernel_size[0] - mask_a, vs.kernel_size[1])
+        hkey = _conv_key(cp, dim, "horiz_stack.weight", 1, hs.kernel_size[1] - mask_a)
         self._mark_mask_a()
         if mask_a and not (_packed_current(vs.weight, vkey) and _packed_current(hs.weight, hkey)):
             self.make_causal()          # P3: once per change of the parameters, right before they are packed
-        t = dict(vert_w=_packed(vs.weight, vkey), vert_b=_f32(vs.bias),
-                 v2h_w=_packed(self.vert_to_horiz.weight, ("prior", 1, 1)), v2h_b=_f32(self.vert_to_horiz.bias),
-                 horiz_w=_packed(hs.weight, hkey), horiz_b=_f32(hs.bias),
-                 resid_w=_packed(self.horiz_resid.weight, ("prior", 1, 1)), resid_b=_f32(self.horiz_resid.bias),
-                 class_emb=_f32(self.class_cond_embedding.weight))
+        v2h, res, emb = self.vert_to_horiz, self.horiz_resid, self.class_cond_embedding
+        t = dict(vert_w=_packed(vs.weight, vkey), vert_b=_vector(vs.bias, cp, dim, "vert_stack.bias"),
+                 v2h_w=_packed(v2h.weight, _conv_key(cp, dim, "vert_to_horiz.weight")),
+                 v2h_b=_vector(v2h.bias, cp, dim, "vert_to_horiz.bias"),
+                 horiz_w=_packed(hs.weight, hkey), horiz_b=_vector(hs.bias, cp, dim, "horiz_stack.bias"),
+                 resid_w=_packed(res.weight, _conv_key(cp, dim, "horiz_resid.weight")),
+                 resid_b=_vector(res.bias, cp, dim, "horiz_resid.bias"),
+                 class_emb=_vector(emb.weight, cp, dim, "class_cond_embedding.weight"))
         keep.extend(t.values())
         return PriorLayerWeights(**{k: v.data_ptr() for k, v in t.items()}, kernel=vs.kernel_size[1],
                                  mask_a=int(mask_a), residual=int(bool(self.residual)))
@@ -212,9 +299,11 @@ class GatedMaskedConv2d(nn.Module):
             return _GatedLayerFunction.apply(self, x_v, x_h, label, *self.parameters())
         keep = []
         w = self._weights(keep)
-        out_v, out_h = ops.prior_layer(w, ops.nchw_to_nhwc(x_v.detach()), ops.nchw_to_nhwc(x_h.detach()), label,
-                                       B=B, H=H, W=W, dim=dim, n_classes=self.class_cond_embedding.num_embeddings)
-        return ops.nhwc_to_nchw(out_v), ops.nhwc_to_nchw(out_h)
+        cp = _padded_dim(dim)
+        out_v, out_h = ops.prior_layer(w, ops.nchw_to_nhwc_pad(x_v.detach(), cp), ops.nchw_to_nhwc_pad(x_h.detach(), cp),
+                                       label, B=B, H=H, W=W, dim=cp,
+                                       n_classes=self.class_cond_embedding.num_embeddings)
+        return ops.nhwc_to_nchw_unpad(out_v, dim), ops.nhwc_to_nchw_unpad(out_h, dim)
 
 
 # PriorLayerGrads / PriorGrads field -> parameter name (within a layer / the model)
@@ -227,23 +316,25 @@ _NET_GRADS = dict(embedding="embedding.weight", out1_w="output_conv.0.weight", o
 
 class _GatedLayerFunction(torch.autograd.Function):
     """GatedMaskedConv2d.forward with gradients: inputs are the layer, x_v, x_h (NCHW), the labels and the layer's
-    parameters in ``parameters()`` order.  NCHW <-> NHWC at the boundary; the forward keeps x_v, x_h (NHWC) and
-    vqb_prior_layer_forward_train_f32's `saved`; the backward (vqb_prior_layer_backward_wide_f32) returns the gradients
-    of x_v, x_h and every parameter, mask A's taps included.  The labels get none."""
+    parameters in ``parameters()`` order.  NCHW <-> NHWC at the boundary (at a padded dim, NCHW with dim channels <->
+    NHWC with Cp, zero-filled); the forward keeps x_v, x_h (NHWC) and vqb_prior_layer_forward_train_f32's `saved`; the
+    backward (vqb_prior_layer_backward_wide_f32) returns the gradients of x_v, x_h and every parameter, mask A's taps
+    included.  The labels get none."""
 
     @staticmethod
     def forward(ctx, layer, x_v, x_h, label, *params):
         B, dim, H, W = x_v.shape
+        cp = _padded_dim(dim)
         keep = []
         w = layer._weights(keep)
-        xv, xh = ops.nchw_to_nhwc(x_v.detach()), ops.nchw_to_nhwc(x_h.detach())
+        xv, xh = ops.nchw_to_nhwc_pad(x_v.detach(), cp), ops.nchw_to_nhwc_pad(x_h.detach(), cp)
         nc = layer.class_cond_embedding.num_embeddings
-        out_v, out_h, saved = ops.prior_layer_forward_train(w, xv, xh, label, B=B, H=H, W=W, dim=dim, n_classes=nc)
+        out_v, out_h, saved = ops.prior_layer_forward_train(w, xv, xh, label, B=B, H=H, W=W, dim=cp, n_classes=nc)
         ctx.layer, ctx.w, ctx.keep, ctx.saved = layer, w, keep, (xv, xh, label, saved)
-        ctx.shape = (B, H, W, dim, nc)
+        ctx.shape = (B, H, W, dim, cp, nc)
         ctx.save_for_backward(x_v, x_h, *params)
         ctx.set_materialize_grads(False)
-        return ops.nhwc_to_nchw(out_v), ops.nhwc_to_nchw(out_h)
+        return ops.nhwc_to_nchw_unpad(out_v, dim), ops.nhwc_to_nchw_unpad(out_h, dim)
 
     @staticmethod
     def backward(ctx, g_v, g_h):
@@ -252,19 +343,18 @@ class _GatedLayerFunction(torch.autograd.Function):
                                "(its saved activations are freed by the first backward)")
         ctx.saved_tensors                 # autograd's check that nothing saved was modified in place
         xv, xh, label, saved = ctx.saved
-        B, H, W, dim, nc = ctx.shape
+        B, H, W, dim, cp, nc = ctx.shape
         if g_h is None:
             g_h = torch.zeros((B, dim, H, W), dtype=torch.float32, device=xv.device)
-        dv = ops.nchw_to_nhwc(g_v) if g_v is not None else None
-        params = dict(ctx.layer.named_parameters())
-        grads = {k: torch.empty(p.shape, dtype=torch.float32, device=xv.device) for k, p in params.items()}
-        table = PriorLayerGrads(**{f: grads[k].data_ptr() for f, k in _LAYER_GRADS.items()})
-        d_x_v, d_x_h = ops.prior_layer_backward(ctx.w, xv, xh, label, dv, ops.nchw_to_nhwc(g_h), saved, table,
-                                                B=B, H=H, W=W, dim=dim, n_classes=nc)
+        dv = ops.nchw_to_nhwc_pad(g_v, cp) if g_v is not None else None
+        grads = _Grads(ctx.layer, xv.device, dim)
+        table = PriorLayerGrads(**{f: grads.ptr(k) for f, k in _LAYER_GRADS.items()})
+        d_x_v, d_x_h = ops.prior_layer_backward(ctx.w, xv, xh, label, dv, ops.nchw_to_nhwc_pad(g_h, cp), saved, table,
+                                                B=B, H=H, W=W, dim=cp, n_classes=nc)
         ctx.saved = ctx.keep = None
         need = ctx.needs_input_grad
-        return (None, ops.nhwc_to_nchw(d_x_v) if need[1] else None, ops.nhwc_to_nchw(d_x_h) if need[2] else None,
-                None) + tuple(grads[k].to(p.dtype) for k, p in params.items())
+        return (None, ops.nhwc_to_nchw_unpad(d_x_v, dim) if need[1] else None,
+                ops.nhwc_to_nchw_unpad(d_x_h, dim) if need[2] else None, None) + grads.finish()
 
 
 class _PriorFunction(torch.autograd.Function):
@@ -288,24 +378,23 @@ class _PriorFunction(torch.autograd.Function):
             raise RuntimeError("GatedPixelCNN: backward through the same forward twice is not supported "
                                "(its saved activations are freed by the first backward)")
         codes, labels = ctx.saved_tensors
-        params, grads, table, _layers = _grad_table(ctx.model, codes.device)
+        grads, table, _layers = _grad_table(ctx.model, codes.device)
         ops.prior_backward(ctx.net, codes, labels, _f32(d_logits), ctx.saved, table, ctx.precision)
         ctx.saved = ctx.keep = None
-        return (None, None, None, None) + tuple(grads[k].to(p.dtype) for k, p in params.items())
+        return (None, None, None, None) + grads.finish()
 
 
 def _grad_table(model, dev):
-    """(parameters by name, an empty fp32 gradient per parameter, the PriorGrads struct pointing at them, its layer
-    array, which must outlive the backward call)."""
-    params = dict(model.named_parameters())
-    grads = {k: torch.empty(p.shape, dtype=torch.float32, device=dev) for k, p in params.items()}
+    """(the model's _Grads, the PriorGrads struct pointing at the tensors the backward writes, its layer array, which
+    must outlive the backward call)."""
+    grads = _Grads(model, dev, model.dim)
     n_layers = len(model.layers)
     layers = (PriorLayerGrads * n_layers)(*[
-        PriorLayerGrads(**{f: grads[f"layers.{i}.{k}"].data_ptr() for f, k in _LAYER_GRADS.items()})
+        PriorLayerGrads(**{f: grads.ptr(f"layers.{i}.{k}") for f, k in _LAYER_GRADS.items()})
         for i in range(n_layers)])
     table = PriorGrads(layers=C.cast(layers, C.POINTER(PriorLayerGrads)), n_layers=n_layers,
-                       **{f: grads[k].data_ptr() for f, k in _NET_GRADS.items()})
-    return params, grads, table, layers
+                       **{f: grads.ptr(k) for f, k in _NET_GRADS.items()})
+    return grads, table, layers
 
 
 class _PriorCEFunction(torch.autograd.Function):
@@ -330,10 +419,10 @@ class _PriorCEFunction(torch.autograd.Function):
             raise RuntimeError("GatedPixelCNN.cross_entropy: backward through the same call twice is not supported "
                                "(its saved activations are freed by the first backward)")
         codes, labels = ctx.saved_tensors
-        params, grads, table, _layers = _grad_table(ctx.model, codes.device)
+        grads, table, _layers = _grad_table(ctx.model, codes.device)
         ops.prior_ce_backward(ctx.net, codes, labels, ctx.reduction, _f32(d_loss), ctx.saved, table, ctx.precision)
         ctx.saved = ctx.keep = None
-        return (None,) * 5 + tuple(grads[k].to(p.dtype) for k, p in params.items())
+        return (None,) * 5 + grads.finish()
 
 
 class GatedPixelCNN(nn.Module):
@@ -375,15 +464,18 @@ class GatedPixelCNN(nn.Module):
                                    f"{PRIOR_MAX_KERNEL}")
 
     def _net(self, keep):
-        """(struct vqb_prior_net, its layer array); every tensor it points into is appended to `keep`."""
+        """(struct vqb_prior_net, its layer array); every tensor it points into is appended to `keep`.  At a dim the
+        kernels do not take, the net at _padded_dim(dim) channels on zero-padded packings (DESIGN §8.5)."""
         self._check_layers()
+        cp = _padded_dim(self.dim)
         layers = (PriorLayerWeights * len(self.layers))(*[l._weights(keep) for l in self.layers])
         o1, o2 = self.output_conv[0], self.output_conv[2]
-        t = dict(embedding=_f32(self.embedding.weight), out1_w=_packed(o1.weight, ("prior", 1, 1)), out1_b=_f32(o1.bias),
+        t = dict(embedding=_vector(self.embedding.weight, cp, self.dim, "embedding.weight"),
+                 out1_w=_packed(o1.weight, _conv_key(cp, self.dim, "output_conv.0.weight")), out1_b=_f32(o1.bias),
                  out2_w=_packed(o2.weight, ("prior", 1, 1)), out2_b=_f32(o2.bias))
         keep.extend(t.values())
         keep.append(layers)
-        return PriorNet(layers=layers, n_layers=len(self.layers), input_dim=self.embedding.num_embeddings, dim=self.dim,
+        return PriorNet(layers=layers, n_layers=len(self.layers), input_dim=self.embedding.num_embeddings, dim=cp,
                         n_classes=self.layers[0].class_cond_embedding.num_embeddings if len(self.layers) else 1,
                         **{k: v.data_ptr() for k, v in t.items()})
 
