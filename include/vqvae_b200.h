@@ -673,6 +673,54 @@ int vqb_prior_ce_backward_tf32(const vqb_prior_net *net, const int64_t *codes, c
                                int W, int reduction, const float *d_loss, const void *saved,
                                const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- the cross-entropy's options: class weights, an ignored code and label smoothing (fp32 and TF32) --------------
+ * nn.CrossEntropyLoss(weight, ignore_index, label_smoothing, reduction) of the same logits, with codes clamped as above.
+ * With w the weights (all ones when weight is NULL), e = label_smoothing, y the clamped code of a position, lse its
+ * log-sum-exp, l its logits and W = sum_k w_k (fp64, on the device in a fixed order):
+ *   loss_p = (1 - e) * w_y * (-lp) + (e / K) * (W * lse - sum_k w_k * l_k)   (lp as vqb_prior_log_prob_*'s term)
+ * and loss_p = 0 at an ignored position: one whose raw code (before clamping) equals ignore_index, when has_ignore.
+ * sum_k w_k * l_k is an fp64 sum in the head (each thread's codes in order, then the lanes' and warps' in a fixed
+ * order, as (M, S)), and the smoothing term is W * logf(S) + (W * M - sum_k w_k l_k) in fp64.  SUM adds loss_p as
+ * VQB_PRIOR_CE_SUM does; MEAN divides that sum by the sum of w_y over the positions not ignored (fp64, the same
+ * order), NaN when it is 0.  The backward's d_l[n, k] = g_n * (q_k * c_n - (1 - e) * w_y * [k = y] - (e / K) * w_k),
+ * q_k = expf((l_k - M) - logf(S)), c_n = (1 - e) * w_y + (e / K) * W, is evaluated in fp32 as
+ * g_n * ((1 - e) * w_y * (q_k - [k = y]) + (e / K) * (W * q_k - w_k)); g_n = 0 at an ignored position, and MEAN's
+ * factor (float)(1.0 / divisor) is read from `saved` on the device.  The weights are read on the device only.
+ * With unit weights, no position ignored and e = 0 every value is bitwise the call without options.
+ * The _ex entry points take a NULL options pointer as the call without options (the same launches and sizes), and
+ * return VQB_ERR_BAD_ARG for has_ignore not 0 or 1 or label_smoothing outside [0, 1] (NaN included), after the
+ * checks above.  The same launch counts as without options.                                                       */
+typedef struct {
+    const float *weight;        /* input_dim fp32 weights on the device, or NULL: all ones */
+    int64_t ignore_index;       /* read when has_ignore = 1 */
+    int has_ignore;
+    float label_smoothing;      /* in [0, 1] */
+} vqb_prior_ce_options;
+/* vqb_prior_ce_saved_bytes, plus 8 bytes (W and MEAN's factor) with options.                                      */
+size_t vqb_prior_ce_saved_bytes_ex(int B, int H, int W, int dim, int n_layers, const vqb_prior_ce_options *options);
+/* vqb_prior_ce_workspace_bytes(_tf32) = b, and with options: round_up(b + 4*B*H*W, 8) + 8*B*H*W*splits, splits 1 in
+ * fp32 and vqb_prior_log_prob_workspace_bytes_tf32's in TF32 (0 = bad sizes).                                     */
+size_t vqb_prior_ce_workspace_bytes_ex(int B, int H, int W, int dim, int n_layers, int K, int train,
+                                       const vqb_prior_ce_options *options);
+size_t vqb_prior_ce_workspace_bytes_ex_tf32(int B, int H, int W, int dim, int n_layers, int K, int train,
+                                            const vqb_prior_ce_options *options);
+int vqb_prior_ce_forward_ex_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                                int W, int reduction, const vqb_prior_ce_options *options, float *loss, void *saved,
+                                size_t saved_bytes, void *workspace, size_t workspace_bytes, void *stream);
+int vqb_prior_ce_forward_ex_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                                 int W, int reduction, const vqb_prior_ce_options *options, float *loss, void *saved,
+                                 size_t saved_bytes, void *workspace, size_t workspace_bytes, void *stream);
+/* The backward workspace is vqb_prior_ce_backward_workspace_bytes's; `saved` from the _ex forward with the same
+ * options.                                                                                                          */
+int vqb_prior_ce_backward_ex_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                                 int W, int reduction, const vqb_prior_ce_options *options, const float *d_loss,
+                                 const void *saved, const vqb_prior_grads *grads, void *workspace,
+                                 size_t workspace_bytes, void *stream);
+int vqb_prior_ce_backward_ex_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H,
+                                  int W, int reduction, const vqb_prior_ce_options *options, const float *d_loss,
+                                  const void *saved, const vqb_prior_grads *grads, void *workspace,
+                                  size_t workspace_bytes, void *stream);
+
 /* ---- optimizer step on device: Adam over many tensors, then every weight packing refreshed --------------------
  * One training step's update of a parameter group is two calls, each normally ONE launch: vqb_adam_multi_f32 updates
  * every parameter and its moments, then vqb_repack_multi rebuilds every packing read from those parameters and

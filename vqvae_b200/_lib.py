@@ -105,6 +105,13 @@ SIGNATURES = {
     "vqb_prior_ce_backward_workspace_bytes": (_sz, [_vp] + [_i] * 3),
     "vqb_prior_ce_backward_f32": (_i, [_vp] * 3 + [_i] * 4 + [_vp] * 4 + [_sz, _vp]),
     "vqb_prior_ce_backward_tf32": (_i, [_vp] * 3 + [_i] * 4 + [_vp] * 4 + [_sz, _vp]),
+    "vqb_prior_ce_saved_bytes_ex": (_sz, [_i] * 5 + [_vp]),
+    "vqb_prior_ce_workspace_bytes_ex": (_sz, [_i] * 7 + [_vp]),
+    "vqb_prior_ce_workspace_bytes_ex_tf32": (_sz, [_i] * 7 + [_vp]),
+    "vqb_prior_ce_forward_ex_f32": (_i, [_vp] * 3 + [_i] * 4 + [_vp, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "vqb_prior_ce_forward_ex_tf32": (_i, [_vp] * 3 + [_i] * 4 + [_vp, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "vqb_prior_ce_backward_ex_f32": (_i, [_vp] * 3 + [_i] * 4 + [_vp] * 5 + [_sz, _vp]),
+    "vqb_prior_ce_backward_ex_tf32": (_i, [_vp] * 3 + [_i] * 4 + [_vp] * 5 + [_sz, _vp]),
     "vqb_relu_backward_f32": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "vqb_conv_wgrad_workspace_bytes": (_sz, [_i] * 10),
     "vqb_conv_wgrad_f32": (_i, [_vp] * 4 + [_i] * 12 + [_vp, _sz, _vp]),
@@ -133,6 +140,11 @@ class PriorNet(C.Structure):
 class PriorSampling(C.Structure):
     """struct vqb_prior_sampling"""
     _fields_ = [("temperature", _f), ("top_k", _i), ("top_p", _f)]
+
+
+class PriorCeOptions(C.Structure):
+    """vqb_prior_ce_options"""
+    _fields_ = [("weight", _vp), ("ignore_index", _i64), ("has_ignore", _i), ("label_smoothing", _f)]
 
 
 class PriorLayerGrads(C.Structure):

@@ -211,10 +211,22 @@ struct ToHbm {
     __device__ __forceinline__ void operator()(int p, int k, float v) const { out[p][k * kstride] = v; }
 };
 
-// A running log-sum-exp per slot over the logits this thread sees, and the logit of the slot's target code (the
-// thread that sees it stores it in t[p], shared memory)
+// The cross-entropy options' sum of w_k * l_k per slot over the logits this thread sees, in fp64 (nothing without)
+template <int P, bool OPT>
+struct WlSum {
+    __device__ __forceinline__ void add(int, int, float) {}
+};
 template <int P>
-struct Lse {
+struct WlSum<P, true> {
+    double wl[P];
+    CeOpt o;
+    __device__ __forceinline__ void add(int p, int k, float v) { wl[p] += (double)v * o.wt(k); }
+};
+
+// A running log-sum-exp per slot over the logits this thread sees, and the logit of the slot's target code (the
+// thread that sees it stores it in t[p], shared memory); OPT: also WlSum's sum
+template <int P, bool OPT = false>
+struct Lse : WlSum<P, OPT> {
     float m[P], s[P];
     int tgt[P];
     float *t;
@@ -226,8 +238,16 @@ struct Lse {
             s[p] += expf(v - m[p]);
         }
         if (k == tgt[p]) t[p] = v;
+        this->add(p, k, v);
     }
 };
+
+// lse_head_kernel's per-warp sums of w_k * l_k (OPT only)
+template <int P>
+__device__ __forceinline__ double (&wl_warps())[NT / 32][P] {
+    __shared__ double w[NT / 32][P];
+    return w;
+}
 
 // (m, s) <- the log-sum-exp pair of the union of (m, s) and (m2, s2); an empty pair (-INFINITY, 0) changes nothing
 __device__ __forceinline__ void lse_merge(float &m, float &s, float m2, float s2) {
@@ -330,19 +350,24 @@ __global__ void __launch_bounds__(NT) head_kernel(Net n, Act in, const long long
 // log-sum-exp per slot over its codes k = tid (mod NT), then the warps' pairs are merged by xor butterflies and the
 // eight warps' in warp order.
 // keep.p != nullptr (the cross-entropy's training forward) also stores the hidden layer there, as head_kernel does.
-template <int P, int Q = 2>
+// OPT (the cross-entropy's options): also each position's sum of w_k * l_k (o's weights) in fp64 into wl[g], merged
+// over the lanes and the warps in the order of (M, S).
+template <int P, int Q = 2, bool OPT = false>
 __global__ void __launch_bounds__(NT) lse_head_kernel(Net n, Act in, const long long *labels, const long long *codes,
-                                                      int B, int H, int W, float *part, Act keep) {
+                                                      int B, int H, int W, float *part, Act keep, CeOpt o = {},
+                                                      double *wl = nullptr) {
     Smem<P, Q> &s = block_smem<P, Q>();
     __shared__ float t[P], wm[NT / 32][P], wsum[NT / 32][P];
     set_slots(s, B, 0, H, 0, W, labels, n.NC);
-    Lse<P> sink;
+    Lse<P, OPT> sink;
 #pragma unroll
     for (int p = 0; p < P; ++p) {
         sink.m[p] = -INFINITY;
         sink.s[p] = 0.f;
         sink.tgt[p] = s.b[p] >= 0 ? clampi(codes[((long long)s.b[p] * H + s.r[p]) * W + s.c[p]], n.K) : -1;
+        if constexpr (OPT) sink.wl[p] = 0.0;
     }
+    if constexpr (OPT) sink.o = o;
     sink.t = t;
     head_positions(s, n, in, sink, H, W, keep);
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
@@ -357,6 +382,11 @@ __global__ void __launch_bounds__(NT) lse_head_kernel(Net n, Act in, const long 
             wm[warp][p] = m;
             wsum[warp][p] = sm;
         }
+        if constexpr (OPT) {
+            double a = sink.wl[p];
+            for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+            if (lane == 0) wl_warps<P>()[warp][p] = a;
+        }
     }
     __syncthreads();
     if (threadIdx.x < P) {
@@ -364,10 +394,16 @@ __global__ void __launch_bounds__(NT) lse_head_kernel(Net n, Act in, const long 
         if (s.b[p] < 0) return;
         float m = wm[0][p], sm = wsum[0][p];
         for (int w = 1; w < NT / 32; ++w) lse_merge(m, sm, wm[w][p], wsum[w][p]);
-        float *q = part + (((long long)s.b[p] * H + s.r[p]) * W + s.c[p]) * 3;
+        const long long g = ((long long)s.b[p] * H + s.r[p]) * W + s.c[p];
+        float *q = part + g * 3;
         q[0] = m;
         q[1] = sm;
         q[2] = t[p];
+        if constexpr (OPT) {
+            double a = wl_warps<P>()[0][p];
+            for (int w = 1; w < NT / 32; ++w) a += wl_warps<P>()[w][p];
+            wl[g] = a;
+        }
     }
 }
 
@@ -727,12 +763,14 @@ void launch_head(cudaStream_t s, const Net &n, const Act &in, const long long *l
     });
 }
 
+template <bool OPT = false>
 void launch_lse_head(cudaStream_t s, const Net &n, const Act &in, const long long *lab, const long long *codes, int B,
-                     int H, int W, float *part, const Act &keep) {
+                     int H, int W, float *part, const Act &keep, const CeOpt &o = {}, double *wl = nullptr) {
     by_q(n.C, [&](auto q) {
         constexpr int Q = decltype(q)::value, P = pf<Q>();
-        lse_head_kernel<P, Q><<<blocks((long long)B * H * W, P), NT, smem_of<lse_head_kernel<P, Q>, P, Q>(), s>>>(
-            n, in, lab, codes, B, H, W, part, keep);
+        lse_head_kernel<P, Q, OPT><<<blocks((long long)B * H * W, P), NT,
+                                     smem_of<lse_head_kernel<P, Q, OPT>, P, Q>(), s>>>(n, in, lab, codes, B, H, W, part,
+                                                                                       keep, o, wl);
     });
 }
 
@@ -1115,8 +1153,13 @@ extern "C" int vqb_prior_forward_train_f32(const vqb_prior_net *net, const int64
 }
 
 extern "C" size_t vqb_prior_ce_saved_bytes(int B, int H, int W, int dim, int n_layers) {
+    return vqb_prior_ce_saved_bytes_ex(B, H, W, dim, n_layers, nullptr);
+}
+
+extern "C" size_t vqb_prior_ce_saved_bytes_ex(int B, int H, int W, int dim, int n_layers,
+                                              const vqb_prior_ce_options *options) {
     if (B <= 0 || H <= 0 || W <= 0 || dim <= 0 || n_layers <= 0) return 0;
-    return (size_t)ce_saved_floats(Saved{(long long)B * H * W, dim, n_layers}) * sizeof(float);
+    return (size_t)ce_saved_floats(Saved{(long long)B * H * W, dim, n_layers}, options != nullptr) * sizeof(float);
 }
 
 extern "C" size_t vqb_prior_ce_workspace_bytes(int B, int H, int W, int dim, int n_layers, int K, int train) {
@@ -1126,17 +1169,28 @@ extern "C" size_t vqb_prior_ce_workspace_bytes(int B, int H, int W, int dim, int
     return (train ? 3 * npos * sizeof(float) : base) + npos * sizeof(float);
 }
 
+extern "C" size_t vqb_prior_ce_workspace_bytes_ex(int B, int H, int W, int dim, int n_layers, int K, int train,
+                                                  const vqb_prior_ce_options *options) {
+    const size_t base = vqb_prior_ce_workspace_bytes(B, H, W, dim, n_layers, K, train);
+    return base && options ? ce_opt_ws_bytes(base, (long long)B * H * W, 1) : base;
+}
+
+namespace {
+
 // log_prob's launches with the finish of the cross-entropy; with `saved`, train_layers in place of forward_layers and
 // the hidden layer kept, so that `saved` is bitwise vqb_prior_forward_train_f32's.  Workspace: the forward's (saved
-// NULL), then one partial per position, then the per-position losses of MEAN and SUM.
-extern "C" int vqb_prior_ce_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
-                                        int H, int W, int reduction, float *loss, void *saved, size_t saved_bytes,
-                                        void *workspace, size_t workspace_bytes, void *stream) {
+// NULL), then one partial per position, then the per-position losses of MEAN and SUM; with options, then
+// ce_opt_ws_bytes's regions.
+int ce_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                   int reduction, const vqb_prior_ce_options *opt, float *loss, void *saved, size_t saved_bytes,
+                   void *workspace, size_t workspace_bytes, void *stream) {
     Net n;
-    const int st = ce_args(net, n, codes, labels, B, H, W, reduction, loss, workspace);
+    int st = ce_args(net, n, codes, labels, B, H, W, reduction, loss, workspace);
     if (st) return st;
-    if (saved && saved_bytes < vqb_prior_ce_saved_bytes(B, H, W, n.C, n.L)) return VQB_ERR_WORKSPACE;
-    if (workspace_bytes < vqb_prior_ce_workspace_bytes(B, H, W, n.C, n.L, n.K, saved != nullptr))
+    CeOpt o{};
+    if (opt && (st = ce_opt_args(opt, o))) return st;
+    if (saved && saved_bytes < vqb_prior_ce_saved_bytes_ex(B, H, W, n.C, n.L, opt)) return VQB_ERR_WORKSPACE;
+    if (workspace_bytes < vqb_prior_ce_workspace_bytes_ex(B, H, W, n.C, n.L, n.K, saved != nullptr, opt))
         return VQB_ERR_WORKSPACE;
     cudaStream_t s = (cudaStream_t)stream;
     const long long *lab = reinterpret_cast<const long long *>(labels), *cd = reinterpret_cast<const long long *>(codes);
@@ -1151,10 +1205,34 @@ extern "C" int vqb_prior_ce_forward_f32(const vqb_prior_net *net, const int64_t 
     } else {
         xL = forward_layers(n, cd, lab, B, H, W, ws, s);
     }
-    launch_lse_head(s, n, xL, lab, cd, B, H, W, part, keep);
-    VQB_COUNT_LAUNCH(1 + ce_finish(s, part, 1, npos, reduction, loss, saved ? sp + sv.total() : nullptr,
-                                   part + 3 * npos));
+    float *lse = saved ? sp + sv.total() : nullptr;
+    if (opt) {
+        double *wl = ce_opt_wl(workspace, vqb_prior_ce_workspace_bytes(B, H, W, n.C, n.L, n.K, saved != nullptr), npos);
+        launch_lse_head<true>(s, n, xL, lab, cd, B, H, W, part, keep, o, wl);
+        VQB_COUNT_LAUNCH(1 + ce_finish<true>(s, part, 1, npos, reduction, loss, lse, part + 3 * npos,
+                                             CeX{o, cd, wl, nullptr, saved ? sp + ce_saved_floats(sv) : nullptr, n.K}));
+    } else {
+        launch_lse_head(s, n, xL, lab, cd, B, H, W, part, keep);
+        VQB_COUNT_LAUNCH(1 + ce_finish(s, part, 1, npos, reduction, loss, lse, part + 3 * npos));
+    }
     return vqb_cuda_status(cudaGetLastError());
+}
+
+}  // namespace
+
+extern "C" int vqb_prior_ce_forward_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                        int H, int W, int reduction, float *loss, void *saved, size_t saved_bytes,
+                                        void *workspace, size_t workspace_bytes, void *stream) {
+    return ce_forward_f32(net, codes, labels, B, H, W, reduction, nullptr, loss, saved, saved_bytes, workspace,
+                          workspace_bytes, stream);
+}
+
+extern "C" int vqb_prior_ce_forward_ex_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                           int H, int W, int reduction, const vqb_prior_ce_options *options,
+                                           float *loss, void *saved, size_t saved_bytes, void *workspace,
+                                           size_t workspace_bytes, void *stream) {
+    return ce_forward_f32(net, codes, labels, B, H, W, reduction, options, loss, saved, saved_bytes, workspace,
+                          workspace_bytes, stream);
 }
 
 extern "C" size_t vqb_prior_layer_train_saved_bytes(int B, int H, int W, int dim) {

@@ -147,40 +147,138 @@ inline int log_prob_ragged_args(const vqb_prior_net *net, Net &n, const int64_t 
 }
 
 // ---- the cross-entropy (vqb_prior_ce_*): log_prob's head partials, then the loss ----------------------------------
+// The options of the _ex entry points (vqb_prior_ce_options, checked by ce_opt_args).  A position is ignored iff its
+// raw code equals `ignore` (has_ignore); its target is the clamped code y, its weight w_y (1 without a weight vector).
+struct CeOpt {
+    const float *w;               // K weights, or nullptr: all ones
+    long long ignore;
+    int has_ignore;
+    float eps;                    // label smoothing
+    __device__ __forceinline__ float wt(int k) const { return w ? __ldg(w + k) : 1.f; }
+    __device__ __forceinline__ bool ignored(long long code) const { return has_ignore && code == ignore; }
+};
+
+// What the options' finish reads and writes besides the no-options finish's arguments
+struct CeX {
+    CeOpt o;
+    const long long *codes;
+    const double *wl;             // the heads' sum of w_k * l_k per partial (splits per position, in range order)
+    float *wy;                    // MEAN: each position's w_y, 0 if ignored (the divisor's terms); else nullptr
+    float *tail;                  // the saved options tail (ce_saved_floats): tail[0] = W, tail[1] = MEAN's 1 / divisor
+    int K;
+};
+
 // Every position g's loss -lp (lp_of: bitwise -log_prob's term) into loss[g], and (M, logf(S)) into lse[2g], lse[2g+1]
-// (lse == nullptr: not kept)
+// (lse == nullptr: not kept).  OPT: loss_p = (1 - eps) * w_y * (-lp) + (eps / K) * (W * lse - sum_k w_k l_k), 0 if
+// ignored; W = sum_k w_k in fp64 (thread t adds k = t, t + NT, ... in turn, then a pairwise tree), in every block.  The
+// smoothing term is fp64: W*logf(S) + (W*M - sum_k w_k l_k), so a common offset of the logits cancels exactly.
+template <bool OPT = false>
 __global__ void __launch_bounds__(NT) ce_finish_kernel(const float *__restrict__ part, int splits, long long npos,
-                                                       float *__restrict__ loss, float *__restrict__ lse) {
-    for (long long g = (long long)blockIdx.x * NT + threadIdx.x; g < npos; g += (long long)gridDim.x * NT)
-        loss[g] = -lp_of(part + g * splits * 3, splits, lse ? lse + 2 * g : nullptr);
+                                                       float *__restrict__ loss, float *__restrict__ lse, CeX x = {}) {
+    if constexpr (!OPT) {
+        for (long long g = (long long)blockIdx.x * NT + threadIdx.x; g < npos; g += (long long)gridDim.x * NT)
+            loss[g] = -lp_of(part + g * splits * 3, splits, lse ? lse + 2 * g : nullptr);
+    } else {
+        __shared__ double red[NT];
+        double a = 0.0;
+        for (int k = threadIdx.x; k < x.K; k += NT) a += x.o.wt(k);
+        red[threadIdx.x] = a;
+        __syncthreads();
+        for (int h = NT / 2; h > 0; h >>= 1) {
+            if (threadIdx.x < h) red[threadIdx.x] += red[threadIdx.x + h];
+            __syncthreads();
+        }
+        const double Wt = red[0];
+        if (x.tail && blockIdx.x == 0 && threadIdx.x == 0) x.tail[0] = (float)Wt;
+        for (long long g = (long long)blockIdx.x * NT + threadIdx.x; g < npos; g += (long long)gridDim.x * NT) {
+            float ml[2];
+            const float lp = lp_of(part + g * splits * 3, splits, ml);
+            if (lse) {
+                lse[2 * g] = ml[0];
+                lse[2 * g + 1] = ml[1];
+            }
+            const long long c = x.codes[g];
+            const bool ign = x.o.ignored(c);
+            const float wy = ign ? 0.f : x.o.wt(clampi(c, x.K));
+            float v = ign ? 0.f : (1.f - x.o.eps) * wy * -lp;
+            if (x.o.eps != 0.f && !ign) {
+                double wl = 0.0;
+                for (int z = 0; z < splits; ++z) wl += x.wl[g * splits + z];
+                v = (float)((double)v + (double)x.o.eps / x.K * (Wt * ml[1] + (Wt * ml[0] - wl)));
+            }
+            loss[g] = v;
+            if (x.wy) x.wy[g] = wy;
+        }
+    }
 }
 
 // One block: *out = (sum of loss[0 .. npos)) / div, rounded to fp32 once.  The sum is fp64 in a fixed order: thread t
 // adds positions t, t + CE_RT, t + 2*CE_RT, ... in turn, then the threads' sums meet in a pairwise tree.
+// OPT with wy (MEAN): the divisor is the sum of wy in the same order (NaN if it is 0, as torch), and
+// scale (if non-null) receives (float)(1.0 / divisor), the backward's factor.
 constexpr int CE_RT = 1024;
+template <bool OPT = false>
 __global__ void __launch_bounds__(CE_RT) ce_total_kernel(const float *__restrict__ loss, long long npos, double div,
-                                                         float *__restrict__ out) {
-    __shared__ double s[CE_RT];
-    double a = 0.0;
-    for (long long g = threadIdx.x; g < npos; g += CE_RT) a += loss[g];
-    s[threadIdx.x] = a;
+                                                         float *__restrict__ out, const float *__restrict__ wy = nullptr,
+                                                         float *__restrict__ scale = nullptr) {
+    __shared__ double s[OPT ? 2 : 1][CE_RT];
+    const bool den = OPT && wy;
+    double a = 0.0, d = 0.0;
+    for (long long g = threadIdx.x; g < npos; g += CE_RT) {
+        a += loss[g];
+        if (den) d += wy[g];
+    }
+    s[0][threadIdx.x] = a;
+    if constexpr (OPT) s[1][threadIdx.x] = d;
     __syncthreads();
     for (int h = CE_RT / 2; h > 0; h >>= 1) {
-        if (threadIdx.x < h) s[threadIdx.x] += s[threadIdx.x + h];
+        if (threadIdx.x < h) {
+            s[0][threadIdx.x] += s[0][threadIdx.x + h];
+            if constexpr (OPT) s[1][threadIdx.x] += s[1][threadIdx.x + h];
+        }
         __syncthreads();
     }
-    if (threadIdx.x == 0) *out = (float)(s[0] / div);
+    if (threadIdx.x == 0) {
+        if (den) {
+            const double q = s[OPT ? 1 : 0][0];
+            *out = q == 0.0 ? NAN : (float)(s[0][0] / q);
+            if (scale) *scale = (float)(1.0 / q);
+        } else {
+            *out = (float)(s[0][0] / div);
+        }
+    }
 }
 
 // The finish of both precisions' forwards: reduction "none" writes the per-position loss to out, "mean" and "sum" to
-// `scratch` and then the scalar to out.  1 or 2 launches, returned.
+// `scratch` and then the scalar to out.  OPT: x's codes, options, wl and tail filled in; MEAN's w_y go to
+// scratch + npos.  1 or 2 launches, returned.
+template <bool OPT = false>
 inline int ce_finish(cudaStream_t st, const float *part, int splits, long long npos, int reduction, float *out,
-                     float *lse, float *scratch) {
+                     float *lse, float *scratch, CeX x = {}) {
     float *loss = reduction == VQB_PRIOR_CE_NONE ? out : scratch;
-    ce_finish_kernel<<<grid_for(npos), NT, 0, st>>>(part, splits, npos, loss, lse);
+    if (OPT && reduction == VQB_PRIOR_CE_MEAN) x.wy = scratch + npos;
+    ce_finish_kernel<OPT><<<grid_for(npos), NT, 0, st>>>(part, splits, npos, loss, lse, x);
     if (reduction == VQB_PRIOR_CE_NONE) return 1;
-    ce_total_kernel<<<1, CE_RT, 0, st>>>(loss, npos, reduction == VQB_PRIOR_CE_MEAN ? (double)npos : 1.0, out);
+    ce_total_kernel<OPT><<<1, CE_RT, 0, st>>>(loss, npos, reduction == VQB_PRIOR_CE_MEAN ? (double)npos : 1.0, out,
+                                              x.wy, x.tail ? x.tail + 1 : nullptr);
     return 2;
+}
+
+// The options' checks (after ce_args): has_ignore 0 or 1, label_smoothing in [0, 1] (NaN rejected); fills o
+inline int ce_opt_args(const vqb_prior_ce_options *opt, CeOpt &o) {
+    if (opt->has_ignore != 0 && opt->has_ignore != 1) return VQB_ERR_BAD_ARG;
+    if (!(opt->label_smoothing >= 0.f && opt->label_smoothing <= 1.f)) return VQB_ERR_BAD_ARG;
+    o = CeOpt{opt->weight, (long long)opt->ignore_index, opt->has_ignore, opt->label_smoothing};
+    return 0;
+}
+
+// The options path's extra workspace after the no-options bytes `base` of npos positions and `splits` head ranges:
+// MEAN's w_y (4*npos bytes, right after the per-position losses), then, 8-byte aligned, the heads' sums of w_k l_k
+inline size_t ce_opt_ws_bytes(size_t base, long long npos, int splits) {
+    return ((base + 4 * (size_t)npos + 7) & ~(size_t)7) + 8 * (size_t)npos * splits;
+}
+inline double *ce_opt_wl(void *ws, size_t base, long long npos) {
+    return reinterpret_cast<double *>(static_cast<char *>(ws) + ((base + 4 * (size_t)npos + 7) & ~(size_t)7));
 }
 
 // The cross-entropy entry points' checks shared by both precisions and directions, in their order; fills n.
@@ -212,8 +310,9 @@ struct Saved {
     long long total() const { return hid() + N * HID; }
 };
 
-// The cross-entropy forward's `saved`: Saved, then each position's (M, logf(S)) at total() (ce_finish_kernel's lse)
-inline long long ce_saved_floats(const Saved &sv) { return sv.total() + 2 * sv.N; }
+// The cross-entropy forward's `saved`: Saved, then each position's (M, logf(S)) at total() (ce_finish_kernel's lse);
+// with options, then two floats: W = sum_k w_k and MEAN's 1 / sum of w_y (CeX::tail)
+inline long long ce_saved_floats(const Saved &sv, bool opt = false) { return sv.total() + 2 * sv.N + (opt ? 2 : 0); }
 
 // What one layer's training forward (vqb_prior_layer_forward_train_f32) keeps, in floats, NHWC (2C) grids: hv and
 // ph as in Saved.

@@ -192,10 +192,25 @@ struct PartialAdd {
     }
 };
 
+// What the options' CeGrad reads besides the no-options one's: the options, and the saved tail (W, MEAN's factor)
+template <bool OPT>
+struct CeGradX {};
+template <>
+struct CeGradX<true> {
+    CeOpt o;
+    const float *tail;
+    bool mean;
+};
+
 // The cross-entropy's d_logits of row m of a chunk of positions starting at c0, from logit n without its bias:
 // l = v + bias (bitwise the forward's logit), d = g * (expf((l - M) - logS) - [n = c]), into out[m][n] (ld K).
 // g = d_loss[p * gstride] * scale; (M, logS) from lse[2p] (ce_finish_kernel); c the clamped code of position p.
-struct CeGrad {
+// OPT: d = g * (q * c_p - (1 - e) * w_c * [n = c] - (e / K) * w_n), c_p = (1 - e) * w_c + (e / K) * W, evaluated as
+// g * (a * (q - [n = c]) + b * (W * q - w_n)), a = (1 - e) * w_c, b = e / K, so that it is exactly 0 where the
+// gradient is (K = 1) and unit weights, nothing ignored and e = 0 give the same bits; g = 0 at an ignored position,
+// and MEAN's scale is tail[1].
+template <bool OPT = false>
+struct CeGrad : CeGradX<OPT> {
     float *out;
     const float *bias, *lse, *d_loss;
     const long long *codes;
@@ -206,8 +221,17 @@ struct CeGrad {
         const long long p = c0 + m;
         const float l = v + __ldg(bias + n);
         const float q = expf((l - __ldg(lse + 2 * p)) - __ldg(lse + 2 * p + 1));
-        const float g = __ldg(d_loss + p * gstride) * scale;
-        out[(long long)m * K + n] = g * (n == clampi(codes[p], K) ? q - 1.f : q);
+        if constexpr (!OPT) {
+            const float g = __ldg(d_loss + p * gstride) * scale;
+            out[(long long)m * K + n] = g * (n == clampi(codes[p], K) ? q - 1.f : q);
+        } else {
+            const CeOpt &o = this->o;
+            const long long c = codes[p];
+            const int y = clampi(c, K);
+            const float g = o.ignored(c) ? 0.f : __ldg(d_loss + p * gstride) * (this->mean ? __ldg(this->tail + 1) : scale);
+            const float a = (1.f - o.eps) * o.wt(y), b = o.eps / K;
+            out[(long long)m * K + n] = g * (a * (n == y ? q - 1.f : q) + b * (__ldg(this->tail) * q - o.wt(n)));
+        }
     }
 };
 
@@ -510,10 +534,13 @@ void forward_tf32(cudaStream_t st, const Net &n, const long long *codes, const l
 // BN logits sit on the four lanes of a quad (wgmma's accumulator layout), so each row's tile max and sum of exp are
 // quad shuffles; the running (m, s) of a row is rescaled to the new max tile by tile, and the logit at the row's
 // clamped code is kept.  One partial (prior.cuh) per position and CTA column y; no logit goes to memory.
-template <int BN, class LA, class LB>
+// OPT (the cross-entropy's options): also each row's sum of w_n * l_n (o's weights) in fp64, each lane's codes in
+// order, then over the quad, into wl[row * splits + y].
+template <int BN, class LA, class LB, bool OPT = false>
 __global__ void __launch_bounds__(TC_T) tc_lse_kernel(LA a, LB b, const float *__restrict__ bias,
                                                       const long long *__restrict__ codes, int M, int N, int K,
-                                                      int per, int a_mode, int b_mode, float *__restrict__ part) {
+                                                      int per, int a_mode, int b_mode, float *__restrict__ part,
+                                                      CeOpt o = {}, double *__restrict__ wl = nullptr) {
     extern __shared__ unsigned char tc_smem[];
     const uint32_t base = (ptx::smem_u32(tc_smem) + 1023u) & ~1023u;
     const int tid = threadIdx.x, wgi = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
@@ -521,6 +548,7 @@ __global__ void __launch_bounds__(TC_T) tc_lse_kernel(LA a, LB b, const float *_
     const int t0 = blockIdx.y * per, t1 = min((N + BN - 1) / BN, t0 + per);
     const int row = m0 + wgi * 64 + warp * 16 + (lane >> 2);
     float m[2] = {-INFINITY, -INFINITY}, s[2] = {0.f, 0.f}, lt[2] = {-INFINITY, -INFINITY};
+    double swl[2] = {0.0, 0.0};
     int tgt[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) tgt[h] = row + 8 * h < M ? clampi(codes[row + 8 * h], N) : -1;
@@ -542,6 +570,7 @@ __global__ void __launch_bounds__(TC_T) tc_lse_kernel(LA a, LB b, const float *_
                         v = v + __ldg(bias + n);
                         mt = fmaxf(mt, v);
                         if (n == tgt[h]) lt[h] = v;
+                        if constexpr (OPT) swl[h] += (double)v * o.wt(n);
                     }
                 }
             mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
@@ -564,12 +593,17 @@ __global__ void __launch_bounds__(TC_T) tc_lse_kernel(LA a, LB b, const float *_
     for (int h = 0; h < 2; ++h) {
         lt[h] = fmaxf(lt[h], __shfl_xor_sync(0xffffffffu, lt[h], 1));
         lt[h] = fmaxf(lt[h], __shfl_xor_sync(0xffffffffu, lt[h], 2));
+        if constexpr (OPT) {
+            swl[h] += __shfl_xor_sync(0xffffffffu, swl[h], 1);
+            swl[h] += __shfl_xor_sync(0xffffffffu, swl[h], 2);
+        }
         const int r = row + 8 * h;
         if ((lane & 3) == 0 && r < M) {
             float *q = part + ((long long)r * splits + blockIdx.y) * 3;
             q[0] = m[h];
             q[1] = s[h];
             q[2] = lt[h];
+            if constexpr (OPT) wl[(long long)r * splits + blockIdx.y] = swl[h];
         }
     }
 }
@@ -586,19 +620,19 @@ int lse_splits(long long npos, int K, int *per = nullptr) {
     return wgrad_cdiv(tiles, p);                    // no empty range
 }
 
-template <int BN, class LA, class LB>
+template <int BN, bool OPT = false, class LA, class LB>
 void tc_lse_launch(cudaStream_t st, const LA &a, const LB &b, const float *bias, const long long *codes, int M, int N,
-                   int K, float *part) {
+                   int K, float *part, const CeOpt &o = {}, double *wl = nullptr) {
     static bool attr_set = false;                   // if this fails, so does the launch, and the caller reports it
     if (!attr_set)
-        attr_set = cudaFuncSetAttribute(tc_lse_kernel<BN, LA, LB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        attr_set = cudaFuncSetAttribute(tc_lse_kernel<BN, LA, LB, OPT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         TcTile<BN>::SMEM) == cudaSuccess;
     int per;
     const int splits = lse_splits(M, N, &per);
     int a_mode, b_mode;
     tc_modes(a, b, N, K, WgradSplit{1, K}, a_mode, b_mode);
-    tc_lse_kernel<BN, LA, LB><<<dim3(wgrad_cdiv(M, TC_BM), splits), TC_T, TcTile<BN>::SMEM, st>>>(
-        a, b, bias, codes, M, N, K, per, a_mode, b_mode, part);
+    tc_lse_kernel<BN, LA, LB, OPT><<<dim3(wgrad_cdiv(M, TC_BM), splits), TC_T, TcTile<BN>::SMEM, st>>>(
+        a, b, bias, codes, M, N, K, per, a_mode, b_mode, part, o, wl);
 }
 
 }  // namespace
@@ -702,17 +736,29 @@ extern "C" size_t vqb_prior_ce_workspace_bytes_tf32(int B, int H, int W, int dim
     return (train ? (size_t)npos * lse_splits(npos, K) * 3 * sizeof(float) : base) + (size_t)npos * sizeof(float);
 }
 
+extern "C" size_t vqb_prior_ce_workspace_bytes_ex_tf32(int B, int H, int W, int dim, int n_layers, int K, int train,
+                                                       const vqb_prior_ce_options *options) {
+    const size_t base = vqb_prior_ce_workspace_bytes_tf32(B, H, W, dim, n_layers, K, train);
+    const long long npos = (long long)B * H * W;
+    return base && options ? ce_opt_ws_bytes(base, npos, lse_splits(npos, K)) : base;
+}
+
+namespace {
+
 // vqb_prior_log_prob_tf32's launches with the finish of the cross-entropy; with `saved`, every activation in the Saved
 // layout (forward_train_tf32's walk up to the hidden layer, so `saved` is bitwise its).  Workspace: the inference
-// forward's (saved NULL), then the head's partials, then the per-position losses of MEAN and SUM.
-extern "C" int vqb_prior_ce_forward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
-                                         int H, int W, int reduction, float *loss, void *saved, size_t saved_bytes,
-                                         void *workspace, size_t workspace_bytes, void *stream) {
+// forward's (saved NULL), then the head's partials, then the per-position losses of MEAN and SUM; with options, then
+// ce_opt_ws_bytes's regions.
+int ce_forward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
+                    int reduction, const vqb_prior_ce_options *opt, float *loss, void *saved, size_t saved_bytes,
+                    void *workspace, size_t workspace_bytes, void *stream) {
     Net n;
-    const int st = ce_args(net, n, codes, labels, B, H, W, reduction, loss, workspace);
+    int st = ce_args(net, n, codes, labels, B, H, W, reduction, loss, workspace);
     if (st) return st;
-    if (saved && saved_bytes < vqb_prior_ce_saved_bytes(B, H, W, n.C, n.L)) return VQB_ERR_WORKSPACE;
-    if (workspace_bytes < vqb_prior_ce_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K, saved != nullptr))
+    CeOpt o{};
+    if (opt && (st = ce_opt_args(opt, o))) return st;
+    if (saved && saved_bytes < vqb_prior_ce_saved_bytes_ex(B, H, W, n.C, n.L, opt)) return VQB_ERR_WORKSPACE;
+    if (workspace_bytes < vqb_prior_ce_workspace_bytes_ex_tf32(B, H, W, n.C, n.L, n.K, saved != nullptr, opt))
         return VQB_ERR_WORKSPACE;
     cudaStream_t s = (cudaStream_t)stream;
     const long long *cd = reinterpret_cast<const long long *>(codes), *lab = reinterpret_cast<const long long *>(labels);
@@ -730,13 +776,40 @@ extern "C" int vqb_prior_ce_forward_tf32(const vqb_prior_net *net, const int64_t
         part = ws + lay.total();
     }
     const Mat a{hid, HID}, b{n.w2, n.K};
-    if (tc_bn(n.K) == 64) tc_lse_launch<64>(s, a, b, n.b2, cd, npos, n.K, HID, part);
-    else tc_lse_launch<128>(s, a, b, n.b2, cd, npos, n.K, HID, part);
     const int splits = lse_splits(npos, n.K);
-    VQB_COUNT_LAUNCH(3 + 4 * n.L + ce_finish(s, part, splits, npos, reduction, loss,
-                                             saved ? sp + Saved{npos, n.C, n.L}.total() : nullptr,
-                                             part + (long long)npos * splits * 3));
+    const Saved sv{npos, n.C, n.L};
+    float *lse = saved ? sp + sv.total() : nullptr, *scratch = part + (long long)npos * splits * 3;
+    if (opt) {
+        double *wl = ce_opt_wl(workspace, vqb_prior_ce_workspace_bytes_tf32(B, H, W, n.C, n.L, n.K, saved != nullptr),
+                               npos);
+        if (tc_bn(n.K) == 64) tc_lse_launch<64, true>(s, a, b, n.b2, cd, npos, n.K, HID, part, o, wl);
+        else tc_lse_launch<128, true>(s, a, b, n.b2, cd, npos, n.K, HID, part, o, wl);
+        VQB_COUNT_LAUNCH(3 + 4 * n.L + ce_finish<true>(s, part, splits, npos, reduction, loss, lse, scratch,
+                                                       CeX{o, cd, wl, nullptr, saved ? sp + ce_saved_floats(sv) : nullptr,
+                                                           n.K}));
+    } else {
+        if (tc_bn(n.K) == 64) tc_lse_launch<64>(s, a, b, n.b2, cd, npos, n.K, HID, part);
+        else tc_lse_launch<128>(s, a, b, n.b2, cd, npos, n.K, HID, part);
+        VQB_COUNT_LAUNCH(3 + 4 * n.L + ce_finish(s, part, splits, npos, reduction, loss, lse, scratch));
+    }
     return vqb_cuda_status(cudaGetLastError());
+}
+
+}  // namespace
+
+extern "C" int vqb_prior_ce_forward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
+                                         int H, int W, int reduction, float *loss, void *saved, size_t saved_bytes,
+                                         void *workspace, size_t workspace_bytes, void *stream) {
+    return ce_forward_tf32(net, codes, labels, B, H, W, reduction, nullptr, loss, saved, saved_bytes, workspace,
+                           workspace_bytes, stream);
+}
+
+extern "C" int vqb_prior_ce_forward_ex_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                            int B, int H, int W, int reduction, const vqb_prior_ce_options *options,
+                                            float *loss, void *saved, size_t saved_bytes, void *workspace,
+                                            size_t workspace_bytes, void *stream) {
+    return ce_forward_tf32(net, codes, labels, B, H, W, reduction, options, loss, saved, saved_bytes, workspace,
+                           workspace_bytes, stream);
 }
 
 extern "C" size_t vqb_prior_backward_workspace_bytes(const vqb_prior_net *net, int B, int H, int W) {
@@ -821,13 +894,16 @@ int net_backward(const vqb_prior_net *net, const int64_t *codes, const int64_t *
 // ce_rows positions.  Per chunk: the logits product of the forward (Mat hid x Mat W2, one k chunk: bitwise the
 // forward's logits) with the CeGrad epilogue into dl; d_hidden = relu' * (dl W2^T); dW2, db2 partials added to acc.
 // Then dW1, db1 and d x_h^L over all positions, one reduce for both head gradients, and body_backward.
+// opt (the _ex entry points): the CeGrad<true> epilogue, with W and MEAN's factor from the saved tail.
 template <class G>
 int ce_backward(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B, int H, int W,
-                int reduction, const float *d_loss, const void *saved, const vqb_prior_grads *grads, void *workspace,
-                size_t workspace_bytes, void *stream) {
+                int reduction, const vqb_prior_ce_options *opt, const float *d_loss, const void *saved,
+                const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes, void *stream) {
     Net n;
-    const int st_ = ce_args(net, n, codes, labels, B, H, W, reduction, d_loss, workspace);
+    int st_ = ce_args(net, n, codes, labels, B, H, W, reduction, d_loss, workspace);
     if (st_) return st_;
+    CeOpt o{};
+    if (opt && (st_ = ce_opt_args(opt, o))) return st_;
     if (!saved || !grads_ok(grads, n.L)) return VQB_ERR_BAD_ARG;
     if (workspace_bytes < vqb_prior_ce_backward_workspace_bytes(net, B, H, W)) return VQB_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
@@ -847,8 +923,14 @@ int ce_backward(const vqb_prior_net *net, const int64_t *codes, const int64_t *l
     for (int c0 = 0; c0 < npos; c0 += rows) {
         const int P = npos - c0 < rows ? npos - c0 : rows;
         const float *hc = hid + (long long)c0 * HID;
-        product<G>(st, Mat{hc, HID}, Mat{n.w2, K}, CeGrad{dl, n.b2, lse, d_loss, cd, scale, K, gstride, c0}, P, K,
-                   HID);
+        if (opt)
+            product<G>(st, Mat{hc, HID}, Mat{n.w2, K},
+                       CeGrad<true>{{o, lse + 2LL * npos, reduction == VQB_PRIOR_CE_MEAN}, dl, n.b2, lse, d_loss, cd,
+                                    1.f, K, gstride, c0},
+                       P, K, HID);
+        else
+            product<G>(st, Mat{hc, HID}, Mat{n.w2, K}, CeGrad<>{{}, dl, n.b2, lse, d_loss, cd, scale, K, gstride, c0},
+                       P, K, HID);
         product<G>(st, Mat{dl, K}, WPacked{n.w2, HID, K}, ReluBack{dhid + (long long)c0 * HID, hc}, P, HID, K);
         G::run(st, MatT{dl, K}, WithOnes<Mat>{Mat{hc, HID}, HID}, PartialAdd{acc, K, HID + 1, c0 == 0}, K, HID + 1, P,
                s2);
@@ -895,16 +977,32 @@ extern "C" int vqb_prior_ce_backward_f32(const vqb_prior_net *net, const int64_t
                                          int H, int W, int reduction, const float *d_loss, const void *saved,
                                          const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
                                          void *stream) {
-    return ce_backward<Ffma>(net, codes, labels, B, H, W, reduction, d_loss, saved, grads, workspace, workspace_bytes,
-                             stream);
+    return ce_backward<Ffma>(net, codes, labels, B, H, W, reduction, nullptr, d_loss, saved, grads, workspace,
+                             workspace_bytes, stream);
+}
+
+extern "C" int vqb_prior_ce_backward_ex_f32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                            int B, int H, int W, int reduction, const vqb_prior_ce_options *options,
+                                            const float *d_loss, const void *saved, const vqb_prior_grads *grads,
+                                            void *workspace, size_t workspace_bytes, void *stream) {
+    return ce_backward<Ffma>(net, codes, labels, B, H, W, reduction, options, d_loss, saved, grads, workspace,
+                             workspace_bytes, stream);
 }
 
 extern "C" int vqb_prior_ce_backward_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels, int B,
                                           int H, int W, int reduction, const float *d_loss, const void *saved,
                                           const vqb_prior_grads *grads, void *workspace, size_t workspace_bytes,
                                           void *stream) {
-    return ce_backward<Tf32>(net, codes, labels, B, H, W, reduction, d_loss, saved, grads, workspace, workspace_bytes,
-                             stream);
+    return ce_backward<Tf32>(net, codes, labels, B, H, W, reduction, nullptr, d_loss, saved, grads, workspace,
+                             workspace_bytes, stream);
+}
+
+extern "C" int vqb_prior_ce_backward_ex_tf32(const vqb_prior_net *net, const int64_t *codes, const int64_t *labels,
+                                            int B, int H, int W, int reduction, const vqb_prior_ce_options *options,
+                                            const float *d_loss, const void *saved, const vqb_prior_grads *grads,
+                                            void *workspace, size_t workspace_bytes, void *stream) {
+    return ce_backward<Tf32>(net, codes, labels, B, H, W, reduction, options, d_loss, saved, grads, workspace,
+                             workspace_bytes, stream);
 }
 
 extern "C" int vqb_prior_gate_backward_f32(const float *x, const float *d_out, float *d_x, int64_t outer, int C,

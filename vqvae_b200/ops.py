@@ -692,40 +692,64 @@ def _prior_ce_reduction(reduction):
     return PRIOR_CE_REDUCTIONS.index(reduction)
 
 
-def prior_ce_forward(net, codes, labels, reduction, precision="fp32", train=False):
+_INT64 = (-2 ** 63, 2 ** 63 - 1)
+
+
+def prior_ce_options(weight=None, ignore_index=None, label_smoothing=0.0):
+    """The vqb_prior_ce_options struct of cross_entropy's options, or None when they are all neutral by default
+    (weight None, ignore_index None, label_smoothing 0): the call without options.  weight: None or a contiguous fp32
+    tensor of K entries on the device, which the struct points at (the caller keeps it alive for the call, or for the
+    graph).  An ignore_index outside int64 matches no code."""
+    if weight is None and ignore_index is None and label_smoothing == 0.0:
+        return None
+    has_ignore = ignore_index is not None and _INT64[0] <= ignore_index <= _INT64[1]
+    return _lib.PriorCeOptions(weight=weight.data_ptr() if weight is not None else None,
+                               ignore_index=int(ignore_index) if has_ignore else 0, has_ignore=int(has_ignore),
+                               label_smoothing=float(label_smoothing))
+
+
+def prior_ce_forward(net, codes, labels, reduction, precision="fp32", train=False, options=None):
     """The cross-entropy of the teacher-forced logits at int64 codes (B,H,W) (clamped to [0, K-1]) without writing the
     logits (vqb_prior_ce_forward_f32, or _tf32 for precision="tf32") -> (loss, saved): loss (B,H,W) fp32 for
     reduction="none", a 0-d fp32 tensor otherwise; saved None, or with train=True the uint8 buffer of
-    vqb_prior_ce_saved_bytes that prior_ce_backward reads."""
+    vqb_prior_ce_saved_bytes that prior_ce_backward reads.  options: None, or a prior_ce_options struct (the _ex
+    entry points, vqb_prior_ce_saved_bytes_ex and vqb_prior_ce_workspace_bytes_ex)."""
     sfx = _prior_precision(precision)
     r = _prior_ce_reduction(reduction)
     B, H, W = codes.shape
     dev = codes.device
     saved = None
+    opt = _lib.C.byref(options) if options is not None else None
     if train:
-        n = lib().vqb_prior_ce_saved_bytes(B, H, W, net.dim, net.n_layers)
+        n = (lib().vqb_prior_ce_saved_bytes(B, H, W, net.dim, net.n_layers) if options is None else
+             lib().vqb_prior_ce_saved_bytes_ex(B, H, W, net.dim, net.n_layers, opt))
         if n == 0:
             raise RuntimeError("prior: bad sizes")
         saved = torch.empty((n,), dtype=torch.uint8, device=dev)
-    ws = _prior_workspace(net, B, H, W, dev, getattr(lib(), "vqb_prior_ce_workspace_bytes" +
-                                                     ("_tf32" if sfx == "tf32" else "")), int(train))
+    tf = "_tf32" if sfx == "tf32" else ""
+    if options is None:
+        ws = _prior_workspace(net, B, H, W, dev, getattr(lib(), "vqb_prior_ce_workspace_bytes" + tf), int(train))
+    else:
+        ws = _prior_workspace(net, B, H, W, dev, getattr(lib(), "vqb_prior_ce_workspace_bytes_ex" + tf), int(train),
+                              opt)
     loss = torch.empty((B, H, W) if r == 0 else (), dtype=torch.float32, device=dev)
     span = _Span(f"prior cross_entropy ({precision}, {reduction}) K={net.input_dim} dim={net.dim} L={net.n_layers} "
                  f"{H}x{W}")
-    check(getattr(lib(), "vqb_prior_ce_forward_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H,
-                                                         W, r, loss.data_ptr(),
-                                                         saved.data_ptr() if saved is not None else None,
-                                                         saved.numel() if saved is not None else 0, ws.data_ptr(),
-                                                         ws.numel(), _stream()),
-          "prior_ce_forward")
+    args = (_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W, r)
+    rest = (loss.data_ptr(), saved.data_ptr() if saved is not None else None, saved.numel() if saved is not None else 0,
+            ws.data_ptr(), ws.numel(), _stream())
+    if options is None:
+        check(getattr(lib(), "vqb_prior_ce_forward_" + sfx)(*args, *rest), "prior_ce_forward")
+    else:
+        check(getattr(lib(), "vqb_prior_ce_forward_ex_" + sfx)(*args, opt, *rest), "prior_ce_forward")
     span.done()
     return loss, saved
 
 
-def prior_ce_backward(net, codes, labels, reduction, d_loss, saved, grads, precision="fp32"):
+def prior_ce_backward(net, codes, labels, reduction, d_loss, saved, grads, precision="fp32", options=None):
     """Every parameter gradient of the prior's cross-entropy (vqb_prior_ce_backward_f32 / _tf32) into the tensors
     `grads` (a PriorGrads struct) points at; d_loss fp32 contiguous on the device, (B,H,W) for reduction="none" and
-    one element otherwise, saved from prior_ce_forward(train=True) on the same net, inputs and reduction."""
+    one element otherwise, saved from prior_ce_forward(train=True) on the same net, inputs, reduction and options."""
     sfx = _prior_precision(precision)
     r = _prior_ce_reduction(reduction)
     B, H, W = codes.shape
@@ -735,10 +759,13 @@ def prior_ce_backward(net, codes, labels, reduction, d_loss, saved, grads, preci
     ws = torch.empty((n,), dtype=torch.uint8, device=codes.device)
     span = _Span(f"prior cross_entropy backward ({precision}, {reduction}) K={net.input_dim} dim={net.dim} "
                  f"L={net.n_layers} {H}x{W}")
-    check(getattr(lib(), "vqb_prior_ce_backward_" + sfx)(_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B,
-                                                          H, W, r, d_loss.data_ptr(), saved.data_ptr(),
-                                                          _lib.C.byref(grads), ws.data_ptr(), ws.numel(), _stream()),
-          "prior_ce_backward")
+    args = (_lib.C.byref(net), codes.data_ptr(), labels.data_ptr(), B, H, W, r)
+    rest = (d_loss.data_ptr(), saved.data_ptr(), _lib.C.byref(grads), ws.data_ptr(), ws.numel(), _stream())
+    if options is None:
+        check(getattr(lib(), "vqb_prior_ce_backward_" + sfx)(*args, *rest), "prior_ce_backward")
+    else:
+        check(getattr(lib(), "vqb_prior_ce_backward_ex_" + sfx)(*args, _lib.C.byref(options), *rest),
+              "prior_ce_backward")
     span.done()
 
 

@@ -398,18 +398,26 @@ def _grad_table(model, dev):
 
 
 class _PriorCEFunction(torch.autograd.Function):
-    """GatedPixelCNN.cross_entropy with gradients: inputs are the model, the precision, the reduction, codes, labels
-    and every parameter in ``parameters()`` order.  The forward keeps the training activations and each position's
-    log-sum-exp (vqb_prior_ce_forward_*), not the logits; the backward (vqb_prior_ce_backward_*, in the forward's
-    precision) recomputes the logits chunk by chunk and returns one gradient per parameter, as _PriorFunction does."""
+    """GatedPixelCNN.cross_entropy and cross_entropy_ex with gradients: inputs are the model, the precision, the reduction, the options
+    (None, or (fp32 weight or None, ignore_index, label_smoothing)), codes, labels and every parameter in
+    ``parameters()`` order.  The forward keeps the training activations and each position's log-sum-exp
+    (vqb_prior_ce_forward_*), not the logits; the backward (vqb_prior_ce_backward_*, in the forward's precision)
+    recomputes the logits chunk by chunk and returns one gradient per parameter, as _PriorFunction does.  The weight
+    takes no gradient."""
 
     @staticmethod
-    def forward(ctx, model, precision, reduction, codes, labels, *params):
+    def forward(ctx, model, precision, reduction, options, codes, labels, *params):
         keep = []
         net = model._net(keep)
-        loss, saved = ops.prior_ce_forward(net, codes, labels, reduction, precision, train=True)
+        if options is None:
+            opt = None
+            loss, saved = ops.prior_ce_forward(net, codes, labels, reduction, precision, train=True)
+        else:
+            opt = ops.prior_ce_options(*options)
+            loss, saved = ops.prior_ce_forward(net, codes, labels, reduction, precision, train=True, options=opt)
         ctx.model, ctx.net, ctx.keep, ctx.saved = model, net, keep, saved
-        ctx.precision, ctx.reduction = precision, reduction
+        # options keeps alive the fp32 weight the struct points at, for the backward
+        ctx.precision, ctx.reduction, ctx.options = precision, reduction, (options, opt)
         ctx.save_for_backward(codes, labels)
         return loss
 
@@ -420,9 +428,13 @@ class _PriorCEFunction(torch.autograd.Function):
                                "(its saved activations are freed by the first backward)")
         codes, labels = ctx.saved_tensors
         grads, table, _layers = _grad_table(ctx.model, codes.device)
-        ops.prior_ce_backward(ctx.net, codes, labels, ctx.reduction, _f32(d_loss), ctx.saved, table, ctx.precision)
-        ctx.saved = ctx.keep = None
-        return (None,) * 5 + grads.finish()
+        if ctx.options[1] is None:
+            ops.prior_ce_backward(ctx.net, codes, labels, ctx.reduction, _f32(d_loss), ctx.saved, table, ctx.precision)
+        else:
+            ops.prior_ce_backward(ctx.net, codes, labels, ctx.reduction, _f32(d_loss), ctx.saved, table, ctx.precision,
+                                  ctx.options[1])
+        ctx.saved = ctx.keep = ctx.options = None
+        return (None,) * 6 + grads.finish()
 
 
 class GatedPixelCNN(nn.Module):
@@ -586,15 +598,64 @@ class GatedPixelCNN(nn.Module):
         capture into one CUDA graph; a second backward through the same call raises.
 
         Codes outside [0, K-1] are clamped, as the embedding clamps them, and scored and differentiated as the clamped
-        code (torch's cross-entropy would raise).  No weight, ignore_index or label_smoothing.  Any layer stack
-        forward takes is taken.  ValueError for a bad precision or reduction; RuntimeError for forward's shape,
-        layer (P5), label and device checks; every host-side check runs before any CUDA check."""
-        what = "GatedPixelCNN.cross_entropy"
+        code (torch's cross-entropy would raise).  For nn.CrossEntropyLoss's weight, ignore_index and label_smoothing
+        use cross_entropy_ex, the same loss on the same kernels with those options.  Any layer stack forward takes is
+        taken.  ValueError for a bad precision or reduction; RuntimeError for forward's shape, layer (P5), label and
+        device checks; every host-side check runs before any CUDA check."""
+        return self._cross_entropy("GatedPixelCNN.cross_entropy", x, label, reduction, None, None, 0.0)
+
+    def cross_entropy_ex(self, x, label, *, reduction="mean", weight=None, ignore_index=None, label_smoothing=0.0):
+        """cross_entropy with nn.CrossEntropyLoss's options: the value of nn.CrossEntropyLoss(weight=weight,
+        ignore_index=ignore_index, label_smoothing=label_smoothing, reduction=reduction)(forward(x, label)
+        .permute(0, 2, 3, 1).reshape(-1, K), x.reshape(-1)), in the model's ``precision``, without the B*K*H*W logits,
+        differentiable and graph-capturable as cross_entropy is.  With every option at its default it is
+        cross_entropy: the same calls and bits.
+
+        Codes are clamped as in cross_entropy.  The options follow torch, with y the clamped code of a position, lse
+        its log-sum-exp, l its logits, w the weights (all ones for None), W = sum_k w_k and e = label_smoothing:
+        loss_p = (1 - e) * w_y * (lse - l_y) + (e / K) * (W * lse - sum_k w_k * l_k).
+          weight: None, or a 1-D floating tensor of K class weights on the codes' device, used as contiguous fp32.
+            It takes no gradient, and its values are only read on the device, so a captured graph uses the values
+            it holds at each replay.
+          ignore_index: None (the default: nothing is ignored; torch's default is -100, which here is a code that is
+            clamped and scored like any other), or an int: a position is ignored iff its raw code, before clamping,
+            equals it.  ignore_index=-100 gives torch's behaviour.  An ignored position scores 0 and takes no
+            gradient, but is still embedded (clamped) as the model's input, since x is both input and target.
+          label_smoothing: a float in [0, 1].
+        "sum" adds loss_p; "mean" divides that sum by the sum of w_y over the positions not ignored, as torch does: a
+        NaN loss when that is 0 (every position ignored gives zero gradients; scored targets of weight 0 give NaN
+        gradients).  Both sums are fp64 in a fixed order, rounded once.  Options at their neutral values (unit
+        weights, an ignore_index that occurs nowhere, 0 smoothing) give the same bits as cross_entropy.
+
+        ValueError for a bad precision, reduction, label_smoothing (not a finite float in [0, 1]), ignore_index (not
+        None or an int; bools rejected) or weight (rank, length, dtype); RuntimeError for a weight on another device
+        than x, then cross_entropy's shape, layer (P5), label and device checks; every host-side check runs before any
+        CUDA check."""
+        return self._cross_entropy("GatedPixelCNN.cross_entropy_ex", x, label, reduction, weight, ignore_index,
+                                   label_smoothing)
+
+    def _cross_entropy(self, what, x, label, reduction, weight, ignore_index, label_smoothing):
+        """cross_entropy and cross_entropy_ex: the checks in their order, then the call (without options when every
+        option is at its default)."""
         precision = self.precision
         if precision not in ops.PRIOR_PRECISIONS:
             raise ValueError(f"GatedPixelCNN.precision must be one of {ops.PRIOR_PRECISIONS}, got {precision!r}")
         if not isinstance(reduction, str) or reduction not in ops.PRIOR_CE_REDUCTIONS:
             raise ValueError(f"{what}: reduction must be one of {ops.PRIOR_CE_REDUCTIONS}, got {reduction!r}")
+        if (isinstance(label_smoothing, bool) or not isinstance(label_smoothing, numbers.Real)
+                or not math.isfinite(label_smoothing) or not 0.0 <= label_smoothing <= 1.0):
+            raise ValueError(f"{what}: label_smoothing must be a finite float in [0, 1], got {label_smoothing!r}")
+        if ignore_index is not None and (isinstance(ignore_index, bool) or not isinstance(ignore_index, numbers.Integral)):
+            raise ValueError(f"{what}: ignore_index must be None or an int, got {ignore_index!r}")
+        if weight is not None:
+            K = self.embedding.num_embeddings
+            if not torch.is_tensor(weight) or weight.dim() != 1 or weight.numel() != K:
+                shape = tuple(weight.shape) if torch.is_tensor(weight) else type(weight).__name__
+                raise ValueError(f"{what}: weight must be a 1-D tensor of {K} entries, got {shape}")
+            if not weight.is_floating_point():
+                raise ValueError(f"{what}: weight must be a floating tensor, got {weight.dtype}")
+            if weight.device != x.device:
+                raise RuntimeError(f"{what}: weight is on {weight.device}, the codes on {x.device}")
         if x.dim() != 3:
             raise RuntimeError(f"{what}: expected codes of shape (B,H,W), got {tuple(x.shape)}")
         B, H, W = x.shape
@@ -606,10 +667,17 @@ class GatedPixelCNN(nn.Module):
         ops._require_cuda(x, what + " codes")
         label = _labels(label, B, x.device, what)
         x = x.detach().to(torch.int64).contiguous()
+        options = None
+        if weight is not None or ignore_index is not None or label_smoothing != 0.0:
+            w = weight.detach().to(torch.float32).contiguous() if weight is not None else None
+            options = (w, None if ignore_index is None else int(ignore_index), float(label_smoothing))
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            return _PriorCEFunction.apply(self, precision, reduction, x, label, *self.parameters())
+            return _PriorCEFunction.apply(self, precision, reduction, options, x, label, *self.parameters())
         keep = []
-        return ops.prior_ce_forward(self._net(keep), x, label, reduction, precision)[0]
+        if options is None:
+            return ops.prior_ce_forward(self._net(keep), x, label, reduction, precision)[0]
+        return ops.prior_ce_forward(self._net(keep), x, label, reduction, precision,
+                                    options=ops.prior_ce_options(*options))[0]
 
     def _check_causal(self, what):
         """P5: the sampler needs a layer 0 that reads only the codes before the one being drawn."""
