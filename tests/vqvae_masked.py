@@ -13,7 +13,8 @@ from oracle.vqvae_train_port import vector_quantizer
 
 
 def res64(x, w1, w2, n, relu, final):
-    """residual.py with every ReLU given: n applications of one layer, then the stack's ReLU if `final`."""
+    """residual.py with every ReLU given: n applications of one layer, then the stack's ReLU if `final` (an empty stack,
+    n = 0, has no weights: w1 and w2 None)."""
     for _ in range(n):
         r = relu(x)
         x = r + F.conv2d(relu(F.conv2d(r, w1, None, 1, 1)), w2)
@@ -24,12 +25,12 @@ def enc64(x, p, n, relu, e="encoder.conv_stack."):
     h = relu(F.conv2d(x, p[e + "0.weight"], p[e + "0.bias"], 2, 1))
     h = relu(F.conv2d(h, p[e + "2.weight"], p[e + "2.bias"], 2, 1))
     h = F.conv2d(h, p[e + "4.weight"], p[e + "4.bias"], 1, 1)
-    return res64(h, p[e + "5.stack.0.res_block.1.weight"], p[e + "5.stack.0.res_block.3.weight"], n, relu, True)
+    return res64(h, p.get(e + "5.stack.0.res_block.1.weight"), p.get(e + "5.stack.0.res_block.3.weight"), n, relu, True)
 
 
 def dec64(z, p, n, relu, d="decoder.inverse_conv_stack."):
     h = F.conv_transpose2d(z, p[d + "0.weight"], p[d + "0.bias"], 1, 1)
-    h = res64(h, p[d + "1.stack.0.res_block.1.weight"], p[d + "1.stack.0.res_block.3.weight"], n, relu, True)
+    h = res64(h, p.get(d + "1.stack.0.res_block.1.weight"), p.get(d + "1.stack.0.res_block.3.weight"), n, relu, True)
     h = relu(F.conv_transpose2d(h, p[d + "2.weight"], p[d + "2.bias"], 2, 1))
     return F.conv_transpose2d(h, p[d + "4.weight"], p[d + "4.bias"], 2, 1)
 
